@@ -1,11 +1,12 @@
 #!/usr/bin/env python
-"""Benchmarks of the B200-native Flowtron hot path (one JSON line per run; contract in the task statement).
+"""Benchmarks of the H100-native Flowtron hot path (one JSON line per run).
 
     python bench.py [--gpus N] [--steps K] [--warmup W]                 # headline: training, BASELINE.json configs[1]
     python bench.py --workload train --config 3 ...                     # configs[2]: LibriTTS-like, 123 speakers, B=64/GPU
     python bench.py --workload infer --batch {1,16} [--frames 400]      # configs[3]: Flowtron.infer, frames/s + RTF
     python bench.py --workload mel [--utterances 10000]                 # configs[4]: TacotronSTFT sweep, GB/s vs HBM
     python bench.py --impl reference [--workload ...]                   # the UNMODIFIED reference on the host CPU cores
+    python bench.py ... --dump-outputs DIR                              # also write the last timed step's outputs as DIR/<name>.npy
 
 train: a step = Flowtron.forward -> FlowtronLoss -> backward -> bucketed NCCL gradient all-reduce (N>1) -> grad-norm clip
 -> RAdam step (train.py:281-331).  `value` = valid mel frames (sum of out_lens over all ranks) per second with inputs
@@ -51,8 +52,37 @@ def parse():
     ap.add_argument("--wav-int16", action="store_true", help="mel: int16 PCM input (832 B/frame) instead of f32 (1344 B/frame)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--streams", type=int, default=1, help="train: 2 = two half-batch pipelines on two CUDA streams")
-    ap.add_argument("--profile", action="store_true", help="short run for ncu: no e2e leg, no CPU baseline, no graph, warm-up as given")
+    ap.add_argument("--profile", action="store_true", help="short run for a profiler: no e2e leg, no CPU baseline, no graph, warm-up as given")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the timed path computed in its last step as DIR/<name>.npy (float32)")
     return ap.parse_args()
+
+
+DUMP_LIMIT = 2 << 20          # elements per dumped array; larger outputs are dumped as a fixed, seeded sample (64 MB cap in all)
+
+
+def snapshot(arrays):
+    """Host float32 copies of the named device tensors, each at most DUMP_LIMIT elements (a seeded sample of larger ones,
+    the same indices on every run) -- taken right after the timed window, before anything else runs."""
+    out = {}
+    for name, t in arrays.items():
+        if not torch.is_tensor(t):
+            continue
+        a = t.detach().float()
+        if a.numel() > DUMP_LIMIT:
+            idx = torch.randint(0, a.numel(), (DUMP_LIMIT,), generator=torch.Generator().manual_seed(0)).sort().values
+            a = a.reshape(-1)[idx.to(a.device)]
+            name += "_sample"
+        out[name] = a.cpu().numpy()
+    assert sum(a.nbytes for a in out.values()) <= 64 << 20, "dumped outputs exceed 64 MB"
+    return out
+
+
+def write_dump(directory, arrays):
+    import numpy as np
+    os.makedirs(directory, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(directory, name + ".npy"), a)
 
 
 # ------------------------------------------------------------------------------------------------ clocks
@@ -89,11 +119,13 @@ class ClockSampler(threading.Thread):
 
 
 def peaks():
+    """(bf16 TFLOP/s, sustained bf16 TFLOP/s, HBM GB/s, source): MEASURED_PEAKS.json where the machine provides one, else
+    NVIDIA's H100 SXM data sheet (dense bf16 at 700 W; no sustained figure is published, so the same value stands in)."""
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(path):
         p = json.load(open(path))
-        return p.get("bf16_tflops", 1590.0), p.get("bf16_tflops_sustained", 1400.0), p.get("hbm_gbs", 6650.0), "measured"
-    return 1590.0, 1400.0, 6650.0, "fallback"
+        return p.get("bf16_tflops", 989.0), p.get("bf16_tflops_sustained", 989.0), p.get("hbm_gbs", 3350.0), "measured"
+    return 989.0, 989.0, 3350.0, "fallback (H100 SXM data sheet)"
 
 
 def dist_env():
@@ -260,10 +292,15 @@ def run_train(args):
 
     loss_static = torch.zeros((), device=dev)
 
+    last = {}
+
     def step_body(d):
         zero_grads()
         out = model(d["mel"], d["speaker_ids"], d["text"], d["in_lens"], d["out_lens"], d["attn_prior"])
         nll, gl, _ = crit(out, d["gate_target"], d["in_lens"], d["out_lens"])
+        # detached views only: a reference into the autograd graph would keep it alive across steps and break graph capture
+        last.update(z=out[0].detach(), log_s=[t.detach() for t in out[1]], gate=out[2].detach(),
+                    attns=[t.detach() for t in out[3] if torch.is_tensor(t)], nll=nll.detach(), gate_loss=gl.detach())
         loss = (nll + gl).sum()
         loss.backward()
         if fused_opt:
@@ -345,6 +382,13 @@ def run_train(args):
     sampler = ClockSampler(local)
     sampler.start()
     ms = timed(step_value, args.steps)
+    dump = None
+    if args.dump_outputs:
+        arrays = {"z": last["z"], "gate": last["gate"], "nll": last["nll"], "gate_loss": last["gate_loss"], "loss": loss_static,
+                  "params_after_step": torch.cat([q.detach().reshape(-1) for q in model.parameters()])}
+        arrays.update({f"log_s{i}": t for i, t in enumerate(last["log_s"])})
+        arrays.update({f"attn{i}": t for i, t in enumerate(last["attns"])})
+        dump = snapshot(arrays)
     ms_e2e = ms
     if not args.profile:
         for s in range(2):
@@ -377,18 +421,12 @@ def run_train(args):
     lstm = {k: v for k, v in by_name.items() if k.startswith("lstm")}
     top = max(lstm.items(), key=lambda kv: kv[1]["ms"]) if lstm else (max(by_name.items(), key=lambda kv: kv[1]["ms"]) if by_name else (None, None))
     roof = None
-    traffic_tab = {}
-    tp = os.path.join(ROOT, "profiles", "ncu_traffic.json")     # dram bytes per launch from the committed ncu --set full capture
-    if os.path.exists(tp):
-        traffic_tab = json.load(open(tp))
     if top[0]:
         t = top[1]
         ach = t["flop"] / (t["ms"] / 1e3) / 1e12
         steps_per_launch = (T - 1)
         roof = {"kernel": top[0], "bound": "tensor", "achieved": ach, "peak": sustained, "unit": "TFLOP/s", "frac": ach / sustained,
-                "traffic": (traffic_tab.get(top[0]) or {}).get("dram_bytes_per_launch") if (B, T) == (32, 1000) else None,
-                "traffic_source": (traffic_tab.get(top[0]) or {}).get("source"),
-                "peak_source": f"{src} bf16 sustained (kernel timed inside a long step)",
+                "traffic": None, "peak_source": f"{src} bf16 sustained (kernel timed inside a long step)",
                 "launches": t["count"], "avg_ms": t["ms"] / t["count"], "share_of_step": t["ms"] / (ms if graph is None else ms),
                 "us_per_recurrent_step": (t["ms"] / t["count"]) * 1e3 / steps_per_launch,
                 "note": "latency-bound T-step dependency chain (DESIGN.md): algorithmic FLOPs = 2*B*1024*4096*(T-1) per launch; "
@@ -407,7 +445,7 @@ def run_train(args):
                    "encoder_overlap": bool(model.overlap_encoder), "padded_frames_per_s": B * T * world * args.steps / (ms / 1e3),
                    "pipe_fwd": os.environ.get("FT_PIPE_FWD", "default"), "pipe_bwd": os.environ.get("FT_PIPE_BWD", "default"),
                    "att_overlap": os.environ.get("FT_ATT_OVERLAP", "default"), "fuse_bwd": os.environ.get("FT_FUSE_BWD", "default"),
-                   "l2": "working set per step (>3 GB of activations) exceeds the 126 MB L2; no explicit flush"},
+                   "l2": "working set per step (>3 GB of activations) exceeds the 50 MB L2; no explicit flush"},
         "e2e": {"value": e2e, "unit": "valid mel-frames/s", "h2d_bytes_per_step": h2d_bytes, "d2h_bytes_per_step": 4,
                 "ms_per_step": ms_e2e / args.steps, "prior": "built on the device from the lengths (ft_attn_prior)",
                 "losses_read": len(e2e_state["losses"]), "last_loss": e2e_state["losses"][-1] if e2e_state["losses"] else None},
@@ -420,6 +458,9 @@ def run_train(args):
         out["invalid"] = "profiling run (timings under a profiler are never reported)"
     elif not args.no_cpu_baseline:
         out["cpu_baseline"] = cpu_baseline_leg("train", world)
+    if dump is not None:
+        write_dump(args.dump_outputs, dump)
+        out["dumped_outputs"] = sorted(dump)
     print(json.dumps(out))
 
 
@@ -469,10 +510,16 @@ def run_infer(args):
     sampler.start()
     _lib.reset_launch_count()
     _lib.timing(True)
-    ms = timed(step, args.steps)
+    last = {}
+
+    def step_timed():
+        last["mel"] = step()
+
+    ms = timed(step_timed, args.steps)
     launches = _lib.launch_count()
     trep = _lib.timing_report()
     _lib.timing(False)
+    dump = snapshot({"mel": last["mel"]}) if args.dump_outputs else None
     ms_e2e = ms if args.profile else timed(step_e2e, args.steps)
     clocks = sampler.stop()
     if rank != 0:
@@ -490,7 +537,7 @@ def run_infer(args):
         "dtype": "f16 weights/operands, f32 accumulate+state", "data": "synthetic",
         "config": {"workload": f"configs[3]: Flowtron.infer, 2-flow, sigma=0.5, batch {B}, {T} frames, {L} text tokens, gate disabled (fixed work)",
                    "batch": B, "frames": T, "text": L, "parallelism": f"replicas x{world}",
-                   "l2": "weights (107 MB fp16 for 2 flows) are re-read every frame; inputs/outputs are KBs -- no flush (the working set IS the L2-resident weight stream)"},
+                   "l2": "weights (107 MB fp16 for 2 flows) are re-read every frame; inputs/outputs are KBs -- no flush"},
         "rtf": {"frames_per_s_per_stream": T * args.steps / (ms / 1e3), "x_real_time_per_stream": T * args.steps / (ms / 1e3) / (22050.0 / 256.0),
                 "us_per_frame_per_flow": ms * 1e3 / args.steps / T / 2},
         "e2e": {"value": fps_e2e, "unit": "mel-frames/s", "h2d_bytes_per_step": res_h.numel() * 4 + text_h.numel() * 8 + spk_h.numel() * 8,
@@ -499,14 +546,16 @@ def run_infer(args):
         "roofline": {"kernel": "infer_kernel", "bound": "hbm", "achieved": ach, "peak": hbm, "unit": "GB/s", "frac": (ach / hbm) if ach else None,
                      "traffic": None, "peak_source": f"{src} HBM copy bandwidth", "launches": kms["count"],
                      "avg_ms": kms["ms"] / max(1, kms["count"]),
-                     "note": f"algorithmic bytes = {wbytes / 1e6:.1f} MB of fp16 weights per frame per flow x {T} frames per launch (batch-independent); "
-                             "the stream is served by the 126 MB L2 after the first frame, so HBM is the rule's bound, not the physical one"},
+                     "note": f"algorithmic bytes = {wbytes / 1e6:.1f} MB of fp16 weights per frame per flow x {T} frames per launch (batch-independent)"},
         "kernels": kernel_table,
     }
     if args.profile:
         out["invalid"] = "profiling run"
     elif not args.no_cpu_baseline:
         out["cpu_baseline"] = cpu_baseline_leg("infer", world)
+    if dump is not None:
+        write_dump(args.dump_outputs, dump)
+        out["dumped_outputs"] = sorted(dump)
     print(json.dumps(out))
 
 
@@ -552,6 +601,7 @@ def run_mel(args):
     launches = _lib.launch_count()
     trep = _lib.timing_report()
     _lib.timing(False)
+    dump = snapshot({"mel": out}) if args.dump_outputs else None
     ms_e2e = ms
     h2d = d2h = 0
     if not args.profile:
@@ -576,17 +626,13 @@ def run_mel(args):
     bpf = MEL_BYTES_PER_FRAME[fmt]
     ach = frames * bpf / (k["ms"] / k["count"] / 1e3) / 1e9
     traffic = None
-    tp = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    if os.path.exists(tp):
-        per_frame = (json.load(open(tp)).get("mel_fused") or {}).get("dram_bytes_per_frame")
-        traffic = per_frame * frames if per_frame and fmt == "f32" else None     # captured on a 2000-utterance launch, scaled by frames
     res = {
         "metric": "mel front-end mel-frames/sec", "value": fps, "unit": "mel-frames/s", "n_gpus": world, "steps": args.steps, "warmup": n_warm,
         "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
         "dtype": "f32" if fmt == "f32" else "int16 PCM in, f32 math", "data": "synthetic",
         "config": {"workload": f"configs[4]: TacotronSTFT mel front-end sweep, 22.05 kHz, hop 256, n_mel 80, {n_utt} utterances U{{1..10}} s, one launch",
                    "utterances": n_utt, "frames": frames, "samples": total, "wav_format": fmt, "parallelism": f"replicas x{world}",
-                   "l2": f"input {total * (2 if fmt == 's16' else 4) / 1e9:.2f} GB + output {frames * 320 / 1e9:.2f} GB per step: far larger than the 126 MB L2"},
+                   "l2": f"input {total * (2 if fmt == 's16' else 4) / 1e9:.2f} GB + output {frames * 320 / 1e9:.2f} GB per step: far larger than the 50 MB L2"},
         "gbs_algorithmic": frames * bpf * args.steps / (ms / 1e3) / 1e9,
         "e2e": {"value": frames * args.steps * world / (ms_e2e / 1e3), "unit": "mel-frames/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
                 "ms_per_step": ms_e2e / args.steps, "note": "PCIe-bound: the whole waveform goes in and the whole mel comes back every step"},
@@ -600,11 +646,15 @@ def run_mel(args):
         res["invalid"] = "profiling run"
     elif not args.no_cpu_baseline:
         res["cpu_baseline"] = cpu_baseline_leg("mel", world)
+    if dump is not None:
+        write_dump(args.dump_outputs, dump)
+        res["dumped_outputs"] = sorted(dump)
     print(json.dumps(res))
 
 
 def main():
     args = parse()
+    torch.manual_seed(1234)       # the encoder's dropout masks are seeded from torch's: identical arguments, identical run
     if args.impl == "reference":
         return run_reference_arm(args)
     if args.workload == "train":

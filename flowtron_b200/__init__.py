@@ -1,2 +1,2 @@
-"""flowtron_b200 — B200-native (sm_100a) implementation of the Flowtron AR-flow hot path."""
+"""flowtron_b200 — H100-native (sm_90a) implementation of the Flowtron AR-flow hot path."""
 from . import _lib  # noqa: F401

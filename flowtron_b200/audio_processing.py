@@ -65,7 +65,7 @@ class STFT(torch.nn.Module):
         """audio_processing.py:207-235: input [B, N] -> (magnitude [B, n_fft/2+1, F], phase [B, n_fft/2+1, F]),
         F = 1 + N // hop, phase = atan2(imag, real).  CUDA only (fused FFT kernel, filter_length 1024)."""
         if not input_data.is_cuda:
-            raise FlowtronB200Error("STFT.transform needs CUDA tensors: the sm_100a path is the only implementation")
+            raise FlowtronB200Error("STFT.transform needs CUDA tensors: the sm_90a path is the only implementation")
         if self.filter_length != 1024:
             raise NotImplementedError("STFT.transform is built for filter_length 1024 (config.json:31)")
         B, N = input_data.shape
@@ -124,7 +124,7 @@ class TacotronSTFT(torch.nn.Module):
         [n_mel, 1 + N_u // hop] blocks concatenated (utterance u = mel_packed[fo[u]*n_mel : fo[u+1]*n_mel].view(n_mel, -1))
         and the host int64 prefix sums fo.  One kernel launch for the whole shard; no host sync."""
         if not flat.is_cuda:
-            raise FlowtronB200Error("TacotronSTFT needs CUDA tensors: the sm_100a path is the only implementation")
+            raise FlowtronB200Error("TacotronSTFT needs CUDA tensors: the sm_90a path is the only implementation")
         if flat.dtype not in (torch.float32, torch.int16):
             raise TypeError("waveform must be float32 in [-1, 1] or int16 PCM")
         hop, n_fft = self.stft_fn.hop_length, self.stft_fn.filter_length
@@ -145,7 +145,7 @@ class TacotronSTFT(torch.nn.Module):
     def mel_spectrogram_ragged(self, wavs):
         """wavs: list of 1-D float tensors in [-1, 1] (any lengths > filter_length/2) -> list of [n_mel, 1 + N//hop]."""
         if not wavs[0].is_cuda:
-            raise FlowtronB200Error("TacotronSTFT needs CUDA tensors: the sm_100a path is the only implementation")
+            raise FlowtronB200Error("TacotronSTFT needs CUDA tensors: the sm_90a path is the only implementation")
         flat = torch.cat([w.reshape(-1).float() for w in wavs]) if len(wavs) > 1 else wavs[0].reshape(-1).float().contiguous()
         out, fo = self.mel_spectrogram_packed(flat, [int(w.numel()) for w in wavs])
         return [out[fo[i] * self.n_mel_channels: fo[i + 1] * self.n_mel_channels].view(self.n_mel_channels, -1)
@@ -156,7 +156,7 @@ class TacotronSTFT(torch.nn.Module):
         assert torch.min(y.data) >= -1
         assert torch.max(y.data) <= 1
         if not y.is_cuda:
-            raise FlowtronB200Error("TacotronSTFT needs CUDA tensors: the cuFFT/sm_100a path is the only implementation")
+            raise FlowtronB200Error("TacotronSTFT needs CUDA tensors: the cuFFT/sm_90a path is the only implementation")
         B, N = y.shape
         hop, n_fft = self.stft_fn.hop_length, self.stft_fn.filter_length
         if N <= n_fft // 2:

@@ -1,4 +1,4 @@
-"""In-tree build of libflowtron_b200.so with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""In-tree build of libflowtron_b200.so with nvcc for sm_90a (cross-compiles without a GPU)."""
 from __future__ import annotations
 
 import os
@@ -10,7 +10,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libflowtron_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v"]
 
 
@@ -52,7 +52,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         list(ex.map(cc, jobs))
     objs = [os.path.join(objdir, s[:-3] + ".o") for s in sources()]
     if force or jobs or _stale(LIB, objs):
-        cmd = [NVCC, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a",
+        cmd = [NVCC, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a",
                "-cudart", "shared", "-lcufft", "-Xlinker", "-rpath,/usr/local/cuda/lib64"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:

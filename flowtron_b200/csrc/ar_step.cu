@@ -94,8 +94,9 @@ struct W16 {
 };
 
 // Layer pipeline (DESIGN.md 4.2; default ON, FT_PIPE_FWD=0 / FT_PIPE_BWD=0 fall back to one launch per layer): lstm layers 0
-// and 1 run as two 64-CTA recurrences one chunk of FT_PIPE_CHUNK steps apart, forward and BPTT.  Measured r2 on B200
-// (B=32, T=1000): 81.97 -> 66.83 ms/step.
+// and 1 run as two 64-CTA recurrences one chunk of FT_PIPE_CHUNK steps apart, forward and BPTT.  On a 132-SM H100 the two
+// recurrences leave 4 SMs to the per-chunk GEMMs, which mostly run between recurrence steps; the schedule still wins there
+// (DESIGN.md 4.11: B=32, T=1000, 74 ms/step with both pipelines, 84 without).
 static bool pipe_fwd_enabled() {
     static int v = -1;
     if (v < 0) { const char* e = getenv("FT_PIPE_FWD"); v = (!e || atoi(e) != 0) ? 1 : 0; }
@@ -221,7 +222,7 @@ int gemm_wgrad(cudaStream_t st, int N, int K, long long R, const void* dY, long 
 }
 
 // Side stream for work that is off the backward critical path (weight gradients, bias column sums): it runs under the
-// next persistent BPTT kernel, which occupies 64 of the 148 SMs.  One side stream + event per caller stream; ordering is
+// next persistent BPTT kernel, which occupies 64 of the SMs.  One side stream + event per caller stream; ordering is
 // by events only (fork: side waits for "main so far"; join: main waits for "side so far").
 struct Side {
     cudaStream_t s = nullptr;
@@ -320,7 +321,7 @@ int ar_step_fwd(const FtArStepDesc& d, const FtArStepWeights& w, const float* me
     Plan pf; pf.base = static_cast<uint8_t*>(scratch);
     FwdScratch F; F.plan(pf, d);
 
-    // fp16 operand copies of the weights (61 M params -> ~0.1 ms; redone every call so optimizer updates are seen)
+    // fp16 operand copies of the weights (61 M params; redone every call so optimizer updates are seen)
     FT_TRY(launch_cast(w.attn_lstm_w_ih, 2, F.w.w_ih_a, 0, static_cast<long long>(G) * n.M, st));
     FT_TRY(launch_cast(w.attn_lstm_w_hh, 2, F.w.w_hh_a, 0, static_cast<long long>(G) * H, st));
     FT_TRY(launch_cast(w.lstm_w_ih0, 2, F.w.w_ih0, 0, static_cast<long long>(G) * n.D, st));
@@ -340,13 +341,11 @@ int ar_step_fwd(const FtArStepDesc& d, const FtArStepWeights& w, const float* me
 
     // Attention-LSTM / attention overlap (FT_ATT_OVERLAP = chunk length in steps, a multiple of 64; default 256, 0 disables; B <= 32 and
     // T >= chunk + 64): the attention LSTM runs as a 64-CTA recurrence in chunks; as soon as a chunk's h is there, a second stream
-    // runs that chunk's query projection, fused attention, gate logits and lstm layer 0's input projection on the 84 free SMs,
-    // underneath the next chunk's recurrence.  Only the last chunk's share of that work stays exposed (attention 0.95 ms + GEMMs
-    // 0.45 ms per flow were serial).  The 64-CTA kernel has no room for the folded 80-channel projection next to its 128 KB weight
-    // slice, so the projection is a per-chunk GEMM on a third stream, one chunk ahead.  Measured on B200, B=32, T=1000
-    // (r2 calls 12 / 30): chunks of 128 LOSE (53.1 vs 51.1 ms/step before the GEMM epilogue rewrite, 49.1 vs 48.6 after: every chunk
-    // boundary costs a kernel drain + launch + 128 KB weight reload on 64 SMs), chunks of 192 / 256 / 320 / 384 / 512 give
-    // 47.9 / 46.4 / 47.2 / 46.4 / 46.5 against 48.6 serial.
+    // runs that chunk's query projection, fused attention, gate logits and lstm layer 0's input projection on the SMs the 64-CTA
+    // recurrence leaves free,
+    // underneath the next chunk's recurrence.  Only the last chunk's share of that work stays exposed.  The 64-CTA kernel has no room for the folded 80-channel projection next to its 128 KB weight
+    // slice, so the projection is a per-chunk GEMM on a third stream, one chunk ahead.  Short chunks lose: every chunk
+    // boundary costs a kernel drain + launch + 128 KB weight reload on 64 SMs.
     static int att_chunk = -1;
     if (att_chunk < 0) { const char* e = getenv("FT_ATT_OVERLAP"); att_chunk = e ? atoi(e) : 256; if (att_chunk % 64) att_chunk = 0; }
     Pipe* pa = (att_chunk > 0 && F.X1 && n.B <= 32 && n.T >= att_chunk + 64) ? get_pipe(st) : nullptr;
@@ -410,7 +409,7 @@ int ar_step_fwd(const FtArStepDesc& d, const FtArStepWeights& w, const float* me
         xproj0_done = true;
     } else {
     // attention_lstm: the 80-channel input projection is folded into the persistent recurrence (no [R,4096] projection
-    // tensor: -0.5 ms GEMM, -1 GB of HBM traffic per flow); h lands in d16[:, 0:H].  FT_LSTM_XIN=0: separate GEMM (r1 path).
+    // tensor: one GEMM and 1 GB of HBM traffic less per flow); h lands in d16[:, 0:H].  FT_LSTM_XIN=0: separate GEMM.
     static int xin = -1;
     if (xin < 0) { const char* e = getenv("FT_LSTM_XIN"); xin = (!e || atoi(e) != 0) ? 1 : 0; }
     if (xin && n.M <= 128 && n.B <= 32) {      // B > 32: the double-buffered x tile no longer fits next to a 64-row h tile
@@ -688,7 +687,7 @@ int ar_step_bwd_attn(const FtArStepDesc& d, const FtArStepWeights& w, const int*
     }
 
     // deferred from ar_step_bwd_main: weight gradients of lstm layer 0 and of the attention projections, on the side stream,
-    // underneath the BPTT kernel below (64 of the 148 SMs)
+    // underneath the BPTT kernel below (64 of the SMs)
     ss = fork_side(sd, st);
     FT_TRY(gemm_wgrad(ss, G, H, Rm, F.dG0 + static_cast<size_t>(n.B) * G, G, S_.h0_16, H, g.lstm_w_hh0, H, iS));
     FT_TRY(gemm_wgrad(ss, G, n.D, R, F.dG0, G, S_.d16, n.D, g.lstm_w_ih0, n.D, iS));

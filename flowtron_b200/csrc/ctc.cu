@@ -13,7 +13,7 @@
 // frame t): the reference un-rolls and un-flips it (:250-256); here it is an index map.
 // Thread s owns state s; alpha_{t-1} / beta_{t+1} live in a double-buffered shared array (two leading / trailing -inf pads
 // make s-1, s-2 / s+1, s+2 unconditional); alpha for all t is parked in global scratch [T, S] per utterance and read back by
-// the SAME thread in the beta sweep.  One __syncthreads per time step; ~T * 0.2 us per launch, all utterances in parallel.
+// the SAME thread in the beta sweep.  One __syncthreads per time step, all utterances in parallel.
 #include <math_constants.h>
 
 #include "ft_internal.h"

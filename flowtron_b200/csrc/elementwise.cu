@@ -122,7 +122,7 @@ int launch_grad_scale(const float* a, long long na, const float* b, long long nb
     n = n > nc ? n : nc;
     if (n > 0) absmax_kernel<<<grid_for(n, 256, 4), 256, 0, st>>>(a, na, b, nb, c, nc, mx);
     // the attention-side external gradients (CTC loss path: d_attn, d_attn_logprob) are multiplied by the same S inside
-    // attn_bwd and their products are cast to fp16 too, so they take part in choosing S (ADVICE r1)
+    // attn_bwd and their products are cast to fp16 too, so they take part in choosing S
     const long long n2 = nd > ne ? nd : ne;
     if (n2 > 0 && (d || e)) absmax_kernel<<<grid_for(n2, 256, 4), 256, 0, st>>>(d, d ? nd : 0, e, e ? ne : 0, nullptr, 0, mx);
     scale_finalize_kernel<<<1, 1, 0, st>>>(mx, target, scale2);
@@ -238,8 +238,8 @@ __global__ void gate_bwd_kernel(const __half* __restrict__ d16, long long ldd, i
                                 float* __restrict__ dwg, float* __restrict__ dbg, const float* __restrict__ scale) {
     const float S = scale ? scale[0] : 1.f;      // dd lives in the loss-scaled domain, dwg / dbg do not
     // A block walks a slab of rows; thread t owns columns t, t+256, ... (<= GB_KJ of them): every row is one coalesced
-    // sweep with GB_KJ independent loads in flight per thread (the first version walked the rows per column: 0.44 ms
-    // for 0.5 GB of traffic, latency-bound).
+    // sweep with GB_KJ independent loads in flight per thread (walking the rows per column instead is
+    // latency-bound).
     constexpr int GB_KJ = 8;                          // K <= 2048 (checked by the launcher)
     const long long rows_per_block = (R + gridDim.x - 1) / gridDim.x;
     const long long r0 = blockIdx.x * rows_per_block, r1 = min(R, r0 + rows_per_block);

@@ -4,7 +4,7 @@
 //
 // Layout: every activation lives channels-last in ONE padded token grid  row(b, l) = b * (L + 4) + 2 + l  with two zero rows
 // on either side of an utterance, so
-//   * the k = 5 convolution is 5 accumulating tcgen05 GEMMs whose A operand is the SAME buffer shifted by k rows (no im2col,
+//   * the k = 5 convolution is 5 accumulating wgmma GEMMs whose A operand is the SAME buffer shifted by k rows (no im2col,
 //     no cuDNN layout transposes); its dgrad / wgrad are the same trick on the gradient grid;
 //   * the recurrence's h_{t-1} / h_{t+1} of the first / last token of an utterance is a zero pad row: no special cases.
 // The BiLSTM recurrences run as TWO CLUSTERS OF 8 CTAs (one per direction) in one launch: CTA r owns 32 hidden units, keeps
@@ -15,7 +15,7 @@
 // The backward recurrence is the mirror image: W_hh^T slices in registers, dG_t exchanged through the [rows, 1024] fp16
 // tensor the weight gradients are GEMMs over, fp32 cell-gradient carry in registers.
 // Precision: SPLIT fp16.  Plain fp16 operands (the flows' choice) measured 1.2-1.5e-3 on the encoder output and 3-5 % on the
-// encoder's small parameter gradients (r2 call 10) -- over the 1e-3 / 1e-2 bars, and the encoder feeds both flows.  So every
+// encoder's small parameter gradients -- over the 1e-3 / 1e-2 bars, and the encoder feeds both flows.  So every
 // tensor-core operand x is stored as hi = fp16(x), lo = fp16(x - hi) (22 significant bits) and every product is
 // hi*hi + lo*hi + hi*lo with fp32 accumulation.  For K-major operands that is ONE GEMM over a 3x longer contraction: activations
 // and gradients are stored as rows [hi | lo | hi], weights as [hi | hi | lo] (or row-stacked [hi ; hi ; lo] when the weight is

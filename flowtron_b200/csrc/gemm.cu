@@ -1,394 +1,9 @@
-// tcgen05 + TMA GEMM for sm_100a:  C[M,N] = act(alpha * A[M,K] * B[N,K]^T + bias (+bias2)) (+ C if beta)
-//
-//  * operands 16-bit (f16 / bf16, kind::f16, UMMA_K=16) or tf32 (fp32 storage, kind::tf32, UMMA_K=8), fp32 accumulation in
-//    TMEM; each operand may be K-major (row-major [rows, K]) or MN-major (row-major [K, rows], i.e. the transposed view of a
-//    natural activation / gradient tensor) -- this is what lets dW = dY^T X and dX = dY W run on the tensors exactly as the
-//    forward pass left them (no transposes anywhere);
-//  * persistent: one CTA per SM walks a static tile list; 4/6-stage TMA ring (SWIZZLE_128B), double-buffered TMEM
-//    accumulators, epilogue overlapped with the next tile's main loop, optional split-K (details at gemm2_kernel).
-//  * warp roles: w0 = TMA producer, w1 = TMEM alloc + single-thread MMA issue, w2..w5 = epilogue.
-//
-// Used for every non-recurrent contraction on the Flowtron hot path (LSTM input projections flowtron.py:654-655, attention
-// Q/K/V projections :568-571, DenseLayer :461-464, 1x1 conv :768, and all their dgrad/wgrad counterparts).
-// The round-1 kernel (non-persistent 128x128 tiles, 3 stages, 2 CTAs/SM) was measured against this one on the training step
-// (profiles/r2_c3_train_gemm_v1.json: 60.7 vs 60.3 ms/step, GEMM kernel time 19.0 vs 15.8 ms) and removed.
+// Host side of the GEMM (kernel: gemm_kernel.cuh): TMA descriptors, tile / split-K / cluster policy, launch.
 #include <cstdlib>
 
-#include "ptx.cuh"
-#include "ft_internal.h"
+#include "gemm_kernel.cuh"
 
 namespace ft {
-
-constexpr int BM = 128;
-constexpr int TILE_BYTES = BM * 128;               // A tile of one stage: 128 rows x 128 B (one SW128 row per matrix row)
-
-struct GemmParams {
-    int M, N, K;
-    int a_fmt, b_fmt;          // 0 f16, 1 bf16, 2 tf32
-    int a_mn, b_mn;            // 1 = operand given MN-major ([K, rows] row-major)
-    const float* bias;         // [N] or null
-    const float* bias2;        // [N] or null
-    int act;                   // 0 none, 1 tanh, 2 multiply by (1 - aux^2)  (tanh backward; aux = saved tanh output)
-    const __half* aux16; long long ldaux;
-    int beta;                  // 1: C32 += result (C32 read-modify-write)
-    float alpha;               // scale on the accumulator before bias
-    const float* alpha_ptr;    // optional device scalar multiplied into alpha (loss-scale undo)
-    float* C32; long long ldc32;
-    void* C16; long long ldc16; int c16_fmt;   // 0 f16, 1 bf16
-    int* status;
-    int tma_out = 0;           // 1: C32, 2: C16 leave through TMA stores of 32-row staging tiles (no beta / split-K), 0: per-lane stores
-    int dbg = 0;               // FT_GEMM_EPI_DEBUG (measurement only): 1 = epilogue reads TMEM but stores nothing, 2 = stores without reading TMEM, 3 = neither
-    int splitk = 1;            // v2 only: K is cut into `splitk` ranges, partial tiles are atomically added into a zeroed C32
-};
-
-// One CTA per SM walks a static list of 128 x BN output tiles (BN = 256, or 128 for narrow outputs):
-//   * a 4-stage (BN = 256: 48 KB per stage) / 6-stage (BN = 128) TMA ring feeds one elected thread issuing
-//     tcgen05.mma 128 x BN x 16: one stage is 512 (256) tensor-core clocks, so the ring covers ~2000 clocks of TMA latency
-//     (the 3-stage 128x128 ring of v1 covered 768: its K <= 1024 shapes ran at 24-43 % of peak), and a 128 x 256 tile reads
-//     96 B of shared memory per tensor-core clock instead of the 128 B (the SM's whole bandwidth) of a 128 x 128 tile;
-//   * TWO accumulators in TMEM (2 x BN columns): the four epilogue warps drain tile i while the MMA warp already
-//     accumulates tile i+1, so the epilogue (and the per-CTA start-up v1 paid on every tile) leaves the critical path;
-//   * epilogue: tcgen05.ld 32 columns -> a 32x36 shared-memory transpose per warp -> float4 per lane, 4 rows x 128 contiguous
-//     bytes per warp instruction, all loads of a chunk hoisted in front of the arithmetic (details at the epilogue).
-constexpr int G2_THREADS = 320;                                 // w0 TMA producer, w1 MMA issuer, w2..w9 epilogue (two per TMEM lane quadrant)
-constexpr int G2_EPI_WARPS = 8;
-constexpr int G2_OUT_TILE = 32 * 128;                          // output staging tile: 32 rows x 128 bytes (32 fp32 or 64 16-bit columns)
-constexpr int G2_PITCH = 36;                                   // floats: 16-byte aligned rows, conflict-free float4 access
-constexpr int G2_STAGE_FLOATS = 32 * G2_PITCH;                 // per-warp transpose tile
-// NCTA = 2 (BN = 256 only): a CTA PAIR (2-CTA cluster, tcgen05 cta_group::2) owns a 256 x 256 tile.  Each CTA stages its own 128
-// rows of A and HALF of B's 256 rows (32 KB per stage instead of 48: 6 stages), the leader issues 256 x 256 x 16 MMAs that read A
-// from both CTAs' shared memory and the two B halves, each CTA's 128 accumulator rows land in its own TMEM and are drained by its
-// own epilogue warps.  Operand bytes per FLOP drop by 1.5x (the 128 x 256 tile is L2->SM bound: 87 FLOP per operand byte).
-template <int BN_, int NCTA = 1> struct G2Cfg {
-    static constexpr int STAGE_BYTES = (BM + BN_ / NCTA) * 128;
-    static constexpr int STAGES = (BN_ == 256 && NCTA == 1) ? 4 : 6;
-    static constexpr int SMEM = STAGES * STAGE_BYTES + G2_EPI_WARPS * G2_OUT_TILE + 256 + 1024;     // + one 4 KB output staging tile per epilogue warp
-};
-
-template <bool kTf32, int BN_, int NCTA = 1>
-__global__ void __launch_bounds__(G2_THREADS, 1)
-gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmC,
-             GemmParams p, int tiles_n, int n_tiles) {
-    using C = G2Cfg<BN_, NCTA>;
-    constexpr int TM = BM * NCTA;                   // rows of a work item's tile
-    const int rank = NCTA == 2 ? static_cast<int>(cluster_ctarank()) : 0;
-    const int wid0 = NCTA == 2 ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);
-    const int wstep = NCTA == 2 ? static_cast<int>(gridDim.x >> 1) : static_cast<int>(gridDim.x);
-    constexpr int ST = C::STAGES;
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t* out_stage = smem + ST * C::STAGE_BYTES;              // [8 epilogue warps][G2_OUT_TILE] (1024-byte aligned)
-    uint64_t* bars = reinterpret_cast<uint64_t*>(out_stage + G2_EPI_WARPS * G2_OUT_TILE);
-    uint64_t* full = bars;                 // [ST]
-    uint64_t* empty = bars + ST;           // [ST]
-    uint64_t* tfull = bars + 2 * ST;       // [2] accumulator ready
-    uint64_t* tempty = bars + 2 * ST + 2;  // [2] accumulator drained (one arrival per epilogue warp of the pair / CTA)
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * ST + 4);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    constexpr int ELT = kTf32 ? 4 : 2;
-    constexpr int BK = 128 / ELT;
-    constexpr int UK = 32 / ELT;
-    const int num_kb_all = (p.K + BK - 1) / BK;
-    const int kb_per_split = (num_kb_all + p.splitk - 1) / p.splitk;     // work item w = split * n_tiles + tile
-    const int n_work = n_tiles * p.splitk;
-
-    if (warp == 0 && lane == 0) {
-        tma_prefetch_desc(&tmA);
-        tma_prefetch_desc(&tmB);
-        if (p.tma_out) tma_prefetch_desc(&tmC);
-        for (int s = 0; s < ST; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        mbar_init(&tfull[0], 1); mbar_init(&tfull[1], 1);
-        mbar_init(&tempty[0], G2_EPI_WARPS * NCTA); mbar_init(&tempty[1], G2_EPI_WARPS * NCTA);
-        fence_mbar_init();
-    }
-    if (NCTA == 2) cluster_sync_all();              // the peer's barriers exist before anything can arrive on them
-    if (warp == 1) { if (NCTA == 2) tmem_alloc_pair<2 * BN_>(tmem_slot); else tmem_alloc<2 * BN_>(tmem_slot); }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp == 0) {
-        // ------------------------------------------------ TMA producer (warp-uniform loop, one elected lane issues)
-        int it = 0;
-        auto ld = [&](void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
-            if (NCTA == 2) tma_load_2d_pair(dst, m, bar, c0, c1); else tma_load_2d(dst, m, bar, c0, c1);
-        };
-        constexpr int BNC = BN_ / NCTA;             // B rows this CTA stages
-        for (int w = wid0; w < n_work; w += wstep) {
-            const int split = w / n_tiles, tile = w - split * n_tiles;
-            const int tile_m = tile / tiles_n, tile_n = tile - tile_m * tiles_n;
-            const int kb0 = split * kb_per_split, kb1 = min(num_kb_all, kb0 + kb_per_split);
-            const int am = tile_m * TM + rank * BM, bn = tile_n * BN_ + rank * BNC;
-            for (int kb = kb0; kb < kb1; ++kb, ++it) {
-                const int s = it % ST, ph = (it / ST) & 1;
-                mbar_wait(&empty[s], ph ^ 1, p.status, 111);
-                uint8_t* a = smem + s * C::STAGE_BYTES;
-                uint8_t* b = a + TILE_BYTES;
-                if (elect_one()) {
-                    if (rank == 0) mbar_expect_tx(&full[s], C::STAGE_BYTES * NCTA);     // the pair's bytes land on the leader's barrier
-                    if (!p.a_mn) {
-                        ld(a, &tmA, &full[s], kb * BK, am);
-                    } else {
-#pragma unroll
-                        for (int j = 0; j < BM / BK; ++j)
-                            ld(a + j * (BK * 128), &tmA, &full[s], am + j * BK, kb * BK);
-                    }
-                    if (!p.b_mn) {
-                        ld(b, &tmB, &full[s], kb * BK, bn);
-                    } else {
-#pragma unroll
-                        for (int j = 0; j < BNC / BK; ++j)
-                            ld(b + j * (BK * 128), &tmB, &full[s], bn + j * BK, kb * BK);
-                    }
-                }
-                __syncwarp();
-            }
-        }
-    } else if (warp == 1 && rank == 0) {
-        // ------------------------------------------------ MMA issuer (the pair's leader only)
-        const uint32_t idesc = umma_idesc(TM, BN_, p.a_fmt, p.b_fmt, p.a_mn, p.b_mn);
-        const uint32_t tmem_d0 = __shfl_sync(0xffffffffu, tmem_base, 0);
-        const uint64_t da0 = p.a_mn ? umma_smem_desc(smem_u32(smem), BK * 128, 1024) : umma_smem_desc(smem_u32(smem), 16, 1024);
-        const uint64_t db0 = p.b_mn ? umma_smem_desc(smem_u32(smem + TILE_BYTES), BK * 128, 1024)
-                                    : umma_smem_desc(smem_u32(smem + TILE_BYTES), 16, 1024);
-        const uint64_t ka = p.a_mn ? (UK * 128) >> 4 : 2, kbs = p.b_mn ? (UK * 128) >> 4 : 2;
-        int it = 0, tc = 0;
-        for (int w = wid0; w < n_work; w += wstep, ++tc) {
-            const int split = w / n_tiles;
-            const int kb0 = split * kb_per_split, kb1 = min(num_kb_all, kb0 + kb_per_split);
-            const int buf = tc & 1, bph = (tc >> 1) & 1;
-            mbar_wait(&tempty[buf], bph ^ 1, p.status, 112);          // the epilogue(s) drained this accumulator (first use: free)
-            tc_fence_after();
-            const uint32_t tmem_d = tmem_d0 + buf * BN_;
-            for (int kb = kb0; kb < kb1; ++kb, ++it) {
-                const int s = it % ST, ph = (it / ST) & 1;
-                mbar_wait(&full[s], ph, p.status, 113);
-                tc_fence_after();
-                const uint64_t so = static_cast<uint64_t>(s) * (C::STAGE_BYTES >> 4);
-                const uint64_t da = da0 + so, db = db0 + so;
-                if (elect_one()) {
-#pragma unroll
-                    for (int k = 0; k < BK / UK; ++k) {
-                        const uint32_t acc = ((kb - kb0) | k) != 0;
-                        if (NCTA == 2) {
-                            if (kTf32) umma_tf32_pair(tmem_d, da + k * ka, db + k * kbs, idesc, acc);
-                            else       umma_f16_pair(tmem_d, da + k * ka, db + k * kbs, idesc, acc);
-                        } else {
-                            if (kTf32) umma_tf32(tmem_d, da + k * ka, db + k * kbs, idesc, acc);
-                            else       umma_f16(tmem_d, da + k * ka, db + k * kbs, idesc, acc);
-                        }
-                    }
-                    if (NCTA == 2) { umma_commit_pair(&empty[s]); if (kb == kb1 - 1) umma_commit_pair(&tfull[buf]); }
-                    else           { umma_commit(&empty[s]); if (kb == kb1 - 1) umma_commit(&tfull[buf]); }
-                }
-                __syncwarp();
-            }
-        }
-    } else if (warp >= 2) {
-        // ------------------------------------------------ epilogue warps (TMEM lane quadrant = warp % 4)
-        // Row per lane, straight from the accumulator: tcgen05.ld hands lane i row (32 q + i) x 32 consecutive columns, so the
-        // lane applies alpha / bias / activation / beta and writes its own 128 contiguous bytes with eight 16-byte stores
-        // (16-bit outputs: four 8-byte stores; the tanh' operand and the beta read come in with matching 8 / 16-byte loads, all
-        // issued before the arithmetic).  ~60 instructions per 32-column chunk and warp.  The r2 form transposed every chunk
-        // through shared memory to get 512-byte-contiguous warp stores: ~780 instructions per chunk (ncu, call 16: 24.9 k
-        // warp-instructions per 128 x 256 tile, one epilogue warp per scheduler at 0.17 IPC = 19 us per tile), which made every
-        // GEMM with K < ~3000 epilogue-bound: 32000 x 4096 x 1664 ran at 54 % of the tensor peak, 32000 x 1024 x 1024 at 31 %,
-        // while K = 4096 / 32000 shapes reached 78-90 %.  A warp store now touches 32 rows (32 L2 requests of 16 bytes instead of
-        // 4 of 128), which the LSU absorbs in ~2 k clocks per tile and warp, far below the main loop's 21 k.
-        // Eight epilogue warps, two per TMEM lane quadrant (q = warp % 4), alternate over the tile's 32-column chunks (pairs of
-        // chunks for 16-bit TMA output tiles): with one warp per scheduler the epilogue was bound by its own dependent-instruction
-        // latency (0.17 IPC per scheduler; r2 call 20: 32000 x 1024 x 1024 + tanh took 0.100 ms even with the stores removed,
-        // 0.048 ms with the arithmetic removed too).
-        const int q = warp & 3, hw = (warp - 2) >> 2;
-        const float alpha = p.alpha_ptr ? p.alpha * __ldg(p.alpha_ptr) : p.alpha;
-        const bool vec_ok = (p.N % 4 == 0) &&
-                            (!p.C32 || (((reinterpret_cast<uintptr_t>(p.C32) & 15) == 0) && (p.ldc32 % 4 == 0))) &&
-                            (!p.C16 || (((reinterpret_cast<uintptr_t>(p.C16) & 7) == 0) && (p.ldc16 % 4 == 0))) &&
-                            (p.act != 2 || (((reinterpret_cast<uintptr_t>(p.aux16) & 7) == 0) && (p.ldaux % 4 == 0))) &&
-                            (!p.bias || (reinterpret_cast<uintptr_t>(p.bias) & 15) == 0) && (!p.bias2 || (reinterpret_cast<uintptr_t>(p.bias2) & 15) == 0);
-        int tc = 0;
-        for (int w = wid0; w < n_work; w += wstep, ++tc) {
-            const int tile = w % n_tiles;
-            const int tile_m = tile / tiles_n, tile_n = tile - tile_m * tiles_n;
-            const int buf = tc & 1, bph = (tc >> 1) & 1;
-            mbar_wait(&tfull[buf], bph, p.status, 114);
-            tc_fence_after();
-            const int ncols = min(BN_, p.N - tile_n * BN_);
-            const long long m = static_cast<long long>(tile_m) * TM + rank * BM + q * 32 + lane;      // this lane's output row
-            const bool row_ok = m < p.M;
-            const int nchunks = (ncols + 31) >> 5;
-            const int gsz = p.tma_out == 2 ? 2 : 1;                   // chunks per group (this warp takes groups hw, hw + 2, ...)
-            const int ngroups = (nchunks + gsz - 1) / gsz;
-            int my_last = -1;                                         // the last chunk THIS warp reads from the accumulator
-            if (ngroups > hw) { const int gl = hw + 2 * ((ngroups - 1 - hw) / 2); my_last = min(nchunks, (gl + 1) * gsz) - 1; }
-#pragma unroll 1
-            for (int cc = 0; cc < nchunks; ++cc) {
-                if (((cc / gsz) & 1) != hw) continue;
-                const int c = cc;
-                float v[32];
-                if (p.dbg == 2 || p.dbg == 3) {
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) v[j] = 1.f;
-                } else {
-                    tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + buf * BN_ + c * 32, v);
-                    tmem_ld_wait();
-                }
-                if (c == my_last) {                                  // everything this warp needs is in registers: hand the
-                    tc_fence_before();                               // accumulator back to the MMA warp before the stores
-                    if (lane == 0) { if (NCTA == 2) mbar_arrive_pair_leader(&tempty[buf]); else mbar_arrive(&tempty[buf]); }
-                }
-                const int nb = tile_n * BN_ + c * 32;                 // first column of the chunk
-                const int nv = min(32, ncols - c * 32);               // valid columns of the chunk
-                if (p.tma_out && (p.dbg == 0 || p.dbg >= 4)) {
-                    // ---- TMA-store path (r2 call 18: with per-lane OR 512-byte-coalesced register stores every GEMM with K < ~3000
-                    // was STORE-bound -- 4 epilogue warps x a handful of outstanding stores each x ~1 us write latency = 3.4 B/clk/SM:
-                    // 32000 x 4096 x 1664 ran 0.56 ms with stores and 0.29 ms (1516 TFLOP/s) without).  The lane converts its row
-                    // segment, writes it into a SWIZZLE_128B staging tile (16-byte piece j of row i at piece j ^ (i & 7): conflict-free),
-                    // and one lane hands the 4 KB tile to the TMA engine; two tiles per warp alternate.
-                    const bool f32out = p.tma_out == 1;
-                    const int sub = f32out ? 0 : (c & 1);             // 16-bit outputs: two 32-column chunks share a 64-column tile
-                    uint8_t* tile_s = out_stage + (warp - 2) * G2_OUT_TILE;
-                    if (sub == 0 && p.dbg != 4 && p.dbg < 5) {         // the tile's previous store must have read it (fast: measured free)
-                        if (lane == 0) bulk_wait_read<0>();
-                        __syncwarp();
-                    }
-                    uint2 aux[8];
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        aux[j] = make_uint2(0u, 0u);
-                        if (p.act == 2 && row_ok && 4 * j < nv) aux[j] = *reinterpret_cast<const uint2*>(p.aux16 + m * p.ldaux + nb + 4 * j);
-                    }
-                    uint8_t* row_s = tile_s + lane * 128;
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        const int n = nb + 4 * j;
-                        float4 bsum = make_float4(0.f, 0.f, 0.f, 0.f);
-                        if (4 * j < nv) {
-                            if (p.bias) bsum = __ldg(reinterpret_cast<const float4*>(p.bias + n));
-                            if (p.bias2) { const float4 t = __ldg(reinterpret_cast<const float4*>(p.bias2 + n)); bsum.x += t.x; bsum.y += t.y; bsum.z += t.z; bsum.w += t.w; }
-                        }
-                        float x[4] = {fmaf(v[4 * j], alpha, bsum.x), fmaf(v[4 * j + 1], alpha, bsum.y), fmaf(v[4 * j + 2], alpha, bsum.z), fmaf(v[4 * j + 3], alpha, bsum.w)};
-                        if (p.act == 1) {
-#pragma unroll
-                            for (int e = 0; e < 4; ++e) x[e] = tanh_f(x[e]);
-                        } else if (p.act == 2) {
-                            const __half2* h = reinterpret_cast<const __half2*>(&aux[j]);
-                            const float2 y0 = __half22float2(h[0]), y1 = __half22float2(h[1]);
-                            x[0] *= (1.f - y0.x * y0.x); x[1] *= (1.f - y0.y * y0.y); x[2] *= (1.f - y1.x * y1.x); x[3] *= (1.f - y1.y * y1.y);
-                        }
-                        if (f32out) {
-                            *reinterpret_cast<float4*>(row_s + ((j ^ (lane & 7)) << 4)) = make_float4(x[0], x[1], x[2], x[3]);
-                        } else {
-                            uint2 pk;
-                            if (p.c16_fmt == 0) {
-                                const __half2 h0 = __floats2half2_rn(fminf(fmaxf(x[0], -65504.f), 65504.f), fminf(fmaxf(x[1], -65504.f), 65504.f));
-                                const __half2 h1 = __floats2half2_rn(fminf(fmaxf(x[2], -65504.f), 65504.f), fminf(fmaxf(x[3], -65504.f), 65504.f));
-                                pk.x = *reinterpret_cast<const uint32_t*>(&h0); pk.y = *reinterpret_cast<const uint32_t*>(&h1);
-                            } else {
-                                const __nv_bfloat162 h0 = __floats2bfloat162_rn(x[0], x[1]), h1 = __floats2bfloat162_rn(x[2], x[3]);
-                                pk.x = *reinterpret_cast<const uint32_t*>(&h0); pk.y = *reinterpret_cast<const uint32_t*>(&h1);
-                            }
-                            // 8-byte piece j of this chunk = half of 16-byte piece (4 sub + j / 2) of the 64-column row
-                            *reinterpret_cast<uint2*>(row_s + (((4 * sub + (j >> 1)) ^ (lane & 7)) << 4) + ((j & 1) << 3)) = pk;
-                        }
-                    }
-                    if (f32out || sub == 1 || c == nchunks - 1) {
-                        if (p.dbg < 6) fence_proxy_async_smem();
-                        __syncwarp();
-                        if (lane == 0 && p.dbg < 5) {
-                            tma_store_2d(&tmC, tile_s, f32out ? nb : nb - 32 * sub, static_cast<int>(m - lane));
-                            bulk_commit();
-                        }
-                    }
-                } else if (p.dbg == 1 || p.dbg == 3) {                // measurement only: keep the loads alive, store nothing
-                    float sacc = 0.f;
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) sacc += v[j];
-                    if (sacc == 1.2345e-30f && p.C32) p.C32[0] = sacc;
-                } else if (vec_ok) {
-                    uint2 aux[8];
-                    float4 old[8];
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        aux[j] = make_uint2(0u, 0u);
-                        old[j] = make_float4(0.f, 0.f, 0.f, 0.f);
-                        if (row_ok && 4 * j < nv) {
-                            if (p.act == 2) aux[j] = *reinterpret_cast<const uint2*>(p.aux16 + m * p.ldaux + nb + 4 * j);
-                            if (p.beta && p.C32) old[j] = *reinterpret_cast<const float4*>(p.C32 + m * p.ldc32 + nb + 4 * j);
-                        }
-                    }
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        if (4 * j < nv) {                              // N % 4 == 0: a 4-group is in or out as a whole
-                            const int n = nb + 4 * j;
-                            float4 bsum = make_float4(0.f, 0.f, 0.f, 0.f);
-                            if (p.bias) bsum = __ldg(reinterpret_cast<const float4*>(p.bias + n));
-                            if (p.bias2) { const float4 t = __ldg(reinterpret_cast<const float4*>(p.bias2 + n)); bsum.x += t.x; bsum.y += t.y; bsum.z += t.z; bsum.w += t.w; }
-                            float x[4] = {fmaf(v[4 * j], alpha, bsum.x), fmaf(v[4 * j + 1], alpha, bsum.y), fmaf(v[4 * j + 2], alpha, bsum.z), fmaf(v[4 * j + 3], alpha, bsum.w)};
-                            if (p.act == 1) {
-#pragma unroll
-                                for (int e = 0; e < 4; ++e) x[e] = tanh_f(x[e]);
-                            } else if (p.act == 2) {
-                                const __half2* h = reinterpret_cast<const __half2*>(&aux[j]);
-                                const float2 y0 = __half22float2(h[0]), y1 = __half22float2(h[1]);
-                                x[0] *= (1.f - y0.x * y0.x); x[1] *= (1.f - y0.y * y0.y); x[2] *= (1.f - y1.x * y1.x); x[3] *= (1.f - y1.y * y1.y);
-                            }
-                            if (p.beta) { x[0] += old[j].x; x[1] += old[j].y; x[2] += old[j].z; x[3] += old[j].w; }
-                            if (row_ok) {
-                                if (p.C32) {
-                                    if (p.splitk > 1) atomicAdd(reinterpret_cast<float4*>(p.C32 + m * p.ldc32 + n), make_float4(x[0], x[1], x[2], x[3]));
-                                    else *reinterpret_cast<float4*>(p.C32 + m * p.ldc32 + n) = make_float4(x[0], x[1], x[2], x[3]);
-                                }
-                                if (p.C16) {
-                                    uint2 pk;
-                                    if (p.c16_fmt == 0) {      // fp16: saturate instead of overflowing to inf
-                                        const __half2 h0 = __floats2half2_rn(fminf(fmaxf(x[0], -65504.f), 65504.f), fminf(fmaxf(x[1], -65504.f), 65504.f));
-                                        const __half2 h1 = __floats2half2_rn(fminf(fmaxf(x[2], -65504.f), 65504.f), fminf(fmaxf(x[3], -65504.f), 65504.f));
-                                        pk.x = *reinterpret_cast<const uint32_t*>(&h0); pk.y = *reinterpret_cast<const uint32_t*>(&h1);
-                                    } else {
-                                        const __nv_bfloat162 h0 = __floats2bfloat162_rn(x[0], x[1]), h1 = __floats2bfloat162_rn(x[2], x[3]);
-                                        pk.x = *reinterpret_cast<const uint32_t*>(&h0); pk.y = *reinterpret_cast<const uint32_t*>(&h1);
-                                    }
-                                    *reinterpret_cast<uint2*>(reinterpret_cast<uint16_t*>(p.C16) + m * p.ldc16 + n) = pk;
-                                }
-                            }
-                        }
-                    }
-                } else {
-                    // unaligned / N % 4 != 0 outputs: scalar walk over the lane's row (rare: no shape on the hot path)
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) {                   // fully unrolled: v[] must stay in registers
-                        const int n = nb + j;
-                        if (j < nv) {
-                            float x = fmaf(v[j], alpha, (p.bias ? __ldg(p.bias + n) : 0.f) + (p.bias2 ? __ldg(p.bias2 + n) : 0.f));
-                            if (p.act == 1) x = tanh_f(x);
-                            if (row_ok) {
-                                if (p.act == 2) { const float y = __half2float(p.aux16[m * p.ldaux + n]); x *= (1.f - y * y); }
-                                if (p.C32) {
-                                    float* dst = p.C32 + m * p.ldc32 + n;
-                                    if (p.splitk > 1) atomicAdd(dst, x);
-                                    else { if (p.beta) x += *dst; *dst = x; }
-                                }
-                                if (p.C16) {
-                                    if (p.c16_fmt == 0) reinterpret_cast<__half*>(p.C16)[m * p.ldc16 + n] = __float2half_rn(fminf(fmaxf(x, -65504.f), 65504.f));
-                                    else reinterpret_cast<__nv_bfloat16*>(p.C16)[m * p.ldc16 + n] = __float2bfloat16_rn(x);
-                                }
-                            }
-                        }
-                    }
-                }
-            }
-            if (my_last < 0) { tc_fence_before(); if (lane == 0) { if (NCTA == 2) mbar_arrive_pair_leader(&tempty[buf]); else mbar_arrive(&tempty[buf]); } }
-        }
-        if (p.tma_out && lane == 0) bulk_wait_all();      // the staging tiles must outlive their stores
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (NCTA == 2) cluster_sync_all();              // both CTAs are done with the pair's TMEM and with each other's shared memory
-    if (warp == 1) { if (NCTA == 2) tmem_dealloc_pair<2 * BN_>(tmem_base); else tmem_dealloc<2 * BN_>(tmem_base); }
-}
 
 // ------------------------------------------------------------------------------------------------ host
 static PFN_encodeTiled g_encode = nullptr;
@@ -428,125 +43,88 @@ int make_tmap_2d(CUtensorMap* out, const void* ptr, int fmt, long long rows, lon
 static int g_pair_mode = -1;        // 0 never, 1 big contractions only, 2 whenever eligible
 void set_gemm_pair_mode(int mode) { g_pair_mode = mode; }
 
+extern template const void* gemm_kernel_ptr<FMT_F16, 0>(int, int, int);
+extern template const void* gemm_kernel_ptr<FMT_F16, 1>(int, int, int);
+extern template const void* gemm_kernel_ptr<FMT_BF16, 0>(int, int, int);
+extern template const void* gemm_kernel_ptr<FMT_BF16, 1>(int, int, int);
+extern template const void* gemm_kernel_ptr<FMT_TF32, 0>(int, int, int);
+
 int launch_gemm(const GemmArgs& g, cudaStream_t st) {
     if (g.M <= 0 || g.N <= 0 || g.K <= 0) return 0;
     const bool tf32 = (g.a_fmt == 2);
     if ((g.a_fmt == 2) != (g.b_fmt == 2)) return ft_set_error("gemm: tf32 must be used for both operands");
+    if (!tf32 && g.a_fmt != g.b_fmt) return ft_set_error("gemm: both 16-bit operands must have the same format");
     if (tf32 && (g.a_mn || g.b_mn)) return ft_set_error("gemm: MN-major tf32 operands not supported");
     const int elt = tf32 ? 4 : 2, BK = 128 / elt;
     CUtensorMap tmA, tmB;
+    GemmParams p;
+    p.M = g.M; p.N = g.N; p.K = g.K;
+    p.bias = g.bias; p.bias2 = g.bias2; p.act = g.act; p.alpha_ptr = g.alpha_ptr; p.aux16 = static_cast<const __half*>(g.aux16); p.ldaux = g.ldaux; p.beta = g.beta; p.alpha = g.alpha;
+    p.C32 = g.C32; p.ldc32 = g.ldc32; p.C16 = g.C16; p.ldc16 = g.ldc16; p.c16_fmt = g.c16_fmt;
+    p.status = ft_status_word();
+    static int sms = 0;
+    if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); }
+    bool wide = (g.N % 256 == 0) || g.N > 1024;
+    if (wide && static_cast<long long>((g.N + 255) / 256) * ((g.M + BM - 1) / BM) < sms) wide = false;   // few tiles: prefer more CTAs
+    const int bn = wide ? 256 : 128;
+    const int tiles_n = (g.N + bn - 1) / bn, tiles_m = (g.M + BM - 1) / BM;
+    const long long n_tiles_ll = static_cast<long long>(tiles_n) * tiles_m;
+    if (n_tiles_ll > 0x7fffffff) return ft_set_error("gemm: too many tiles");
+    int n_tiles = static_cast<int>(n_tiles_ll);
+    // split-K: long reductions with few output tiles (the dense / projection weight gradients: K = T*B rows, 8-64 tiles)
+    // would leave most SMs idle; each K range is reduced by its own CTA and added atomically into a zeroed C32
+    const int num_kb_all = (g.K + BK - 1) / BK;
+    int splitk = 1;
+    const bool splittable = g.C32 && !g.C16 && !g.beta && !g.bias && !g.bias2 && g.act == 0 && (g.N % 4 == 0) &&
+                            g.ldc32 == g.N && ((reinterpret_cast<uintptr_t>(g.C32) & 15) == 0);
+    if (splittable && n_tiles * 2 <= sms && num_kb_all >= 64) {
+        splitk = sms / n_tiles;
+        if (splitk > 16) splitk = 16;
+        while (splitk > 1 && num_kb_all / splitk < 16) --splitk;
+    }
+    if (splitk > 1) {
+        if (cudaMemsetAsync(g.C32, 0, sizeof(float) * static_cast<size_t>(g.M) * g.N, st) != cudaSuccess) return ft_set_error("gemm: memset failed");
+    }
+    p.splitk = splitk;
+    // 2-CTA clusters (B multicast) for wide outputs with enough 256 x 256 tiles to fill the machine.  Mode 1 (default;
+    // FT_GEMM_2CTA / ft_set_gemm_pair_mode override): only for the big contractions (>= 1e11 FLOP).  Mode 2: whenever eligible.
+    if (g_pair_mode < 0) { const char* e = getenv("FT_GEMM_2CTA"); g_pair_mode = e ? atoi(e) : 1; }
+    const long long tiles_m2 = (g.M + 2 * BM - 1) / (2 * BM);
+    const bool big = 2.0 * g.M * g.N * g.K >= 1e11;
+    const int ncta = ((g_pair_mode == 2 || (g_pair_mode == 1 && big)) && wide && splitk == 1 && tiles_m2 * tiles_n >= sms / 2) ? 2 : 1;
     int rc;
     if (!g.a_mn) rc = make_tmap_2d(&tmA, g.A, g.a_fmt, g.M, g.K, g.lda, BK, BM);
     else         rc = make_tmap_2d(&tmA, g.A, g.a_fmt, g.K, g.M, g.lda, BK, BK);
     if (rc) return rc;
-    if (!g.b_mn) rc = make_tmap_2d(&tmB, g.B, g.b_fmt, g.N, g.K, g.ldb, BK, 128);
+    if (!g.b_mn) rc = make_tmap_2d(&tmB, g.B, g.b_fmt, g.N, g.K, g.ldb, BK, bn / ncta);     // each CTA of a pair fetches half of B
     else         rc = make_tmap_2d(&tmB, g.B, g.b_fmt, g.K, g.N, g.ldb, BK, BK);
     if (rc) return rc;
-    GemmParams p;
-    p.M = g.M; p.N = g.N; p.K = g.K; p.a_fmt = g.a_fmt; p.b_fmt = g.b_fmt; p.a_mn = g.a_mn; p.b_mn = g.b_mn;
-    p.bias = g.bias; p.bias2 = g.bias2; p.act = g.act; p.alpha_ptr = g.alpha_ptr; p.aux16 = static_cast<const __half*>(g.aux16); p.ldaux = g.ldaux; p.beta = g.beta; p.alpha = g.alpha;
-    p.C32 = g.C32; p.ldc32 = g.ldc32; p.C16 = g.C16; p.ldc16 = g.ldc16; p.c16_fmt = g.c16_fmt;
-    p.status = ft_status_word();
-    // output through TMA stores when there is exactly one output tensor, nothing is accumulated into it and it is TMA-addressable
-    CUtensorMap tmC = tmA;
-    {
-        static int tma_env = -1;
-        if (tma_env < 0) { const char* e = getenv("FT_GEMM_TMA_STORE"); tma_env = (!e || atoi(e) != 0) ? 1 : 0; }
-        const bool one = (g.C32 != nullptr) != (g.C16 != nullptr);
-        const bool plain = !g.beta && (g.N % 4 == 0) && (!g.bias || (reinterpret_cast<uintptr_t>(g.bias) & 15) == 0) &&
-                           (!g.bias2 || (reinterpret_cast<uintptr_t>(g.bias2) & 15) == 0) &&
-                           (g.act != 2 || (((reinterpret_cast<uintptr_t>(g.aux16) & 7) == 0) && (g.ldaux % 4 == 0)));
-        if (tma_env && one && plain) {
-            const void* cp = g.C32 ? static_cast<const void*>(g.C32) : g.C16;
-            const long long ldc = g.C32 ? g.ldc32 : g.ldc16;
-            const int elt_c = g.C32 ? 4 : 2;
-            if ((reinterpret_cast<uintptr_t>(cp) & 15) == 0 && ((ldc * elt_c) & 15) == 0) {
-                const int fmt_c = g.C32 ? 2 : g.c16_fmt;
-                if (make_tmap_2d(&tmC, cp, fmt_c, g.M, g.N, ldc, 128 / elt_c, 32)) return -1;
-                p.tma_out = g.C32 ? 1 : 2;
-            }
-        }
+    if (ncta == 2) n_tiles = static_cast<int>(tiles_m2 * tiles_n);
+    const long long n_work = static_cast<long long>(n_tiles) * splitk;
+    const int units = ncta == 2 ? sms / 2 : sms;
+    const int grid = ncta * static_cast<int>(n_work < units ? n_work : units);
+    const int smem = bn == 256 ? G2Cfg<256>::SMEM : G2Cfg<128>::SMEM;
+    const void* fn = g.a_fmt == FMT_TF32 ? gemm_kernel_ptr<FMT_TF32, 0>(bn, ncta, 0)
+                   : g.a_fmt == FMT_BF16 ? (g.a_mn ? gemm_kernel_ptr<FMT_BF16, 1>(bn, ncta, g.b_mn) : gemm_kernel_ptr<FMT_BF16, 0>(bn, ncta, g.b_mn))
+                                         : (g.a_mn ? gemm_kernel_ptr<FMT_F16, 1>(bn, ncta, g.b_mn) : gemm_kernel_ptr<FMT_F16, 0>(bn, ncta, g.b_mn));
+    static bool attr_set[3][2][2][2][2] = {};
+    bool& done = attr_set[g.a_fmt][bn == 256][ncta - 1][g.a_mn][g.b_mn];
+    if (!done) {
+        if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) return ft_set_error("gemm: shared-memory opt-in failed");
+        done = true;
     }
-    { static int dbg = -1; if (dbg < 0) { const char* e = getenv("FT_GEMM_EPI_DEBUG"); dbg = e ? atoi(e) : 0; } p.dbg = dbg; }
-    {
-        static int sms = 0;
-        if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); }
-        bool wide = (g.N % 256 == 0) || g.N > 1024;
-        if (wide && static_cast<long long>((g.N + 255) / 256) * ((g.M + BM - 1) / BM) < sms) wide = false;   // few tiles: prefer more CTAs
-        const int bn = wide ? 256 : 128;
-        const int tiles_n = (g.N + bn - 1) / bn, tiles_m = (g.M + BM - 1) / BM;
-        const long long n_tiles_ll = static_cast<long long>(tiles_n) * tiles_m;
-        if (n_tiles_ll > 0x7fffffff) return ft_set_error("gemm: too many tiles");
-        const int n_tiles = static_cast<int>(n_tiles_ll);
-        // split-K: long reductions with few output tiles (the dense / projection weight gradients: K = T*B rows, 8-64 tiles)
-        // would leave most SMs idle; each K range is reduced by its own CTA and added atomically into a zeroed C32
-        const int num_kb_all = (g.K + BK - 1) / BK;
-        int splitk = 1;
-        const bool splittable = g.C32 && !g.C16 && !g.beta && !g.bias && !g.bias2 && g.act == 0 && (g.N % 4 == 0) &&
-                                g.ldc32 == g.N && ((reinterpret_cast<uintptr_t>(g.C32) & 15) == 0);
-        if (splittable && n_tiles * 2 <= sms && num_kb_all >= 64) {
-            splitk = sms / n_tiles;
-            if (splitk > 16) splitk = 16;
-            while (splitk > 1 && num_kb_all / splitk < 16) --splitk;
-        }
-        if (splitk > 1) p.tma_out = 0;              // partial tiles are added atomically
-        if (splitk > 1) {
-            if (cudaMemsetAsync(g.C32, 0, sizeof(float) * static_cast<size_t>(g.M) * g.N, st) != cudaSuccess) return ft_set_error("gemm: memset failed");
-        }
-        p.splitk = splitk;
-        // CTA pairs for wide outputs with enough 256 x 256 tiles to fill the machine.  Mode 1 (default; FT_GEMM_2CTA / ft_set_gemm_pair_mode
-        // override): only for the big contractions (>= 1e11 FLOP) -- measured r2 call 15 on the training step: weight gradients
-        // 4096 x 1664 x 32000 +5 % (709 -> 746 TFLOP/s), the layer-0 projection 32000 x 4096 x 1664 -1 %, the per-chunk 3200-row GEMMs
-        // that run beside the recurrences on ~20 SMs -18 % (74 pairs queue worse than 148 single CTAs there).  Mode 2: whenever eligible.
-        if (g_pair_mode < 0) { const char* e = getenv("FT_GEMM_2CTA"); g_pair_mode = e ? atoi(e) : 1; }
-        const long long tiles_m2 = (g.M + 2 * BM - 1) / (2 * BM);
-        const bool big = 2.0 * g.M * g.N * g.K >= 1e11;
-        if ((g_pair_mode == 2 || (g_pair_mode == 1 && big)) && wide && splitk == 1 && tiles_m2 * tiles_n >= sms / 2) {
-            const int n_tiles2 = static_cast<int>(tiles_m2 * tiles_n);
-            const int n_pairs = n_tiles2 < sms / 2 ? n_tiles2 : sms / 2;
-            if (!g.b_mn) { if (make_tmap_2d(&tmB, g.B, g.b_fmt, g.N, g.K, g.ldb, BK, 128)) return -1; }    // half of B's rows per CTA
-            static bool attr_pair = false;
-            if (!attr_pair) {
-                cudaFuncSetAttribute(gemm2_kernel<false, 256, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, G2Cfg<256, 2>::SMEM);
-                cudaFuncSetAttribute(gemm2_kernel<true, 256, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, G2Cfg<256, 2>::SMEM);
-                attr_pair = true;
-            }
-            cudaLaunchConfig_t cfg = {};
-            cfg.gridDim = dim3(2 * n_pairs); cfg.blockDim = dim3(G2_THREADS); cfg.dynamicSmemBytes = G2Cfg<256, 2>::SMEM; cfg.stream = st;
-            cudaLaunchAttribute attr[1];
-            attr[0].id = cudaLaunchAttributeClusterDimension;
-            attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-            cfg.attrs = attr; cfg.numAttrs = 1;
-            TimeScope ts(g.a_mn ? "gemm_wgrad" : (g.b_mn ? "gemm_dgrad" : "gemm_fwd"), g.M, g.N, g.K, st);
-            cudaError_t e = tf32 ? cudaLaunchKernelEx(&cfg, gemm2_kernel<true, 256, 2>, tmA, tmB, tmC, p, tiles_n, n_tiles2)
-                                 : cudaLaunchKernelEx(&cfg, gemm2_kernel<false, 256, 2>, tmA, tmB, tmC, p, tiles_n, n_tiles2);
-            if (e != cudaSuccess) return ft_set_error(cudaGetErrorString(e));
-            ft_count_launch(1);
-            return ft_check_launch("gemm2_kernel<pair>");
-        }
-        const long long n_work = static_cast<long long>(n_tiles) * splitk;
-        const int grid2 = n_work < sms ? static_cast<int>(n_work) : sms;
-        // operand boxes: K-major A {BK, 128}; K-major B {BK, bn}; MN-major boxes are {BK, BK} as in v1
-        if (!g.b_mn && bn == 256) { if (make_tmap_2d(&tmB, g.B, g.b_fmt, g.N, g.K, g.ldb, BK, 256)) return -1; }
-        static bool attr2 = false;
-        if (!attr2) {
-            cudaFuncSetAttribute(gemm2_kernel<false, 256>, cudaFuncAttributeMaxDynamicSharedMemorySize, G2Cfg<256>::SMEM);
-            cudaFuncSetAttribute(gemm2_kernel<false, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, G2Cfg<128>::SMEM);
-            cudaFuncSetAttribute(gemm2_kernel<true, 256>, cudaFuncAttributeMaxDynamicSharedMemorySize, G2Cfg<256>::SMEM);
-            cudaFuncSetAttribute(gemm2_kernel<true, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, G2Cfg<128>::SMEM);
-            attr2 = true;
-        }
-        TimeScope ts(g.a_mn ? "gemm_wgrad" : (g.b_mn ? "gemm_dgrad" : "gemm_fwd"), g.M, g.N, g.K, st);
-        if (tf32) {
-            if (wide) gemm2_kernel<true, 256><<<grid2, G2_THREADS, G2Cfg<256>::SMEM, st>>>(tmA, tmB, tmC, p, tiles_n, n_tiles);
-            else      gemm2_kernel<true, 128><<<grid2, G2_THREADS, G2Cfg<128>::SMEM, st>>>(tmA, tmB, tmC, p, tiles_n, n_tiles);
-        } else {
-            if (wide) gemm2_kernel<false, 256><<<grid2, G2_THREADS, G2Cfg<256>::SMEM, st>>>(tmA, tmB, tmC, p, tiles_n, n_tiles);
-            else      gemm2_kernel<false, 128><<<grid2, G2_THREADS, G2Cfg<128>::SMEM, st>>>(tmA, tmB, tmC, p, tiles_n, n_tiles);
-        }
-        ft_count_launch(1);
-        return ft_check_launch("gemm2_kernel");
-    }
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(G2_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = st;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr; cfg.numAttrs = ncta == 2 ? 1 : 0;
+    void* args[] = {&tmA, &tmB, &p, const_cast<int*>(&tiles_n), &n_tiles};
+    TimeScope ts(g.a_mn ? "gemm_wgrad" : (g.b_mn ? "gemm_dgrad" : "gemm_fwd"), g.M, g.N, g.K, st);
+    cudaError_t e = cudaLaunchKernelExC(&cfg, fn, args);
+    if (e != cudaSuccess) return ft_set_error(cudaGetErrorString(e));
+    ft_count_launch(1);
+    return ft_check_launch(ncta == 2 ? "gemm2_kernel<pair>" : "gemm2_kernel");
 }
 
 }  // namespace ft

@@ -1,0 +1,6 @@
+// GEMM kernel instantiations: bf16 operands, A K-major.
+#include "gemm_kernel.cuh"
+
+namespace ft {
+template const void* gemm_kernel_ptr<FMT_BF16, 0>(int, int, int);
+}  // namespace ft

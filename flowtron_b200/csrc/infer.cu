@@ -3,11 +3,10 @@
 // (z - b)/exp(log_s) -> gate  runs for all T frames without returning to the host (the reference issues ~25
 // launches and one host sync per frame, and re-projects K/V every frame; here K/V are projected once).
 //
-// Round-2 design (r1 was warp-per-4-rows CUDA-core FMAs: B=16 cost 2.9x B=1, 9 grid barriers per frame, loads issued one
-// dependent iteration at a time):
+// Design:
 //   * every matrix-vector phase runs on the TENSOR CORES with the batch as the M = 16 rows of mma.sync.m16n8k16 and 8 weight
-//     rows as N, so batches up to 16 cost what B = 1 costs.  Why warp-level mma.sync and not tcgen05: a tcgen05 instruction
-//     needs M >= 64 rows and BOTH operands in shared memory -- for an N <= 16 matvec that is 2.5-3 KB of shared-memory operand
+//     rows as N, so batches up to 16 cost what B = 1 costs.  Why warp-level mma.sync and not wgmma: a wgmma instruction
+//     needs M >= 64 rows and its B operand in shared memory -- for an N <= 16 matvec that is 2.5-3 KB of shared-memory operand
 //     reads (20+ clk) per K = 16 plus a shared-memory staging pass for 54 MB of weights per frame, while mma.sync takes the
 //     weights straight from L2 into registers (one 16-byte load per lane per 32 k) with no padding rows.  The phase is bound
 //     by L2 latency/bandwidth, not by tensor throughput, either way;
@@ -20,7 +19,7 @@
 //     do not depend on them), and so are the lane's biases, cell states and residual frame; scores run over all warps of the
 //     grid (query rows staged in shared memory), then one (utterance, 64- or 128-channel slice) context item per CTA with the
 //     softmax (+ prior posterior) recomputed per item; the gate logit of utterance b is computed by CTA b off the critical path;
-//   * NO grid barriers (r2 call 7 trace: 9 barriers x 1.4 us + 9 staging round trips x 0.6 us = 18 of a frame's 39 us): the
+//   * NO grid barriers (nine barriers and staging round trips per frame would take a large share of the frame): the
 //     DATA IS THE FLAG.  Every exchanged activation lives in a ring of 3 frame slots pre-filled with a sentinel (0xFFFF per
 //     fp16, 0xFFFFFFFF per fp32 word: bit patterns no conversion produces); producers store results with st.relaxed.gpu and
 //     reset the same elements of the NEXT slot to the sentinel; consumers fetch the very words they need into shared memory
@@ -76,8 +75,8 @@ static long long* g_infer_trace = nullptr;
 #define IT_TRACE(slot) do { if (p.trace && blockIdx.x == 0 && threadIdx.x == 0) p.trace[i * 32 + (slot)] = clock64(); } while (0)
 
 constexpr uint32_t SENT = 0xFFFFFFFFu;
-constexpr int NREP = 1;                        // replicas of the all-to-all exchanged tensors (CTA c reads replica c % NREP); r2 call 11: 8 replicas
-                                               // (to spread the 128-CTA reads of the same lines over more L2 slices) were SLOWER: 26.6 -> 29.9 us/frame
+constexpr int NREP = 1;                        // replicas of the all-to-all exchanged tensors (CTA c reads replica c % NREP); more replicas
+                                               // spread the reads of the same lines over more L2 slices but add stores
 #define SL(ptr, k) (reinterpret_cast<decltype(ptr)>(reinterpret_cast<char*>(ptr) + (k)))     /* ring slot: k = slot index * slot_bytes */
 __device__ __forceinline__ uint32_t ld_rlx_u32(const void* p) {
     uint32_t v;
@@ -114,7 +113,7 @@ __device__ __forceinline__ float poll_f32(const float* g, int* status, int code)
 // B = 16); the 512 first packets of a CTA sample all producers.  Batch rows >= B stay zero.  K, pitch, columns: multiples of
 // the 16-byte packet.  Callers finish with __syncthreads().
 // B <= 8 variant: a thread has at most ~3 packets, so plain index arithmetic is cheapest (the shift / mask set-up of the variant
-// below costs more than it saves: 26.6 vs 31.2 us per frame at B = 1, r2 calls 10 / 12).
+// below costs more than it saves at such small batches).
 template <bool kF32>
 __device__ __forceinline__ void stage3_small(__half* sx, int cA, const void* srcA, int KA, int pitchA, int cB, const void* srcB, int KB, int pitchB,
                                              int cC, const void* srcC, int KC, int pitchC, int B, int* status) {
@@ -161,7 +160,7 @@ __device__ __forceinline__ void stage3_big(__half* sx, int cA, const void* srcA,
                                            int cC, const void* srcC, int KC, int pitchC, int B, int* status) {
     constexpr int EPP = kF32 ? 4 : 8, EB = kF32 ? 4 : 2;          // elements per packet, bytes per element
     // thread -> (packet column i8 = tid & (kp - 1), row group tid / kp) per source, kp = packets per row rounded up to a power of
-    // two (shift / mask arithmetic only: with divisions a round of the B = 16 loops cost 2.6 us of instruction issue); a source
+    // two (shift / mask arithmetic only: divisions would dominate the instruction issue of a round of the B = 16 loops); a source
     // needs `it` = ceil(B / (512 / kp)) iterations, pending bit = 4 * source + iteration (B <= 16, kp <= 512: it <= 4 when kp <= 128;
     // wider rows use up to 8 bits, sources are then limited to what fits in 32 bits)
     const void* src[3] = {srcA, srcB, srcC};
@@ -261,8 +260,7 @@ __device__ __forceinline__ void mv_partial(const __half* __restrict__ Wt, int m0
 }
 
 // Weights do not depend on the activations a phase waits for: the first PFN k-blocks of a warp's share of the NEXT phase are
-// loaded into registers BEFORE the grid barrier and land while the CTA waits (trace: a phase spent 1-3 load round trips of
-// ~1.2 us each after its barrier).
+// loaded into registers BEFORE the grid barrier and land while the CTA waits instead of costing load round trips after it.
 constexpr int PFN = 11;
 struct Prefetch { uint4 w[PFN]; };
 __device__ __forceinline__ void mv_prefetch(Prefetch& pf, const __half* __restrict__ W, int n_tasks, int nm, int S) {
@@ -376,7 +374,7 @@ __device__ __forceinline__ void lstm_pre(const InferParams& p, const float* bias
 // Context of utterance b, channels [CW s, CW s + CW) (CW = 64 or 128), inside one CTA: warp 0 turns the scores into attention weights (softmax,
 // prior posterior -- or the forced alignment), all 16 warps then take L/16 keys each (every V load of the CTA in flight at
 // once), partial sums meet in shared memory.  Writes ctx (fp16 for lstm layer 0, fp32 for the gate) and, from slice 0, the
-// attention weights.  (r2 call 8: one CTA per utterance doing all 640 channels pulled 256 KB through one SM: 7.4 us.)
+// attention weights.  (One CTA per utterance doing all 640 channels would pull 256 KB through one SM.)
 template <int CW>
 __device__ __forceinline__ void context_item(const InferParams& p, float* sf, int i, int b, int s, long long cur, long long nxt, bool forced) {
     constexpr int NV = CW / 32;                                    // channels per lane
@@ -732,7 +730,7 @@ static int pack(__half* dst, float* bias_dst, const float* WA, int Ka, int Kap, 
                 int n_tasks, int nm, int kind, int M, cudaStream_t st) {
     const long long total = static_cast<long long>(n_tasks) * nm * 256;
     int blocks = static_cast<int>((total + 255) / 256);
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;     // 16 CTAs per SM of an H100 SXM
     pack_weights_kernel<<<blocks, 256, 0, st>>>(dst, bias_dst, WA, Ka, Kap, WB, Kb, b1, b2, n_tasks, nm, kind, M);
     ft_count_launch(1);
     return ft_check_launch("pack_weights_kernel");

@@ -1,4 +1,4 @@
-// Persistent LSTM recurrence kernels for sm_100a (forward and BPTT), hidden size 1024.
+// Persistent LSTM recurrence kernels for sm_90a (forward and BPTT), hidden size 1024.
 //
 // Reference semantics: torch.nn.LSTM as used by AR_Step (flowtron.py:654-655, 671-695): gate order
 // i,f,g,o; c' = s(f) c + s(i) tanh(g); h' = s(o) tanh(c'); zero initial state; outputs are 0 at
@@ -7,12 +7,12 @@
 //
 // Forward (lstm_fwd_kernel), one cooperative launch, 128 CTAs:
 //   * CTA c owns hidden units [8c, 8c+8): its 32 rows of W_hh (4 gates x 8 units, fp16, 64 KB) are
-//     TMA-loaded once and stay resident in shared memory as the UMMA B operand (N = 32).
+//     TMA-loaded once and stay resident in shared memory as the wgmma A operand (M = 64, 32 real rows).
 //   * every step: h_{t-1} ([B,1024] fp16, read straight out of the layer's output tensor) arrives through
 //     TWO 3-D TMA loads (8 K-chunks each, box {64 elems, B rows, 8 chunks}: the smem image is chunk-major
-//     SWIZZLE_128B K-major tiles, the UMMA A operand with M = 128 rows of which the first B are real),
-//     tcgen05.mma accumulates the 32 gate pre-activations in TMEM, the accumulator rows are handed to all
-//     four epilogue warps through shared memory, which add the input projection, apply the cell in fp32
+//     SWIZZLE_128B K-major tiles, the wgmma B operand with N = B rounded up to 16 / 32 / 64); the CTA's one
+//     warpgroup accumulates the 32 gate pre-activations in registers, hands them through shared memory to
+//     the thread that owns each (batch row, unit pair), adds the input projection, applies the cell in fp32
 //     (cell state lives in registers for the whole sequence), store h_t (fp16) and publish ONE release per
 //     CTA into a per-(step, chunk) counter; consumers poll the 16 counters in parallel (one lane each),
 //     fence the async proxy, and issue the next loads.  gates / c for the backward pass are stored AFTER
@@ -21,10 +21,11 @@
 //   (fp16, 128 KB), dG_t ([B,4096] fp16, loss-scaled) streamed in groups of chunks through a small ring,
 //   the pointwise LSTM backward in the epilogue; dG is written once and reused by the wgrad/dgrad GEMMs.
 //
-// History (profiles/, tools/trace_lstm.py): v1 polled the chunk flags and issued 16 (64) 2-D TMA loads
-// serially from one thread: 4 us of an 8.9 us forward step was TMA issue, 0.85 us a single-warp epilogue,
-// 1 us fence+release behind 112 B/lane of stores.
+// Warp roles: warps 0-3 form one warpgroup that issues the wgmma of a step and runs the cell epilogue on the
+// accumulator; warp 4 is the TMA producer.  Loads are issued as few multi-chunk 3-D boxes: issuing 16 (64) 2-D loads
+// serially from one thread puts the issue time on the recurrence's critical path.
 #include <cstdlib>
+#include <type_traits>
 
 #include "ptx.cuh"
 #include "ft_internal.h"
@@ -38,8 +39,9 @@ void set_lstm_trace(long long* p) { g_lstm_trace = p; }
 constexpr int LH = 1024;
 constexpr int LG = 4 * LH;
 constexpr int KCH = 64;                        // K elements per 128-byte chunk (16-bit operands)
-constexpr int LSTM_THREADS = 192;              // warp 0 producer, warp 1 MMA, warps 2-5 epilogue
+constexpr int LSTM_THREADS = 160;              // warps 0-3: one warpgroup (wgmma + cell epilogue), warp 4: TMA producer
 constexpr int EPI_THREADS = 128;
+constexpr int PRODUCER_WARP = 4;
 
 __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2) {
     asm volatile(
@@ -47,7 +49,22 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
         ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
         : "memory");
 }
-__device__ __forceinline__ void epi_bar() { asm volatile("bar.sync 1, 128;" ::: "memory"); }   // the 4 epilogue warps
+__device__ __forceinline__ void epi_bar() { asm volatile("bar.sync 1, 128;" ::: "memory"); }   // the 4 warps of the warpgroup
+__device__ __forceinline__ void st_dsmem_f2(uint32_t cluster_addr, float a, float b) {
+    asm volatile("st.shared::cluster.v2.f32 [%0], {%1, %2};" ::"r"(cluster_addr), "f"(a), "f"(b) : "memory");
+}
+
+// `nch` K chunks (64 elements each, SWIZZLE_128B K-major) of D[64 x N] += A * B^T on the warpgroup; the first instruction
+// overwrites the accumulator when `zero` is set.
+template <int N>
+__device__ __forceinline__ void mma_chunks(float* acc, uint64_t da, uint64_t db, int nch, uint64_t a_chunk, uint64_t b_chunk, bool zero) {
+    for (int c = 0; c < nch; ++c) {
+#pragma unroll
+        for (int k = 0; k < KCH / 16; ++k) wgmma_k<N, FMT_F16, 0, 0>(acc, da + 2 * k, db + 2 * k, (zero && c == 0 && k == 0) ? 0u : 1u);
+        da += a_chunk;
+        db += b_chunk;
+    }
+}
 
 // ------------------------------------------------------------------------------------------- forward
 constexpr int FWD_NCH = LH / KCH;                  // 16 chunks / step
@@ -97,30 +114,22 @@ lstm_bwd_kernel(const __grid_constant__ CUtensorMap tmWT, const __grid_constant_
     uint64_t* bars = reinterpret_cast<uint64_t*>(sAcc + 128 * 17 + 1);
     bars = reinterpret_cast<uint64_t*>((reinterpret_cast<uintptr_t>(bars) + 7) & ~uintptr_t(7));
     uint64_t* full = bars;                       // [nring]
-    uint64_t* empty = bars + 8;                  // [nring]
+    uint64_t* empty = bars + 8;                  // [nring]: one arrival per warp of the warpgroup
     uint64_t* wbar = bars + 16;
-    uint64_t* accum_full = bars + 17;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 18);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int cta = blockIdx.x;
-    const int nq = (p.B + 31) / 32;
 
-    if (warp == 0 && lane == 0) {
+    if (warp == PRODUCER_WARP && lane == 0) {
         tma_prefetch_desc(&tmWT);
         tma_prefetch_desc(&tmG);
-        for (int s = 0; s < p.nring; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
+        for (int s = 0; s < p.nring; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 4); }
         mbar_init(wbar, 1);
-        mbar_init(accum_full, 1);
         fence_mbar_init();
     }
-    if (warp == 1) tmem_alloc<32>(tmem_slot);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == PRODUCER_WARP) {
         if (lane == 0) {
             mbar_expect_tx(wbar, BWD_W_BYTES);
             for (int kc = 0; kc < BWD_NCH; ++kc)       // W_hh^T rows [16c,16c+16), K chunk kc
@@ -145,48 +154,18 @@ lstm_bwd_kernel(const __grid_constant__ CUtensorMap tmWT, const __grid_constant_
                 if (++s == p.nring) { s = 0; ph ^= 1; }
             }
         }
-    } else if (warp == 1) {
-        mbar_wait(wbar, 0, p.status, 213);
-        const uint32_t idesc = umma_idesc(128, BWD_UNITS, FMT_F16, FMT_F16, 0, 0);
-        const uint32_t tmem_d = __shfl_sync(0xffffffffu, tmem_base, 0);
-        const uint64_t da_ring = umma_smem_desc(smem_u32(ring), 16, 1024), db_base = umma_smem_desc(smem_u32(sW), 16, 1024);
-        const uint64_t a_chunk = static_cast<uint64_t>(slot_bytes >> 4), a_group = static_cast<uint64_t>(group_bytes >> 4);
-        const uint64_t b_chunk = (BWD_UNITS * 128) >> 4;
-        int s = 0, ph = 0;
-        uint64_t da_slot = da_ring;
-        for (int t = p.T - 2; t >= 0; --t) {
-            uint64_t db = db_base;
-            for (int g = 0; g < p.ng; ++g) {
-                mbar_wait(&full[s], ph, p.status, 214);
-                tc_fence_after();
-                if (elect_one()) {
-                    if (g == 0) FT_TRACE(p, t, 2);
-                    uint64_t xa = da_slot, xb = db;
-                    uint32_t acc = g != 0;
-                    for (int c = 0; c < p.gs; ++c) {
-#pragma unroll
-                        for (int k = 0; k < 4; ++k) {
-                            umma_f16(tmem_d, xa + 2 * k, xb + 2 * k, idesc, acc);
-                            acc = 1;
-                        }
-                        xa += a_chunk;
-                        xb += b_chunk;
-                    }
-                    umma_commit(&empty[s]);
-                    if (g == p.ng - 1) { FT_TRACE(p, t, 3); umma_commit(accum_full); }
-                }
-                __syncwarp();
-                db += static_cast<uint64_t>(p.gs) * b_chunk;
-                da_slot += a_group;
-                if (++s == p.nring) { s = 0; ph ^= 1; da_slot = da_ring; }
-            }
-        }
     } else {
         // ---------------------------------------------------------------- epilogue: items (batch row, 4 units)
-        const int q = warp & 3;
-        const int et = threadIdx.x - 64;
+        const int et = threadIdx.x;
         const int n_items = p.B * 4;
         const int u0 = BWD_UNITS * cta;
+        // dh_{t} = dG_{t+1} W_hh on the warpgroup: A = the dG ring (M = 64 batch rows, of which the first Bbox are real),
+        // B = the resident W_hh^T slice (N = 16 units)
+        const uint64_t da_ring = wgmma_desc(smem_u32(ring), 16, 1024), db_base = wgmma_desc(smem_u32(sW), 16, 1024);
+        const uint64_t a_chunk = static_cast<uint64_t>(slot_bytes >> 4), a_group = static_cast<uint64_t>(group_bytes >> 4);
+        const uint64_t b_chunk = (BWD_UNITS * 128) >> 4;
+        int rs_slot = 0, rs_ph = 0;
+        mbar_wait(wbar, 0, p.status, 213);
         float dcs[2][4];
 #pragma unroll
         for (int s = 0; s < 2; ++s)
@@ -226,17 +205,27 @@ lstm_bwd_kernel(const __grid_constant__ CUtensorMap tmWT, const __grid_constant_
                 }
             }
             if (step > 0) {
-                if (q < nq) {
-                    float acc[16];
-                    mbar_wait(accum_full, (step - 1) & 1, p.status, 215);
-                    tc_fence_after();
-                    if (et == 64) FT_TRACE(p, t, 4);
-                    tmem_ld_32x16(tmem_base + (static_cast<uint32_t>(q * 32) << 16), acc);
-                    tmem_ld_wait();
-                    tc_fence_before();
-                    float* dst = sAcc + (q * 32 + lane) * 17;
+                float acc[8];
+                uint64_t db = db_base;
+                for (int g = 0; g < p.ng; ++g) {
+                    mbar_wait(&full[rs_slot], rs_ph, p.status, 214);
+                    if (g == 0 && et == 0) FT_TRACE(p, t, 2);
+                    wgmma_fence_acc<8>(acc);
+                    wgmma_fence();
+                    mma_chunks<16>(acc, da_ring + rs_slot * a_group, db, p.gs, a_chunk, b_chunk, g == 0);
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    wgmma_fence_acc<8>(acc);
+                    if (lane == 0) mbar_arrive(&empty[rs_slot]);
+                    db += static_cast<uint64_t>(p.gs) * b_chunk;
+                    if (++rs_slot == p.nring) { rs_slot = 0; rs_ph ^= 1; }
+                }
+                if (et == 0) FT_TRACE(p, t, 4);
+                const int r0 = 16 * warp + (lane >> 2), c0 = 2 * (lane & 3);
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) dst[j] = acc[j];
+                for (int j = 0; j < 2; ++j) {
+                    sAcc[r0 * 17 + 8 * j + c0] = acc[4 * j]; sAcc[r0 * 17 + 8 * j + c0 + 1] = acc[4 * j + 1];
+                    sAcc[(r0 + 8) * 17 + 8 * j + c0] = acc[4 * j + 2]; sAcc[(r0 + 8) * 17 + 8 * j + c0 + 1] = acc[4 * j + 3];
                 }
                 epi_bar();
             }
@@ -290,16 +279,13 @@ lstm_bwd_kernel(const __grid_constant__ CUtensorMap tmWT, const __grid_constant_
             if (et == 0) FT_TRACE(p, t, 7);
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc<32>(tmem_base);
 }
 
 // ------------------------------------------------------------------------------------------- backward, split-K cluster
 // 64 CTAs in 16 clusters of 4.  Cluster c owns hidden units [64c, 64c+64); rank r reduces over gate r's quarter of
 // the contraction (K = 1024 of 4096):  partial_r[b, u] = sum_{k in gate r} dG_{t+1}[b, k] W_hh[k, u].
 //   * the rank's W_hh^T block [64 units x 1024] (fp16, 128 KB) is resident; per step it streams only ITS quarter of
-//     dG_{t+1} (B x 1024 fp16 = 64 KB at B=32; the v2 kernel broadcast all 256 KB to every CTA, 6.3 us of an 8.7 us step);
+//     dG_{t+1} (B x 1024 fp16 = 64 KB at B=32 instead of all 256 KB broadcast to every CTA);
 //   * partial sums (fp32 [B, 64]) go to shared memory; a cluster-scope mbarrier (4 remote arrives) publishes them;
 //     each rank then finishes 16 of the 64 units, reading the 3 other partials over DSMEM;
 //   * pointwise LSTM backward + dG_t stores + per-chunk release flags exactly as in the single-CTA kernel.
@@ -328,9 +314,7 @@ lstm_bwd4_kernel(const __grid_constant__ CUtensorMap tmWT, const __grid_constant
     uint64_t* bars = reinterpret_cast<uint64_t*>(sPart + B4_XCHG_FLOATS);
     uint64_t* full = bars;                       // [2]
     uint64_t* wbar = bars + 2;
-    uint64_t* accum_full = bars + 3;
     uint64_t* part_bar = bars + 4;               // [2] : 4 cluster-scope arrivals each
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 6);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int rank = static_cast<int>(cluster_ctarank());
@@ -339,23 +323,17 @@ lstm_bwd4_kernel(const __grid_constant__ CUtensorMap tmWT, const __grid_constant
     const bool top = p.t1 == p.T;                                // the chunk that holds the last time step
     const int t_hi = top ? p.T - 2 : p.t1 - 1;                   // highest step that has a recurrent term (dG_{t+1} exists)
 
-    if (warp == 0 && lane == 0) {
+    if (warp == PRODUCER_WARP && lane == 0) {
         tma_prefetch_desc(&tmWT);
         tma_prefetch_desc(&tmG);
         mbar_init(&full[0], 1); mbar_init(&full[1], 1);
         mbar_init(wbar, 1);
-        mbar_init(accum_full, 1);
         mbar_init(&part_bar[0], B4_CLUSTER); mbar_init(&part_bar[1], B4_CLUSTER);
         fence_mbar_init();
     }
-    if (warp == 1) tmem_alloc<32>(tmem_slot);                    // accumulator: 64 lanes (units) x Bbox <= 32 columns
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     cluster_sync_all();                                          // every rank's barriers exist before any remote arrive
 
-    if (warp == 0) {
+    if (warp == PRODUCER_WARP) {
         if (lane == 0) {
             mbar_expect_tx(wbar, B4_W_BYTES);
             for (int kc = 0; kc < B4_NCH; ++kc)                  // W_hh^T rows [64c, 64c+64), columns of gate `rank`
@@ -378,42 +356,14 @@ lstm_bwd4_kernel(const __grid_constant__ CUtensorMap tmWT, const __grid_constant
             }
             __syncwarp();
         }
-    } else if (warp == 1) {
-        mbar_wait(wbar, 0, p.status, 233);
-        // swapped operands (see lstm_fwd_kernel): A = resident W_hh^T block (M = 64 units), B = dG_{t+1} quarter (N = Bbox rows)
-        const uint32_t idesc = umma_idesc(64, p.Bbox, FMT_F16, FMT_F16, 0, 0);
-        const uint32_t tmem_d = __shfl_sync(0xffffffffu, tmem_base, 0);
-        const uint64_t da_base = umma_smem_desc(smem_u32(sW), 16, 1024), db_base = umma_smem_desc(smem_u32(sA), 16, 1024);
-        const uint64_t a_chunk = (B4_UNITS * 128) >> 4, b_chunk = static_cast<uint64_t>(slot_bytes >> 4);
-        int step = 0;
-        for (int t = t_hi; t >= p.t0; --t, ++step) {
-            const int ph = step & 1;
-            uint64_t da = da_base, db = db_base;
-#pragma unroll
-            for (int g = 0; g < NG; ++g) {
-                mbar_wait(&full[g], ph, p.status, 234);
-                tc_fence_after();
-                if (elect_one()) {
-                    if (g == 0) FT_TRACE(p, t, 2);
-                    uint64_t xa = da, xb = db;
-#pragma unroll
-                    for (int c = 0; c < GS; ++c) {
-#pragma unroll
-                        for (int k = 0; k < KCH / 16; ++k)
-                            umma_f16(tmem_d, xa + 2 * k, xb + 2 * k, idesc, (g | c | k) != 0);
-                        xa += a_chunk;
-                        xb += b_chunk;
-                    }
-                    if (g == NG - 1) { FT_TRACE(p, t, 3); umma_commit(accum_full); }
-                }
-                __syncwarp();
-                da += GS * a_chunk;
-                db += GS * b_chunk;
-            }
-        }
     } else {
-        const int q = warp & 3;
-        const int et = threadIdx.x - 64;
+        const int q = warp;
+        const int et = threadIdx.x;
+        // swapped operands (see lstm_fwd_kernel): A = resident W_hh^T block (M = 64 units), B = dG_{t+1} quarter (N = 32 >= Bbox
+        // batch rows; the rows beyond Bbox are read from the next chunk and never used)
+        const uint64_t da_base = wgmma_desc(smem_u32(sW), 16, 1024), db_base = wgmma_desc(smem_u32(sA), 16, 1024);
+        const uint64_t a_chunk = (B4_UNITS * 128) >> 4, b_chunk = static_cast<uint64_t>(slot_bytes >> 4);
+        mbar_wait(wbar, 0, p.status, 233);
         const int n_items = p.B * 4;                              // (batch row, quad of units) over this rank's 16 final units
         const int u0 = B4_UNITS * cl + B4_OWN * rank;
         const int item = et;
@@ -455,24 +405,33 @@ lstm_bwd4_kernel(const __grid_constant__ CUtensorMap tmWT, const __grid_constant
                 // (slot of THIS source rank, [unit][batch] rows of 32 floats), then one release-arrive per rank publishes them
                 // and every rank sums four LOCAL slices -- one DSMEM hop on the critical path (r1 pulled: arrive, then a remote
                 // load round trip), and all four epilogue warps move data instead of one.
-                mbar_wait(accum_full, rs & 1, p.status, 235);
-                tc_fence_after();
-                if (et == 64) FT_TRACE(p, t, 4);
                 {
-                    float acc[32];
-                    tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(q * 32) << 16), acc);
-                    tmem_ld_wait();
-                    if (lane < 16) {
-                        const uint32_t dst = mapa_shared(smem_u32(sPart) + static_cast<uint32_t>((((par * 4 + rank) * 16 + lane) * B4_UP) * 4), q);
+                    float acc[16];
 #pragma unroll
-                        for (int j = 0; j < 32; j += 4) st_dsmem_f4(dst + j * 4, acc[j], acc[j + 1], acc[j + 2], acc[j + 3]);
+                    for (int g = 0; g < NG; ++g) {
+                        mbar_wait(&full[g], rs & 1, p.status, 234);
+                        if (g == 0 && et == 0) FT_TRACE(p, t, 2);
+                        wgmma_fence_acc<16>(acc);
+                        wgmma_fence();
+                        mma_chunks<32>(acc, da_base + g * GS * a_chunk, db_base + g * GS * b_chunk, GS, a_chunk, b_chunk, g == 0);
+                        wgmma_commit();
+                    }
+                    wgmma_wait<0>();
+                    wgmma_fence_acc<16>(acc);
+                    if (et == 0) FT_TRACE(p, t, 4);
+                    // fragment rows 16 q + lane / 4 (+ 8) = units of rank q, columns = batch rows 8 j + 2 (lane % 4) (+ 1)
+                    const int u = lane >> 2, b = 2 * (lane & 3);
+                    const uint32_t dst = mapa_shared(smem_u32(sPart) + static_cast<uint32_t>((((par * 4 + rank) * 16 + u) * B4_UP + b) * 4), q);
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) {
+                        st_dsmem_f2(dst + 32 * j, acc[4 * j], acc[4 * j + 1]);
+                        st_dsmem_f2(dst + (8 * B4_UP + 8 * j) * 4, acc[4 * j + 2], acc[4 * j + 3]);
                     }
                 }
-                tc_fence_before();
                 if (et == 64) FT_TRACE(p, t, 6);
                 epi_bar();
                 // publish: one release-arrive on every rank's barrier, issued by 4 different threads so the four
-                // cluster-scope releases overlap (issued serially by one thread they cost ~1.8 us per step)
+                // cluster-scope releases overlap (issued serially by one thread they would queue behind each other)
                 if (et < B4_CLUSTER) mbar_arrive_cluster(mapa_shared(smem_u32(&part_bar[par]), et));
                 mbar_wait_cluster(&part_bar[par], (rs >> 1) & 1, p.status, 236);
                 if (et == 0) FT_TRACE(p, t, 1);               // all partials visible
@@ -531,10 +490,7 @@ lstm_bwd4_kernel(const __grid_constant__ CUtensorMap tmWT, const __grid_constant
             *reinterpret_cast<float4*>(p.dc_carry + static_cast<long long>(ib) * LH + B4_UNITS * cl + B4_OWN * rank + 4 * uq) =
                 make_float4(dcs[0], dcs[1], dcs[2], dcs[3]);
     }
-    tc_fence_before();
-    __syncthreads();
     cluster_sync_all();                                          // nobody exits while a peer may still read its partials
-    if (warp == 1) tmem_dealloc<32>(tmem_base);
 }
 
 
@@ -550,7 +506,7 @@ struct LstmFwdChunkParams : LstmFwdParams {
 // kXIn: the layer's INPUT projection is folded into the recurrent contraction (narrow inputs: the attention LSTM's 80 mel
 // channels).  The step's input row block x_t ([B, <=128] fp16, zero-filled by TMA beyond the real width) is loaded next to
 // h_{t-1} as XCH more K chunks, W_ih's slice sits next to W_hh's in shared memory, and b_ih + b_hh are added in the epilogue:
-// no [T*B, 4096] fp32 projection tensor is written (0.5 ms GEMM + 524 MB write + 524 MB read per flow at B=32, T=1000).
+// no [T*B, 4096] fp32 projection tensor is written (one GEMM + 524 MB write + 524 MB read per flow at B=32, T=1000).
 // Requires x_0 == 0 (the teacher-forcing shift guarantees it): step 0 has no contraction at all.
 constexpr int XCH = 2;                                           // extra K chunks (128 input channels max)
 
@@ -573,31 +529,24 @@ lstm_fwd_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__
     uint64_t* bars = reinterpret_cast<uint64_t*>(sAcc + ((nq * 32 * AP + 1) & ~1));
     uint64_t* full = bars;                       // [FWD_NG] (<= 16)
     uint64_t* wbar = bars + 16;
-    uint64_t* accum_full = bars + 17;
     uint64_t* xfull = bars + 18;                 // [2] (kXIn)
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 20);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int cta = blockIdx.x;
     const int tm0 = p.t0 > 1 ? p.t0 : 1;                         // first step with a recurrent term
 
-    if (warp == 0 && lane == 0) {
+    if (warp == PRODUCER_WARP && lane == 0) {
         tma_prefetch_desc(&tmW);
         tma_prefetch_desc(&tmH);
         if (kXIn) { tma_prefetch_desc(&tmWx); tma_prefetch_desc(&tmX); }
         for (int g = 0; g < FWD_NG; ++g) mbar_init(&full[g], 1);
         mbar_init(wbar, 1);
-        mbar_init(accum_full, 1);
         mbar_init(&xfull[0], 1); mbar_init(&xfull[1], 1);
         fence_mbar_init();
     }
-    if (warp == 1) tmem_alloc<64>(tmem_slot);             // accumulator: 64 lanes (W rows) x Bbox <= 64 columns
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == PRODUCER_WARP) {
         if (lane == 0) {
             // resident W_hh slice: chunk kc, gate g -> FWD_UNITS rows x 128 B
             mbar_expect_tx(wbar, FWD_W_BYTES);
@@ -631,7 +580,7 @@ lstm_fwd_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__
                 }
                 if (kXIn && t + 1 < p.t1) {
                     // x_{t+1} does not depend on the recurrence: prefetch it one step ahead (it comes from HBM, not from L2
-                    // like h: riding on this step's barrier cost 0.6 us per step).  Its buffer was last read by step t-1's MMAs,
+                    // like h: riding on this step's barrier would put its latency on the critical path).  Its buffer was last read by step t-1's MMAs,
                     // which have retired (all flags of step t-1, ours included, were seen above).
                     const int xs = (t + 1 - tm0) & 1;
                     mbar_expect_tx(&xfull[xs], XCH * slot_bytes);
@@ -643,61 +592,50 @@ lstm_fwd_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__
             }
             __syncwarp();
         }
-    } else if (warp == 1) {
-        // warp-uniform loop, one elected lane issues (see gemm.cu: descriptors must be uniform-register operands)
-        mbar_wait(wbar, 0, p.status, 213);
-        // SWAPPED operands (r2): A = the resident W slice (M = 64 accumulator rows: the CTA's 4*UNITS gate rows, plus -- for
-        // UNITS = 8 -- 32 don't-care rows read from the next chunk), B = h_{t-1} (N = Bbox batch rows, exactly what TMA
-        // delivered).  The r1 form (A = h padded to M = 128, B = W) made every instruction read 128 rows x 32 B of A from
-        // shared memory, 3/4 of it padding: 5-6 KB per MMA against the SM's 128 B/clk = 40-48 clk per instruction instead of the
-        // 16-clk tensor floor (trace: 64 MMAs took 1.2-1.5 us of a 4-5 us step).  Now 2 KB + 1 KB per instruction.
-        const uint32_t idesc = umma_idesc(64, p.Bbox, FMT_F16, FMT_F16, 0, 0);
-        const uint32_t tmem_d = __shfl_sync(0xffffffffu, tmem_base, 0);
-        const uint64_t da_base = umma_smem_desc(smem_u32(sW), 16, 1024), db_base = umma_smem_desc(smem_u32(sA), 16, 1024);
-        const uint64_t a_chunk = (FWD_N * 128) >> 4, b_chunk = static_cast<uint64_t>(slot_bytes >> 4);
-        for (int t = tm0; t < p.t1; ++t) {
-            const int ph = (t - tm0) & 1;
-            uint64_t da = da_base, db = db_base;
-#pragma unroll
-            if (kXIn) mbar_wait(&xfull[(t - tm0) & 1], ((t - tm0) >> 1) & 1, p.status, 216);
-            for (int g = 0; g < FWD_NG; ++g) {
-                mbar_wait(&full[g], ph, p.status, 214);
-                tc_fence_after();
-                if (elect_one()) {
-                    if (g == 0) FT_TRACE(p, t, 2);
-                    if (g == FWD_NG - 1) FT_TRACE(p, t, 5);
-                    if (kXIn && g == 0) {                       // the (prefetched) input chunks open the accumulation
-                        const int xs = (t - tm0) & 1;
-                        uint64_t ya = da_base + FWD_NCH * a_chunk, yb = db_base + (FWD_NCH + xs * XCH) * b_chunk;
-#pragma unroll
-                        for (int c = 0; c < XCH; ++c) {
-#pragma unroll
-                            for (int k = 0; k < KCH / 16; ++k)
-                                umma_f16(tmem_d, ya + 2 * k, yb + 2 * k, idesc, (c | k) != 0);
-                            ya += a_chunk;
-                            yb += b_chunk;
-                        }
-                    }
-                    uint64_t xa = da, xb = db;
-#pragma unroll
-                    for (int c = 0; c < FWD_GS; ++c) {
-#pragma unroll
-                        for (int k = 0; k < KCH / 16; ++k)
-                            umma_f16(tmem_d, xa + 2 * k, xb + 2 * k, idesc, kXIn || (g | c | k) != 0);
-                        xa += a_chunk;
-                        xb += b_chunk;
-                    }
-                    if (g == FWD_NG - 1) { FT_TRACE(p, t, 3); umma_commit(accum_full); }
-                }
-                __syncwarp();
-                da += FWD_GS * a_chunk;
-                db += FWD_GS * b_chunk;
-            }
-        }
     } else {
-        // ---------------------------------------------------------------- epilogue: 4 warps, 128 threads
-        const int q = warp & 3;                               // TMEM lane quadrant this warp may read
-        const int et = threadIdx.x - 64;                      // 0..127
+        // ---------------------------------------------------------------- warpgroup: recurrent contraction + cell, 128 threads
+        const int et = threadIdx.x;                           // 0..127
+        // SWAPPED operands: A = the resident W slice (M = 64 accumulator rows: the CTA's 4*UNITS gate rows, plus -- for
+        // UNITS = 8 -- 32 don't-care rows read from the next chunk), B = h_{t-1} (N = Bbox batch rows rounded up to 16 / 32 / 64;
+        // rows beyond Bbox are read from the next chunk and never used).  A = h padded to 64 rows would make every
+        // instruction read mostly padding from shared memory.
+        const uint64_t da_base = wgmma_desc(smem_u32(sW), 16, 1024), db_base = wgmma_desc(smem_u32(sA), 16, 1024);
+        const uint64_t a_chunk = (FWD_N * 128) >> 4, b_chunk = static_cast<uint64_t>(slot_bytes >> 4);
+        const int nsel = p.Bbox <= 16 ? 16 : (p.Bbox <= 32 ? 32 : 64);
+        // one step's contraction: [x_t chunks (kXIn)] + the 16 h_{t-1} chunks as they arrive, accumulator -> sAcc[batch][row]
+        auto contract = [&](auto nb, int t) {
+            constexpr int N = decltype(nb)::value;
+            float acc[N / 2];
+            const int xs = (t - tm0) & 1;
+            // every operand chunk has landed before the first wgmma: a wait (a divergent polling loop) between wgmma
+            // instructions would make ptxas serialize them
+            if (kXIn) mbar_wait(&xfull[xs], ((t - tm0) >> 1) & 1, p.status, 216);
+#pragma unroll
+            for (int g = 0; g < FWD_NG; ++g) {
+                mbar_wait(&full[g], (t - tm0) & 1, p.status, 214);
+                if (et == 0 && g == 0) FT_TRACE(p, t, 2);
+            }
+            if (et == 0) FT_TRACE(p, t, 5);
+            wgmma_fence_acc<N / 2>(acc);
+            wgmma_fence();
+            if (kXIn)                                         // the (prefetched) input chunks open the accumulation
+                mma_chunks<N>(acc, da_base + FWD_NCH * a_chunk, db_base + (FWD_NCH + xs * XCH) * b_chunk, XCH, a_chunk, b_chunk, true);
+            mma_chunks<N>(acc, da_base, db_base, FWD_NCH, a_chunk, b_chunk, !kXIn);
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_acc<N / 2>(acc);
+            if (et == 0) FT_TRACE(p, t, 4);
+            const int r0 = 16 * warp + (lane >> 2), b0 = 2 * (lane & 3);
+#pragma unroll
+            for (int j = 0; j < N / 8; ++j) {
+                const int b = 8 * j + b0;
+                if (b < nq * 32) {
+                    if (r0 < FWD_N) { sAcc[b * AP + r0] = acc[4 * j]; sAcc[(b + 1) * AP + r0] = acc[4 * j + 1]; }
+                    if (r0 + 8 < FWD_N) { sAcc[b * AP + r0 + 8] = acc[4 * j + 2]; sAcc[(b + 1) * AP + r0 + 8] = acc[4 * j + 3]; }
+                }
+            }
+        };
+        mbar_wait(wbar, 0, p.status, 213);
         // work items: (batch row b, unit pair up) -> item = b * UP + up ; thread handles items et, et + 128
         constexpr int UP = FWD_UNITS / 2;
         const int n_items = p.B * UP;
@@ -757,22 +695,9 @@ lstm_fwd_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__
                 }
             }
             if (t > 0) {
-                if (q < FWD_N / 16) {                         // M = 64 accumulator: row r lives in TMEM lane 32 (r / 16) + r % 16
-                    mbar_wait(accum_full, (t - tm0) & 1, p.status, 215);     // (measured on B200: tools/probe/m64_layout.cu)
-                    tc_fence_after();
-                    if (et == 64) FT_TRACE(p, t, 4);          // warp 4 == quadrant 0
-                    const int r = 16 * q + lane;              // W-slice row = gate * UNITS + unit (lanes 16..31 hold nothing)
-                    for (int h = 0; h < nq; ++h) {            // 32 batch columns at a time
-                        float acc[32];
-                        tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + h * 32, acc);
-                        tmem_ld_wait();
-                        if (lane < 16) {
-#pragma unroll
-                            for (int j = 0; j < 32; ++j) sAcc[(h * 32 + j) * AP + r] = acc[j];   // [batch][row]: readers unchanged
-                        }
-                    }
-                    tc_fence_before();
-                }
+                if (nsel == 16) contract(std::integral_constant<int, 16>(), t);
+                else if (nsel == 32) contract(std::integral_constant<int, 32>(), t);
+                else contract(std::integral_constant<int, 64>(), t);
                 epi_bar();
                 if (et == 0) FT_TRACE(p, t, 8);               // accumulator transposed into shared memory
 #pragma unroll
@@ -834,9 +759,6 @@ lstm_fwd_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__
             }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc<64>(tmem_base);
 }
 
 
@@ -855,7 +777,7 @@ PFN_encodeTiled get_tma_encoder();     // gemm.cu
 
 // 3-D view of a row-major [rows, 64*nchunks] 16-bit tensor as {64 elems, rows, chunks}; box {64, box_rows, box_chunks}.
 // The shared-memory image of one box is chunk-major: [chunk][row][128 B], SWIZZLE_128B -- i.e. `box_chunks`
-// consecutive K-major UMMA tiles.
+// consecutive K-major wgmma tiles.
 static int make_tmap_chunks(CUtensorMap* out, const void* ptr, long long rows, int nchunks, long long ld, int box_rows,
                             int box_chunks) {
     PFN_encodeTiled enc = get_tma_encoder();
@@ -970,7 +892,7 @@ static int launch_bwd4(int T, int B, int t0, int t1, const float* dh_ext, long l
     attrs[0].val.clusterDim.x = B4_CLUSTER; attrs[0].val.clusterDim.y = 1; attrs[0].val.clusterDim.z = 1;
     attrs[1].id = cudaLaunchAttributeCooperative;
     attrs[1].val.cooperative = 1;
-    static int coop = -1;          // FT_BWD_COOP=0: plain cluster launch (ncu cannot replay cooperative + cluster launches)
+    static int coop = -1;          // FT_BWD_COOP=0: plain cluster launch (for profilers that cannot replay cooperative + cluster launches)
     if (coop < 0) { const char* e = getenv("FT_BWD_COOP"); coop = e ? atoi(e) : 1; }
     cfg.attrs = attrs; cfg.numAttrs = coop ? 2 : 1;
     TimeScope ts("lstm_bwd", t1 - t0, B, 0, st);

@@ -75,9 +75,9 @@ struct FrameSrc {
     }
 };
 
-// kOcc: CTAs per SM the kernel is compiled for.  3 (default since r2 call 15): 80 registers instead of 128 and the analysis window read
+// kOcc: CTAs per SM the kernel is compiled for.  3 (default): 80 registers instead of 128 and the analysis window read
 // through the read-only cache instead of a shared-memory copy (72.5 KB per CTA), for 24 instead of 16 FFT warps per SM -- the
-// kernel is latency-bound on its shared-memory FFT passes (ncu: 25 % occupancy, shared-memory pipe at 48 %).
+// kernel is latency-bound on its shared-memory FFT passes.
 template <int kFmt, bool kTransform, int kOcc>
 __global__ void __launch_bounds__(MF_THREADS, kOcc)
 mel_fused_kernel(MelFusedParams p) {
@@ -188,7 +188,7 @@ static int ensure_twiddle() {
 
 template <int kFmt, bool kTransform>
 static int launch_mel_fused(MelFusedParams& p, cudaStream_t st) {
-    static int occ = -1;           // FT_MEL_OCC=2: the r2 call-6 configuration (128 registers, window in shared memory)
+    static int occ = -1;           // FT_MEL_OCC=2: 128 registers, window in shared memory
     if (occ < 0) { const char* e = getenv("FT_MEL_OCC"); occ = (e && atoi(e) == 2) ? 2 : 3; }
     const size_t smem = 1024 * 8 + (occ == 2 ? 1024 * 4 : 0) + sizeof(float) * MF_WARPS * MF_WARP_FLOATS +
                         sizeof(float) * ((p.n_mel * 33 + 1) & ~1) + MF_TILE * 8 + MF_TILE * 4 + 16;

@@ -200,8 +200,8 @@ int ft_radam_step(float* p, const float* g, float* m, float* v, long long n, dou
     a.beta1 = static_cast<float>(beta1); a.beta2 = static_cast<float>(beta2);
     a.omb1 = static_cast<float>(1.0 - beta1); a.omb2 = static_cast<float>(1.0 - beta2); a.eps = static_cast<float>(eps);
     a.wd_lr = static_cast<float>(weight_decay_lr); a.step_size = static_cast<float>(step_size); a.use_denom = use_denom;
-    // 148 SMs x 8 resident CTAs of 256 threads, 4 elements per thread-iteration
-    ft::radam_kernel<<<ft::grid_1d((n + 3) / 4, 148 * 8), ft::OPT_THREADS, 0, st>>>(p, g, m, v, n, a, grad_coef);
+    // 132 SMs (H100 SXM) x 8 resident CTAs of 256 threads, 4 elements per thread-iteration
+    ft::radam_kernel<<<ft::grid_1d((n + 3) / 4, 132 * 8), ft::OPT_THREADS, 0, st>>>(p, g, m, v, n, a, grad_coef);
     ft::ft_count_launch(1);
     return ft::ft_check_launch("radam_kernel");
 }
@@ -218,7 +218,7 @@ int ft_radam_step_dev(float* p, const float* g, float* m, float* v, long long n,
     if (n == 0) return 0;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     ft::RAdamHyper h{beta1, beta2, eps, weight_decay, lr};
-    ft::radam_dev_kernel<<<ft::grid_1d((n + 3) / 4, 148 * 8), ft::OPT_THREADS, 0, st>>>(p, g, m, v, n, h, step_dev, grad_coef);
+    ft::radam_dev_kernel<<<ft::grid_1d((n + 3) / 4, 132 * 8), ft::OPT_THREADS, 0, st>>>(p, g, m, v, n, h, step_dev, grad_coef);
     ft::ft_count_launch(1);
     return ft::ft_check_launch("radam_dev_kernel");
 }

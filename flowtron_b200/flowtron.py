@@ -5,7 +5,7 @@ Same class names, constructor signatures, attribute names and ``state_dict`` lay
 Attention :528-592, DenseLayer :453-464, LinearNorm :278-288, Encoder :467-525, FlowtronLoss :185-275), so a
 reference checkpoint loads with ``strict=True`` and callers switch by changing the import.
 
-The flow steps, the NLL/gate loss and inference run on hand-written sm_100a kernels through the C ABI
+The flow steps, the NLL/gate loss and inference run on hand-written sm_90a kernels through the C ABI
 (include/flowtron_b200.h).  There is NO torch/CPU fallback for that path: CPU tensors raise.  The Encoder and
 the embeddings (run once per utterance over L tokens, <2% of FLOPs; SURVEY.md §8f "next") stay ordinary
 PyTorch modules, written device-agnostically.
@@ -191,7 +191,7 @@ class Encoder(nn.Module):
         self.convolutions = nn.ModuleList(convolutions)
         self.lstm = nn.LSTM(encoder_embedding_dim, int(encoder_embedding_dim / 2), 1, batch_first=True, bidirectional=True)
         self.p_dropout = 0.5        # flowtron.py:502 hard-codes 0.5; exposed so tests can run deterministic train-mode steps
-        # FT_ENC_STREAMS=1: run the two LSTM directions concurrently (parity-tested; measured r1: only -0.4 ms/step, so off)
+        # FT_ENC_STREAMS=1: run the two LSTM directions concurrently (parity-tested; off by default)
         self.two_streams = os.environ.get("FT_ENC_STREAMS", "0") != "0"
         self.use_kernels = os.environ.get("FT_ENC_KERNELS", "1") != "0"
         self._rng = None
@@ -373,7 +373,7 @@ class _ArStepFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, state, step, reversed_flag, token, mel, text, in_lens, out_lens, attn_prior, *params_b):
         if not mel.is_cuda:
-            raise FlowtronB200Error("AR_Step needs CUDA tensors: the sm_100a kernels are the only implementation")
+            raise FlowtronB200Error("AR_Step needs CUDA tensors: the sm_90a kernels are the only implementation")
         T, B, M = mel.shape
         L, _, E = text.shape
         dev = mel.device
@@ -447,15 +447,15 @@ class _ArStepFn(torch.autograd.Function):
 
 
 class AR_Step(nn.Module):
-    """flowtron.py:645-828.  Same parameters / state_dict keys; forward/infer run on the sm_100a kernels."""
+    """flowtron.py:645-828.  Same parameters / state_dict keys; forward/infer run on the sm_90a kernels."""
 
     def __init__(self, n_mel_channels, n_speaker_dim, n_text_channels, n_in_channels, n_hidden, n_attn_channels,
                  n_lstm_layers, add_gate, use_cumm_attention):
         super().__init__()
         if use_cumm_attention:
-            raise NotImplementedError("use_cumm_attention is outside the B200 hot-path scope (off in every shipped config)")
+            raise NotImplementedError("use_cumm_attention is outside the hot-path scope (off in every shipped config)")
         if n_lstm_layers != 2 or n_hidden != 1024:
-            raise NotImplementedError("the sm_100a kernels are built for n_lstm_layers=2, n_hidden=1024 (config.json:56-57)")
+            raise NotImplementedError("the sm_90a kernels are built for n_lstm_layers=2, n_hidden=1024 (config.json:56-57)")
         self.use_cumm_attention = use_cumm_attention
         self.conv = nn.Conv1d(n_hidden, 2 * n_mel_channels, 1)
         self.conv.weight.data = 0.0 * self.conv.weight.data
@@ -535,7 +535,7 @@ class Flowtron(nn.Module):
                  mean_scale, dummy_speaker_embedding, use_cumm_attention):
         super().__init__()
         if n_components > 1:
-            raise NotImplementedError("the GMM prior (n_components > 1) is outside the B200 hot-path scope")
+            raise NotImplementedError("the GMM prior (n_components > 1) is outside the hot-path scope")
         norm_fn = MaskedInstanceNorm1d
         self.speaker_embedding = nn.Embedding(n_speakers, n_speaker_dim)
         self.embedding = nn.Embedding(n_text, n_text_dim)
@@ -551,15 +551,15 @@ class Flowtron(nn.Module):
     # Optional: run two half batches as independent pipelines on two CUDA streams (each recurrence then uses a 64-SM
     # persistent kernel, so both are co-resident).  This does NOT shorten the recurrence chain (a half batch takes as
     # many dependent steps as the full batch); it only lets one half's GEMMs / attention / launch gaps overlap the other
-    # half's recurrences.  Measured on B200 (B=32, T=1000): 91.5 -> 89.1 ms/step (+2.7 %).  Off by default.
+    # half's recurrences.  Off by default.
     n_streams = 1
-    # run the Encoder underneath the first flow's attention LSTM (measured r1: 85.5 -> 82.4 ms/step); FT_ENC_OVERLAP=0 disables
+    # run the Encoder underneath the first flow's attention LSTM; FT_ENC_OVERLAP=0 disables
     overlap_encoder = os.environ.get("FT_ENC_OVERLAP", "1") != "0"
     min_split_batch = 8
 
     # Utterances per kernel launch.  The kernels take up to 64, but the fast paths (cluster BPTT, layer pipeline, folded input
-    # projection) are B <= 32 paths: a B = 64 batch (configs[2]) runs faster as two consecutive 32-utterance launches than as
-    # one 64-utterance launch on the fallback kernels (r2: 118.8 ms/step as one launch).  FT_MAX_KERNEL_BATCH overrides.
+    # projection) are B <= 32 paths, so a B = 64 batch (configs[2]) runs as two consecutive 32-utterance launches rather than
+    # one 64-utterance launch on the fallback kernels.  FT_MAX_KERNEL_BATCH overrides.
     max_kernel_batch = int(os.environ.get("FT_MAX_KERNEL_BATCH", "32"))
 
     def _run_flows(self, mel, encoder_outputs, mask, out_lens, attn_prior):
@@ -734,7 +734,7 @@ class _AttnCtcFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, attn_logprob, in_lens, out_lens, time_reversed, blank_logprob):
         if not attn_logprob.is_cuda:
-            raise FlowtronB200Error("AttentionCTCLoss needs CUDA tensors: the sm_100a kernel is the only implementation")
+            raise FlowtronB200Error("AttentionCTCLoss needs CUDA tensors: the sm_90a kernel is the only implementation")
         lp = attn_logprob.detach().float().contiguous()
         dev = lp.device
         cost = torch.empty(lp.size(0), device=dev)
@@ -772,7 +772,7 @@ class FlowtronLoss(nn.Module):
     def __init__(self, sigma=1.0, gm_loss=False, gate_loss=True, use_ctc_loss=False, ctc_loss_weight=0.0, blank_logprob=-1):
         super().__init__()
         if gm_loss:
-            raise NotImplementedError("gm_loss (GMM prior) is outside the B200 hot-path scope")
+            raise NotImplementedError("gm_loss (GMM prior) is outside the hot-path scope")
         self.sigma = sigma
         self.gm_loss = gm_loss
         self.gate_loss = gate_loss

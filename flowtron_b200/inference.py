@@ -17,7 +17,7 @@ def ar_step_infer(step, residual, text, attns, attn_prior=None, reversed_flag=Fa
     (B == 1, the reference's ``attns[i][None, None]``), a [T, B, L] tensor, or the list of T per-frame weights this
     function returns ([B, 1, L] each).  Like the reference, a back step consumes them in its own (flipped) time order."""
     if not residual.is_cuda:
-        raise FlowtronB200Error("AR_Step.infer needs CUDA tensors: the sm_100a kernel is the only implementation")
+        raise FlowtronB200Error("AR_Step.infer needs CUDA tensors: the sm_90a kernel is the only implementation")
     T, B, M = residual.shape
     L, _, E = text.shape
     dev = residual.device

@@ -1,4 +1,4 @@
-/* flowtron_b200 — C ABI of the B200-native Flowtron hot path (libflowtron_b200.so).
+/* flowtron_b200 — C ABI of the H100-native Flowtron hot path (libflowtron_b200.so).
  *
  * The reference (NVIDIA/flowtron) has no FFI: the hot path sits behind Python nn.Modules.  These entry
  * points are what a binding for that path replaces; each cites the reference interface it stands for.
@@ -33,7 +33,7 @@ int ft_timing_report(char* buf, int cap);   /* synchronises; "name m n k count t
 long long ft_launch_count(void);
 void ft_reset_launch_count(void);
 
-/* C[M,N] = act(alpha * A[M,K] B[N,K]^T + bias + bias2) (+ C32 if beta).  tcgen05/TMA GEMM.
+/* C[M,N] = act(alpha * A[M,K] B[N,K]^T + bias + bias2) (+ C32 if beta).  wgmma/TMA GEMM.
  * a_mn / b_mn = 1: operand is given MN-major, i.e. A points at a row-major [K, M] tensor.
  * Replaces: nn.Linear / Conv1d(k=1) / LSTM input projections (flowtron.py:278-288, 651, 654-655) and
  * their autograd dgrad / wgrad. */
@@ -57,7 +57,7 @@ void ft_debug_set_infer_trace(long long* buf);
 /* Process-wide switch: 1 = ft_lstm_fwd (and ft_ar_step_fwd) use the 64-CTA recurrence kernel so two half-batch
  * launches on two streams run concurrently (the BPTT kernel always uses 64 CTAs for B <= 32). */
 void ft_set_lstm_half_sm(int on);
-/* ft_gemm tile policy: 0 = one CTA per 128 x 256 tile always; 1 (default) = CTA pairs (tcgen05 cta_group::2, 256 x 256 tiles) for
+/* ft_gemm tile policy: 0 = one CTA per 128 x 256 tile always; 1 (default) = CTA pairs (2-CTA clusters sharing B by TMA multicast, 256 x 256 tiles) for
  * contractions >= 1e11 FLOP; 2 = CTA pairs whenever the output is wide and has >= SMs/2 such tiles. */
 void ft_set_gemm_pair_mode(int mode);
 

@@ -11,7 +11,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device")
     config.addinivalue_line("markers", "needs_reference: needs /root/reference (build container only)")
 
 

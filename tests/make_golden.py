@@ -112,7 +112,7 @@ def mel_case():
 def radam_case():
     """Trajectory of the UNMODIFIED reference optimizer (radam.py:25-122) preceded by train.py:326's clip, CPU fp32."""
     import warnings
-    sys.path.insert(0, "/root/reference")
+    sys.path.insert(0, ref_shims.REF)
     from radam import RAdam
     g = torch.Generator().manual_seed(77)
     shapes = [(7, 5), (33,), (1,)]
@@ -139,6 +139,62 @@ def radam_case():
     print("radam: 9 steps recorded")
 
 
+def collate_batch():
+    """The ragged 4-utterance batch of test_oracle_data.py (prior from the data oracle, equal to the reference's)."""
+    from oracle import data_oracle as D
+    g = torch.Generator().manual_seed(0)
+    batch = []
+    for F_, P_ in [(29, 11), (40, 17), (5, 17), (33, 3)]:
+        batch.append((torch.randn(80, F_, generator=g), torch.LongTensor([F_ % 3]), torch.randint(1, 100, (P_,), generator=g),
+                      D.beta_binomial_prior_distribution(P_, F_, 1.0)))
+    return batch
+
+
+def reference_checks_case():
+    """Outputs of reference functions the CPU tests compare against: state_dict layout (flowtron.py), beta-binomial prior and
+    DataCollate (data.py), STFT.transform (audio_processing.py), AR_Step / AR_Back_Step.infer with forced attentions."""
+    import types
+    rec = {}
+    cfg = dict(synth.DEFAULT_MODEL_CONFIG)
+    _, model = ref_shims.reference_model(cfg, synth.synth_params(cfg, 5))
+    sd = model.state_dict()
+    rec["sd_keys"] = np.array(list(sd.keys()))
+    rec["sd_shapes"] = np.array([",".join(str(d) for d in v.shape) for v in sd.values()])
+    cwd = os.getcwd()
+    os.chdir(ref_shims.REF)                                 # text/__init__ opens data/cmudict_dictionary relative to the cwd
+    try:
+        ref_shims.import_audio_processing()                 # librosa stub before data.py imports audio_processing
+        for name in ("unidecode", "inflect"):                # text-cleaning dependencies (absent here, unused by the collate)
+            if name not in sys.modules:
+                m = types.ModuleType(name)
+                m.unidecode = lambda s: s
+                m.engine = lambda: None
+                sys.modules[name] = m
+        sys.path.insert(0, ref_shims.REF)
+        import data as RD
+        rec["prior_11_29"] = RD.beta_binomial_prior_distribution(11, 29, 1.0).numpy()
+        for i, t in enumerate(RD.DataCollate(1, use_attn_prior=True)(collate_batch())):
+            rec[f"collate_{i}"] = t.numpy()
+    finally:
+        os.chdir(cwd)
+    AP = ref_shims.import_audio_processing()
+    y = torch.rand(2, 3000, generator=torch.Generator().manual_seed(3)) * 1.9 - 0.95
+    m_ref, p_ref = AP.STFT(1024, 256, 1024).transform(y)
+    rec["stft_y"], rec["stft_mag"], rec["stft_phase"] = y.numpy(), m_ref.numpy(), p_ref.numpy()
+    cfg = dict(synth.DEFAULT_MODEL_CONFIG, n_flows=2, use_gate_layer=False)
+    _, model = ref_shims.reference_model(cfg, synth.synth_params(cfg, 17))
+    g = torch.Generator().manual_seed(2)
+    T, L = 10, 6
+    residual = torch.randn(T, 1, 80, generator=g) * 0.5
+    enc = torch.randn(L, 1, 640, generator=g)
+    attns = torch.softmax(torch.randn(T, L, generator=g), -1)
+    with torch.no_grad():
+        rec["forced_r0"] = model.flows[0].infer(residual, enc, attns)[0].numpy()
+        rec["forced_r1"] = model.flows[1].infer(residual, enc, attns)[0].numpy()
+    np.savez_compressed(os.path.join(OUT, "reference_checks.npz"), **rec)
+    print("reference checks:", sorted(rec))
+
+
 def big_cases():
     """BASELINE-shape fixtures (VERDICT r1 #1): a T=1000 training step (cfg 2 shapes at the largest B the CPU reference
     finishes in minutes) and cfg-4 inference requests (T=400 default, T=1000), all 2-flow."""
@@ -163,6 +219,7 @@ def main():
     infer_case("b4nogate", n_flows=2, B=4, T=32, L=16, seed=8, gate_bias=0.0, use_gate=False)
     mel_case()
     radam_case()
+    reference_checks_case()
     big_cases()
 
 
@@ -173,6 +230,8 @@ if __name__ == "__main__":
         torch.manual_seed(0)
         torch.set_num_threads(8)
         train_case("f2ctc", n_flows=2, B=3, T=80, L=20, out_lens=[80, 47, 66], with_prior=True, seed=777, ctc_weight=1.0)
+    elif len(sys.argv) > 1 and sys.argv[1] == "refchecks":     # only the reference-function outputs of the CPU tests
+        reference_checks_case()
     elif len(sys.argv) > 1 and sys.argv[1] == "big":     # only the BASELINE-shape fixtures (minutes of CPU time)
         torch.manual_seed(0)
         torch.set_num_threads(8)

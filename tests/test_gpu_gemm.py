@@ -1,4 +1,4 @@
-"""GPU: tcgen05/TMA GEMM primitive vs torch fp64 matmul (through the C ABI)."""
+"""GPU: wgmma/TMA GEMM primitive vs torch fp64 matmul (through the C ABI)."""
 import pytest
 import torch
 
@@ -31,7 +31,7 @@ CASES = [
     (256, 256, 256, torch.bfloat16, False, True),     # B given as [K, N]
     (1024, 1664, 2000, torch.bfloat16, True, True),   # wgrad shape: dW = dY^T X
     (500, 1664, 4096, torch.bfloat16, False, True),   # dgrad shape: dX = dY W
-    # persistent kernel: more tiles than SMs (every CTA loops, both TMEM accumulators and all ring phases wrap)
+    # persistent kernel: more tiles than SMs (every CTA loops, all ring phases wrap)
     (128 * 37, 2048, 192, torch.float16, False, False),       # 37 x 8 = 296 wide tiles, short K: epilogue-bound
     (128 * 41 + 5, 640, 320, torch.float16, False, False),    # narrow (BN=128) path, 5 x 42 = 210 tiles, M tail
     (4096, 1664, 128 * 9, torch.float16, True, True),         # wgrad, wide N with a tail tile (1664 = 6.5 x 256)

@@ -1,4 +1,4 @@
-"""GPU: persistent tcgen05 LSTM recurrence (forward + BPTT) vs the CPU oracle, through the C ABI."""
+"""GPU: persistent wgmma LSTM recurrence (forward + BPTT) vs the CPU oracle, through the C ABI."""
 import pytest
 import torch
 

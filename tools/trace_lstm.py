@@ -29,9 +29,9 @@ def main():
         torch.cuda.synchronize()
         print(f"run {it}: {e0.elapsed_time(e1) * 1e3 / T:.2f} us/step")
     L.ft_debug_set_lstm_trace(None)
-    report(trace, T, "forward", ["flags_seen", "tma_issued", "first_group_landed", "all_mma_issued", "accum_done(epi)",
-                                 "last_group_landed", "proxy_fence_done", "release_issued",
-                                 "acc_in_smem(epi)", "cell_done_h_stored", "epi_barrier_done"])
+    report(trace, T, "forward", {0: "flags_seen", 1: "tma_issued", 2: "first_group_landed", 4: "accum_done(wgmma)",
+                                 5: "last_group_landed", 6: "proxy_fence_done", 7: "release_issued",
+                                 8: "acc_in_smem", 9: "cell_done_h_stored", 10: "epi_barrier_done"})
     if os.environ.get("FT_TRACE_FWD_ONLY"):
         return
     # ---- backward
@@ -49,8 +49,8 @@ def main():
         torch.cuda.synchronize()
         print(f"bwd run {it}: {e0.elapsed_time(e1) * 1e3 / T:.2f} us/step")
     L.ft_debug_set_lstm_trace(None)
-    report(trace, T, "backward", ["flags_seen", "partials_visible(cluster)", "first_group_landed", "all_mma_issued", "accum_done(epi)",
-                                  "dG_stored", "own_partial_written", "release_issued"], reverse=True)
+    report(trace, T, "backward", {0: "flags_seen", 1: "partials_visible(cluster)", 2: "first_group_landed", 4: "accum_done(wgmma)",
+                                  5: "dG_stored", 6: "own_partial_written", 7: "release_issued"}, reverse=True)
 
 
 def report(trace, T, title, names, reverse=False):
@@ -59,14 +59,15 @@ def report(trace, T, title, names, reverse=False):
         tr = torch.flip(tr, (0,))
     print(f"== {title}")
     period = (tr[1:, 0] - tr[:-1, 0]).mean().item()
-    print(f"step period: {period:.0f} clk = {period / 1.965e3:.2f} us @1.965GHz")
+    print(f"step period: {period:.0f} clk = {period / 1.98e3:.2f} us @1.98GHz")
     base = tr[:, 0:1]
     rel = (tr - base).mean(0)
-    for n, v in zip(names, rel.tolist()):
-        print(f"  {n:24s} +{v:8.0f} clk ({v / 1965:.2f} us)")
+    for slot, n in names.items():               # {trace slot: phase}; slots a kernel does not stamp are not listed
+        v = rel[slot].item()
+        print(f"  {n:24s} +{v:8.0f} clk ({v / 1980:.2f} us)")
     # time from own release (slot 7, step t) to flags_seen of step t+1
     gap = (tr[1:, 0] - tr[:-1, 7]).mean().item()
-    print(f"  own release(t) -> flags_seen(t+1): {gap:.0f} clk ({gap / 1965:.2f} us)")
+    print(f"  own release(t) -> flags_seen(t+1): {gap:.0f} clk ({gap / 1980:.2f} us)")
 
 if __name__ == "__main__":
     main()
