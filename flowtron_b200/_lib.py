@@ -53,6 +53,21 @@ class FtEncoderGrads(Structure):
     _fields_ = [("d_" + n, c_void_p * k) for n, k in ENC_PARAM_FIELDS]
 
 
+class FtWaveGlowDesc(Structure):
+    _fields_ = [("n_mel", c_int), ("n_flows", c_int), ("n_group", c_int), ("n_early_every", c_int), ("n_early_size", c_int),
+                ("n_layers", c_int), ("n_channels", c_int), ("kernel_size", c_int), ("B", c_int), ("F_max", c_int),
+                ("frames", POINTER(c_int))]
+
+
+WG_MAX_FLOWS, WG_MAX_LAYERS = 16, 8
+
+
+class FtWaveGlowWeights(Structure):
+    _fields_ = [("up_w", c_void_p), ("up_b", c_void_p)] + \
+        [(n, (c_void_p * WG_MAX_LAYERS) * WG_MAX_FLOWS) for n in ("in_w", "in_b", "rs_w", "rs_b")] + \
+        [(n, c_void_p * WG_MAX_FLOWS) for n in ("start_w", "start_b", "end_w", "end_b", "inv_w")]
+
+
 class FlowtronB200Error(RuntimeError):
     pass
 
@@ -164,6 +179,11 @@ def _declare(L):
     L.ft_encoder_bwd_tokens.argtypes = [POINTER(FtEncoderDesc), POINTER(FtEncoderWeights), c_void_p, c_longlong, c_longlong, c_void_p,
                                         c_void_p, c_int, c_void_p, POINTER(FtEncoderGrads), c_void_p, c_void_p]
     L.ft_encoder_bwd_tokens.restype = c_int
+    L.ft_waveglow_scratch_bytes.argtypes = [POINTER(FtWaveGlowDesc)]
+    L.ft_waveglow_scratch_bytes.restype = c_size_t
+    L.ft_waveglow_infer.argtypes = [POINTER(FtWaveGlowDesc), POINTER(FtWaveGlowWeights), c_void_p, c_void_p, c_float, c_void_p,
+                                    c_void_p, c_void_p]
+    L.ft_waveglow_infer.restype = c_int
 
 
 def check(rc: int, what: str = ""):
@@ -512,3 +532,15 @@ def encoder_bwd(desc, params, d_out, saved, need_dx=True, tokens=None, emb_weigh
     check(L.ft_encoder_bwd_tokens(byref(desc), byref(w), ptr(d_out), d_out.stride(0), d_out.stride(1), ptr(saved), ptr(tokens),
                                   emb_weight.size(0), ptr(d_emb), byref(g), ptr(scratch), stream_ptr()), "ft_encoder_bwd_tokens")
     return d_emb, grads
+
+
+# ------------------------------------------------------------------------------------------------ WaveGlow
+def waveglow_infer(desc, weights, mel, noise, sigma, audio):
+    """mel f32 [B,80,F_max], noise f32 [B,8,32 F_max], audio f32 [B,256 F_max] (written); desc.frames set by the caller."""
+    _need_cuda(mel, noise, audio)
+    nbytes = int(lib().ft_waveglow_scratch_bytes(byref(desc)))
+    if nbytes == 0:
+        raise FlowtronB200Error(f"ft_waveglow_scratch_bytes rejected the configuration: {lib().ft_last_error().decode()}")
+    scratch = scratch_buffer(nbytes, mel.device)
+    check(lib().ft_waveglow_infer(byref(desc), byref(weights), ptr(mel), ptr(noise), float(sigma), ptr(audio), ptr(scratch),
+                                  stream_ptr()), "ft_waveglow_infer")

@@ -163,3 +163,92 @@ def ljs_like_lengths(B: int, T: int, seed: int, lo_frac: float = 0.5):
     out_lens[0] = T
     in_lens = torch.clamp((out_lens.float() / 6.5).round().long(), 40, 160)
     return out_lens, in_lens
+
+
+# ------------------------------------------------------------------------------------------------ WaveGlow
+DEFAULT_WAVEGLOW_CONFIG = dict(  # tacotron2/waveglow/config.json "waveglow_config" (waveglow_256channels_v4.pt)
+    n_mel_channels=80, n_flows=12, n_group=8, n_early_every=4, n_early_size=2,
+    WN_config=dict(n_layers=8, n_channels=256, kernel_size=3))
+
+
+def waveglow_channels(cfg: dict):
+    """[(n_remaining_channels, n_half)] per flow k, as WaveGlow.__init__ assigns them."""
+    out, c = [], cfg["n_group"]
+    for k in range(cfg["n_flows"]):
+        if k % cfg["n_early_every"] == 0 and k > 0:
+            c -= cfg["n_early_size"]
+        out.append((c, c // 2))
+    return out
+
+
+def waveglow_param_shapes(cfg: dict, weight_norm: bool = True) -> Dict[str, Tuple[int, ...]]:
+    """state_dict key -> shape of the reference WaveGlow(**cfg), in weight-norm form (weight_g / weight_v) or, with
+    weight_norm=False, as after WaveGlow.remove_weightnorm (plain weight)."""
+    M, G = cfg["n_mel_channels"], cfg["n_group"]
+    wn = cfg["WN_config"]
+    L, C, K = wn["n_layers"], wn["n_channels"], wn["kernel_size"]
+    s: Dict[str, Tuple[int, ...]] = {"upsample.weight": (M, M, 1024), "upsample.bias": (M,)}
+
+    def conv(pre, co, ci, k, normed=True):
+        s[f"{pre}.bias"] = (co,)
+        if normed and weight_norm:
+            s[f"{pre}.weight_g"] = (co, 1, 1)
+            s[f"{pre}.weight_v"] = (co, ci, k)
+        else:
+            s[f"{pre}.weight"] = (co, ci, k)
+
+    for k, (c, nh) in enumerate(waveglow_channels(cfg)):
+        pre = f"WN.{k}"
+        for i in range(L):
+            conv(f"{pre}.in_layers.{i}", 2 * C, C, K)
+        for i in range(L):
+            conv(f"{pre}.res_skip_layers.{i}", 2 * C if i < L - 1 else C, C, 1)
+        conv(f"{pre}.start", C, nh, 1)
+        conv(f"{pre}.end", 2 * nh, C, 1, normed=False)
+        conv(f"{pre}.cond_layer", 2 * C * L, M * G, 1)
+        s[f"convinv.{k}.conv.weight"] = (c, c, 1)
+    return s
+
+
+def synth_waveglow_params(cfg: dict = DEFAULT_WAVEGLOW_CONFIG, seed: int = 1234) -> Dict[str, torch.Tensor]:
+    """Deterministic WaveGlow weights in weight-norm form (reference state_dict keys).  weight_g differs from |weight_v| so a
+    weight-norm fold is exercised; `end` is non-zero (max |log_s| of about 0.1-0.5 on synth_waveglow_mel inputs) so every
+    affine coupling acts; convinv is orthonormal with det > 0 like Invertible1x1Conv's initialisation."""
+    g_ranges = {"start": (0.8, 1.2), "in_layers": (0.5, 1.0), "res_skip_layers": (0.3, 0.6), "cond_layer": (0.3, 0.6)}
+    out = {}
+    for name, shape in waveglow_param_shapes(cfg, weight_norm=True).items():
+        g = torch.Generator(device="cpu")
+        g.manual_seed((seed * 1000003 + zlib.crc32(name.encode())) % (2 ** 63 - 1))
+        if name.startswith("convinv"):
+            c = shape[0]
+            q = torch.linalg.qr(torch.randn(c, c, generator=g, dtype=torch.float64))[0]
+            if torch.det(q) < 0:
+                q[:, 0] = -q[:, 0]
+            t = q.float().view(c, c, 1)
+        elif name.endswith("weight_g"):
+            lo, hi = g_ranges[name.split(".")[2]]
+            t = lo + (hi - lo) * torch.rand(shape, generator=g)
+        elif name.endswith("weight_v"):
+            t = torch.randn(shape, generator=g)
+        elif name == "upsample.weight":
+            t = torch.randn(shape, generator=g) * 0.01
+        elif name.endswith("end.weight"):
+            t = torch.randn(shape, generator=g) * 0.012
+        elif name.endswith("end.bias"):
+            t = torch.randn(shape, generator=g) * 0.01
+        else:                                                  # biases
+            t = torch.randn(shape, generator=g) * 0.05
+        out[name] = t.contiguous()
+    return out
+
+
+def synth_waveglow_mel(B: int, F: int, seed: int) -> torch.Tensor:
+    """Log-mel-like input [B, 80, F] (the statistics of synth_batch(logmel_stats=True))."""
+    g = torch.Generator(device="cpu").manual_seed(seed)
+    return (torch.randn(B, 80, F, generator=g) * 2.0 - 5.5).clamp_(-11.5, 2.0)
+
+
+def synth_waveglow_noise(B: int, F: int, seed: int) -> torch.Tensor:
+    """N(0, 1) noise [B, 8, 32 F] in WaveGlow.infer's `noise` layout."""
+    g = torch.Generator(device="cpu").manual_seed(seed + 7919)
+    return torch.randn(B, 8, 32 * F, generator=g)

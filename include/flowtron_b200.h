@@ -289,6 +289,46 @@ int ft_encoder_bwd_tokens(const FtEncoderDesc* d, const FtEncoderWeights* w, con
 int ft_encoder_bwd(const FtEncoderDesc* d, const FtEncoderWeights* w, const float* d_out, long long d_stride_b,
                    long long d_stride_l, const void* saved, float* d_x, const FtEncoderGrads* grads, void* scratch, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------
+ * WaveGlow vocoder, inference direction (tacotron2/waveglow/glow.py:251-293 WaveGlow.infer): log-mel -> audio.
+ * Built for n_mel 80, n_group 8, WN n_channels 256, kernel_size 3; n_flows <= 16, n_layers <= 8.
+ * ---------------------------------------------------------------------------------------------------- */
+#define FT_WG_MAX_FLOWS 16
+#define FT_WG_MAX_LAYERS 8
+
+typedef struct {
+    int n_mel, n_flows, n_group, n_early_every, n_early_size;   /* 80, 12, 8, 4, 2 (waveglow config.json)        */
+    int n_layers, n_channels, kernel_size;                      /* WN_config: 8, 256, 3                           */
+    int B;                                                      /* utterances (1..128)                            */
+    int F_max;                                                  /* padded mel frames of `mel`                     */
+    const int* frames;                                          /* HOST int[B]: frames of utterance b (1..F_max)  */
+} FtWaveGlowDesc;
+
+/* Device pointers to the packed weights of WaveGlow (flowtron_b200/waveglow.py packs them once per weight version):
+ *   up_w   fp16 [20480, 384]: the ConvTranspose1d(80, 80, 1024, stride 256) as one GEMM over frames f-3..f (4 x 96 K, mel
+ *          channels zero-padded to 96); column n = g*640 + c*8 + j is sample 8g + j of channel c within the frame; up_b [20480]
+ *   in_w   fp16 [512, 1408] per (flow, layer): [tap0 | tap1 | tap2 | cond_layer slice] of the weight-norm-folded in_layer and
+ *          cond_layer, rows interleaved (2c = tanh channel c, 2c+1 = sigmoid channel c); in_b [512] = in_layer + cond bias
+ *   rs_w   fp16 [512 (256 for the last layer), 256]: res_skip_layer; rs_b fp32
+ *   start_w fp32 [256, n_half], start_b [256]; end_w fp32 [2 n_half, 256], end_b [2 n_half]; inv_w fp32 [c, c] = convinv^-1 */
+typedef struct {
+    const void* up_w; const float* up_b;
+    const void* in_w[FT_WG_MAX_FLOWS][FT_WG_MAX_LAYERS]; const float* in_b[FT_WG_MAX_FLOWS][FT_WG_MAX_LAYERS];
+    const void* rs_w[FT_WG_MAX_FLOWS][FT_WG_MAX_LAYERS]; const float* rs_b[FT_WG_MAX_FLOWS][FT_WG_MAX_LAYERS];
+    const float* start_w[FT_WG_MAX_FLOWS]; const float* start_b[FT_WG_MAX_FLOWS];
+    const float* end_w[FT_WG_MAX_FLOWS]; const float* end_b[FT_WG_MAX_FLOWS];
+    const float* inv_w[FT_WG_MAX_FLOWS];
+} FtWaveGlowWeights;
+
+/* Bytes of the caller-owned scratch of ft_waveglow_infer (0 if the descriptor is rejected). */
+size_t ft_waveglow_scratch_bytes(const FtWaveGlowDesc* d);
+/* mel fp32 [B, 80, F_max]; noise fp32 [B, 8, 32 F_max]: channels of WaveGlow.forward's z -- the first flow's draw on the
+ * highest channels (4:8 for the shipped config), each early injection on the channels just below (2:4 after flow 8, 0:2
+ * after flow 4); it is multiplied by sigma.  audio fp32 [B, 256 F_max]: utterance b fills its first 256 frames[b] samples,
+ * the rest is zero.  About n_flows * (2 n_layers + 1) + 3 launches, no host synchronisation (CUDA-graph capturable). */
+int ft_waveglow_infer(const FtWaveGlowDesc* d, const FtWaveGlowWeights* w, const float* mel, const float* noise, float sigma,
+                      float* audio, void* scratch, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
