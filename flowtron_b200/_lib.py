@@ -136,6 +136,9 @@ def _declare(L):
     L.ft_stft_transform.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_int, c_int, c_void_p, c_void_p,
                                     c_void_p]
     L.ft_stft_transform.restype = c_int
+    L.ft_stft_inverse.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_int, c_int, c_void_p,
+                                  c_float, c_void_p, c_void_p]
+    L.ft_stft_inverse.restype = c_int
     L.ft_attn_prior.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_float, c_void_p, c_void_p]
     L.ft_attn_prior.restype = c_int
     L.ft_collate_mel.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]
@@ -443,6 +446,26 @@ def stft_transform(wav, sample_offsets, frame_offsets, n_utt, total_frames, wind
     _need_cuda(wav, magnitude, phase)
     check(lib().ft_stft_transform(ptr(wav), ptr(sample_offsets), ptr(frame_offsets), int(n_utt), int(total_frames), ptr(window),
                                   int(n_fft), int(hop), ptr(magnitude), ptr(phase), stream_ptr()), "ft_stft_transform")
+
+
+STFT_INVERSE_HOPS = (128, 256, 512)
+
+
+def stft_inverse(magnitude, phase, frame_offsets, out_offsets, n_utt, total_frames, window, n_fft, hop, out, bias=None,
+                 strength=0.0):
+    """magnitude / phase: per-utterance [513, F_u] blocks (f32 CUDA, ft_stft_transform's layout); frame_offsets int64 [n_utt+1];
+    out_offsets int64 [n_utt] (where utterance u's (F_u - 1) * hop samples go in ``out``); bias: optional f32 [513], applied as
+    max(m - strength * bias, 0).  One kernel (csrc/istft.cu)."""
+    if n_fft != 1024 or hop not in STFT_INVERSE_HOPS:
+        raise NotImplementedError(f"the inverse STFT kernel is built for filter_length 1024 and hop 128, 256 or 512 "
+                                  f"(got {n_fft}, {hop})")
+    _need_cuda(magnitude, phase, frame_offsets, out_offsets, window, out, bias)
+    assert magnitude.dtype == phase.dtype == torch.float32 and magnitude.is_contiguous() and phase.is_contiguous()
+    assert frame_offsets.dtype == out_offsets.dtype == torch.int64 and out.dtype == torch.float32
+    assert bias is None or (bias.dtype == torch.float32 and bias.is_contiguous() and bias.numel() == n_fft // 2 + 1)
+    check(lib().ft_stft_inverse(ptr(magnitude), ptr(phase), ptr(frame_offsets), ptr(out_offsets), int(n_utt), int(total_frames),
+                                ptr(window), int(n_fft), int(hop), ptr(bias), float(strength), ptr(out), stream_ptr()),
+          "ft_stft_inverse")
 
 
 def attn_prior(in_lens, out_lens, T, L, scaling, threshold, prior):

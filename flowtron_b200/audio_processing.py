@@ -6,8 +6,10 @@ filterbank, log; waveform read once, mel written once), for other sizes as frami
 magnitude / filterbank / log (csrc/mel.cu).  ``mel_spectrogram_packed`` / ``mel_spectrogram_ragged`` are the batched
 forms for a whole dataset shard (what data.py:149-155 does one utterance at a time on a CPU worker); int16 PCM input is
 scaled by 1/32768 on load (data.py:150).  ``STFT.transform`` returns (magnitude, phase) like the reference.
+``STFT.inverse`` (:237-265) is one kernel for filter_length 1024 and hop 128 / 256 / 512 (csrc/istft.cu: per-warp inverse
+FFT, window, overlap-add and the window sum-square normalisation), ``STFT.forward`` is transform + inverse, and
+``griffin_lim`` (:59-75) alternates the two; the WaveGlow Denoiser built on them is flowtron_b200.denoiser.
 Buffers ``mel_basis``, ``stft_fn.forward_basis``, ``stft_fn.inverse_basis`` keep the reference's state_dict layout.
-The inverse STFT / Griffin-Lim are not called by training or inference (SURVEY.md §2.1 row 5) and are not provided.
 """
 from __future__ import annotations
 
@@ -47,6 +49,13 @@ def _padded_window(win_length, filter_length):
     return np.pad(w, (lp, filter_length - win_length - lp))
 
 
+def aligned_waveform(x):
+    """x as a contiguous float32 tensor whose storage starts on an 8-byte boundary: the transform kernel reads sample pairs
+    as float2, so a view that starts at an odd float offset (e.g. one row of an odd-length batch) is copied first."""
+    x = x.detach().float().contiguous()
+    return x if x.data_ptr() % 8 == 0 else x.clone()
+
+
 class STFT(torch.nn.Module):
     def __init__(self, filter_length=800, hop_length=200, win_length=800, window='hann'):
         super().__init__()
@@ -84,7 +93,46 @@ class STFT(torch.nn.Module):
         return magnitude, phase
 
     def inverse(self, magnitude, phase):
-        raise NotImplementedError("inverse STFT is not on the Flowtron training/inference path")
+        """audio_processing.py:237-265: (magnitude, phase) [B, n_fft/2+1, F] -> [B, 1, (F-1) * hop].  CUDA only (one
+        kernel, filter_length 1024, hop 128 / 256 / 512); F == 1 gives an empty signal."""
+        if self.filter_length != 1024 or self.hop_length not in _lib.STFT_INVERSE_HOPS:
+            raise NotImplementedError("STFT.inverse is built for filter_length 1024 and hop_length 128, 256 or 512")
+        cutoff = self.filter_length // 2 + 1
+        if magnitude.dim() != 3 or magnitude.shape[1] != cutoff or magnitude.shape != phase.shape:
+            raise ValueError(f"magnitude and phase must both be [B, {cutoff}, F], got {tuple(magnitude.shape)} and "
+                             f"{tuple(phase.shape)}")
+        if not magnitude.is_cuda or not phase.is_cuda:
+            raise FlowtronB200Error("STFT.inverse needs CUDA tensors: the sm_90a path is the only implementation")
+        B, _, F = magnitude.shape
+        hop, dev = self.hop_length, magnitude.device
+        out = torch.empty(B, 1, (F - 1) * hop, device=dev)
+        if F == 1 or B == 0:
+            return out
+        fo = torch.arange(B + 1, device=dev, dtype=torch.int64) * F
+        oo = torch.arange(B, device=dev, dtype=torch.int64) * ((F - 1) * hop)
+        _lib.stft_inverse(magnitude.detach().float().contiguous(), phase.detach().float().contiguous(), fo, oo, B, B * F,
+                          self._window, self.filter_length, hop, out)
+        return out
+
+    def forward(self, input_data):
+        """audio_processing.py:267-270: transform, keep (magnitude, phase), return their inverse."""
+        self.magnitude, self.phase = self.transform(aligned_waveform(input_data))
+        return self.inverse(self.magnitude, self.phase)
+
+
+def griffin_lim(magnitudes, stft_fn, n_iters=30, *, angles=None):
+    """audio_processing.py:59-75: phase reconstruction from magnitudes [B, n_fft/2+1, F] (CUDA) -> signal [B, (F-1) * hop].
+    angles=None draws the initial phase as the reference does (numpy's global generator, so a numpy seed reproduces the
+    reference's draw) and copies it to the device once; explicit ``angles`` (CUDA, like magnitudes) make the call
+    1 + 2 n_iters kernel launches with no host work in between, so it can be captured in a CUDA graph."""
+    if angles is None:
+        a = np.angle(np.exp(2j * np.pi * np.random.rand(*magnitudes.size()))).astype(np.float32)
+        angles = torch.from_numpy(a).to(magnitudes.device)
+    signal = stft_fn.inverse(magnitudes, angles).squeeze(1)
+    for _ in range(n_iters):
+        _, angles = stft_fn.transform(signal)
+        signal = stft_fn.inverse(magnitudes, angles).squeeze(1)
+    return signal
 
 
 class TacotronSTFT(torch.nn.Module):

@@ -99,5 +99,23 @@ __host__ __device__ __forceinline__ cf split_bin(int k, const float* zr, const f
     return cadd(E, cmul(O, cf{w.x, w.y}));
 }
 
+// Inverse real FFT (istft.cu), the split run backwards: for a half spectrum X[0..512] the 1024-point irfft is
+//   z[n] = x[2n] + i x[2n+1] = IDFT512(Z)[n],  Z[k] = (X[k] + conj X[512-k])/2 + i (X[k] - conj X[512-k]) W1024^{-k}/2,
+// and IDFT512(Z) = conj(DFT512(conj Z))/512, so pass A..C above run unchanged on conj Z.  Like numpy's irfft, the
+// imaginary parts of X[0] and X[512] are ignored (a real signal's DC and Nyquist bins are real).
+// inv_pretwiddle returns conj Z[k] for k in [0, 512) from xk = X[k] and xc = X[512-k].
+__host__ __device__ __forceinline__ cf inv_pretwiddle(int k, cf xk, cf xc, const float2* tw) {
+    if (k == 0) { xk.y = 0.f; xc.y = 0.f; }
+    const cf E = {0.5f * (xk.x + xc.x), 0.5f * (xk.y - xc.y)};              // (X[k] + conj X')/2
+    const cf D = {0.5f * (xk.x - xc.x), 0.5f * (xk.y + xc.y)};              // (X[k] - conj X')/2
+    const float2 w = tw[k];
+    const cf O = cmul(D, cf{w.x, -w.y});                                     // * W1024^{-k}
+    return {E.x - O.y, -(E.y + O.x)};                                        // conj(E + i O)
+}
+// read-out after pass C on conj Z (zr / zi in natural order): sample m in [0, 1024) of the irfft
+__host__ __device__ __forceinline__ float inv_readout(int m, const float* zr, const float* zi) {
+    return (m & 1) ? -zi[m >> 1] * (1.0f / 512.0f) : zr[m >> 1] * (1.0f / 512.0f);
+}
+
 }  // namespace melfft
 }  // namespace ft

@@ -252,3 +252,26 @@ def synth_waveglow_noise(B: int, F: int, seed: int) -> torch.Tensor:
     """N(0, 1) noise [B, 8, 32 F] in WaveGlow.infer's `noise` layout."""
     g = torch.Generator(device="cpu").manual_seed(seed + 7919)
     return torch.randn(B, 8, 32 * F, generator=g)
+
+
+# ------------------------------------------------------------------------------------------------ inverse STFT / Denoiser
+def synth_istft_audio(B: int, N: int, seed: int) -> torch.Tensor:
+    """Speech-band test signal [B, N] in [-1, 1]: a few sinusoids with random frequencies, phases and slow amplitude
+    envelopes, plus white noise at -40 dB."""
+    g = torch.Generator(device="cpu").manual_seed(seed)
+    t = torch.arange(N, dtype=torch.float64)[None, None, :] / 22050.0
+    f = 80.0 + 3920.0 * torch.rand(B, 6, 1, generator=g, dtype=torch.float64)
+    ph = 2 * np.pi * torch.rand(B, 6, 1, generator=g, dtype=torch.float64)
+    env = 0.5 + 0.5 * torch.sin(2 * np.pi * (0.5 + 3.0 * torch.rand(B, 6, 1, generator=g, dtype=torch.float64)) * t)
+    y = (env * torch.sin(2 * np.pi * f * t + ph)).sum(1) / 6.0
+    y = y + 0.01 * torch.randn(B, N, generator=g, dtype=torch.float64)
+    return y.clamp(-1.0, 1.0).float()
+
+
+def synth_istft_spectrum(B: int, F: int, seed: int, n_bins: int = 513):
+    """A random, inconsistent (magnitude, phase) pair, each [B, n_bins, F] float32: magnitudes U[0, 2), phases U[-pi, pi),
+    non-zero phase at the DC and Nyquist bins included."""
+    g = torch.Generator(device="cpu").manual_seed(seed)
+    mag = 2.0 * torch.rand(B, n_bins, F, generator=g)
+    phase = (2.0 * torch.rand(B, n_bins, F, generator=g) - 1.0) * float(np.pi)
+    return mag, phase

@@ -213,6 +213,18 @@ int ft_stft_transform(const float* wav, const long long* sample_offsets, const l
                       long long total_frames, const float* window, int n_fft, int hop, float* magnitude, float* phase,
                       void* stream);
 
+/* STFT.inverse (audio_processing.py:237-265), n_fft == 1024, hop in {128, 256, 512}: magnitude / phase as per-utterance
+ * [513, F_u] blocks at frame_offsets[u] (prefix sums, n_utt + 1 entries, the layout ft_stft_transform writes) ->
+ * (F_u - 1) * hop samples per utterance written at out[out_offsets[u]] (n_utt entries read: prefix sums for a packed
+ * output, row starts for a padded one).  Frames are irfft'd, windowed with `window` (the zero-padded analysis window,
+ * 1024 floats), overlap-added, divided by the window's sum-square envelope where it exceeds FLT_MIN, and 512 samples
+ * are dropped at each end.  bias (513 floats, optional): the magnitude becomes max(m - strength * bias[k], 0) on load
+ * (tacotron2/waveglow/denoiser.py), so transform + inverse is the whole Denoiser.  One launch, deterministic (each
+ * sample sums its frames in utterance-local order: ragged rows equal B = 1 runs), no host sync. */
+int ft_stft_inverse(const float* magnitude, const float* phase, const long long* frame_offsets, const long long* out_offsets,
+                    int n_utt, long long total_frames, const float* window, int n_fft, int hop, const float* bias,
+                    float strength, float* out, void* stream);
+
 /* Data layer on the device (SURVEY.md 8f row 1).
  * ft_attn_prior: beta_binomial_prior_distribution (data.py:31-41) for a whole batch directly in DataCollate's zero-padded
  *   [B,T,L] layout (data.py:222-243): prior[b,i-1,k] = BetaBinomial(k; n=in_lens[b]-1, a=s*i, b=s*(out_lens[b]+1-i)) for
