@@ -230,10 +230,8 @@ struct Side {
 };
 static std::map<cudaStream_t, Side> g_sides;
 static std::mutex g_side_mu;
-static bool g_side_enabled = true;
 
 static Side* get_side(cudaStream_t main) {
-    if (!g_side_enabled) return nullptr;
     std::lock_guard<std::mutex> lk(g_side_mu);
     auto it = g_sides.find(main);
     if (it != g_sides.end()) return &it->second;
@@ -256,20 +254,13 @@ static void join_side(Side* sd, cudaStream_t main) {
     cudaStreamWaitEvent(main, sd->ev_side, 0);
 }
 
-// Streams of the experimental layer pipeline: sB runs the second recurrence, sC its per-chunk input-projection GEMMs.
+// Streams of the layer pipeline and the attention overlap.  sA / sB run the two recurrences at HIGH priority, so that when a
+// chunk ends its 64 SMs go to the next chunk (a cooperative launch that needs all of them at once) and not to queued CTAs of
+// the GEMM / attention kernels that share the machine; sC runs their per-chunk GEMMs one priority level above default streams.
 struct Pipe {
-    cudaStream_t sA = nullptr, sB = nullptr, sC = nullptr, sD = nullptr;      // sA / sB: HIGH-priority streams of the two recurrences, sC: their GEMMs,
-                                                                              // sD: lowest priority, work nobody waits for yet
-    cudaEvent_t evA = nullptr, evG = nullptr, evB = nullptr, ev0 = nullptr, evJ = nullptr, evD = nullptr;
+    cudaStream_t sA = nullptr, sB = nullptr, sC = nullptr;
+    cudaEvent_t evA = nullptr, evG = nullptr, evB = nullptr, ev0 = nullptr, evJ = nullptr;
 };
-// FT_PIPE_PRIO (default 1): the chunk kernels of the pipelined recurrences are launched on high-priority streams, so that when a
-// chunk ends its 64 SMs go to the next chunk (a cooperative launch that needs all of them at once) and not to queued CTAs of the
-// GEMM / attention kernels that share the machine.
-static bool pipe_prio() {
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("FT_PIPE_PRIO"); v = (!e || atoi(e) != 0) ? 1 : 0; }
-    return v == 1;
-}
 static std::map<cudaStream_t, Pipe> g_pipes;
 static Pipe* get_pipe(cudaStream_t main) {
     std::lock_guard<std::mutex> lk(g_side_mu);
@@ -278,14 +269,11 @@ static Pipe* get_pipe(cudaStream_t main) {
     Pipe pp;
     int prio_lo = 0, prio_hi = 0;
     cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);            // hi is numerically smaller
-    const int pr = pipe_prio() ? prio_hi : prio_lo;
-    if (cudaStreamCreateWithPriority(&pp.sA, cudaStreamNonBlocking, pr) != cudaSuccess) return nullptr;
-    if (cudaStreamCreateWithPriority(&pp.sB, cudaStreamNonBlocking, pr) != cudaSuccess) return nullptr;
-    const int mid = pipe_prio() && prio_hi < prio_lo - 1 ? prio_lo - 1 : prio_lo;      // the pipeline's own GEMMs beat sD's
+    if (cudaStreamCreateWithPriority(&pp.sA, cudaStreamNonBlocking, prio_hi) != cudaSuccess) return nullptr;
+    if (cudaStreamCreateWithPriority(&pp.sB, cudaStreamNonBlocking, prio_hi) != cudaSuccess) return nullptr;
+    const int mid = prio_hi < prio_lo - 1 ? prio_lo - 1 : prio_lo;
     if (cudaStreamCreateWithPriority(&pp.sC, cudaStreamNonBlocking, mid) != cudaSuccess) return nullptr;
-    if (cudaStreamCreateWithPriority(&pp.sD, cudaStreamNonBlocking, prio_lo) != cudaSuccess) return nullptr;
     cudaEventCreateWithFlags(&pp.evJ, cudaEventDisableTiming);
-    cudaEventCreateWithFlags(&pp.evD, cudaEventDisableTiming);
     cudaEventCreateWithFlags(&pp.evA, cudaEventDisableTiming);
     cudaEventCreateWithFlags(&pp.evG, cudaEventDisableTiming);
     cudaEventCreateWithFlags(&pp.evB, cudaEventDisableTiming);
@@ -382,9 +370,9 @@ int ar_step_fwd(const FtArStepDesc& d, const FtArStepWeights& w, const float* me
             return gemm_fwd(s2, rows, G, n.M, S.mel_in16 + r0 * n.M, n.M, F.w.w_ih_a, n.M, w.attn_lstm_b_ih, w.attn_lstm_b_hh, 0,
                             F.X1 + r0 * G, G, nullptr, 0);
         };
-        cudaStream_t sr = pipe_prio() ? pa->sA : st;                 // the attention LSTM's stream
+        cudaStream_t sr = pa->sA;                                    // the attention LSTM's stream
         cudaEventRecord(pa->ev0, st);
-        if (sr != st) cudaStreamWaitEvent(sr, pa->ev0, 0);
+        cudaStreamWaitEvent(sr, pa->ev0, 0);
         cudaStreamWaitEvent(pa->sB, pa->ev0, 0);
         cudaStreamWaitEvent(pa->sC, pa->ev0, 0);
         FT_TRY(kv_projections(pa->sC));
@@ -405,14 +393,13 @@ int ar_step_fwd(const FtArStepDesc& d, const FtArStepWeights& w, const float* me
         }
         cudaEventRecord(pa->evG, pa->sC);
         cudaStreamWaitEvent(st, pa->evG, 0);
-        if (sr != st) { cudaEventRecord(pa->evJ, sr); cudaStreamWaitEvent(st, pa->evJ, 0); }
+        cudaEventRecord(pa->evJ, sr);
+        cudaStreamWaitEvent(st, pa->evJ, 0);
         xproj0_done = true;
     } else {
     // attention_lstm: the 80-channel input projection is folded into the persistent recurrence (no [R,4096] projection
-    // tensor: one GEMM and 1 GB of HBM traffic less per flow); h lands in d16[:, 0:H].  FT_LSTM_XIN=0: separate GEMM.
-    static int xin = -1;
-    if (xin < 0) { const char* e = getenv("FT_LSTM_XIN"); xin = (!e || atoi(e) != 0) ? 1 : 0; }
-    if (xin && n.M <= 128 && n.B <= 32) {      // B > 32: the double-buffered x tile no longer fits next to a 64-row h tile
+    // tensor: one GEMM and 1 GB of HBM traffic less per flow); h lands in d16[:, 0:H].
+    if (n.M <= 128 && n.B <= 32) {             // B > 32: the double-buffered x tile no longer fits next to a 64-row h tile
         FT_TRY(launch_lstm_fwd_xin(n.T, n.B, S.mel_in16, n.M, n.M, F.w.w_ih_a, w.attn_lstm_b_ih, w.attn_lstm_b_hh, F.w.w_hh_a, out_lens,
                                    S.d16, n.D, S.gatesA, S.cA, F.hA32, H, F.flags, st));
     } else {
@@ -433,9 +420,9 @@ int ar_step_fwd(const FtArStepDesc& d, const FtArStepWeights& w, const float* me
         int* flagsA = F.flags;
         int* flagsB = F.flags + static_cast<size_t>(S_) * 16;
         if (!xproj0_done) FT_TRY(gemm_fwd(st, n.R, G, n.D, S.d16, n.D, F.w.w_ih0, n.D, w.lstm_b_ih0, w.lstm_b_hh0, 0, F.X, G, nullptr, 0));
-        cudaStream_t sr = pipe_prio() ? pp->sA : st;                 // layer 0's recurrence stream
+        cudaStream_t sr = pp->sA;                                    // layer 0's recurrence stream
         cudaEventRecord(pp->ev0, st);
-        if (sr != st) cudaStreamWaitEvent(sr, pp->ev0, 0);
+        cudaStreamWaitEvent(sr, pp->ev0, 0);
         cudaStreamWaitEvent(pp->sB, pp->ev0, 0);
         cudaStreamWaitEvent(pp->sC, pp->ev0, 0);
         for (int t0 = 0; t0 < n.T; t0 += S_) {
@@ -452,7 +439,8 @@ int ar_step_fwd(const FtArStepDesc& d, const FtArStepWeights& w, const float* me
         }
         cudaEventRecord(pp->evB, pp->sB);
         cudaStreamWaitEvent(st, pp->evB, 0);
-        if (sr != st) { cudaEventRecord(pp->evJ, sr); cudaStreamWaitEvent(st, pp->evJ, 0); }
+        cudaEventRecord(pp->evJ, sr);
+        cudaStreamWaitEvent(st, pp->evJ, 0);
     } else {
         if (!xproj0_done) FT_TRY(gemm_fwd(st, n.R, G, n.D, S.d16, n.D, F.w.w_ih0, n.D, w.lstm_b_ih0, w.lstm_b_hh0, 0, F.X, G, nullptr, 0));
         FT_TRY(launch_lstm_fwd(n.T, n.B, F.X, F.w.w_hh0, out_lens, S.h0_16, H, S.gates0, S.c0, nullptr, 0, F.flags, st));
@@ -474,8 +462,7 @@ int ar_step_fwd(const FtArStepDesc& d, const FtArStepWeights& w, const float* me
 int ar_step_bwd_main(const FtArStepDesc& d, const FtArStepWeights& w, const float* mel, const int* in_lens, const int* out_lens,
                      const float* attn, const float* d_mel_out, const float* d_log_s, const float* d_gates, const float* d_attn,
                      const float* d_logprob, float* d_text, const FtArStepWeights& g, void* saved, void* scratch, void* carry,
-                     cudaStream_t st, bool may_fuse_bptt = false, bool* bptt_done = nullptr) {
-    if (bptt_done) *bptt_done = false;
+                     cudaStream_t st) {
     FT_TRY(check_desc(d));
     const Dims n(d);
     Plan ps; ps.base = static_cast<uint8_t*>(saved);
@@ -507,8 +494,6 @@ int ar_step_bwd_main(const FtArStepDesc& d, const FtArStepWeights& w, const floa
     const float* S = C.scale;            // S[0] = scale, S[1] = 1/scale
     const float* iS = C.scale + 1;
 
-    static int side_env = -1;
-    if (side_env < 0) { const char* e = getenv("FT_SIDE_STREAM"); side_env = e ? atoi(e) : 1; g_side_enabled = side_env != 0; }
     Side* sd = get_side(st);
     cudaStream_t ss;
 
@@ -540,33 +525,6 @@ int ar_step_bwd_main(const FtArStepDesc& d, const FtArStepWeights& w, const floa
         FT_TRY(zero(g.gate_w, sizeof(float) * n.D, st));
         FT_TRY(zero(g.gate_b, sizeof(float), st));
     }
-    // Steps 6b-9a for the time steps [t0, t1): lstm layer 0's input gradient (dd = [dhA ; dctx]), the gate layer, the attention
-    // backward (tanh recompute; dK / dV / dv accumulate over calls) and the query projection's share of dhA.
-    auto attention_bwd_rows = [&](cudaStream_t s2, int t0, int t1) -> int {
-        const long long r0 = static_cast<long long>(t0) * n.B, rows = static_cast<long long>(t1 - t0) * n.B;
-        FT_TRY(gemm_dgrad(s2, rows, n.D, G, F.dG0 + r0 * G, G, F.w.w_ih0, n.D, 0, C.dd + r0 * n.D, n.D, nullptr, 0, nullptr, 0));
-        // 7. gate layer (last flow only): dd is in the scaled domain, the gate's own parameter gradients are not
-        if (d.has_gate && g.gate_w && d_gates)
-            FT_TRY(launch_gate_bwd(S_.d16 + r0 * n.D, n.D, n.D, w.gate_w, d_gates + r0, rows, C.dd + r0 * n.D, n.D, g.gate_w, g.gate_b, S, s2));
-        // 8. attention (score/softmax/context) with tanh recompute
-        AttnBwdArgs a;
-        a.T = n.T; a.B = n.B; a.L = n.L; a.A = n.A;
-        a.Q = S_.Q; a.ldq = n.A; a.K = S_.Kp; a.ldk = n.A; a.V = S_.Vp; a.ldv = n.A; a.v = w.att_v;
-        a.in_lens = in_lens; a.out_lens = out_lens; a.attn = attn; a.p_save = S_.p_save; a.temperature = d.temperature;
-        a.dctx = C.dd + H; a.lddc = n.D; a.dattn_ext = d_attn; a.dlp_ext = d_logprob; a.scale = S;
-        a.dQ = F.dQ; a.lddq = n.A; a.dK = F.dK; a.lddk = n.A; a.dV = F.dV; a.lddv = n.A; a.dv = g.att_v;
-        a.t_begin = t0; a.t_end = t1;
-        FT_TRY(launch_attn_bwd(a, s2));
-        // 9a. query projection (d16 = [hA ; ctx] saved in fp16, row pitch D)
-        FT_TRY(launch_cast(F.dQ + r0 * n.A, 2, F.dQ16 + r0 * n.A, 0, rows * n.A, s2));
-        FT_TRY(gemm_dgrad(s2, rows, H, n.A, F.dQ16 + r0 * n.A, n.A, F.w.wq, H, 1, C.dd + r0 * n.D, n.D, nullptr, 0, nullptr, 0));   // dhA += dQ Wq
-        return 0;
-    };
-    // FT_ATTB_PIPE=1 (needs FT_PIPE_CHUNK % 64 == 0): the attention backward of every chunk lstm layer 0's BPTT has finished runs on a
-    // lowest-priority stream on whatever the two recurrences and their GEMMs leave free, instead of after the pipeline.
-    static int attb_pipe = -1;
-    if (attb_pipe < 0) { const char* e = getenv("FT_ATTB_PIPE"); attb_pipe = e ? atoi(e) : 0; }
-    bool attention_bwd_done = false;
     Pipe* pp = (F.dcarry1 && n.B <= 32 && 2 * pipe_chunk_steps() <= n.T) ? get_pipe(st) : nullptr;
     if (pp) {
         // EXPERIMENTAL 5+6: BPTT of layer 1 (st) and layer 0 (sB) one chunk apart; the layer-1 dgrad of a finished chunk
@@ -575,9 +533,9 @@ int ar_step_bwd_main(const FtArStepDesc& d, const FtArStepWeights& w, const floa
         const int S_c = pipe_chunk_steps();
         int* flagsA = F.flags;
         int* flagsB = F.flags + static_cast<size_t>(S_c) * 64;
-        cudaStream_t sr = pipe_prio() ? pp->sA : st;                 // layer 1's BPTT stream
+        cudaStream_t sr = pp->sA;                                    // layer 1's BPTT stream
         cudaEventRecord(pp->ev0, st);
-        if (sr != st) cudaStreamWaitEvent(sr, pp->ev0, 0);
+        cudaStreamWaitEvent(sr, pp->ev0, 0);
         cudaStreamWaitEvent(pp->sB, pp->ev0, 0);
         cudaStreamWaitEvent(pp->sC, pp->ev0, 0);
         const int n_chunks = (n.T + S_c - 1) / S_c;
@@ -591,17 +549,10 @@ int ar_step_bwd_main(const FtArStepDesc& d, const FtArStepWeights& w, const floa
             cudaEventRecord(pp->evG, pp->sC);
             cudaStreamWaitEvent(pp->sB, pp->evG, 0);
             FT_TRY(launch_lstm_bwd_chunk(n.T, n.B, t0, t1, F.dh, H, F.w.w_hh0, S_.gates0, S_.c0, out_lens, F.dG0, F.dcarry0, flagsB, pp->sB));
-            if (attb_pipe && S_c % 64 == 0) {
-                if (c == n_chunks - 1) cudaStreamWaitEvent(pp->sD, pp->ev0, 0);
-                cudaEventRecord(pp->evD, pp->sB);
-                cudaStreamWaitEvent(pp->sD, pp->evD, 0);
-                FT_TRY(attention_bwd_rows(pp->sD, t0, t1));
-                attention_bwd_done = true;
-            }
         }
-        if (attention_bwd_done) { cudaEventRecord(pp->evD, pp->sD); cudaStreamWaitEvent(st, pp->evD, 0); }
         // layer-1 weight gradients run under the tail of layer 0 (side stream forks from st = all of layer 1 done)
-        if (sr != st) { cudaEventRecord(pp->evJ, sr); cudaStreamWaitEvent(st, pp->evJ, 0); }
+        cudaEventRecord(pp->evJ, sr);
+        cudaStreamWaitEvent(st, pp->evJ, 0);
         ss = fork_side(sd, st);
         FT_TRY(gemm_wgrad(ss, G, H, Rm, F.dG1 + static_cast<size_t>(n.B) * G, G, S_.h1_16, H, g.lstm_w_hh1, H, iS));
         FT_TRY(gemm_wgrad(ss, G, H, R, F.dG1, G, S_.h0_16, H, g.lstm_w_ih1, H, iS));
@@ -624,35 +575,23 @@ int ar_step_bwd_main(const FtArStepDesc& d, const FtArStepWeights& w, const floa
     }
     // (the weight gradients of lstm layer 0 and of the attention projections are launched by ar_step_bwd_attn, on the side
     //  stream underneath the attention LSTM's BPTT: dG0, dQ16, dK16, dV16 stay in the scratch area until then)
-    // Attention backward / attention-LSTM BPTT overlap (the mirror image of the forward overlap; FT_ATT_OVERLAP_BWD = chunk length,
-    // default 256, 0 disables): only when the caller lets this call run the attention LSTM's BPTT as well (ft_ar_step_bwd: flows
-    // whose d_text nobody is waiting for).  Highest chunk first: the second stream prepares chunk c's dhA while the BPTT kernel
-    // (64 SMs) works on chunk c + 1.
-    static int attb_chunk = -1;
-    if (attb_chunk < 0) { const char* e = getenv("FT_ATT_OVERLAP_BWD"); attb_chunk = e ? atoi(e) : 256; if (attb_chunk % 64) attb_chunk = 0; }
-    Pipe* pq = (may_fuse_bptt && !attention_bwd_done && attb_chunk > 0 && F.dcarry1 && n.B <= 32 && n.T >= attb_chunk + 64) ? get_pipe(st) : nullptr;
-    if (pq) {
-        FT_TRY(launch_cast(w.attn_lstm_w_ih, 2, F.w.w_ih_a, 0, static_cast<long long>(G) * n.M, st));
-        FT_TRY(launch_transpose_cast_f16(w.attn_lstm_w_hh, F.w.w_hh_a, G, H, st));
-        cudaStream_t sr = pipe_prio() ? pq->sA : st;
-        cudaEventRecord(pq->ev0, st);
-        if (sr != st) cudaStreamWaitEvent(sr, pq->ev0, 0);
-        cudaStreamWaitEvent(pq->sC, pq->ev0, 0);
-        const int CH = attb_chunk, n_chunks = (n.T + CH - 1) / CH;
-        for (int c = n_chunks - 1; c >= 0; --c) {
-            const int t0 = c * CH, t1 = t0 + CH < n.T ? t0 + CH : n.T;
-            FT_TRY(attention_bwd_rows(pq->sC, t0, t1));
-            cudaEventRecord(pq->evG, pq->sC);
-            cudaStreamWaitEvent(sr, pq->evG, 0);
-            // 10. attention_lstm  (dhA = C.dd[:, 0:H], pitch D)
-            FT_TRY(launch_lstm_bwd_chunk(n.T, n.B, t0, t1, C.dd, n.D, F.w.w_hh_a, S_.gatesA, S_.cA, out_lens, F.dGa, F.dcarry1, F.flags, sr));
-        }
-        cudaStreamWaitEvent(st, pq->evG, 0);          // all of sC (the last record) ...
-        if (sr != st) { cudaEventRecord(pq->evJ, sr); cudaStreamWaitEvent(st, pq->evJ, 0); }     // ... and the BPTT
-        if (bptt_done) *bptt_done = true;
-    } else if (!attention_bwd_done) {
-        FT_TRY(attention_bwd_rows(st, 0, n.T));
-    }
+    // 6b. lstm layer 0's input gradient: dd = [dhA ; dctx]
+    FT_TRY(gemm_dgrad(st, R, n.D, G, F.dG0, G, F.w.w_ih0, n.D, 0, C.dd, n.D, nullptr, 0, nullptr, 0));
+    // 7. gate layer (last flow only): dd is in the scaled domain, the gate's own parameter gradients are not
+    if (d.has_gate && g.gate_w && d_gates)
+        FT_TRY(launch_gate_bwd(S_.d16, n.D, n.D, w.gate_w, d_gates, R, C.dd, n.D, g.gate_w, g.gate_b, S, st));
+    // 8. attention (score/softmax/context) with tanh recompute; dK / dV / dv accumulate
+    AttnBwdArgs a;
+    a.T = n.T; a.B = n.B; a.L = n.L; a.A = n.A;
+    a.Q = S_.Q; a.ldq = n.A; a.K = S_.Kp; a.ldk = n.A; a.V = S_.Vp; a.ldv = n.A; a.v = w.att_v;
+    a.in_lens = in_lens; a.out_lens = out_lens; a.attn = attn; a.p_save = S_.p_save; a.temperature = d.temperature;
+    a.dctx = C.dd + H; a.lddc = n.D; a.dattn_ext = d_attn; a.dlp_ext = d_logprob; a.scale = S;
+    a.dQ = F.dQ; a.lddq = n.A; a.dK = F.dK; a.lddk = n.A; a.dV = F.dV; a.lddv = n.A; a.dv = g.att_v;
+    a.t_begin = 0; a.t_end = n.T;
+    FT_TRY(launch_attn_bwd(a, st));
+    // 9a. query projection (d16 = [hA ; ctx] saved in fp16, row pitch D)
+    FT_TRY(launch_cast(F.dQ, 2, F.dQ16, 0, R * n.A, st));
+    FT_TRY(gemm_dgrad(st, R, H, n.A, F.dQ16, n.A, F.w.wq, H, 1, C.dd, n.D, nullptr, 0, nullptr, 0));   // dhA += dQ Wq
 
     // 9b. key / value projections -> d_text
     FT_TRY(launch_cast(F.dK, 2, F.dK16, 0, RL * n.A, st));
@@ -667,7 +606,7 @@ int ar_step_bwd_main(const FtArStepDesc& d, const FtArStepWeights& w, const floa
 // Attention-LSTM part: BPTT over dhA (carry), its weight gradients, and the input gradient d_mel (coupling path from carry +
 // the shifted attention-LSTM path, back to natural time, loss scale undone).
 int ar_step_bwd_attn(const FtArStepDesc& d, const FtArStepWeights& w, const int* out_lens, float* d_mel, const FtArStepWeights& g,
-                     void* saved, void* scratch, void* carry, cudaStream_t st, bool bptt_done = false) {
+                     void* saved, void* scratch, void* carry, cudaStream_t st) {
     FT_TRY(check_desc(d));
     const Dims n(d);
     Plan ps; ps.base = static_cast<uint8_t*>(saved);
@@ -681,10 +620,8 @@ int ar_step_bwd_attn(const FtArStepDesc& d, const FtArStepWeights& w, const int*
     Side* sd = get_side(st);
     cudaStream_t ss;
     const long long RL = n.RL;
-    if (!bptt_done) {                    // (a fused ar_step_bwd_main made these copies and ran the BPTT already)
-        FT_TRY(launch_cast(w.attn_lstm_w_ih, 2, F.w.w_ih_a, 0, static_cast<long long>(G) * n.M, st));
-        FT_TRY(launch_transpose_cast_f16(w.attn_lstm_w_hh, F.w.w_hh_a, G, H, st));
-    }
+    FT_TRY(launch_cast(w.attn_lstm_w_ih, 2, F.w.w_ih_a, 0, static_cast<long long>(G) * n.M, st));
+    FT_TRY(launch_transpose_cast_f16(w.attn_lstm_w_hh, F.w.w_hh_a, G, H, st));
 
     // deferred from ar_step_bwd_main: weight gradients of lstm layer 0 and of the attention projections, on the side stream,
     // underneath the BPTT kernel below (64 of the SMs)
@@ -698,7 +635,7 @@ int ar_step_bwd_attn(const FtArStepDesc& d, const FtArStepWeights& w, const int*
     FT_TRY(gemm_wgrad(ss, n.A, n.E, RL, F.dV16, n.A, S_.text16, n.E, g.att_value, n.E, iS));
 
     // 10. attention_lstm  (dhA = C.dd[:, 0:H], pitch D)
-    if (!bptt_done) FT_TRY(launch_lstm_bwd(n.T, n.B, C.dd, n.D, F.w.w_hh_a, S_.gatesA, S_.cA, out_lens, F.dGa, F.flags, st));
+    FT_TRY(launch_lstm_bwd(n.T, n.B, C.dd, n.D, F.w.w_hh_a, S_.gatesA, S_.cA, out_lens, F.dGa, F.flags, st));
     ss = fork_side(sd, st);
     FT_TRY(gemm_wgrad(ss, G, H, Rm, F.dGa + static_cast<size_t>(n.B) * G, G, S_.d16, n.D, g.attn_lstm_w_hh, H, iS));
     FT_TRY(gemm_wgrad(ss, G, n.M, R, F.dGa, G, S_.mel_in16, n.M, g.attn_lstm_w_ih, n.M, iS));
@@ -759,10 +696,9 @@ int ft_ar_step_bwd(const FtArStepDesc* d, const FtArStepWeights* w, const float*
     if (!d || !w || !mel || !attn || !d_text || !g || !saved || !scratch) return ft::ft_set_error("ft_ar_step_bwd: NULL argument");
     ft::Plan pb; ft::BwdScratch b; b.plan(pb, *d);
     void* carry = static_cast<uint8_t*>(scratch) + ((pb.off + 255) & ~static_cast<size_t>(255));
-    bool bptt_done = false;           // the one-call form may overlap the attention backward with the attention LSTM's BPTT
     if (ft::ar_step_bwd_main(*d, *w, mel, in_lens, out_lens, attn, d_mel_out, d_log_s, d_gates, d_attn, d_attn_logprob, d_text, *g,
-                             saved, scratch, carry, static_cast<cudaStream_t>(stream), true, &bptt_done) != 0) return -1;
-    return ft::ar_step_bwd_attn(*d, *w, out_lens, d_mel, *g, saved, scratch, carry, static_cast<cudaStream_t>(stream), bptt_done);
+                             saved, scratch, carry, static_cast<cudaStream_t>(stream)) != 0) return -1;
+    return ft::ar_step_bwd_attn(*d, *w, out_lens, d_mel, *g, saved, scratch, carry, static_cast<cudaStream_t>(stream));
 }
 
 int ft_ar_step_bwd_main(const FtArStepDesc* d, const FtArStepWeights* w, const float* mel, const int* in_lens,

@@ -24,7 +24,6 @@
 // Warp roles: warps 0-3 form one warpgroup that issues the wgmma of a step and runs the cell epilogue on the
 // accumulator; warp 4 is the TMA producer.  Loads are issued as few multi-chunk 3-D boxes: issuing 16 (64) 2-D loads
 // serially from one thread puts the issue time on the recurrence's critical path.
-#include <cstdlib>
 #include <type_traits>
 
 #include "ptx.cuh"
@@ -68,6 +67,7 @@ __device__ __forceinline__ void mma_chunks(float* acc, uint64_t da, uint64_t db,
 
 // ------------------------------------------------------------------------------------------- forward
 constexpr int FWD_NCH = LH / KCH;                  // 16 chunks / step
+constexpr int FWD_GS = 8;                          // K chunks per TMA group: 2 groups per step
 // FWD_UNITS hidden units per CTA: 8 -> 128 CTAs (whole GPU, lowest latency), 16 -> 64 CTAs (two such launches on two
 // streams -- one per half batch -- run concurrently and hide each other's exchange latency)
 
@@ -510,7 +510,7 @@ struct LstmFwdChunkParams : LstmFwdParams {
 // Requires x_0 == 0 (the teacher-forcing shift guarantees it): step 0 has no contraction at all.
 constexpr int XCH = 2;                                           // extra K chunks (128 input channels max)
 
-template <int FWD_GS, int FWD_UNITS, bool kXIn>
+template <int FWD_UNITS, bool kXIn>
 __global__ void __launch_bounds__(LSTM_THREADS, 1)
 lstm_fwd_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmH, const __grid_constant__ CUtensorMap tmWx,
                 const __grid_constant__ CUtensorMap tmX, LstmFwdChunkParams p) {
@@ -799,7 +799,7 @@ void set_lstm_half_sm(int on) { g_half_sm = on != 0; }
 
 // Steps [t0, t1) of one layer's forward recurrence on 1024 / UNITS CTAs.  `flags` needs (t1 - t0) * 16 ints.
 // x16 != null: folded input projection (kXIn): x16 [T*B, kx] fp16 (row pitch ldx), wih16 [4096, kx] fp16, biases fp32.
-template <int GS, int UNITS, bool kXIn>
+template <int UNITS, bool kXIn>
 static int launch_fwd_t(int T, int B, int t0, int t1, const float* xproj, const void* whh16, const int* lens, void* hseq16,
                         long long ldh, void* gates16, float* cstate, float* h32, long long ldh32, int* flags, cudaStream_t st,
                         const void* x16 = nullptr, long long ldx = 0, int kx = 0, const void* wih16 = nullptr,
@@ -816,7 +816,7 @@ static int launch_fwd_t(int T, int B, int t0, int t1, const float* xproj, const 
     if (smem > smem_optin()) return ft_set_error("lstm_fwd: not enough shared memory");
     CUtensorMap tmW, tmH, tmWx, tmX;
     if (make_tmap_2d(&tmW, whh16, FMT_F16, LG, LH, LH, KCH, UNITS)) return -1;
-    if (make_tmap_chunks(&tmH, hseq16, static_cast<long long>(T) * B, FWD_NCH, ldh, p.Bbox, GS)) return -1;
+    if (make_tmap_chunks(&tmH, hseq16, static_cast<long long>(T) * B, FWD_NCH, ldh, p.Bbox, FWD_GS)) return -1;
     if (kXIn) {
         if (kx <= 0 || kx > XCH * KCH) return ft_set_error("lstm_fwd: folded input width must be in (0, 128]");
         if (make_tmap_2d(&tmWx, wih16, FMT_F16, LG, kx, kx, KCH, UNITS)) return -1;
@@ -825,7 +825,7 @@ static int launch_fwd_t(int T, int B, int t0, int t1, const float* xproj, const 
         tmWx = tmW; tmX = tmH;                                   // unused
     }
     if (cudaMemsetAsync(flags, 0, sizeof(int) * (t1 - t0) * FWD_NCH, st) != cudaSuccess) return ft_set_error("lstm_fwd: memset failed");
-    void* fn = reinterpret_cast<void*>(lstm_fwd_kernel<GS, UNITS, kXIn>);
+    void* fn = reinterpret_cast<void*>(lstm_fwd_kernel<UNITS, kXIn>);
     cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     TimeScope ts("lstm_fwd", t1 - t0, B, 0, st);
     void* args[] = {&tmW, &tmH, &tmWx, &tmX, &p};
@@ -839,12 +839,8 @@ int launch_lstm_fwd(int T, int B, const float* xproj, const void* whh16, const i
                     void* gates16, float* cstate, float* h32, long long ldh32, int* flags, cudaStream_t st) {
     if (T <= 0 || B <= 0) return 0;
     if (B > 64) return ft_set_error("lstm_fwd: batch > 64 per call not supported (split the batch)");
-    if (g_half_sm && B <= 32) return launch_fwd_t<8, 16, false>(T, B, 0, T, xproj, whh16, lens, hseq16, ldh, gates16, cstate, h32, ldh32, flags, st);
-    static int gs = -1;            // FT_LSTM_FWD_GS: K-chunks per TMA group (16 / gs groups per step), tuning knob
-    if (gs < 0) { const char* e = getenv("FT_LSTM_FWD_GS"); gs = e ? atoi(e) : 8; }
-    if (gs == 4) return launch_fwd_t<4, 8, false>(T, B, 0, T, xproj, whh16, lens, hseq16, ldh, gates16, cstate, h32, ldh32, flags, st);
-    if (gs == 16) return launch_fwd_t<16, 8, false>(T, B, 0, T, xproj, whh16, lens, hseq16, ldh, gates16, cstate, h32, ldh32, flags, st);
-    return launch_fwd_t<8, 8, false>(T, B, 0, T, xproj, whh16, lens, hseq16, ldh, gates16, cstate, h32, ldh32, flags, st);
+    if (g_half_sm && B <= 32) return launch_fwd_t<16, false>(T, B, 0, T, xproj, whh16, lens, hseq16, ldh, gates16, cstate, h32, ldh32, flags, st);
+    return launch_fwd_t<8, false>(T, B, 0, T, xproj, whh16, lens, hseq16, ldh, gates16, cstate, h32, ldh32, flags, st);
 }
 
 // Whole sequence with the input projection folded in (narrow inputs, kx <= 128; x16 row 0..B-1 must be zero: step 0 skips the
@@ -856,8 +852,8 @@ int launch_lstm_fwd_xin(int T, int B, const void* x16, long long ldx, int kx, co
     if (B > 64) return ft_set_error("lstm_fwd: batch > 64 per call not supported (split the batch)");
     if (!x16 || !wih16 || !b_ih || !b_hh) return ft_set_error("lstm_fwd_xin: NULL argument");
     if (g_half_sm && B <= 32)
-        return launch_fwd_t<8, 16, true>(T, B, 0, T, nullptr, whh16, lens, hseq16, ldh, gates16, cstate, h32, ldh32, flags, st, x16, ldx, kx, wih16, b_ih, b_hh);
-    return launch_fwd_t<8, 8, true>(T, B, 0, T, nullptr, whh16, lens, hseq16, ldh, gates16, cstate, h32, ldh32, flags, st, x16, ldx, kx, wih16, b_ih, b_hh);
+        return launch_fwd_t<16, true>(T, B, 0, T, nullptr, whh16, lens, hseq16, ldh, gates16, cstate, h32, ldh32, flags, st, x16, ldx, kx, wih16, b_ih, b_hh);
+    return launch_fwd_t<8, true>(T, B, 0, T, nullptr, whh16, lens, hseq16, ldh, gates16, cstate, h32, ldh32, flags, st, x16, ldx, kx, wih16, b_ih, b_hh);
 }
 
 // Steps [t0, t1) of a layer on 64 CTAs (layer pipeline, ar_step.cu).  `flags` needs (t1 - t0) * 16 ints.
@@ -866,7 +862,7 @@ int launch_lstm_fwd_chunk(int T, int B, int t0, int t1, const float* xproj, cons
     if (T <= 0 || B <= 0 || t1 <= t0) return 0;
     if (B > 64 || t0 < 0 || t1 > T) return ft_set_error("lstm_fwd_chunk: bad batch or step range");
     if (t0 > 0 && !cstate) return ft_set_error("lstm_fwd_chunk: resuming a chunk needs the saved cell states");
-    return launch_fwd_t<8, 16, false>(T, B, t0, t1, xproj, whh16, lens, hseq16, ldh, gates16, cstate, h32, ldh32, flags, st);
+    return launch_fwd_t<16, false>(T, B, t0, t1, xproj, whh16, lens, hseq16, ldh, gates16, cstate, h32, ldh32, flags, st);
 }
 
 // Steps [t0, t1) of a layer's BPTT with the split-K cluster kernel, B <= 32.  `flags` needs (t1 - t0) * 64 ints; `dc_carry`
@@ -892,9 +888,7 @@ static int launch_bwd4(int T, int B, int t0, int t1, const float* dh_ext, long l
     attrs[0].val.clusterDim.x = B4_CLUSTER; attrs[0].val.clusterDim.y = 1; attrs[0].val.clusterDim.z = 1;
     attrs[1].id = cudaLaunchAttributeCooperative;
     attrs[1].val.cooperative = 1;
-    static int coop = -1;          // FT_BWD_COOP=0: plain cluster launch (for profilers that cannot replay cooperative + cluster launches)
-    if (coop < 0) { const char* e = getenv("FT_BWD_COOP"); coop = e ? atoi(e) : 1; }
-    cfg.attrs = attrs; cfg.numAttrs = coop ? 2 : 1;
+    cfg.attrs = attrs; cfg.numAttrs = 2;
     TimeScope ts("lstm_bwd", t1 - t0, B, 0, st);
     cudaError_t e = cudaLaunchKernelEx(&cfg, lstm_bwd4_kernel, tmWT, tmG, p);
     if (e != cudaSuccess) {                                  // co-residency is implied by 64 CTAs <= SMs; retry without the attribute
@@ -918,9 +912,7 @@ int launch_lstm_bwd(int T, int B, const float* dh_ext, long long ldd, const void
                     const float* cstate, const int* lens, void* dG16, int* flags, cudaStream_t st) {
     if (T <= 0 || B <= 0) return 0;
     if (B > 64) return ft_set_error("lstm_bwd: batch > 64 per call not supported (split the batch)");
-    static int use_cluster = -1;
-    if (use_cluster < 0) { const char* e = getenv("FT_LSTM_BWD_CLUSTER"); use_cluster = e ? atoi(e) : 1; }
-    if (B <= 32 && use_cluster)
+    if (B <= 32)
         return launch_bwd4(T, B, 0, T, dh_ext, ldd, whhT16, gates16, cstate, lens, dG16, nullptr, flags, st);
     LstmBwdParams p;
     p.T = T; p.B = B; p.Bbox = (B + 7) & ~7;
@@ -928,7 +920,6 @@ int launch_lstm_bwd(int T, int B, const float* dh_ext, long long ldd, const void
     const int fixed = BWD_W_BYTES + 128 * 17 * 4 + 512 + 1024;
     const int avail = smem_optin() - fixed;
     int gs = 8;
-    { const char* e = getenv("FT_LSTM_BWD_GS"); if (e) { int v = atoi(e); if (v == 2 || v == 4 || v == 8 || v == 16) gs = v; } }
     while (gs > 2 && 2 * gs * slot > avail) gs >>= 1;          // at least a 2-deep ring of groups (gs stays even)
     int nring = avail / (gs * slot);
     if (nring > 8) nring = 8;

@@ -12,7 +12,6 @@
 // consecutive frames) and the output.  Bound: HBM by the task's rule (1,344 B/frame); in practice the fp32 FFT
 // (~30 kFLOP/frame) and its shared-memory exchange (~25 KB/frame) are the limiters (DESIGN.md 4.5).
 // Waveform formats: f32 in [-1, 1], or int16 PCM scaled by 1/32768 on load (data.py:150 `audio / max_wav_value`).
-#include <cstdlib>
 #include "ft_internal.h"
 #include "mel_fft.cuh"
 #include "../../include/flowtron_b200.h"
@@ -44,7 +43,7 @@ __device__ __forceinline__ int mf_find_utt(const long long* __restrict__ frame_o
 
 template <int kFmt>
 struct FrameSrc {
-    const void* wav; long long s0, N, start; const float* swin; bool fast; bool win_global;
+    const void* wav; long long s0, N, start; const float* window; bool fast;
     __device__ __forceinline__ float ld(long long i) const {
         if (kFmt == 0) return __ldg(static_cast<const float*>(wav) + s0 + i);
         return static_cast<float>(__ldg(static_cast<const short*>(wav) + s0 + i)) * (1.0f / 32768.0f);
@@ -70,28 +69,27 @@ struct FrameSrc {
             i1 = i1 < 0 ? 0 : (i1 >= N ? N - 1 : i1);
             a = ld(i0); b = ld(i1);
         }
-        const float2 w = win_global ? __ldg(reinterpret_cast<const float2*>(swin + m)) : *reinterpret_cast<const float2*>(swin + m);
+        const float2 w = __ldg(reinterpret_cast<const float2*>(window + m));
         return make_float2(a * w.x, b * w.y);
     }
 };
 
-// kOcc: CTAs per SM the kernel is compiled for.  3 (default): 80 registers instead of 128 and the analysis window read
-// through the read-only cache instead of a shared-memory copy (72.5 KB per CTA), for 24 instead of 16 FFT warps per SM -- the
-// kernel is latency-bound on its shared-memory FFT passes.
-template <int kFmt, bool kTransform, int kOcc>
-__global__ void __launch_bounds__(MF_THREADS, kOcc)
+// Compiled for MF_OCC CTAs per SM (at most 80 registers): 24 FFT warps per SM rather than 16, because the kernel is
+// latency-bound on its shared-memory FFT passes.
+constexpr int MF_OCC = 3;
+
+template <int kFmt, bool kTransform>
+__global__ void __launch_bounds__(MF_THREADS, MF_OCC)
 mel_fused_kernel(MelFusedParams p) {
     extern __shared__ __align__(16) uint8_t smem_raw[];
     float2* stw = reinterpret_cast<float2*>(smem_raw);                       // [1024]
-    float* swin_s = reinterpret_cast<float*>(stw + 1024);                    // [1024] (kOcc == 2 only)
-    float* sx = swin_s + (kOcc == 2 ? 1024 : 0);                             // [8 warps][MF_WARP_FLOATS]
-    const float* swin = kOcc == 2 ? swin_s : p.window;
+    float* sx = reinterpret_cast<float*>(stw + 1024);                        // [8 warps][MF_WARP_FLOATS]
     float* smel = sx + MF_WARPS * MF_WARP_FLOATS;                            // [n_mel][33]
     long long* sbase = reinterpret_cast<long long*>(smel + ((p.n_mel * 33 + 1) & ~1));   // [32] output offset of (m = 0, frame)
     int* sFu = reinterpret_cast<int*>(sbase + MF_TILE);                      // [32] frames of the frame's utterance (0 = no frame)
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    for (int i = threadIdx.x; i < 1024; i += MF_THREADS) { stw[i] = p.twiddle[i]; if (kOcc == 2) swin_s[i] = p.window[i]; }
+    for (int i = threadIdx.x; i < 1024; i += MF_THREADS) stw[i] = p.twiddle[i];
     __syncthreads();
     float* xr = sx + warp * MF_WARP_FLOATS;
     float* xi = xr + XBUF;
@@ -108,7 +106,7 @@ mel_fused_kernel(MelFusedParams p) {
             const int Fu = static_cast<int>(__ldg(p.frame_offsets + u + 1) - fo);
             const long long j = f - fo;
             FrameSrc<kFmt> src;
-            src.wav = p.wav; src.swin = swin; src.win_global = (kOcc != 2);
+            src.wav = p.wav; src.window = p.window;
             src.s0 = __ldg(p.sample_offsets + u);
             src.N = __ldg(p.sample_offsets + u + 1) - src.s0;
             src.start = j * p.hop - NFFT / 2;
@@ -188,17 +186,15 @@ static int ensure_twiddle() {
 
 template <int kFmt, bool kTransform>
 static int launch_mel_fused(MelFusedParams& p, cudaStream_t st) {
-    static int occ = -1;           // FT_MEL_OCC=2: 128 registers, window in shared memory
-    if (occ < 0) { const char* e = getenv("FT_MEL_OCC"); occ = (e && atoi(e) == 2) ? 2 : 3; }
-    const size_t smem = 1024 * 8 + (occ == 2 ? 1024 * 4 : 0) + sizeof(float) * MF_WARPS * MF_WARP_FLOATS +
+    const size_t smem = 1024 * 8 + sizeof(float) * MF_WARPS * MF_WARP_FLOATS +
                         sizeof(float) * ((p.n_mel * 33 + 1) & ~1) + MF_TILE * 8 + MF_TILE * 4 + 16;
-    auto fn = occ == 2 ? mel_fused_kernel<kFmt, kTransform, 2> : mel_fused_kernel<kFmt, kTransform, 3>;
+    auto fn = mel_fused_kernel<kFmt, kTransform>;
     cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
     int dev = 0, sms = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const long long n_tiles = (p.total_frames + MF_TILE - 1) / MF_TILE;
-    const long long cap = static_cast<long long>(sms) * occ;           // persistent: `occ` CTAs per SM
+    const long long cap = static_cast<long long>(sms) * MF_OCC;        // persistent: MF_OCC CTAs per SM
     const int grid = static_cast<int>(n_tiles < cap ? n_tiles : cap);
     TimeScope ts(kTransform ? "stft_fused" : "mel_fused", p.total_frames, NFFT, p.n_mel, st);
     fn<<<grid, MF_THREADS, smem, st>>>(p);

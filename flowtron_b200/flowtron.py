@@ -102,13 +102,6 @@ def _encoder_overlap_stream(device):
     return _enc_streams[key]
 
 
-def _encoder_side_stream(device):
-    key = (device.type, device.index)
-    if key not in _enc_streams:
-        _enc_streams[key] = torch.cuda.Stream(device=device)
-    return _enc_streams[key]
-
-
 class _EncoderFn(torch.autograd.Function):
     """Encoder.forward / Encoder.infer on the CUDA kernels (ft_encoder_fwd / ft_encoder_bwd)."""
 
@@ -191,8 +184,6 @@ class Encoder(nn.Module):
         self.convolutions = nn.ModuleList(convolutions)
         self.lstm = nn.LSTM(encoder_embedding_dim, int(encoder_embedding_dim / 2), 1, batch_first=True, bidirectional=True)
         self.p_dropout = 0.5        # flowtron.py:502 hard-codes 0.5; exposed so tests can run deterministic train-mode steps
-        # FT_ENC_STREAMS=1: run the two LSTM directions concurrently (parity-tested; off by default)
-        self.two_streams = os.environ.get("FT_ENC_STREAMS", "0") != "0"
         self.use_kernels = os.environ.get("FT_ENC_KERNELS", "1") != "0"
         self._rng = None
 
@@ -246,10 +237,8 @@ class Encoder(nn.Module):
         """Same result as the reference's packed BiLSTM (flowtron.py:505-512) without packing: the forward direction is
         causal, so running it over the padded batch and zeroing t >= len is identical; the reverse direction runs on
         each utterance reversed inside its own length (one gather in, one gather out).  No pack/unpack and no host sync
-        (`in_lens.cpu()`); cuDNN still launches its per-time-step fp32 kernels (measured: same GPU time as packed), and
-        they are latency-bound, so with ``two_streams`` the two directions run concurrently on two CUDA streams (autograd
-        replays each direction's backward on the stream its forward ran on).  Requires the text batch to be padded to
-        max(in_lens), which DataCollate guarantees (data.py:200-208)."""
+        (`in_lens.cpu()`); cuDNN still launches its per-time-step fp32 kernels (measured: same GPU time as packed).
+        Requires the text batch to be padded to max(in_lens), which DataCollate guarantees (data.py:200-208)."""
         if self._kernels_ok(x):
             return _EncoderFn.apply(self, x, in_lens, x.size(0) > 1, self.p_dropout if self.training else 0.0, *self._kernel_params())
         Bn, _, L = x.shape
@@ -262,18 +251,8 @@ class Encoder(nn.Module):
             x = F.dropout(F.relu(norm(conv(x), mask=mask)), self.p_dropout, self.training)
         x = x.transpose(1, 2).contiguous()                                        # [B, L, C]
         rev = torch.where(valid, in_lens[:, None] - 1 - ar[None, :], ar[None, :])   # per-utterance time reversal (involution)
-        if self.two_streams and x.is_cuda:
-            cur = torch.cuda.current_stream(x.device)
-            side = _encoder_side_stream(x.device)
-            side.wait_stream(cur)
-            with torch.cuda.stream(side):
-                bwd = self._reverse_dir(x, rev)
-            fwd = self._lstm_dir(x, "")
-            cur.wait_stream(side)
-            bwd.record_stream(cur)                # allocated from the side stream's pool, consumed on the caller's stream
-        else:
-            fwd = self._lstm_dir(x, "")
-            bwd = self._reverse_dir(x, rev)
+        fwd = self._lstm_dir(x, "")
+        bwd = self._reverse_dir(x, rev)
         return torch.cat([fwd, bwd], -1) * valid[..., None].to(x.dtype)
 
     def infer(self, x):
@@ -325,8 +304,7 @@ _MAIN_HALF = tuple(i for i in range(24) if i not in _ATTN_HALF)
 
 class _FlowState:
     """What the two autograd nodes of one flow step share between forward and the two backward calls."""
-    __slots__ = ("desc", "saved", "plist", "mel_c", "in_lens", "out_lens", "attn", "carry", "grads", "text_shape", "has_gate",
-                 "fuse_bwd", "d_mel")
+    __slots__ = ("desc", "saved", "plist", "mel_c", "in_lens", "out_lens", "attn", "carry", "grads", "text_shape", "has_gate")
 
     def clear(self):
         for k in self.__slots__:
@@ -347,11 +325,6 @@ class _ArStepAttnLstmFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_token):
         st = ctx.state
-        if st is not None and st.d_mel is not None:          # node B ran the whole backward in one call (ft_ar_step_bwd)
-            d_mel, grads_a = st.d_mel, [st.grads[i] for i in _ATTN_HALF]
-            st.clear()
-            ctx.state = None
-            return (None, d_mel, *grads_a)
         if st is None or st.saved is None or st.carry is None:
             raise FlowtronB200Error("AR_Step backward ran twice: the flow's saved activations are released after the first "
                                     "backward (retain_graph is not supported on the CUDA path)")
@@ -404,7 +377,6 @@ class _ArStepFn(torch.autograd.Function):
         state.desc, state.saved, state.plist = desc, saved, plist
         state.mel_c, state.in_lens, state.out_lens, state.attn = mel_c, in_lens, out_lens, attn
         state.text_shape, state.has_gate = text.shape, has_gate
-        state.fuse_bwd = bool(getattr(step, "_fuse_bwd", False))
         ctx.state = state
         ctx.has_gate = has_gate
         if has_gate:
@@ -430,16 +402,9 @@ class _ArStepFn(torch.autograd.Function):
         st.grads = [None if p is None else torch.empty_like(p) for p in st.plist]
         _, scratch_bytes = _lib.ar_step_sizes(desc)
         scratch = _lib.scratch_buffer(scratch_bytes, dev)
-        if st.fuse_bwd:
-            # nobody waits for this flow's d_text alone (the encoder's backward starts after the FIRST flow's): run the whole
-            # backward in one call, which overlaps the attention backward with the attention LSTM's BPTT chunk by chunk
-            st.d_mel = torch.empty_like(st.mel_c)
-            _lib.ar_step_bwd(desc, _lib.make_weights(st.plist), st.mel_c, st.in_lens, st.out_lens, st.attn, d_mel_out, d_log_s,
-                             d_gates, d_attn, d_lp, st.d_mel, d_text, _lib.make_weights(st.grads), st.saved, scratch)
-        else:
-            st.carry = torch.empty(_lib.ar_step_bwd_carry_bytes(desc), dtype=torch.uint8, device=dev)
-            _lib.ar_step_bwd_main(desc, _lib.make_weights(st.plist), st.mel_c, st.in_lens, st.out_lens, st.attn, d_mel_out, d_log_s,
-                                  d_gates, d_attn, d_lp, d_text, _lib.make_weights(st.grads), st.saved, scratch, st.carry)
+        st.carry = torch.empty(_lib.ar_step_bwd_carry_bytes(desc), dtype=torch.uint8, device=dev)
+        _lib.ar_step_bwd_main(desc, _lib.make_weights(st.plist), st.mel_c, st.in_lens, st.out_lens, st.attn, d_mel_out, d_log_s,
+                              d_gates, d_attn, d_lp, d_text, _lib.make_weights(st.grads), st.saved, scratch, st.carry)
         grads_b = [st.grads[i] for i in _MAIN_HALF]
         ctx.state = None
         # (state, step, reversed, token, mel, text, in_lens, out_lens, prior, *params_b): mel's gradient comes out of node A
@@ -580,9 +545,6 @@ class Flowtron(nn.Module):
         for i, flow in enumerate(self.flows):
             # the module whose kernels run first gets the text-ready event (AR_Back_Step wraps its AR_Step as .ar_step)
             getattr(flow, "ar_step", flow)._text_event = getattr(self, "_text_event", None) if i == 0 else None
-            # flows after the first: the encoder's backward cannot start before the first flow's d_text exists, so their backward
-            # may run as one call (attention backward overlapped with the attention-LSTM BPTT); FT_FUSE_BWD=0 disables
-            getattr(flow, "ar_step", flow)._fuse_bwd = (i != 0) and os.environ.get("FT_FUSE_BWD", "0") != "0"
             mel, log_s, gate, attn_out, attn_logprob_out = flow(mel, encoder_outputs, mask, out_lens, attn_prior)
             log_s_list.append(log_s)
             attns_list.append(attn_out)

@@ -192,21 +192,19 @@ def test_batches_larger_than_a_launch_are_chunked():
 
 
 def test_encoder_streams_and_overlap_equal_serial():
-    """Encoder.two_streams (the two BiLSTM directions on two CUDA streams) and Flowtron.overlap_encoder (the whole
-    encoder underneath the first flow's attention LSTM, joined inside ft_ar_step_fwd by the text-ready event) only
-    change scheduling: outputs are bit-identical and gradients equal up to the order of atomic accumulation.  Repeated a
-    few times so a missing dependency would have a chance to show."""
+    """Flowtron.overlap_encoder (the whole encoder on its own stream underneath the first flow's attention LSTM, joined
+    inside ft_ar_step_fwd by the text-ready event) only changes scheduling: outputs are bit-identical and gradients equal
+    up to the order of atomic accumulation.  Repeated a few times so a missing dependency would have a chance to show."""
     from flowtron_b200.flowtron import FlowtronLoss
     torch.backends.cudnn.allow_tf32 = False
     cfg = dict(synth.DEFAULT_MODEL_CONFIG, n_flows=2)
     batch = synth.synth_batch(6, 64, 20, cfg, 23, with_prior=True, in_lens=[20, 20, 17, 11, 9, 5])
     cu = {k: (v.cuda() if torch.is_tensor(v) else v) for k, v in batch.items()}
 
-    def run(two_streams, overlap):
+    def run(overlap):
         model = build_model(cfg, 37)
         model.train()
         model.encoder.p_dropout = 0.0
-        model.encoder.two_streams = two_streams
         model.overlap_encoder = overlap
         out = model(cu["mel"], cu["speaker_ids"], cu["text"], cu["in_lens"], cu["out_lens"], cu["attn_prior"])
         nll, gl, _ = FlowtronLoss()(out, cu["gate_target"], cu["in_lens"], cu["out_lens"])
@@ -214,20 +212,19 @@ def test_encoder_streams_and_overlap_equal_serial():
         torch.cuda.synchronize()
         return out, float(nll), {n: p.grad.clone() for n, p in model.named_parameters()}
 
-    o1, n1, g1 = run(False, False)
+    o1, n1, g1 = run(False)
     gmax = max(v.norm().item() for v in g1.values())
-    for rep in range(2):
-        for flags in ((True, False), (False, True), (True, True)):
-            o2, n2, g2 = run(*flags)
-            assert torch.equal(o1[0], o2[0]) and torch.equal(o1[2], o2[2]), flags
-            for a, b in zip(o1[1] + o1[3] + o1[4], o2[1] + o2[3] + o2[4]):
-                assert torch.equal(a, b), flags
-            assert abs(n1 - n2) <= 1e-6 * abs(n1)                  # the loss sums use float atomics
-            for k in g1:
-                d = (g1[k] - g2[k]).norm().item()
-                # schedules differ only in the order of fp32 atomic accumulation (attention reductions, split-K weight
-                # gradients); tensors that are small sums of large partials see a few 1e-4 of their own norm
-                assert d <= 1e-3 * (g1[k].norm().item() + 1e-4 * gmax), (flags, k, d)
+    for rep in range(4):
+        o2, n2, g2 = run(True)
+        assert torch.equal(o1[0], o2[0]) and torch.equal(o1[2], o2[2]), rep
+        for a, b in zip(o1[1] + o1[3] + o1[4], o2[1] + o2[3] + o2[4]):
+            assert torch.equal(a, b), rep
+        assert abs(n1 - n2) <= 1e-6 * abs(n1)                  # the loss sums use float atomics
+        for k in g1:
+            d = (g1[k] - g2[k]).norm().item()
+            # schedules differ only in the order of fp32 atomic accumulation (attention reductions, split-K weight
+            # gradients); tensors that are small sums of large partials see a few 1e-4 of their own norm
+            assert d <= 1e-3 * (g1[k].norm().item() + 1e-4 * gmax), (rep, k, d)
 
 
 def test_batch_above_32_uses_the_wide_paths_and_matches_split_runs():
