@@ -179,8 +179,9 @@ struct BwdScratch {
 int check_desc(const FtArStepDesc& d) {
     if (d.n_hidden != H) return ft_set_error("ar_step: this build supports n_hidden == 1024 only");
     if (d.T <= 0 || d.B <= 0 || d.L <= 0) return ft_set_error("ar_step: empty shape");
-    if (d.B > 64) return ft_set_error("ar_step: batch > 64 per call not supported (split the batch)");
-    if (d.n_mel % 8 || d.n_attn % 64 || d.n_text % 8) return ft_set_error("ar_step: n_mel %8, n_attn %64, n_text %8 required");
+    if (d.B > 32) return ft_set_error("ar_step: batch > 32 per call not supported (split the batch)");
+    if (d.n_mel > 128 || d.n_mel % 8 || d.n_attn % 64 || d.n_text % 8)
+        return ft_set_error("ar_step: n_mel <= 128 and %8, n_attn %64, n_text %8 required");
     if (d.L > 256) return ft_set_error("ar_step: L > 256 not supported");
     return 0;
 }
@@ -327,7 +328,7 @@ int ar_step_fwd(const FtArStepDesc& d, const FtArStepWeights& w, const float* me
     FT_TRY(launch_prep_mel(mel, out_lens, n.T, n.B, n.M, d.reversed, S.mel_in16, S.mel_flow, st));
     const float* mel_flow = d.reversed ? S.mel_flow : mel;
 
-    // Attention-LSTM / attention overlap (FT_ATT_OVERLAP = chunk length in steps, a multiple of 64; default 256, 0 disables; B <= 32 and
+    // Attention-LSTM / attention overlap (FT_ATT_OVERLAP = chunk length in steps, a multiple of 64; default 256, 0 disables;
     // T >= chunk + 64): the attention LSTM runs as a 64-CTA recurrence in chunks; as soon as a chunk's h is there, a second stream
     // runs that chunk's query projection, fused attention, gate logits and lstm layer 0's input projection on the SMs the 64-CTA
     // recurrence leaves free,
@@ -336,7 +337,7 @@ int ar_step_fwd(const FtArStepDesc& d, const FtArStepWeights& w, const float* me
     // boundary costs a kernel drain + launch + 128 KB weight reload on 64 SMs.
     static int att_chunk = -1;
     if (att_chunk < 0) { const char* e = getenv("FT_ATT_OVERLAP"); att_chunk = e ? atoi(e) : 256; if (att_chunk % 64) att_chunk = 0; }
-    Pipe* pa = (att_chunk > 0 && F.X1 && n.B <= 32 && n.T >= att_chunk + 64) ? get_pipe(st) : nullptr;
+    Pipe* pa = (att_chunk > 0 && F.X1 && n.T >= att_chunk + 64) ? get_pipe(st) : nullptr;
     bool xproj0_done = false;
     auto attention_rows = [&](cudaStream_t s2, int t0, int t1) -> int {      // Q projection, attention, gate logits of steps [t0, t1)
         const long long r0 = static_cast<long long>(t0) * n.B, rows = static_cast<long long>(t1 - t0) * n.B;
@@ -399,20 +400,15 @@ int ar_step_fwd(const FtArStepDesc& d, const FtArStepWeights& w, const float* me
     } else {
     // attention_lstm: the 80-channel input projection is folded into the persistent recurrence (no [R,4096] projection
     // tensor: one GEMM and 1 GB of HBM traffic less per flow); h lands in d16[:, 0:H].
-    if (n.M <= 128 && n.B <= 32) {             // B > 32: the double-buffered x tile no longer fits next to a 64-row h tile
-        FT_TRY(launch_lstm_fwd_xin(n.T, n.B, S.mel_in16, n.M, n.M, F.w.w_ih_a, w.attn_lstm_b_ih, w.attn_lstm_b_hh, F.w.w_hh_a, out_lens,
-                                   S.d16, n.D, S.gatesA, S.cA, F.hA32, H, F.flags, st));
-    } else {
-        FT_TRY(gemm_fwd(st, n.R, G, n.M, S.mel_in16, n.M, F.w.w_ih_a, n.M, w.attn_lstm_b_ih, w.attn_lstm_b_hh, 0, F.X, G, nullptr, 0));
-        FT_TRY(launch_lstm_fwd(n.T, n.B, F.X, F.w.w_hh_a, out_lens, S.d16, n.D, S.gatesA, S.cA, F.hA32, H, F.flags, st));
-    }
+    FT_TRY(launch_lstm_fwd_xin(n.T, n.B, S.mel_in16, n.M, n.M, F.w.w_ih_a, w.attn_lstm_b_ih, w.attn_lstm_b_hh, F.w.w_hh_a, out_lens,
+                               S.d16, n.D, S.gatesA, S.cA, F.hA32, H, F.flags, st));
     // attention: K/V/Q projections, fused score+softmax(+prior)+context; ctx lands in d16[:, H:H+A]
     FT_TRY(kv_projections(st));
     FT_TRY(attention_rows(st, 0, n.T));
     }
 
     // 2-layer lstm
-    Pipe* pp = (F.X1 && n.B <= 32 && n.T > pipe_chunk_steps()) ? get_pipe(st) : nullptr;
+    Pipe* pp = (F.X1 && n.T > pipe_chunk_steps()) ? get_pipe(st) : nullptr;
     if (pp) {
         // EXPERIMENTAL: layer 1 at step t needs layer 0 only up to t, so the two recurrences run as two 64-CTA kernels
         // one chunk apart: st = layer 0, sC = layer-1 input projection of a finished chunk, sB = layer 1.
@@ -525,7 +521,7 @@ int ar_step_bwd_main(const FtArStepDesc& d, const FtArStepWeights& w, const floa
         FT_TRY(zero(g.gate_w, sizeof(float) * n.D, st));
         FT_TRY(zero(g.gate_b, sizeof(float), st));
     }
-    Pipe* pp = (F.dcarry1 && n.B <= 32 && 2 * pipe_chunk_steps() <= n.T) ? get_pipe(st) : nullptr;
+    Pipe* pp = (F.dcarry1 && 2 * pipe_chunk_steps() <= n.T) ? get_pipe(st) : nullptr;
     if (pp) {
         // EXPERIMENTAL 5+6: BPTT of layer 1 (st) and layer 0 (sB) one chunk apart; the layer-1 dgrad of a finished chunk
         // (sC) turns dG1 rows into layer 0's incoming dh rows (F.dh is reused row-disjointly: layer 1 only reads rows

@@ -10,19 +10,20 @@
 //     TMA-loaded once and stay resident in shared memory as the wgmma A operand (M = 64, 32 real rows).
 //   * every step: h_{t-1} ([B,1024] fp16, read straight out of the layer's output tensor) arrives through
 //     TWO 3-D TMA loads (8 K-chunks each, box {64 elems, B rows, 8 chunks}: the smem image is chunk-major
-//     SWIZZLE_128B K-major tiles, the wgmma B operand with N = B rounded up to 16 / 32 / 64); the CTA's one
+//     SWIZZLE_128B K-major tiles, the wgmma B operand with N = B rounded up to 16 / 32); the CTA's one
 //     warpgroup accumulates the 32 gate pre-activations in registers, hands them through shared memory to
 //     the thread that owns each (batch row, unit pair), adds the input projection, applies the cell in fp32
 //     (cell state lives in registers for the whole sequence), store h_t (fp16) and publish ONE release per
 //     CTA into a per-(step, chunk) counter; consumers poll the 16 counters in parallel (one lane each),
 //     fence the async proxy, and issue the next loads.  gates / c for the backward pass are stored AFTER
 //     the release so they stay off the critical path.
-// Backward (lstm_bwd_kernel), 64 CTAs x 16 units: dh_{t-1} = dG_t W_hh with the W_hh^T slice resident
-//   (fp16, 128 KB), dG_t ([B,4096] fp16, loss-scaled) streamed in groups of chunks through a small ring,
-//   the pointwise LSTM backward in the epilogue; dG is written once and reused by the wgrad/dgrad GEMMs.
+// Backward (lstm_bwd4_kernel), 16 clusters of 4 CTAs: dh_{t-1} = dG_t W_hh split over the four gates, the pointwise
+//   LSTM backward in the epilogue; dG ([B,4096] fp16, loss-scaled) is written once and reused by the wgrad/dgrad GEMMs.
+//
+// Every kernel here takes at most 32 batch rows per launch (one 32-row wgmma tile); larger batches are split by the caller.
 //
 // Warp roles: warps 0-3 form one warpgroup that issues the wgmma of a step and runs the cell epilogue on the
-// accumulator; warp 4 is the TMA producer.  Loads are issued as few multi-chunk 3-D boxes: issuing 16 (64) 2-D loads
+// accumulator; warp 4 is the TMA producer.  Loads are issued as few multi-chunk 3-D boxes: issuing 16 2-D loads
 // serially from one thread puts the issue time on the recurrence's critical path.
 #include <type_traits>
 
@@ -85,202 +86,6 @@ struct LstmFwdParams {
     long long* trace;          // optional [T][8] clock64 stamps of CTA 0 (debug/profiling), or null
 };
 
-// ------------------------------------------------------------------------------------------- backward
-constexpr int BWD_CTAS = 64, BWD_UNITS = 16, BWD_NCH = LG / KCH;                   // 64 chunks / step
-constexpr int BWD_W_BYTES = BWD_NCH * BWD_UNITS * 128;                              // 128 KB
-
-struct LstmBwdParams {
-    int T, B, Bbox;
-    int gs, ng, nring;         // chunks per TMA group, groups per step (64 / gs), ring depth in groups
-    const float* dh_ext; long long ldd;   // [T*B, ldd] gradient w.r.t. the layer outputs (fp32, loss-scaled)
-    const __half* gates;       // [T*B, 4096] saved i,f,g,o
-    const float* cstate;       // [T*B, 1024] saved c_t
-    const int* lens;
-    __half* dG;                // [T*B, 4096] out: (loss-scaled) gradient w.r.t. gate pre-activations (fp16, saturating)
-    int* flags;                // [T * 64]
-    int* status;
-    long long* trace;
-};
-
-__global__ void __launch_bounds__(LSTM_THREADS, 1)
-lstm_bwd_kernel(const __grid_constant__ CUtensorMap tmWT, const __grid_constant__ CUtensorMap tmG, LstmBwdParams p) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    const int slot_bytes = p.Bbox * 128;
-    const int group_bytes = p.gs * slot_bytes;
-    uint8_t* ring = smem;                                        // [nring groups][gs chunks][Bbox rows][128 B]
-    uint8_t* sW = smem + p.nring * group_bytes;                  // over-read of the last ring chunk lands here
-    float* sAcc = reinterpret_cast<float*>(sW + BWD_W_BYTES);    // [128 rows][17]
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sAcc + 128 * 17 + 1);
-    bars = reinterpret_cast<uint64_t*>((reinterpret_cast<uintptr_t>(bars) + 7) & ~uintptr_t(7));
-    uint64_t* full = bars;                       // [nring]
-    uint64_t* empty = bars + 8;                  // [nring]: one arrival per warp of the warpgroup
-    uint64_t* wbar = bars + 16;
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int cta = blockIdx.x;
-
-    if (warp == PRODUCER_WARP && lane == 0) {
-        tma_prefetch_desc(&tmWT);
-        tma_prefetch_desc(&tmG);
-        for (int s = 0; s < p.nring; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 4); }
-        mbar_init(wbar, 1);
-        fence_mbar_init();
-    }
-    __syncthreads();
-
-    if (warp == PRODUCER_WARP) {
-        if (lane == 0) {
-            mbar_expect_tx(wbar, BWD_W_BYTES);
-            for (int kc = 0; kc < BWD_NCH; ++kc)       // W_hh^T rows [16c,16c+16), K chunk kc
-                tma_load_2d(sW + kc * (BWD_UNITS * 128), &tmWT, wbar, kc * KCH, BWD_UNITS * cta);
-        }
-        int s = 0, ph = 0;                             // ring slot / phase, advanced incrementally (no div/mod)
-        for (int t = p.T - 2; t >= 0; --t) {
-            for (int c = lane; c < BWD_NCH; c += 32)   // parallel poll: 4 producer CTAs per 64-column chunk of dG_{t+1}
-                wait_flag_ge(&p.flags[(t + 1) * BWD_NCH + c], 4, p.status, 212);
-            __syncwarp();
-            if (elect_one()) { FT_TRACE(p, t, 0); fence_proxy_async_global(); }
-            __syncwarp();
-            for (int g = 0; g < p.ng; ++g) {
-                mbar_wait(&empty[s], ph ^ 1, p.status, 211);
-                if (elect_one()) {
-                    mbar_expect_tx(&full[s], group_bytes);
-                    tma_load_3d(ring + s * group_bytes, &tmG, &full[s], 0, (t + 1) * p.B, g * p.gs);
-                    if (g == 0) FT_TRACE(p, t, 1);
-                    if (g == p.ng - 1) FT_TRACE(p, t, 6);
-                }
-                __syncwarp();
-                if (++s == p.nring) { s = 0; ph ^= 1; }
-            }
-        }
-    } else {
-        // ---------------------------------------------------------------- epilogue: items (batch row, 4 units)
-        const int et = threadIdx.x;
-        const int n_items = p.B * 4;
-        const int u0 = BWD_UNITS * cta;
-        // dh_{t} = dG_{t+1} W_hh on the warpgroup: A = the dG ring (M = 64 batch rows, of which the first Bbox are real),
-        // B = the resident W_hh^T slice (N = 16 units)
-        const uint64_t da_ring = wgmma_desc(smem_u32(ring), 16, 1024), db_base = wgmma_desc(smem_u32(sW), 16, 1024);
-        const uint64_t a_chunk = static_cast<uint64_t>(slot_bytes >> 4), a_group = static_cast<uint64_t>(group_bytes >> 4);
-        const uint64_t b_chunk = (BWD_UNITS * 128) >> 4;
-        int rs_slot = 0, rs_ph = 0;
-        mbar_wait(wbar, 0, p.status, 213);
-        float dcs[2][4];
-#pragma unroll
-        for (int s = 0; s < 2; ++s)
-#pragma unroll
-            for (int j = 0; j < 4; ++j) dcs[s][j] = 0.f;
-        int len_i[2];
-#pragma unroll
-        for (int s = 0; s < 2; ++s) {
-            const int item = et + s * EPI_THREADS;
-            len_i[s] = (item < n_items && p.lens) ? p.lens[item >> 2] : p.T;
-        }
-        int step = 0;
-        for (int t = p.T - 1; t >= 0; --t, ++step) {
-            float dh[2][4], ct[2][4], cp[2][4];
-            __half2 gt[2][4][2];                              // [item][gate][2 x half2]
-            bool valid[2];
-#pragma unroll
-            for (int s = 0; s < 2; ++s) {
-                const int item = et + s * EPI_THREADS;
-                valid[s] = (item < n_items) && (t < len_i[s]);
-                if (valid[s]) {
-                    const int b = item >> 2, uq = item & 3;
-                    const long long r = static_cast<long long>(t) * p.B + b;
-                    const int uo = u0 + 4 * uq;
-                    const float4 v = __ldg(reinterpret_cast<const float4*>(p.dh_ext + r * p.ldd + uo));
-                    dh[s][0] = v.x; dh[s][1] = v.y; dh[s][2] = v.z; dh[s][3] = v.w;
-                    const float4 cc = __ldg(reinterpret_cast<const float4*>(p.cstate + r * LH + uo));
-                    ct[s][0] = cc.x; ct[s][1] = cc.y; ct[s][2] = cc.z; ct[s][3] = cc.w;
-                    float4 pp = make_float4(0.f, 0.f, 0.f, 0.f);
-                    if (t > 0) pp = __ldg(reinterpret_cast<const float4*>(p.cstate + (r - p.B) * LH + uo));
-                    cp[s][0] = pp.x; cp[s][1] = pp.y; cp[s][2] = pp.z; cp[s][3] = pp.w;
-#pragma unroll
-                    for (int g = 0; g < 4; ++g) {
-                        const uint2 pk = __ldg(reinterpret_cast<const uint2*>(p.gates + r * LG + g * LH + uo));
-                        *reinterpret_cast<uint2*>(&gt[s][g][0]) = pk;
-                    }
-                }
-            }
-            if (step > 0) {
-                float acc[8];
-                uint64_t db = db_base;
-                for (int g = 0; g < p.ng; ++g) {
-                    mbar_wait(&full[rs_slot], rs_ph, p.status, 214);
-                    if (g == 0 && et == 0) FT_TRACE(p, t, 2);
-                    wgmma_fence_acc<8>(acc);
-                    wgmma_fence();
-                    mma_chunks<16>(acc, da_ring + rs_slot * a_group, db, p.gs, a_chunk, b_chunk, g == 0);
-                    wgmma_commit();
-                    wgmma_wait<0>();
-                    wgmma_fence_acc<8>(acc);
-                    if (lane == 0) mbar_arrive(&empty[rs_slot]);
-                    db += static_cast<uint64_t>(p.gs) * b_chunk;
-                    if (++rs_slot == p.nring) { rs_slot = 0; rs_ph ^= 1; }
-                }
-                if (et == 0) FT_TRACE(p, t, 4);
-                const int r0 = 16 * warp + (lane >> 2), c0 = 2 * (lane & 3);
-#pragma unroll
-                for (int j = 0; j < 2; ++j) {
-                    sAcc[r0 * 17 + 8 * j + c0] = acc[4 * j]; sAcc[r0 * 17 + 8 * j + c0 + 1] = acc[4 * j + 1];
-                    sAcc[(r0 + 8) * 17 + 8 * j + c0] = acc[4 * j + 2]; sAcc[(r0 + 8) * 17 + 8 * j + c0 + 1] = acc[4 * j + 3];
-                }
-                epi_bar();
-            }
-#pragma unroll
-            for (int s = 0; s < 2; ++s) {
-                const int item = et + s * EPI_THREADS;
-                if (item < n_items) {
-                    const int b = item >> 2, uq = item & 3;
-                    const long long r = static_cast<long long>(t) * p.B + b;
-                    __half2 out[4][2];
-                    if (valid[s]) {
-#pragma unroll
-                        for (int j2 = 0; j2 < 2; ++j2) {
-                            float da[4][2];
-#pragma unroll
-                            for (int e = 0; e < 2; ++e) {
-                                const int j = 2 * j2 + e;
-                                const float gi = e ? __high2float(gt[s][0][j2]) : __low2float(gt[s][0][j2]);
-                                const float gf = e ? __high2float(gt[s][1][j2]) : __low2float(gt[s][1][j2]);
-                                const float gg = e ? __high2float(gt[s][2][j2]) : __low2float(gt[s][2][j2]);
-                                const float go = e ? __high2float(gt[s][3][j2]) : __low2float(gt[s][3][j2]);
-                                float dht = dh[s][j];
-                                if (step > 0) dht += sAcc[b * 17 + 4 * uq + j];
-                                const float tc = tanh_f(ct[s][j]);
-                                const float dc = dcs[s][j] + dht * go * (1.f - tc * tc);
-                                da[3][e] = dht * tc * go * (1.f - go);
-                                da[0][e] = dc * gg * gi * (1.f - gi);
-                                da[2][e] = dc * gi * (1.f - gg * gg);
-                                da[1][e] = dc * cp[s][j] * gf * (1.f - gf);
-                                dcs[s][j] = dc * gf;
-                            }
-#pragma unroll
-                            for (int g = 0; g < 4; ++g)
-                                out[g][j2] = __floats2half2_rn(fminf(fmaxf(da[g][0], -65504.f), 65504.f),
-                                                               fminf(fmaxf(da[g][1], -65504.f), 65504.f));
-                        }
-                    } else {
-#pragma unroll
-                        for (int g = 0; g < 4; ++g) { out[g][0] = __floats2half2_rn(0.f, 0.f); out[g][1] = out[g][0]; }
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) dcs[s][j] = 0.f;
-                    }
-#pragma unroll
-                    for (int g = 0; g < 4; ++g)
-                        *reinterpret_cast<uint2*>(p.dG + r * LG + g * LH + u0 + 4 * uq) = *reinterpret_cast<uint2*>(&out[g][0]);
-                }
-            }
-            epi_bar();                                        // every dG_t store of this CTA precedes the releases
-            if (et == 0) FT_TRACE(p, t, 5);
-            if (et < 4) red_release_add(&p.flags[t * BWD_NCH + et * 16 + cta / 4], 1);   // one release per gate chunk
-            if (et == 0) FT_TRACE(p, t, 7);
-        }
-    }
-}
-
 // ------------------------------------------------------------------------------------------- backward, split-K cluster
 // 64 CTAs in 16 clusters of 4.  Cluster c owns hidden units [64c, 64c+64); rank r reduces over gate r's quarter of
 // the contraction (K = 1024 of 4096):  partial_r[b, u] = sum_{k in gate r} dG_{t+1}[b, k] W_hh[k, u].
@@ -288,7 +93,8 @@ lstm_bwd_kernel(const __grid_constant__ CUtensorMap tmWT, const __grid_constant_
 //     dG_{t+1} (B x 1024 fp16 = 64 KB at B=32 instead of all 256 KB broadcast to every CTA);
 //   * partial sums (fp32 [B, 64]) go to shared memory; a cluster-scope mbarrier (4 remote arrives) publishes them;
 //     each rank then finishes 16 of the 64 units, reading the 3 other partials over DSMEM;
-//   * pointwise LSTM backward + dG_t stores + per-chunk release flags exactly as in the single-CTA kernel.
+//   * then the pointwise LSTM backward, the dG_t stores and one release flag per 64-column chunk of dG_t.
+constexpr int BWD_NCH = LG / KCH;                                                                  // 64 dG chunks / step
 constexpr int B4_CTAS = 64, B4_CLUSTER = 4, B4_UNITS = 64, B4_OWN = 16, B4_NCH = LH / KCH;     // 16 chunks / step / rank
 constexpr int B4_W_BYTES = B4_NCH * B4_UNITS * 128;                                               // 128 KB
 constexpr int B4_UP = 36;                                                                          // received-slice row pitch (floats): 32 batch columns, 16-byte aligned rows
@@ -298,7 +104,16 @@ constexpr int B4_XCHG_FLOATS = 2 * 4 * 16 * B4_UP;                              
 // one chunk of the layer pipeline (ar_step.cu), resuming dc*f from `dc_carry` ([B,1024] fp32, written by the chunk above) and
 // dG_{t1} from the dG tensor.  Flags are indexed relative to t0, mbarrier phases are counted over the steps that have a
 // recurrent term.
-struct LstmBwdChunkParams : LstmBwdParams {
+struct LstmBwdChunkParams {
+    int T, B, Bbox;
+    const float* dh_ext; long long ldd;   // [T*B, ldd] gradient w.r.t. the layer outputs (fp32, loss-scaled)
+    const __half* gates;       // [T*B, 4096] saved i,f,g,o
+    const float* cstate;       // [T*B, 1024] saved c_t
+    const int* lens;
+    __half* dG;                // [T*B, 4096] out: (loss-scaled) gradient w.r.t. gate pre-activations (fp16, saturating)
+    int* flags;
+    int* status;
+    long long* trace;
     int t0, t1;                // steps [t0, t1); flags: [(t1 - t0) * 64] ints, zeroed by the launcher
     float* dc_carry;           // [B, 1024]
 };
@@ -524,9 +339,8 @@ lstm_fwd_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__
     const int slot_bytes = p.Bbox * 128;
     uint8_t* sA = smem;                                          // [16 (+2x2) chunks][Bbox rows][128 B]: h chunks, then two x buffers
     uint8_t* sW = smem + A_SLOTS * slot_bytes;
-    float* sAcc = reinterpret_cast<float*>(sW + FWD_W_BYTES);    // [32 * nq rows][AP]
-    const int nq = (p.B + 31) / 32;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sAcc + ((nq * 32 * AP + 1) & ~1));
+    float* sAcc = reinterpret_cast<float*>(sW + FWD_W_BYTES);    // [32 rows][AP]
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sAcc + ((32 * AP + 1) & ~1));
     uint64_t* full = bars;                       // [FWD_NG] (<= 16)
     uint64_t* wbar = bars + 16;
     uint64_t* xfull = bars + 18;                 // [2] (kXIn)
@@ -596,12 +410,12 @@ lstm_fwd_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__
         // ---------------------------------------------------------------- warpgroup: recurrent contraction + cell, 128 threads
         const int et = threadIdx.x;                           // 0..127
         // SWAPPED operands: A = the resident W slice (M = 64 accumulator rows: the CTA's 4*UNITS gate rows, plus -- for
-        // UNITS = 8 -- 32 don't-care rows read from the next chunk), B = h_{t-1} (N = Bbox batch rows rounded up to 16 / 32 / 64;
+        // UNITS = 8 -- 32 don't-care rows read from the next chunk), B = h_{t-1} (N = Bbox batch rows rounded up to 16 / 32;
         // rows beyond Bbox are read from the next chunk and never used).  A = h padded to 64 rows would make every
         // instruction read mostly padding from shared memory.
         const uint64_t da_base = wgmma_desc(smem_u32(sW), 16, 1024), db_base = wgmma_desc(smem_u32(sA), 16, 1024);
         const uint64_t a_chunk = (FWD_N * 128) >> 4, b_chunk = static_cast<uint64_t>(slot_bytes >> 4);
-        const int nsel = p.Bbox <= 16 ? 16 : (p.Bbox <= 32 ? 32 : 64);
+        const bool n16 = p.Bbox <= 16;
         // one step's contraction: [x_t chunks (kXIn)] + the 16 h_{t-1} chunks as they arrive, accumulator -> sAcc[batch][row]
         auto contract = [&](auto nb, int t) {
             constexpr int N = decltype(nb)::value;
@@ -629,10 +443,8 @@ lstm_fwd_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__
 #pragma unroll
             for (int j = 0; j < N / 8; ++j) {
                 const int b = 8 * j + b0;
-                if (b < nq * 32) {
-                    if (r0 < FWD_N) { sAcc[b * AP + r0] = acc[4 * j]; sAcc[(b + 1) * AP + r0] = acc[4 * j + 1]; }
-                    if (r0 + 8 < FWD_N) { sAcc[b * AP + r0 + 8] = acc[4 * j + 2]; sAcc[(b + 1) * AP + r0 + 8] = acc[4 * j + 3]; }
-                }
+                if (r0 < FWD_N) { sAcc[b * AP + r0] = acc[4 * j]; sAcc[(b + 1) * AP + r0] = acc[4 * j + 1]; }
+                if (r0 + 8 < FWD_N) { sAcc[b * AP + r0 + 8] = acc[4 * j + 2]; sAcc[(b + 1) * AP + r0 + 8] = acc[4 * j + 3]; }
             }
         };
         mbar_wait(wbar, 0, p.status, 213);
@@ -695,9 +507,8 @@ lstm_fwd_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__
                 }
             }
             if (t > 0) {
-                if (nsel == 16) contract(std::integral_constant<int, 16>(), t);
-                else if (nsel == 32) contract(std::integral_constant<int, 32>(), t);
-                else contract(std::integral_constant<int, 64>(), t);
+                if (n16) contract(std::integral_constant<int, 16>(), t);
+                else contract(std::integral_constant<int, 32>(), t);
                 epi_bar();
                 if (et == 0) FT_TRACE(p, t, 8);               // accumulator transposed into shared memory
 #pragma unroll
@@ -811,8 +622,8 @@ static int launch_fwd_t(int T, int B, int t0, int t1, const float* xproj, const 
     p.xproj = xproj; p.b_ih = b_ih; p.b_hh = b_hh; p.lens = lens; p.hseq = static_cast<__half*>(hseq16); p.ldh = ldh;
     p.gates = static_cast<__half*>(gates16); p.cstate = cstate; p.h32 = h32; p.ldh32 = ldh32;
     p.flags = flags; p.status = ft_status_word(); p.trace = (t0 == 0 && t1 == T) ? g_lstm_trace : nullptr;
-    const int slot = p.Bbox * 128, nq = (B + 31) / 32;
-    const int smem = (FWD_NCH + (kXIn ? 2 * XCH : 0)) * slot + W_BYTES + nq * 32 * (N + 1) * 4 + 8 + 256 + 1024;
+    const int slot = p.Bbox * 128;
+    const int smem = (FWD_NCH + (kXIn ? 2 * XCH : 0)) * slot + W_BYTES + 32 * (N + 1) * 4 + 8 + 256 + 1024;
     if (smem > smem_optin()) return ft_set_error("lstm_fwd: not enough shared memory");
     CUtensorMap tmW, tmH, tmWx, tmX;
     if (make_tmap_2d(&tmW, whh16, FMT_F16, LG, LH, LH, KCH, UNITS)) return -1;
@@ -838,8 +649,8 @@ static int launch_fwd_t(int T, int B, int t0, int t1, const float* xproj, const 
 int launch_lstm_fwd(int T, int B, const float* xproj, const void* whh16, const int* lens, void* hseq16, long long ldh,
                     void* gates16, float* cstate, float* h32, long long ldh32, int* flags, cudaStream_t st) {
     if (T <= 0 || B <= 0) return 0;
-    if (B > 64) return ft_set_error("lstm_fwd: batch > 64 per call not supported (split the batch)");
-    if (g_half_sm && B <= 32) return launch_fwd_t<16, false>(T, B, 0, T, xproj, whh16, lens, hseq16, ldh, gates16, cstate, h32, ldh32, flags, st);
+    if (B > 32) return ft_set_error("lstm_fwd: batch > 32 per call not supported (split the batch)");
+    if (g_half_sm) return launch_fwd_t<16, false>(T, B, 0, T, xproj, whh16, lens, hseq16, ldh, gates16, cstate, h32, ldh32, flags, st);
     return launch_fwd_t<8, false>(T, B, 0, T, xproj, whh16, lens, hseq16, ldh, gates16, cstate, h32, ldh32, flags, st);
 }
 
@@ -849,9 +660,9 @@ int launch_lstm_fwd_xin(int T, int B, const void* x16, long long ldx, int kx, co
                         const void* whh16, const int* lens, void* hseq16, long long ldh, void* gates16, float* cstate, float* h32,
                         long long ldh32, int* flags, cudaStream_t st) {
     if (T <= 0 || B <= 0) return 0;
-    if (B > 64) return ft_set_error("lstm_fwd: batch > 64 per call not supported (split the batch)");
+    if (B > 32) return ft_set_error("lstm_fwd: batch > 32 per call not supported (split the batch)");
     if (!x16 || !wih16 || !b_ih || !b_hh) return ft_set_error("lstm_fwd_xin: NULL argument");
-    if (g_half_sm && B <= 32)
+    if (g_half_sm)
         return launch_fwd_t<16, true>(T, B, 0, T, nullptr, whh16, lens, hseq16, ldh, gates16, cstate, h32, ldh32, flags, st, x16, ldx, kx, wih16, b_ih, b_hh);
     return launch_fwd_t<8, true>(T, B, 0, T, nullptr, whh16, lens, hseq16, ldh, gates16, cstate, h32, ldh32, flags, st, x16, ldx, kx, wih16, b_ih, b_hh);
 }
@@ -860,17 +671,17 @@ int launch_lstm_fwd_xin(int T, int B, const void* x16, long long ldx, int kx, co
 int launch_lstm_fwd_chunk(int T, int B, int t0, int t1, const float* xproj, const void* whh16, const int* lens, void* hseq16,
                           long long ldh, void* gates16, float* cstate, int* flags, cudaStream_t st, float* h32, long long ldh32) {
     if (T <= 0 || B <= 0 || t1 <= t0) return 0;
-    if (B > 64 || t0 < 0 || t1 > T) return ft_set_error("lstm_fwd_chunk: bad batch or step range");
+    if (B > 32 || t0 < 0 || t1 > T) return ft_set_error("lstm_fwd_chunk: bad batch or step range");
     if (t0 > 0 && !cstate) return ft_set_error("lstm_fwd_chunk: resuming a chunk needs the saved cell states");
     return launch_fwd_t<16, false>(T, B, t0, t1, xproj, whh16, lens, hseq16, ldh, gates16, cstate, h32, ldh32, flags, st);
 }
 
-// Steps [t0, t1) of a layer's BPTT with the split-K cluster kernel, B <= 32.  `flags` needs (t1 - t0) * 64 ints; `dc_carry`
+// Steps [t0, t1) of a layer's BPTT with the split-K cluster kernel.  `flags` needs (t1 - t0) * 64 ints; `dc_carry`
 // ([B,1024] fp32) is only touched when the range is a proper chunk.
 static int launch_bwd4(int T, int B, int t0, int t1, const float* dh_ext, long long ldd, const void* whhT16, const void* gates16,
                        const float* cstate, const int* lens, void* dG16, float* dc_carry, int* flags, cudaStream_t st) {
     LstmBwdChunkParams p;
-    p.T = T; p.B = B; p.Bbox = (B + 7) & ~7; p.gs = 8; p.ng = 2; p.nring = 0; p.t0 = t0; p.t1 = t1; p.dc_carry = dc_carry;
+    p.T = T; p.B = B; p.Bbox = (B + 7) & ~7; p.t0 = t0; p.t1 = t1; p.dc_carry = dc_carry;
     const int slot = p.Bbox * 128;
     p.dh_ext = dh_ext; p.ldd = ldd; p.gates = static_cast<const __half*>(gates16); p.cstate = cstate; p.lens = lens;
     p.dG = static_cast<__half*>(dG16); p.flags = flags; p.status = ft_status_word();
@@ -911,35 +722,8 @@ int launch_lstm_bwd_chunk(int T, int B, int t0, int t1, const float* dh_ext, lon
 int launch_lstm_bwd(int T, int B, const float* dh_ext, long long ldd, const void* whhT16, const void* gates16,
                     const float* cstate, const int* lens, void* dG16, int* flags, cudaStream_t st) {
     if (T <= 0 || B <= 0) return 0;
-    if (B > 64) return ft_set_error("lstm_bwd: batch > 64 per call not supported (split the batch)");
-    if (B <= 32)
-        return launch_bwd4(T, B, 0, T, dh_ext, ldd, whhT16, gates16, cstate, lens, dG16, nullptr, flags, st);
-    LstmBwdParams p;
-    p.T = T; p.B = B; p.Bbox = (B + 7) & ~7;
-    const int slot = p.Bbox * 128;
-    const int fixed = BWD_W_BYTES + 128 * 17 * 4 + 512 + 1024;
-    const int avail = smem_optin() - fixed;
-    int gs = 8;
-    while (gs > 2 && 2 * gs * slot > avail) gs >>= 1;          // at least a 2-deep ring of groups (gs stays even)
-    int nring = avail / (gs * slot);
-    if (nring > 8) nring = 8;
-    if (nring < 2) return ft_set_error("lstm_bwd: not enough shared memory for the dG ring");
-    p.gs = gs; p.ng = BWD_NCH / gs; p.nring = nring;
-    p.dh_ext = dh_ext; p.ldd = ldd; p.gates = static_cast<const __half*>(gates16); p.cstate = cstate; p.lens = lens;
-    p.dG = static_cast<__half*>(dG16); p.flags = flags; p.status = ft_status_word(); p.trace = g_lstm_trace;
-    CUtensorMap tmWT, tmG;
-    if (make_tmap_2d(&tmWT, whhT16, FMT_F16, LH, LG, LG, KCH, BWD_UNITS)) return -1;
-    if (make_tmap_chunks(&tmG, dG16, static_cast<long long>(T) * B, BWD_NCH, LG, p.Bbox, gs)) return -1;
-    if (cudaMemsetAsync(flags, 0, sizeof(int) * T * BWD_NCH, st) != cudaSuccess) return ft_set_error("lstm_bwd: memset failed");
-    const int smem = nring * gs * slot + fixed;
-    cudaFuncSetAttribute(lstm_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    TimeScope ts("lstm_bwd", T, B, 0, st);
-    void* args[] = {&tmWT, &tmG, &p};
-    cudaError_t e = cudaLaunchCooperativeKernel(reinterpret_cast<void*>(lstm_bwd_kernel), dim3(BWD_CTAS),
-                                                dim3(LSTM_THREADS), args, smem, st);
-    if (e != cudaSuccess) return ft_set_error(cudaGetErrorString(e));
-    ft_count_launch(1);
-    return ft_check_launch("lstm_bwd_kernel");
+    if (B > 32) return ft_set_error("lstm_bwd: batch > 32 per call not supported (split the batch)");
+    return launch_bwd4(T, B, 0, T, dh_ext, ldd, whhT16, gates16, cstate, lens, dG16, nullptr, flags, st);
 }
 
 }  // namespace ft

@@ -522,10 +522,9 @@ class Flowtron(nn.Module):
     overlap_encoder = os.environ.get("FT_ENC_OVERLAP", "1") != "0"
     min_split_batch = 8
 
-    # Utterances per kernel launch.  The kernels take up to 64, but the fast paths (cluster BPTT, layer pipeline, folded input
-    # projection) are B <= 32 paths, so a B = 64 batch (configs[2]) runs as two consecutive 32-utterance launches rather than
-    # one 64-utterance launch on the fallback kernels.  FT_MAX_KERNEL_BATCH overrides.
-    max_kernel_batch = int(os.environ.get("FT_MAX_KERNEL_BATCH", "32"))
+    # Utterances per flow-kernel launch: the flow kernels take at most 32, so a larger batch (configs[2]: B = 64) runs as
+    # consecutive launches of up to 32 utterances each.
+    max_kernel_batch = 32
 
     def _run_flows(self, mel, encoder_outputs, mask, out_lens, attn_prior):
         B = mel.size(1)

@@ -45,7 +45,7 @@ int ft_gemm(int M, int N, int K, const void* A, long long lda, int a_fmt, int a_
  * run_padded_sequence :671-695).  xproj = W_ih x + b_ih + b_hh for all T*B rows (row = t*B + b), fp32
  * [T*B, 4096], gate order i,f,g,o.  whh16: fp16 copy of weight_hh [4096,1024].  Writes h (fp16, zero at
  * t >= lens[b]) to hseq16 [T*B, ldh] and, when non-null, the post-activation gates (fp16 [T*B,4096]) and
- * cell state (fp32 [T*B,1024]) needed by ft_lstm_bwd.  flags: int scratch [T*16].  B <= 128. */
+ * cell state (fp32 [T*B,1024]) needed by ft_lstm_bwd.  flags: int scratch [T*16].  B <= 32. */
 int ft_lstm_fwd(int T, int B, const float* xproj, const void* whh16, const int* lens, void* hseq16, long long ldh,
                 void* gates16, float* cstate, float* h32, long long ldh32, int* flags, void* stream);
 
@@ -55,7 +55,7 @@ void ft_debug_set_lstm_trace(long long* buf);
 void ft_debug_set_infer_trace(long long* buf);
 
 /* Process-wide switch: 1 = ft_lstm_fwd (and ft_ar_step_fwd) use the 64-CTA recurrence kernel so two half-batch
- * launches on two streams run concurrently (the BPTT kernel always uses 64 CTAs for B <= 32). */
+ * launches on two streams run concurrently (the BPTT kernel always uses 64 CTAs). */
 void ft_set_lstm_half_sm(int on);
 /* ft_gemm tile policy: 0 = one CTA per 128 x 256 tile always; 1 (default) = CTA pairs (2-CTA clusters sharing B by TMA multicast, 256 x 256 tiles) for
  * contractions >= 1e11 FLOP; 2 = CTA pairs whenever the output is wide and has >= SMs/2 such tiles. */
@@ -65,7 +65,7 @@ void ft_set_gemm_pair_mode(int mode);
  * [T*B, ldd] (ignored at t >= lens[b]; the caller may pre-multiply it by a power-of-two loss scale).  whhT16:
  * fp16 copy of weight_hh^T [1024,4096].  Writes dG (fp16 [T*B,4096], saturating), the gradient w.r.t. the gate
  * pre-activations; dW_ih, dW_hh, db and dx are GEMMs / column sums over dG done by the caller.
- * flags: int scratch [T*64]. */
+ * flags: int scratch [T*64].  B <= 32. */
 int ft_lstm_bwd(int T, int B, const float* dh_ext, long long ldd, const void* whhT16, const void* gates16,
                 const float* cstate, const int* lens, void* dG16, int* flags, void* stream);
 
@@ -74,7 +74,8 @@ int ft_lstm_bwd(int T, int B, const float* dh_ext, long long ldd, const void* wh
  * ---------------------------------------------------------------------------------------------------- */
 typedef struct {
     int T, B, L;        /* mel frames (padded max), batch, text tokens (padded max) */
-    int n_mel;          /* 80  (n_mel_channels)                                     */
+                        /* B <= 32 per training call (ft_ar_step_infer: <= 16)      */
+    int n_mel;          /* 80  (n_mel_channels, <= 128)                             */
     int n_hidden;       /* 1024 (must be 1024 in this build)                        */
     int n_attn;         /* 640 (n_attn_channels)                                    */
     int n_text;         /* 640 = n_text_dim + n_speaker_dim                         */

@@ -177,7 +177,8 @@ def test_two_stream_half_batches_equal_single_stream():
 
 
 def test_batches_larger_than_a_launch_are_chunked():
-    """B > 64 runs as consecutive <= 64-utterance launches; rows must equal the unchunked result."""
+    """B > max_kernel_batch runs as consecutive launches of at most max_kernel_batch utterances; rows must equal the
+    unchunked result."""
     cfg = dict(synth.DEFAULT_MODEL_CONFIG, n_flows=2)
     model = build_model(cfg, 13)
     batch = synth.synth_batch(6, 24, 10, cfg, 3)
@@ -227,10 +228,10 @@ def test_encoder_streams_and_overlap_equal_serial():
             assert d <= 1e-3 * (g1[k].norm().item() + 1e-4 * gmax), (rep, k, d)
 
 
-def test_batch_above_32_uses_the_wide_paths_and_matches_split_runs():
-    """B in (32, 64] takes different kernels (no folded attention-LSTM projection, no layer pipeline, single-CTA-ownership
-    BPTT): rows must equal the same utterances run as two B = 20 batches, and the backward must produce the same gradients
-    as the sum of the two halves (cfg 3 runs B = 64 per GPU)."""
+def test_batch_above_32_runs_as_32_plus_8_and_matches_split_runs():
+    """A B = 40 batch runs as a 32-utterance and an 8-utterance flow launch (cfg 3 runs B = 64 per GPU as 32 + 32): rows
+    must equal the same utterances run as two B = 20 batches, and the backward must produce the same gradients as the sum
+    of the two halves."""
     from flowtron_b200 import _lib
     from flowtron_b200.flowtron import FlowtronLoss
     torch.backends.cudnn.allow_tf32 = False
@@ -264,3 +265,20 @@ def test_batch_above_32_uses_the_wide_paths_and_matches_split_runs():
     for k in gf:
         d = (gf[k] - (ga[k] + gb[k])).norm().item()
         assert d <= 2e-2 * (gf[k].norm().item() + 1e-3 * gmax), (k, d, gf[k].norm().item())
+
+
+def test_ar_step_rejects_more_than_32_utterances_per_call():
+    """A flow step called directly takes at most 32 utterances (Flowtron.forward splits larger batches itself)."""
+    from flowtron_b200 import _lib
+    cfg = dict(synth.DEFAULT_MODEL_CONFIG, n_flows=2)
+    step = build_model(cfg, 5).flows[0]
+    T, B, L = 16, 33, 8
+    E = cfg["n_text_dim"] + cfg["n_speaker_dim"]
+    mel = torch.randn(T, B, cfg["n_mel_channels"], device="cuda")
+    text = torch.randn(L, B, E, device="cuda")
+    mask = torch.zeros(B, L, 1, dtype=torch.bool, device="cuda")
+    out_lens = torch.full((B,), T, dtype=torch.long, device="cuda")
+    with torch.no_grad(), pytest.raises(_lib.FlowtronB200Error, match="batch > 32"):
+        step(mel, text, mask, out_lens)
+    torch.cuda.synchronize()
+    assert _lib.device_status() == 0

