@@ -53,6 +53,12 @@ struct InferParams {
     const float* attn_forced;              // [T,B,L] forced alignments (flowtron.py:585-588, 797): scoring is skipped
     float inv_temperature, gate_threshold;
     int has_gate;
+    // ragged batches (ft_ar_step_infer_ragged; all null / 0 for ft_ar_step_infer): keys l >= in_lens[b] take no part in the
+    // softmax; utterance b generates at most frame_lens[b] frames (default T); reversed: frame i reads residual row
+    // frame_lens[b] - 1 - i (the residual is then in natural time order)
+    const int* in_lens;
+    const int* frame_lens;
+    int reversed;
     // outputs
     float* out;                            // [T,B,M]
     float* attn_out;                       // [T,B,L]
@@ -371,6 +377,15 @@ __device__ __forceinline__ void lstm_pre(const InferParams& p, const float* bias
     }
 }
 
+// Residual of frame i, utterance b, channel m.  Frames past the utterance's budget are never read (0: such frames are not
+// emitted); a reversed flow reads its own frames back to front.
+__device__ __forceinline__ float residual_at(const InferParams& p, int i, int b, int m) {
+    const int n = p.frame_lens ? p.frame_lens[b] : p.T;
+    if (i >= n) return 0.f;
+    const int t = p.reversed ? n - 1 - i : i;
+    return p.residual[(static_cast<long long>(t) * p.B + b) * p.M + m];
+}
+
 // Context of utterance b, channels [CW s, CW s + CW) (CW = 64 or 128), inside one CTA: warp 0 turns the scores into attention weights (softmax,
 // prior posterior -- or the forced alignment), all 16 warps then take L/16 keys each (every V load of the CTA in flight at
 // once), partial sums meet in shared memory.  Writes ctx (fp16 for lstm layer 0, fp32 for the gate) and, from slice 0, the
@@ -380,6 +395,7 @@ __device__ __forceinline__ void context_item(const InferParams& p, float* sf, in
     constexpr int NV = CW / 32;                                    // channels per lane
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     float* se = sf; float* sp = sf + LMAX;                         // attn [LMAX], partials [16 warps][CW]
+    const int Lb = p.in_lens ? p.in_lens[b] : p.L;                 // key mask: tokens l >= Lb get weight 0 (as if L were Lb)
     if (warp == 0) {
         float w[8];
         if (!forced) {                                            // softmax over L in registers: lane holds l = lane + 32 jj
@@ -388,14 +404,14 @@ __device__ __forceinline__ void context_item(const InferParams& p, float* sf, in
             for (int jj = 0; jj < 8; ++jj) {
                 const int l = lane + 32 * jj;
                 w[jj] = -INFINITY;
-                if (l < p.L) w[jj] = poll_f32(SL(p.e, cur) + b * p.L + l, p.status, 303);
+                if (l < Lb) w[jj] = poll_f32(SL(p.e, cur) + b * p.L + l, p.status, 303);
                 mx = fmaxf(mx, w[jj]);
             }
 #pragma unroll
             for (int o = 16; o; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
             float sum = 0.f;
 #pragma unroll
-            for (int jj = 0; jj < 8; ++jj) { w[jj] = (lane + 32 * jj < p.L) ? expf(w[jj] - mx) : 0.f; sum += w[jj]; }
+            for (int jj = 0; jj < 8; ++jj) { w[jj] = (lane + 32 * jj < Lb) ? expf(w[jj] - mx) : 0.f; sum += w[jj]; }
 #pragma unroll
             for (int o = 16; o; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
             const float inv = 1.f / sum;
@@ -406,7 +422,7 @@ __device__ __forceinline__ void context_item(const InferParams& p, float* sf, in
 #pragma unroll
                 for (int jj = 0; jj < 8; ++jj) {
                     const int l = lane + 32 * jj;
-                    if (l < p.L) {
+                    if (l < Lb) {
                         const float pr = p.prior[(static_cast<long long>(b) * p.T + i) * p.L + l];
                         w[jj] = logf(w[jj] + 1e-20f) + logf(pr + 1e-20f);
                         m2 = fmaxf(m2, w[jj]);
@@ -416,7 +432,7 @@ __device__ __forceinline__ void context_item(const InferParams& p, float* sf, in
                 for (int o = 16; o; o >>= 1) m2 = fmaxf(m2, __shfl_xor_sync(0xffffffffu, m2, o));
                 float s2 = 0.f;
 #pragma unroll
-                for (int jj = 0; jj < 8; ++jj) { w[jj] = (lane + 32 * jj < p.L) ? expf(w[jj] - m2) : 0.f; s2 += w[jj]; }
+                for (int jj = 0; jj < 8; ++jj) { w[jj] = (lane + 32 * jj < Lb) ? expf(w[jj] - m2) : 0.f; s2 += w[jj]; }
 #pragma unroll
                 for (int o = 16; o; o >>= 1) s2 += __shfl_xor_sync(0xffffffffu, s2, o);
                 const float inv2 = 1.f / s2;
@@ -439,13 +455,13 @@ __device__ __forceinline__ void context_item(const InferParams& p, float* sf, in
 #pragma unroll
         for (int e = 0; e < NV; ++e) acc[e] = 0.f;
         constexpr int CU = 8;
-        for (int l0 = warp; l0 < p.L; l0 += CU * INF_WARPS) {
+        for (int l0 = warp; l0 < Lb; l0 += CU * INF_WARPS) {
             float v[CU][NV];
 #pragma unroll
             for (int u = 0; u < CU; ++u) {
                 const int l = l0 + u * INF_WARPS;
                 const float* vr = p.Vp + (static_cast<long long>(l) * p.B + b) * p.A + CW * s + NV * lane;
-                if (l < p.L) {
+                if (l < Lb) {
                     if (NV == 2) { const float2 t = *reinterpret_cast<const float2*>(vr); v[u][0] = t.x; v[u][1] = t.y; }
                     else { const float4 t = *reinterpret_cast<const float4*>(vr); v[u][0] = t.x; v[u][1] = t.y; v[u][NV - 2] = t.z; v[u][NV - 1] = t.w; }
                 } else {
@@ -456,7 +472,7 @@ __device__ __forceinline__ void context_item(const InferParams& p, float* sf, in
 #pragma unroll
             for (int u = 0; u < CU; ++u) {
                 const int l = l0 + u * INF_WARPS;
-                const float w = l < p.L ? se[l] : 0.f;
+                const float w = l < Lb ? se[l] : 0.f;
 #pragma unroll
                 for (int e = 0; e < NV; ++e) acc[e] = fmaf(w, v[u][e], acc[e]);
             }
@@ -614,6 +630,7 @@ infer_kernel(InferParams p) {
                     for (int w2 = 0; w2 < INF_WARPS; ++w2) tot += sf[w2];
                     if (was_alive && sigmoid_f(tot + p.bg[0]) > p.gate_threshold) alive = false;
                 }
+                if (p.frame_lens && i + 1 >= p.frame_lens[b]) alive = false;       // the row's frame budget is spent
                 if (was_alive) p.n_frames[b] = i + 1;
                 st_rlx_u32(SL(p.alive, cur) + b, alive ? 1u : 0u);
                 st_rlx_u32(SL(p.alive, nxt) + b, SENT);
@@ -668,8 +685,8 @@ infer_kernel(InferParams p) {
         if (act_conv && warp == 0) {
             const int j = lane & 3, r = lane >> 2, m = 4 * blockIdx.x + j;
             cb0 = p.bc[blockIdx.x * 8 + 2 * j]; cb1 = p.bc[blockIdx.x * 8 + 2 * j + 1];
-            if (r < p.B) rpre[0] = p.residual[(static_cast<long long>(i) * p.B + r) * p.M + m];
-            if (kB16 && r + 8 < p.B) rpre[1] = p.residual[(static_cast<long long>(i) * p.B + r + 8) * p.M + m];
+            if (r < p.B) rpre[0] = residual_at(p, i, r, m);
+            if (kB16 && r + 8 < p.B) rpre[1] = residual_at(p, i, r + 8, m);
         }
         if (act_conv) stage3<false, kB16>(sx, 0, SL(p.y216, cur_r), IH, IH, 0, nullptr, 0, 0, 0, nullptr, 0, 0, p.B, p.status);
         __syncthreads();
@@ -686,7 +703,7 @@ infer_kernel(InferParams p) {
                     // a sample that stopped at an earlier frame emits zeros; the frame that trips the gate is still emitted
                     // (s_nfr: updated above from the flags every CTA read)
                     const bool emit = (i < s_nfr[b]);
-                    const float res = first ? rpre[half] : p.residual[ro + m];
+                    const float res = first ? rpre[half] : residual_at(p, i, b, m);
                     const float val = (res - (d[2 * half + 1] + bb)) / expf(d[2 * half] + bl);
                     p.out[ro + m] = emit ? val : 0.f;
 #pragma unroll
@@ -777,20 +794,25 @@ static InferScratch plan_infer(const FtArStepDesc& d, uint8_t* base) {
     return s;
 }
 
-}  // namespace ft
+// After a ragged launch: row (i, b) with i >= n_frames[b] gets zero attention weights; a reversed flow's emitted frames are
+// flipped within n_frames[b] (frame j <-> n - 1 - j, swapped by the CTA that owns the lower of the two rows).
+__global__ void infer_ragged_finish_kernel(float* __restrict__ out, float* __restrict__ attn_out, const int* __restrict__ n_frames,
+                                           int T, int B, int M, int L, int reversed) {
+    for (int row = blockIdx.x; row < T * B; row += gridDim.x) {
+        const int i = row / B, b = row - i * B, n = n_frames[b];
+        if (i >= n) {
+            for (int l = threadIdx.x; l < L; l += blockDim.x) attn_out[static_cast<long long>(row) * L + l] = 0.f;
+        } else if (reversed && 2 * i + 1 < n) {
+            float* x = out + static_cast<long long>(row) * M;
+            float* y = out + (static_cast<long long>(n - 1 - i) * B + b) * M;
+            for (int m = threadIdx.x; m < M; m += blockDim.x) { const float t = x[m]; x[m] = y[m]; y[m] = t; }
+        }
+    }
+}
 
-extern "C" {
-
-/* debug: device buffer [T][32] receiving clock64 stamps of CTA 0 of the next ft_ar_step_infer launches (NULL disables) */
-void ft_debug_set_infer_trace(long long* buf) { ft::g_infer_trace = buf; }
-
-size_t ft_ar_step_infer_scratch_bytes(const FtArStepDesc* d) { return ft::plan_infer(*d, nullptr).total + 256; }
-
-int ft_ar_step_infer(const FtArStepDesc* d, const FtArStepWeights* w, const float* residual, const float* text,
-                     const float* attn_prior, const float* attn_forced, float gate_threshold, float* out, float* attn_out,
-                     int* n_frames, void* scratch, void* stream) {
-    using namespace ft;
-    if (!d || !w || !residual || !text || !out || !attn_out || !n_frames || !scratch) return ft_set_error("ft_ar_step_infer: NULL argument");
+static int infer_impl(const FtArStepDesc* d, const FtArStepWeights* w, const float* residual, const float* text,
+                      const float* attn_prior, const float* attn_forced, const int* in_lens, const int* frame_lens, int reversed,
+                      float gate_threshold, float* out, float* attn_out, int* n_frames, void* scratch, void* stream) {
     if (d->n_hidden != IH) return ft_set_error("infer: n_hidden must be 1024");
     if (d->L > LMAX) return ft_set_error("infer: L > 256 not supported");
     if (d->B > 16) return ft_set_error("infer: batch > 16 per call not supported (run the batch in slices of 16)");
@@ -831,6 +853,7 @@ int ft_ar_step_infer(const FtArStepDesc* d, const FtArStepWeights* w, const floa
     p.v = w->att_v; p.wg = w->gate_w; p.bg = w->gate_b;
     p.Kp = s.Kp; p.Vp = s.Vp; p.residual = residual; p.prior = d->has_prior ? attn_prior : nullptr;
     p.attn_forced = attn_forced;
+    p.in_lens = in_lens; p.frame_lens = frame_lens; p.reversed = reversed;
     p.inv_temperature = 1.0f / d->temperature; p.gate_threshold = gate_threshold;
     p.has_gate = d->has_gate && w->gate_w;
     p.out = out; p.attn_out = attn_out; p.n_frames = n_frames;
@@ -874,6 +897,44 @@ int ft_ar_step_infer(const FtArStepDesc* d, const FtArStepWeights* w, const floa
     if (e != cudaSuccess) return ft_set_error(cudaGetErrorString(e));
     ft_count_launch(1);
     return ft_check_launch("infer_kernel");
+}
+
+}  // namespace ft
+
+extern "C" {
+
+/* debug: device buffer [T][32] receiving clock64 stamps of CTA 0 of the next ft_ar_step_infer launches (NULL disables) */
+void ft_debug_set_infer_trace(long long* buf) { ft::g_infer_trace = buf; }
+
+size_t ft_ar_step_infer_scratch_bytes(const FtArStepDesc* d) { return ft::plan_infer(*d, nullptr).total + 256; }
+
+int ft_ar_step_infer(const FtArStepDesc* d, const FtArStepWeights* w, const float* residual, const float* text,
+                     const float* attn_prior, const float* attn_forced, float gate_threshold, float* out, float* attn_out,
+                     int* n_frames, void* scratch, void* stream) {
+    using namespace ft;
+    if (!d || !w || !residual || !text || !out || !attn_out || !n_frames || !scratch) return ft_set_error("ft_ar_step_infer: NULL argument");
+    return infer_impl(d, w, residual, text, attn_prior, attn_forced, nullptr, nullptr, 0, gate_threshold, out, attn_out, n_frames,
+                          scratch, stream);
+}
+
+int ft_ar_step_infer_ragged(const FtArStepDesc* d, const FtArStepWeights* w, const float* residual, const float* text,
+                            const int* in_lens, const int* frame_lens, float gate_threshold, float* out, float* attn_out,
+                            int* n_frames, void* scratch, void* stream) {
+    using namespace ft;
+    if (!d || !w || !residual || !text || !out || !attn_out || !n_frames || !scratch) return ft_set_error("ft_ar_step_infer_ragged: NULL argument");
+    if (d->has_prior) return ft_set_error("ft_ar_step_infer_ragged: attn_prior is not supported");
+    const int rev = d->reversed ? 1 : 0;
+    if (infer_impl(d, w, residual, text, nullptr, nullptr, in_lens, frame_lens, rev, gate_threshold, out, attn_out, n_frames,
+                   scratch, stream) != 0)
+        return -1;
+    // frames are generated back to front by a reversed flow: flip each row within its own n_frames (the B = 1 flip), and clear
+    // the attention rows of frames a stopped utterance computed but did not emit
+    const int rows = d->T * d->B;
+    if (rows <= 0) return 0;
+    infer_ragged_finish_kernel<<<rows < 4096 ? rows : 4096, 128, 0, static_cast<cudaStream_t>(stream)>>>(
+        out, attn_out, n_frames, d->T, d->B, d->n_mel, d->L, rev);
+    ft_count_launch(1);
+    return ft_check_launch("infer_ragged_finish_kernel");
 }
 
 }  // extern "C"

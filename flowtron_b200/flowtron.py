@@ -210,6 +210,20 @@ class Encoder(nn.Module):
         return _EncoderTokensFn.apply(self, tokens, embedding.weight, None, False, self.p_dropout if self.training else 0.0,
                                       *self._kernel_params())
 
+    def infer_ragged_tokens(self, tokens, embedding, in_lens):
+        """Encoder.forward(embedding(tokens).transpose(1, 2), in_lens) without dropout for a padded batch in any length
+        order, masked at every batch size: row b equals Encoder.infer on its own first in_lens[b] tokens."""
+        if tokens.size(0) > 64:              # the encoder kernels take up to 64 utterances per call
+            return torch.cat([self.infer_ragged_tokens(tokens[b0:b0 + 64], embedding, in_lens[b0:b0 + 64])
+                              for b0 in range(0, tokens.size(0), 64)], 0)
+        if self._tokens_ok(tokens, embedding):
+            return _EncoderTokensFn.apply(self, tokens, embedding.weight, in_lens, True, 0.0, *self._kernel_params())
+        x = embedding(tokens).transpose(1, 2)
+        if self._kernels_ok(x):
+            return _EncoderFn.apply(self, x, in_lens, True, 0.0, *self._kernel_params())
+        raise FlowtronB200Error("ragged inference needs the encoder kernels (CUDA tensors, 512 channels, 3 convolutions of "
+                                "width 5, MaskedInstanceNorm1d, FT_ENC_KERNELS not 0)")
+
     def _tokens_ok(self, tokens, embedding):
         return (self.use_kernels and tokens.is_cuda and embedding.weight.size(1) == 512 and len(self.convolutions) == 3
                 and tokens.size(0) <= 64 and embedding.padding_idx is None and embedding.max_norm is None
@@ -471,6 +485,12 @@ class AR_Step(nn.Module):
         from .inference import ar_step_infer
         return ar_step_infer(self, residual, text, attns, attn_prior, reversed_flag=False)
 
+    def infer_ragged(self, residual, text, in_lens, frame_lens):
+        """Ragged batch: residual [T,B,M], text [L,B,E], in_lens / frame_lens int32 CUDA [B] -> (out, attention [T,B,L],
+        n_frames); see inference.ar_step_infer_ragged."""
+        from .inference import ar_step_infer_ragged
+        return ar_step_infer_ragged(self, residual, text, in_lens, frame_lens, reversed_flag=False)
+
 
 class AR_Back_Step(nn.Module):
     """flowtron.py:595-642.  The flip/roll of the reference is an index map inside the kernels (no copies, no host syncs)."""
@@ -490,8 +510,30 @@ class AR_Back_Step(nn.Module):
         from .inference import ar_step_infer
         return ar_step_infer(self.ar_step, residual, text, attns, attn_prior, reversed_flag=True)
 
+    def infer_ragged(self, residual, text, in_lens, frame_lens):
+        """As AR_Step.infer_ragged; row b runs back to front over its own first frame_lens[b] frames."""
+        from .inference import ar_step_infer_ragged
+        return ar_step_infer_ragged(self.ar_step, residual, text, in_lens, frame_lens, reversed_flag=True)
+
 
 # --------------------------------------------------------------------------------------------- model
+def _ragged_lengths(v, B: int, hi: int, name: str) -> Tensor:
+    """Per-row lengths for Flowtron.infer_batch: a CUDA tensor is trusted (only its size is checked); host values must be
+    B integers in [1, hi]."""
+    if torch.is_tensor(v) and v.is_cuda:
+        if v.dim() != 1 or v.numel() != B:
+            raise ValueError(f"{name} must hold {B} values, got shape {tuple(v.shape)}")
+        return v
+    t = torch.as_tensor(v)
+    if t.dim() != 1 or t.numel() != B:
+        raise ValueError(f"{name} must hold {B} values, got shape {tuple(t.shape)}")
+    if t.is_floating_point() or t.dtype == torch.bool:
+        raise ValueError(f"{name} must be integers")
+    if bool((t < 1).any()) or bool((t > hi).any()):
+        raise ValueError(f"{name} must lie in [1, {hi}], got {t.tolist()}")
+    return t
+
+
 class Flowtron(nn.Module):
     """flowtron.py:831-961 (n_components=0 / no cumulative attention: the variants every shipped config uses)."""
 
@@ -644,6 +686,56 @@ class Flowtron(nn.Module):
             residual, attention_weight = flow.infer(residual, encoder_outputs, attn, attn_prior=attn_prior)
             attention_weights.append(attention_weight)
         return residual.permute(1, 2, 0), attention_weights
+
+    def infer_batch(self, residual, speaker_ids, text, in_lens, temperature=1.0, gate_threshold=0.5, *, max_frames=None,
+                    attns=None, attn_prior=None):
+        """Inference over a padded batch of texts of different lengths, each with its own frame budget.
+
+        residual [B, 80, T] f32, speaker_ids [B] int64, text [B, L] int64 (row b valid in [0, in_lens[b])), in_lens [B],
+        max_frames [B] (default: T for every row) -> (mel [B, 80, T], mel_lens int64 [B], attention_weights).
+
+        Row b of ``mel[:, :, :mel_lens[b]]`` equals ``infer(residual[b:b+1, :, :max_frames[b]], speaker_ids[b:b+1],
+        text[b:b+1, :in_lens[b]])[0]`` and ``mel_lens[b]`` its length; ``mel`` is zero past ``mel_lens[b]``.  Text tokens at or
+        past in_lens[b] and residual frames at or past max_frames[b] are never used.  ``attention_weights``: one [B, T, L]
+        tensor per flow in the order ``infer`` returns them, in that flow's generation order, zero past the flow's output
+        length and at tokens >= in_lens[b].
+
+        The rows may come in any length order.  The first flow applied gets the budgets ``max_frames``, every later flow the
+        previous flow's frame counts, on the device: there is no host synchronisation (and no "Hitting gate limit" print),
+        so with lengths given as CUDA tensors the whole call can be captured in a CUDA graph.  Lengths given as host
+        sequences or CPU tensors are checked first (ValueError unless 1 <= in_lens[b] <= L <= 256 and
+        1 <= max_frames[b] <= T); CUDA length tensors are trusted, as ``forward`` trusts ``in_lens``.  Any B works; the flows
+        run in slices of at most 16 utterances per kernel launch.  Forced alignments (``attns``) and ``attn_prior`` are
+        not supported here."""
+        if attns is not None or attn_prior is not None:
+            raise ValueError("infer_batch does not take attns or attn_prior (use infer)")
+        if residual.dim() != 3 or text.dim() != 2 or speaker_ids.dim() != 1:
+            raise ValueError("infer_batch expects residual [B, n_mel, T], speaker_ids [B] and text [B, L]")
+        B, _, T = residual.shape
+        L = text.size(1)
+        if text.size(0) != B or speaker_ids.size(0) != B or B < 1 or T < 1 or L < 1:
+            raise ValueError(f"batch sizes disagree or are empty: residual {tuple(residual.shape)}, "
+                             f"speaker_ids {tuple(speaker_ids.shape)}, text {tuple(text.shape)}")
+        if L > 256:
+            raise ValueError(f"text length {L} > 256 is not supported by the inference kernel")
+        in_lens = _ragged_lengths(in_lens, B, L, "in_lens")
+        max_frames = _ragged_lengths([T] * B if max_frames is None else max_frames, B, T, "max_frames")
+        if not (residual.is_cuda and text.is_cuda and speaker_ids.is_cuda):
+            raise FlowtronB200Error("Flowtron.infer_batch needs CUDA tensors: the sm_90a kernels are the only implementation")
+        dev = residual.device
+        in_lens = in_lens.to(device=dev, dtype=torch.int32)
+        lens = max_frames.to(device=dev, dtype=torch.int32)
+        speaker_ids = speaker_ids * 0 if self.dummy_speaker_embedding else speaker_ids
+        speaker_vecs = self.speaker_embedding(speaker_ids)
+        text = self.encoder.infer_ragged_tokens(text, self.embedding, in_lens).transpose(0, 1)
+        encoder_outputs = torch.cat([text, speaker_vecs.expand(text.size(0), -1, -1)], 2)
+        residual = residual.permute(2, 0, 1)
+        attention_weights = []
+        for flow in reversed(self.flows):
+            self.set_temperature_and_gate(flow, temperature, gate_threshold)
+            residual, attn, lens = flow.infer_ragged(residual, encoder_outputs, in_lens, lens)
+            attention_weights.append(attn.transpose(0, 1))
+        return residual.permute(1, 2, 0), lens.long(), attention_weights
 
     @staticmethod
     def set_temperature_and_gate(flow, temperature, gate_threshold):

@@ -72,3 +72,35 @@ def ar_step_infer(step, residual, text, attns, attn_prior=None, reversed_flag=Fa
     if reversed_flag:
         out = torch.flip(out, (0,))
     return out, [a.unsqueeze(1) for a in attn_out]
+
+
+def ar_step_infer_ragged(step, residual, text, in_lens, frame_lens, reversed_flag=False):
+    """Ragged-batch inverse of one flow over ft_ar_step_infer_ragged: row b equals its own B == 1 ``ar_step_infer`` on
+    ``residual[:frame_lens[b], b]`` and ``text[:in_lens[b], b]``.
+
+    residual [T,B,M] in natural time order (AR_Back_Step's reversal happens per row inside the C call), text [L,B,E],
+    in_lens / frame_lens int32 CUDA [B] -> (out [T,B,M] zero past n_frames[b], attention [T,B,L] in generation order,
+    n_frames int32 CUDA [B]).  No host synchronisation; batches above 16 run as slices of 16 that carry their lengths."""
+    if not residual.is_cuda:
+        raise FlowtronB200Error("AR_Step.infer_ragged needs CUDA tensors: the sm_90a kernel is the only implementation")
+    T, B, M = residual.shape
+    L, _, E = text.shape
+    if B > 16:
+        parts = [ar_step_infer_ragged(step, residual[:, b0:b0 + 16], text[:, b0:b0 + 16], in_lens[b0:b0 + 16],
+                                      frame_lens[b0:b0 + 16], reversed_flag) for b0 in range(0, B, 16)]
+        return (torch.cat([p[0] for p in parts], 1), torch.cat([p[1] for p in parts], 1),
+                torch.cat([p[2] for p in parts], 0))
+    dev = residual.device
+    has_gate = hasattr(step, 'gate_layer')
+    desc = _lib.FtArStepDesc(T, B, L, M, step.lstm.hidden_size, step.attention_layer.query.linear_layer.out_features, E,
+                             int(reversed_flag), int(has_gate), 0, float(step.attention_layer.temperature))
+    plist = [None if p is None else p.detach().contiguous() for p in step._param_list()]
+    weights = _lib.make_weights(plist)
+    out = torch.empty(T, B, M, device=dev)
+    attn_out = torch.empty(T, B, L, device=dev)
+    n_frames = torch.empty(B, dtype=torch.int32, device=dev)
+    thr = float(getattr(step, 'gate_threshold', 0.5))
+    _lib.ar_step_infer_ragged(desc, weights, residual.detach().float().contiguous(), text.detach().float().contiguous(),
+                              in_lens.to(device=dev, dtype=torch.int32).contiguous(),
+                              frame_lens.to(device=dev, dtype=torch.int32).contiguous(), thr, out, attn_out, n_frames)
+    return out, attn_out, n_frames

@@ -189,6 +189,24 @@ int ft_ar_step_infer(const FtArStepDesc* d, const FtArStepWeights* w, const floa
                      const float* attn_prior, const float* attn_forced, float gate_threshold, float* out, float* attn_out,
                      int* n_frames, void* scratch, void* stream);
 
+/* The same inverse for a ragged batch: row b equals its own B == 1 ft_ar_step_infer run on its unpadded inputs.
+ *   residual [T,B,M] f32 in NATURAL time order (no caller flip), text [L,B,E] f32; scratch: ft_ar_step_infer_scratch_bytes(d).
+ *   in_lens [B] int32 device or NULL (all L): text length of row b; keys l >= in_lens[b] take no part in the softmax and get
+ *     attention weight 0.
+ *   frame_lens [B] int32 device or NULL (all T): frame budget of row b; row b generates while i < frame_lens[b] and its gate
+ *     has not fired; residual rows t >= frame_lens[b] are never read.
+ *   d->reversed = 1 (AR_Back_Step): frame i reads residual[frame_lens[b] - 1 - i], and the emitted frames come back flipped
+ *     within the row's own n_frames[b] (the B == 1 flip), so `out` is in natural time order too.
+ *   out [T,B,M]: zero at t >= n_frames[b]; attn_out [T,B,L] in generation order, zero at i >= n_frames[b] and l >= in_lens[b];
+ *   n_frames [B] int32 = min(gate stop (the frame that trips the gate is emitted), frame_lens[b]).
+ *   Lengths must satisfy 1 <= in_lens[b] <= L and 1 <= frame_lens[b] <= T; they are read on the device only.
+ *   Limits as ft_ar_step_infer: B <= 16, L <= 256; d->has_prior must be 0 (no attn_prior, no forced alignments).
+ *   Two launches (the persistent kernel, then a small per-row flip / attention clear), no host synchronisation:
+ *   CUDA-graph capturable. */
+int ft_ar_step_infer_ragged(const FtArStepDesc* d, const FtArStepWeights* w, const float* residual, const float* text,
+                            const int* in_lens, const int* frame_lens, float gate_threshold, float* out, float* attn_out,
+                            int* n_frames, void* scratch, void* stream);
+
 /* TacotronSTFT.mel_spectrogram (audio_processing.py:117-134) for a ragged batch.  wav: concatenated utterances
  * (f32 in [-1,1]); sample_offsets / frame_offsets: device int64 [n_utt+1] prefix sums (frames of utterance u =
  * 1 + N_u / hop); window [n_fft] (periodic Hann, centre-padded); mel_basis [n_mel, n_fft/2+1] with its non-zero

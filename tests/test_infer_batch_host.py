@@ -1,0 +1,105 @@
+"""CPU: Flowtron.infer_batch argument checks, the oracle's restatement of its contract against the reference-generated
+fixtures (tests/make_golden_infer_batch.py), and the register budget of the inference kernel."""
+import os
+import re
+import shutil
+import subprocess
+
+import numpy as np
+import pytest
+import torch
+
+from conftest import GOLDEN, ROOT
+from flowtron_b200 import synth
+
+NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
+HAVE_NVCC = os.path.exists(NVCC) or shutil.which("nvcc") is not None
+
+
+def _params(g):
+    cfg = dict(synth.DEFAULT_MODEL_CONFIG, n_flows=int(g["cfg_n_flows"]), n_speakers=int(g["n_speakers"]))
+    p = synth.synth_params(cfg, int(g["seed"]))
+    kb = [k for k in p if k.endswith("gate_layer.linear_layer.bias")][0]
+    kw = [k for k in p if k.endswith("gate_layer.linear_layer.weight")][0]
+    p[kb] = torch.full_like(p[kb], float(g["gate_bias"]))
+    p[kw] = p[kw] * float(g["gate_scale"])
+    return cfg, p
+
+
+@pytest.fixture(scope="module")
+def cpu_model():
+    from flowtron_b200.flowtron import Flowtron
+    cfg = dict(synth.DEFAULT_MODEL_CONFIG, n_flows=2)
+    m = Flowtron(**cfg)
+    m.load_state_dict(synth.synth_params(cfg, 3), strict=True)
+    return m.eval()
+
+
+def test_argument_validation(cpu_model):
+    from flowtron_b200._lib import FlowtronB200Error
+    B, T, L = 3, 20, 9
+    res = torch.zeros(B, 80, T)
+    spk = torch.zeros(B, dtype=torch.long)
+    text = torch.zeros(B, L, dtype=torch.long)
+    bad = [
+        dict(in_lens=[9, 4]),                                   # wrong count
+        dict(in_lens=[9, 0, 4]),                                # empty text
+        dict(in_lens=[9, 10, 4]),                               # longer than L
+        dict(in_lens=torch.tensor([9, 4, 4, 4])),
+        dict(in_lens=[9.0, 4.0, 4.0]),
+        dict(in_lens=[9, 4, 4], max_frames=[20, 21, 5]),        # budget above T
+        dict(in_lens=[9, 4, 4], max_frames=[20, 0, 5]),
+        dict(in_lens=[9, 4, 4], max_frames=torch.tensor([20, 5])),
+        dict(in_lens=[9, 4, 4], attns=[torch.zeros(T, L)] * 2),
+        dict(in_lens=[9, 4, 4], attn_prior=torch.zeros(B, T, L)),
+    ]
+    for kw in bad:
+        with pytest.raises(ValueError):
+            cpu_model.infer_batch(res, spk, text, **kw)
+    with pytest.raises(ValueError):                             # longer than the kernel's 256 keys
+        cpu_model.infer_batch(res, spk, torch.zeros(B, 257, dtype=torch.long), [9, 4, 4])
+    with pytest.raises(ValueError):                             # batch sizes disagree
+        cpu_model.infer_batch(res[:2], spk, text, [9, 4, 4])
+    # valid arguments, but CPU tensors: there is no CPU implementation
+    with pytest.raises(FlowtronB200Error):
+        cpu_model.infer_batch(res, spk, text, [9, 4, 4], max_frames=[20, 7, 13])
+    with pytest.raises(FlowtronB200Error):
+        cpu_model.infer_batch(res, spk, text, torch.tensor([9, 4, 4]))
+
+
+@pytest.mark.parametrize("tag", ["f2", "f3", "t400"])
+def test_oracle_infer_batch_matches_reference_fixtures(tag):
+    from infer_batch_oracle import flowtron_infer_batch
+    g = dict(np.load(os.path.join(GOLDEN, f"infer_ragged_{tag}.npz")))
+    _, p = _params(g)
+    torch.set_num_threads(max(1, min(8, os.cpu_count() or 1)))
+    with torch.no_grad():
+        mel, lens = flowtron_infer_batch(p, torch.from_numpy(g["residual"]), torch.from_numpy(g["speaker_ids"]),
+                                         torch.from_numpy(g["text"]), g["in_lens"].tolist(),
+                                         max_frames=g["max_frames"].tolist())
+    assert lens.tolist() == g["mel_lens"].tolist()
+    ref = torch.from_numpy(g["mel"])
+    err = (mel - ref).abs().max().item() / ref.abs().max().item()
+    assert err <= 1e-5, err
+
+
+def test_fixtures_cover_gate_stops_and_budgets():
+    for tag, need_stops in (("f2", 2), ("f3", 2), ("t400", 0)):
+        g = np.load(os.path.join(GOLDEN, f"infer_ragged_{tag}.npz"))
+        stopped = int((g["mel_lens"] < g["max_frames"]).sum())
+        assert stopped >= need_stops and len(g["mel_lens"]) - stopped >= 2, (tag, g["mel_lens"], g["max_frames"])
+        assert (np.diff(g["in_lens"]) > 0).any() and (np.diff(g["in_lens"]) < 0).any()     # not sorted
+
+
+@pytest.mark.skipif(not HAVE_NVCC, reason="nvcc not available")
+def test_infer_kernel_does_not_spill(tmp_path):
+    r = subprocess.run([NVCC, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "--expt-relaxed-constexpr",
+                        "-Xptxas", "-v", "-c", os.path.join(ROOT, "flowtron_b200", "csrc", "infer.cu"), "-o",
+                        str(tmp_path / "infer.o")], capture_output=True, text=True)
+    assert r.returncode == 0, r.stderr
+    parts = r.stderr.split("Compiling entry function")
+    logs = [s for s in parts if "infer_kernel" in s.splitlines()[0]]
+    assert len(logs) == 2, r.stderr                             # the B <= 8 and B <= 16 instantiations
+    for log in logs:
+        m = re.search(r"(\d+) bytes spill stores, (\d+) bytes spill loads", log)
+        assert m and m.groups() == ("0", "0"), log
