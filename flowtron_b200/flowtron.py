@@ -5,15 +5,13 @@ Same class names, constructor signatures, attribute names and ``state_dict`` lay
 Attention :528-592, DenseLayer :453-464, LinearNorm :278-288, Encoder :467-525, FlowtronLoss :185-275), so a
 reference checkpoint loads with ``strict=True`` and callers switch by changing the import.
 
-The flow steps, the NLL/gate loss and inference run on hand-written sm_90a kernels through the C ABI
-(include/flowtron_b200.h).  There is NO torch/CPU fallback for that path: CPU tensors raise.  The Encoder and
-the embeddings (run once per utterance over L tokens, <2% of FLOPs; SURVEY.md §8f "next") stay ordinary
-PyTorch modules, written device-agnostically.
+The text encoder (with the text-embedding lookup fused in), the flow steps, the NLL/gate loss and inference run on
+hand-written sm_90a kernels through the C ABI (include/flowtron_b200.h).  There is NO torch/CPU fallback: CPU tensors
+raise, and sizes the kernels are not built for raise NotImplementedError at construction.  The speaker embedding and
+the [text ; speaker] concatenation stay ordinary PyTorch.
 """
 from __future__ import annotations
 
-import os
-import warnings
 from typing import Optional
 
 import torch
@@ -34,7 +32,7 @@ def get_mask_from_lengths(lengths: Tensor) -> Tensor:
 get_gate_mask_from_lengths = get_mask_from_lengths
 
 
-# --------------------------------------------------------------------------------------------- encoder (torch)
+# --------------------------------------------------------------------------------------------- encoder
 def masked_instance_norm(input, mask, weight, bias, eps: float = 1e-5):
     """flowtron.py:53-92 with use_input_stats=True, no running stats."""
     lengths = mask.sum((-1,))
@@ -103,78 +101,57 @@ def _encoder_overlap_stream(device):
 
 
 class _EncoderFn(torch.autograd.Function):
-    """Encoder.forward / Encoder.infer on the CUDA kernels (ft_encoder_fwd / ft_encoder_bwd)."""
+    """Encoder forward / backward on the CUDA kernels for up to 64 utterances: ft_encoder_fwd / ft_encoder_bwd on x [B, 512, L],
+    or, given tokens [B, L] and the embedding weight instead of x, ft_encoder_fwd_tokens / ft_encoder_bwd_tokens, which fuse the
+    row gather into the first kernel and scatter the embedding gradient from the last one."""
 
     @staticmethod
-    def forward(ctx, enc, x, in_lens, masked, dropout_p, *flat_params):
-        B, C, L = x.shape
-        names = [n for n, _ in _lib.ENC_PARAM_FIELDS]
-        counts = [k for _, k in _lib.ENC_PARAM_FIELDS]
-        params, i = {}, 0
-        for n, k in zip(names, counts):
-            params[n] = [t.detach().contiguous() for t in flat_params[i:i + k]]
-            i += k
-        desc = _lib.encoder_desc(B, L, masked, dropout_p, enc.convolutions[0][1].eps)
-        lens32 = in_lens.to(torch.int32) if masked else None
-        x = x.detach().contiguous().float()
-        out = torch.empty(B, L, C, dtype=torch.float32, device=x.device)
-        rng = enc._rng_state(x.device) if dropout_p > 0 else None
-        saved = _lib.encoder_fwd(desc, params, x, lens32, rng, out, out.stride(0), out.stride(1))
-        ctx.desc, ctx.params, ctx.saved = desc, params, saved
-        ctx.need_dx = x.requires_grad or ctx.needs_input_grad[1]
-        return out
-
-    @staticmethod
-    def backward(ctx, d_out):
-        if ctx.saved is None:
-            raise RuntimeError("Encoder backward called twice (the saved activations were released)")
-        d_x, grads = _lib.encoder_bwd(ctx.desc, ctx.params, d_out.contiguous().float(), ctx.saved, need_dx=ctx.need_dx)
-        ctx.saved = None
-        flat = []
-        for n, _ in _lib.ENC_PARAM_FIELDS:
-            flat += grads[n]
-        return (None, d_x, None, None, None, *flat)
-
-
-class _EncoderTokensFn(torch.autograd.Function):
-    """embedding(text) + Encoder.forward / .infer on the CUDA kernels with the row gather fused into the first kernel and the
-    embedding gradient scattered by the last one (ft_encoder_fwd_tokens / ft_encoder_bwd_tokens)."""
-
-    @staticmethod
-    def forward(ctx, enc, tokens, emb_weight, in_lens, masked, dropout_p, *flat_params):
-        B, L = tokens.shape
+    def forward(ctx, enc, x, tokens, emb_weight, in_lens, masked, dropout_p, *flat_params):
         params, i = {}, 0
         for n, k in _lib.ENC_PARAM_FIELDS:
             params[n] = [t.detach().contiguous() for t in flat_params[i:i + k]]
             i += k
+        if x is None:
+            B, L = tokens.shape
+            tokens, emb_weight, dev = tokens.contiguous(), emb_weight.detach().contiguous(), tokens.device
+        else:
+            B, _, L = x.shape
+            x, dev = x.detach().contiguous().float(), x.device
         desc = _lib.encoder_desc(B, L, masked, dropout_p, enc.convolutions[0][1].eps)
         lens32 = in_lens.to(torch.int32) if masked else None
-        tokens = tokens.contiguous()
-        embw = emb_weight.detach().contiguous()
-        out = torch.empty(B, L, embw.size(1), dtype=torch.float32, device=tokens.device)
-        rng = enc._rng_state(tokens.device) if dropout_p > 0 else None
-        saved = _lib.encoder_fwd(desc, params, None, lens32, rng, out, out.stride(0), out.stride(1), tokens=tokens, emb_weight=embw)
-        ctx.desc, ctx.params, ctx.saved, ctx.tokens, ctx.embw = desc, params, saved, tokens, embw
+        out = torch.empty(B, L, 512, dtype=torch.float32, device=dev)
+        rng = enc._rng_state(dev) if dropout_p > 0 else None
+        saved = _lib.encoder_fwd(desc, params, x, lens32, rng, out, out.stride(0), out.stride(1), tokens=tokens, emb_weight=emb_weight)
+        ctx.desc, ctx.params, ctx.saved, ctx.tokens, ctx.emb_weight = desc, params, saved, tokens, emb_weight
         return out
 
     @staticmethod
     def backward(ctx, d_out):
         if ctx.saved is None:
             raise RuntimeError("Encoder backward called twice (the saved activations were released)")
-        d_emb, grads = _lib.encoder_bwd(ctx.desc, ctx.params, d_out.contiguous().float(), ctx.saved, tokens=ctx.tokens, emb_weight=ctx.embw)
+        d_in, grads = _lib.encoder_bwd(ctx.desc, ctx.params, d_out.contiguous().float(), ctx.saved, need_dx=ctx.needs_input_grad[1],
+                                       tokens=ctx.tokens, emb_weight=ctx.emb_weight)
         ctx.saved = None
         flat = []
         for n, _ in _lib.ENC_PARAM_FIELDS:
             flat += grads[n]
-        return (None, None, d_emb, None, None, None, *flat)
+        d_x, d_emb = (d_in, None) if ctx.tokens is None else (None, d_in)
+        return (None, d_x, None, d_emb, None, None, None, *flat)
+
+
+_ENC_MAX_BATCH = 64                  # utterances per encoder-kernel call (the kernels reject more)
 
 
 class Encoder(nn.Module):
-    """flowtron.py:467-525 (3 x conv+masked instance norm+relu+dropout, packed BiLSTM).  CUDA tensors run on the encoder kernels
-    (csrc/encoder.cu); the torch code below is the module's CPU mirror (host-logic tests) and the FT_ENC_KERNELS=0 A/B path."""
+    """flowtron.py:467-525 (3 x conv+masked instance norm+relu+dropout, packed BiLSTM) on the encoder kernels
+    (csrc/encoder.cu), which are built for 512 channels, 3 convolutions of width 5 and MaskedInstanceNorm1d."""
 
     def __init__(self, encoder_n_convolutions=3, encoder_embedding_dim=512, encoder_kernel_size=5, norm_fn=nn.BatchNorm1d):
         super().__init__()
+        if (encoder_n_convolutions != 3 or encoder_kernel_size != 5 or encoder_embedding_dim != 512
+                or norm_fn is not MaskedInstanceNorm1d):
+            raise NotImplementedError("the sm_90a encoder kernels are built for encoder_n_convolutions=3, encoder_kernel_size=5, "
+                                      "encoder_embedding_dim=512 and norm_fn=MaskedInstanceNorm1d (Flowtron with n_text_dim=512)")
         convolutions = []
         for _ in range(encoder_n_convolutions):
             convolutions.append(nn.Sequential(
@@ -184,7 +161,6 @@ class Encoder(nn.Module):
         self.convolutions = nn.ModuleList(convolutions)
         self.lstm = nn.LSTM(encoder_embedding_dim, int(encoder_embedding_dim / 2), 1, batch_first=True, bidirectional=True)
         self.p_dropout = 0.5        # flowtron.py:502 hard-codes 0.5; exposed so tests can run deterministic train-mode steps
-        self.use_kernels = os.environ.get("FT_ENC_KERNELS", "1") != "0"
         self._rng = None
 
     def _rng_state(self, device):
@@ -200,87 +176,43 @@ class Encoder(nn.Module):
             flat += [getattr(self.lstm, n), getattr(self.lstm, n + "_reverse")]
         return flat
 
+    def _run(self, x, tokens, emb_weight, in_lens, masked, dropout=True):
+        """x [B, 512, L], or tokens [B, L] with the embedding weight -> [B, L, 512].  A batch above 64 utterances runs as
+        consecutive calls of at most 64 (utterances are independent); `masked` is decided from the whole batch, so a 1-row
+        tail call is masked like the rest."""
+        src = x if tokens is None else tokens
+        if not src.is_cuda:
+            raise FlowtronB200Error("Encoder needs CUDA tensors: the sm_90a kernels are the only implementation")
+        C = (x if tokens is None else emb_weight).size(1)
+        if C != 512:
+            raise ValueError(f"the encoder kernels take 512 channels, got {C}")
+        dropout_p = self.p_dropout if dropout and self.training else 0.0
+        params = self._kernel_params()
+        rows = lambda t, b0: None if t is None else t[b0:b0 + _ENC_MAX_BATCH]
+        outs = [_EncoderFn.apply(self, rows(x, b0), rows(tokens, b0), emb_weight, rows(in_lens, b0), masked, dropout_p, *params)
+                for b0 in range(0, src.size(0), _ENC_MAX_BATCH)]
+        return outs[0] if len(outs) == 1 else torch.cat(outs, 0)
+
+    def forward(self, x, in_lens):
+        """x [B, 512, L] padded to max(in_lens) (DataCollate guarantees it, data.py:200-208) -> [B, L, 512], zero at
+        l >= in_lens[b]: the reference's packed BiLSTM without packing and without a host sync on in_lens."""
+        return self._run(x, None, None, in_lens, x.size(0) > 1)
+
+    def infer(self, x):
+        return self._run(x, None, None, None, False)
+
     def forward_tokens(self, tokens, embedding, in_lens):
         """Encoder.forward(embedding(tokens).transpose(1, 2), in_lens) with the lookup fused into the encoder kernels."""
-        return _EncoderTokensFn.apply(self, tokens, embedding.weight, in_lens, tokens.size(0) > 1,
-                                      self.p_dropout if self.training else 0.0, *self._kernel_params())
+        return self._run(None, tokens, embedding.weight, in_lens, tokens.size(0) > 1)
 
     def infer_tokens(self, tokens, embedding):
         """Encoder.infer(embedding(tokens).transpose(1, 2)) likewise."""
-        return _EncoderTokensFn.apply(self, tokens, embedding.weight, None, False, self.p_dropout if self.training else 0.0,
-                                      *self._kernel_params())
+        return self._run(None, tokens, embedding.weight, None, False)
 
     def infer_ragged_tokens(self, tokens, embedding, in_lens):
         """Encoder.forward(embedding(tokens).transpose(1, 2), in_lens) without dropout for a padded batch in any length
         order, masked at every batch size: row b equals Encoder.infer on its own first in_lens[b] tokens."""
-        if tokens.size(0) > 64:              # the encoder kernels take up to 64 utterances per call
-            return torch.cat([self.infer_ragged_tokens(tokens[b0:b0 + 64], embedding, in_lens[b0:b0 + 64])
-                              for b0 in range(0, tokens.size(0), 64)], 0)
-        if self._tokens_ok(tokens, embedding):
-            return _EncoderTokensFn.apply(self, tokens, embedding.weight, in_lens, True, 0.0, *self._kernel_params())
-        x = embedding(tokens).transpose(1, 2)
-        if self._kernels_ok(x):
-            return _EncoderFn.apply(self, x, in_lens, True, 0.0, *self._kernel_params())
-        raise FlowtronB200Error("ragged inference needs the encoder kernels (CUDA tensors, 512 channels, 3 convolutions of "
-                                "width 5, MaskedInstanceNorm1d, FT_ENC_KERNELS not 0)")
-
-    def _tokens_ok(self, tokens, embedding):
-        return (self.use_kernels and tokens.is_cuda and embedding.weight.size(1) == 512 and len(self.convolutions) == 3
-                and tokens.size(0) <= 64 and embedding.padding_idx is None and embedding.max_norm is None
-                and self.convolutions[0][0].conv.kernel_size[0] == 5 and isinstance(self.convolutions[0][1], MaskedInstanceNorm1d))
-
-    def _kernels_ok(self, x):
-        return (self.use_kernels and x.is_cuda and x.size(1) == 512 and len(self.convolutions) == 3 and x.size(0) <= 64
-                and self.convolutions[0][0].conv.kernel_size[0] == 5 and isinstance(self.convolutions[0][1], MaskedInstanceNorm1d))
-
-    def _lstm_dir(self, x, sfx):
-        """One direction of the BiLSTM on a padded [B, L, C] batch."""
-        w = [getattr(self.lstm, n + sfx) for n in ("weight_ih_l0", "weight_hh_l0", "bias_ih_l0", "bias_hh_l0")]
-        h0 = x.new_zeros(1, x.size(0), self.lstm.hidden_size)
-        with warnings.catch_warnings():           # "weights are not part of single contiguous chunk": one direction at a time
-            warnings.simplefilter("ignore", UserWarning)
-            out, _, _ = torch._VF.lstm(x, (h0, h0), w, True, 1, 0.0, self.training, False, True)
-        return out
-
-    def _reverse_dir(self, x, rev):
-        gidx = rev[..., None].expand(-1, -1, x.size(2))
-        out = self._lstm_dir(torch.gather(x, 1, gidx), "_reverse")
-        return torch.gather(out, 1, rev[..., None].expand(-1, -1, out.size(2)))
-
-    def forward(self, x, in_lens):
-        """Same result as the reference's packed BiLSTM (flowtron.py:505-512) without packing: the forward direction is
-        causal, so running it over the padded batch and zeroing t >= len is identical; the reverse direction runs on
-        each utterance reversed inside its own length (one gather in, one gather out).  No pack/unpack and no host sync
-        (`in_lens.cpu()`); cuDNN still launches its per-time-step fp32 kernels (measured: same GPU time as packed).
-        Requires the text batch to be padded to max(in_lens), which DataCollate guarantees (data.py:200-208)."""
-        if self._kernels_ok(x):
-            return _EncoderFn.apply(self, x, in_lens, x.size(0) > 1, self.p_dropout if self.training else 0.0, *self._kernel_params())
-        Bn, _, L = x.shape
-        ar = torch.arange(L, device=x.device)
-        valid = ar[None, :] < in_lens[:, None]                                   # [B, L]
-        mask = valid.unsqueeze(1) if Bn > 1 else None
-        for conv, norm in self.convolutions:
-            if mask is not None:
-                x = x.masked_fill(~mask, 0.)
-            x = F.dropout(F.relu(norm(conv(x), mask=mask)), self.p_dropout, self.training)
-        x = x.transpose(1, 2).contiguous()                                        # [B, L, C]
-        rev = torch.where(valid, in_lens[:, None] - 1 - ar[None, :], ar[None, :])   # per-utterance time reversal (involution)
-        fwd = self._lstm_dir(x, "")
-        bwd = self._reverse_dir(x, rev)
-        return torch.cat([fwd, bwd], -1) * valid[..., None].to(x.dtype)
-
-    def infer(self, x):
-        if self._kernels_ok(x):
-            return _EncoderFn.apply(self, x, None, False, self.p_dropout if self.training else 0.0, *self._kernel_params())
-        for conv in self.convolutions:
-            x = F.dropout(F.relu(conv(x)), self.p_dropout, self.training)
-        x = x.transpose(1, 2)
-        # no self.lstm.flatten_parameters() (flowtron.py:521): on cuDNN it moves the weights into a new buffer (param.set_),
-        # which would detach them from a flat-buffer optimizer / all-reduce bucket built earlier
-        with warnings.catch_warnings():
-            warnings.simplefilter("ignore", UserWarning)
-            outputs, _ = self.lstm(x)
-        return outputs
+        return self._run(None, tokens, embedding.weight, in_lens, True, dropout=False)
 
 
 # --------------------------------------------------------------------------------------------- attention params
@@ -560,8 +492,8 @@ class Flowtron(nn.Module):
     # many dependent steps as the full batch); it only lets one half's GEMMs / attention / launch gaps overlap the other
     # half's recurrences.  Off by default.
     n_streams = 1
-    # run the Encoder underneath the first flow's attention LSTM; FT_ENC_OVERLAP=0 disables
-    overlap_encoder = os.environ.get("FT_ENC_OVERLAP", "1") != "0"
+    # run the Encoder underneath the first flow's attention LSTM
+    overlap_encoder = True
     min_split_batch = 8
 
     # Utterances per flow-kernel launch: the flow kernels take at most 32, so a larger batch (configs[2]: B = 64) runs as
@@ -596,11 +528,7 @@ class Flowtron(nn.Module):
         """flowtron.py:871-880: embeddings + Encoder + speaker vector concat -> [L, B, n_text + n_speaker]."""
         speaker_ids = speaker_ids * 0 if self.dummy_speaker_embedding else speaker_ids
         speaker_vecs = self.speaker_embedding(speaker_ids)
-        if self.encoder._tokens_ok(text, self.embedding):
-            text = self.encoder.forward_tokens(text, self.embedding, in_lens)     # embedding gather fused into the encoder kernels
-        else:
-            text = self.encoder(self.embedding(text).transpose(1, 2), in_lens)
-        text = text.transpose(0, 1)
+        text = self.encoder.forward_tokens(text, self.embedding, in_lens).transpose(0, 1)
         return torch.cat([text, speaker_vecs.expand(text.size(0), -1, -1)], 2)
 
     def forward(self, mel, speaker_ids, text, in_lens, out_lens, attn_prior=None):
@@ -672,11 +600,7 @@ class Flowtron(nn.Module):
     def infer(self, residual, speaker_ids, text, temperature=1.0, gate_threshold=0.5, attns=None, attn_prior=None):
         speaker_ids = speaker_ids * 0 if self.dummy_speaker_embedding else speaker_ids
         speaker_vecs = self.speaker_embedding(speaker_ids)
-        if self.encoder._tokens_ok(text, self.embedding):
-            text = self.encoder.infer_tokens(text, self.embedding)
-        else:
-            text = self.encoder.infer(self.embedding(text).transpose(1, 2))
-        text = text.transpose(0, 1)
+        text = self.encoder.infer_tokens(text, self.embedding).transpose(0, 1)
         encoder_outputs = torch.cat([text, speaker_vecs.expand(text.size(0), -1, -1)], 2)
         residual = residual.permute(2, 0, 1)
         attention_weights = []

@@ -70,24 +70,29 @@ def test_product_package_never_imports_oracle():
                 assert not re.search(r"^\s*(from|import)\s+oracle\b", src, flags=re.M), f
 
 
-def test_encoder_matches_oracle_restatement():
-    """The torch Encoder kept on the host side equals the oracle's explicit restatement (eval mode)."""
+def test_encoder_rejects_sizes_the_kernels_are_not_built_for():
+    from flowtron_b200.flowtron import Encoder, MaskedInstanceNorm1d
+    Encoder(norm_fn=MaskedInstanceNorm1d)
+    for kw in (dict(encoder_embedding_dim=256), dict(encoder_n_convolutions=2), dict(encoder_kernel_size=3)):
+        with pytest.raises(NotImplementedError):
+            Encoder(norm_fn=MaskedInstanceNorm1d, **kw)
+    with pytest.raises(NotImplementedError):
+        Encoder(norm_fn=torch.nn.BatchNorm1d)
+
+
+def test_encoder_fails_loudly_on_cpu():
+    from flowtron_b200._lib import FlowtronB200Error
     from flowtron_b200.flowtron import Flowtron
-    from oracle import flowtron_oracle as O
     cfg = dict(synth.DEFAULT_MODEL_CONFIG, n_flows=1)
-    p = synth.synth_params(cfg, 9)
-    m = Flowtron(**cfg)
-    m.load_state_dict(p, strict=True)
-    m.eval()
+    m = Flowtron(**cfg).eval()
     b = synth.synth_batch(3, 8, 11, cfg, 2)
-    with torch.no_grad():
-        x = m.embedding(b["text"]).transpose(1, 2)
-        ours = m.encoder(x, b["in_lens"])
-        ref = O.encoder_forward(p, torch.nn.functional.embedding(b["text"], p["embedding.weight"]).transpose(1, 2), b["in_lens"])
-        assert (ours - ref).abs().max().item() < 1e-5
-        ours_i = m.encoder.infer(x[:1])
-        ref_i = O.encoder_forward(p, x[:1], None, infer=True)
-        assert (ours_i - ref_i).abs().max().item() < 1e-5
+    x = m.embedding(b["text"]).transpose(1, 2)
+    for call in (lambda: m.encoder(x, b["in_lens"]), lambda: m.encoder.infer(x[:1]),
+                 lambda: m.encoder.forward_tokens(b["text"], m.embedding, b["in_lens"]),
+                 lambda: m.encoder.infer_tokens(b["text"], m.embedding),
+                 lambda: m.encoder.infer_ragged_tokens(b["text"], m.embedding, b["in_lens"])):
+        with pytest.raises(FlowtronB200Error):
+            call()
 
 
 def test_default_switches_are_the_validated_configuration():
@@ -95,8 +100,7 @@ def test_default_switches_are_the_validated_configuration():
     pipeline ON (forward and BPTT), CUDA-graph step ON in bench.py.  Anything else is opt-in through the environment
     (DESIGN.md 4.9)."""
     import flowtron_b200.flowtron as F
-    if "FT_ENC_OVERLAP" not in os.environ:                 # class attribute, read at import
-        assert F.Flowtron.overlap_encoder is True
+    assert F.Flowtron.overlap_encoder is True
     src = open(os.path.join(ROOT, "bench.py")).read()
     assert 'os.environ.get("FT_FUSED_OPT", "1")' in src
     csrc = open(os.path.join(ROOT, "flowtron_b200", "csrc", "ar_step.cu")).read()

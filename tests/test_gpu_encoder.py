@@ -30,7 +30,7 @@ def rel(a, b):
     return (a - b).abs().max().item() / max(b.abs().max().item(), 1e-12)
 
 
-@pytest.mark.parametrize("B,L,lens", [(5, 37, [37, 30, 22, 9, 1]), (32, 150, None), (1, 50, [50]), (48, 64, None)])
+@pytest.mark.parametrize("B,L,lens", [(5, 37, [37, 30, 22, 9, 1]), (32, 150, None), (1, 50, [50]), (48, 64, None), (72, 40, None)])
 def test_encoder_forward_matches_oracle(B, L, lens):
     m, p = _model(3)
     m.eval()
@@ -64,7 +64,7 @@ def test_encoder_infer_matches_oracle():
     assert err < 1e-3, err
 
 
-@pytest.mark.parametrize("B,L,lens", [(4, 29, [29, 20, 11, 3]), (1, 33, [33]), (32, 120, None)])
+@pytest.mark.parametrize("B,L,lens", [(4, 29, [29, 20, 11, 3]), (1, 33, [33]), (32, 120, None), (72, 40, None)])
 def test_encoder_backward_matches_fp32_autograd(B, L, lens):
     m, p = _model(6)
     m.train()
@@ -160,3 +160,44 @@ def test_encoder_token_path_equals_embedding_then_encoder():
     used = set(tokens[torch.arange(L, device="cuda")[None, :] < in_lens[:, None]].tolist())
     unused = [t for t in range(m.embedding.num_embeddings) if t not in used]
     assert float(e1[unused].abs().max()) == 0.0
+
+
+def test_encoder_batch_above_64_equals_calls_of_at_most_64():
+    """The kernels take at most 64 utterances per call: B = 72 runs as 64 + 8 rows, and in eval mode every row equals, bit for
+    bit, the same rows run as batches of 64 and 8 (embedded-input and token forms)."""
+    m, _ = _model(10)
+    m.eval()
+    B, L = 72, 40
+    g = torch.Generator().manual_seed(15)
+    x = _x(B, L, 16).cuda()
+    tokens = torch.randint(0, m.embedding.num_embeddings, (B, L), generator=g).cuda()
+    in_lens = torch.randint(1, L + 1, (B,), generator=g)
+    in_lens[0] = L
+    in_lens = in_lens.cuda()
+    with torch.no_grad():
+        full = m.encoder(x, in_lens)
+        parts = torch.cat([m.encoder(x[:64], in_lens[:64]), m.encoder(x[64:], in_lens[64:])])
+        full_t = m.encoder.infer_ragged_tokens(tokens, m.embedding, in_lens)
+        parts_t = torch.cat([m.encoder.infer_ragged_tokens(tokens[:64], m.embedding, in_lens[:64]),
+                             m.encoder.infer_ragged_tokens(tokens[64:], m.embedding, in_lens[64:])])
+    assert full.shape == (B, L, 512) and torch.equal(full, parts)
+    assert torch.equal(full_t, parts_t)
+
+
+def test_flowtron_train_step_above_64_utterances():
+    """Flowtron.forward + backward at B = 72: the encoder (token form) runs as 64 + 8 rows, the flows as 32-row launches."""
+    from flowtron_b200 import _lib
+    from flowtron_b200.flowtron import FlowtronLoss
+    m, _ = _model(11)
+    m.train()
+    m.encoder.p_dropout = 0.0
+    batch = synth.synth_batch(72, 16, 10, synth.DEFAULT_MODEL_CONFIG, 17)
+    cu = {k: (v.cuda() if torch.is_tensor(v) else v) for k, v in batch.items()}
+    out = m(cu["mel"], cu["speaker_ids"], cu["text"], cu["in_lens"], cu["out_lens"])
+    nll, gl, _ = FlowtronLoss()(out, cu["gate_target"], cu["in_lens"], cu["out_lens"])
+    (nll + gl).sum().backward()
+    torch.cuda.synchronize()
+    assert _lib.device_status() == 0
+    assert out[0].shape[1] == 72 and torch.isfinite(out[0]).all()
+    for p in (m.embedding.weight, m.encoder.lstm.weight_ih_l0, m.encoder.convolutions[0][0].conv.weight):
+        assert torch.isfinite(p.grad).all() and p.grad.abs().max() > 0

@@ -45,16 +45,15 @@ def test_forward_loss_backward_match_reference_goldens(tag):
     gold = _load(f"train_{tag}.npz")
     n_flows, B, T, L = (int(gold[k]) for k in ("cfg_n_flows", "B", "T", "L"))
     cfg = dict(synth.DEFAULT_MODEL_CONFIG, n_flows=n_flows)
-    # the torch Encoder (outside the kernel scope) must run in true fp32 for a parity test: cuDNN convs / RNN default
-    # to TF32 on this GPU, which alone puts 4-5 % noise on the embedding / encoder-conv gradients
+    # any torch GEMM or convolution left on the path runs in true fp32 for a parity test
     torch.backends.cudnn.allow_tf32 = False
     torch.backends.cuda.matmul.allow_tf32 = False
     model = build_model(cfg, int(gold["seed"]))
     batch = synth.synth_batch(B, T, L, cfg, int(gold["seed"]), out_lens=OUT_LENS[tag], with_prior=bool(gold["with_prior"]))
     dev = "cuda"
     cu = {k: (v.to(dev) if torch.is_tensor(v) else v) for k, v in batch.items()}
-    model.train()                      # cuDNN's encoder BiLSTM needs train mode for backward ...
-    model.encoder.p_dropout = 0.0      # ... with the (random) encoder dropout disabled, like the golden generator
+    model.train()
+    model.encoder.p_dropout = 0.0      # the (random) encoder dropout disabled, like the golden generator
     for p in model.parameters():
         p.requires_grad_(True)
     out = model(cu["mel"], cu["speaker_ids"], cu["text"], cu["in_lens"], cu["out_lens"], cu["attn_prior"])
