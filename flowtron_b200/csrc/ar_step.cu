@@ -6,7 +6,7 @@
 // Precision plan (DESIGN.md): forward tensor-core operands are fp16 (11-bit significand, same as tf32; every
 // forward operand is either a weight or a bounded activation); backward operands are fp16 too, on gradients
 // multiplied by a per-flow power-of-two loss scale chosen on the device (launch_grad_scale); accumulation, LSTM cell state, softmax, exp/log and all reductions are fp32.
-#include <cstdlib>
+#include <algorithm>
 #include <cstring>
 #include <map>
 #include <mutex>
@@ -93,38 +93,28 @@ struct W16 {
     }
 };
 
-// Layer pipeline (DESIGN.md 4.2; default ON, FT_PIPE_FWD=0 / FT_PIPE_BWD=0 fall back to one launch per layer): lstm layers 0
-// and 1 run as two 64-CTA recurrences one chunk of FT_PIPE_CHUNK steps apart, forward and BPTT.  On a 132-SM H100 the two
-// recurrences leave 4 SMs to the per-chunk GEMMs, which mostly run between recurrence steps; the schedule still wins there
-// (DESIGN.md 4.11: B=32, T=1000, 74 ms/step with both pipelines, 84 without).
-static bool pipe_fwd_enabled() {
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("FT_PIPE_FWD"); v = (!e || atoi(e) != 0) ? 1 : 0; }
-    return v == 1;
-}
-static bool pipe_bwd_enabled() {
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("FT_PIPE_BWD"); v = (!e || atoi(e) != 0) ? 1 : 0; }
-    return v == 1;
-}
-static int pipe_chunk_steps() {
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("FT_PIPE_CHUNK"); v = e ? atoi(e) : 100; if (v < 8) v = 8; }
-    return v;
-}
+// Layer pipeline (DESIGN.md 4.2): lstm layers 0 and 1 run as two 64-CTA recurrences one chunk of kLayerChunk steps apart,
+// forward and BPTT; a sequence of at most kLayerChunk steps is a single chunk.  On a 132-SM H100 the two recurrences leave
+// 4 SMs to the per-chunk GEMMs, which mostly run between recurrence steps; the schedule still wins there (DESIGN.md 4.11:
+// B=32, T=1000, 74 ms/step with both pipelines, 84 without).
+constexpr int kLayerChunk = 100;
+// Attention-LSTM overlap chunk in steps (a multiple of 64): the overlap runs when T >= kAttnChunk + 64.
+constexpr int kAttnChunk = 256;
+
+static int layer_chunk(int T) { return T < kLayerChunk ? T : kLayerChunk; }
 
 struct FwdScratch {
     W16 w;
     float* X;
     int* flags;
-    float* X1 = nullptr;        // second input-projection buffer (pipelined layers only)
+    float* X1;                  // second input-projection buffer: the attention LSTM's (overlap), then layer 1's (pipeline)
     float *hA32 = nullptr, *ctx32 = nullptr;     // fp32 copies of [hA ; ctx] for the gate logits (gated flow only)
     void plan(Plan& p, const FtArStepDesc& d) {
         const Dims n(d);
         w.plan(p, n);
         X = p.get<float>("X", n.R * G);
         flags = p.get<int>("flags", static_cast<size_t>(n.T) * 64);
-        if (pipe_fwd_enabled()) X1 = p.get<float>("X1", n.R * G);
+        X1 = p.get<float>("X1", n.R * G);
         if (d.has_gate) {
             hA32 = p.get<float>("hA32", n.R * H);
             ctx32 = p.get<float>("ctx32", n.R * n.A);
@@ -150,7 +140,7 @@ struct BwdScratch {
     uint16_t *dG1, *dG0, *dGa, *do16, *dy2, *dy1, *dQ16, *dK16, *dV16;
     float *dh, *dQ, *dK, *dV, *dmel_in;
     int* flags;
-    float *dcarry1 = nullptr, *dcarry0 = nullptr;      // dc*f hand-over between BPTT chunks (pipelined layers only)
+    float *dcarry1, *dcarry0;   // dc*f hand-over between BPTT chunks of the layer pipeline
     void plan(Plan& p, const FtArStepDesc& d) {
         const Dims n(d);
         w.plan(p, n);
@@ -168,11 +158,10 @@ struct BwdScratch {
         dK = p.get<float>("dK", n.RL * n.A);
         dV = p.get<float>("dV", n.RL * n.A);
         dmel_in = p.get<float>("dmel_in", n.R * n.M);
-        flags = p.get<int>("flags", static_cast<size_t>(n.T) * 64);
-        if (pipe_bwd_enabled()) {
-            dcarry1 = p.get<float>("dcarry1", static_cast<size_t>(n.B) * H);
-            dcarry0 = p.get<float>("dcarry0", static_cast<size_t>(n.B) * H);
-        }
+        // 64 per step: T steps for the attention LSTM's BPTT, one chunk for each of the layer pipeline's two recurrences
+        flags = p.get<int>("flags", static_cast<size_t>(std::max(n.T, 2 * layer_chunk(n.T))) * 64);
+        dcarry1 = p.get<float>("dcarry1", static_cast<size_t>(n.B) * H);
+        dcarry0 = p.get<float>("dcarry0", static_cast<size_t>(n.B) * H);
     }
 };
 
@@ -328,17 +317,15 @@ int ar_step_fwd(const FtArStepDesc& d, const FtArStepWeights& w, const float* me
     FT_TRY(launch_prep_mel(mel, out_lens, n.T, n.B, n.M, d.reversed, S.mel_in16, S.mel_flow, st));
     const float* mel_flow = d.reversed ? S.mel_flow : mel;
 
-    // Attention-LSTM / attention overlap (FT_ATT_OVERLAP = chunk length in steps, a multiple of 64; default 256, 0 disables;
-    // T >= chunk + 64): the attention LSTM runs as a 64-CTA recurrence in chunks; as soon as a chunk's h is there, a second stream
-    // runs that chunk's query projection, fused attention, gate logits and lstm layer 0's input projection on the SMs the 64-CTA
-    // recurrence leaves free,
-    // underneath the next chunk's recurrence.  Only the last chunk's share of that work stays exposed.  The 64-CTA kernel has no room for the folded 80-channel projection next to its 128 KB weight
-    // slice, so the projection is a per-chunk GEMM on a third stream, one chunk ahead.  Short chunks lose: every chunk
-    // boundary costs a kernel drain + launch + 128 KB weight reload on 64 SMs.
-    static int att_chunk = -1;
-    if (att_chunk < 0) { const char* e = getenv("FT_ATT_OVERLAP"); att_chunk = e ? atoi(e) : 256; if (att_chunk % 64) att_chunk = 0; }
-    Pipe* pa = (att_chunk > 0 && F.X1 && n.T >= att_chunk + 64) ? get_pipe(st) : nullptr;
-    bool xproj0_done = false;
+    Pipe* pp = get_pipe(st);
+    if (!pp) return ft_set_error("ar_step_fwd: could not create the pipeline streams");
+
+    // Attention-LSTM / attention overlap (T >= kAttnChunk + 64): the attention LSTM runs as a 64-CTA recurrence in chunks of
+    // kAttnChunk steps; as soon as a chunk's h is there, a second stream runs that chunk's query projection, fused attention,
+    // gate logits and lstm layer 0's input projection on the SMs the 64-CTA recurrence leaves free, underneath the next
+    // chunk's recurrence.  Only the last chunk's share of that work stays exposed.  The 64-CTA kernel has no room for the
+    // folded 80-channel projection next to its 128 KB weight slice, so the projection is a per-chunk GEMM on a third stream,
+    // one chunk ahead.  Short chunks lose: every chunk boundary costs a kernel drain + launch + 128 KB weight reload on 64 SMs.
     auto attention_rows = [&](cudaStream_t s2, int t0, int t1) -> int {      // Q projection, attention, gate logits of steps [t0, t1)
         const long long r0 = static_cast<long long>(t0) * n.B, rows = static_cast<long long>(t1 - t0) * n.B;
         FT_TRY(gemm_fwd(s2, rows, n.A, H, S.d16 + r0 * n.D, n.D, F.w.wq, H, nullptr, nullptr, 0, S.Q + r0 * n.A, n.A, nullptr, 0));
@@ -364,85 +351,75 @@ int ar_step_fwd(const FtArStepDesc& d, const FtArStepWeights& w, const float* me
         FT_TRY(gemm_fwd(s2, n.RL, n.A, n.E, S.text16, n.E, F.w.wv, n.E, nullptr, nullptr, 0, S.Vp, n.A, nullptr, 0));
         return 0;
     };
-    if (pa) {
-        const int CH = att_chunk;
+    if (n.T >= kAttnChunk + 64) {
+        const int CH = kAttnChunk;
         auto xa = [&](cudaStream_t s2, int t0, int t1) {              // attention-LSTM input projection of steps [t0, t1) -> F.X1 rows
             const long long r0 = static_cast<long long>(t0) * n.B, rows = static_cast<long long>(t1 - t0) * n.B;
             return gemm_fwd(s2, rows, G, n.M, S.mel_in16 + r0 * n.M, n.M, F.w.w_ih_a, n.M, w.attn_lstm_b_ih, w.attn_lstm_b_hh, 0,
                             F.X1 + r0 * G, G, nullptr, 0);
         };
-        cudaStream_t sr = pa->sA;                                    // the attention LSTM's stream
-        cudaEventRecord(pa->ev0, st);
-        cudaStreamWaitEvent(sr, pa->ev0, 0);
-        cudaStreamWaitEvent(pa->sB, pa->ev0, 0);
-        cudaStreamWaitEvent(pa->sC, pa->ev0, 0);
-        FT_TRY(kv_projections(pa->sC));
-        FT_TRY(xa(sr, 0, CH < n.T ? CH : n.T));
-        for (int t0 = 0; t0 < n.T; t0 += CH) {
-            const int t1 = t0 + CH < n.T ? t0 + CH : n.T;
-            if (t1 < n.T) {                                            // next chunk's projection, one chunk ahead, on sB
-                FT_TRY(xa(pa->sB, t1, t1 + CH < n.T ? t1 + CH : n.T));
-                cudaEventRecord(pa->evB, pa->sB);
-            }
-            FT_TRY(launch_lstm_fwd_chunk(n.T, n.B, t0, t1, F.X1, F.w.w_hh_a, out_lens, S.d16, n.D, S.gatesA, S.cA, F.flags, sr, F.hA32, H));
-            cudaEventRecord(pa->evA, sr);
-            if (t1 < n.T) cudaStreamWaitEvent(sr, pa->evB, 0);        // the next launch on sr needs its projection
-            cudaStreamWaitEvent(pa->sC, pa->evA, 0);
-            FT_TRY(attention_rows(pa->sC, t0, t1));
-            const long long r0 = static_cast<long long>(t0) * n.B, rows = static_cast<long long>(t1 - t0) * n.B;
-            FT_TRY(gemm_fwd(pa->sC, rows, G, n.D, S.d16 + r0 * n.D, n.D, F.w.w_ih0, n.D, w.lstm_b_ih0, w.lstm_b_hh0, 0, F.X + r0 * G, G, nullptr, 0));
-        }
-        cudaEventRecord(pa->evG, pa->sC);
-        cudaStreamWaitEvent(st, pa->evG, 0);
-        cudaEventRecord(pa->evJ, sr);
-        cudaStreamWaitEvent(st, pa->evJ, 0);
-        xproj0_done = true;
-    } else {
-    // attention_lstm: the 80-channel input projection is folded into the persistent recurrence (no [R,4096] projection
-    // tensor: one GEMM and 1 GB of HBM traffic less per flow); h lands in d16[:, 0:H].
-    FT_TRY(launch_lstm_fwd_xin(n.T, n.B, S.mel_in16, n.M, n.M, F.w.w_ih_a, w.attn_lstm_b_ih, w.attn_lstm_b_hh, F.w.w_hh_a, out_lens,
-                               S.d16, n.D, S.gatesA, S.cA, F.hA32, H, F.flags, st));
-    // attention: K/V/Q projections, fused score+softmax(+prior)+context; ctx lands in d16[:, H:H+A]
-    FT_TRY(kv_projections(st));
-    FT_TRY(attention_rows(st, 0, n.T));
-    }
-
-    // 2-layer lstm
-    Pipe* pp = (F.X1 && n.T > pipe_chunk_steps()) ? get_pipe(st) : nullptr;
-    if (pp) {
-        // EXPERIMENTAL: layer 1 at step t needs layer 0 only up to t, so the two recurrences run as two 64-CTA kernels
-        // one chunk apart: st = layer 0, sC = layer-1 input projection of a finished chunk, sB = layer 1.
-        const int S_ = pipe_chunk_steps();
-        int* flagsA = F.flags;
-        int* flagsB = F.flags + static_cast<size_t>(S_) * 16;
-        if (!xproj0_done) FT_TRY(gemm_fwd(st, n.R, G, n.D, S.d16, n.D, F.w.w_ih0, n.D, w.lstm_b_ih0, w.lstm_b_hh0, 0, F.X, G, nullptr, 0));
-        cudaStream_t sr = pp->sA;                                    // layer 0's recurrence stream
+        cudaStream_t sr = pp->sA;                                    // the attention LSTM's stream
         cudaEventRecord(pp->ev0, st);
         cudaStreamWaitEvent(sr, pp->ev0, 0);
         cudaStreamWaitEvent(pp->sB, pp->ev0, 0);
         cudaStreamWaitEvent(pp->sC, pp->ev0, 0);
-        for (int t0 = 0; t0 < n.T; t0 += S_) {
-            const int t1 = t0 + S_ < n.T ? t0 + S_ : n.T;
-            const long long r0 = static_cast<long long>(t0) * n.B, rows = static_cast<long long>(t1 - t0) * n.B;
-            FT_TRY(launch_lstm_fwd_chunk(n.T, n.B, t0, t1, F.X, F.w.w_hh0, out_lens, S.h0_16, H, S.gates0, S.c0, flagsA, sr));
+        FT_TRY(kv_projections(pp->sC));
+        FT_TRY(xa(sr, 0, CH < n.T ? CH : n.T));
+        for (int t0 = 0; t0 < n.T; t0 += CH) {
+            const int t1 = t0 + CH < n.T ? t0 + CH : n.T;
+            if (t1 < n.T) {                                            // next chunk's projection, one chunk ahead, on sB
+                FT_TRY(xa(pp->sB, t1, t1 + CH < n.T ? t1 + CH : n.T));
+                cudaEventRecord(pp->evB, pp->sB);
+            }
+            FT_TRY(launch_lstm_fwd_chunk(n.T, n.B, t0, t1, F.X1, F.w.w_hh_a, out_lens, S.d16, n.D, S.gatesA, S.cA, F.flags, sr, F.hA32, H));
             cudaEventRecord(pp->evA, sr);
+            if (t1 < n.T) cudaStreamWaitEvent(sr, pp->evB, 0);        // the next launch on sr needs its projection
             cudaStreamWaitEvent(pp->sC, pp->evA, 0);
-            FT_TRY(gemm_fwd(pp->sC, rows, G, H, S.h0_16 + r0 * H, H, F.w.w_ih1, H, w.lstm_b_ih1, w.lstm_b_hh1, 0,
-                            F.X1 + r0 * G, G, nullptr, 0));
-            cudaEventRecord(pp->evG, pp->sC);
-            cudaStreamWaitEvent(pp->sB, pp->evG, 0);
-            FT_TRY(launch_lstm_fwd_chunk(n.T, n.B, t0, t1, F.X1, F.w.w_hh1, out_lens, S.h1_16, H, S.gates1, S.c1, flagsB, pp->sB));
+            FT_TRY(attention_rows(pp->sC, t0, t1));
+            const long long r0 = static_cast<long long>(t0) * n.B, rows = static_cast<long long>(t1 - t0) * n.B;
+            FT_TRY(gemm_fwd(pp->sC, rows, G, n.D, S.d16 + r0 * n.D, n.D, F.w.w_ih0, n.D, w.lstm_b_ih0, w.lstm_b_hh0, 0, F.X + r0 * G, G, nullptr, 0));
         }
-        cudaEventRecord(pp->evB, pp->sB);
-        cudaStreamWaitEvent(st, pp->evB, 0);
+        cudaEventRecord(pp->evG, pp->sC);
+        cudaStreamWaitEvent(st, pp->evG, 0);
         cudaEventRecord(pp->evJ, sr);
         cudaStreamWaitEvent(st, pp->evJ, 0);
     } else {
-        if (!xproj0_done) FT_TRY(gemm_fwd(st, n.R, G, n.D, S.d16, n.D, F.w.w_ih0, n.D, w.lstm_b_ih0, w.lstm_b_hh0, 0, F.X, G, nullptr, 0));
-        FT_TRY(launch_lstm_fwd(n.T, n.B, F.X, F.w.w_hh0, out_lens, S.h0_16, H, S.gates0, S.c0, nullptr, 0, F.flags, st));
-        FT_TRY(gemm_fwd(st, n.R, G, H, S.h0_16, H, F.w.w_ih1, H, w.lstm_b_ih1, w.lstm_b_hh1, 0, F.X, G, nullptr, 0));
-        FT_TRY(launch_lstm_fwd(n.T, n.B, F.X, F.w.w_hh1, out_lens, S.h1_16, H, S.gates1, S.c1, nullptr, 0, F.flags, st));
+        // attention_lstm: the 80-channel input projection is folded into the persistent recurrence (no [R,4096] projection
+        // tensor: one GEMM and 1 GB of HBM traffic less per flow); h lands in d16[:, 0:H].
+        FT_TRY(launch_lstm_fwd_xin(n.T, n.B, S.mel_in16, n.M, n.M, F.w.w_ih_a, w.attn_lstm_b_ih, w.attn_lstm_b_hh, F.w.w_hh_a, out_lens,
+                                   S.d16, n.D, S.gatesA, S.cA, F.hA32, H, F.flags, st));
+        // attention: K/V/Q projections, fused score+softmax(+prior)+context; ctx lands in d16[:, H:H+A]
+        FT_TRY(kv_projections(st));
+        FT_TRY(attention_rows(st, 0, n.T));
+        FT_TRY(gemm_fwd(st, n.R, G, n.D, S.d16, n.D, F.w.w_ih0, n.D, w.lstm_b_ih0, w.lstm_b_hh0, 0, F.X, G, nullptr, 0));
     }
+
+    // 2-layer lstm: layer 1 at step t needs layer 0 only up to t, so the two recurrences run as two 64-CTA kernels one chunk
+    // apart: sA = layer 0, sC = layer-1 input projection of a finished chunk, sB = layer 1.
+    const int CH = layer_chunk(n.T);
+    int* flagsA = F.flags;
+    int* flagsB = F.flags + static_cast<size_t>(CH) * 16;
+    cudaStream_t sr = pp->sA;                                    // layer 0's recurrence stream
+    cudaEventRecord(pp->ev0, st);
+    cudaStreamWaitEvent(sr, pp->ev0, 0);
+    cudaStreamWaitEvent(pp->sB, pp->ev0, 0);
+    cudaStreamWaitEvent(pp->sC, pp->ev0, 0);
+    for (int t0 = 0; t0 < n.T; t0 += CH) {
+        const int t1 = t0 + CH < n.T ? t0 + CH : n.T;
+        const long long r0 = static_cast<long long>(t0) * n.B, rows = static_cast<long long>(t1 - t0) * n.B;
+        FT_TRY(launch_lstm_fwd_chunk(n.T, n.B, t0, t1, F.X, F.w.w_hh0, out_lens, S.h0_16, H, S.gates0, S.c0, flagsA, sr));
+        cudaEventRecord(pp->evA, sr);
+        cudaStreamWaitEvent(pp->sC, pp->evA, 0);
+        FT_TRY(gemm_fwd(pp->sC, rows, G, H, S.h0_16 + r0 * H, H, F.w.w_ih1, H, w.lstm_b_ih1, w.lstm_b_hh1, 0,
+                        F.X1 + r0 * G, G, nullptr, 0));
+        cudaEventRecord(pp->evG, pp->sC);
+        cudaStreamWaitEvent(pp->sB, pp->evG, 0);
+        FT_TRY(launch_lstm_fwd_chunk(n.T, n.B, t0, t1, F.X1, F.w.w_hh1, out_lens, S.h1_16, H, S.gates1, S.c1, flagsB, pp->sB));
+    }
+    cudaEventRecord(pp->evB, pp->sB);
+    cudaStreamWaitEvent(st, pp->evB, 0);
+    cudaEventRecord(pp->evJ, sr);
+    cudaStreamWaitEvent(st, pp->evJ, 0);
 
     // dense x2 (tanh fused in the GEMM epilogue), 1x1 conv, affine coupling
     FT_TRY(gemm_fwd(st, n.R, H, H, S.h1_16, H, F.w.w1, H, w.dense_b0, nullptr, 1, nullptr, 0, S.y1_16, H));
@@ -521,54 +498,41 @@ int ar_step_bwd_main(const FtArStepDesc& d, const FtArStepWeights& w, const floa
         FT_TRY(zero(g.gate_w, sizeof(float) * n.D, st));
         FT_TRY(zero(g.gate_b, sizeof(float), st));
     }
-    Pipe* pp = (F.dcarry1 && 2 * pipe_chunk_steps() <= n.T) ? get_pipe(st) : nullptr;
-    if (pp) {
-        // EXPERIMENTAL 5+6: BPTT of layer 1 (st) and layer 0 (sB) one chunk apart; the layer-1 dgrad of a finished chunk
-        // (sC) turns dG1 rows into layer 0's incoming dh rows (F.dh is reused row-disjointly: layer 1 only reads rows
-        // below the chunk it has finished).  Highest chunk first.
-        const int S_c = pipe_chunk_steps();
-        int* flagsA = F.flags;
-        int* flagsB = F.flags + static_cast<size_t>(S_c) * 64;
-        cudaStream_t sr = pp->sA;                                    // layer 1's BPTT stream
-        cudaEventRecord(pp->ev0, st);
-        cudaStreamWaitEvent(sr, pp->ev0, 0);
-        cudaStreamWaitEvent(pp->sB, pp->ev0, 0);
-        cudaStreamWaitEvent(pp->sC, pp->ev0, 0);
-        const int n_chunks = (n.T + S_c - 1) / S_c;
-        for (int c = n_chunks - 1; c >= 0; --c) {
-            const int t0 = c * S_c, t1 = t0 + S_c < n.T ? t0 + S_c : n.T;
-            const long long r0 = static_cast<long long>(t0) * n.B, rows = static_cast<long long>(t1 - t0) * n.B;
-            FT_TRY(launch_lstm_bwd_chunk(n.T, n.B, t0, t1, F.dh, H, F.w.w_hh1, S_.gates1, S_.c1, out_lens, F.dG1, F.dcarry1, flagsA, sr));
-            cudaEventRecord(pp->evA, sr);
-            cudaStreamWaitEvent(pp->sC, pp->evA, 0);
-            FT_TRY(gemm_dgrad(pp->sC, rows, H, G, F.dG1 + r0 * G, G, F.w.w_ih1, H, 0, F.dh + r0 * H, H, nullptr, 0, nullptr, 0));
-            cudaEventRecord(pp->evG, pp->sC);
-            cudaStreamWaitEvent(pp->sB, pp->evG, 0);
-            FT_TRY(launch_lstm_bwd_chunk(n.T, n.B, t0, t1, F.dh, H, F.w.w_hh0, S_.gates0, S_.c0, out_lens, F.dG0, F.dcarry0, flagsB, pp->sB));
-        }
-        // layer-1 weight gradients run under the tail of layer 0 (side stream forks from st = all of layer 1 done)
-        cudaEventRecord(pp->evJ, sr);
-        cudaStreamWaitEvent(st, pp->evJ, 0);
-        ss = fork_side(sd, st);
-        FT_TRY(gemm_wgrad(ss, G, H, Rm, F.dG1 + static_cast<size_t>(n.B) * G, G, S_.h1_16, H, g.lstm_w_hh1, H, iS));
-        FT_TRY(gemm_wgrad(ss, G, H, R, F.dG1, G, S_.h0_16, H, g.lstm_w_ih1, H, iS));
-        FT_TRY(launch_colsum(F.dG1, 0, G, R, G, g.lstm_b_ih1, iS, ss));
-        FT_TRY(copy_f32(g.lstm_b_hh1, g.lstm_b_ih1, G, ss));
-        cudaEventRecord(pp->evB, pp->sB);
-        cudaStreamWaitEvent(st, pp->evB, 0);
-    } else {
-    // 5. lstm layer 1
-    FT_TRY(launch_lstm_bwd(n.T, n.B, F.dh, H, F.w.w_hh1, S_.gates1, S_.c1, out_lens, F.dG1, F.flags, st));
+    // 5 + 6. lstm layers 1 and 0: BPTT of layer 1 (sA) and layer 0 (sB) one chunk apart; the layer-1 dgrad of a finished chunk
+    // (sC) turns dG1 rows into layer 0's incoming dh rows (F.dh is reused row-disjointly: layer 1 only reads rows below the
+    // chunk it has finished).  Highest chunk first.
+    Pipe* pp = get_pipe(st);
+    if (!pp) return ft_set_error("ar_step_bwd: could not create the pipeline streams");
+    const int CH = layer_chunk(n.T);
+    int* flagsA = F.flags;
+    int* flagsB = F.flags + static_cast<size_t>(CH) * 64;
+    cudaStream_t sr = pp->sA;                                    // layer 1's BPTT stream
+    cudaEventRecord(pp->ev0, st);
+    cudaStreamWaitEvent(sr, pp->ev0, 0);
+    cudaStreamWaitEvent(pp->sB, pp->ev0, 0);
+    cudaStreamWaitEvent(pp->sC, pp->ev0, 0);
+    const int n_chunks = (n.T + CH - 1) / CH;
+    for (int c = n_chunks - 1; c >= 0; --c) {
+        const int t0 = c * CH, t1 = t0 + CH < n.T ? t0 + CH : n.T;
+        const long long r0 = static_cast<long long>(t0) * n.B, rows = static_cast<long long>(t1 - t0) * n.B;
+        FT_TRY(launch_lstm_bwd_chunk(n.T, n.B, t0, t1, F.dh, H, F.w.w_hh1, S_.gates1, S_.c1, out_lens, F.dG1, F.dcarry1, flagsA, sr));
+        cudaEventRecord(pp->evA, sr);
+        cudaStreamWaitEvent(pp->sC, pp->evA, 0);
+        FT_TRY(gemm_dgrad(pp->sC, rows, H, G, F.dG1 + r0 * G, G, F.w.w_ih1, H, 0, F.dh + r0 * H, H, nullptr, 0, nullptr, 0));
+        cudaEventRecord(pp->evG, pp->sC);
+        cudaStreamWaitEvent(pp->sB, pp->evG, 0);
+        FT_TRY(launch_lstm_bwd_chunk(n.T, n.B, t0, t1, F.dh, H, F.w.w_hh0, S_.gates0, S_.c0, out_lens, F.dG0, F.dcarry0, flagsB, pp->sB));
+    }
+    // layer-1 weight gradients run under the tail of layer 0 (side stream forks from st = all of layer 1 done)
+    cudaEventRecord(pp->evJ, sr);
+    cudaStreamWaitEvent(st, pp->evJ, 0);
     ss = fork_side(sd, st);
     FT_TRY(gemm_wgrad(ss, G, H, Rm, F.dG1 + static_cast<size_t>(n.B) * G, G, S_.h1_16, H, g.lstm_w_hh1, H, iS));
     FT_TRY(gemm_wgrad(ss, G, H, R, F.dG1, G, S_.h0_16, H, g.lstm_w_ih1, H, iS));
     FT_TRY(launch_colsum(F.dG1, 0, G, R, G, g.lstm_b_ih1, iS, ss));
     FT_TRY(copy_f32(g.lstm_b_hh1, g.lstm_b_ih1, G, ss));
-    FT_TRY(gemm_dgrad(st, R, H, G, F.dG1, G, F.w.w_ih1, H, 0, F.dh, H, nullptr, 0, nullptr, 0));
-
-    // 6. lstm layer 0
-    FT_TRY(launch_lstm_bwd(n.T, n.B, F.dh, H, F.w.w_hh0, S_.gates0, S_.c0, out_lens, F.dG0, F.flags, st));
-    }
+    cudaEventRecord(pp->evB, pp->sB);
+    cudaStreamWaitEvent(st, pp->evB, 0);
     // (the weight gradients of lstm layer 0 and of the attention projections are launched by ar_step_bwd_attn, on the side
     //  stream underneath the attention LSTM's BPTT: dG0, dQ16, dK16, dV16 stay in the scratch area until then)
     // 6b. lstm layer 0's input gradient: dd = [dhA ; dctx]

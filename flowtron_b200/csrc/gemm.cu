@@ -1,6 +1,4 @@
 // Host side of the GEMM (kernel: gemm_kernel.cuh): TMA descriptors, tile / split-K / cluster policy, launch.
-#include <cstdlib>
-
 #include "gemm_kernel.cuh"
 
 namespace ft {
@@ -40,7 +38,7 @@ int make_tmap_2d(CUtensorMap* out, const void* ptr, int fmt, long long rows, lon
     return 0;
 }
 
-static int g_pair_mode = -1;        // 0 never, 1 big contractions only, 2 whenever eligible
+static int g_pair_mode = 1;         // 0 never, 1 big contractions only, 2 whenever eligible
 void set_gemm_pair_mode(int mode) { g_pair_mode = mode; }
 
 extern template const void* gemm_kernel_ptr<FMT_F16, 0>(int, int, int);
@@ -87,8 +85,7 @@ int launch_gemm(const GemmArgs& g, cudaStream_t st) {
     }
     p.splitk = splitk;
     // 2-CTA clusters (B multicast) for wide outputs with enough 256 x 256 tiles to fill the machine.  Mode 1 (default;
-    // FT_GEMM_2CTA / ft_set_gemm_pair_mode override): only for the big contractions (>= 1e11 FLOP).  Mode 2: whenever eligible.
-    if (g_pair_mode < 0) { const char* e = getenv("FT_GEMM_2CTA"); g_pair_mode = e ? atoi(e) : 1; }
+    // ft_set_gemm_pair_mode overrides): only for the big contractions (>= 1e11 FLOP).  Mode 2: whenever eligible.
     const long long tiles_m2 = (g.M + 2 * BM - 1) / (2 * BM);
     const bool big = 2.0 * g.M * g.N * g.K >= 1e11;
     const int ncta = ((g_pair_mode == 2 || (g_pair_mode == 1 && big)) && wide && splitk == 1 && tiles_m2 * tiles_n >= sms / 2) ? 2 : 1;

@@ -5,13 +5,14 @@
 // t >= len (pack_padded/pad_packed).  The input projection W_ih x + b_ih + b_hh is a plain GEMM done
 // beforehand (gemm.cu); these kernels run the T-step dependency chain without returning to the host.
 //
-// Forward (lstm_fwd_kernel), one cooperative launch, 128 CTAs:
-//   * CTA c owns hidden units [8c, 8c+8): its 32 rows of W_hh (4 gates x 8 units, fp16, 64 KB) are
-//     TMA-loaded once and stay resident in shared memory as the wgmma A operand (M = 64, 32 real rows).
+// Forward (lstm_fwd_kernel), one cooperative launch of 64 CTAs (U = 16 hidden units each), or of 128 CTAs (U = 8) for
+// the attention LSTM with its input projection folded in:
+//   * CTA c owns hidden units [Uc, Uc+U): its 4U rows of W_hh (4 gates x U units, fp16, 128 / 64 KB) are
+//     TMA-loaded once and stay resident in shared memory as the wgmma A operand (M = 64, 4U real rows).
 //   * every step: h_{t-1} ([B,1024] fp16, read straight out of the layer's output tensor) arrives through
 //     TWO 3-D TMA loads (8 K-chunks each, box {64 elems, B rows, 8 chunks}: the smem image is chunk-major
 //     SWIZZLE_128B K-major tiles, the wgmma B operand with N = B rounded up to 16 / 32); the CTA's one
-//     warpgroup accumulates the 32 gate pre-activations in registers, hands them through shared memory to
+//     warpgroup accumulates the 4U gate pre-activations in registers, hands them through shared memory to
 //     the thread that owns each (batch row, unit pair), adds the input projection, applies the cell in fp32
 //     (cell state lives in registers for the whole sequence), store h_t (fp16) and publish ONE release per
 //     CTA into a per-(step, chunk) counter; consumers poll the 16 counters in parallel (one lane each),
@@ -70,7 +71,7 @@ __device__ __forceinline__ void mma_chunks(float* acc, uint64_t da, uint64_t db,
 constexpr int FWD_NCH = LH / KCH;                  // 16 chunks / step
 constexpr int FWD_GS = 8;                          // K chunks per TMA group: 2 groups per step
 // FWD_UNITS hidden units per CTA: 8 -> 128 CTAs (whole GPU, lowest latency), 16 -> 64 CTAs (two such launches on two
-// streams -- one per half batch -- run concurrently and hide each other's exchange latency)
+// streams -- the layer pipeline's two layers, or two half batches -- run concurrently and hide each other's exchange latency)
 
 struct LstmFwdParams {
     int T, B, Bbox;
@@ -605,7 +606,7 @@ static int make_tmap_chunks(CUtensorMap* out, const void* ptr, long long rows, i
     return 0;
 }
 
-static bool g_half_sm = false;       // 64-CTA forward kernel (for two concurrent half-batch launches)
+static bool g_half_sm = false;       // 64-CTA folded-projection forward (for two concurrent half-batch launches)
 void set_lstm_half_sm(int on) { g_half_sm = on != 0; }
 
 // Steps [t0, t1) of one layer's forward recurrence on 1024 / UNITS CTAs.  `flags` needs (t1 - t0) * 16 ints.
@@ -646,12 +647,12 @@ static int launch_fwd_t(int T, int B, int t0, int t1, const float* xproj, const 
     return ft_check_launch("lstm_fwd_kernel");
 }
 
+// Whole sequence on 64 CTAs: the kernel of launch_lstm_fwd_chunk over [0, T).
 int launch_lstm_fwd(int T, int B, const float* xproj, const void* whh16, const int* lens, void* hseq16, long long ldh,
                     void* gates16, float* cstate, float* h32, long long ldh32, int* flags, cudaStream_t st) {
     if (T <= 0 || B <= 0) return 0;
     if (B > 32) return ft_set_error("lstm_fwd: batch > 32 per call not supported (split the batch)");
-    if (g_half_sm) return launch_fwd_t<16, false>(T, B, 0, T, xproj, whh16, lens, hseq16, ldh, gates16, cstate, h32, ldh32, flags, st);
-    return launch_fwd_t<8, false>(T, B, 0, T, xproj, whh16, lens, hseq16, ldh, gates16, cstate, h32, ldh32, flags, st);
+    return launch_fwd_t<16, false>(T, B, 0, T, xproj, whh16, lens, hseq16, ldh, gates16, cstate, h32, ldh32, flags, st);
 }
 
 // Whole sequence with the input projection folded in (narrow inputs, kx <= 128; x16 row 0..B-1 must be zero: step 0 skips the

@@ -45,7 +45,8 @@ int ft_gemm(int M, int N, int K, const void* A, long long lda, int a_fmt, int a_
  * run_padded_sequence :671-695).  xproj = W_ih x + b_ih + b_hh for all T*B rows (row = t*B + b), fp32
  * [T*B, 4096], gate order i,f,g,o.  whh16: fp16 copy of weight_hh [4096,1024].  Writes h (fp16, zero at
  * t >= lens[b]) to hseq16 [T*B, ldh] and, when non-null, the post-activation gates (fp16 [T*B,4096]) and
- * cell state (fp32 [T*B,1024]) needed by ft_lstm_bwd.  flags: int scratch [T*16].  B <= 32. */
+ * cell state (fp32 [T*B,1024]) needed by ft_lstm_bwd.  flags: int scratch [T*16].  B <= 32.  Runs the 64-CTA
+ * recurrence kernel (16 hidden units per CTA). */
 int ft_lstm_fwd(int T, int B, const float* xproj, const void* whh16, const int* lens, void* hseq16, long long ldh,
                 void* gates16, float* cstate, float* h32, long long ldh32, int* flags, void* stream);
 
@@ -54,8 +55,9 @@ void ft_debug_set_lstm_trace(long long* buf);
 /* same for ft_ar_step_infer: [T][32] stamps of CTA 0 (phase boundaries, tools/trace_infer.py) */
 void ft_debug_set_infer_trace(long long* buf);
 
-/* Process-wide switch: 1 = ft_lstm_fwd (and ft_ar_step_fwd) use the 64-CTA recurrence kernel so two half-batch
- * launches on two streams run concurrently (the BPTT kernel always uses 64 CTAs). */
+/* Process-wide switch: 1 = ft_ar_step_fwd runs the attention LSTM's folded-projection recurrence (T < 320) on 64 CTAs
+ * instead of 128, so two half-batch launches on two streams run concurrently (every other recurrence kernel, forward
+ * and BPTT, always uses 64 CTAs). */
 void ft_set_lstm_half_sm(int on);
 /* ft_gemm tile policy: 0 = one CTA per 128 x 256 tile always; 1 (default) = CTA pairs (2-CTA clusters sharing B by TMA multicast, 256 x 256 tiles) for
  * contractions >= 1e11 FLOP; 2 = CTA pairs whenever the output is wide and has >= SMs/2 such tiles. */

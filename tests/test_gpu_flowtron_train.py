@@ -90,12 +90,18 @@ def test_forward_loss_backward_match_reference_goldens(tag):
                               batch["attn_prior"], fast=True)
     onll, ogl = O.flowtron_loss(oout, batch["gate_target"], batch["in_lens"], batch["out_lens"])
     (onll + ogl).sum().backward()
-    gmax = max(float(gold[f"gnorm::{n}"]) for n, _ in model.named_parameters())
+    _assert_grads_match(f"train_{tag}", model, op, {n: float(gold[f"gnorm::{n}"]) for n, _ in model.named_parameters()})
+
+
+def _assert_grads_match(tag, model, op, gnorm):
+    """Every parameter gradient of `model` against the CPU oracle's (op[name].grad): norm within 1e-2 of gnorm[name],
+    relative L2 <= 4e-2 and cosine >= 0.999."""
+    gmax = max(gnorm.values())
     rows, bad = [], {}
     for name, p in model.named_parameters():
         g = p.grad.detach().reshape(-1).double().cpu()
         r = op[name].grad.reshape(-1).double()
-        gn = float(gold[f"gnorm::{name}"])
+        gn = gnorm[name]
         e_norm = abs(float(g.norm()) - gn) / (gn + 1e-4 * gmax)
         rel_l2 = float((g - r).norm()) / (float(r.norm()) + 1e-4 * gmax)
         cos = float((g @ r) / (g.norm() * r.norm() + 1e-30)) if gn > 1e-4 * gmax else 1.0
@@ -103,10 +109,51 @@ def test_forward_loss_backward_match_reference_goldens(tag):
         if not (e_norm <= 1e-2 and rel_l2 <= 4e-2 and cos >= 0.999):   # tightened once the fp16-scaled backward landed
             bad[name] = (e_norm, rel_l2, cos)
     rows.sort(key=lambda x: -x[2])
-    record_parity(f"train_{tag}_grads", {"norm_err_worst": max(r[1] for r in rows), "rel_l2_worst": max(r[2] for r in rows),
-                                         "cos_worst": min(r[3] for r in rows), "worst_tensor": rows[0][0]})
+    record_parity(f"{tag}_grads", {"norm_err_worst": max(r[1] for r in rows), "rel_l2_worst": max(r[2] for r in rows),
+                                   "cos_worst": min(r[3] for r in rows), "worst_tensor": rows[0][0]})
     print("worst grads (name, norm err, rel L2, cosine):", [(n, f"{a:.1e}", f"{b:.1e}", f"{c:.5f}") for n, a, b, c in rows[:8]])
     assert not bad, bad
+
+
+@pytest.mark.parametrize("T", [77, 200, 250, 347])
+def test_chunked_schedules_match_oracle(T):
+    """The flow steps' chunked schedules (csrc/ar_step.cu) at the shapes where they change: lstm layers 0/1 run in 100-step
+    chunks, one chunk apart (T = 77: one chunk; 200: two; 250: a ragged 50-step tail), and from T = 320 on the attention
+    LSTM runs in 256-step chunks under its attention (347 = 256 + 91).  Forward outputs and every parameter gradient of a
+    training step against the CPU oracle, at the bars of the reference-golden test above."""
+    from flowtron_b200 import _lib
+    from flowtron_b200.flowtron import FlowtronLoss
+    from oracle import flowtron_oracle as O
+    B, L, seed = 5, 12, 9
+    cfg = dict(synth.DEFAULT_MODEL_CONFIG, n_flows=2)
+    torch.backends.cudnn.allow_tf32 = False
+    torch.backends.cuda.matmul.allow_tf32 = False
+    model = build_model(cfg, seed).train()
+    model.encoder.p_dropout = 0.0
+    batch = synth.synth_batch(B, T, L, cfg, seed, with_prior=True)
+    cu = {k: (v.cuda() if torch.is_tensor(v) else v) for k, v in batch.items()}
+    out = model(cu["mel"], cu["speaker_ids"], cu["text"], cu["in_lens"], cu["out_lens"], cu["attn_prior"])
+    nll, gl, _ = FlowtronLoss(sigma=1.0, gate_loss=True)(out, cu["gate_target"], cu["in_lens"], cu["out_lens"])
+    (nll + gl).sum().backward()
+    torch.cuda.synchronize()
+    assert _lib.device_status() == 0
+
+    op = {k: v.clone().requires_grad_(True) for k, v in synth.synth_params(cfg, seed).items()}
+    oout = O.flowtron_forward(op, batch["mel"], batch["speaker_ids"], batch["text"], batch["in_lens"], batch["out_lens"],
+                              batch["attn_prior"], fast=True)
+    onll, ogl = O.flowtron_loss(oout, batch["gate_target"], batch["in_lens"], batch["out_lens"])
+    (onll + ogl).sum().backward()
+    vm = (torch.arange(T)[:, None] < batch["out_lens"][None, :])
+    errs = {"z": rel_err(out[0].detach().cpu()[vm], oout[0].detach()[vm]),
+            "gate": rel_err(out[2].detach().cpu()[vm], oout[2].detach()[vm])}
+    for i in range(cfg["n_flows"]):
+        errs[f"log_s_{i}"] = rel_err(out[1][i].detach().cpu()[vm], oout[1][i].detach()[vm])
+        errs[f"attn_{i}"] = rel_err(out[3][i].detach().cpu()[vm.t()], oout[3][i].detach()[vm.t()])
+    errs["nll"] = abs(float(nll) - float(onll)) / abs(float(onll))
+    record_parity(f"chunked_t{T}_forward", errs)
+    bad = {k: v for k, v in errs.items() if not v <= 1e-3}
+    assert not bad, bad
+    _assert_grads_match(f"chunked_t{T}", model, op, {n: float(op[n].grad.norm()) for n, _ in model.named_parameters()})
 
 
 def test_zero_init_identity_flow():
