@@ -107,7 +107,7 @@ def _declare(L):
     L.ft_ar_step_scratch_bytes.restype = c_size_t
     L.ft_ar_step_saved_lookup.argtypes = [POINTER(FtArStepDesc), c_char_p, POINTER(c_size_t), POINTER(c_size_t)]
     L.ft_ar_step_saved_lookup.restype = c_int
-    L.ft_ar_step_fwd.argtypes = [POINTER(FtArStepDesc), POINTER(FtArStepWeights)] + [c_void_p] * 13
+    L.ft_ar_step_fwd.argtypes = [POINTER(FtArStepDesc), POINTER(FtArStepWeights)] + [c_void_p] * 14
     L.ft_ar_step_fwd.restype = c_int
     L.ft_ar_step_bwd.argtypes = [POINTER(FtArStepDesc), POINTER(FtArStepWeights)] + [c_void_p] * 11 + \
         [POINTER(FtArStepWeights), c_void_p, c_void_p, c_void_p]
@@ -156,8 +156,6 @@ def _declare(L):
     L.ft_nll_grad.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_void_p, c_void_p,
                               c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
     L.ft_nll_grad.restype = c_int
-    L.ft_ar_step_set_text_ready_event.argtypes = [c_void_p]
-    L.ft_ar_step_set_text_ready_event.restype = None
     L.ft_sumsq_partials.argtypes = [c_void_p, c_longlong, c_void_p, c_void_p]
     L.ft_sumsq_partials.restype = c_int
     L.ft_clip_coef.argtypes = [c_void_p, c_int, c_float, c_void_p, c_void_p]
@@ -294,10 +292,6 @@ def lstm_bwd(dh_ext, whhT16, gates16, cstate, lens, dG16):
 _scratch = {}
 
 
-def set_lstm_half_sm(on: bool):
-    lib().ft_set_lstm_half_sm(1 if on else 0)
-
-
 def scratch_buffer(nbytes: int, device) -> torch.Tensor:
     """Per-(device, stream) transient work area shared by every flow on that stream (grown on demand)."""
     key = (device.type, device.index, torch.cuda.current_stream(device).cuda_stream)
@@ -332,15 +326,13 @@ def ar_step_saved_view(desc: FtArStepDesc, saved: torch.Tensor, name: str, dtype
     return saved[off.value: off.value + nb.value].view(dtype)
 
 
-def ar_step_fwd(desc, weights, mel, text, in_lens, out_lens, prior, mel_out, log_s, gates, attn, logprob, saved, scratch):
+def ar_step_fwd(desc, weights, mel, text, in_lens, out_lens, prior, mel_out, log_s, gates, attn, logprob, saved, scratch,
+                text_ready=None):
+    """text_ready: a recorded torch.cuda.Event (or None) that the call waits for before it first reads `text`."""
     check(lib().ft_ar_step_fwd(byref(desc), byref(weights), ptr(mel), ptr(text), ptr(in_lens), ptr(out_lens), ptr(prior),
                                ptr(mel_out), ptr(log_s), ptr(gates), ptr(attn), ptr(logprob), ptr(saved), ptr(scratch),
-                               stream_ptr()), "ft_ar_step_fwd")
-
-
-def set_text_ready_event(event):
-    """event: a recorded torch.cuda.Event (or None).  Consumed by the next ar_step_fwd on this thread."""
-    lib().ft_ar_step_set_text_ready_event(c_void_p(event.cuda_event) if event is not None else None)
+                               None if text_ready is None else c_void_p(text_ready.cuda_event), stream_ptr()),
+          "ft_ar_step_fwd")
 
 
 def ar_step_bwd(desc, weights, mel, in_lens, out_lens, attn, d_mel_out, d_log_s, d_gates, d_attn, d_logprob, d_mel, d_text,

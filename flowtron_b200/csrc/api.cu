@@ -124,10 +124,6 @@ int ft_gemm(int M, int N, int K, const void* A, long long lda, int a_fmt, int a_
 /* debug: device buffer [T][8] receiving clock64 stamps of CTA 0 of the next lstm_fwd launches (NULL disables) */
 void ft_debug_set_lstm_trace(long long* buf) { ft::set_lstm_trace(buf); }
 
-/* 1: ft_ar_step_fwd's folded-projection attention LSTM uses its 64-CTA variant (16 units per CTA) so that two
- * launches -- one per half batch, on two streams -- are co-resident on the GPU's SMs and hide each other's per-step
- * exchange latency. */
-void ft_set_lstm_half_sm(int on) { ft::set_lstm_half_sm(on); }
 void ft_set_gemm_pair_mode(int mode) { ft::set_gemm_pair_mode(mode); }
 
 int ft_lstm_fwd(int T, int B, const float* xproj, const void* whh16, const int* lens, void* hseq16, long long ldh,

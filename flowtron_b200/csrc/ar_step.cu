@@ -282,14 +282,9 @@ int copy_f32(float* dst, const float* src, size_t n, cudaStream_t st) {
 }  // namespace
 
 // =================================================================================================== forward
-static thread_local cudaEvent_t g_text_ready = nullptr;
-void set_text_ready_event(void* ev) { g_text_ready = static_cast<cudaEvent_t>(ev); }
-
 int ar_step_fwd(const FtArStepDesc& d, const FtArStepWeights& w, const float* mel, const float* text, const int* in_lens,
                 const int* out_lens, const float* prior, float* mel_out, float* log_s, float* gates, float* attn,
-                float* logprob, void* saved, void* scratch, cudaStream_t st) {
-    cudaEvent_t text_ready = g_text_ready;        // one-shot: consumed by this call whatever happens next
-    g_text_ready = nullptr;
+                float* logprob, void* saved, void* scratch, cudaEvent_t text_ready, cudaStream_t st) {
     FT_TRY(check_desc(d));
     if (d.has_prior && !prior) return ft_set_error("ar_step_fwd: has_prior set but attn_prior is NULL");
     if (d.has_gate && (!gates || !w.gate_w)) return ft_set_error("ar_step_fwd: has_gate set but gate pointers are NULL");
@@ -341,8 +336,8 @@ int ar_step_fwd(const FtArStepDesc& d, const FtArStepWeights& w, const float* me
         return 0;
     };
     auto kv_projections = [&](cudaStream_t s2) -> int {
-        // First use of `text`: if the caller produced it on another stream it handed us the event to wait for, so the encoder
-        // ran underneath everything above (ft_ar_step_set_text_ready_event).
+        // First use of `text`: if the caller produced it on another stream it passed the event to wait for, so the encoder
+        // ran underneath everything above.
         if (text_ready) {
             if (cudaStreamWaitEvent(s2, text_ready, 0) != cudaSuccess) return ft_set_error("ar_step_fwd: cudaStreamWaitEvent(text_ready) failed");
         }
@@ -638,15 +633,14 @@ int ft_ar_step_saved_lookup(const FtArStepDesc* d, const char* name, size_t* off
     return ft::ft_set_error("ft_ar_step_saved_lookup: unknown region");
 }
 
-void ft_ar_step_set_text_ready_event(void* cuda_event) { ft::set_text_ready_event(cuda_event); }
-
 int ft_ar_step_fwd(const FtArStepDesc* d, const FtArStepWeights* w, const float* mel, const float* text,
                    const int* in_lens, const int* out_lens, const float* attn_prior, float* mel_out, float* log_s,
-                   float* gates, float* attn, float* attn_logprob, void* saved, void* scratch, void* stream) {
+                   float* gates, float* attn, float* attn_logprob, void* saved, void* scratch, void* text_ready_event,
+                   void* stream) {
     if (!d || !w || !mel || !text || !mel_out || !log_s || !attn || !attn_logprob || !saved || !scratch)
         return ft::ft_set_error("ft_ar_step_fwd: NULL argument");
     return ft::ar_step_fwd(*d, *w, mel, text, in_lens, out_lens, attn_prior, mel_out, log_s, gates, attn, attn_logprob,
-                           saved, scratch, static_cast<cudaStream_t>(stream));
+                           saved, scratch, static_cast<cudaEvent_t>(text_ready_event), static_cast<cudaStream_t>(stream));
 }
 
 int ft_ar_step_bwd(const FtArStepDesc* d, const FtArStepWeights* w, const float* mel, const int* in_lens,

@@ -41,7 +41,6 @@ int make_tmap_2d(CUtensorMap* out, const void* ptr, int fmt, long long rows, lon
                  int box_cols, int box_rows);
 
 void set_lstm_trace(long long* p);
-void set_lstm_half_sm(int on);
 int launch_lstm_fwd(int T, int B, const float* xproj, const void* whh16, const int* lens, void* hseq16, long long ldh,
                     void* gates16, float* cstate, float* h32, long long ldh32, int* flags, cudaStream_t st);
 int launch_lstm_fwd_xin(int T, int B, const void* x16, long long ldx, int kx, const void* wih16, const float* b_ih, const float* b_hh,

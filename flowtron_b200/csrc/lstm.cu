@@ -606,9 +606,6 @@ static int make_tmap_chunks(CUtensorMap* out, const void* ptr, long long rows, i
     return 0;
 }
 
-static bool g_half_sm = false;       // 64-CTA folded-projection forward (for two concurrent half-batch launches)
-void set_lstm_half_sm(int on) { g_half_sm = on != 0; }
-
 // Steps [t0, t1) of one layer's forward recurrence on 1024 / UNITS CTAs.  `flags` needs (t1 - t0) * 16 ints.
 // x16 != null: folded input projection (kXIn): x16 [T*B, kx] fp16 (row pitch ldx), wih16 [4096, kx] fp16, biases fp32.
 template <int UNITS, bool kXIn>
@@ -656,15 +653,13 @@ int launch_lstm_fwd(int T, int B, const float* xproj, const void* whh16, const i
 }
 
 // Whole sequence with the input projection folded in (narrow inputs, kx <= 128; x16 row 0..B-1 must be zero: step 0 skips the
-// contraction).  128 CTAs (or 64 with the half-SM switch).
+// contraction).  128 CTAs.
 int launch_lstm_fwd_xin(int T, int B, const void* x16, long long ldx, int kx, const void* wih16, const float* b_ih, const float* b_hh,
                         const void* whh16, const int* lens, void* hseq16, long long ldh, void* gates16, float* cstate, float* h32,
                         long long ldh32, int* flags, cudaStream_t st) {
     if (T <= 0 || B <= 0) return 0;
     if (B > 32) return ft_set_error("lstm_fwd: batch > 32 per call not supported (split the batch)");
     if (!x16 || !wih16 || !b_ih || !b_hh) return ft_set_error("lstm_fwd_xin: NULL argument");
-    if (g_half_sm)
-        return launch_fwd_t<16, true>(T, B, 0, T, nullptr, whh16, lens, hseq16, ldh, gates16, cstate, h32, ldh32, flags, st, x16, ldx, kx, wih16, b_ih, b_hh);
     return launch_fwd_t<8, true>(T, B, 0, T, nullptr, whh16, lens, hseq16, ldh, gates16, cstate, h32, ldh32, flags, st, x16, ldx, kx, wih16, b_ih, b_hh);
 }
 

@@ -290,7 +290,7 @@ class _ArStepFn(torch.autograd.Function):
     """Autograd node B: ft_ar_step_fwd (the whole forward) / ft_ar_step_bwd_main."""
 
     @staticmethod
-    def forward(ctx, state, step, reversed_flag, token, mel, text, in_lens, out_lens, attn_prior, *params_b):
+    def forward(ctx, state, step, reversed_flag, token, mel, text, in_lens, out_lens, attn_prior, text_ready, *params_b):
         if not mel.is_cuda:
             raise FlowtronB200Error("AR_Step needs CUDA tensors: the sm_90a kernels are the only implementation")
         T, B, M = mel.shape
@@ -314,12 +314,9 @@ class _ArStepFn(torch.autograd.Function):
         gates = torch.empty(T, B, 1, device=dev) if has_gate else None
         attn = torch.empty(B, T, L, device=dev)
         logprob = torch.empty(B, T, L, device=dev)
-        ev = getattr(step, "_text_event", None)
-        if ev is not None:                        # `text` was produced on another stream: wait inside the flow, not here
-            step._text_event = None
-            _lib.set_text_ready_event(ev)
+        # text_ready: `text` was produced on another stream; the flow waits for it inside the C call, not here
         _lib.ar_step_fwd(desc, weights, mel_c, text_c, in_lens, out_lens, prior_c, mel_out, log_s, gates, attn, logprob,
-                         saved, scratch)
+                         saved, scratch, text_ready)
         state.desc, state.saved, state.plist = desc, saved, plist
         state.mel_c, state.in_lens, state.out_lens, state.attn = mel_c, in_lens, out_lens, attn
         state.text_shape, state.has_gate = text.shape, has_gate
@@ -353,8 +350,9 @@ class _ArStepFn(torch.autograd.Function):
                               d_gates, d_attn, d_lp, d_text, _lib.make_weights(st.grads), st.saved, scratch, st.carry)
         grads_b = [st.grads[i] for i in _MAIN_HALF]
         ctx.state = None
-        # (state, step, reversed, token, mel, text, in_lens, out_lens, prior, *params_b): mel's gradient comes out of node A
-        return (None, None, None, torch.zeros(1, device=dev), None, d_text, None, None, None, *grads_b)
+        # (state, step, reversed, token, mel, text, in_lens, out_lens, prior, text_ready, *params_b): mel's gradient comes
+        # out of node A
+        return (None, None, None, torch.zeros(1, device=dev), None, d_text, None, None, None, None, *grads_b)
 
 
 class AR_Step(nn.Module):
@@ -393,7 +391,7 @@ class AR_Step(nn.Module):
                 self.conv.weight, self.conv.bias,
                 None if gate is None else gate.linear_layer.weight, None if gate is None else gate.linear_layer.bias]
 
-    def _run(self, mel, text, mask, out_lens, attn_prior, reversed_flag):
+    def _run(self, mel, text, mask, out_lens, attn_prior, reversed_flag, text_ready):
         dev = mel.device
         in_lens = None
         if mask is not None:
@@ -403,15 +401,16 @@ class AR_Step(nn.Module):
         state.clear()
         token = _ArStepAttnLstmFn.apply(state, mel, *[plist[i] for i in _ATTN_HALF])
         out = _ArStepFn.apply(state, self, reversed_flag, token, mel, text, in_lens, _lens_i32(out_lens, dev), attn_prior,
-                              *[plist[i] for i in _MAIN_HALF])
+                              text_ready, *[plist[i] for i in _MAIN_HALF])
         if hasattr(self, 'gate_layer'):
             mel_out, log_s, gates, attn, lp = out
         else:
             (mel_out, log_s, attn, lp), gates = out, None
         return mel_out, log_s, gates, attn, lp
 
-    def forward(self, mel, text, mask, out_lens, attn_prior=None):
-        return self._run(mel, text, mask, out_lens, attn_prior, False)
+    def forward(self, mel, text, mask, out_lens, attn_prior=None, *, text_ready=None):
+        """text_ready: a recorded torch.cuda.Event for `text` when another stream produces it (None: already there)."""
+        return self._run(mel, text, mask, out_lens, attn_prior, False, text_ready)
 
     def infer(self, residual, text, attns, attn_prior=None):
         from .inference import ar_step_infer
@@ -433,10 +432,10 @@ class AR_Back_Step(nn.Module):
         self.ar_step = AR_Step(n_mel_channels, n_speaker_dim, n_text_dim, n_mel_channels + n_speaker_dim, n_hidden,
                                n_attn_channels, n_lstm_layers, add_gate, use_cumm_attention)
 
-    def forward(self, mel, text, mask, out_lens, attn_prior=None):
+    def forward(self, mel, text, mask, out_lens, attn_prior=None, *, text_ready=None):
         if out_lens is None:
             out_lens = torch.full((mel.size(1),), mel.size(0), dtype=torch.long, device=mel.device)
-        return self.ar_step._run(mel, text, mask, out_lens, attn_prior, True)
+        return self.ar_step._run(mel, text, mask, out_lens, attn_prior, True, text_ready)
 
     def infer(self, residual, text, attns, attn_prior=None):
         from .inference import ar_step_infer
@@ -487,10 +486,9 @@ class Flowtron(nn.Module):
             self.flows.append(cls(n_mel_channels, n_speaker_dim, n_text_dim, n_mel_channels + n_speaker_dim, n_hidden,
                                   n_attn_channels, n_lstm_layers, add_gate, use_cumm_attention))
 
-    # Optional: run two half batches as independent pipelines on two CUDA streams (each recurrence then uses a 64-SM
-    # persistent kernel, so both are co-resident).  This does NOT shorten the recurrence chain (a half batch takes as
-    # many dependent steps as the full batch); it only lets one half's GEMMs / attention / launch gaps overlap the other
-    # half's recurrences.  Off by default.
+    # Optional: run two half batches as independent pipelines on two CUDA streams.  This does NOT shorten the recurrence
+    # chain (a half batch takes as many dependent steps as the full batch); it only lets one half's GEMMs / attention /
+    # launch gaps overlap the other half's recurrences.  Off by default.
     n_streams = 1
     # run the Encoder underneath the first flow's attention LSTM
     overlap_encoder = True
@@ -500,29 +498,50 @@ class Flowtron(nn.Module):
     # consecutive launches of up to 32 utterances each.
     max_kernel_batch = 32
 
-    def _run_flows(self, mel, encoder_outputs, mask, out_lens, attn_prior):
+    def _run_flows(self, mel, encoder_outputs, mask, out_lens, attn_prior, text_ready=None, text_slices=None):
+        """Every flow over the batch, in launches of at most max_kernel_batch utterances; the first flow of each launch
+        waits for `text_ready`.  text_slices: the launches' text, made contiguous on the stream that produced it."""
         B = mel.size(1)
-        if B > self.max_kernel_batch:          # larger batches run as consecutive chunks (utterances are independent)
-            ech = getattr(self, "_enc_chunks", None) or {}      # contiguous text slices made on the encoder's stream (forward())
-            outs = [self._run_flows(mel[:, b0:b0 + self.max_kernel_batch], ech.get(b0, encoder_outputs[:, b0:b0 + self.max_kernel_batch]),
-                                    mask[b0:b0 + self.max_kernel_batch],
-                                    None if out_lens is None else out_lens[b0:b0 + self.max_kernel_batch],
-                                    None if attn_prior is None else attn_prior[b0:b0 + self.max_kernel_batch])
-                    for b0 in range(0, B, self.max_kernel_batch)]
-            n_flows = len(self.flows)
-            return (torch.cat([o[0] for o in outs], 1), [torch.cat([o[1][i] for o in outs], 1) for i in range(n_flows)],
-                    None if outs[0][2] is None else torch.cat([o[2] for o in outs], 1),
-                    [torch.cat([o[3][i] for o in outs], 0) for i in range(n_flows)],
-                    [torch.cat([o[4][i] for o in outs], 0) for i in range(n_flows)])
+        mkb = self.max_kernel_batch
+        if B > mkb:                            # larger batches run as consecutive chunks (utterances are independent)
+            return self._run_slices([(b0, min(b0 + mkb, B)) for b0 in range(0, B, mkb)], mel, encoder_outputs, mask,
+                                    out_lens, attn_prior, text_ready, text_slices)
         log_s_list, attns_list, attns_logprob_list, gate = [], [], [], None
         for i, flow in enumerate(self.flows):
-            # the module whose kernels run first gets the text-ready event (AR_Back_Step wraps its AR_Step as .ar_step)
-            getattr(flow, "ar_step", flow)._text_event = getattr(self, "_text_event", None) if i == 0 else None
-            mel, log_s, gate, attn_out, attn_logprob_out = flow(mel, encoder_outputs, mask, out_lens, attn_prior)
+            mel, log_s, gate, attn_out, attn_logprob_out = flow(mel, encoder_outputs, mask, out_lens, attn_prior,
+                                                                text_ready=text_ready if i == 0 else None)
             log_s_list.append(log_s)
             attns_list.append(attn_out)
             attns_logprob_list.append(attn_logprob_out)
         return mel, log_s_list, gate, attns_list, attns_logprob_list
+
+    def _run_slices(self, bounds, mel, encoder_outputs, mask, out_lens, attn_prior, text_ready=None, text_slices=None,
+                    streams=None):
+        """_run_flows on each batch slice [b0, b1) of `bounds`, outputs concatenated along the batch.  text_slices[k]
+        replaces slice k of `encoder_outputs` when given.  With `streams`, slice k runs on streams[k] and the outputs are
+        joined back onto the caller's stream."""
+        cur = torch.cuda.current_stream() if streams else None
+        parts = []
+        for k, (b0, b1) in enumerate(bounds):
+            if streams:
+                streams[k].wait_stream(cur)
+            with torch.cuda.stream(streams[k] if streams else None):     # None: stay on the current stream
+                parts.append(self._run_flows(mel[:, b0:b1], encoder_outputs[:, b0:b1] if text_slices is None else text_slices[k],
+                                             mask[b0:b1], None if out_lens is None else out_lens[b0:b1],
+                                             None if attn_prior is None else attn_prior[b0:b1], text_ready))
+        for s in streams or ():
+            cur.wait_stream(s)
+
+        def cat(ts, dim):
+            if streams:
+                for t in ts:
+                    t.record_stream(cur)
+            return torch.cat(ts, dim)
+        n_flows = len(self.flows)
+        return (cat([p[0] for p in parts], 1), [cat([p[1][i] for p in parts], 1) for i in range(n_flows)],
+                None if parts[0][2] is None else cat([p[2] for p in parts], 1),
+                [cat([p[3][i] for p in parts], 0) for i in range(n_flows)],
+                [cat([p[4][i] for p in parts], 0) for i in range(n_flows)])
 
     def _encode(self, speaker_ids, text, in_lens):
         """flowtron.py:871-880: embeddings + Encoder + speaker vector concat -> [L, B, n_text + n_speaker]."""
@@ -537,65 +556,39 @@ class Flowtron(nn.Module):
         B = mel.size(0)
         # The first flow needs the text encoding only after its attention LSTM (T dependent steps that read mel alone), so
         # the encoder's ~700 small latency-bound kernels can run on a second stream underneath it; the flow's C entry
-        # point waits for `text_event` right before it first reads the encoding (ft_ar_step_set_text_ready_event).
+        # point waits for `text_ready` right before it first reads the encoding.
         overlap = self.overlap_encoder and mel.is_cuda and self.n_streams <= 1 and B <= 64
-        self._text_event = None
+        text_ready, text_slices = None, None
         if overlap:
             cur = torch.cuda.current_stream(mel.device)
             es = _encoder_overlap_stream(mel.device)
             es.wait_stream(cur)
-            self._enc_chunks = None
             with torch.cuda.stream(es):
                 encoder_outputs = self._encode(speaker_ids, text, in_lens)
                 if B > self.max_kernel_batch:
                     # the flows will run on slices of the batch: make them contiguous HERE, on the encoder's stream, in front of
                     # the event (a .contiguous() issued later on the caller's stream would read the encoding before it exists)
                     mkb = self.max_kernel_batch
-                    self._enc_chunks = {b0: encoder_outputs[:, b0:b0 + mkb].contiguous() for b0 in range(0, B, mkb)}
-                    for t in self._enc_chunks.values():
+                    text_slices = [encoder_outputs[:, b0:b0 + mkb].contiguous() for b0 in range(0, B, mkb)]
+                    for t in text_slices:
                         t.record_stream(cur)
-                ev = torch.cuda.Event()
-                ev.record(es)
+                text_ready = torch.cuda.Event()
+                text_ready.record(es)
             encoder_outputs.record_stream(cur)
-            self._text_event = ev
         else:
-            self._enc_chunks = None
             encoder_outputs = self._encode(speaker_ids, text, in_lens)
         mel = mel.permute(2, 0, 1)
         # key-padding mask from the padded text length (== max(in_lens) by the collate contract): no .item() host sync
         mask = ~(torch.arange(n_text, device=in_lens.device)[None, :] < in_lens[:, None])[..., None]
         split = self.n_streams > 1 and mel.is_cuda and B >= self.min_split_batch and out_lens is not None
-        if mel.is_cuda:
-            _lib.set_lstm_half_sm(split)
         if not split:
-            mel, log_s_list, gate, attns_list, attns_logprob_list = self._run_flows(mel, encoder_outputs, mask, out_lens, attn_prior)
-            return (mel, log_s_list, gate, attns_list, attns_logprob_list, mean, log_var, prob)
-
-        cur = torch.cuda.current_stream()
-        if not hasattr(self, "_side_streams") or self._side_streams[0].device != mel.device:
-            self._side_streams = [torch.cuda.Stream(device=mel.device) for _ in range(2)]
-        bounds = [(0, B // 2), (B // 2, B)]
-        parts = []
-        for (b0, b1), s in zip(bounds, self._side_streams):
-            s.wait_stream(cur)
-            with torch.cuda.stream(s):
-                part = self._run_flows(mel[:, b0:b1], encoder_outputs[:, b0:b1], mask[b0:b1], out_lens[b0:b1],
-                                       None if attn_prior is None else attn_prior[b0:b1])
-            parts.append(part)
-        for s in self._side_streams:
-            cur.wait_stream(s)
-
-        def cat(ts, dim):
-            for t in ts:
-                t.record_stream(cur)
-            return torch.cat(ts, dim)
-        n_flows = len(self.flows)
-        mel = cat([p[0] for p in parts], 1)
-        log_s_list = [cat([p[1][i] for p in parts], 1) for i in range(n_flows)]
-        gate = None if parts[0][2] is None else cat([p[2] for p in parts], 1)
-        attns_list = [cat([p[3][i] for p in parts], 0) for i in range(n_flows)]
-        attns_logprob_list = [cat([p[4][i] for p in parts], 0) for i in range(n_flows)]
-        return (mel, log_s_list, gate, attns_list, attns_logprob_list, mean, log_var, prob)
+            out = self._run_flows(mel, encoder_outputs, mask, out_lens, attn_prior, text_ready, text_slices)
+        else:
+            if not hasattr(self, "_side_streams") or self._side_streams[0].device != mel.device:
+                self._side_streams = [torch.cuda.Stream(device=mel.device) for _ in range(2)]
+            out = self._run_slices([(0, B // 2), (B // 2, B)], mel, encoder_outputs, mask, out_lens, attn_prior,
+                                   streams=self._side_streams)
+        return (*out, mean, log_var, prob)
 
     def infer(self, residual, speaker_ids, text, temperature=1.0, gate_threshold=0.5, attns=None, attn_prior=None):
         speaker_ids = speaker_ids * 0 if self.dummy_speaker_embedding else speaker_ids

@@ -55,10 +55,6 @@ void ft_debug_set_lstm_trace(long long* buf);
 /* same for ft_ar_step_infer: [T][32] stamps of CTA 0 (phase boundaries, tools/trace_infer.py) */
 void ft_debug_set_infer_trace(long long* buf);
 
-/* Process-wide switch: 1 = ft_ar_step_fwd runs the attention LSTM's folded-projection recurrence (T < 320) on 64 CTAs
- * instead of 128, so two half-batch launches on two streams run concurrently (every other recurrence kernel, forward
- * and BPTT, always uses 64 CTAs). */
-void ft_set_lstm_half_sm(int on);
 /* ft_gemm tile policy: 0 = one CTA per 128 x 256 tile always; 1 (default) = CTA pairs (2-CTA clusters sharing B by TMA multicast, 256 x 256 tiles) for
  * contractions >= 1e11 FLOP; 2 = CTA pairs whenever the output is wide and has >= SMs/2 such tiles. */
 void ft_set_gemm_pair_mode(int mode);
@@ -110,16 +106,14 @@ int ft_ar_step_saved_lookup(const FtArStepDesc* d, const char* name, size_t* off
  *   mel [T,B,M] f32, text [L,B,E] f32 (encoder outputs), in_lens/out_lens int32 [B] (NULL = no padding),
  *   attn_prior [B,T,L] f32 or NULL  ->  mel_out [T,B,M], log_s [T,B,M], gates [T,B] (NULL if !has_gate),
  *   attn [B,T,L], attn_logprob [B,T,L].  For reversed flows log_s/gates/attn are in flipped time exactly as
- *   the reference returns them. */
+ *   the reference returns them.
+ *   text_ready_event: a cudaEvent_t recorded on whatever stream produced `text`, or NULL.  The call waits for it right
+ *   before it first reads `text` -- i.e. after the attention LSTM, which depends on mel only -- so the caller can run
+ *   the text encoder (flowtron.py:871-880) concurrently with the first third of the flow instead of in front of it. */
 int ft_ar_step_fwd(const FtArStepDesc* d, const FtArStepWeights* w, const float* mel, const float* text,
                    const int* in_lens, const int* out_lens, const float* attn_prior, float* mel_out, float* log_s,
-                   float* gates, float* attn, float* attn_logprob, void* saved, void* scratch, void* stream);
-
-/* Optional, one-shot, per host thread: the NEXT ft_ar_step_fwd call on this thread waits for `cuda_event` (a
- * cudaEvent_t recorded on whatever stream produced `text`) on its own stream right before it first reads `text` --
- * i.e. after the attention LSTM, which depends on mel only -- so the caller can run the text encoder
- * (flowtron.py:871-880) concurrently with the first third of the flow instead of in front of it.  NULL clears it. */
-void ft_ar_step_set_text_ready_event(void* cuda_event);
+                   float* gates, float* attn, float* attn_logprob, void* saved, void* scratch, void* text_ready_event,
+                   void* stream);
 
 /* Autograd of the above.  Incoming gradients (any may be NULL = zero): d_mel_out, d_log_s [T,B,M], d_gates [T,B],
  * d_attn, d_attn_logprob [B,T,L].  Outputs: d_mel [T,B,M], d_text [L,B,E] (overwritten), parameter gradients

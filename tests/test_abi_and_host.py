@@ -108,6 +108,23 @@ def test_validated_defaults_and_no_native_environment_switches():
     assert 'os.environ.get("FT_GRAPH", "1")' in src
 
 
+def test_flow_step_has_no_hidden_process_state():
+    """What ft_ar_step_fwd launches follows from its arguments: the library has no process-wide kernel switch and no
+    per-thread side channel for the text-ready event, and Flowtron.forward hands that event to the flows as an argument,
+    not through module attributes."""
+    from flowtron_b200 import build
+    L = ctypes.CDLL(build.build())
+    for name in ("ft_set_lstm_half_sm", "ft_ar_step_set_text_ready_event"):
+        assert not hasattr(L, name), name
+    csrc = os.path.join(ROOT, "flowtron_b200", "csrc")
+    per_thread = [(f, line.strip()) for f in sorted(os.listdir(csrc)) for line in open(os.path.join(csrc, f))
+                  if "thread_local" in line]
+    # the one per-thread variable is the message ft_last_error returns, which is per thread like errno
+    assert per_thread == [("api.cu", "static thread_local std::string g_err;")], per_thread
+    src = open(os.path.join(ROOT, "flowtron_b200", "flowtron.py")).read()
+    assert "_text_event" not in src and "_enc_chunks" not in src
+
+
 def test_encoder_abi_host_side():
     """ft_encoder_*_bytes are pure host functions: sizes grow with the batch, an unsupported descriptor gives 0 and an error
     string (no GPU needed)."""

@@ -16,9 +16,6 @@ def main():
     trace = torch.zeros(T, 16, dtype=torch.int64, device="cuda")
     L = _lib.lib()
     L.ft_debug_set_lstm_trace.argtypes = [ctypes.c_void_p]
-    if len(sys.argv) > 2 and sys.argv[2] == "half":      # the 64-CTA x 16-unit forward kernel of the layer pipeline
-        _lib.set_lstm_half_sm(True)
-        print("64-CTA forward kernel (16 units per CTA)")
     for it in range(3):
         if it == 2:
             L.ft_debug_set_lstm_trace(ctypes.c_void_p(trace.data_ptr()))
