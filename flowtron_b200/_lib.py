@@ -72,6 +72,17 @@ class FlowtronB200Error(RuntimeError):
     pass
 
 
+# Longest text (tokens) the flow-step kernels take in training and inference: FT_MAX_TEXT_LEN in include/flowtron_b200.h
+# (ft_max_text_len()).  Texts of up to 256 tokens run the short-text kernel variants, longer ones the long-text variants.
+MAX_TEXT_LEN = 1024
+
+
+def check_text_len(L: int, where: str) -> None:
+    """ValueError for a padded text length the kernels do not take, before any allocation or launch."""
+    if L > MAX_TEXT_LEN:
+        raise ValueError(f"{where}: text length {L} > {MAX_TEXT_LEN} tokens (MAX_TEXT_LEN) is not supported")
+
+
 def lib() -> ctypes.CDLL:
     global _lib
     if _lib is None:
@@ -101,6 +112,7 @@ def _declare(L):
     L.ft_lstm_bwd.restype = c_int
 
 
+    L.ft_max_text_len.restype = c_int
     L.ft_ar_step_saved_bytes.argtypes = [POINTER(FtArStepDesc)]
     L.ft_ar_step_saved_bytes.restype = c_size_t
     L.ft_ar_step_scratch_bytes.argtypes = [POINTER(FtArStepDesc)]

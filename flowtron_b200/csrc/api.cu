@@ -68,6 +68,7 @@ TimeScope::~TimeScope() {
 extern "C" {
 
 int ft_version(void) { return 100; }
+int ft_max_text_len(void) { return FT_MAX_TEXT_LEN; }
 
 const char* ft_last_error(void) { return ft::g_err.c_str(); }
 

@@ -109,6 +109,7 @@ struct FwdScratch {
     int* flags;
     float* X1;                  // second input-projection buffer: the attention LSTM's (overlap), then layer 1's (pipeline)
     float *hA32 = nullptr, *ctx32 = nullptr;     // fp32 copies of [hA ; ctx] for the gate logits (gated flow only)
+    float* attn_rows = nullptr;                  // long texts: the attention's score rows (attn_rows_in_global)
     void plan(Plan& p, const FtArStepDesc& d) {
         const Dims n(d);
         w.plan(p, n);
@@ -119,6 +120,7 @@ struct FwdScratch {
             hA32 = p.get<float>("hA32", n.R * H);
             ctx32 = p.get<float>("ctx32", n.R * n.A);
         }
+        if (attn_rows_in_global(n.L, n.A)) attn_rows = p.get<float>("attn_rows", attn_rows_floats(n.T, n.B, n.L));
     }
 };
 
@@ -141,6 +143,7 @@ struct BwdScratch {
     float *dh, *dQ, *dK, *dV, *dmel_in;
     int* flags;
     float *dcarry1, *dcarry0;   // dc*f hand-over between BPTT chunks of the layer pipeline
+    float* attn_rows = nullptr; // long texts: the attention backward's gradient rows (attn_rows_in_global)
     void plan(Plan& p, const FtArStepDesc& d) {
         const Dims n(d);
         w.plan(p, n);
@@ -162,6 +165,7 @@ struct BwdScratch {
         flags = p.get<int>("flags", static_cast<size_t>(std::max(n.T, 2 * layer_chunk(n.T))) * 64);
         dcarry1 = p.get<float>("dcarry1", static_cast<size_t>(n.B) * H);
         dcarry0 = p.get<float>("dcarry0", static_cast<size_t>(n.B) * H);
+        if (attn_rows_in_global(n.L, n.A)) attn_rows = p.get<float>("attn_rows", attn_rows_floats(n.T, n.B, n.L));
     }
 };
 
@@ -171,7 +175,7 @@ int check_desc(const FtArStepDesc& d) {
     if (d.B > 32) return ft_set_error("ar_step: batch > 32 per call not supported (split the batch)");
     if (d.n_mel > 128 || d.n_mel % 8 || d.n_attn % 64 || d.n_text % 8)
         return ft_set_error("ar_step: n_mel <= 128 and %8, n_attn %64, n_text %8 required");
-    if (d.L > 256) return ft_set_error("ar_step: L > 256 not supported");
+    if (d.L > FT_MAX_TEXT_LEN) return ft_set_error("ar_step: L > FT_MAX_TEXT_LEN (1024) not supported");
     return 0;
 }
 
@@ -330,7 +334,7 @@ int ar_step_fwd(const FtArStepDesc& d, const FtArStepWeights& w, const float* me
         a.in_lens = in_lens; a.out_lens = out_lens; a.prior = d.has_prior ? prior : nullptr; a.reversed = d.reversed;
         a.temperature = d.temperature; a.attn = attn; a.logprob = logprob; a.p_save = S.p_save;
         a.ctx16 = S.d16 + H; a.ldc = n.D; a.ctx32 = F.ctx32; a.ldc32 = n.A;
-        a.t_begin = t0; a.t_end = t1;
+        a.t_begin = t0; a.t_end = t1; a.rows = F.attn_rows;
         FT_TRY(launch_attn_fwd(a, s2));
         if (d.has_gate) FT_TRY(launch_gate_fwd_f32(F.hA32 + r0 * H, H, H, F.ctx32 + r0 * n.A, n.A, n.A, w.gate_w, w.gate_b, rows, gates + r0, s2));
         return 0;
@@ -542,7 +546,7 @@ int ar_step_bwd_main(const FtArStepDesc& d, const FtArStepWeights& w, const floa
     a.in_lens = in_lens; a.out_lens = out_lens; a.attn = attn; a.p_save = S_.p_save; a.temperature = d.temperature;
     a.dctx = C.dd + H; a.lddc = n.D; a.dattn_ext = d_attn; a.dlp_ext = d_logprob; a.scale = S;
     a.dQ = F.dQ; a.lddq = n.A; a.dK = F.dK; a.lddk = n.A; a.dV = F.dV; a.lddv = n.A; a.dv = g.att_v;
-    a.t_begin = 0; a.t_end = n.T;
+    a.t_begin = 0; a.t_end = n.T; a.rows = F.attn_rows;
     FT_TRY(launch_attn_bwd(a, st));
     // 9a. query projection (d16 = [hA ; ctx] saved in fp16, row pitch D)
     FT_TRY(launch_cast(F.dQ, 2, F.dQ16, 0, R * n.A, st));

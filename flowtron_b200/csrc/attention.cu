@@ -12,8 +12,12 @@
 // 2 FMA + 1 MUFU.RCP per (t,l,a) -- the kernel is bound by the SFU pipe (16 rcp/clk/SM), not by HBM.
 // The backward kernel recomputes the tile the same way and reduces dQ (shuffles), dK/dV (shared +
 // global float atomics across t-tiles) and dv.
+// Both kernels keep a 64-query tile's rows of scores (forward) / attention gradients (backward) in shared memory while
+// they fit in a block's 227 KiB (L <= 672 at A = 640); longer texts run the kGlobalRows instantiations, which keep those
+// rows in a caller-provided global area instead (attn_rows_floats) and are otherwise the same code (DESIGN.md 4.16).
 #include "ptx.cuh"
 #include "ft_internal.h"
+#include "../../include/flowtron_b200.h"
 
 namespace ft {
 
@@ -40,6 +44,7 @@ struct AttnFwdParams {
     float* p_save;                       // [B,T,L] first softmax (only when prior), or null
     __half* ctx16; long long ldc;        // ctx (fp16) written at ctx16[(t*B+b)*ldc + a]
     float* ctx32; long long ldc32;       // optional fp32 ctx (null ok)
+    float* rows;                         // kGlobalRows: score rows [B][T rounded up to 64][Lr + 4]
 };
 
 __device__ __forceinline__ int back_index(int t, int len, int T) {     // flowtron.py:606-613 as an index map
@@ -79,19 +84,28 @@ __device__ __forceinline__ void score_chunk(float (&acc)[4][8], const float* __r
     }
 }
 
+// A tile's rows in the global row area: rows [t0, t0 + 64) of utterance b.  t_begin is a multiple of 64 and a launch
+// ends at a multiple of 64 or at T, so every tile of the area belongs to one launch only (the overlapped chunks of the
+// training forward never share one).
+__device__ __forceinline__ float* tile_rows(float* rows, int b, int T, int t0, int ld) {
+    const int Tp = (T + AT_TT - 1) / AT_TT * AT_TT;
+    return rows + (static_cast<long long>(b) * Tp + t0) * ld;
+}
+
+template <bool kGlobalRows>
 __global__ void __launch_bounds__(AT_THREADS, 2)
 attn_fwd_kernel(AttnFwdParams p) {
     extern __shared__ float smf[];
     const int Lr = (p.L + 31) & ~31;                  // score row pitch: keys rounded up to a warp
-    float* sQ = smf;                                  // [AT_AC][SQ_LD]
-    float* sK = sQ + AT_AC * SQ_LD;                   // [AT_AC][SK_LD]   (also the V chunk [64][AT_AC+4])
-    float* sE = sK + AT_AC * SK_LD;                   // [AT_TT][Lr+4]
-    float* sv = sE + AT_TT * (Lr + 4);                // [A]
-    __shared__ float s_sumv;
     const int SE_LD = Lr + 4;
-
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int b = blockIdx.y, t0 = p.t_begin + blockIdx.x * AT_TT;
+    float* sQ = smf;                                  // [AT_AC][SQ_LD]
+    float* sK = sQ + AT_AC * SQ_LD;                   // [AT_AC][SK_LD]   (also the V chunk [64][AT_AC+4])
+    float* sE = kGlobalRows ? tile_rows(p.rows, b, p.T, t0, SE_LD) : sK + AT_AC * SK_LD;   // [AT_TT][Lr+4]
+    float* sv = kGlobalRows ? sK + AT_AC * SK_LD : sE + AT_TT * (Lr + 4);                  // [A]
+    __shared__ float s_sumv;
+
     const int out_len = p.out_lens ? p.out_lens[b] : p.T;
     const int in_len = p.in_lens ? p.in_lens[b] : p.L;
     const int nrows = min(AT_TT, p.t_end - t0);
@@ -301,22 +315,24 @@ struct AttnBwdParams {
     float* dK; long long lddk;            // [L*B, A] accumulated (atomicAdd; caller zeroes)
     float* dV; long long lddv;            // [L*B, A] accumulated
     float* dv;                            // [A] accumulated
+    float* rows;                          // kGlobalRows: dattn / de rows [B][T rounded up to 64][Lr + 4]
 };
 
+template <bool kGlobalRows>
 __global__ void __launch_bounds__(AT_THREADS, 2)
 attn_bwd_kernel(AttnBwdParams p) {
     extern __shared__ float smf[];
     const int Lr = (p.L + 31) & ~31;
     const int SE_LD = Lr + 4;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int b = blockIdx.y, t0 = p.t_begin + blockIdx.x * AT_TT;
     float* sQ = smf;                                  // [AT_AC][SQ_LD]   (phase 3: e^{2q} as [AT_TT][65])
     float* sK = sQ + AT_AC * SQ_LD;                   // [AT_AC][SK_LD]   (phase 3: e^{2k} as [AT_LB][65])
-    float* sD = sK + AT_AC * SK_LD;                   // [AT_TT][SE_LD]  dattn -> de
-    float* sv = sD + AT_TT * SE_LD;                   // [A]
+    float* sD = kGlobalRows ? tile_rows(p.rows, b, p.T, t0, SE_LD) : sK + AT_AC * SK_LD;   // [AT_TT][SE_LD]  dattn -> de
+    float* sv = kGlobalRows ? sK + AT_AC * SK_LD : sD + AT_TT * SE_LD;                     // [A]
     float* sdv = sv + p.A;                            // [A]
     __shared__ float s_sumde;                         // sum of de over the tile (dv needs sum de (1 - 2r) = sum de - 2 sum de r)
 
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int b = blockIdx.y, t0 = p.t_begin + blockIdx.x * AT_TT;
     const int out_len = p.out_lens ? p.out_lens[b] : p.T;
     const int in_len = p.in_lens ? p.in_lens[b] : p.L;
     const int nrows = min(AT_TT, p.t_end - t0);
@@ -591,18 +607,32 @@ attn_bwd_kernel(AttnBwdParams p) {
 }
 
 // =================================================================================================== host
-static size_t attn_fwd_smem(int L, int A) {
+constexpr size_t kSmemPerBlock = 227 * 1024;     // H100 opt-in shared memory per block
+
+static size_t attn_fwd_smem(int L, int A, bool global_rows) {
     const int Lr = (L + 31) & ~31;
-    return sizeof(float) * (static_cast<size_t>(AT_AC) * SQ_LD + AT_AC * SK_LD + AT_TT * (Lr + 4) + A) + 64;
+    const size_t rows = global_rows ? 0 : static_cast<size_t>(AT_TT) * (Lr + 4);
+    return sizeof(float) * (static_cast<size_t>(AT_AC) * SQ_LD + AT_AC * SK_LD + rows + A) + 64;
 }
-static size_t attn_bwd_smem(int L, int A) {
+static size_t attn_bwd_smem(int L, int A, bool global_rows) {
     const int Lr = (L + 31) & ~31;
-    return sizeof(float) * (static_cast<size_t>(AT_AC) * SQ_LD + AT_AC * SK_LD + AT_TT * (Lr + 4) + 2 * A) + 64;
+    const size_t rows = global_rows ? 0 : static_cast<size_t>(AT_TT) * (Lr + 4);
+    return sizeof(float) * (static_cast<size_t>(AT_AC) * SQ_LD + AT_AC * SK_LD + rows + 2 * A) + 64;
+}
+
+// One rule for both directions (the backward needs A floats more): the shared-memory kernels run while the backward's rows
+// fit, i.e. up to L = 672 at A = 640.
+bool attn_rows_in_global(int L, int A) { return attn_bwd_smem(L, A, false) > kSmemPerBlock; }
+size_t attn_rows_floats(int T, int B, int L) {
+    const size_t Tp = (static_cast<size_t>(T) + AT_TT - 1) / AT_TT * AT_TT;
+    return static_cast<size_t>(B) * Tp * (((L + 31) & ~31) + 4);
 }
 
 int launch_attn_fwd(const AttnFwdArgs& a, cudaStream_t st) {
-    if (a.L > 512) return ft_set_error("attention: L > 512 not supported");
+    if (a.L > FT_MAX_TEXT_LEN) return ft_set_error("attention: L > FT_MAX_TEXT_LEN (1024) not supported");
     if (a.A % 4) return ft_set_error("attention: A must be a multiple of 4");
+    const bool global_rows = attn_rows_in_global(a.L, a.A);
+    if (global_rows && !a.rows) return ft_set_error("attention: this L needs the global row area (AttnFwdArgs::rows)");
     AttnFwdParams p;
     p.T = a.T; p.B = a.B; p.L = a.L; p.A = a.A;
     p.Q = a.Q; p.ldq = a.ldq; p.K = a.K; p.ldk = a.ldk; p.V = a.V; p.ldv = a.ldv; p.v = a.v;
@@ -610,19 +640,23 @@ int launch_attn_fwd(const AttnFwdArgs& a, cudaStream_t st) {
     p.inv_temperature = 1.0f / a.temperature;
     p.attn = a.attn; p.logprob = a.logprob; p.p_save = a.p_save;
     p.ctx16 = static_cast<__half*>(a.ctx16); p.ldc = a.ldc; p.ctx32 = a.ctx32; p.ldc32 = a.ldc32;
-    const size_t smem = attn_fwd_smem(a.L, a.A);
-    cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+    p.rows = a.rows;
+    const size_t smem = attn_fwd_smem(a.L, a.A, global_rows);
+    auto kern = global_rows ? attn_fwd_kernel<true> : attn_fwd_kernel<false>;
+    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
     p.t_begin = a.t_begin; p.t_end = a.t_end > 0 ? a.t_end : a.T;
     if (p.t_begin % AT_TT || p.t_begin < 0 || p.t_end > a.T || p.t_end <= p.t_begin) return ft_set_error("attention: bad query range");
     dim3 grid((p.t_end - p.t_begin + AT_TT - 1) / AT_TT, a.B);
     TimeScope ts("attn_fwd", p.t_end - p.t_begin, a.B, a.L, st);
-    attn_fwd_kernel<<<grid, AT_THREADS, smem, st>>>(p);
+    kern<<<grid, AT_THREADS, smem, st>>>(p);
     ft_count_launch(1);
     return ft_check_launch("attn_fwd_kernel");
 }
 
 int launch_attn_bwd(const AttnBwdArgs& a, cudaStream_t st) {
-    if (a.L > 256) return ft_set_error("attention backward: L > 256 not supported");
+    if (a.L > FT_MAX_TEXT_LEN) return ft_set_error("attention backward: L > FT_MAX_TEXT_LEN (1024) not supported");
+    const bool global_rows = attn_rows_in_global(a.L, a.A);
+    if (global_rows && !a.rows) return ft_set_error("attention backward: this L needs the global row area (AttnBwdArgs::rows)");
     AttnBwdParams p;
     p.T = a.T; p.B = a.B; p.L = a.L; p.A = a.A;
     p.Q = a.Q; p.ldq = a.ldq; p.K = a.K; p.ldk = a.ldk; p.V = a.V; p.ldv = a.ldv; p.v = a.v;
@@ -630,13 +664,15 @@ int launch_attn_bwd(const AttnBwdArgs& a, cudaStream_t st) {
     p.has_prior = a.p_save != nullptr; p.inv_temperature = 1.0f / a.temperature;
     p.dctx = a.dctx; p.lddc = a.lddc; p.dattn_ext = a.dattn_ext; p.dlp_ext = a.dlp_ext; p.scale = a.scale;
     p.dQ = a.dQ; p.lddq = a.lddq; p.dK = a.dK; p.lddk = a.lddk; p.dV = a.dV; p.lddv = a.lddv; p.dv = a.dv;
-    const size_t smem = attn_bwd_smem(a.L, a.A);
-    cudaFuncSetAttribute(attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+    p.rows = a.rows;
+    const size_t smem = attn_bwd_smem(a.L, a.A, global_rows);
+    auto kern = global_rows ? attn_bwd_kernel<true> : attn_bwd_kernel<false>;
+    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
     p.t_begin = a.t_begin; p.t_end = a.t_end > 0 ? a.t_end : a.T;
     if (p.t_begin % AT_TT || p.t_begin < 0 || p.t_end > a.T || p.t_end <= p.t_begin) return ft_set_error("attention backward: bad query range");
     dim3 grid((p.t_end - p.t_begin + AT_TT - 1) / AT_TT, a.B);
     TimeScope ts("attn_bwd", p.t_end - p.t_begin, a.B, a.L, st);
-    attn_bwd_kernel<<<grid, AT_THREADS, smem, st>>>(p);
+    kern<<<grid, AT_THREADS, smem, st>>>(p);
     ft_count_launch(1);
     return ft_check_launch("attn_bwd_kernel");
 }

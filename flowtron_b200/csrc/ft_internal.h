@@ -84,6 +84,7 @@ struct AttnFwdArgs {
     const int* in_lens; const int* out_lens; const float* prior; int reversed; float temperature;
     float* attn; float* logprob; float* p_save; void* ctx16; long long ldc; float* ctx32; long long ldc32;
     int t_begin = 0, t_end = 0;          // query rows of this launch (t_end == 0: all T; t_begin a multiple of 64)
+    float* rows = nullptr;               // attn_rows_in_global(L, A): attn_rows_floats(T, B, L) floats of scratch
 };
 struct AttnBwdArgs {
     int T, B, L, A;
@@ -93,7 +94,12 @@ struct AttnBwdArgs {
     const float* scale;      // device [2] = {S, 1/S}: external grads are multiplied by S, dv by 1/S (null = 1)
     float* dQ; long long lddq; float* dK; long long lddk; float* dV; long long lddv; float* dv;
     int t_begin = 0, t_end = 0;          // query rows of this launch (t_end == 0: all T; t_begin a multiple of 64); dK / dV / dv accumulate
+    float* rows = nullptr;               // attn_rows_in_global(L, A): attn_rows_floats(T, B, L) floats of scratch
 };
+// The attention kernels keep a 64-query tile's score / gradient rows in shared memory while they fit (L <= 672 at A = 640);
+// past that they keep them in a global area of attn_rows_floats(T, B, L) floats the caller passes as `rows`.
+bool attn_rows_in_global(int L, int A);
+size_t attn_rows_floats(int T, int B, int L);
 int launch_attn_fwd(const AttnFwdArgs& a, cudaStream_t st);
 int launch_attn_bwd(const AttnBwdArgs& a, cudaStream_t st);
 

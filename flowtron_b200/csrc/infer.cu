@@ -39,7 +39,8 @@ constexpr int INF_THREADS = 512, INF_WARPS = 16;
 constexpr int KMAX = 1664 + 1024;              // widest phase input: [d ; h0]
 constexpr int KP = KMAX + 32;                  // activation row pitch (halfs): 5440 B = 64 mod 128 -> conflict-free 16-byte reads
 constexpr int XPAD = 96;                       // the 80 mel channels of the attention LSTM's input, padded to 3 k-blocks
-constexpr int LMAX = 256;
+constexpr int LMAX = 256;                      // keys of the short-text kernels (one row of scores in registers per lane)
+constexpr int LMAX_LONG = FT_MAX_TEXT_LEN;     // keys of the long-text kernels (the row staged in shared memory)
 
 struct InferParams {
     int T, B, L, M, A, E, D;
@@ -386,17 +387,63 @@ __device__ __forceinline__ float residual_at(const InferParams& p, int i, int b,
     return p.residual[(static_cast<long long>(t) * p.B + b) * p.M + m];
 }
 
+// Long texts (kLong, L > LMAX): warp 0 runs the same softmax / prior posterior / forced alignment over the row staged in
+// shared memory, 32 keys per pass, instead of holding it in registers.  Each lane handles the same keys in the same order
+// as the register path, so the two agree bit for bit where both apply.
+__device__ __forceinline__ void attn_row_long(const InferParams& p, float* se, int i, int b, long long cur, bool forced, int Lb) {
+    const int lane = threadIdx.x & 31;
+    if (!forced) {
+        float mx = -INFINITY;
+        for (int l = lane; l < p.L; l += 32) {
+            const float x = l < Lb ? poll_f32(SL(p.e, cur) + b * p.L + l, p.status, 303) : -INFINITY;
+            se[l] = x;
+            mx = fmaxf(mx, x);
+        }
+#pragma unroll
+        for (int o = 16; o; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+        float sum = 0.f;
+        for (int l = lane; l < p.L; l += 32) { const float x = l < Lb ? expf(se[l] - mx) : 0.f; se[l] = x; sum += x; }
+#pragma unroll
+        for (int o = 16; o; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+        const float inv = 1.f / sum;
+        for (int l = lane; l < p.L; l += 32) se[l] *= inv;
+        if (p.prior) {
+            float m2 = -INFINITY;
+            for (int l = lane; l < Lb; l += 32) {
+                const float pr = p.prior[(static_cast<long long>(b) * p.T + i) * p.L + l];
+                const float x = logf(se[l] + 1e-20f) + logf(pr + 1e-20f);
+                se[l] = x;
+                m2 = fmaxf(m2, x);
+            }
+#pragma unroll
+            for (int o = 16; o; o >>= 1) m2 = fmaxf(m2, __shfl_xor_sync(0xffffffffu, m2, o));
+            float s2 = 0.f;
+            for (int l = lane; l < p.L; l += 32) { const float x = l < Lb ? expf(se[l] - m2) : 0.f; se[l] = x; s2 += x; }
+#pragma unroll
+            for (int o = 16; o; o >>= 1) s2 += __shfl_xor_sync(0xffffffffu, s2, o);
+            const float inv2 = 1.f / s2;
+            for (int l = lane; l < p.L; l += 32) se[l] *= inv2;
+        }
+    } else {
+        for (int l = lane; l < p.L; l += 32) se[l] = p.attn_forced[(static_cast<long long>(i) * p.B + b) * p.L + l];
+    }
+}
+
 // Context of utterance b, channels [CW s, CW s + CW) (CW = 64 or 128), inside one CTA: warp 0 turns the scores into attention weights (softmax,
 // prior posterior -- or the forced alignment), all 16 warps then take L/16 keys each (every V load of the CTA in flight at
 // once), partial sums meet in shared memory.  Writes ctx (fp16 for lstm layer 0, fp32 for the gate) and, from slice 0, the
 // attention weights.  (One CTA per utterance doing all 640 channels would pull 256 KB through one SM.)
-template <int CW>
+template <int CW, bool kLong>
 __device__ __forceinline__ void context_item(const InferParams& p, float* sf, int i, int b, int s, long long cur, long long nxt, bool forced) {
     constexpr int NV = CW / 32;                                    // channels per lane
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    float* se = sf; float* sp = sf + LMAX;                         // attn [LMAX], partials [16 warps][CW]
+    float* se = sf; float* sp = sf + (kLong ? LMAX_LONG : LMAX);   // attn [LMAX or LMAX_LONG], partials [16 warps][CW]
     const int Lb = p.in_lens ? p.in_lens[b] : p.L;                 // key mask: tokens l >= Lb get weight 0 (as if L were Lb)
-    if (warp == 0) {
+    if (kLong && warp == 0) {
+        attn_row_long(p, se, i, b, cur, forced, Lb);
+        if (s == 0)
+            for (int l = lane; l < p.L; l += 32) p.attn_out[(static_cast<long long>(i) * p.B + b) * p.L + l] = se[l];
+    } else if (warp == 0) {
         float w[8];
         if (!forced) {                                            // softmax over L in registers: lane holds l = lane + 32 jj
             float mx = -INFINITY;
@@ -493,13 +540,14 @@ __device__ __forceinline__ void context_item(const InferParams& p, float* sf, in
     __syncthreads();
 }
 
-template <bool kB16>
-__global__ void __launch_bounds__(INF_THREADS, 1)
-infer_kernel(InferParams p) {
+// kLong: texts of LMAX < L <= LMAX_LONG keys (context_item's softmax over a shared-memory row): infer_long_kernel.  The
+// L <= LMAX instantiations are infer_kernel, the short-text kernels.
+template <bool kB16, bool kLong>
+__device__ __forceinline__ void infer_body(const InferParams& p) {
     extern __shared__ __align__(16) uint8_t smem_raw[];
     __half* sx = reinterpret_cast<__half*>(smem_raw);                          // [16][KP] fp16 activations of the phase
     float* spart = reinterpret_cast<float*>(sx + 16 * KP);                     // [16 warps][32 lanes][4] partial accumulators
-    float* sf = spart + INF_WARPS * 128;                                       // attention scratch: attn[LMAX], partials[16][128]
+    float* sf = spart + INF_WARPS * 128;                                       // attention scratch: attn[LMAX or LMAX_LONG], partials[16][128]
     __shared__ int s_alive[16], s_nfr[16];                                     // every CTA tracks every sample's gate state
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     for (int i = threadIdx.x; i < 16 * KP; i += INF_THREADS) sx[i] = __float2half_rn(0.f);     // batch rows >= B: zero forever
@@ -593,8 +641,8 @@ infer_kernel(InferParams p) {
             IT_TRACE(6);
         }
         // ---- P3b softmax + context, one (utterance, channel slice) item per CTA
-        if (wide_ctx) { for (int it = blockIdx.x; it < p.B * (p.A / 128); it += gridDim.x) context_item<128>(p, sf, i, it / (p.A / 128), it % (p.A / 128), cur, nxt, forced); }
-        else          { for (int it = blockIdx.x; it < p.B * (p.A / 64); it += gridDim.x) context_item<64>(p, sf, i, it / (p.A / 64), it % (p.A / 64), cur, nxt, forced); }
+        if (wide_ctx) { for (int it = blockIdx.x; it < p.B * (p.A / 128); it += gridDim.x) context_item<128, kLong>(p, sf, i, it / (p.A / 128), it % (p.A / 128), cur, nxt, forced); }
+        else          { for (int it = blockIdx.x; it < p.B * (p.A / 64); it += gridDim.x) context_item<64, kLong>(p, sf, i, it / (p.A / 64), it % (p.A / 64), cur, nxt, forced); }
         IT_TRACE(7);
         // ---- P4 lstm layer 0 on [hA ; ctx ; h0_{i-1}]
         lstm_pre(p, p.b0, p.c0, cpre, bpre);
@@ -719,6 +767,14 @@ infer_kernel(InferParams p) {
     }
 }
 
+template <bool kB16>
+__global__ void __launch_bounds__(INF_THREADS, 1)
+infer_kernel(InferParams p) { infer_body<kB16, false>(p); }
+
+template <bool kB16>
+__global__ void __launch_bounds__(INF_THREADS, 1)
+infer_long_kernel(InferParams p) { infer_body<kB16, true>(p); }
+
 // ------------------------------------------------------------------------------------------------ weight packing
 // dst[task][m][n][kk] (fp16) <- W[row(task, n)][32 m + kk] over the virtual K = [A part (Ka real columns, padded to Kap) ; B part]
 //   kind 0: LSTM      row = (n % 4) * 1024 + 2 task + n / 4        (rows i0,f0,g0,o0,i1,f1,g1,o1)
@@ -814,7 +870,7 @@ static int infer_impl(const FtArStepDesc* d, const FtArStepWeights* w, const flo
                       const float* attn_prior, const float* attn_forced, const int* in_lens, const int* frame_lens, int reversed,
                       float gate_threshold, float* out, float* attn_out, int* n_frames, void* scratch, void* stream) {
     if (d->n_hidden != IH) return ft_set_error("infer: n_hidden must be 1024");
-    if (d->L > LMAX) return ft_set_error("infer: L > 256 not supported");
+    if (d->L > LMAX_LONG) return ft_set_error("infer: L > FT_MAX_TEXT_LEN (1024) not supported");
     if (d->B > 16) return ft_set_error("infer: batch > 16 per call not supported (run the batch in slices of 16)");
     if (d->n_mel > XPAD || d->n_mel % 8 || d->n_attn % 64 || d->n_text % 8 || d->n_attn > 4 * INF_THREADS)
         return ft_set_error("infer: n_mel <= 96 and %8, n_attn %64 and <= 2048, n_text %8 required");
@@ -888,8 +944,10 @@ static int infer_impl(const FtArStepDesc* d, const FtArStepWeights* w, const flo
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     if (sms < B) return ft_set_error("infer: fewer SMs than utterances");
-    void* fn = B > 8 ? reinterpret_cast<void*>(infer_kernel<true>) : reinterpret_cast<void*>(infer_kernel<false>);
-    const int smem = 16 * KP * 2 + INF_WARPS * 128 * 4 + (LMAX + INF_WARPS * 128 + 64) * 4;
+    const bool long_text = d->L > LMAX;
+    void* fn = long_text ? (B > 8 ? reinterpret_cast<void*>(infer_long_kernel<true>) : reinterpret_cast<void*>(infer_long_kernel<false>))
+                         : (B > 8 ? reinterpret_cast<void*>(infer_kernel<true>) : reinterpret_cast<void*>(infer_kernel<false>));
+    const int smem = 16 * KP * 2 + INF_WARPS * 128 * 4 + ((long_text ? LMAX_LONG : LMAX) + INF_WARPS * 128 + 64) * 4;
     cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     TimeScope ts("infer", d->T, B, d->L, st);
     void* args[] = {&p};

@@ -392,6 +392,7 @@ class AR_Step(nn.Module):
                 None if gate is None else gate.linear_layer.weight, None if gate is None else gate.linear_layer.bias]
 
     def _run(self, mel, text, mask, out_lens, attn_prior, reversed_flag, text_ready):
+        _lib.check_text_len(text.size(0), "AR_Step")
         dev = mel.device
         in_lens = None
         if mask is not None:
@@ -551,8 +552,10 @@ class Flowtron(nn.Module):
         return torch.cat([text, speaker_vecs.expand(text.size(0), -1, -1)], 2)
 
     def forward(self, mel, speaker_ids, text, in_lens, out_lens, attn_prior=None):
+        """Texts of up to _lib.MAX_TEXT_LEN (1024) tokens; longer ones raise ValueError before any work."""
         mean, log_var, prob = None, None, None
         n_text = text.size(1)
+        _lib.check_text_len(n_text, "Flowtron.forward")
         B = mel.size(0)
         # The first flow needs the text encoding only after its attention LSTM (T dependent steps that read mel alone), so
         # the encoder's ~700 small latency-bound kernels can run on a second stream underneath it; the flow's C entry
@@ -591,6 +594,8 @@ class Flowtron(nn.Module):
         return (*out, mean, log_var, prob)
 
     def infer(self, residual, speaker_ids, text, temperature=1.0, gate_threshold=0.5, attns=None, attn_prior=None):
+        """Texts of up to _lib.MAX_TEXT_LEN (1024) tokens; longer ones raise ValueError before any work."""
+        _lib.check_text_len(text.size(-1), "Flowtron.infer")
         speaker_ids = speaker_ids * 0 if self.dummy_speaker_embedding else speaker_ids
         speaker_vecs = self.speaker_embedding(speaker_ids)
         text = self.encoder.infer_tokens(text, self.embedding).transpose(0, 1)
@@ -633,7 +638,7 @@ class Flowtron(nn.Module):
         if text.size(0) != B or speaker_ids.size(0) != B or B < 1 or T < 1 or L < 1:
             raise ValueError(f"batch sizes disagree or are empty: residual {tuple(residual.shape)}, "
                              f"speaker_ids {tuple(speaker_ids.shape)}, text {tuple(text.shape)}")
-        if L > 256:
+        if L > 256:             # the ragged entry point is validated up to 256 tokens; infer takes up to MAX_TEXT_LEN
             raise ValueError(f"text length {L} > 256 is not supported by the inference kernel")
         in_lens = _ragged_lengths(in_lens, B, L, "in_lens")
         max_frames = _ragged_lengths([T] * B if max_frames is None else max_frames, B, T, "max_frames")

@@ -15,7 +15,10 @@ def ar_step_infer(step, residual, text, attns, attn_prior=None, reversed_flag=Fa
 
     ``attns`` (forced alignments, flowtron.py:585-588, 797): frame i uses ``attns[i]`` instead of scoring -- a [T, L] tensor
     (B == 1, the reference's ``attns[i][None, None]``), a [T, B, L] tensor, or the list of T per-frame weights this
-    function returns ([B, 1, L] each).  Like the reference, a back step consumes them in its own (flipped) time order."""
+    function returns ([B, 1, L] each).  Like the reference, a back step consumes them in its own (flipped) time order.
+
+    L <= _lib.MAX_TEXT_LEN (1024): texts of up to 256 tokens run the short-text kernel, longer ones the long-text kernel."""
+    _lib.check_text_len(text.size(0), "AR_Step.infer")
     if not residual.is_cuda:
         raise FlowtronB200Error("AR_Step.infer needs CUDA tensors: the sm_90a kernel is the only implementation")
     T, B, M = residual.shape

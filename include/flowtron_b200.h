@@ -21,7 +21,13 @@ extern "C" {
 #define FT_BF16 1
 #define FT_TF32 2   /* fp32 storage, tf32 tensor-core math */
 
+/* Longest text (tokens, the padded L of FtArStepDesc) the flow-step kernels take, training and inference.  Texts of up to
+ * 256 tokens run the short-text kernel variants; longer ones the long-text variants (DESIGN.md 4.16).  The Python layer
+ * mirrors it as flowtron_b200._lib.MAX_TEXT_LEN; ft_max_text_len() returns it. */
+#define FT_MAX_TEXT_LEN 1024
+
 int ft_version(void);
+int ft_max_text_len(void);
 const char* ft_last_error(void);
 /* 0 = ok; non-zero = code written by a device-side watchdog (a bounded spin-wait expired). Synchronises. */
 int ft_device_status(void);
@@ -71,7 +77,7 @@ int ft_lstm_bwd(int T, int B, const float* dh_ext, long long ldd, const void* wh
  * AR_Step / AR_Back_Step (flowtron.py:595-828): one autoregressive flow step, training direction.
  * ---------------------------------------------------------------------------------------------------- */
 typedef struct {
-    int T, B, L;        /* mel frames (padded max), batch, text tokens (padded max) */
+    int T, B, L;        /* mel frames (padded max), batch, text tokens (padded max, <= FT_MAX_TEXT_LEN) */
                         /* B <= 32 per training call (ft_ar_step_infer: <= 16)      */
     int n_mel;          /* 80  (n_mel_channels, <= 128)                             */
     int n_hidden;       /* 1024 (must be 1024 in this build)                        */
@@ -175,7 +181,8 @@ int ft_step_increment(int* step_dev, void* stream);
  *   residual [T,B,M] f32 in flow-time order (the caller flips for AR_Back_Step, :629-642), text [L,B,E] f32,
  *   attn_prior [B,T,L] or NULL (row i is used at frame i); attn_forced [T,B,L] or NULL: forced alignments (the `attns`
  *   argument, flowtron.py:585-588, 797: scoring, softmax and the prior are skipped, context = attn_forced[i] . V).
- *   Uses d->T/B/L/n_*, has_gate, has_prior, temperature.
+ *   Uses d->T/B/L/n_*, has_gate, has_prior, temperature.  B <= 16, L <= FT_MAX_TEXT_LEN (texts over 256 tokens run the
+ *   long-text kernel variant, which stages the row of scores in shared memory).
  *   out [T,B,M]: generated frames (zeros after a sample's gate fired; the frame that trips the gate is emitted),
  *   attn_out [T,B,L]: per-frame attention weights, n_frames [B] int32: frames emitted per sample.
  *   With B == 1 this is exactly the reference's loop-with-break; B > 1 with a gate is the per-sample-stop
@@ -196,7 +203,8 @@ int ft_ar_step_infer(const FtArStepDesc* d, const FtArStepWeights* w, const floa
  *   out [T,B,M]: zero at t >= n_frames[b]; attn_out [T,B,L] in generation order, zero at i >= n_frames[b] and l >= in_lens[b];
  *   n_frames [B] int32 = min(gate stop (the frame that trips the gate is emitted), frame_lens[b]).
  *   Lengths must satisfy 1 <= in_lens[b] <= L and 1 <= frame_lens[b] <= T; they are read on the device only.
- *   Limits as ft_ar_step_infer: B <= 16, L <= 256; d->has_prior must be 0 (no attn_prior, no forced alignments).
+ *   Limits as ft_ar_step_infer: B <= 16, L <= FT_MAX_TEXT_LEN; d->has_prior must be 0 (no attn_prior, no forced
+ *   alignments).  Flowtron.infer_batch, the host layer over this entry point, takes texts of up to 256 tokens.
  *   Two launches (the persistent kernel, then a small per-row flip / attention clear), no host synchronisation:
  *   CUDA-graph capturable. */
 int ft_ar_step_infer_ragged(const FtArStepDesc* d, const FtArStepWeights* w, const float* residual, const float* text,
