@@ -125,6 +125,18 @@ int ft_gemm(int M, int N, int K, const void* A, long long lda, int a_fmt, int a_
 /* debug: device buffer [T][8] receiving clock64 stamps of CTA 0 of the next lstm_fwd launches (NULL disables) */
 void ft_debug_set_lstm_trace(long long* buf) { ft::set_lstm_trace(buf); }
 
+/* debug: how many 4-CTA clusters of the BPTT cluster kernel fit on the device at its launch configuration for batch B
+   (cudaOccupancyMaxActiveClusters), or -1 */
+int ft_debug_lstm_bwd_max_clusters(int B) { return ft::lstm_bwd_max_clusters(B); }
+
+/* debug: steps [t0, t1) of one layer-pipeline BPTT chunk, on the flat kernel (xchg non-null) or the cluster kernel (NULL) */
+int ft_debug_lstm_bwd_chunk(int T, int B, int t0, int t1, const float* dh_ext, long long ldd, const void* whhT16,
+                            const void* gates16, const float* cstate, const int* lens, void* dG16, float* dc_carry, int* flags,
+                            float* xchg, void* stream) {
+    return ft::launch_lstm_bwd_chunk(T, B, t0, t1, dh_ext, ldd, whhT16, gates16, cstate, lens, dG16, dc_carry, flags, xchg,
+                                     static_cast<cudaStream_t>(stream));
+}
+
 void ft_set_gemm_pair_mode(int mode) { ft::set_gemm_pair_mode(mode); }
 
 int ft_lstm_fwd(int T, int B, const float* xproj, const void* whh16, const int* lens, void* hseq16, long long ldh,

@@ -102,6 +102,7 @@ constexpr int kLayerChunk = 100;
 constexpr int kAttnChunk = 256;
 
 static int layer_chunk(int T) { return T < kLayerChunk ? T : kLayerChunk; }
+constexpr int kBwdXchgPerRow = 2 * 16 * 4 * 64;   // flat BPTT partial-sum ring, floats per batch row: [2][16 groups][4 ranks][B][64]
 
 struct FwdScratch {
     W16 w;
@@ -143,6 +144,7 @@ struct BwdScratch {
     float *dh, *dQ, *dK, *dV, *dmel_in;
     int* flags;
     float *dcarry1, *dcarry0;   // dc*f hand-over between BPTT chunks of the layer pipeline
+    float *xchg1, *xchg0;       // partial-sum rings of the two pipelined BPTT recurrences (flat kernel, lstm.cu)
     float* attn_rows = nullptr; // long texts: the attention backward's gradient rows (attn_rows_in_global)
     void plan(Plan& p, const FtArStepDesc& d) {
         const Dims n(d);
@@ -161,10 +163,13 @@ struct BwdScratch {
         dK = p.get<float>("dK", n.RL * n.A);
         dV = p.get<float>("dV", n.RL * n.A);
         dmel_in = p.get<float>("dmel_in", n.R * n.M);
-        // 64 per step: T steps for the attention LSTM's BPTT, one chunk for each of the layer pipeline's two recurrences
-        flags = p.get<int>("flags", static_cast<size_t>(std::max(n.T, 2 * layer_chunk(n.T))) * 64);
+        // 64 per step for the attention LSTM's BPTT (T steps), 128 per step for one chunk of each of the layer pipeline's two
+        // recurrences (dG release + partial-sum exchange flags)
+        flags = p.get<int>("flags", std::max(static_cast<size_t>(n.T) * 64, static_cast<size_t>(2 * layer_chunk(n.T)) * 128));
         dcarry1 = p.get<float>("dcarry1", static_cast<size_t>(n.B) * H);
         dcarry0 = p.get<float>("dcarry0", static_cast<size_t>(n.B) * H);
+        xchg1 = p.get<float>("xchg1", static_cast<size_t>(kBwdXchgPerRow) * n.B);
+        xchg0 = p.get<float>("xchg0", static_cast<size_t>(kBwdXchgPerRow) * n.B);
         if (attn_rows_in_global(n.L, n.A)) attn_rows = p.get<float>("attn_rows", attn_rows_floats(n.T, n.B, n.L));
     }
 };
@@ -504,7 +509,7 @@ int ar_step_bwd_main(const FtArStepDesc& d, const FtArStepWeights& w, const floa
     if (!pp) return ft_set_error("ar_step_bwd: could not create the pipeline streams");
     const int CH = layer_chunk(n.T);
     int* flagsA = F.flags;
-    int* flagsB = F.flags + static_cast<size_t>(CH) * 64;
+    int* flagsB = F.flags + static_cast<size_t>(CH) * 128;
     cudaStream_t sr = pp->sA;                                    // layer 1's BPTT stream
     cudaEventRecord(pp->ev0, st);
     cudaStreamWaitEvent(sr, pp->ev0, 0);
@@ -514,13 +519,13 @@ int ar_step_bwd_main(const FtArStepDesc& d, const FtArStepWeights& w, const floa
     for (int c = n_chunks - 1; c >= 0; --c) {
         const int t0 = c * CH, t1 = t0 + CH < n.T ? t0 + CH : n.T;
         const long long r0 = static_cast<long long>(t0) * n.B, rows = static_cast<long long>(t1 - t0) * n.B;
-        FT_TRY(launch_lstm_bwd_chunk(n.T, n.B, t0, t1, F.dh, H, F.w.w_hh1, S_.gates1, S_.c1, out_lens, F.dG1, F.dcarry1, flagsA, sr));
+        FT_TRY(launch_lstm_bwd_chunk(n.T, n.B, t0, t1, F.dh, H, F.w.w_hh1, S_.gates1, S_.c1, out_lens, F.dG1, F.dcarry1, flagsA, F.xchg1, sr));
         cudaEventRecord(pp->evA, sr);
         cudaStreamWaitEvent(pp->sC, pp->evA, 0);
         FT_TRY(gemm_dgrad(pp->sC, rows, H, G, F.dG1 + r0 * G, G, F.w.w_ih1, H, 0, F.dh + r0 * H, H, nullptr, 0, nullptr, 0));
         cudaEventRecord(pp->evG, pp->sC);
         cudaStreamWaitEvent(pp->sB, pp->evG, 0);
-        FT_TRY(launch_lstm_bwd_chunk(n.T, n.B, t0, t1, F.dh, H, F.w.w_hh0, S_.gates0, S_.c0, out_lens, F.dG0, F.dcarry0, flagsB, pp->sB));
+        FT_TRY(launch_lstm_bwd_chunk(n.T, n.B, t0, t1, F.dh, H, F.w.w_hh0, S_.gates0, S_.c0, out_lens, F.dG0, F.dcarry0, flagsB, F.xchg0, pp->sB));
     }
     // layer-1 weight gradients run under the tail of layer 0 (side stream forks from st = all of layer 1 done)
     cudaEventRecord(pp->evJ, sr);

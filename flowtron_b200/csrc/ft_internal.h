@@ -50,7 +50,8 @@ int launch_lstm_fwd_chunk(int T, int B, int t0, int t1, const float* xproj, cons
                           long long ldh, void* gates16, float* cstate, int* flags, cudaStream_t st, float* h32 = nullptr,
                           long long ldh32 = 0);
 int launch_lstm_bwd_chunk(int T, int B, int t0, int t1, const float* dh_ext, long long ldd, const void* whhT16, const void* gates16,
-                          const float* cstate, const int* lens, void* dG16, float* dc_carry, int* flags, cudaStream_t st);   // experimental
+                          const float* cstate, const int* lens, void* dG16, float* dc_carry, int* flags, float* xchg, cudaStream_t st);
+int lstm_bwd_max_clusters(int B);
 int launch_lstm_bwd(int T, int B, const float* dh_ext, long long ldd, const void* whhT16, const void* gates16,
                     const float* cstate, const int* lens, void* dG16, int* flags, cudaStream_t st);
 

@@ -20,6 +20,8 @@
 //     the release so they stay off the critical path.
 // Backward (lstm_bwd4_kernel), 16 clusters of 4 CTAs: dh_{t-1} = dG_t W_hh split over the four gates, the pointwise
 //   LSTM backward in the epilogue; dG ([B,4096] fp16, loss-scaled) is written once and reused by the wgrad/dgrad GEMMs.
+//   lstm_bwd_flat_kernel is the same computation without clusters (partial sums exchanged through L2) for the layer
+//   pipeline's chunks, whose two concurrent launches do not fit on an H100 as 4-CTA clusters.
 //
 // Every kernel here takes at most 32 batch rows per launch (one 32-row wgmma tile); larger batches are split by the caller.
 //
@@ -115,25 +117,33 @@ struct LstmBwdChunkParams {
     int* flags;
     int* status;
     long long* trace;
-    int t0, t1;                // steps [t0, t1); flags: [(t1 - t0) * 64] ints, zeroed by the launcher
+    int t0, t1;                // steps [t0, t1); flags: [(t1 - t0) * 64] ints (flat kernel: [(t1 - t0) * 128]), zeroed by the launcher
     float* dc_carry;           // [B, 1024]
+    float* xchg;               // flat kernel: partial-sum ring [2 parities][16 groups][4 ranks][B][64] fp32
 };
 
-__global__ void __launch_bounds__(LSTM_THREADS, 1)
-lstm_bwd4_kernel(const __grid_constant__ CUtensorMap tmWT, const __grid_constant__ CUtensorMap tmG, LstmBwdChunkParams p) {
+// ------------------------------------------------------------------------------------------- backward, split-K flat
+// lstm_bwd_flat_kernel: the same work split with no cluster -- CTA 4g + r plays rank r of group g.  A plain cooperative launch
+// of 64 CTAs places them on any 64 SMs, so the layer pipeline's two BPTT chunks fit side by side; 4-CTA clusters must each fit
+// in one GPC, and 32 of them (two chunks) do not reliably fit on an H100 (DESIGN §4.2).  The DSMEM exchange becomes an L2 one:
+// each rank stores its whole fp32 partial [B, 64] to the ring `xchg` and releases one flag per (step, group, rank) (flags
+// [(t1 - t0) * 64, (t1 - t0) * 128)); the rank that finishes units [64g + 16r, +16) acquires the other three ranks' flags and
+// reads its slice of all four partials from L2, summing them in the cluster kernel's order (bit-identical results).
+template <bool kFlat>
+__device__ __forceinline__ void lstm_bwd_body(const CUtensorMap& tmWT, const CUtensorMap& tmG, const LstmBwdChunkParams& p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     const int slot_bytes = p.Bbox * 128;
     uint8_t* sA = smem;                                          // [16 chunks][Bbox rows][128 B]
     uint8_t* sW = smem + B4_NCH * slot_bytes;                    // [16 chunks][64 rows][128 B]
     float* sPart = reinterpret_cast<float*>(sW + B4_W_BYTES);    // received partial sums: [2 parities][4 source ranks][16 units][B4_UP]
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sPart + B4_XCHG_FLOATS);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sPart + (kFlat ? 0 : B4_XCHG_FLOATS));
     uint64_t* full = bars;                       // [2]
     uint64_t* wbar = bars + 2;
     uint64_t* part_bar = bars + 4;               // [2] : 4 cluster-scope arrivals each
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int rank = static_cast<int>(cluster_ctarank());
+    const int rank = kFlat ? static_cast<int>(blockIdx.x % B4_CLUSTER) : static_cast<int>(cluster_ctarank());
     const int cl = blockIdx.x / B4_CLUSTER;
     constexpr int GS = 8, NG = B4_NCH / GS;
     const bool top = p.t1 == p.T;                                // the chunk that holds the last time step
@@ -144,10 +154,11 @@ lstm_bwd4_kernel(const __grid_constant__ CUtensorMap tmWT, const __grid_constant
         tma_prefetch_desc(&tmG);
         mbar_init(&full[0], 1); mbar_init(&full[1], 1);
         mbar_init(wbar, 1);
-        mbar_init(&part_bar[0], B4_CLUSTER); mbar_init(&part_bar[1], B4_CLUSTER);
+        if (!kFlat) { mbar_init(&part_bar[0], B4_CLUSTER); mbar_init(&part_bar[1], B4_CLUSTER); }
         fence_mbar_init();
     }
-    cluster_sync_all();                                          // every rank's barriers exist before any remote arrive
+    if (kFlat) __syncthreads();
+    else cluster_sync_all();                                     // every rank's barriers exist before any remote arrive
 
     if (warp == PRODUCER_WARP) {
         if (lane == 0) {
@@ -237,26 +248,51 @@ lstm_bwd4_kernel(const __grid_constant__ CUtensorMap tmWT, const __grid_constant
                     if (et == 0) FT_TRACE(p, t, 4);
                     // fragment rows 16 q + lane / 4 (+ 8) = units of rank q, columns = batch rows 8 j + 2 (lane % 4) (+ 1)
                     const int u = lane >> 2, b = 2 * (lane & 3);
-                    const uint32_t dst = mapa_shared(smem_u32(sPart) + static_cast<uint32_t>((((par * 4 + rank) * 16 + u) * B4_UP + b) * 4), q);
+                    if (kFlat) {                                  // the whole partial [B][64] to this rank's ring slot
+                        float* dst = p.xchg + static_cast<long long>((par * 16 + cl) * 4 + rank) * p.B * B4_UNITS + 16 * q + u;
 #pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        st_dsmem_f2(dst + 32 * j, acc[4 * j], acc[4 * j + 1]);
-                        st_dsmem_f2(dst + (8 * B4_UP + 8 * j) * 4, acc[4 * j + 2], acc[4 * j + 3]);
+                        for (int j = 0; j < 4; ++j) {
+                            const int bj = 8 * j + b;
+                            if (bj < p.B) { dst[bj * B4_UNITS] = acc[4 * j]; dst[bj * B4_UNITS + 8] = acc[4 * j + 2]; }
+                            if (bj + 1 < p.B) { dst[(bj + 1) * B4_UNITS] = acc[4 * j + 1]; dst[(bj + 1) * B4_UNITS + 8] = acc[4 * j + 3]; }
+                        }
+                    } else {
+                        const uint32_t dst = mapa_shared(smem_u32(sPart) + static_cast<uint32_t>((((par * 4 + rank) * 16 + u) * B4_UP + b) * 4), q);
+#pragma unroll
+                        for (int j = 0; j < 4; ++j) {
+                            st_dsmem_f2(dst + 32 * j, acc[4 * j], acc[4 * j + 1]);
+                            st_dsmem_f2(dst + (8 * B4_UP + 8 * j) * 4, acc[4 * j + 2], acc[4 * j + 3]);
+                        }
                     }
                 }
                 if (et == 64) FT_TRACE(p, t, 6);
                 epi_bar();
-                // publish: one release-arrive on every rank's barrier, issued by 4 different threads so the four
-                // cluster-scope releases overlap (issued serially by one thread they would queue behind each other)
-                if (et < B4_CLUSTER) mbar_arrive_cluster(mapa_shared(smem_u32(&part_bar[par]), et));
-                mbar_wait_cluster(&part_bar[par], (rs >> 1) & 1, p.status, 236);
+                if (kFlat) {
+                    // publish this rank's partial (gpu-scope release, cumulative over the CTA's stores ordered by the barrier),
+                    // then acquire the three other ranks' flags in parallel; the ring is read from L2 (ld.cg) below
+                    int* xf = p.flags + static_cast<long long>(p.t1 - p.t0 + t - p.t0) * BWD_NCH + cl * B4_CLUSTER;
+                    if (et == 0) red_release_add(&xf[rank], 1);
+                    if (et < B4_CLUSTER && et != rank) wait_flag_ge(&xf[et], 1, p.status, 237);
+                    epi_bar();
+                } else {
+                    // publish: one release-arrive on every rank's barrier, issued by 4 different threads so the four
+                    // cluster-scope releases overlap (issued serially by one thread they would queue behind each other)
+                    if (et < B4_CLUSTER) mbar_arrive_cluster(mapa_shared(smem_u32(&part_bar[par]), et));
+                    mbar_wait_cluster(&part_bar[par], (rs >> 1) & 1, p.status, 236);
+                }
                 if (et == 0) FT_TRACE(p, t, 1);               // all partials visible
                 if (has_item) {
 #pragma unroll
                     for (int rr = 0; rr < B4_CLUSTER; ++rr) {
-                        const float* src = sPart + ((par * 4 + rr) * 16 + 4 * uq) * B4_UP + ib;
+                        if (kFlat) {
+                            const float4 v = __ldcg(reinterpret_cast<const float4*>(
+                                p.xchg + (static_cast<long long>((par * 16 + cl) * 4 + rr) * p.B + ib) * B4_UNITS + B4_OWN * rank + 4 * uq));
+                            rec[0] += v.x; rec[1] += v.y; rec[2] += v.z; rec[3] += v.w;
+                        } else {
+                            const float* src = sPart + ((par * 4 + rr) * 16 + 4 * uq) * B4_UP + ib;
 #pragma unroll
-                        for (int j = 0; j < 4; ++j) rec[j] += src[j * B4_UP];
+                            for (int j = 0; j < 4; ++j) rec[j] += src[j * B4_UP];
+                        }
                     }
                 }
             }
@@ -306,7 +342,17 @@ lstm_bwd4_kernel(const __grid_constant__ CUtensorMap tmWT, const __grid_constant
             *reinterpret_cast<float4*>(p.dc_carry + static_cast<long long>(ib) * LH + B4_UNITS * cl + B4_OWN * rank + 4 * uq) =
                 make_float4(dcs[0], dcs[1], dcs[2], dcs[3]);
     }
-    cluster_sync_all();                                          // nobody exits while a peer may still read its partials
+    if (!kFlat) cluster_sync_all();                              // nobody exits while a peer may still read its partials
+}
+
+__global__ void __launch_bounds__(LSTM_THREADS, 1)
+lstm_bwd4_kernel(const __grid_constant__ CUtensorMap tmWT, const __grid_constant__ CUtensorMap tmG, LstmBwdChunkParams p) {
+    lstm_bwd_body<false>(tmWT, tmG, p);
+}
+
+__global__ void __launch_bounds__(LSTM_THREADS, 1)
+lstm_bwd_flat_kernel(const __grid_constant__ CUtensorMap tmWT, const __grid_constant__ CUtensorMap tmG, LstmBwdChunkParams p) {
+    lstm_bwd_body<true>(tmWT, tmG, p);
 }
 
 
@@ -672,12 +718,14 @@ int launch_lstm_fwd_chunk(int T, int B, int t0, int t1, const float* xproj, cons
     return launch_fwd_t<16, false>(T, B, t0, t1, xproj, whh16, lens, hseq16, ldh, gates16, cstate, h32, ldh32, flags, st);
 }
 
-// Steps [t0, t1) of a layer's BPTT with the split-K cluster kernel.  `flags` needs (t1 - t0) * 64 ints; `dc_carry`
-// ([B,1024] fp32) is only touched when the range is a proper chunk.
-static int launch_bwd4(int T, int B, int t0, int t1, const float* dh_ext, long long ldd, const void* whhT16, const void* gates16,
-                       const float* cstate, const int* lens, void* dG16, float* dc_carry, int* flags, cudaStream_t st) {
+// Steps [t0, t1) of a layer's BPTT.  Cluster kernel (xchg == null): `flags` needs (t1 - t0) * 64 ints.  Flat kernel: `flags`
+// needs (t1 - t0) * 128 ints and `xchg` 2 * 16 * 4 * B * 64 floats.  `dc_carry` ([B,1024] fp32) is only touched when the
+// range is a proper chunk.
+static int launch_bwd(int T, int B, int t0, int t1, const float* dh_ext, long long ldd, const void* whhT16, const void* gates16,
+                      const float* cstate, const int* lens, void* dG16, float* dc_carry, int* flags, float* xchg, cudaStream_t st) {
+    const bool flat = xchg != nullptr;
     LstmBwdChunkParams p;
-    p.T = T; p.B = B; p.Bbox = (B + 7) & ~7; p.t0 = t0; p.t1 = t1; p.dc_carry = dc_carry;
+    p.T = T; p.B = B; p.Bbox = (B + 7) & ~7; p.t0 = t0; p.t1 = t1; p.dc_carry = dc_carry; p.xchg = xchg;
     const int slot = p.Bbox * 128;
     p.dh_ext = dh_ext; p.ldd = ldd; p.gates = static_cast<const __half*>(gates16); p.cstate = cstate; p.lens = lens;
     p.dG = static_cast<__half*>(dG16); p.flags = flags; p.status = ft_status_word();
@@ -685,7 +733,19 @@ static int launch_bwd4(int T, int B, int t0, int t1, const float* dh_ext, long l
     CUtensorMap tmWT, tmG;
     if (make_tmap_2d(&tmWT, whhT16, FMT_F16, LH, LG, LG, KCH, B4_UNITS)) return -1;
     if (make_tmap_chunks(&tmG, dG16, static_cast<long long>(T) * B, BWD_NCH, LG, p.Bbox, 8)) return -1;
-    if (cudaMemsetAsync(flags, 0, sizeof(int) * (t1 - t0) * BWD_NCH, st) != cudaSuccess) return ft_set_error("lstm_bwd: memset failed");
+    if (cudaMemsetAsync(flags, 0, sizeof(int) * (t1 - t0) * BWD_NCH * (flat ? 2 : 1), st) != cudaSuccess)
+        return ft_set_error("lstm_bwd: memset failed");
+    if (flat) {
+        const int smem = B4_NCH * slot + B4_W_BYTES + 256 + 1024;
+        cudaFuncSetAttribute(lstm_bwd_flat_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+        TimeScope ts("lstm_bwd", t1 - t0, B, 0, st);
+        void* args[] = {&tmWT, &tmG, &p};
+        cudaError_t e = cudaLaunchCooperativeKernel(reinterpret_cast<void*>(lstm_bwd_flat_kernel), dim3(B4_CTAS), dim3(LSTM_THREADS),
+                                                    args, smem, st);
+        if (e != cudaSuccess) return ft_set_error(cudaGetErrorString(e));
+        ft_count_launch(1);
+        return ft_check_launch("lstm_bwd_flat_kernel");
+    }
     const int smem = B4_NCH * slot + B4_W_BYTES + B4_XCHG_FLOATS * 4 + 256 + 1024;
     cudaFuncSetAttribute(lstm_bwd4_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     cudaLaunchConfig_t cfg = {};
@@ -708,18 +768,36 @@ static int launch_bwd4(int T, int B, int t0, int t1, const float* dh_ext, long l
     return ft_check_launch("lstm_bwd4_kernel");
 }
 
-int launch_lstm_bwd_chunk(int T, int B, int t0, int t1, const float* dh_ext, long long ldd, const void* whhT16, const void* gates16,
-                          const float* cstate, const int* lens, void* dG16, float* dc_carry, int* flags, cudaStream_t st) {
-    if (T <= 0 || B <= 0 || t1 <= t0) return 0;
-    if (B > 32 || t0 < 0 || t1 > T || !dc_carry) return ft_set_error("lstm_bwd_chunk: bad batch, step range or carry buffer");
-    return launch_bwd4(T, B, t0, t1, dh_ext, ldd, whhT16, gates16, cstate, lens, dG16, dc_carry, flags, st);
+int lstm_bwd_max_clusters(int B) {
+    const int smem = B4_NCH * (((B + 7) & ~7) * 128) + B4_W_BYTES + B4_XCHG_FLOATS * 4 + 256 + 1024;
+    if (cudaFuncSetAttribute(lstm_bwd4_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) return -1;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(B4_CTAS); cfg.blockDim = dim3(LSTM_THREADS); cfg.dynamicSmemBytes = smem;
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = B4_CLUSTER; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
+    cfg.attrs = &attr; cfg.numAttrs = 1;
+    int n = -1;
+    if (cudaOccupancyMaxActiveClusters(&n, lstm_bwd4_kernel, &cfg) != cudaSuccess) return -1;
+    return n;
 }
 
+// Steps [t0, t1) of a layer's BPTT (layer pipeline, ar_step.cu).  `xchg` non-null: the flat kernel, whose 64 CTAs fit next
+// to the other layer's chunk; null: the cluster kernel.  See launch_bwd for the sizes of `flags` and `xchg`.
+int launch_lstm_bwd_chunk(int T, int B, int t0, int t1, const float* dh_ext, long long ldd, const void* whhT16, const void* gates16,
+                          const float* cstate, const int* lens, void* dG16, float* dc_carry, int* flags, float* xchg, cudaStream_t st) {
+    if (T <= 0 || B <= 0 || t1 <= t0) return 0;
+    if (B > 32 || t0 < 0 || t1 > T || !dc_carry) return ft_set_error("lstm_bwd_chunk: bad batch, step range or carry buffer");
+    return launch_bwd(T, B, t0, t1, dh_ext, ldd, whhT16, gates16, cstate, lens, dG16, dc_carry, flags, xchg, st);
+}
+
+// Whole sequence (the attention LSTM's BPTT, which runs alone) on the cluster kernel: alone, its DSMEM exchange is the
+// faster one -- 3.96 us/step against the flat kernel's 4.27 (T = 1000, B = 32, H100 80GB HBM3, tools/bptt_overlap.py).
 int launch_lstm_bwd(int T, int B, const float* dh_ext, long long ldd, const void* whhT16, const void* gates16,
                     const float* cstate, const int* lens, void* dG16, int* flags, cudaStream_t st) {
     if (T <= 0 || B <= 0) return 0;
     if (B > 32) return ft_set_error("lstm_bwd: batch > 32 per call not supported (split the batch)");
-    return launch_bwd4(T, B, 0, T, dh_ext, ldd, whhT16, gates16, cstate, lens, dG16, nullptr, flags, st);
+    return launch_bwd(T, B, 0, T, dh_ext, ldd, whhT16, gates16, cstate, lens, dG16, nullptr, flags, nullptr, st);
 }
 
 }  // namespace ft

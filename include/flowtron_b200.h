@@ -60,6 +60,15 @@ int ft_lstm_fwd(int T, int B, const float* xproj, const void* whh16, const int* 
 void ft_debug_set_lstm_trace(long long* buf);
 /* same for ft_ar_step_infer: [T][32] stamps of CTA 0 (phase boundaries, tools/trace_infer.py) */
 void ft_debug_set_infer_trace(long long* buf);
+/* debug: 4-CTA clusters of the BPTT cluster kernel that fit on the device at once, at its launch configuration for
+ * batch B (cudaOccupancyMaxActiveClusters); -1 on error */
+int ft_debug_lstm_bwd_max_clusters(int B);
+/* debug: steps [t0, t1) of one BPTT chunk of the layer pipeline (B <= 32), resuming dc*f from / handing it on through
+ * dc_carry [B,1024] fp32 and dG_{t1} from dG16.  xchg non-NULL: the flat kernel the pipeline runs (flags [(t1-t0)*128],
+ * xchg [2*16*4*B*64] fp32); NULL: the 4-CTA cluster kernel (flags [(t1-t0)*64]).  Both give bit-identical results. */
+int ft_debug_lstm_bwd_chunk(int T, int B, int t0, int t1, const float* dh_ext, long long ldd, const void* whhT16,
+                            const void* gates16, const float* cstate, const int* lens, void* dG16, float* dc_carry, int* flags,
+                            float* xchg, void* stream);
 
 /* ft_gemm tile policy: 0 = one CTA per 128 x 256 tile always; 1 (default) = CTA pairs (2-CTA clusters sharing B by TMA multicast, 256 x 256 tiles) for
  * contractions >= 1e11 FLOP; 2 = CTA pairs whenever the output is wide and has >= SMs/2 such tiles. */
