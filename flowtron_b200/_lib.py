@@ -200,6 +200,8 @@ def _declare(L):
     L.ft_waveglow_infer.argtypes = [POINTER(FtWaveGlowDesc), POINTER(FtWaveGlowWeights), c_void_p, c_void_p, c_float, c_void_p,
                                     c_void_p, c_void_p]
     L.ft_waveglow_infer.restype = c_int
+    L.ft_posterior_mean.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_float, c_void_p, c_void_p]
+    L.ft_posterior_mean.restype = c_int
 
 
 def check(rc: int, what: str = ""):
@@ -507,6 +509,19 @@ def attn_ctc_loss(logprob, in_lens, out_lens, time_reversed, blank_logprob, cost
     scratch = scratch_buffer(int(lib().ft_attn_ctc_scratch_bytes(B, T, L)), logprob.device)
     check(lib().ft_attn_ctc_loss(ptr(logprob), ptr(in_lens), ptr(out_lens), B, T, L, 1 if time_reversed else 0,
                                  float(blank_logprob), ptr(cost), ptr(dlogprob), ptr(scratch), stream_ptr()), "ft_attn_ctc_loss")
+
+
+POSTERIOR_BATCH, POSTERIOR_TIME_AND_BATCH = 0, 1
+
+
+def posterior_mean(z, out_lens, n_frames, mode, scale, out):
+    """z f32 [T,B,M] contiguous CUDA, out_lens int32 CUDA [B]; out f32 [M, n_frames] (mode 0) or [M] (mode 1), written.
+    One launch (csrc/style.cu)."""
+    _need_cuda(z, out_lens, out)
+    T, B, M = z.shape
+    assert z.dtype == torch.float32 and z.is_contiguous() and out_lens.dtype == torch.int32 and out.is_contiguous()
+    check(lib().ft_posterior_mean(ptr(z), int(T), int(B), int(M), ptr(out_lens), int(n_frames), int(mode), float(scale),
+                                  ptr(out), stream_ptr()), "ft_posterior_mean")
 
 
 def radam_step_dev_raw(p_ptr, g_ptr, m_ptr, v_ptr, n, beta1, beta2, eps, weight_decay, lr, step_dev, coef_ptr=0):

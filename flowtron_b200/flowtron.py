@@ -449,6 +449,11 @@ class AR_Back_Step(nn.Module):
 
 
 # --------------------------------------------------------------------------------------------- model
+# Padded frame count from which ft_ar_step_fwd runs the attention LSTM's input projection as a separate GEMM rather than
+# folded into the recurrence (kAttnChunk + 64 in csrc/ar_step.cu); the two paths round differently.
+_ATTN_OVERLAP_MIN_T = 320
+
+
 def _ragged_lengths(v, B: int, hi: int, name: str) -> Tensor:
     """Per-row lengths for Flowtron.infer_batch: a CUDA tensor is trusted (only its size is checked); host values must be
     B integers in [1, hi]."""
@@ -592,6 +597,74 @@ class Flowtron(nn.Module):
             out = self._run_slices([(0, B // 2), (B // 2, B)], mel, encoder_outputs, mask, out_lens, attn_prior,
                                    streams=self._side_streams)
         return (*out, mean, log_var, prob)
+
+    def encode(self, mel, speaker_ids, text, in_lens, out_lens, attn_prior=None):
+        """The mel -> z direction for a padded batch of reference utterances, as style transfer uses it.
+
+        mel [B, 80, T] f32, speaker_ids [B], text [B, L] int64 (row b valid in [0, in_lens[b])), in_lens [B], out_lens [B],
+        attn_prior [B, T, L] or None -> z [B, 80, T], zero at t >= out_lens[b].
+
+        Row b of ``z[:, :, :out_lens[b]]`` equals ``forward(mel[b:b+1, :, :out_lens[b]], speaker_ids[b:b+1],
+        text[b:b+1, :in_lens[b]], ...)[0].permute(1, 2, 0)``: the reference notebook's one-utterance-at-a-time call.  The
+        flows run as in ``forward`` (launches of at most 32 utterances) and the text encoder on its masked kernels without
+        dropout, under ``torch.no_grad()`` whatever ``self.training`` is; no autograd state is kept.  ``z`` is a view of the
+        flows' ``[T, B, 80]`` output, so ``style.posterior_mean`` reads it without a copy.
+
+        Lengths given as host sequences or CPU tensors are checked (ValueError unless 1 <= in_lens[b] <= L and
+        1 <= out_lens[b] <= T); CUDA length tensors are trusted, as ``forward`` trusts them, and the call makes no host
+        synchronisation, so it can be captured in a CUDA graph.  Texts over _lib.MAX_TEXT_LEN tokens raise ValueError.
+
+        The flow step computes the attention LSTM's input projection one of two ways, chosen from the padded frame count
+        (folded into the recurrence below _ATTN_OVERLAP_MIN_T frames, a separate GEMM from there on), and the two round
+        differently.  With host out_lens, a batch padded to at least that many frames runs its shorter rows as a separate
+        launch padded to their own longest, so every row takes the path its B = 1 run takes and equals it bit for bit.
+        CUDA out_lens cannot be split without a host synchronisation: such rows then differ from their B = 1 run by
+        rounding (about 6e-5 of max |z| on the H100)."""
+        if mel.dim() != 3 or text.dim() != 2 or speaker_ids.dim() != 1:
+            raise ValueError("encode expects mel [B, n_mel, T], speaker_ids [B] and text [B, L]")
+        B, _, T = mel.shape
+        L = text.size(1)
+        _lib.check_text_len(L, "Flowtron.encode")
+        if text.size(0) != B or speaker_ids.size(0) != B or B < 1 or T < 1 or L < 1:
+            raise ValueError(f"batch sizes disagree or are empty: mel {tuple(mel.shape)}, "
+                             f"speaker_ids {tuple(speaker_ids.shape)}, text {tuple(text.shape)}")
+        if attn_prior is not None and tuple(attn_prior.shape) != (B, T, L):
+            raise ValueError(f"attn_prior must be [B, T, L] = {(B, T, L)}, got {tuple(attn_prior.shape)}")
+        in_lens = _ragged_lengths(in_lens, B, L, "in_lens")
+        out_lens = _ragged_lengths(out_lens, B, T, "out_lens")
+        if not (mel.is_cuda and text.is_cuda and speaker_ids.is_cuda and (attn_prior is None or attn_prior.is_cuda)):
+            raise FlowtronB200Error("Flowtron.encode needs CUDA tensors: the sm_90a kernels are the only implementation")
+        dev = mel.device
+        groups = None                       # host lengths: (rows, their longest) on each side of _ATTN_OVERLAP_MIN_T
+        if not out_lens.is_cuda:
+            lens = out_lens.tolist()
+            short = [b for b in range(B) if lens[b] < _ATTN_OVERLAP_MIN_T]
+            long_rows = [b for b in range(B) if lens[b] >= _ATTN_OVERLAP_MIN_T]
+            groups = [(rows, max(lens[b] for b in rows)) for rows in (short, long_rows) if rows]
+        in_lens = in_lens.to(device=dev, dtype=torch.int32)
+        out_lens = out_lens.to(device=dev, dtype=torch.int32)
+        with torch.no_grad():
+            if groups is None or groups == [(list(range(B)), T)]:
+                return self._encode_rows(mel, speaker_ids, text, in_lens, out_lens, attn_prior).permute(1, 2, 0)
+            z = torch.zeros(T, B, mel.size(1), device=dev)
+            for rows, t in groups:
+                idx = torch.tensor(rows, device=dev)
+                prior = None if attn_prior is None else attn_prior[idx, :t]
+                zg = self._encode_rows(mel[idx, :, :t], speaker_ids[idx], text[idx], in_lens[idx], out_lens[idx], prior)
+                z[:t].index_copy_(1, idx, zg)
+        return z.permute(1, 2, 0)
+
+    def _encode_rows(self, mel, speaker_ids, text, in_lens, out_lens, attn_prior):
+        """Flowtron.encode's work on checked inputs (lengths int32 on the device) -> z [T, B, 80], zero past out_lens."""
+        T, dev = mel.size(2), mel.device
+        speaker_ids = speaker_ids * 0 if self.dummy_speaker_embedding else speaker_ids
+        speaker_vecs = self.speaker_embedding(speaker_ids)
+        text = self.encoder.infer_ragged_tokens(text, self.embedding, in_lens).transpose(0, 1)
+        encoder_outputs = torch.cat([text, speaker_vecs.expand(text.size(0), -1, -1)], 2)
+        mask = ~(torch.arange(text.size(0), device=dev)[None, :] < in_lens[:, None])[..., None]
+        z = self._run_flows(mel.permute(2, 0, 1), encoder_outputs, mask, out_lens, attn_prior)[0]
+        # forward leaves frames at or past out_lens[b] undefined
+        return z.masked_fill_(torch.arange(T, device=dev)[:, None, None] >= out_lens[None, :, None], 0.0)
 
     def infer(self, residual, speaker_ids, text, temperature=1.0, gate_threshold=0.5, attns=None, attn_prior=None):
         """Texts of up to _lib.MAX_TEXT_LEN (1024) tokens; longer ones raise ValueError before any work."""

@@ -373,6 +373,20 @@ size_t ft_waveglow_scratch_bytes(const FtWaveGlowDesc* d);
 int ft_waveglow_infer(const FtWaveGlowDesc* d, const FtWaveGlowWeights* w, const float* mel, const float* noise, float sigma,
                       float* audio, void* scratch, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------
+ * Style transfer by posterior sampling (the reference's inference_style_transfer.ipynb): the posterior mean of the z of
+ * B reference utterances (csrc/style.cu).
+ * ---------------------------------------------------------------------------------------------------- */
+/* z fp32 [T, B, M] (Flowtron.forward's flow layout, row t*B + b), M <= 128; out_lens int32 [B] on the device, each in
+ * [1, T] (not checked);  mode 0 ('batch'): out fp32 [M, n_frames],
+ *   out[m, t] = scale * (1/B) sum_b z[t mod out_lens[b], b, m]                      (each z repeated in time to n_frames);
+ * mode 1 ('time_and_batch'): out fp32 [M],
+ *   out[m] = scale * (1/B) sum_b (1/out_lens[b]) sum_{t < out_lens[b]} z[t, b, m].
+ * scale = ratio / (ratio + 1) with ratio = B / lambda.  One launch, fp32 sums in a fixed order (no atomics: replays are
+ * bit-identical), no allocation, no host synchronisation.  Rejects B < 1, T < 1, n_frames < 1 and M > 128. */
+int ft_posterior_mean(const float* z, int T, int B, int M, const int* out_lens, int n_frames, int mode, float scale,
+                      float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
