@@ -140,6 +140,9 @@ def _declare(L):
     L.ft_ar_step_infer_ragged.argtypes = [POINTER(FtArStepDesc), POINTER(FtArStepWeights), c_void_p, c_void_p, c_void_p,
                                           c_void_p, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
     L.ft_ar_step_infer_ragged.restype = c_int
+    L.ft_ar_step_infer_aligned.argtypes = [POINTER(FtArStepDesc), POINTER(FtArStepWeights), c_void_p, c_void_p, c_void_p,
+                                           c_void_p, c_void_p, c_int, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
+    L.ft_ar_step_infer_aligned.restype = c_int
     L.ft_mel_scratch_bytes.argtypes = [c_int, c_longlong]
     L.ft_mel_scratch_bytes.restype = c_size_t
     L.ft_mel_spectrogram.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_void_p, c_void_p, c_void_p,
@@ -439,6 +442,17 @@ def ar_step_infer_ragged(desc, weights, residual, text, in_lens, frame_lens, gat
     check(lib().ft_ar_step_infer_ragged(byref(desc), byref(weights), ptr(residual), ptr(text), ptr(in_lens), ptr(frame_lens),
                                         float(gate_threshold), ptr(out), ptr(attn_out), ptr(n_frames), ptr(scratch),
                                         stream_ptr()), "ft_ar_step_infer_ragged")
+
+
+def ar_step_infer_aligned(desc, weights, residual, text, in_lens, frame_lens, attn_forced, gate_threshold, out, attn_out,
+                          n_frames):
+    """As ar_step_infer_ragged with forced alignments: attn_forced f32 CUDA [B, Ta, L] contiguous, row (b, i) = generation
+    step i of utterance b, Ta >= max frame_lens."""
+    nbytes = int(lib().ft_ar_step_infer_scratch_bytes(byref(desc)))
+    scratch = scratch_buffer(nbytes, residual.device)
+    check(lib().ft_ar_step_infer_aligned(byref(desc), byref(weights), ptr(residual), ptr(text), ptr(in_lens), ptr(frame_lens),
+                                         ptr(attn_forced), int(attn_forced.size(1)), float(gate_threshold), ptr(out),
+                                         ptr(attn_out), ptr(n_frames), ptr(scratch), stream_ptr()), "ft_ar_step_infer_aligned")
 
 
 def mel_spectrogram(wav, sample_offsets, frame_offsets, n_utt, total_frames, window, basis, band_lo, band_hi, n_fft, hop,

@@ -76,6 +76,10 @@ struct InferParams {
     uint32_t* alive;                       // [B] per slot: 1 while the sample keeps generating after this frame, 0 once stopped
     int* status;
     long long* trace;                      // debug: [T][32] clock64 stamps of CTA 0 (tools/trace_infer.py), or null
+    // ft_ar_step_infer_aligned (the kAligned kernels): attn_forced is batch-major [B,Ta,L], each row in its flow's own generation
+    // order; step i of utterance b reads keys l < in_lens[b] of row (b, i) while i < frame_lens[b]: every other weight is 0
+    // whatever the buffer holds
+    int Ta;
 };
 
 static long long* g_infer_trace = nullptr;
@@ -387,9 +391,17 @@ __device__ __forceinline__ float residual_at(const InferParams& p, int i, int b,
     return p.residual[(static_cast<long long>(t) * p.B + b) * p.M + m];
 }
 
+// kAligned: the forced weights of utterance b at generation step i (row (b, i) of the batch-major buffer) and how many of its
+// keys are read: in_lens[b], none once the row's frame budget is spent.
+__device__ __forceinline__ const float* aligned_row(const InferParams& p, int i, int b, int Lb, int& Lf) {
+    Lf = (p.frame_lens && i >= p.frame_lens[b]) ? 0 : Lb;
+    return p.attn_forced + (static_cast<long long>(b) * p.Ta + i) * p.L;
+}
+
 // Long texts (kLong, L > LMAX): warp 0 runs the same softmax / prior posterior / forced alignment over the row staged in
 // shared memory, 32 keys per pass, instead of holding it in registers.  Each lane handles the same keys in the same order
 // as the register path, so the two agree bit for bit where both apply.
+template <bool kAligned>
 __device__ __forceinline__ void attn_row_long(const InferParams& p, float* se, int i, int b, long long cur, bool forced, int Lb) {
     const int lane = threadIdx.x & 31;
     if (!forced) {
@@ -424,6 +436,10 @@ __device__ __forceinline__ void attn_row_long(const InferParams& p, float* se, i
             const float inv2 = 1.f / s2;
             for (int l = lane; l < p.L; l += 32) se[l] *= inv2;
         }
+    } else if (kAligned) {
+        int Lf;
+        const float* fr = aligned_row(p, i, b, Lb, Lf);
+        for (int l = lane; l < p.L; l += 32) se[l] = l < Lf ? fr[l] : 0.f;
     } else {
         for (int l = lane; l < p.L; l += 32) se[l] = p.attn_forced[(static_cast<long long>(i) * p.B + b) * p.L + l];
     }
@@ -433,14 +449,14 @@ __device__ __forceinline__ void attn_row_long(const InferParams& p, float* se, i
 // prior posterior -- or the forced alignment), all 16 warps then take L/16 keys each (every V load of the CTA in flight at
 // once), partial sums meet in shared memory.  Writes ctx (fp16 for lstm layer 0, fp32 for the gate) and, from slice 0, the
 // attention weights.  (One CTA per utterance doing all 640 channels would pull 256 KB through one SM.)
-template <int CW, bool kLong>
+template <int CW, bool kLong, bool kAligned>
 __device__ __forceinline__ void context_item(const InferParams& p, float* sf, int i, int b, int s, long long cur, long long nxt, bool forced) {
     constexpr int NV = CW / 32;                                    // channels per lane
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     float* se = sf; float* sp = sf + (kLong ? LMAX_LONG : LMAX);   // attn [LMAX or LMAX_LONG], partials [16 warps][CW]
     const int Lb = p.in_lens ? p.in_lens[b] : p.L;                 // key mask: tokens l >= Lb get weight 0 (as if L were Lb)
     if (kLong && warp == 0) {
-        attn_row_long(p, se, i, b, cur, forced, Lb);
+        attn_row_long<kAligned>(p, se, i, b, cur, forced, Lb);
         if (s == 0)
             for (int l = lane; l < p.L; l += 32) p.attn_out[(static_cast<long long>(i) * p.B + b) * p.L + l] = se[l];
     } else if (warp == 0) {
@@ -486,6 +502,11 @@ __device__ __forceinline__ void context_item(const InferParams& p, float* sf, in
 #pragma unroll
                 for (int jj = 0; jj < 8; ++jj) w[jj] *= inv2;
             }
+        } else if (kAligned) {
+            int Lf;
+            const float* fr = aligned_row(p, i, b, Lb, Lf) + lane;
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) w[jj] = lane + 32 * jj < Lf ? __ldg(fr + 32 * jj) : 0.f;
         } else {
 #pragma unroll
             for (int jj = 0; jj < 8; ++jj) { const int l = lane + 32 * jj; w[jj] = l < p.L ? p.attn_forced[(static_cast<long long>(i) * p.B + b) * p.L + l] : 0.f; }
@@ -541,8 +562,9 @@ __device__ __forceinline__ void context_item(const InferParams& p, float* sf, in
 }
 
 // kLong: texts of LMAX < L <= LMAX_LONG keys (context_item's softmax over a shared-memory row): infer_long_kernel.  The
-// L <= LMAX instantiations are infer_kernel, the short-text kernels.
-template <bool kB16, bool kLong>
+// L <= LMAX instantiations are infer_kernel, the short-text kernels.  kAligned: ft_ar_step_infer_aligned's forced alignments
+// (always forced, so the query / score phases are not compiled in): infer_aligned_kernel.
+template <bool kB16, bool kLong, bool kAligned>
 __device__ __forceinline__ void infer_body(const InferParams& p) {
     extern __shared__ __align__(16) uint8_t smem_raw[];
     __half* sx = reinterpret_cast<__half*>(smem_raw);                          // [16][KP] fp16 activations of the phase
@@ -560,7 +582,7 @@ __device__ __forceinline__ void infer_body(const InferParams& p) {
     // by a store, and the ring-slot reuse argument relies on read -> store chains)
     const bool act_lstm = static_cast<int>(blockIdx.x) * 4 < IH / 2, act_q = static_cast<int>(blockIdx.x) < p.A / 8;
     const bool act_dense = static_cast<int>(blockIdx.x) < IH / 8, act_conv = static_cast<int>(blockIdx.x) < p.M / 4;
-    const bool forced = p.attn_forced != nullptr;    // `attn` given (flowtron.py:585-588): no query / score / softmax / prior
+    const bool forced = kAligned || p.attn_forced != nullptr;    // `attn` given (flowtron.py:585-588): no query / score / softmax / prior
     // context work items: (utterance, channel slice); 64-channel slices unless that needs a second pass over the grid
     const bool wide_ctx = (p.A % 128 == 0) && p.B * (p.A / 64) > static_cast<int>(gridDim.x);
     Prefetch pf;
@@ -641,8 +663,8 @@ __device__ __forceinline__ void infer_body(const InferParams& p) {
             IT_TRACE(6);
         }
         // ---- P3b softmax + context, one (utterance, channel slice) item per CTA
-        if (wide_ctx) { for (int it = blockIdx.x; it < p.B * (p.A / 128); it += gridDim.x) context_item<128, kLong>(p, sf, i, it / (p.A / 128), it % (p.A / 128), cur, nxt, forced); }
-        else          { for (int it = blockIdx.x; it < p.B * (p.A / 64); it += gridDim.x) context_item<64, kLong>(p, sf, i, it / (p.A / 64), it % (p.A / 64), cur, nxt, forced); }
+        if (wide_ctx) { for (int it = blockIdx.x; it < p.B * (p.A / 128); it += gridDim.x) context_item<128, kLong, kAligned>(p, sf, i, it / (p.A / 128), it % (p.A / 128), cur, nxt, forced); }
+        else          { for (int it = blockIdx.x; it < p.B * (p.A / 64); it += gridDim.x) context_item<64, kLong, kAligned>(p, sf, i, it / (p.A / 64), it % (p.A / 64), cur, nxt, forced); }
         IT_TRACE(7);
         // ---- P4 lstm layer 0 on [hA ; ctx ; h0_{i-1}]
         lstm_pre(p, p.b0, p.c0, cpre, bpre);
@@ -769,11 +791,15 @@ __device__ __forceinline__ void infer_body(const InferParams& p) {
 
 template <bool kB16>
 __global__ void __launch_bounds__(INF_THREADS, 1)
-infer_kernel(InferParams p) { infer_body<kB16, false>(p); }
+infer_kernel(InferParams p) { infer_body<kB16, false, false>(p); }
 
 template <bool kB16>
 __global__ void __launch_bounds__(INF_THREADS, 1)
-infer_long_kernel(InferParams p) { infer_body<kB16, true>(p); }
+infer_long_kernel(InferParams p) { infer_body<kB16, true, false>(p); }
+
+template <bool kB16, bool kLong>
+__global__ void __launch_bounds__(INF_THREADS, 1)
+infer_aligned_kernel(InferParams p) { infer_body<kB16, kLong, true>(p); }
 
 // ------------------------------------------------------------------------------------------------ weight packing
 // dst[task][m][n][kk] (fp16) <- W[row(task, n)][32 m + kk] over the virtual K = [A part (Ka real columns, padded to Kap) ; B part]
@@ -867,8 +893,8 @@ __global__ void infer_ragged_finish_kernel(float* __restrict__ out, float* __res
 }
 
 static int infer_impl(const FtArStepDesc* d, const FtArStepWeights* w, const float* residual, const float* text,
-                      const float* attn_prior, const float* attn_forced, const int* in_lens, const int* frame_lens, int reversed,
-                      float gate_threshold, float* out, float* attn_out, int* n_frames, void* scratch, void* stream) {
+                      const float* attn_prior, const float* attn_forced, int Ta, const int* in_lens, const int* frame_lens,
+                      int reversed, float gate_threshold, float* out, float* attn_out, int* n_frames, void* scratch, void* stream) {
     if (d->n_hidden != IH) return ft_set_error("infer: n_hidden must be 1024");
     if (d->L > LMAX_LONG) return ft_set_error("infer: L > FT_MAX_TEXT_LEN (1024) not supported");
     if (d->B > 16) return ft_set_error("infer: batch > 16 per call not supported (run the batch in slices of 16)");
@@ -908,7 +934,7 @@ static int infer_impl(const FtArStepDesc* d, const FtArStepWeights* w, const flo
     p.bA = s.bA; p.b0 = s.b0; p.b1 = s.b1; p.bd1 = s.bd1; p.bd2 = s.bd2; p.bc = s.bc;
     p.v = w->att_v; p.wg = w->gate_w; p.bg = w->gate_b;
     p.Kp = s.Kp; p.Vp = s.Vp; p.residual = residual; p.prior = d->has_prior ? attn_prior : nullptr;
-    p.attn_forced = attn_forced;
+    p.attn_forced = attn_forced; p.Ta = Ta;                      // Ta > 0: batch-major forced alignments, the kAligned kernels
     p.in_lens = in_lens; p.frame_lens = frame_lens; p.reversed = reversed;
     p.inv_temperature = 1.0f / d->temperature; p.gate_threshold = gate_threshold;
     p.has_gate = d->has_gate && w->gate_w;
@@ -947,6 +973,9 @@ static int infer_impl(const FtArStepDesc* d, const FtArStepWeights* w, const flo
     const bool long_text = d->L > LMAX;
     void* fn = long_text ? (B > 8 ? reinterpret_cast<void*>(infer_long_kernel<true>) : reinterpret_cast<void*>(infer_long_kernel<false>))
                          : (B > 8 ? reinterpret_cast<void*>(infer_kernel<true>) : reinterpret_cast<void*>(infer_kernel<false>));
+    if (Ta > 0)
+        fn = long_text ? (B > 8 ? reinterpret_cast<void*>(infer_aligned_kernel<true, true>) : reinterpret_cast<void*>(infer_aligned_kernel<false, true>))
+                       : (B > 8 ? reinterpret_cast<void*>(infer_aligned_kernel<true, false>) : reinterpret_cast<void*>(infer_aligned_kernel<false, false>));
     const int smem = 16 * KP * 2 + INF_WARPS * 128 * 4 + ((long_text ? LMAX_LONG : LMAX) + INF_WARPS * 128 + 64) * 4;
     cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     TimeScope ts("infer", d->T, B, d->L, st);
@@ -955,6 +984,24 @@ static int infer_impl(const FtArStepDesc* d, const FtArStepWeights* w, const flo
     if (e != cudaSuccess) return ft_set_error(cudaGetErrorString(e));
     ft_count_launch(1);
     return ft_check_launch("infer_kernel");
+}
+
+// ft_ar_step_infer_ragged / ft_ar_step_infer_aligned: the persistent kernel on per-row lengths (attn_forced: batch-major
+// [B,Ta,L] or null), then the per-row finish.
+static int infer_ragged_impl(const FtArStepDesc* d, const FtArStepWeights* w, const float* residual, const float* text,
+                             const int* in_lens, const int* frame_lens, const float* attn_forced, int Ta, float gate_threshold,
+                             float* out, float* attn_out, int* n_frames, void* scratch, void* stream) {
+    const int rev = d->reversed ? 1 : 0;
+    if (infer_impl(d, w, residual, text, nullptr, attn_forced, Ta, in_lens, frame_lens, rev, gate_threshold, out, attn_out, n_frames, scratch, stream) != 0)
+        return -1;
+    // frames are generated back to front by a reversed flow: flip each row within its own n_frames (the B = 1 flip), and clear
+    // the attention rows of frames a stopped utterance computed but did not emit
+    const int rows = d->T * d->B;
+    if (rows <= 0) return 0;
+    infer_ragged_finish_kernel<<<rows < 4096 ? rows : 4096, 128, 0, static_cast<cudaStream_t>(stream)>>>(
+        out, attn_out, n_frames, d->T, d->B, d->n_mel, d->L, rev);
+    ft_count_launch(1);
+    return ft_check_launch("infer_ragged_finish_kernel");
 }
 
 }  // namespace ft
@@ -971,8 +1018,8 @@ int ft_ar_step_infer(const FtArStepDesc* d, const FtArStepWeights* w, const floa
                      int* n_frames, void* scratch, void* stream) {
     using namespace ft;
     if (!d || !w || !residual || !text || !out || !attn_out || !n_frames || !scratch) return ft_set_error("ft_ar_step_infer: NULL argument");
-    return infer_impl(d, w, residual, text, attn_prior, attn_forced, nullptr, nullptr, 0, gate_threshold, out, attn_out, n_frames,
-                          scratch, stream);
+    return infer_impl(d, w, residual, text, attn_prior, attn_forced, 0, nullptr, nullptr, 0, gate_threshold, out, attn_out, n_frames,
+                      scratch, stream);
 }
 
 int ft_ar_step_infer_ragged(const FtArStepDesc* d, const FtArStepWeights* w, const float* residual, const float* text,
@@ -981,18 +1028,18 @@ int ft_ar_step_infer_ragged(const FtArStepDesc* d, const FtArStepWeights* w, con
     using namespace ft;
     if (!d || !w || !residual || !text || !out || !attn_out || !n_frames || !scratch) return ft_set_error("ft_ar_step_infer_ragged: NULL argument");
     if (d->has_prior) return ft_set_error("ft_ar_step_infer_ragged: attn_prior is not supported");
-    const int rev = d->reversed ? 1 : 0;
-    if (infer_impl(d, w, residual, text, nullptr, nullptr, in_lens, frame_lens, rev, gate_threshold, out, attn_out, n_frames,
-                   scratch, stream) != 0)
-        return -1;
-    // frames are generated back to front by a reversed flow: flip each row within its own n_frames (the B = 1 flip), and clear
-    // the attention rows of frames a stopped utterance computed but did not emit
-    const int rows = d->T * d->B;
-    if (rows <= 0) return 0;
-    infer_ragged_finish_kernel<<<rows < 4096 ? rows : 4096, 128, 0, static_cast<cudaStream_t>(stream)>>>(
-        out, attn_out, n_frames, d->T, d->B, d->n_mel, d->L, rev);
-    ft_count_launch(1);
-    return ft_check_launch("infer_ragged_finish_kernel");
+    return infer_ragged_impl(d, w, residual, text, in_lens, frame_lens, nullptr, 0, gate_threshold, out, attn_out, n_frames, scratch, stream);
+}
+
+int ft_ar_step_infer_aligned(const FtArStepDesc* d, const FtArStepWeights* w, const float* residual, const float* text,
+                             const int* in_lens, const int* frame_lens, const float* attn_forced, int Ta, float gate_threshold,
+                             float* out, float* attn_out, int* n_frames, void* scratch, void* stream) {
+    using namespace ft;
+    if (!d || !w || !residual || !text || !attn_forced || !out || !attn_out || !n_frames || !scratch)
+        return ft_set_error("ft_ar_step_infer_aligned: NULL argument");
+    if (d->has_prior) return ft_set_error("ft_ar_step_infer_aligned: attn_prior is not supported");
+    if (Ta < 1 || (!frame_lens && Ta < d->T)) return ft_set_error("ft_ar_step_infer_aligned: attn_forced must cover every frame budget (Ta >= max frame_lens)");
+    return infer_ragged_impl(d, w, residual, text, in_lens, frame_lens, attn_forced, Ta, gate_threshold, out, attn_out, n_frames, scratch, stream);
 }
 
 }  // extern "C"

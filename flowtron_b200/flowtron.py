@@ -423,6 +423,12 @@ class AR_Step(nn.Module):
         from .inference import ar_step_infer_ragged
         return ar_step_infer_ragged(self, residual, text, in_lens, frame_lens, reversed_flag=False)
 
+    def infer_aligned(self, residual, text, in_lens, frame_lens, attns):
+        """infer_ragged with forced alignments: attns [B, Ta, L] as this flow's ``forward`` returns its attention; see
+        inference.ar_step_infer_aligned."""
+        from .inference import ar_step_infer_aligned
+        return ar_step_infer_aligned(self, residual, text, in_lens, frame_lens, attns, reversed_flag=False)
+
 
 class AR_Back_Step(nn.Module):
     """flowtron.py:595-642.  The flip/roll of the reference is an index map inside the kernels (no copies, no host syncs)."""
@@ -446,6 +452,12 @@ class AR_Back_Step(nn.Module):
         """As AR_Step.infer_ragged; row b runs back to front over its own first frame_lens[b] frames."""
         from .inference import ar_step_infer_ragged
         return ar_step_infer_ragged(self.ar_step, residual, text, in_lens, frame_lens, reversed_flag=True)
+
+    def infer_aligned(self, residual, text, in_lens, frame_lens, attns):
+        """As AR_Step.infer_aligned; row (b, i) of attns is generation step i, i.e. natural frame frame_lens[b] - 1 - i: the
+        flipped order this flow's ``forward`` returns."""
+        from .inference import ar_step_infer_aligned
+        return ar_step_infer_aligned(self.ar_step, residual, text, in_lens, frame_lens, attns, reversed_flag=True)
 
 
 # --------------------------------------------------------------------------------------------- model
@@ -598,7 +610,7 @@ class Flowtron(nn.Module):
                                    streams=self._side_streams)
         return (*out, mean, log_var, prob)
 
-    def encode(self, mel, speaker_ids, text, in_lens, out_lens, attn_prior=None):
+    def encode(self, mel, speaker_ids, text, in_lens, out_lens, attn_prior=None, return_attns=False):
         """The mel -> z direction for a padded batch of reference utterances, as style transfer uses it.
 
         mel [B, 80, T] f32, speaker_ids [B], text [B, L] int64 (row b valid in [0, in_lens[b])), in_lens [B], out_lens [B],
@@ -619,7 +631,11 @@ class Flowtron(nn.Module):
         differently.  With host out_lens, a batch padded to at least that many frames runs its shorter rows as a separate
         launch padded to their own longest, so every row takes the path its B = 1 run takes and equals it bit for bit.
         CUDA out_lens cannot be split without a host synchronisation: such rows then differ from their B = 1 run by
-        rounding (about 6e-5 of max |z| on the H100)."""
+        rounding (about 6e-5 of max |z| on the H100).
+
+        ``return_attns=True`` returns ``(z, attns)``: ``attns[f]`` [B, T, L] is flow f's attention as ``forward`` returns it in
+        ``attns_list`` (row b left-aligned in that flow's own time order: an AR_Back_Step's rows run back to front over
+        their out_lens[b] frames), zero at t >= out_lens[b] and l >= in_lens[b] -- what ``infer_aligned`` takes."""
         if mel.dim() != 3 or text.dim() != 2 or speaker_ids.dim() != 1:
             raise ValueError("encode expects mel [B, n_mel, T], speaker_ids [B] and text [B, L]")
         B, _, T = mel.shape
@@ -645,26 +661,38 @@ class Flowtron(nn.Module):
         out_lens = out_lens.to(device=dev, dtype=torch.int32)
         with torch.no_grad():
             if groups is None or groups == [(list(range(B)), T)]:
-                return self._encode_rows(mel, speaker_ids, text, in_lens, out_lens, attn_prior).permute(1, 2, 0)
-            z = torch.zeros(T, B, mel.size(1), device=dev)
-            for rows, t in groups:
-                idx = torch.tensor(rows, device=dev)
-                prior = None if attn_prior is None else attn_prior[idx, :t]
-                zg = self._encode_rows(mel[idx, :, :t], speaker_ids[idx], text[idx], in_lens[idx], out_lens[idx], prior)
-                z[:t].index_copy_(1, idx, zg)
-        return z.permute(1, 2, 0)
+                z, attns = self._encode_rows(mel, speaker_ids, text, in_lens, out_lens, attn_prior, return_attns)
+            else:
+                z = torch.zeros(T, B, mel.size(1), device=dev)
+                attns = [torch.zeros(B, T, L, device=dev) for _ in self.flows] if return_attns else None
+                for rows, t in groups:
+                    idx = torch.tensor(rows, device=dev)
+                    prior = None if attn_prior is None else attn_prior[idx, :t]
+                    zg, ag = self._encode_rows(mel[idx, :, :t], speaker_ids[idx], text[idx], in_lens[idx], out_lens[idx], prior,
+                                               return_attns)
+                    z[:t].index_copy_(1, idx, zg)
+                    for a, g in zip(attns or (), ag or ()):
+                        a[:, :t].index_copy_(0, idx, g)
+        z = z.permute(1, 2, 0)
+        return (z, attns) if return_attns else z
 
-    def _encode_rows(self, mel, speaker_ids, text, in_lens, out_lens, attn_prior):
-        """Flowtron.encode's work on checked inputs (lengths int32 on the device) -> z [T, B, 80], zero past out_lens."""
+    def _encode_rows(self, mel, speaker_ids, text, in_lens, out_lens, attn_prior, return_attns=False):
+        """Flowtron.encode's work on checked inputs (lengths int32 on the device) -> (z [T, B, 80], zero past out_lens;
+        the flows' attention [B, T, L] zeroed outside each row's lengths, or None)."""
         T, dev = mel.size(2), mel.device
         speaker_ids = speaker_ids * 0 if self.dummy_speaker_embedding else speaker_ids
         speaker_vecs = self.speaker_embedding(speaker_ids)
         text = self.encoder.infer_ragged_tokens(text, self.embedding, in_lens).transpose(0, 1)
         encoder_outputs = torch.cat([text, speaker_vecs.expand(text.size(0), -1, -1)], 2)
         mask = ~(torch.arange(text.size(0), device=dev)[None, :] < in_lens[:, None])[..., None]
-        z = self._run_flows(mel.permute(2, 0, 1), encoder_outputs, mask, out_lens, attn_prior)[0]
+        out = self._run_flows(mel.permute(2, 0, 1), encoder_outputs, mask, out_lens, attn_prior)
         # forward leaves frames at or past out_lens[b] undefined
-        return z.masked_fill_(torch.arange(T, device=dev)[:, None, None] >= out_lens[None, :, None], 0.0)
+        past = torch.arange(T, device=dev)[:, None] >= out_lens[None, :]
+        z = out[0].masked_fill_(past[:, :, None], 0.0)
+        if not return_attns:
+            return z, None
+        outside = past.t()[:, :, None] | mask.transpose(1, 2)                 # [B, T, 1] | [B, 1, L]
+        return z, [a.masked_fill(outside, 0.0) for a in out[3]]
 
     def infer(self, residual, speaker_ids, text, temperature=1.0, gate_threshold=0.5, attns=None, attn_prior=None):
         """Texts of up to _lib.MAX_TEXT_LEN (1024) tokens; longer ones raise ValueError before any work."""
@@ -731,6 +759,76 @@ class Flowtron(nn.Module):
             residual, attn, lens = flow.infer_ragged(residual, encoder_outputs, in_lens, lens)
             attention_weights.append(attn.transpose(0, 1))
         return residual.permute(1, 2, 0), lens.long(), attention_weights
+
+    def infer_aligned(self, residual, speaker_ids, text, in_lens, attns, n_frames, gate_threshold=1.0):
+        """Inference over a padded batch with forced alignments: every flow uses the given attention weights instead of
+        computing its own, so each row keeps the text-to-frame timing of ``attns`` (voice conversion with the z of a recorded
+        utterance, rhythm transfer with a sampled z).
+
+        residual [B, 80, T] f32, speaker_ids [B], text [B, L] int64 (row b valid in [0, in_lens[b])), in_lens [B],
+        attns: one [B, Ta, L] f32 tensor per flow in flow-index order, Ta >= max n_frames -- what
+        ``encode(return_attns=True)`` returns -- n_frames [B]: frames of row b -> (mel [B, 80, T], mel_lens int64 [B]).
+
+        Row b of ``mel[:, :, :mel_lens[b]]`` equals ``infer(residual[b:b+1, :, :n_frames[b]], speaker_ids[b:b+1],
+        text[b:b+1, :in_lens[b]], gate_threshold=gate_threshold, attns=[a[b, :n_frames[b], :in_lens[b]] for a in attns])[0]``;
+        ``mel`` is zero past ``mel_lens[b]``.  Weights at tokens >= in_lens[b] and frames >= n_frames[b], padded text and
+        residual frames past n_frames[b] are never used.  The default gate_threshold of 1 disables the gate, so
+        ``mel_lens == n_frames``; below 1 a row stops where its gate fires.  The first flow applied gets the budgets
+        ``n_frames``, every later flow the previous flow's frame counts, on the device.
+
+        Texts of up to _lib.MAX_TEXT_LEN tokens, any B (slices of 16 utterances per kernel launch), rows in any length
+        order.  Host lengths are checked (ValueError unless 1 <= in_lens[b] <= L and 1 <= n_frames[b] <= min(T, Ta)); CUDA
+        length tensors are trusted and the call then makes no host synchronisation, so it can be captured in a CUDA graph."""
+        if residual.dim() != 3 or text.dim() != 2 or speaker_ids.dim() != 1:
+            raise ValueError("infer_aligned expects residual [B, n_mel, T], speaker_ids [B] and text [B, L]")
+        B, _, T = residual.shape
+        L = text.size(1)
+        _lib.check_text_len(L, "Flowtron.infer_aligned")
+        if text.size(0) != B or speaker_ids.size(0) != B or B < 1 or T < 1 or L < 1:
+            raise ValueError(f"batch sizes disagree or are empty: residual {tuple(residual.shape)}, "
+                             f"speaker_ids {tuple(speaker_ids.shape)}, text {tuple(text.shape)}")
+        if not isinstance(attns, (list, tuple)) or len(attns) != len(self.flows):
+            raise ValueError(f"attns must be a list of {len(self.flows)} tensors, one per flow")
+        Ta = attns[0].size(1) if torch.is_tensor(attns[0]) and attns[0].dim() == 3 else 0
+        for a in attns:
+            if not torch.is_tensor(a) or tuple(a.shape) != (B, Ta, L) or Ta < 1 or not a.is_floating_point():
+                raise ValueError(f"every attns[f] must be a float tensor [B, Ta, L] = ({B}, Ta, {L}), got "
+                                 f"{tuple(a.shape) if torch.is_tensor(a) else type(a).__name__}")
+        in_lens = _ragged_lengths(in_lens, B, L, "in_lens")
+        lens = _ragged_lengths(n_frames, B, min(T, Ta), "n_frames")
+        if not (residual.is_cuda and text.is_cuda and speaker_ids.is_cuda and all(a.is_cuda for a in attns)):
+            raise FlowtronB200Error("Flowtron.infer_aligned needs CUDA tensors: the sm_90a kernels are the only implementation")
+        dev = residual.device
+        in_lens = in_lens.to(device=dev, dtype=torch.int32)
+        lens = lens.to(device=dev, dtype=torch.int32)
+        with torch.no_grad():
+            speaker_ids = speaker_ids * 0 if self.dummy_speaker_embedding else speaker_ids
+            speaker_vecs = self.speaker_embedding(speaker_ids)
+            text = self.encoder.infer_ragged_tokens(text, self.embedding, in_lens).transpose(0, 1)
+            encoder_outputs = torch.cat([text, speaker_vecs.expand(text.size(0), -1, -1)], 2)
+            residual = residual.permute(2, 0, 1)
+            for f in reversed(range(len(self.flows))):
+                step = getattr(self.flows[f], "ar_step", self.flows[f])
+                if hasattr(step, 'gate_layer'):
+                    step.gate_threshold = gate_threshold
+                residual, _, lens = self.flows[f].infer_aligned(residual, encoder_outputs, in_lens, lens, attns[f])
+        return residual.permute(1, 2, 0), lens.long()
+
+    def convert(self, mel, speaker_ids, target_speaker_ids, text, in_lens, out_lens, attn_prior=None):
+        """Voice conversion of a padded batch of recorded utterances: each is mapped to z with its own speaker
+        (``encode``), then z is inverted with ``target_speaker_ids`` under the alignments the first direction found
+        (``infer_aligned``), so the converted utterance keeps the recording's timing.
+
+        mel [B, 80, T] f32, speaker_ids / target_speaker_ids [B], text [B, L] int64, in_lens [B], out_lens [B], attn_prior
+        [B, T, L] or None (used by the mel -> z direction only) -> mel_converted [B, 80, T], out_lens[b] frames per row, zero
+        past them.  With target_speaker_ids == speaker_ids the result is ``mel`` again up to rounding.
+
+        Arguments are checked as ``encode`` checks them; the gate is off.  With CUDA length tensors the whole call makes no
+        host synchronisation and can be captured in a CUDA graph."""
+        if target_speaker_ids.dim() != 1 or target_speaker_ids.size(0) != mel.size(0):
+            raise ValueError(f"target_speaker_ids must hold {mel.size(0)} values, got shape {tuple(target_speaker_ids.shape)}")
+        z, attns = self.encode(mel, speaker_ids, text, in_lens, out_lens, attn_prior, return_attns=True)
+        return self.infer_aligned(z, target_speaker_ids, text, in_lens, attns, out_lens)[0]
 
     @staticmethod
     def set_temperature_and_gate(flow, temperature, gate_threshold):

@@ -84,13 +84,34 @@ def ar_step_infer_ragged(step, residual, text, in_lens, frame_lens, reversed_fla
     residual [T,B,M] in natural time order (AR_Back_Step's reversal happens per row inside the C call), text [L,B,E],
     in_lens / frame_lens int32 CUDA [B] -> (out [T,B,M] zero past n_frames[b], attention [T,B,L] in generation order,
     n_frames int32 CUDA [B]).  No host synchronisation; batches above 16 run as slices of 16 that carry their lengths."""
+    return _infer_ragged(step, residual, text, in_lens, frame_lens, None, reversed_flag, "AR_Step.infer_ragged")
+
+
+def ar_step_infer_aligned(step, residual, text, in_lens, frame_lens, attns, reversed_flag=False):
+    """``ar_step_infer_ragged`` with forced alignments, over ft_ar_step_infer_aligned: row b equals its own B == 1
+    ``ar_step_infer(..., attns=attns[b, :frame_lens[b], :in_lens[b]])``.
+
+    attns f32 CUDA [B, Ta, L], Ta >= max frame_lens: row (b, i) holds the weights of generation step i of utterance b -- the
+    layout and, for an AR_Back_Step, the flipped per-row time order in which the flow's ``forward`` returns its attention,
+    so that tensor is read where it lies.  Weights at keys >= in_lens[b] or steps >= frame_lens[b] are never read.  The
+    returned attention [T,B,L] is the weights used."""
+    _lib.check_text_len(text.size(0), "AR_Step.infer_aligned")
+    B = residual.size(1)
+    if attns.dim() != 3 or attns.size(0) != B or attns.size(2) != text.size(0) or attns.size(1) < 1:
+        raise ValueError(f"attns must be [B, Ta, L] = ({B}, Ta, {text.size(0)}), got {tuple(attns.shape)}")
+    if not attns.is_cuda:
+        raise FlowtronB200Error("AR_Step.infer_aligned needs CUDA tensors: the sm_90a kernel is the only implementation")
+    return _infer_ragged(step, residual, text, in_lens, frame_lens, attns, reversed_flag, "AR_Step.infer_aligned")
+
+
+def _infer_ragged(step, residual, text, in_lens, frame_lens, attns, reversed_flag, where):
     if not residual.is_cuda:
-        raise FlowtronB200Error("AR_Step.infer_ragged needs CUDA tensors: the sm_90a kernel is the only implementation")
+        raise FlowtronB200Error(f"{where} needs CUDA tensors: the sm_90a kernel is the only implementation")
     T, B, M = residual.shape
     L, _, E = text.shape
     if B > 16:
-        parts = [ar_step_infer_ragged(step, residual[:, b0:b0 + 16], text[:, b0:b0 + 16], in_lens[b0:b0 + 16],
-                                      frame_lens[b0:b0 + 16], reversed_flag) for b0 in range(0, B, 16)]
+        parts = [_infer_ragged(step, residual[:, b0:b0 + 16], text[:, b0:b0 + 16], in_lens[b0:b0 + 16], frame_lens[b0:b0 + 16],
+                               None if attns is None else attns[b0:b0 + 16], reversed_flag, where) for b0 in range(0, B, 16)]
         return (torch.cat([p[0] for p in parts], 1), torch.cat([p[1] for p in parts], 1),
                 torch.cat([p[2] for p in parts], 0))
     dev = residual.device
@@ -103,7 +124,10 @@ def ar_step_infer_ragged(step, residual, text, in_lens, frame_lens, reversed_fla
     attn_out = torch.empty(T, B, L, device=dev)
     n_frames = torch.empty(B, dtype=torch.int32, device=dev)
     thr = float(getattr(step, 'gate_threshold', 0.5))
-    _lib.ar_step_infer_ragged(desc, weights, residual.detach().float().contiguous(), text.detach().float().contiguous(),
-                              in_lens.to(device=dev, dtype=torch.int32).contiguous(),
-                              frame_lens.to(device=dev, dtype=torch.int32).contiguous(), thr, out, attn_out, n_frames)
+    args = (desc, weights, residual.detach().float().contiguous(), text.detach().float().contiguous(),
+            in_lens.to(device=dev, dtype=torch.int32).contiguous(), frame_lens.to(device=dev, dtype=torch.int32).contiguous())
+    if attns is None:
+        _lib.ar_step_infer_ragged(*args, thr, out, attn_out, n_frames)
+    else:
+        _lib.ar_step_infer_aligned(*args, attns.detach().float().contiguous(), thr, out, attn_out, n_frames)
     return out, attn_out, n_frames

@@ -212,13 +212,29 @@ int ft_ar_step_infer(const FtArStepDesc* d, const FtArStepWeights* w, const floa
  *   out [T,B,M]: zero at t >= n_frames[b]; attn_out [T,B,L] in generation order, zero at i >= n_frames[b] and l >= in_lens[b];
  *   n_frames [B] int32 = min(gate stop (the frame that trips the gate is emitted), frame_lens[b]).
  *   Lengths must satisfy 1 <= in_lens[b] <= L and 1 <= frame_lens[b] <= T; they are read on the device only.
- *   Limits as ft_ar_step_infer: B <= 16, L <= FT_MAX_TEXT_LEN; d->has_prior must be 0 (no attn_prior, no forced
- *   alignments).  Flowtron.infer_batch, the host layer over this entry point, takes texts of up to 256 tokens.
+ *   Limits as ft_ar_step_infer: B <= 16, L <= FT_MAX_TEXT_LEN; d->has_prior must be 0 (no attn_prior; forced alignments
+ *   go through ft_ar_step_infer_aligned).  Flowtron.infer_batch, the host layer over this entry point, takes texts of up to 256 tokens.
  *   Two launches (the persistent kernel, then a small per-row flip / attention clear), no host synchronisation:
  *   CUDA-graph capturable. */
 int ft_ar_step_infer_ragged(const FtArStepDesc* d, const FtArStepWeights* w, const float* residual, const float* text,
                             const int* in_lens, const int* frame_lens, float gate_threshold, float* out, float* attn_out,
                             int* n_frames, void* scratch, void* stream);
+
+/* The ragged inverse with per-row FORCED ALIGNMENTS (voice conversion, rhythm transfer): everything as
+ * ft_ar_step_infer_ragged, except that the attention weights are given instead of computed (no query projection, scores,
+ * softmax or prior; context = weights . V), as ft_ar_step_infer does with attn_forced.
+ *   attn_forced [B,Ta,L] f32, batch-major, the layout ft_ar_step_fwd writes its attention in: row (b, i) holds the weights
+ *     of GENERATION STEP i of utterance b.  Generation steps are counted in the flow's own order: with d->reversed = 1, step
+ *     i produces natural frame frame_lens[b] - 1 - i, the order in which AR_Back_Step.forward returns its attention, so a
+ *     flow's forward attention feeds the same flow's inverse with no transpose or flip.
+ *   Ta >= max frame_lens[b] (>= d->T when frame_lens is NULL); only keys l < in_lens[b] of rows i < frame_lens[b] are
+ *     read, every other weight is 0 whatever the buffer holds.
+ *   attn_out [T,B,L]: the weights used, in generation order, zero at i >= n_frames[b] and l >= in_lens[b].
+ *   n_frames[b] = min(gate stop, frame_lens[b]): a gate_threshold >= 1 disables stopping.
+ *   Limits, scratch, launches and graph capture as ft_ar_step_infer_ragged; every L <= FT_MAX_TEXT_LEN. */
+int ft_ar_step_infer_aligned(const FtArStepDesc* d, const FtArStepWeights* w, const float* residual, const float* text,
+                             const int* in_lens, const int* frame_lens, const float* attn_forced, int Ta, float gate_threshold,
+                             float* out, float* attn_out, int* n_frames, void* scratch, void* stream);
 
 /* TacotronSTFT.mel_spectrogram (audio_processing.py:117-134) for a ragged batch.  wav: concatenated utterances
  * (f32 in [-1,1]); sample_offsets / frame_offsets: device int64 [n_utt+1] prefix sums (frames of utterance u =

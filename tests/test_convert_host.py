@@ -1,0 +1,182 @@
+"""CPU: argument checks of Flowtron.infer_aligned / convert / encode(return_attns=), the oracle's restatement of their
+contract against the reference-generated fixtures (tests/make_golden_convert.py), what those fixtures cover, and the
+register budget of the forced-alignment instantiations of the inference kernel."""
+import os
+import re
+import shutil
+import subprocess
+
+import numpy as np
+import pytest
+import torch
+
+from conftest import GOLDEN, ROOT
+from flowtron_b200 import synth
+
+NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
+HAVE_NVCC = os.path.exists(NVCC) or shutil.which("nvcc") is not None
+TAGS = ["f2", "f3", "long"]
+
+
+def _load(tag):
+    return dict(np.load(os.path.join(GOLDEN, f"convert_{tag}.npz")))
+
+
+def _params(g):
+    cfg = dict(synth.DEFAULT_MODEL_CONFIG, n_flows=int(g["cfg_n_flows"]), n_speakers=int(g["n_speakers"]))
+    p = synth.synth_params(cfg, int(g["seed"]))
+    kb = [k for k in p if k.endswith("gate_layer.linear_layer.bias")][0]
+    p[kb] = torch.full_like(p[kb], float(g["gate_bias"]))
+    return cfg, p
+
+
+@pytest.fixture(scope="module")
+def cpu_model():
+    from flowtron_b200.flowtron import Flowtron
+    cfg = dict(synth.DEFAULT_MODEL_CONFIG, n_flows=2, n_speakers=2)
+    m = Flowtron(**cfg)
+    m.load_state_dict(synth.synth_params(cfg, 3), strict=True)
+    return m.eval()
+
+
+def test_infer_aligned_argument_validation(cpu_model):
+    from flowtron_b200._lib import FlowtronB200Error
+    B, T, L = 3, 20, 9
+    res = torch.zeros(B, 80, T)
+    spk = torch.zeros(B, dtype=torch.long)
+    text = torch.zeros(B, L, dtype=torch.long)
+    attns = [torch.zeros(B, T, L)] * 2
+    ok = dict(in_lens=[9, 4, 4], attns=attns, n_frames=[20, 7, 13])
+    bad = [
+        dict(ok, in_lens=[9, 4]),                                # wrong count
+        dict(ok, in_lens=[9, 0, 4]),                             # empty text
+        dict(ok, in_lens=[9, 10, 4]),                            # longer than L
+        dict(ok, in_lens=[9.0, 4.0, 4.0]),
+        dict(ok, n_frames=[20, 21, 5]),                          # above T
+        dict(ok, n_frames=[20, 0, 5]),
+        dict(ok, n_frames=torch.tensor([20, 5])),
+        dict(ok, attns=attns[:1]),                               # one map per flow
+        dict(ok, attns=attns + attns[:1]),
+        dict(ok, attns=attns[0]),                                # not a list
+        dict(ok, attns=[torch.zeros(B, T, L), torch.zeros(B, T, L + 1)]),
+        dict(ok, attns=[torch.zeros(T, B, L)] * 2),              # time-major
+        dict(ok, attns=[torch.zeros(B, T, L, dtype=torch.long)] * 2),
+        dict(ok, attns=[torch.zeros(B, 12, L)] * 2),             # covers 12 frames, row 0 wants 20
+    ]
+    for kw in bad:
+        with pytest.raises(ValueError):
+            cpu_model.infer_aligned(res, spk, text, **kw)
+    with pytest.raises(ValueError):                              # batch sizes disagree
+        cpu_model.infer_aligned(res[:2], spk, text, **ok)
+    with pytest.raises(ValueError, match="1024"):                # over MAX_TEXT_LEN, before any device work
+        cpu_model.infer_aligned(res, spk, torch.zeros(B, 1025, dtype=torch.long), [9, 4, 4], [torch.zeros(B, T, 1025)] * 2,
+                                [20, 7, 13])
+    # valid arguments, but CPU tensors: there is no CPU implementation
+    with pytest.raises(FlowtronB200Error):
+        cpu_model.infer_aligned(res, spk, text, **ok)
+    with pytest.raises(FlowtronB200Error):                       # shorter maps are fine when no row needs more
+        cpu_model.infer_aligned(res, spk, text, [9, 4, 4], [torch.zeros(B, 12, L)] * 2, torch.tensor([12, 7, 9]))
+    with pytest.raises(FlowtronB200Error):                       # texts past 256 tokens are accepted
+        cpu_model.infer_aligned(res, spk, torch.zeros(B, 300, dtype=torch.long), [300, 4, 4], [torch.zeros(B, T, 300)] * 2,
+                                [20, 7, 13])
+
+
+def test_convert_and_encode_argument_validation(cpu_model):
+    from flowtron_b200._lib import FlowtronB200Error
+    B, T, L = 3, 20, 9
+    mel = torch.zeros(B, 80, T)
+    spk = torch.zeros(B, dtype=torch.long)
+    text = torch.zeros(B, L, dtype=torch.long)
+    with pytest.raises(ValueError):
+        cpu_model.convert(mel, spk, spk[:2], text, [9, 4, 4], [20, 7, 13])
+    with pytest.raises(ValueError):
+        cpu_model.convert(mel, spk, spk, text, [9, 4, 4], [20, 21, 13])
+    with pytest.raises(ValueError):
+        cpu_model.convert(mel, spk, spk, text, [9, 10, 4], [20, 7, 13])
+    with pytest.raises(ValueError):
+        cpu_model.convert(mel, spk, spk, text, [9, 4, 4], [20, 7, 13], attn_prior=torch.zeros(B, T, L + 1))
+    with pytest.raises(FlowtronB200Error):
+        cpu_model.convert(mel, spk, spk, text, [9, 4, 4], [20, 7, 13])
+    with pytest.raises(ValueError):
+        cpu_model.encode(mel, spk, text, [9, 4, 4], [20, 21, 13], return_attns=True)
+    with pytest.raises(FlowtronB200Error):
+        cpu_model.encode(mel, spk, text, [9, 4, 4], [20, 7, 13], return_attns=True)
+
+
+def test_flow_infer_aligned_argument_validation(cpu_model):
+    from flowtron_b200._lib import FlowtronB200Error
+    lens = torch.tensor([8, 5], dtype=torch.int32)
+    for flow in cpu_model.flows:
+        with pytest.raises(ValueError):                          # [T, B, L] instead of [B, Ta, L]
+            flow.infer_aligned(torch.zeros(8, 2, 80), torch.zeros(6, 2, 640), lens, lens, torch.zeros(8, 2, 6))
+        with pytest.raises(ValueError, match="1024"):
+            flow.infer_aligned(torch.zeros(8, 2, 80), torch.zeros(1025, 2, 640), lens, lens, torch.zeros(2, 8, 1025))
+        with pytest.raises(FlowtronB200Error):
+            flow.infer_aligned(torch.zeros(8, 2, 80), torch.zeros(6, 2, 640), lens, lens, torch.zeros(2, 8, 6))
+
+
+@pytest.mark.parametrize("tag", TAGS)
+def test_oracle_convert_matches_reference_fixtures(tag):
+    from convert_oracle import flowtron_convert, flowtron_infer_aligned
+    g = _load(tag)
+    _, p = _params(g)
+    torch.set_num_threads(max(1, min(8, os.cpu_count() or 1)))
+    t = lambda k: torch.from_numpy(g[k])
+    in_lens, out_lens = g["in_lens"].tolist(), g["out_lens"].tolist()
+    with torch.no_grad():
+        mel, z, attns = flowtron_convert(p, t("mel"), t("speaker_ids"), t("target_speaker_ids"), t("text"), in_lens, out_lens)
+    rel = lambda x, ref: (x - ref).abs().max().item() / ref.abs().max().item()
+    assert rel(z, t("z")) <= 1e-5
+    for f, a in enumerate(attns):
+        assert (a - t(f"attn_{f}")).abs().max().item() <= 1e-5, f
+    assert rel(mel, t("mel_converted")) <= 1e-5
+    if "mel_rhythm" in g:
+        with torch.no_grad():
+            rhy = flowtron_infer_aligned(p, t("noise"), t("target_speaker_ids"), t("text"), in_lens,
+                                         [t(f"attn_{f}") for f in range(len(attns))], out_lens)
+        assert rel(rhy, t("mel_rhythm")) <= 1e-5
+
+
+def test_fixtures_cover_their_cases():
+    for tag in TAGS:
+        g = _load(tag)
+        n_flows, B = int(g["cfg_n_flows"]), len(g["in_lens"])
+        assert (g["speaker_ids"] != g["target_speaker_ids"]).all()               # every row changes voice
+        assert len(set(g["speaker_ids"].tolist())) >= 2 and len(set(g["target_speaker_ids"].tolist())) >= 2
+        assert g["mel"].shape == g["mel_converted"].shape == g["z"].shape
+        for b in range(B):
+            nt, nl = int(g["out_lens"][b]), int(g["in_lens"][b])
+            assert (g["mel_converted"][b, :, nt:] == 0).all() and np.abs(g["mel_converted"][b, :, :nt]).max() > 0
+            assert np.abs(g["mel_converted"][b, :, :nt] - g["mel"][b, :, :nt]).max() > 0.1    # the voice matters
+            for f in range(n_flows):
+                a = g[f"attn_{f}"][b]
+                assert (a[nt:] == 0).all() and (a[:, nl:] == 0).all()
+                assert np.abs(a[:nt].sum(-1) - 1).max() <= 1e-5
+        for f in range(1, n_flows, 2):                                           # a back step's map is not the forward step's
+            assert np.abs(g[f"attn_{f}"] - g[f"attn_{f - 1}"]).max() > 1e-3
+    for tag in ("f2", "f3"):
+        g = _load(tag)
+        for k in ("in_lens", "out_lens"):
+            assert (np.diff(g[k]) > 0).any() and (np.diff(g[k]) < 0).any(), (tag, k)   # not sorted
+    assert int(_load("f2")["cfg_n_flows"]) == 2 and int(_load("f3")["cfg_n_flows"]) == 3
+    assert "mel_rhythm" in _load("f2")                                           # z replaced by fresh noise
+    g = _load("long")
+    assert g["text"].shape[1] > 256 and (g["in_lens"] > 256).all() and g["in_lens"][0] != g["in_lens"][1]
+    for tag in TAGS:
+        assert os.path.getsize(os.path.join(GOLDEN, f"convert_{tag}.npz")) < 1 << 20
+
+
+@pytest.mark.skipif(not HAVE_NVCC, reason="nvcc not available")
+def test_aligned_kernels_fit_the_register_budget(tmp_path):
+    """infer_aligned_kernel<batch > 8, long text>: four instantiations of the persistent kernel's body, 512 threads each, so
+    128 registers at most, and no spills."""
+    r = subprocess.run([NVCC, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "--expt-relaxed-constexpr",
+                        "-Xptxas", "-v", "-c", os.path.join(ROOT, "flowtron_b200", "csrc", "infer.cu"), "-o",
+                        str(tmp_path / "infer.o")], capture_output=True, text=True)
+    assert r.returncode == 0, r.stderr
+    logs = [s for s in r.stderr.split("Compiling entry function") if "infer_aligned_kernel" in s.splitlines()[0]]
+    assert len(logs) == 4, r.stderr
+    for log in logs:
+        regs = int(re.search(r"Used (\d+) registers", log).group(1))
+        spill = re.search(r"(\d+) bytes spill stores, (\d+) bytes spill loads", log)
+        assert regs <= 128 and spill.groups() == ("0", "0"), log
