@@ -134,15 +134,9 @@ def _declare(L):
     L.ft_ar_step_bwd_attn_lstm.restype = c_int
     L.ft_ar_step_infer_scratch_bytes.argtypes = [POINTER(FtArStepDesc)]
     L.ft_ar_step_infer_scratch_bytes.restype = c_size_t
-    L.ft_ar_step_infer.argtypes = [POINTER(FtArStepDesc), POINTER(FtArStepWeights), c_void_p, c_void_p, c_void_p, c_void_p,
-                                   c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
+    L.ft_ar_step_infer.argtypes = [POINTER(FtArStepDesc), POINTER(FtArStepWeights)] + [c_void_p] * 6 + \
+        [c_int, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
     L.ft_ar_step_infer.restype = c_int
-    L.ft_ar_step_infer_ragged.argtypes = [POINTER(FtArStepDesc), POINTER(FtArStepWeights), c_void_p, c_void_p, c_void_p,
-                                          c_void_p, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
-    L.ft_ar_step_infer_ragged.restype = c_int
-    L.ft_ar_step_infer_aligned.argtypes = [POINTER(FtArStepDesc), POINTER(FtArStepWeights), c_void_p, c_void_p, c_void_p,
-                                           c_void_p, c_void_p, c_int, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
-    L.ft_ar_step_infer_aligned.restype = c_int
     L.ft_mel_scratch_bytes.argtypes = [c_int, c_longlong]
     L.ft_mel_scratch_bytes.restype = c_size_t
     L.ft_mel_spectrogram.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_void_p, c_void_p, c_void_p,
@@ -427,32 +421,15 @@ def radam_step_raw(p_ptr, g_ptr, m_ptr, v_ptr, n, beta1, beta2, eps, weight_deca
                               c_void_p(coef_ptr) if coef_ptr else None, stream_ptr()), "ft_radam_step")
 
 
-def ar_step_infer(desc, weights, residual, text, prior, attn_forced, gate_threshold, out, attn_out, n_frames):
+def ar_step_infer(desc, weights, residual, text, in_lens, frame_lens, prior, attn_forced, gate_threshold, out, attn_out,
+                  n_frames):
+    """in_lens / frame_lens: int32 CUDA [B] or None (all L / all T); attn_forced: f32 CUDA [B, Ta, L] contiguous or None."""
     nbytes = int(lib().ft_ar_step_infer_scratch_bytes(byref(desc)))
     scratch = scratch_buffer(nbytes, residual.device)
-    check(lib().ft_ar_step_infer(byref(desc), byref(weights), ptr(residual), ptr(text), ptr(prior), ptr(attn_forced),
-                                 float(gate_threshold), ptr(out), ptr(attn_out), ptr(n_frames), ptr(scratch), stream_ptr()),
-          "ft_ar_step_infer")
-
-
-def ar_step_infer_ragged(desc, weights, residual, text, in_lens, frame_lens, gate_threshold, out, attn_out, n_frames):
-    """in_lens / frame_lens: int32 CUDA [B] (or None: all L / all T); desc.reversed selects the per-row time reversal."""
-    nbytes = int(lib().ft_ar_step_infer_scratch_bytes(byref(desc)))
-    scratch = scratch_buffer(nbytes, residual.device)
-    check(lib().ft_ar_step_infer_ragged(byref(desc), byref(weights), ptr(residual), ptr(text), ptr(in_lens), ptr(frame_lens),
-                                        float(gate_threshold), ptr(out), ptr(attn_out), ptr(n_frames), ptr(scratch),
-                                        stream_ptr()), "ft_ar_step_infer_ragged")
-
-
-def ar_step_infer_aligned(desc, weights, residual, text, in_lens, frame_lens, attn_forced, gate_threshold, out, attn_out,
-                          n_frames):
-    """As ar_step_infer_ragged with forced alignments: attn_forced f32 CUDA [B, Ta, L] contiguous, row (b, i) = generation
-    step i of utterance b, Ta >= max frame_lens."""
-    nbytes = int(lib().ft_ar_step_infer_scratch_bytes(byref(desc)))
-    scratch = scratch_buffer(nbytes, residual.device)
-    check(lib().ft_ar_step_infer_aligned(byref(desc), byref(weights), ptr(residual), ptr(text), ptr(in_lens), ptr(frame_lens),
-                                         ptr(attn_forced), int(attn_forced.size(1)), float(gate_threshold), ptr(out),
-                                         ptr(attn_out), ptr(n_frames), ptr(scratch), stream_ptr()), "ft_ar_step_infer_aligned")
+    Ta = 0 if attn_forced is None else int(attn_forced.size(1))
+    check(lib().ft_ar_step_infer(byref(desc), byref(weights), ptr(residual), ptr(text), ptr(in_lens), ptr(frame_lens), ptr(prior),
+                                 ptr(attn_forced), Ta, float(gate_threshold), ptr(out), ptr(attn_out), ptr(n_frames),
+                                 ptr(scratch), stream_ptr()), "ft_ar_step_infer")
 
 
 def mel_spectrogram(wav, sample_offsets, frame_offsets, n_utt, total_frames, window, basis, band_lo, band_hi, n_fft, hop,

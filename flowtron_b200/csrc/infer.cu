@@ -49,14 +49,16 @@ struct InferParams {
     const float *bA, *b0, *b1, *bd1, *bd2, *bc;
     const float *v, *wg, *bg;
     const float* Kp; const float* Vp;      // [L*B, A] projected once
-    const float* residual;                 // [T,B,M] flow-time order
+    const float* residual;                 // [T,B,M] natural time order
     const float* prior;                    // [B,T,L] (row i used at frame i) or null
-    const float* attn_forced;              // [T,B,L] forced alignments (flowtron.py:585-588, 797): scoring is skipped
+    // kForced: forced alignments (flowtron.py:585-588, 797), batch-major [B,Ta,L], each row in its flow's own generation
+    // order; step i of utterance b reads keys l < in_lens[b] of row (b, i) while i < frame_lens[b]: every other weight is 0
+    // whatever the buffer holds
+    const float* attn_forced;
     float inv_temperature, gate_threshold;
     int has_gate;
-    // ragged batches (ft_ar_step_infer_ragged; all null / 0 for ft_ar_step_infer): keys l >= in_lens[b] take no part in the
-    // softmax; utterance b generates at most frame_lens[b] frames (default T); reversed: frame i reads residual row
-    // frame_lens[b] - 1 - i (the residual is then in natural time order)
+    // keys l >= in_lens[b] take no part in the softmax; utterance b generates at most frame_lens[b] frames (null: L / T);
+    // reversed: frame i reads residual row frame_lens[b] - 1 - i
     const int* in_lens;
     const int* frame_lens;
     int reversed;
@@ -76,10 +78,7 @@ struct InferParams {
     uint32_t* alive;                       // [B] per slot: 1 while the sample keeps generating after this frame, 0 once stopped
     int* status;
     long long* trace;                      // debug: [T][32] clock64 stamps of CTA 0 (tools/trace_infer.py), or null
-    // ft_ar_step_infer_aligned (the kAligned kernels): attn_forced is batch-major [B,Ta,L], each row in its flow's own generation
-    // order; step i of utterance b reads keys l < in_lens[b] of row (b, i) while i < frame_lens[b]: every other weight is 0
-    // whatever the buffer holds
-    int Ta;
+    int Ta;                                // rows per utterance of attn_forced
 };
 
 static long long* g_infer_trace = nullptr;
@@ -391,9 +390,9 @@ __device__ __forceinline__ float residual_at(const InferParams& p, int i, int b,
     return p.residual[(static_cast<long long>(t) * p.B + b) * p.M + m];
 }
 
-// kAligned: the forced weights of utterance b at generation step i (row (b, i) of the batch-major buffer) and how many of its
+// kForced: the forced weights of utterance b at generation step i (row (b, i) of the batch-major buffer) and how many of its
 // keys are read: in_lens[b], none once the row's frame budget is spent.
-__device__ __forceinline__ const float* aligned_row(const InferParams& p, int i, int b, int Lb, int& Lf) {
+__device__ __forceinline__ const float* forced_row(const InferParams& p, int i, int b, int Lb, int& Lf) {
     Lf = (p.frame_lens && i >= p.frame_lens[b]) ? 0 : Lb;
     return p.attn_forced + (static_cast<long long>(b) * p.Ta + i) * p.L;
 }
@@ -401,10 +400,10 @@ __device__ __forceinline__ const float* aligned_row(const InferParams& p, int i,
 // Long texts (kLong, L > LMAX): warp 0 runs the same softmax / prior posterior / forced alignment over the row staged in
 // shared memory, 32 keys per pass, instead of holding it in registers.  Each lane handles the same keys in the same order
 // as the register path, so the two agree bit for bit where both apply.
-template <bool kAligned>
-__device__ __forceinline__ void attn_row_long(const InferParams& p, float* se, int i, int b, long long cur, bool forced, int Lb) {
+template <bool kForced>
+__device__ __forceinline__ void attn_row_long(const InferParams& p, float* se, int i, int b, long long cur, int Lb) {
     const int lane = threadIdx.x & 31;
-    if (!forced) {
+    if (!kForced) {
         float mx = -INFINITY;
         for (int l = lane; l < p.L; l += 32) {
             const float x = l < Lb ? poll_f32(SL(p.e, cur) + b * p.L + l, p.status, 303) : -INFINITY;
@@ -436,12 +435,10 @@ __device__ __forceinline__ void attn_row_long(const InferParams& p, float* se, i
             const float inv2 = 1.f / s2;
             for (int l = lane; l < p.L; l += 32) se[l] *= inv2;
         }
-    } else if (kAligned) {
-        int Lf;
-        const float* fr = aligned_row(p, i, b, Lb, Lf);
-        for (int l = lane; l < p.L; l += 32) se[l] = l < Lf ? fr[l] : 0.f;
     } else {
-        for (int l = lane; l < p.L; l += 32) se[l] = p.attn_forced[(static_cast<long long>(i) * p.B + b) * p.L + l];
+        int Lf;
+        const float* fr = forced_row(p, i, b, Lb, Lf);
+        for (int l = lane; l < p.L; l += 32) se[l] = l < Lf ? fr[l] : 0.f;
     }
 }
 
@@ -449,19 +446,19 @@ __device__ __forceinline__ void attn_row_long(const InferParams& p, float* se, i
 // prior posterior -- or the forced alignment), all 16 warps then take L/16 keys each (every V load of the CTA in flight at
 // once), partial sums meet in shared memory.  Writes ctx (fp16 for lstm layer 0, fp32 for the gate) and, from slice 0, the
 // attention weights.  (One CTA per utterance doing all 640 channels would pull 256 KB through one SM.)
-template <int CW, bool kLong, bool kAligned>
-__device__ __forceinline__ void context_item(const InferParams& p, float* sf, int i, int b, int s, long long cur, long long nxt, bool forced) {
+template <int CW, bool kLong, bool kForced>
+__device__ __forceinline__ void context_item(const InferParams& p, float* sf, int i, int b, int s, long long cur, long long nxt) {
     constexpr int NV = CW / 32;                                    // channels per lane
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     float* se = sf; float* sp = sf + (kLong ? LMAX_LONG : LMAX);   // attn [LMAX or LMAX_LONG], partials [16 warps][CW]
     const int Lb = p.in_lens ? p.in_lens[b] : p.L;                 // key mask: tokens l >= Lb get weight 0 (as if L were Lb)
     if (kLong && warp == 0) {
-        attn_row_long<kAligned>(p, se, i, b, cur, forced, Lb);
+        attn_row_long<kForced>(p, se, i, b, cur, Lb);
         if (s == 0)
             for (int l = lane; l < p.L; l += 32) p.attn_out[(static_cast<long long>(i) * p.B + b) * p.L + l] = se[l];
     } else if (warp == 0) {
         float w[8];
-        if (!forced) {                                            // softmax over L in registers: lane holds l = lane + 32 jj
+        if (!kForced) {                                           // softmax over L in registers: lane holds l = lane + 32 jj
             float mx = -INFINITY;
 #pragma unroll
             for (int jj = 0; jj < 8; ++jj) {
@@ -502,14 +499,11 @@ __device__ __forceinline__ void context_item(const InferParams& p, float* sf, in
 #pragma unroll
                 for (int jj = 0; jj < 8; ++jj) w[jj] *= inv2;
             }
-        } else if (kAligned) {
+        } else {
             int Lf;
-            const float* fr = aligned_row(p, i, b, Lb, Lf) + lane;
+            const float* fr = forced_row(p, i, b, Lb, Lf) + lane;
 #pragma unroll
             for (int jj = 0; jj < 8; ++jj) w[jj] = lane + 32 * jj < Lf ? __ldg(fr + 32 * jj) : 0.f;
-        } else {
-#pragma unroll
-            for (int jj = 0; jj < 8; ++jj) { const int l = lane + 32 * jj; w[jj] = l < p.L ? p.attn_forced[(static_cast<long long>(i) * p.B + b) * p.L + l] : 0.f; }
         }
 #pragma unroll
         for (int jj = 0; jj < 8; ++jj) {
@@ -561,11 +555,12 @@ __device__ __forceinline__ void context_item(const InferParams& p, float* sf, in
     __syncthreads();
 }
 
-// kLong: texts of LMAX < L <= LMAX_LONG keys (context_item's softmax over a shared-memory row): infer_long_kernel.  The
-// L <= LMAX instantiations are infer_kernel, the short-text kernels.  kAligned: ft_ar_step_infer_aligned's forced alignments
-// (always forced, so the query / score phases are not compiled in): infer_aligned_kernel.
-template <bool kB16, bool kLong, bool kAligned>
-__device__ __forceinline__ void infer_body(const InferParams& p) {
+// kB16: batches of 9-16 utterances (the mma's upper 8 rows are live).  kLong: texts of LMAX < L <= LMAX_LONG keys
+// (context_item's softmax over a shared-memory row).  kForced: attention weights given in attn_forced, so the query / score
+// phases are not compiled in.
+template <bool kB16, bool kLong, bool kForced>
+__global__ void __launch_bounds__(INF_THREADS, 1)
+infer_kernel(InferParams p) {
     extern __shared__ __align__(16) uint8_t smem_raw[];
     __half* sx = reinterpret_cast<__half*>(smem_raw);                          // [16][KP] fp16 activations of the phase
     float* spart = reinterpret_cast<float*>(sx + 16 * KP);                     // [16 warps][32 lanes][4] partial accumulators
@@ -582,7 +577,6 @@ __device__ __forceinline__ void infer_body(const InferParams& p) {
     // by a store, and the ring-slot reuse argument relies on read -> store chains)
     const bool act_lstm = static_cast<int>(blockIdx.x) * 4 < IH / 2, act_q = static_cast<int>(blockIdx.x) < p.A / 8;
     const bool act_dense = static_cast<int>(blockIdx.x) < IH / 8, act_conv = static_cast<int>(blockIdx.x) < p.M / 4;
-    const bool forced = kAligned || p.attn_forced != nullptr;    // `attn` given (flowtron.py:585-588): no query / score / softmax / prior
     // context work items: (utterance, channel slice); 64-channel slices unless that needs a second pass over the grid
     const bool wide_ctx = (p.A % 128 == 0) && p.B * (p.A / 64) > static_cast<int>(gridDim.x);
     Prefetch pf;
@@ -609,10 +603,10 @@ __device__ __forceinline__ void infer_body(const InferParams& p) {
         mv_phase<kB16>(p.wA, IH / 2, nmA, 4, spart, sx, pf, [&](int task, float (&d)[4], bool first) {
             lstm_epi(p, task, d, p.bA, p.cA, SL(p.hA, cur), SL(p.hA, nxt), SL(p.hA16, cur), SL(p.hA16, nxt), first, cpre, bpre);
         });
-        if (forced) mv_prefetch(pf, p.w0, IH / 2, nm0, 4); else mv_prefetch(pf, p.wq, p.A / 8, nmd, INF_WARPS);
+        if (kForced) mv_prefetch(pf, p.w0, IH / 2, nm0, 4); else mv_prefetch(pf, p.wq, p.A / 8, nmd, INF_WARPS);
         IT_TRACE(2);
 
-        if (!forced) {
+        if (!kForced) {
             // ---- P2 query projection (no bias)
             if (act_q) stage3<false, kB16>(sx, 0, SL(p.hA16, cur_r), IH, IH, 0, nullptr, 0, 0, 0, nullptr, 0, 0, p.B, p.status);
             __syncthreads();
@@ -663,8 +657,8 @@ __device__ __forceinline__ void infer_body(const InferParams& p) {
             IT_TRACE(6);
         }
         // ---- P3b softmax + context, one (utterance, channel slice) item per CTA
-        if (wide_ctx) { for (int it = blockIdx.x; it < p.B * (p.A / 128); it += gridDim.x) context_item<128, kLong, kAligned>(p, sf, i, it / (p.A / 128), it % (p.A / 128), cur, nxt, forced); }
-        else          { for (int it = blockIdx.x; it < p.B * (p.A / 64); it += gridDim.x) context_item<64, kLong, kAligned>(p, sf, i, it / (p.A / 64), it % (p.A / 64), cur, nxt, forced); }
+        if (wide_ctx) { for (int it = blockIdx.x; it < p.B * (p.A / 128); it += gridDim.x) context_item<128, kLong, kForced>(p, sf, i, it / (p.A / 128), it % (p.A / 128), cur, nxt); }
+        else          { for (int it = blockIdx.x; it < p.B * (p.A / 64); it += gridDim.x) context_item<64, kLong, kForced>(p, sf, i, it / (p.A / 64), it % (p.A / 64), cur, nxt); }
         IT_TRACE(7);
         // ---- P4 lstm layer 0 on [hA ; ctx ; h0_{i-1}]
         lstm_pre(p, p.b0, p.c0, cpre, bpre);
@@ -789,18 +783,6 @@ __device__ __forceinline__ void infer_body(const InferParams& p) {
     }
 }
 
-template <bool kB16>
-__global__ void __launch_bounds__(INF_THREADS, 1)
-infer_kernel(InferParams p) { infer_body<kB16, false, false>(p); }
-
-template <bool kB16>
-__global__ void __launch_bounds__(INF_THREADS, 1)
-infer_long_kernel(InferParams p) { infer_body<kB16, true, false>(p); }
-
-template <bool kB16, bool kLong>
-__global__ void __launch_bounds__(INF_THREADS, 1)
-infer_aligned_kernel(InferParams p) { infer_body<kB16, kLong, true>(p); }
-
 // ------------------------------------------------------------------------------------------------ weight packing
 // dst[task][m][n][kk] (fp16) <- W[row(task, n)][32 m + kk] over the virtual K = [A part (Ka real columns, padded to Kap) ; B part]
 //   kind 0: LSTM      row = (n % 4) * 1024 + 2 task + n / 4        (rows i0,f0,g0,o0,i1,f1,g1,o1)
@@ -876,10 +858,10 @@ static InferScratch plan_infer(const FtArStepDesc& d, uint8_t* base) {
     return s;
 }
 
-// After a ragged launch: row (i, b) with i >= n_frames[b] gets zero attention weights; a reversed flow's emitted frames are
-// flipped within n_frames[b] (frame j <-> n - 1 - j, swapped by the CTA that owns the lower of the two rows).
-__global__ void infer_ragged_finish_kernel(float* __restrict__ out, float* __restrict__ attn_out, const int* __restrict__ n_frames,
-                                           int T, int B, int M, int L, int reversed) {
+// After the persistent kernel: row (i, b) with i >= n_frames[b] gets zero attention weights; a reversed flow's emitted frames
+// are flipped within n_frames[b] (frame j <-> n - 1 - j, swapped by the CTA that owns the lower of the two rows).
+__global__ void infer_finish_kernel(float* __restrict__ out, float* __restrict__ attn_out, const int* __restrict__ n_frames,
+                                    int T, int B, int M, int L, int reversed) {
     for (int row = blockIdx.x; row < T * B; row += gridDim.x) {
         const int i = row / B, b = row - i * B, n = n_frames[b];
         if (i >= n) {
@@ -893,8 +875,11 @@ __global__ void infer_ragged_finish_kernel(float* __restrict__ out, float* __res
 }
 
 static int infer_impl(const FtArStepDesc* d, const FtArStepWeights* w, const float* residual, const float* text,
-                      const float* attn_prior, const float* attn_forced, int Ta, const int* in_lens, const int* frame_lens,
-                      int reversed, float gate_threshold, float* out, float* attn_out, int* n_frames, void* scratch, void* stream) {
+                      const int* in_lens, const int* frame_lens, const float* attn_prior, const float* attn_forced, int Ta,
+                      float gate_threshold, float* out, float* attn_out, int* n_frames, void* scratch, void* stream) {
+    if (!d || !w || !residual || !text || !out || !attn_out || !n_frames || !scratch) return ft_set_error("ft_ar_step_infer: NULL argument");
+    if (attn_forced && (Ta < 1 || (!frame_lens && Ta < d->T)))
+        return ft_set_error("ft_ar_step_infer: attn_forced must cover every frame budget (Ta >= max frame_lens)");
     if (d->n_hidden != IH) return ft_set_error("infer: n_hidden must be 1024");
     if (d->L > LMAX_LONG) return ft_set_error("infer: L > FT_MAX_TEXT_LEN (1024) not supported");
     if (d->B > 16) return ft_set_error("infer: batch > 16 per call not supported (run the batch in slices of 16)");
@@ -934,8 +919,8 @@ static int infer_impl(const FtArStepDesc* d, const FtArStepWeights* w, const flo
     p.bA = s.bA; p.b0 = s.b0; p.b1 = s.b1; p.bd1 = s.bd1; p.bd2 = s.bd2; p.bc = s.bc;
     p.v = w->att_v; p.wg = w->gate_w; p.bg = w->gate_b;
     p.Kp = s.Kp; p.Vp = s.Vp; p.residual = residual; p.prior = d->has_prior ? attn_prior : nullptr;
-    p.attn_forced = attn_forced; p.Ta = Ta;                      // Ta > 0: batch-major forced alignments, the kAligned kernels
-    p.in_lens = in_lens; p.frame_lens = frame_lens; p.reversed = reversed;
+    p.attn_forced = attn_forced; p.Ta = Ta;
+    p.in_lens = in_lens; p.frame_lens = frame_lens; p.reversed = d->reversed ? 1 : 0;
     p.inv_temperature = 1.0f / d->temperature; p.gate_threshold = gate_threshold;
     p.has_gate = d->has_gate && w->gate_w;
     p.out = out; p.attn_out = attn_out; p.n_frames = n_frames;
@@ -971,11 +956,10 @@ static int infer_impl(const FtArStepDesc* d, const FtArStepWeights* w, const flo
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     if (sms < B) return ft_set_error("infer: fewer SMs than utterances");
     const bool long_text = d->L > LMAX;
-    void* fn = long_text ? (B > 8 ? reinterpret_cast<void*>(infer_long_kernel<true>) : reinterpret_cast<void*>(infer_long_kernel<false>))
-                         : (B > 8 ? reinterpret_cast<void*>(infer_kernel<true>) : reinterpret_cast<void*>(infer_kernel<false>));
-    if (Ta > 0)
-        fn = long_text ? (B > 8 ? reinterpret_cast<void*>(infer_aligned_kernel<true, true>) : reinterpret_cast<void*>(infer_aligned_kernel<false, true>))
-                       : (B > 8 ? reinterpret_cast<void*>(infer_aligned_kernel<true, false>) : reinterpret_cast<void*>(infer_aligned_kernel<false, false>));
+    using Kernel = void (*)(InferParams);
+    static const Kernel kernels[2][2][2] = {{{infer_kernel<false, false, false>, infer_kernel<false, false, true>}, {infer_kernel<false, true, false>, infer_kernel<false, true, true>}},
+                                            {{infer_kernel<true, false, false>, infer_kernel<true, false, true>}, {infer_kernel<true, true, false>, infer_kernel<true, true, true>}}};
+    void* fn = reinterpret_cast<void*>(kernels[B > 8][long_text][attn_forced != nullptr]);
     const int smem = 16 * KP * 2 + INF_WARPS * 128 * 4 + ((long_text ? LMAX_LONG : LMAX) + INF_WARPS * 128 + 64) * 4;
     cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     TimeScope ts("infer", d->T, B, d->L, st);
@@ -983,26 +967,16 @@ static int infer_impl(const FtArStepDesc* d, const FtArStepWeights* w, const flo
     cudaError_t e = cudaLaunchCooperativeKernel(fn, dim3(sms), dim3(INF_THREADS), args, smem, st);
     if (e != cudaSuccess) return ft_set_error(cudaGetErrorString(e));
     ft_count_launch(1);
-    return ft_check_launch("infer_kernel");
-}
-
-// ft_ar_step_infer_ragged / ft_ar_step_infer_aligned: the persistent kernel on per-row lengths (attn_forced: batch-major
-// [B,Ta,L] or null), then the per-row finish.
-static int infer_ragged_impl(const FtArStepDesc* d, const FtArStepWeights* w, const float* residual, const float* text,
-                             const int* in_lens, const int* frame_lens, const float* attn_forced, int Ta, float gate_threshold,
-                             float* out, float* attn_out, int* n_frames, void* scratch, void* stream) {
-    const int rev = d->reversed ? 1 : 0;
-    if (infer_impl(d, w, residual, text, nullptr, attn_forced, Ta, in_lens, frame_lens, rev, gate_threshold, out, attn_out, n_frames, scratch, stream) != 0)
-        return -1;
+    if (ft_check_launch("infer_kernel") != 0) return -1;
     // frames are generated back to front by a reversed flow: flip each row within its own n_frames (the B = 1 flip), and clear
     // the attention rows of frames a stopped utterance computed but did not emit
-    const int rows = d->T * d->B;
+    const int rows = d->T * B;
     if (rows <= 0) return 0;
-    infer_ragged_finish_kernel<<<rows < 4096 ? rows : 4096, 128, 0, static_cast<cudaStream_t>(stream)>>>(
-        out, attn_out, n_frames, d->T, d->B, d->n_mel, d->L, rev);
+    infer_finish_kernel<<<rows < 4096 ? rows : 4096, 128, 0, st>>>(out, attn_out, n_frames, d->T, B, M, d->L, p.reversed);
     ft_count_launch(1);
-    return ft_check_launch("infer_ragged_finish_kernel");
+    return ft_check_launch("infer_finish_kernel");
 }
+
 
 }  // namespace ft
 
@@ -1013,33 +987,11 @@ void ft_debug_set_infer_trace(long long* buf) { ft::g_infer_trace = buf; }
 
 size_t ft_ar_step_infer_scratch_bytes(const FtArStepDesc* d) { return ft::plan_infer(*d, nullptr).total + 256; }
 
-int ft_ar_step_infer(const FtArStepDesc* d, const FtArStepWeights* w, const float* residual, const float* text,
-                     const float* attn_prior, const float* attn_forced, float gate_threshold, float* out, float* attn_out,
-                     int* n_frames, void* scratch, void* stream) {
-    using namespace ft;
-    if (!d || !w || !residual || !text || !out || !attn_out || !n_frames || !scratch) return ft_set_error("ft_ar_step_infer: NULL argument");
-    return infer_impl(d, w, residual, text, attn_prior, attn_forced, 0, nullptr, nullptr, 0, gate_threshold, out, attn_out, n_frames,
-                      scratch, stream);
-}
-
-int ft_ar_step_infer_ragged(const FtArStepDesc* d, const FtArStepWeights* w, const float* residual, const float* text,
-                            const int* in_lens, const int* frame_lens, float gate_threshold, float* out, float* attn_out,
-                            int* n_frames, void* scratch, void* stream) {
-    using namespace ft;
-    if (!d || !w || !residual || !text || !out || !attn_out || !n_frames || !scratch) return ft_set_error("ft_ar_step_infer_ragged: NULL argument");
-    if (d->has_prior) return ft_set_error("ft_ar_step_infer_ragged: attn_prior is not supported");
-    return infer_ragged_impl(d, w, residual, text, in_lens, frame_lens, nullptr, 0, gate_threshold, out, attn_out, n_frames, scratch, stream);
-}
-
-int ft_ar_step_infer_aligned(const FtArStepDesc* d, const FtArStepWeights* w, const float* residual, const float* text,
-                             const int* in_lens, const int* frame_lens, const float* attn_forced, int Ta, float gate_threshold,
-                             float* out, float* attn_out, int* n_frames, void* scratch, void* stream) {
-    using namespace ft;
-    if (!d || !w || !residual || !text || !attn_forced || !out || !attn_out || !n_frames || !scratch)
-        return ft_set_error("ft_ar_step_infer_aligned: NULL argument");
-    if (d->has_prior) return ft_set_error("ft_ar_step_infer_aligned: attn_prior is not supported");
-    if (Ta < 1 || (!frame_lens && Ta < d->T)) return ft_set_error("ft_ar_step_infer_aligned: attn_forced must cover every frame budget (Ta >= max frame_lens)");
-    return infer_ragged_impl(d, w, residual, text, in_lens, frame_lens, attn_forced, Ta, gate_threshold, out, attn_out, n_frames, scratch, stream);
+int ft_ar_step_infer(const FtArStepDesc* d, const FtArStepWeights* w, const float* residual, const float* text, const int* in_lens,
+                     const int* frame_lens, const float* attn_prior, const float* attn_forced, int Ta, float gate_threshold,
+                     float* out, float* attn_out, int* n_frames, void* scratch, void* stream) {
+    return ft::infer_impl(d, w, residual, text, in_lens, frame_lens, attn_prior, attn_forced, Ta, gate_threshold, out, attn_out,
+                          n_frames, scratch, stream);
 }
 
 }  // extern "C"

@@ -20,6 +20,7 @@ from torch.nn import functional as F
 
 from . import _lib
 from ._lib import FlowtronB200Error
+from .inference import ar_step_infer, ar_step_infer_trimmed, batch_major
 
 
 def get_mask_from_lengths(lengths: Tensor) -> Tensor:
@@ -414,20 +415,13 @@ class AR_Step(nn.Module):
         return self._run(mel, text, mask, out_lens, attn_prior, False, text_ready)
 
     def infer(self, residual, text, attns, attn_prior=None):
-        from .inference import ar_step_infer
-        return ar_step_infer(self, residual, text, attns, attn_prior, reversed_flag=False)
+        return ar_step_infer_trimmed(self, residual, text, attns, attn_prior, reversed_flag=False)
 
-    def infer_ragged(self, residual, text, in_lens, frame_lens):
-        """Ragged batch: residual [T,B,M], text [L,B,E], in_lens / frame_lens int32 CUDA [B] -> (out, attention [T,B,L],
-        n_frames); see inference.ar_step_infer_ragged."""
-        from .inference import ar_step_infer_ragged
-        return ar_step_infer_ragged(self, residual, text, in_lens, frame_lens, reversed_flag=False)
-
-    def infer_aligned(self, residual, text, in_lens, frame_lens, attns):
-        """infer_ragged with forced alignments: attns [B, Ta, L] as this flow's ``forward`` returns its attention; see
-        inference.ar_step_infer_aligned."""
-        from .inference import ar_step_infer_aligned
-        return ar_step_infer_aligned(self, residual, text, in_lens, frame_lens, attns, reversed_flag=False)
+    def infer_ragged(self, residual, text, in_lens, frame_lens, attns=None, attn_prior=None):
+        """Ragged batch: residual [T,B,M], text [L,B,E], in_lens / frame_lens int32 CUDA [B] or None, forced alignments
+        attns [B, Ta, L] as this flow's ``forward`` returns its attention -> (out, attention [T,B,L], n_frames); see
+        inference.ar_step_infer."""
+        return ar_step_infer(self, residual, text, False, in_lens, frame_lens, attns, attn_prior)
 
 
 class AR_Back_Step(nn.Module):
@@ -445,19 +439,13 @@ class AR_Back_Step(nn.Module):
         return self.ar_step._run(mel, text, mask, out_lens, attn_prior, True, text_ready)
 
     def infer(self, residual, text, attns, attn_prior=None):
-        from .inference import ar_step_infer
-        return ar_step_infer(self.ar_step, residual, text, attns, attn_prior, reversed_flag=True)
+        return ar_step_infer_trimmed(self.ar_step, residual, text, attns, attn_prior, reversed_flag=True)
 
-    def infer_ragged(self, residual, text, in_lens, frame_lens):
-        """As AR_Step.infer_ragged; row b runs back to front over its own first frame_lens[b] frames."""
-        from .inference import ar_step_infer_ragged
-        return ar_step_infer_ragged(self.ar_step, residual, text, in_lens, frame_lens, reversed_flag=True)
-
-    def infer_aligned(self, residual, text, in_lens, frame_lens, attns):
-        """As AR_Step.infer_aligned; row (b, i) of attns is generation step i, i.e. natural frame frame_lens[b] - 1 - i: the
-        flipped order this flow's ``forward`` returns."""
-        from .inference import ar_step_infer_aligned
-        return ar_step_infer_aligned(self.ar_step, residual, text, in_lens, frame_lens, attns, reversed_flag=True)
+    def infer_ragged(self, residual, text, in_lens, frame_lens, attns=None, attn_prior=None):
+        """As AR_Step.infer_ragged; row b runs back to front over its own first frame_lens[b] frames, and row (b, i) of
+        attns is generation step i, i.e. natural frame frame_lens[b] - 1 - i: the flipped order this flow's ``forward``
+        returns."""
+        return ar_step_infer(self.ar_step, residual, text, True, in_lens, frame_lens, attns, attn_prior)
 
 
 # --------------------------------------------------------------------------------------------- model
@@ -561,12 +549,15 @@ class Flowtron(nn.Module):
                 [cat([p[3][i] for p in parts], 0) for i in range(n_flows)],
                 [cat([p[4][i] for p in parts], 0) for i in range(n_flows)])
 
-    def _encode(self, speaker_ids, text, in_lens):
-        """flowtron.py:871-880: embeddings + Encoder + speaker vector concat -> [L, B, n_text + n_speaker]."""
+    def _with_speaker(self, speaker_ids, text):
+        """flowtron.py:871-880: the Encoder's [B, L, n_text] output + the speaker vector -> [L, B, n_text + n_speaker]."""
         speaker_ids = speaker_ids * 0 if self.dummy_speaker_embedding else speaker_ids
         speaker_vecs = self.speaker_embedding(speaker_ids)
-        text = self.encoder.forward_tokens(text, self.embedding, in_lens).transpose(0, 1)
+        text = text.transpose(0, 1)
         return torch.cat([text, speaker_vecs.expand(text.size(0), -1, -1)], 2)
+
+    def _encode(self, speaker_ids, text, in_lens):
+        return self._with_speaker(speaker_ids, self.encoder.forward_tokens(text, self.embedding, in_lens))
 
     def forward(self, mel, speaker_ids, text, in_lens, out_lens, attn_prior=None):
         """Texts of up to _lib.MAX_TEXT_LEN (1024) tokens; longer ones raise ValueError before any work."""
@@ -680,11 +671,8 @@ class Flowtron(nn.Module):
         """Flowtron.encode's work on checked inputs (lengths int32 on the device) -> (z [T, B, 80], zero past out_lens;
         the flows' attention [B, T, L] zeroed outside each row's lengths, or None)."""
         T, dev = mel.size(2), mel.device
-        speaker_ids = speaker_ids * 0 if self.dummy_speaker_embedding else speaker_ids
-        speaker_vecs = self.speaker_embedding(speaker_ids)
-        text = self.encoder.infer_ragged_tokens(text, self.embedding, in_lens).transpose(0, 1)
-        encoder_outputs = torch.cat([text, speaker_vecs.expand(text.size(0), -1, -1)], 2)
-        mask = ~(torch.arange(text.size(0), device=dev)[None, :] < in_lens[:, None])[..., None]
+        encoder_outputs = self._with_speaker(speaker_ids, self.encoder.infer_ragged_tokens(text, self.embedding, in_lens))
+        mask = ~(torch.arange(encoder_outputs.size(0), device=dev)[None, :] < in_lens[:, None])[..., None]
         out = self._run_flows(mel.permute(2, 0, 1), encoder_outputs, mask, out_lens, attn_prior)
         # forward leaves frames at or past out_lens[b] undefined
         past = torch.arange(T, device=dev)[:, None] >= out_lens[None, :]
@@ -695,20 +683,40 @@ class Flowtron(nn.Module):
         return z, [a.masked_fill(outside, 0.0) for a in out[3]]
 
     def infer(self, residual, speaker_ids, text, temperature=1.0, gate_threshold=0.5, attns=None, attn_prior=None):
-        """Texts of up to _lib.MAX_TEXT_LEN (1024) tokens; longer ones raise ValueError before any work."""
+        """residual [B, 80, T] -> (mel [B, 80, T'], attention_weights: per flow in application order, T' rows [B, 1, L]).
+
+        T' is the longest row: with B == 1 it is where the gate fired (the reference's ``break``); with B > 1 every row
+        equals its own B == 1 run and emits zeros after its own gate fired (the reference raises there, SURVEY.md 3.2).
+        ``attns``: one forced alignment per flow, in flow-index order, each covering the T frames (see
+        ``inference.batch_major`` for the accepted forms); ``attn_prior`` [B, >= T, L].  One host synchronisation, at the
+        end.  Texts of up to _lib.MAX_TEXT_LEN (1024) tokens; longer ones raise ValueError before any work."""
         _lib.check_text_len(text.size(-1), "Flowtron.infer")
-        speaker_ids = speaker_ids * 0 if self.dummy_speaker_embedding else speaker_ids
-        speaker_vecs = self.speaker_embedding(speaker_ids)
-        text = self.encoder.infer_tokens(text, self.embedding).transpose(0, 1)
-        encoder_outputs = torch.cat([text, speaker_vecs.expand(text.size(0), -1, -1)], 2)
-        residual = residual.permute(2, 0, 1)
-        attention_weights = []
-        for i, flow in enumerate(reversed(self.flows)):
-            attn = None if attns is None else list(reversed(attns))[i]
+        B, _, T = residual.shape
+        L = text.size(-1)
+        if attns is not None:
+            attns = [batch_major(a, B, L).to(residual.device) for a in attns]
+            if any(a.size(1) < T for a in attns):
+                raise ValueError(f"attns cover {[a.size(1) for a in attns]} frames, residual has {T}")
+        encoder_outputs = self._with_speaker(speaker_ids, self.encoder.infer_tokens(text, self.embedding))
+        for flow in self.flows:
             self.set_temperature_and_gate(flow, temperature, gate_threshold)
-            residual, attention_weight = flow.infer(residual, encoder_outputs, attn, attn_prior=attn_prior)
-            attention_weights.append(attention_weight)
-        return residual.permute(1, 2, 0), attention_weights
+        out, attention, n_frames = self._infer_flows(residual, encoder_outputs, None, None, attns, attn_prior)
+        n = int(n_frames.max().item())
+        if n < T:                               # only a gate stops a row before T here
+            print("Hitting gate limit")
+        return out[:n].permute(1, 2, 0), [[a.unsqueeze(1) for a in attn[:n]] for attn in attention]
+
+    def _infer_flows(self, residual, encoder_outputs, in_lens, n_frames, attns=None, attn_prior=None):
+        """The per-row inverse of every flow, last flow first: residual [B, 80, T] -> (out [T, B, 80] zero past each row's
+        n_frames, the flows' attention [T, B, L] in application order, n_frames int32 [B]).  The first flow applied gets
+        the budgets ``n_frames`` (None: T), every later flow the previous flow's frame counts, on the device."""
+        residual = residual.permute(2, 0, 1)
+        attention = []
+        for f in reversed(range(len(self.flows))):
+            residual, attn, n_frames = self.flows[f].infer_ragged(residual, encoder_outputs, in_lens, n_frames,
+                                                                  None if attns is None else attns[f], attn_prior)
+            attention.append(attn)
+        return residual, attention, n_frames
 
     def infer_batch(self, residual, speaker_ids, text, in_lens, temperature=1.0, gate_threshold=0.5, *, max_frames=None,
                     attns=None, attn_prior=None):
@@ -748,17 +756,11 @@ class Flowtron(nn.Module):
         dev = residual.device
         in_lens = in_lens.to(device=dev, dtype=torch.int32)
         lens = max_frames.to(device=dev, dtype=torch.int32)
-        speaker_ids = speaker_ids * 0 if self.dummy_speaker_embedding else speaker_ids
-        speaker_vecs = self.speaker_embedding(speaker_ids)
-        text = self.encoder.infer_ragged_tokens(text, self.embedding, in_lens).transpose(0, 1)
-        encoder_outputs = torch.cat([text, speaker_vecs.expand(text.size(0), -1, -1)], 2)
-        residual = residual.permute(2, 0, 1)
-        attention_weights = []
-        for flow in reversed(self.flows):
+        encoder_outputs = self._with_speaker(speaker_ids, self.encoder.infer_ragged_tokens(text, self.embedding, in_lens))
+        for flow in self.flows:
             self.set_temperature_and_gate(flow, temperature, gate_threshold)
-            residual, attn, lens = flow.infer_ragged(residual, encoder_outputs, in_lens, lens)
-            attention_weights.append(attn.transpose(0, 1))
-        return residual.permute(1, 2, 0), lens.long(), attention_weights
+        out, attention, lens = self._infer_flows(residual, encoder_outputs, in_lens, lens)
+        return out.permute(1, 2, 0), lens.long(), [a.transpose(0, 1) for a in attention]
 
     def infer_aligned(self, residual, speaker_ids, text, in_lens, attns, n_frames, gate_threshold=1.0):
         """Inference over a padded batch with forced alignments: every flow uses the given attention weights instead of
@@ -802,17 +804,13 @@ class Flowtron(nn.Module):
         in_lens = in_lens.to(device=dev, dtype=torch.int32)
         lens = lens.to(device=dev, dtype=torch.int32)
         with torch.no_grad():
-            speaker_ids = speaker_ids * 0 if self.dummy_speaker_embedding else speaker_ids
-            speaker_vecs = self.speaker_embedding(speaker_ids)
-            text = self.encoder.infer_ragged_tokens(text, self.embedding, in_lens).transpose(0, 1)
-            encoder_outputs = torch.cat([text, speaker_vecs.expand(text.size(0), -1, -1)], 2)
-            residual = residual.permute(2, 0, 1)
-            for f in reversed(range(len(self.flows))):
-                step = getattr(self.flows[f], "ar_step", self.flows[f])
+            encoder_outputs = self._with_speaker(speaker_ids, self.encoder.infer_ragged_tokens(text, self.embedding, in_lens))
+            for flow in self.flows:
+                step = getattr(flow, "ar_step", flow)
                 if hasattr(step, 'gate_layer'):
                     step.gate_threshold = gate_threshold
-                residual, _, lens = self.flows[f].infer_aligned(residual, encoder_outputs, in_lens, lens, attns[f])
-        return residual.permute(1, 2, 0), lens.long()
+            out, _, lens = self._infer_flows(residual, encoder_outputs, in_lens, lens, attns)
+        return out.permute(1, 2, 0), lens.long()
 
     def convert(self, mel, speaker_ids, target_speaker_ids, text, in_lens, out_lens, attn_prior=None):
         """Voice conversion of a padded batch of recorded utterances: each is mapped to z with its own speaker

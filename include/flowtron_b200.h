@@ -186,55 +186,36 @@ int ft_radam_step_dev(float* p, const float* g, float* m, float* v, long long n,
                       double weight_decay, double lr, const int* step_dev, const float* grad_coef, void* stream);
 int ft_step_increment(int* step_dev, void* stream);
 
-/* AR_Step.infer (flowtron.py:775-828): sequential inverse of one flow for all T frames in ONE persistent launch.
- *   residual [T,B,M] f32 in flow-time order (the caller flips for AR_Back_Step, :629-642), text [L,B,E] f32,
- *   attn_prior [B,T,L] or NULL (row i is used at frame i); attn_forced [T,B,L] or NULL: forced alignments (the `attns`
- *   argument, flowtron.py:585-588, 797: scoring, softmax and the prior are skipped, context = attn_forced[i] . V).
- *   Uses d->T/B/L/n_*, has_gate, has_prior, temperature.  B <= 16, L <= FT_MAX_TEXT_LEN (texts over 256 tokens run the
- *   long-text kernel variant, which stages the row of scores in shared memory).
- *   out [T,B,M]: generated frames (zeros after a sample's gate fired; the frame that trips the gate is emitted),
- *   attn_out [T,B,L]: per-frame attention weights, n_frames [B] int32: frames emitted per sample.
- *   With B == 1 this is exactly the reference's loop-with-break; B > 1 with a gate is the per-sample-stop
- *   extension (the reference raises there, SURVEY.md 3.2). */
-size_t ft_ar_step_infer_scratch_bytes(const FtArStepDesc* d);
-int ft_ar_step_infer(const FtArStepDesc* d, const FtArStepWeights* w, const float* residual, const float* text,
-                     const float* attn_prior, const float* attn_forced, float gate_threshold, float* out, float* attn_out,
-                     int* n_frames, void* scratch, void* stream);
-
-/* The same inverse for a ragged batch: row b equals its own B == 1 ft_ar_step_infer run on its unpadded inputs.
- *   residual [T,B,M] f32 in NATURAL time order (no caller flip), text [L,B,E] f32; scratch: ft_ar_step_infer_scratch_bytes(d).
+/* AR_Step.infer / AR_Back_Step.infer (flowtron.py:775-828, 629-642): sequential inverse of one flow for a padded batch,
+ * all T frames in ONE persistent launch.  Row b equals its own B == 1 run on its unpadded inputs.
+ *   residual [T,B,M] f32 in NATURAL time order, text [L,B,E] f32; scratch: ft_ar_step_infer_scratch_bytes(d).
  *   in_lens [B] int32 device or NULL (all L): text length of row b; keys l >= in_lens[b] take no part in the softmax and get
  *     attention weight 0.
  *   frame_lens [B] int32 device or NULL (all T): frame budget of row b; row b generates while i < frame_lens[b] and its gate
  *     has not fired; residual rows t >= frame_lens[b] are never read.
  *   d->reversed = 1 (AR_Back_Step): frame i reads residual[frame_lens[b] - 1 - i], and the emitted frames come back flipped
- *     within the row's own n_frames[b] (the B == 1 flip), so `out` is in natural time order too.
- *   out [T,B,M]: zero at t >= n_frames[b]; attn_out [T,B,L] in generation order, zero at i >= n_frames[b] and l >= in_lens[b];
- *   n_frames [B] int32 = min(gate stop (the frame that trips the gate is emitted), frame_lens[b]).
+ *     within the row's own n_frames[b], so `out` is in natural time order too.
+ *   attn_prior [B,T,L] f32 or NULL (used when d->has_prior): row i is used at generation step i; for a back step the
+ *     caller flips it (the reference's torch.flip(attn_prior, (1,))).
+ *   attn_forced [B,Ta,L] f32 or NULL: forced alignments (the `attns` argument, flowtron.py:585-588, 797).  Row (b, i) holds
+ *     the weights of GENERATION STEP i of utterance b: with d->reversed = 1, step i produces natural frame
+ *     frame_lens[b] - 1 - i, the order in which AR_Back_Step.forward returns its attention, so a flow's forward attention
+ *     feeds the same flow's inverse with no transpose or flip.  Scoring, softmax and the prior are skipped; context =
+ *     weights . V.  Ta >= max frame_lens[b] (>= d->T when frame_lens is NULL); only keys l < in_lens[b] of rows
+ *     i < frame_lens[b] are read, every other weight is 0 whatever the buffer holds.
+ *   out [T,B,M]: zero at t >= n_frames[b]; attn_out [T,B,L]: the weights used, in generation order, zero at i >= n_frames[b]
+ *     and l >= in_lens[b]; n_frames [B] int32 = min(gate stop (the frame that trips the gate is emitted), frame_lens[b]);
+ *     a gate_threshold >= 1 disables stopping.
  *   Lengths must satisfy 1 <= in_lens[b] <= L and 1 <= frame_lens[b] <= T; they are read on the device only.
- *   Limits as ft_ar_step_infer: B <= 16, L <= FT_MAX_TEXT_LEN; d->has_prior must be 0 (no attn_prior; forced alignments
- *   go through ft_ar_step_infer_aligned).  Flowtron.infer_batch, the host layer over this entry point, takes texts of up to 256 tokens.
- *   Two launches (the persistent kernel, then a small per-row flip / attention clear), no host synchronisation:
- *   CUDA-graph capturable. */
-int ft_ar_step_infer_ragged(const FtArStepDesc* d, const FtArStepWeights* w, const float* residual, const float* text,
-                            const int* in_lens, const int* frame_lens, float gate_threshold, float* out, float* attn_out,
-                            int* n_frames, void* scratch, void* stream);
-
-/* The ragged inverse with per-row FORCED ALIGNMENTS (voice conversion, rhythm transfer): everything as
- * ft_ar_step_infer_ragged, except that the attention weights are given instead of computed (no query projection, scores,
- * softmax or prior; context = weights . V), as ft_ar_step_infer does with attn_forced.
- *   attn_forced [B,Ta,L] f32, batch-major, the layout ft_ar_step_fwd writes its attention in: row (b, i) holds the weights
- *     of GENERATION STEP i of utterance b.  Generation steps are counted in the flow's own order: with d->reversed = 1, step
- *     i produces natural frame frame_lens[b] - 1 - i, the order in which AR_Back_Step.forward returns its attention, so a
- *     flow's forward attention feeds the same flow's inverse with no transpose or flip.
- *   Ta >= max frame_lens[b] (>= d->T when frame_lens is NULL); only keys l < in_lens[b] of rows i < frame_lens[b] are
- *     read, every other weight is 0 whatever the buffer holds.
- *   attn_out [T,B,L]: the weights used, in generation order, zero at i >= n_frames[b] and l >= in_lens[b].
- *   n_frames[b] = min(gate stop, frame_lens[b]): a gate_threshold >= 1 disables stopping.
- *   Limits, scratch, launches and graph capture as ft_ar_step_infer_ragged; every L <= FT_MAX_TEXT_LEN. */
-int ft_ar_step_infer_aligned(const FtArStepDesc* d, const FtArStepWeights* w, const float* residual, const float* text,
-                             const int* in_lens, const int* frame_lens, const float* attn_forced, int Ta, float gate_threshold,
-                             float* out, float* attn_out, int* n_frames, void* scratch, void* stream);
+ *   B <= 16, L <= FT_MAX_TEXT_LEN (texts over 256 tokens run the long-text kernel variant, which stages the row of scores in
+ *   shared memory).  With B == 1 this is exactly the reference's loop-with-break; B > 1 with a gate is the per-row-stop
+ *   extension (the reference raises there, SURVEY.md 3.2).
+ *   Two launches (the persistent kernel, then a small per-row flip / attention clear), no allocation, no host
+ *   synchronisation: CUDA-graph capturable. */
+size_t ft_ar_step_infer_scratch_bytes(const FtArStepDesc* d);
+int ft_ar_step_infer(const FtArStepDesc* d, const FtArStepWeights* w, const float* residual, const float* text, const int* in_lens,
+                     const int* frame_lens, const float* attn_prior, const float* attn_forced, int Ta, float gate_threshold,
+                     float* out, float* attn_out, int* n_frames, void* scratch, void* stream);
 
 /* TacotronSTFT.mel_spectrogram (audio_processing.py:117-134) for a ragged batch.  wav: concatenated utterances
  * (f32 in [-1,1]); sample_offsets / frame_offsets: device int64 [n_utt+1] prefix sums (frames of utterance u =

@@ -1,5 +1,5 @@
 """GPU: voice conversion and rhythm transfer -- Flowtron.encode(return_attns=True), Flowtron.infer_aligned (over
-ft_ar_step_infer_aligned) and Flowtron.convert against the reference-generated fixtures (tests/make_golden_convert.py), a
+ft_ar_step_infer with forced alignments) and Flowtron.convert against the reference-generated fixtures (tests/make_golden_convert.py), a
 two-launch batch against per-row B = 1 Flowtron.infer(attns=) runs, the identity conversion, padding invariance, CUDA-graph
 replay and the chain into WaveGlow and the Denoiser."""
 import os
@@ -178,7 +178,7 @@ def test_identity_conversion_returns_the_mel():
         assert (other[b, :, :n] - mel[b, :, :n]).abs().max().item() > 0.05 and (other[b, :, n:] == 0).all()
 
 
-def test_flow_attention_out_is_the_forced_alignment():
+def test_flow_infer_ragged_attention_out_is_the_forced_alignment():
     """Per flow: the returned attention is the given map, in generation order, masked to each row's lengths."""
     m = _model(2, 81)
     B, T, L = 4, 30, 16
@@ -191,8 +191,8 @@ def test_flow_attention_out_is_the_forced_alignment():
     text2 = text.clone()
     text2[:, :, 512:] += 0.1                                     # the speaker part of the encoding
     for flow, a in zip(m.flows, attns):
-        out, attn, n = flow.infer_aligned(res, text, il, fl, a)
-        out2, attn2, _ = flow.infer_aligned(res, text2, il, fl, a)
+        out, attn, n = flow.infer_ragged(res, text, il, fl, attns=a)
+        out2, attn2, _ = flow.infer_ragged(res, text2, il, fl, attns=a)
         assert n.tolist() == n_frames
         want = a.transpose(0, 1).clone()
         for b in range(B):

@@ -11,12 +11,14 @@ from flowtron_b200 import synth
 pytestmark = pytest.mark.gpu
 
 
-def _model(cfg, seed, gate_bias=None):
+def _model(cfg, seed, gate_bias=None, gate_scale=1.0):
     from flowtron_b200.flowtron import Flowtron
     p = synth.synth_params(cfg, seed)
     if gate_bias is not None:
         key = [k for k in p if k.endswith("gate_layer.linear_layer.bias")][0]
         p[key] = torch.full_like(p[key], gate_bias)
+        key = [k for k in p if k.endswith("gate_layer.linear_layer.weight")][0]
+        p[key] = p[key] * gate_scale
     m = Flowtron(**cfg)
     m.load_state_dict(p, strict=True)
     return m.cuda().eval()
@@ -81,6 +83,36 @@ def test_batched_rows_equal_single_runs():
             got = mel_b[b, :, :n] if mel_b.shape[-1] >= n else None
             assert got is not None
             assert (got - ref).abs().max().item() <= 2e-3 * ref.abs().max().item()
+
+
+@pytest.mark.parametrize("n_flows, seed, gate_bias, fixture_rows", [
+    (2, 61, -0.3, None),                # the steep gates of test_gpu_infer_batch.py
+    (3, 62, -6.0, [0, 3, 5]),           # (3 flows: on rows of infer_ragged_f3.npz that stop at different frames)
+])
+def test_rows_stopping_at_different_frames_equal_single_runs(n_flows, seed, gate_bias, fixture_rows):
+    """B=3, a gate that stops the rows at different frames: each row equals its own B=1 run bit for bit and is zero after
+    it (a back step flips each row within its own length; later flows see each row's length)."""
+    if fixture_rows is None:
+        cfg = dict(synth.DEFAULT_MODEL_CONFIG, n_flows=n_flows)
+        g = torch.Generator().manual_seed(4)
+        B, T, L = 3, 24, 10
+        res = (torch.randn(B, 80, T, generator=g) * 0.5).cuda()
+        text = torch.randint(0, 185, (B, L), generator=g).cuda()
+        spk = torch.zeros(B, dtype=torch.long, device="cuda")
+    else:
+        gold = np.load(os.path.join(GOLDEN, "infer_ragged_f3.npz"))
+        cfg = dict(synth.DEFAULT_MODEL_CONFIG, n_flows=n_flows, n_speakers=int(gold["n_speakers"]))
+        res, text, spk = [torch.from_numpy(gold[k][fixture_rows]).cuda() for k in ("residual", "text", "speaker_ids")]
+        B = len(fixture_rows)
+    m = _model(cfg, seed, gate_bias, gate_scale=40.0)
+    with torch.no_grad():
+        mel_b, _ = m.infer(res, spk, text)
+        singles = [m.infer(res[b:b + 1], spk[b:b + 1], text[b:b + 1])[0][0] for b in range(B)]
+    lens = [s.shape[-1] for s in singles]
+    assert mel_b.shape[-1] == max(lens) and len(set(lens)) > 1, (mel_b.shape, lens)
+    for b, ref in enumerate(singles):
+        n = lens[b]
+        assert torch.equal(mel_b[b, :, :n], ref) and (mel_b[b, :, n:] == 0).all(), (b, lens)
 
 
 def test_forced_alignments_attns_argument():

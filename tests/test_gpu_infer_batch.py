@@ -1,4 +1,4 @@
-"""GPU: Flowtron.infer_batch (ragged-batch inference over ft_ar_step_infer_ragged) against the reference-generated
+"""GPU: Flowtron.infer_batch (ragged-batch inference over ft_ar_step_infer) against the reference-generated
 fixtures (tests/make_golden_infer_batch.py), B = 1 and equal-length bit-identity with Flowtron.infer, a two-launch batch
 against per-row B = 1 runs, padding invariance, CUDA-graph replay, and the chain into WaveGlow and the Denoiser."""
 import os

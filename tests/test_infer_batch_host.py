@@ -1,5 +1,5 @@
 """CPU: Flowtron.infer_batch argument checks, the oracle's restatement of its contract against the reference-generated
-fixtures (tests/make_golden_infer_batch.py), and the register budget of the inference kernel."""
+fixtures (tests/make_golden_infer_batch.py), and the register budget of the inference kernels."""
 import os
 import re
 import shutil
@@ -92,14 +92,20 @@ def test_fixtures_cover_gate_stops_and_budgets():
 
 
 @pytest.mark.skipif(not HAVE_NVCC, reason="nvcc not available")
-def test_infer_kernel_does_not_spill(tmp_path):
+def test_infer_kernels_fit_the_register_budget(tmp_path):
+    """infer_kernel<batch > 8, long text, forced>: eight instantiations of the persistent kernel, 512 threads each, so 128
+    registers at most, and no spills; the finish kernel likewise."""
     r = subprocess.run([NVCC, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "--expt-relaxed-constexpr",
                         "-Xptxas", "-v", "-c", os.path.join(ROOT, "flowtron_b200", "csrc", "infer.cu"), "-o",
                         str(tmp_path / "infer.o")], capture_output=True, text=True)
     assert r.returncode == 0, r.stderr
-    parts = r.stderr.split("Compiling entry function")
-    logs = [s for s in parts if "infer_kernel" in s.splitlines()[0]]
-    assert len(logs) == 2, r.stderr                             # the B <= 8 and B <= 16 instantiations
-    for log in logs:
-        m = re.search(r"(\d+) bytes spill stores, (\d+) bytes spill loads", log)
-        assert m and m.groups() == ("0", "0"), log
+    logs = {}
+    for part in r.stderr.split("Compiling entry function")[1:]:
+        logs[re.match(r"\s*'(\S+)'", part).group(1)] = part
+    want = [f"_ZN2ft12infer_kernelILb{a}ELb{b}ELb{c}EEEvNS_11InferParamsE" for a in "01" for b in "01" for c in "01"]
+    want.append("_ZN2ft19infer_finish_kernelEPfS0_PKiiiiii")
+    assert all(k in logs for k in want), sorted(logs)
+    for k in want:
+        regs = int(re.search(r"Used (\d+) registers", logs[k]).group(1))
+        spill = re.search(r"(\d+) bytes spill stores, (\d+) bytes spill loads", logs[k])
+        assert regs <= 128 and spill.groups() == ("0", "0"), logs[k]

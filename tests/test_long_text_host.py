@@ -100,13 +100,10 @@ def _ptxas(src, tmp_path):
 
 
 @pytest.mark.skipif(not HAVE_NVCC, reason="nvcc not available")
-def test_short_text_kernels_keep_their_register_budget(tmp_path):
+def test_short_text_training_kernels_keep_their_register_budget(tmp_path):
     """The L <= 256 kernels are the parent's: same registers, no spills (the long-text variants are separate
-    instantiations: infer_long_kernel, attn_*_kernel<true>, attn_ctc_long_kernel)."""
-    infer = _ptxas("infer.cu", tmp_path)
-    short = {k: v for k, v in infer.items() if "12infer_kernel" in k}
-    assert len(short) == 2 and all(v == (128, ("0", "0")) for v in short.values()), short
-    assert len([k for k in infer if "infer_long_kernel" in k]) == 2
+    instantiations: attn_*_kernel<true>, attn_ctc_long_kernel; the inference kernels' budget is checked in
+    test_infer_batch_host.py)."""
     attn = _ptxas("attention.cu", tmp_path)
     assert attn["_ZN2ft15attn_fwd_kernelILb0EEEvNS_13AttnFwdParamsE"] == (96, ("0", "0"))
     assert attn["_ZN2ft15attn_bwd_kernelILb0EEEvNS_13AttnBwdParamsE"] == (126, ("0", "0"))
