@@ -53,6 +53,27 @@ class FtEncoderGrads(Structure):
     _fields_ = [("d_" + n, c_void_p * k) for n, k in ENC_PARAM_FIELDS]
 
 
+class FtMelEncoderDesc(Structure):
+    _fields_ = [("B", c_int), ("T", c_int), ("eps", c_float), ("dropout_p", c_float)]
+
+
+MEL_ENC_PARAM_FIELDS = [("conv_w", 2), ("conv_b", 2), ("norm_w", 2), ("norm_b", 2), ("w_ih", 2), ("w_hh", 2), ("b_ih", 2), ("b_hh", 2)]
+MEL_ENC_MAX_BATCH = 64          # FT_MEL_ENC_MAX_BATCH
+GMM_MAX_COMPONENTS = 32         # FT_GMM_MAX_COMPONENTS
+
+
+class FtMelEncoderWeights(Structure):
+    _fields_ = [(n, c_void_p * k) for n, k in MEL_ENC_PARAM_FIELDS]
+
+
+class FtMelEncoderGrads(Structure):
+    _fields_ = [("d_" + n, c_void_p * k) for n, k in MEL_ENC_PARAM_FIELDS]
+
+
+class FtGmmDesc(Structure):
+    _fields_ = [("T", c_int), ("B", c_int), ("M", c_int), ("K", c_int), ("per_row", c_int)]
+
+
 class FtWaveGlowDesc(Structure):
     _fields_ = [("n_mel", c_int), ("n_flows", c_int), ("n_group", c_int), ("n_early_every", c_int), ("n_early_size", c_int),
                 ("n_layers", c_int), ("n_channels", c_int), ("kernel_size", c_int), ("B", c_int), ("F_max", c_int),
@@ -199,6 +220,21 @@ def _declare(L):
     L.ft_waveglow_infer.restype = c_int
     L.ft_posterior_mean.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_float, c_void_p, c_void_p]
     L.ft_posterior_mean.restype = c_int
+    for fn in ("ft_mel_encoder_saved_bytes", "ft_mel_encoder_fwd_scratch_bytes", "ft_mel_encoder_bwd_scratch_bytes"):
+        getattr(L, fn).argtypes = [POINTER(FtMelEncoderDesc)]
+        getattr(L, fn).restype = c_size_t
+    L.ft_mel_encoder_fwd.argtypes = [POINTER(FtMelEncoderDesc), POINTER(FtMelEncoderWeights), c_void_p, c_void_p, c_void_p, c_int,
+                                     c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
+    L.ft_mel_encoder_fwd.restype = c_int
+    L.ft_mel_encoder_bwd.argtypes = [POINTER(FtMelEncoderDesc), POINTER(FtMelEncoderWeights), c_void_p, c_void_p,
+                                     POINTER(FtMelEncoderGrads), c_void_p, c_void_p]
+    L.ft_mel_encoder_bwd.restype = c_int
+    L.ft_gmm_nll_scratch_bytes.argtypes = [POINTER(FtGmmDesc)]
+    L.ft_gmm_nll_scratch_bytes.restype = c_size_t
+    L.ft_gmm_nll_reduce.argtypes = [POINTER(FtGmmDesc)] + [c_void_p] * 8
+    L.ft_gmm_nll_reduce.restype = c_int
+    L.ft_gmm_nll_grad.argtypes = [POINTER(FtGmmDesc)] + [c_void_p] * 11
+    L.ft_gmm_nll_grad.restype = c_int
 
 
 def check(rc: int, what: str = ""):
@@ -577,6 +613,62 @@ def encoder_bwd(desc, params, d_out, saved, need_dx=True, tokens=None, emb_weigh
     check(L.ft_encoder_bwd_tokens(byref(desc), byref(w), ptr(d_out), d_out.stride(0), d_out.stride(1), ptr(saved), ptr(tokens),
                                   emb_weight.size(0), ptr(d_emb), byref(g), ptr(scratch), stream_ptr()), "ft_encoder_bwd_tokens")
     return d_emb, grads
+
+
+# ------------------------------------------------------------------------------------------------ mel encoder (GMM prior)
+def _mel_enc_struct(cls, prefix, tensors):
+    st = cls()
+    for n, k in MEL_ENC_PARAM_FIELDS:
+        setattr(st, prefix + n, (c_void_p * k)(*[c_void_p(t.data_ptr()) for t in tensors[n]]))
+    return st
+
+
+def mel_encoder_fwd(params, mel, out_lens_i32, all_lens_i32, rng_state, dropout_p, eps, emb):
+    """ft_mel_encoder_fwd on mel [B, 80, T] (B <= 64) -> emb [B, 512] (written).  all_lens_i32: the whole batch's lengths (their
+    maximum divides the time sum).  Returns (desc, saved) for mel_encoder_bwd."""
+    _need_cuda(mel, out_lens_i32, all_lens_i32, emb)
+    L = lib()
+    desc = FtMelEncoderDesc(B=mel.size(0), T=mel.size(2), eps=float(eps), dropout_p=float(dropout_p))
+    saved = torch.empty(L.ft_mel_encoder_saved_bytes(byref(desc)), dtype=torch.uint8, device=mel.device)
+    scratch = torch.empty(L.ft_mel_encoder_fwd_scratch_bytes(byref(desc)), dtype=torch.uint8, device=mel.device)
+    w = _mel_enc_struct(FtMelEncoderWeights, "", params)
+    check(L.ft_mel_encoder_fwd(byref(desc), byref(w), ptr(mel), ptr(out_lens_i32), ptr(all_lens_i32), all_lens_i32.numel(),
+                               ptr(rng_state), ptr(emb), ptr(saved), ptr(scratch), stream_ptr()), "ft_mel_encoder_fwd")
+    return desc, saved
+
+
+def mel_encoder_bwd(desc, params, d_emb, saved):
+    """ft_mel_encoder_bwd: dict of weight gradients like `params`."""
+    _need_cuda(d_emb, saved)
+    L = lib()
+    grads = {n: [torch.empty_like(t) for t in params[n]] for n, _ in MEL_ENC_PARAM_FIELDS}
+    scratch = torch.empty(L.ft_mel_encoder_bwd_scratch_bytes(byref(desc)), dtype=torch.uint8, device=d_emb.device)
+    w = _mel_enc_struct(FtMelEncoderWeights, "", params)
+    g = _mel_enc_struct(FtMelEncoderGrads, "d_", grads)
+    check(L.ft_mel_encoder_bwd(byref(desc), byref(w), ptr(d_emb), ptr(saved), byref(g), ptr(scratch), stream_ptr()),
+          "ft_mel_encoder_bwd")
+    return grads
+
+
+# ------------------------------------------------------------------------------------------------ mixture NLL
+def gmm_nll_reduce(z, out_lens_i32, mean, log_var, prob, per_row, sums):
+    """ft_gmm_nll_reduce: sums[0] = NLL, sums[1] = valid frames.  z [T, B, M], mean / log_var [B or 1, M, K], prob [B, K]."""
+    _need_cuda(z, out_lens_i32, mean, log_var, prob, sums)
+    T, B, M = z.shape
+    desc = FtGmmDesc(T=T, B=B, M=M, K=prob.size(1), per_row=int(per_row))
+    scratch = torch.empty(lib().ft_gmm_nll_scratch_bytes(byref(desc)), dtype=torch.uint8, device=z.device)
+    check(lib().ft_gmm_nll_reduce(byref(desc), ptr(z), ptr(out_lens_i32), ptr(mean), ptr(log_var), ptr(prob), ptr(sums),
+                                  ptr(scratch), stream_ptr()), "ft_gmm_nll_reduce")
+
+
+def gmm_nll_grad(z, out_lens_i32, mean, log_var, prob, per_row, g_nll, dz, dmean, dlog_var, dprob):
+    """ft_gmm_nll_grad: gradients of g_nll[0] * NLL (dmean / dlog_var None for shared Gaussians)."""
+    _need_cuda(z, out_lens_i32, mean, log_var, prob, g_nll, dz, dprob)
+    T, B, M = z.shape
+    desc = FtGmmDesc(T=T, B=B, M=M, K=prob.size(1), per_row=int(per_row))
+    scratch = torch.empty(lib().ft_gmm_nll_scratch_bytes(byref(desc)), dtype=torch.uint8, device=z.device)
+    check(lib().ft_gmm_nll_grad(byref(desc), ptr(z), ptr(out_lens_i32), ptr(mean), ptr(log_var), ptr(prob), ptr(g_nll), ptr(dz),
+                                ptr(dmean), ptr(dlog_var), ptr(dprob), ptr(scratch), stream_ptr()), "ft_gmm_nll_grad")
 
 
 # ------------------------------------------------------------------------------------------------ WaveGlow

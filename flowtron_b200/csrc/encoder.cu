@@ -23,39 +23,11 @@
 // buffers.  The recurrences issue three mma.sync per tile with W_hh's hi and lo fragments both resident in registers.  The
 // encoder is < 1 % of the step's FLOPs, so 3x of it is free; the backward pass additionally runs on S * grad with a power-of-two
 // S picked on the device from max|d_out| and multiplies everything leaving the encoder by 1/S.
-#include "ptx.cuh"
-#include "ft_internal.h"
+#include "encoder_kernels.cuh"
 #include "../../include/flowtron_b200.h"
 
 namespace ft {
 
-constexpr int EC = 512, EH = 256, EG = 4 * EH;      // embedding / conv channels, hidden per direction, gate rows
-constexpr int EK = 5, EPADR = 2;                    // conv taps, pad rows on either side of an utterance
-constexpr int ENC_THREADS = 256, ENC_CLUSTER = 8, ENC_UNITS = EH / ENC_CLUSTER;   // 32 units per CTA
-
-__device__ __forceinline__ void mma16816(float (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]) : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ uint32_t pack_h2(float a, float b) { const __half2 h = __floats2half2_rn(a, b); return *reinterpret_cast<const uint32_t*>(&h); }
-__device__ __forceinline__ uint4 ldcg_v4(const void* p) {
-    uint4 v;
-    asm volatile("ld.global.cg.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ float sat16(float x) { return fminf(fmaxf(x, -65504.f), 65504.f); }
-// x -> (hi, lo) fp16 pair with hi + lo = x to ~22 bits (saturating)
-__device__ __forceinline__ void split16(float x, __half& hi, __half& lo) {
-    x = sat16(x);
-    hi = __float2half_rn(x);
-    lo = __float2half_rn(x - __half2float(hi));
-}
-// row of an activation / gradient grid: [hi (W) | lo (W) | hi (W)]
-__device__ __forceinline__ void store_hlh(__half* row, int W, int c, float x) {
-    __half hi, lo;
-    split16(x, hi, lo);
-    row[c] = hi; row[W + c] = lo; row[2 * W + c] = hi;
-}
 
 // ------------------------------------------------------------------------------------------------ layout kernels
 // x [B, C, L] fp32 (embedding output, channels first) -> grid rows (split fp16 [hi|lo|hi], channels last); tokens at l >= len are zeroed
@@ -259,16 +231,6 @@ enc_norm_bwd_kernel(const float* __restrict__ DX, const __half* __restrict__ xou
 __global__ void enc_rng_advance_kernel(unsigned long long* rng) { rng[1] += 1; }
 
 // ------------------------------------------------------------------------------------------------ BiLSTM forward
-struct EncLstmFwdParams {
-    int B, L;
-    const int* lens;               // [B] or null (all L)
-    const float* xproj;            // [rows, 2 * 1024] fp32: W_ih x + b_ih + b_hh, direction-major columns
-    const float* whh[2];           // [1024, 256] fp32 per direction (PyTorch layout, gate order i,f,g,o)
-    __half* hseq[2];               // [rows, 2 * 256] split fp16 [hi | lo] per direction: h_t, zero at pads / l >= len
-    __half* gates[2];              // [rows, 1024] fp16 post-activation i,f,g,o (or null)
-    float* cstate[2];              // [rows, 256] fp32 (or null)
-    float* out; long long out_sb, out_sl;   // fp32 output [.., 512]: element (b, l, dir * 256 + u) at out + b * out_sb + l * out_sl + ..
-};
 
 // grid = 16 CTAs per 32 utterances = clusters of 8; cluster id = (batch half, direction), rank r owns hidden units [32 r, 32 r + 32).
 // Warp w: units u0 = 32 r + 4 w .. +3; its two n8 tiles hold gate rows (i,f) and (g,o) of the 4 units interleaved
@@ -398,15 +360,6 @@ enc_bilstm_fwd_kernel(EncLstmFwdParams p) {
 }
 
 // ------------------------------------------------------------------------------------------------ BiLSTM backward
-struct EncLstmBwdParams {
-    int B, L;
-    const int* lens;
-    const float* d_out; long long d_sb, d_sl;    // gradient w.r.t. the encoder output (fp32, unscaled), same indexing as the forward output
-    const float* scale2;                        // device {S, 1/S}
-    const float* whh[2];
-    const __half* gates[2]; const float* cstate[2];
-    __half* dG[2];                               // [rows, 3 * 1024] split fp16 [hi|lo|hi], zero-initialised: S * d(gate pre-activations)
-};
 
 // Mirror of the forward kernel: cluster = (batch half, direction), rank r owns units [32 r, 32 r + 32); per step
 //   dh_rec[b, u] = sum over the 1024 gate rows k of dG_next[b, k] W_hh[k, u]
@@ -607,11 +560,11 @@ template <int MT> static int launch_bilstm_bwd(const EncLstmBwdParams& p, cudaSt
     ft_count_launch(1);
     return ft_check_launch("enc_bilstm_bwd_kernel");
 }
+int enc_bilstm_fwd(const EncLstmFwdParams& p, cudaStream_t st) { return p.B <= 16 ? launch_bilstm_fwd<1>(p, st) : launch_bilstm_fwd<2>(p, st); }
+int enc_bilstm_bwd(const EncLstmBwdParams& p, cudaStream_t st) { return p.B <= 16 ? launch_bilstm_bwd<1>(p, st) : launch_bilstm_bwd<2>(p, st); }
 
-// wgrad over split grids: C32[M, N] = alpha * (A_hi^T B_hi + A_lo^T B_hi + A_hi^T B_lo); A [K rows, 3 wa] (M = wa), B [K rows, ldb] with
-// its hi / lo column blocks `wb` apart
-static int wgrad3(cudaStream_t st, int M, int N, long long K, const __half* A, int wa, const __half* B, long long ldb, int wb,
-                  const float* alpha_ptr, float* C32) {
+int enc_wgrad3(cudaStream_t st, int M, int N, long long K, const __half* A, int wa, const __half* B, long long ldb, int wb,
+               const float* alpha_ptr, float* C32) {
     for (int term = 0; term < 3; ++term) {
         GemmArgs g;
         g.M = M; g.N = N; g.K = static_cast<int>(K);
@@ -693,8 +646,7 @@ static int encoder_fwd_impl(const FtEncoderDesc* d, const FtEncoderWeights* w, c
     p.B = B; p.L = L; p.lens = lens; p.xproj = P.xproj;
     for (int k = 0; k < 2; ++k) { p.whh[k] = w->w_hh[k]; p.hseq[k] = P.hseq[k]; p.gates[k] = P.gates[k]; p.cstate[k] = P.cstate[k]; }
     p.out = out; p.out_sb = out_stride_b; p.out_sl = out_stride_l;
-    if (B <= 16) return launch_bilstm_fwd<1>(p, st);
-    return launch_bilstm_fwd<2>(p, st);
+    return enc_bilstm_fwd(p, st);
 }
 
 int ft_encoder_fwd(const FtEncoderDesc* d, const FtEncoderWeights* w, const float* x, const int* in_lens, unsigned long long* rng_state,
@@ -726,17 +678,16 @@ static int encoder_bwd_impl(const FtEncoderDesc* d, const FtEncoderWeights* w, c
     EncLstmBwdParams p;
     p.B = B; p.L = L; p.lens = lens; p.d_out = d_out; p.d_sb = d_stride_b; p.d_sl = d_stride_l; p.scale2 = P.scale2;
     for (int k = 0; k < 2; ++k) { p.whh[k] = w->w_hh[k]; p.gates[k] = P.gates[k]; p.cstate[k] = P.cstate[k]; p.dG[k] = P.dG[k]; }
-    if (B <= 16) FT_TRYE(launch_bilstm_bwd<1>(p, st));
-    else FT_TRYE(launch_bilstm_bwd<2>(p, st));
+    FT_TRYE(enc_bilstm_bwd(p, st));
     const float* iS = P.scale2 + 1;
     // BiLSTM parameter gradients and the gradient w.r.t. its input (fp32 grid, still x S)
     for (int k = 0; k < 2; ++k) {
         __half* wih = P.wih16_b + static_cast<size_t>(k) * 3 * EG * EC;
         enc_pack_wih_kernel<<<296, 256, 0, st>>>(w->w_ih[k], nullptr, wih);
         ft_count_launch(1);
-        FT_TRYE(wgrad3(st, EG, EC, rows, P.dG[k], EG, P.X16[3], 3 * EC, EC, iS, gr->d_w_ih[k]));             // dW_ih = dG^T x3
+        FT_TRYE(enc_wgrad3(st, EG, EC, rows, P.dG[k], EG, P.X16[3], 3 * EC, EC, iS, gr->d_w_ih[k]));             // dW_ih = dG^T x3
         // dW_hh = dG_t^T h_{t -+ 1}: the same grids one row apart
-        FT_TRYE(wgrad3(st, EG, EH, rows - 1, P.dG[k] + (k == 0 ? 3 * EG : 0), EG, P.hseq[k] + (k == 0 ? 0 : 2 * EH), 2 * EH, EH, iS, gr->d_w_hh[k]));
+        FT_TRYE(enc_wgrad3(st, EG, EH, rows - 1, P.dG[k] + (k == 0 ? 3 * EG : 0), EG, P.hseq[k] + (k == 0 ? 0 : 2 * EH), 2 * EH, EH, iS, gr->d_w_hh[k]));
         enc_colsum_hilo_kernel<<<EG / 32, 256, 0, st>>>(P.dG[k], rows, EG, iS, gr->d_b_ih[k]);
         ft_count_launch(1);
         FT_CU(cudaMemcpyAsync(gr->d_b_hh[k], gr->d_b_ih[k], sizeof(float) * EG, cudaMemcpyDeviceToDevice, st));
@@ -760,7 +711,7 @@ static int encoder_bwd_impl(const FtEncoderDesc* d, const FtEncoderWeights* w, c
         enc_pack_conv_kernel<<<592, 256, 0, st>>>(w->conv_w[i], nullptr, P.wconv16_b);
         ft_count_launch(1);
         for (int k = 0; k < EK; ++k)                                  // dW_k = dY^T x_i shifted by tap k
-            FT_TRYE(wgrad3(st, EC, EC, rows - 2 * EPADR, P.dY16 + static_cast<size_t>(EPADR) * 3 * EC, EC,
+            FT_TRYE(enc_wgrad3(st, EC, EC, rows - 2 * EPADR, P.dY16 + static_cast<size_t>(EPADR) * 3 * EC, EC,
                            P.X16[i] + static_cast<size_t>(k) * 3 * EC, 3 * EC, EC, iS, P.dwk + static_cast<size_t>(k) * EC * EC));
         enc_unpack_conv_grad_kernel<<<592, 256, 0, st>>>(P.dwk, gr->d_conv_w[i]);
         ft_count_launch(1);

@@ -12,8 +12,10 @@ the [text ; speaker] concatenation stay ordinary PyTorch.
 """
 from __future__ import annotations
 
+import math
 from typing import Optional
 
+import numpy as np
 import torch
 from torch import nn, Tensor
 from torch.nn import functional as F
@@ -96,6 +98,13 @@ _enc_streams = {}
 
 def _encoder_overlap_stream(device):
     key = ("overlap", device.type, device.index)
+    if key not in _enc_streams:
+        _enc_streams[key] = torch.cuda.Stream(device=device)
+    return _enc_streams[key]
+
+
+def _mel_encoder_stream(device):
+    key = ("mel", device.type, device.index)
     if key not in _enc_streams:
         _enc_streams[key] = torch.cuda.Stream(device=device)
     return _enc_streams[key]
@@ -214,6 +223,136 @@ class Encoder(nn.Module):
         """Encoder.forward(embedding(tokens).transpose(1, 2), in_lens) without dropout for a padded batch in any length
         order, masked at every batch size: row b equals Encoder.infer on its own first in_lens[b] tokens."""
         return self._run(None, tokens, embedding.weight, in_lens, True, dropout=False)
+
+
+class _MelEncoderFn(torch.autograd.Function):
+    """MelEncoder forward / backward on the CUDA kernels for up to 64 utterances (ft_mel_encoder_fwd / ft_mel_encoder_bwd).
+    all_lens: the whole batch's lengths, whose maximum divides the time sum."""
+
+    @staticmethod
+    def forward(ctx, enc, mel, out_lens, all_lens, dropout_p, *flat_params):
+        params, i = {}, 0
+        for n, k in _lib.MEL_ENC_PARAM_FIELDS:
+            params[n] = [t.detach().contiguous() for t in flat_params[i:i + k]]
+            i += k
+        mel = mel.detach().contiguous().float()
+        emb = torch.empty(mel.size(0), 512, dtype=torch.float32, device=mel.device)
+        rng = enc._rng_state(mel.device) if dropout_p > 0 else None
+        ctx.desc, ctx.saved = _lib.mel_encoder_fwd(params, mel, out_lens, all_lens, rng, dropout_p, enc.convolutions[0][1].eps, emb)
+        ctx.params = params
+        return emb
+
+    @staticmethod
+    def backward(ctx, d_emb):
+        if ctx.saved is None:
+            raise RuntimeError("MelEncoder backward called twice (the saved activations were released)")
+        grads = _lib.mel_encoder_bwd(ctx.desc, ctx.params, d_emb.contiguous().float(), ctx.saved)
+        ctx.saved = None
+        flat = []
+        for n, _ in _lib.MEL_ENC_PARAM_FIELDS:
+            flat += grads[n]
+        return (None, None, None, None, None, *flat)
+
+
+class MelEncoder(nn.Module):
+    """flowtron.py:416-439, the mel encoder of the Gaussian-mixture prior (2 x conv k=3 + masked instance norm + relu + dropout,
+    packed BiLSTM, mean over time) on its CUDA kernels (csrc/mel_encoder.cu), built for 512 channels, 2 convolutions of width 3
+    and MaskedInstanceNorm1d.
+
+    Every batch size runs masked; the reference leaves a single utterance unmasked, which is the same computation when its
+    length is T (the collate contract T == max(out_lens)).  The time mean divides by max(out_lens), as the reference does, so a
+    row's embedding depends on the longest row of its batch.  The caller's mel is only read; frames past a row's length are
+    never read."""
+
+    def __init__(self, encoder_embedding_dim=512, encoder_kernel_size=3, encoder_n_convolutions=2, norm_fn=MaskedInstanceNorm1d):
+        super().__init__()
+        if (encoder_n_convolutions != 2 or encoder_kernel_size != 3 or encoder_embedding_dim != 512
+                or norm_fn is not MaskedInstanceNorm1d):
+            raise NotImplementedError("the sm_90a mel-encoder kernels are built for encoder_n_convolutions=2, encoder_kernel_size=3, "
+                                      "encoder_embedding_dim=512 and norm_fn=MaskedInstanceNorm1d (mel_encoder_n_hidden=512)")
+        convolutions = []
+        for i in range(encoder_n_convolutions):
+            convolutions.append(nn.Sequential(
+                ConvNorm(80 if i == 0 else encoder_embedding_dim, encoder_embedding_dim, kernel_size=encoder_kernel_size, stride=1,
+                         padding=int((encoder_kernel_size - 1) / 2), dilation=1, w_init_gain='relu'),
+                norm_fn(encoder_embedding_dim, affine=True)))
+        self.convolutions = nn.ModuleList(convolutions)
+        self.lstm = nn.LSTM(encoder_embedding_dim, int(encoder_embedding_dim / 2), 1, bidirectional=True)
+        self.p_dropout = 0.5        # flowtron.py:431 hard-codes 0.5; exposed so tests can run deterministic train-mode steps
+        self._rng = None
+
+    def _rng_state(self, device):
+        """device uint64[2] = {seed, call counter} of the dropout masks; the seed differs from the text encoder's so the two
+        encoders draw independent masks."""
+        if self._rng is None or self._rng.device != device:
+            seed = (torch.initial_seed() ^ 0x5DEECE66D) & 0x7FFFFFFFFFFFFFFF
+            self._rng = torch.tensor([seed, 0], dtype=torch.int64, device=device)
+        return self._rng
+
+    def _kernel_params(self):
+        cs = self.convolutions
+        flat = [c[0].conv.weight for c in cs] + [c[0].conv.bias for c in cs] + [c[1].weight for c in cs] + [c[1].bias for c in cs]
+        for n in ("weight_ih_l0", "weight_hh_l0", "bias_ih_l0", "bias_hh_l0"):
+            flat += [getattr(self.lstm, n), getattr(self.lstm, n + "_reverse")]
+        return flat
+
+    def forward(self, x, lens):
+        """x [B, 80, T] with T == max(lens), lens [B] -> [B, 512].  Batches above 64 utterances run as consecutive calls of at
+        most 64, each divided by the whole batch's longest length."""
+        if not x.is_cuda:
+            raise FlowtronB200Error("MelEncoder needs CUDA tensors: the sm_90a kernels are the only implementation")
+        if x.dim() != 3 or x.size(1) != 80:
+            raise ValueError(f"MelEncoder takes mel [B, 80, T], got {tuple(x.shape)}")
+        if lens is None or lens.numel() != x.size(0):
+            raise ValueError("MelEncoder needs one length per utterance")
+        lens32 = lens.to(device=x.device, dtype=torch.int32).contiguous()
+        dropout_p = self.p_dropout if self.training else 0.0
+        params = self._kernel_params()
+        mb = _lib.MEL_ENC_MAX_BATCH
+        outs = [_MelEncoderFn.apply(self, x[b0:b0 + mb], lens32[b0:b0 + mb], lens32, dropout_p, *params)
+                for b0 in range(0, x.size(0), mb)]
+        return outs[0] if len(outs) == 1 else torch.cat(outs, 0)
+
+    def infer(self, x):
+        raise NotImplementedError("MelEncoder.infer (flowtron.py:441-450) is never called by the reference; use forward")
+
+
+class GaussianMixture(nn.Module):
+    """flowtron.py:313-363: mixture weights, means and log-variances of the prior from the mel embedding (three linear layers
+    and a softmax, in PyTorch like the speaker embedding), or fixed mean / log_var buffers [1, n_mel, K]."""
+
+    def __init__(self, n_hidden, n_components, n_mel_channels, fixed_gaussian, mean_scale):
+        super().__init__()
+        self.n_mel_channels = n_mel_channels
+        self.n_components = n_components
+        self.fixed_gaussian = fixed_gaussian
+        self.mean_scale = mean_scale
+        self.prob_layer = LinearNorm(n_hidden, n_components)
+        if not fixed_gaussian:
+            self.mean_layer = LinearNorm(n_hidden, n_mel_channels * n_components)
+            self.log_var_layer = LinearNorm(n_hidden, n_mel_channels * n_components)
+        else:
+            self.register_buffer('mean', self.generate_mean(n_mel_channels, n_components, mean_scale).float())
+            self.register_buffer('log_var', self.generate_log_var(n_mel_channels, n_components).float())
+
+    def generate_mean(self, n_dimensions, n_components, scale=3):
+        ids = np.random.choice(range(n_dimensions), n_components, replace=False)
+        return (torch.eye(n_dimensions).float()[ids] * scale).transpose(0, 1)[None]
+
+    def generate_log_var(self, n_dimensions, n_components):
+        return torch.zeros(1, n_dimensions, n_components).float()
+
+    def generate_prob(self):
+        return torch.ones(1, 1).float()
+
+    def forward(self, outputs, bs):
+        prob = torch.softmax(self.prob_layer(outputs), dim=1)
+        if not self.fixed_gaussian:
+            mean = self.mean_layer(outputs).view(bs, self.n_mel_channels, self.n_components)
+            log_var = self.log_var_layer(outputs).view(bs, self.n_mel_channels, self.n_components)
+        else:
+            mean, log_var = self.mean, self.log_var
+        return mean, log_var, prob
 
 
 # --------------------------------------------------------------------------------------------- attention params
@@ -472,20 +611,22 @@ def _ragged_lengths(v, B: int, hi: int, name: str) -> Tensor:
 
 
 class Flowtron(nn.Module):
-    """flowtron.py:831-961 (n_components=0 / no cumulative attention: the variants every shipped config uses)."""
+    """flowtron.py:831-961 without cumulative attention; n_components > 1 adds the Gaussian-mixture prior (MelEncoder +
+    GaussianMixture), whose mean, log_var and prob `forward` returns for FlowtronLoss(gm_loss=True)."""
 
     def __init__(self, n_speakers, n_speaker_dim, n_text, n_text_dim, n_flows, n_mel_channels, n_hidden,
                  n_attn_channels, n_lstm_layers, use_gate_layer, mel_encoder_n_hidden, n_components, fixed_gaussian,
                  mean_scale, dummy_speaker_embedding, use_cumm_attention):
         super().__init__()
-        if n_components > 1:
-            raise NotImplementedError("the GMM prior (n_components > 1) is outside the hot-path scope")
         norm_fn = MaskedInstanceNorm1d
         self.speaker_embedding = nn.Embedding(n_speakers, n_speaker_dim)
         self.embedding = nn.Embedding(n_text, n_text_dim)
         self.flows = nn.ModuleList()
         self.encoder = Encoder(norm_fn=norm_fn, encoder_embedding_dim=n_text_dim)
         self.dummy_speaker_embedding = dummy_speaker_embedding
+        if n_components > 1:
+            self.mel_encoder = MelEncoder(mel_encoder_n_hidden, norm_fn=norm_fn)
+            self.gaussian_mixture = GaussianMixture(mel_encoder_n_hidden, n_components, n_mel_channels, fixed_gaussian, mean_scale)
         for i in range(n_flows):
             add_gate = True if (i == (n_flows - 1) and use_gate_layer) else False
             cls = AR_Step if i % 2 == 0 else AR_Back_Step
@@ -588,6 +729,17 @@ class Flowtron(nn.Module):
             encoder_outputs.record_stream(cur)
         else:
             encoder_outputs = self._encode(speaker_ids, text, in_lens)
+        # The mixture prior needs only mel: its encoder runs on a third stream beside the flows and joins the caller's stream
+        # after them, so the loss (the first reader of mean / log_var / prob) waits for it on the device.
+        gm_stream = None
+        if hasattr(self, 'gaussian_mixture'):
+            if mel.is_cuda:
+                cur = torch.cuda.current_stream(mel.device)
+                gm_stream = _mel_encoder_stream(mel.device)
+                gm_stream.wait_stream(cur)
+            with torch.cuda.stream(gm_stream):
+                mel_embedding = self.mel_encoder(mel, out_lens)
+                mean, log_var, prob = self.gaussian_mixture(mel_embedding, mel_embedding.size(0))
         mel = mel.permute(2, 0, 1)
         # key-padding mask from the padded text length (== max(in_lens) by the collate contract): no .item() host sync
         mask = ~(torch.arange(n_text, device=in_lens.device)[None, :] < in_lens[:, None])[..., None]
@@ -599,6 +751,10 @@ class Flowtron(nn.Module):
                 self._side_streams = [torch.cuda.Stream(device=mel.device) for _ in range(2)]
             out = self._run_slices([(0, B // 2), (B // 2, B)], mel, encoder_outputs, mask, out_lens, attn_prior,
                                    streams=self._side_streams)
+        if gm_stream is not None:
+            cur.wait_stream(gm_stream)
+            for t in (mean, log_var, prob):
+                t.record_stream(cur)
         return (*out, mean, log_var, prob)
 
     def encode(self, mel, speaker_ids, text, in_lens, out_lens, attn_prior=None, return_attns=False):
@@ -872,6 +1028,43 @@ class _NllGateFn(torch.autograd.Function):
         return (None, dz, dgate, None, None, *([dls] * ctx.n_flows))
 
 
+class _GmmNllFn(torch.autograd.Function):
+    """Mixture NLL of the Gaussian-mixture prior over n * n_mel valid elements (flowtron.py:217-235 without the log-det term) on
+    ft_gmm_nll_reduce / ft_gmm_nll_grad.  mean / log_var: [B, M, K] learned or [1, M, K] buffers (no gradient)."""
+
+    @staticmethod
+    def forward(ctx, z, out_lens, mean, log_var, prob):
+        T, B, M = z.shape
+        K = prob.size(1)
+        if K > _lib.GMM_MAX_COMPONENTS:
+            raise ValueError(f"the mixture-NLL kernels take at most {_lib.GMM_MAX_COMPONENTS} components, got {K}")
+        if not z.is_cuda:
+            raise FlowtronB200Error("FlowtronLoss needs CUDA tensors")
+        learned = ctx.needs_input_grad[2] or ctx.needs_input_grad[3]
+        if mean.size(0) not in (1, B) or (learned and mean.size(0) != B):
+            raise ValueError(f"mean / log_var must be [B, M, K], or [1, M, K] buffers without a gradient; got {tuple(mean.shape)}")
+        per_row = mean.size(0) == B
+        zc = z.detach().float().contiguous()
+        mc, lc, pc = (t.detach().float().contiguous() for t in (mean, log_var, prob))
+        lens = _lens_i32(out_lens, z.device)
+        sums = torch.empty(2, device=z.device)
+        _lib.gmm_nll_reduce(zc, lens, mc, lc, pc, per_row, sums)
+        ctx.save = (zc, lens, mc, lc, pc, per_row, sums)
+        ctx.learned = learned
+        return sums[0] / (sums[1] * M)
+
+    @staticmethod
+    def backward(ctx, g):
+        zc, lens, mc, lc, pc, per_row, sums = ctx.save
+        gn = (g.reshape(1).float() / (sums[1] * zc.size(2))).contiguous()
+        learned = ctx.learned
+        dz, dprob = torch.empty_like(zc), torch.empty_like(pc)
+        dmean = torch.empty_like(mc) if learned else None
+        dlog_var = torch.empty_like(lc) if learned else None
+        _lib.gmm_nll_grad(zc, lens, mc, lc, pc, per_row, gn, dz, dmean, dlog_var, dprob)
+        return dz, None, dmean, dlog_var, dprob
+
+
 class _AttnCtcFn(torch.autograd.Function):
     """Batched attention-CTC cost per utterance and its gradient in one launch (ft_attn_ctc_loss, csrc/ctc.cu)."""
 
@@ -915,8 +1108,6 @@ class AttentionCTCLoss(nn.Module):
 class FlowtronLoss(nn.Module):
     def __init__(self, sigma=1.0, gm_loss=False, gate_loss=True, use_ctc_loss=False, ctc_loss_weight=0.0, blank_logprob=-1):
         super().__init__()
-        if gm_loss:
-            raise NotImplementedError("gm_loss (GMM prior) is outside the hot-path scope")
         self.sigma = sigma
         self.gm_loss = gm_loss
         self.gate_loss = gate_loss
@@ -928,8 +1119,15 @@ class FlowtronLoss(nn.Module):
     def forward(self, model_output, gate_target, in_lengths, out_lengths, is_validation=False):
         z, log_s_list, gate_pred, attn_list, attn_logprob_list, mean, log_var, prob = model_output
         use_gate = self.gate_loss > 0 and gate_pred is not None
-        loss, gate_loss = _NllGateFn.apply(self.sigma, z, gate_pred if use_gate else None, gate_target, out_lengths,
-                                           *log_s_list)
+        if self.gm_loss:
+            # sigma = inf turns the Gaussian term of ft_nll_reduce off: it then gives -sum log_s / (n M) and the gate loss
+            # (z is passed detached, so its zero gradient is dropped); the mixture NLL replaces the Gaussian term
+            loss, gate_loss = _NllGateFn.apply(math.inf, z.detach(), gate_pred if use_gate else None, gate_target, out_lengths,
+                                               *log_s_list)
+            loss = loss + _GmmNllFn.apply(z, out_lengths, mean, log_var, prob)
+        else:
+            loss, gate_loss = _NllGateFn.apply(self.sigma, z, gate_pred if use_gate else None, gate_target, out_lengths,
+                                               *log_s_list)
         if not use_gate:
             gate_loss = torch.zeros(1, device=z.device)
         loss_ctc = torch.zeros_like(gate_loss)

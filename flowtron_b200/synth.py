@@ -100,6 +100,49 @@ def synth_params(cfg: dict, seed: int = 1234, scale: float = 1.0, dtype=torch.fl
     return out
 
 
+def gmm_param_shapes(cfg: dict) -> Dict[str, Tuple[int, ...]]:
+    """state_dict key -> shape of the Gaussian-mixture prior's modules (mel_encoder, gaussian_mixture) for
+    Flowtron(**cfg) with n_components > 1; learned Gaussians only (the fixed ones are buffers, see synth_gmm_params)."""
+    Hm, K, M = cfg["mel_encoder_n_hidden"], cfg["n_components"], cfg["n_mel_channels"]
+    s: Dict[str, Tuple[int, ...]] = {}
+    for i in range(2):
+        s[f"mel_encoder.convolutions.{i}.0.conv.weight"] = (Hm, M if i == 0 else Hm, 3)
+        s[f"mel_encoder.convolutions.{i}.0.conv.bias"] = (Hm,)
+        s[f"mel_encoder.convolutions.{i}.1.weight"] = (Hm,)
+        s[f"mel_encoder.convolutions.{i}.1.bias"] = (Hm,)
+    for sfx in ("", "_reverse"):
+        s[f"mel_encoder.lstm.weight_ih_l0{sfx}"] = (4 * (Hm // 2), Hm)
+        s[f"mel_encoder.lstm.weight_hh_l0{sfx}"] = (4 * (Hm // 2), Hm // 2)
+        s[f"mel_encoder.lstm.bias_ih_l0{sfx}"] = (4 * (Hm // 2),)
+        s[f"mel_encoder.lstm.bias_hh_l0{sfx}"] = (4 * (Hm // 2),)
+    layers = ("prob",) if cfg["fixed_gaussian"] else ("prob", "mean", "log_var")
+    for n in layers:
+        out = K if n == "prob" else M * K
+        s[f"gaussian_mixture.{n}_layer.linear_layer.weight"] = (out, Hm)
+        s[f"gaussian_mixture.{n}_layer.linear_layer.bias"] = (out,)
+    return s
+
+
+def synth_gmm_params(cfg: dict, seed: int = 1234) -> Dict[str, torch.Tensor]:
+    """Deterministic weights for every state_dict key of Flowtron(**cfg) with n_components > 1: synth_params for the rest of
+    the model, the same per-name rule for the prior's parameters and, with fixed_gaussian, the reference's buffers
+    (mean = mean_scale * n_components distinct unit vectors, log_var = 0) from a seeded choice of the unit vectors."""
+    out = synth_params(dict(cfg, n_components=0), seed)
+    for name, shape in gmm_param_shapes(cfg).items():
+        g = torch.Generator(device="cpu")
+        g.manual_seed((seed * 1000003 + zlib.crc32(name.encode())) % (2 ** 63 - 1))
+        t = torch.randn(shape, generator=g, dtype=torch.float32) * _std_for(name, shape)
+        out[name] = t + 1.0 if name.endswith(".1.weight") else t
+    if cfg["fixed_gaussian"]:
+        M, K = cfg["n_mel_channels"], cfg["n_components"]
+        g = torch.Generator(device="cpu")
+        g.manual_seed(seed)
+        ids = torch.randperm(M, generator=g)[:K]
+        out["gaussian_mixture.mean"] = (torch.eye(M)[ids] * float(cfg["mean_scale"])).transpose(0, 1)[None].contiguous()
+        out["gaussian_mixture.log_var"] = torch.zeros(1, M, K)
+    return out
+
+
 def synth_batch(B: int, T: int, L: int, cfg: dict = DEFAULT_MODEL_CONFIG, seed: int = 1234,
                 out_lens=None, in_lens=None, with_prior: bool = False, logmel_stats: bool = False):
     """Synthetic training batch in DataCollate layout (data.py:197-246):

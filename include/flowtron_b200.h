@@ -331,6 +331,64 @@ int ft_encoder_bwd(const FtEncoderDesc* d, const FtEncoderWeights* w, const floa
                    long long d_stride_l, const void* saved, float* d_x, const FtEncoderGrads* grads, void* scratch, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------
+ * MelEncoder of the Gaussian-mixture prior (flowtron.py:416-439): 2 x [conv k=3 (80 -> 512, 512 -> 512) -> masked instance
+ * norm (affine) -> relu -> dropout], packed BiLSTM 512 -> 2 x 256, mean over time.  Same conventions as the text encoder.
+ * ---------------------------------------------------------------------------------------------------- */
+#define FT_MEL_ENC_MAX_BATCH 64
+
+typedef struct {
+    int B, T;                 /* utterances in this call (1..64), padded frames (any T: limited by memory only) */
+    float eps, dropout_p;     /* instance-norm eps; dropout probability (0: eval)                                 */
+} FtMelEncoderDesc;
+
+typedef struct {
+    const float* conv_w[2]; const float* conv_b[2];    /* [512,80,3] / [512,512,3], [512] */
+    const float* norm_w[2]; const float* norm_b[2];    /* [512]                           */
+    const float* w_ih[2]; const float* w_hh[2];        /* [1024,512], [1024,256]          */
+    const float* b_ih[2]; const float* b_hh[2];        /* [1024]                          */
+} FtMelEncoderWeights;
+
+typedef struct {                                       /* gradients, same shapes, OVERWRITTEN */
+    float* d_conv_w[2]; float* d_conv_b[2];
+    float* d_norm_w[2]; float* d_norm_b[2];
+    float* d_w_ih[2]; float* d_w_hh[2];
+    float* d_b_ih[2]; float* d_b_hh[2];
+} FtMelEncoderGrads;
+
+size_t ft_mel_encoder_saved_bytes(const FtMelEncoderDesc* d);
+size_t ft_mel_encoder_fwd_scratch_bytes(const FtMelEncoderDesc* d);
+size_t ft_mel_encoder_bwd_scratch_bytes(const FtMelEncoderDesc* d);
+/* mel [B, 80, T] fp32 (read only; frames at t >= out_lens[b] are never read); out_lens int32 [B], every length in [1, T];
+ * all_lens int32 [n_all]: the lengths of the whole batch this call is a slice of, whose maximum divides the time sum (the
+ * reference's torch.mean over the padded LSTM output); rng_state as for ft_encoder_fwd; emb [B, 512] fp32. */
+int ft_mel_encoder_fwd(const FtMelEncoderDesc* d, const FtMelEncoderWeights* w, const float* mel, const int* out_lens,
+                       const int* all_lens, int n_all, unsigned long long* rng_state, float* emb, void* saved, void* scratch,
+                       void* stream);
+/* d_emb [B, 512] fp32; weight gradients only (no gradient w.r.t. the mel). */
+int ft_mel_encoder_bwd(const FtMelEncoderDesc* d, const FtMelEncoderWeights* w, const float* d_emb, const void* saved,
+                       const FtMelEncoderGrads* grads, void* scratch, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------
+ * Gaussian-mixture NLL (FlowtronLoss gm_loss=True, flowtron.py:217-235):
+ *   nll = -sum_{t < out_lens[b], b, m} logsumexp_k [log prob_bk - log_var_bmk / 2 - (z_tbm - mean_bmk)^2 / (2 exp log_var_bmk)]
+ * z [T, B, M] fp32; mean / log_var [B, M, K] (per_row = 1) or [1, M, K] (per_row = 0); prob [B, K].  K <= 32, M <= 80.
+ * Fixed summation order, no atomics: replays are bit-identical.
+ * ---------------------------------------------------------------------------------------------------- */
+#define FT_GMM_MAX_COMPONENTS 32
+
+typedef struct { int T, B, M, K, per_row; } FtGmmDesc;
+
+size_t ft_gmm_nll_scratch_bytes(const FtGmmDesc* d);
+/* sums[0] = nll, sums[1] = number of valid frames */
+int ft_gmm_nll_reduce(const FtGmmDesc* d, const float* z, const int* out_lens, const float* mean, const float* log_var,
+                      const float* prob, float* sums, void* scratch, void* stream);
+/* gradients of g_nll[0] * nll: dz [T, B, M] (zero past the lengths), dprob [B, K], and dmean / dlog_var [B, M, K] (both NULL
+ * when the Gaussians are shared buffers: per_row must then be 0 or they are ignored) -- all overwritten. */
+int ft_gmm_nll_grad(const FtGmmDesc* d, const float* z, const int* out_lens, const float* mean, const float* log_var,
+                    const float* prob, const float* g_nll, float* dz, float* dmean, float* dlog_var, float* dprob, void* scratch,
+                    void* stream);
+
+/* ------------------------------------------------------------------------------------------------------
  * WaveGlow vocoder, inference direction (tacotron2/waveglow/glow.py:251-293 WaveGlow.infer): log-mel -> audio.
  * Built for n_mel 80, n_group 8, WN n_channels 256, kernel_size 3; n_flows <= 16, n_layers <= 8.
  * ---------------------------------------------------------------------------------------------------- */
