@@ -220,6 +220,12 @@ def _declare(L):
     L.ft_waveglow_infer.restype = c_int
     L.ft_posterior_mean.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_float, c_void_p, c_void_p]
     L.ft_posterior_mean.restype = c_int
+    L.ft_mas_align_scratch_bytes.argtypes = [c_int, c_int, c_int]
+    L.ft_mas_align_scratch_bytes.restype = c_size_t
+    L.ft_mas_align.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]
+    L.ft_mas_align.restype = c_int
+    L.ft_durations_to_attn.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]
+    L.ft_durations_to_attn.restype = c_int
     for fn in ("ft_mel_encoder_saved_bytes", "ft_mel_encoder_fwd_scratch_bytes", "ft_mel_encoder_bwd_scratch_bytes"):
         getattr(L, fn).argtypes = [POINTER(FtMelEncoderDesc)]
         getattr(L, fn).restype = c_size_t
@@ -549,6 +555,28 @@ def posterior_mean(z, out_lens, n_frames, mode, scale, out):
     assert z.dtype == torch.float32 and z.is_contiguous() and out_lens.dtype == torch.int32 and out.is_contiguous()
     check(lib().ft_posterior_mean(ptr(z), int(T), int(B), int(M), ptr(out_lens), int(n_frames), int(mode), float(scale),
                                   ptr(out), stream_ptr()), "ft_posterior_mean")
+
+
+def mas_align(logp, in_lens, out_lens, time_reversed, durations, token_of_frame):
+    """logp [B,T,L] f32 CUDA, in_lens / out_lens int32 CUDA [B]; durations int32 [B,L], token_of_frame int32 [B,T] written.
+    One launch (csrc/align.cu)."""
+    _need_cuda(logp, in_lens, out_lens, durations, token_of_frame)
+    B, T, L = logp.shape
+    assert logp.dtype == torch.float32 and logp.is_contiguous() and in_lens.dtype == torch.int32 and out_lens.dtype == torch.int32
+    assert durations.dtype == torch.int32 and token_of_frame.dtype == torch.int32
+    scratch = scratch_buffer(int(lib().ft_mas_align_scratch_bytes(B, T, L)), logp.device)
+    check(lib().ft_mas_align(ptr(logp), ptr(in_lens), ptr(out_lens), B, T, L, 1 if time_reversed else 0, ptr(durations),
+                             ptr(token_of_frame), ptr(scratch), stream_ptr()), "ft_mas_align")
+
+
+def durations_to_attn(durations, in_lens, time_reversed, out):
+    """durations int32 CUDA [B,L], in_lens int32 CUDA [B]; out f32 [B,Ta,L] (written).  One launch (csrc/align.cu)."""
+    _need_cuda(durations, in_lens, out)
+    B, Ta, L = out.shape
+    assert durations.dtype == torch.int32 and durations.is_contiguous() and in_lens.dtype == torch.int32
+    assert out.dtype == torch.float32 and out.is_contiguous()
+    check(lib().ft_durations_to_attn(ptr(durations), ptr(in_lens), B, L, Ta, 1 if time_reversed else 0, ptr(out),
+                                     stream_ptr()), "ft_durations_to_attn")
 
 
 def radam_step_dev_raw(p_ptr, g_ptr, m_ptr, v_ptr, n, beta1, beta2, eps, weight_decay, lr, step_dev, coef_ptr=0):

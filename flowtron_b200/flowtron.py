@@ -783,11 +783,19 @@ class Flowtron(nn.Module):
         ``return_attns=True`` returns ``(z, attns)``: ``attns[f]`` [B, T, L] is flow f's attention as ``forward`` returns it in
         ``attns_list`` (row b left-aligned in that flow's own time order: an AR_Back_Step's rows run back to front over
         their out_lens[b] frames), zero at t >= out_lens[b] and l >= in_lens[b] -- what ``infer_aligned`` takes."""
+        checked = self._encode_args(mel, speaker_ids, text, in_lens, out_lens, attn_prior, "Flowtron.encode")
+        z, attns, _ = self._encode_batch(mel, speaker_ids, text, attn_prior, *checked, return_attns)
+        z = z.permute(1, 2, 0)
+        return (z, attns) if return_attns else z
+
+    def _encode_args(self, mel, speaker_ids, text, in_lens, out_lens, attn_prior, where):
+        """encode's argument checks -> (in_lens, out_lens int32 on the device, groups: None, or for host lengths the
+        (rows, their longest) on each side of _ATTN_OVERLAP_MIN_T)."""
         if mel.dim() != 3 or text.dim() != 2 or speaker_ids.dim() != 1:
-            raise ValueError("encode expects mel [B, n_mel, T], speaker_ids [B] and text [B, L]")
+            raise ValueError(f"{where} expects mel [B, n_mel, T], speaker_ids [B] and text [B, L]")
         B, _, T = mel.shape
         L = text.size(1)
-        _lib.check_text_len(L, "Flowtron.encode")
+        _lib.check_text_len(L, where)
         if text.size(0) != B or speaker_ids.size(0) != B or B < 1 or T < 1 or L < 1:
             raise ValueError(f"batch sizes disagree or are empty: mel {tuple(mel.shape)}, "
                              f"speaker_ids {tuple(speaker_ids.shape)}, text {tuple(text.shape)}")
@@ -796,7 +804,7 @@ class Flowtron(nn.Module):
         in_lens = _ragged_lengths(in_lens, B, L, "in_lens")
         out_lens = _ragged_lengths(out_lens, B, T, "out_lens")
         if not (mel.is_cuda and text.is_cuda and speaker_ids.is_cuda and (attn_prior is None or attn_prior.is_cuda)):
-            raise FlowtronB200Error("Flowtron.encode needs CUDA tensors: the sm_90a kernels are the only implementation")
+            raise FlowtronB200Error(f"{where} needs CUDA tensors: the sm_90a kernels are the only implementation")
         dev = mel.device
         groups = None                       # host lengths: (rows, their longest) on each side of _ATTN_OVERLAP_MIN_T
         if not out_lens.is_cuda:
@@ -804,28 +812,36 @@ class Flowtron(nn.Module):
             short = [b for b in range(B) if lens[b] < _ATTN_OVERLAP_MIN_T]
             long_rows = [b for b in range(B) if lens[b] >= _ATTN_OVERLAP_MIN_T]
             groups = [(rows, max(lens[b] for b in rows)) for rows in (short, long_rows) if rows]
-        in_lens = in_lens.to(device=dev, dtype=torch.int32)
-        out_lens = out_lens.to(device=dev, dtype=torch.int32)
+        return in_lens.to(device=dev, dtype=torch.int32), out_lens.to(device=dev, dtype=torch.int32), groups
+
+    def _encode_batch(self, mel, speaker_ids, text, attn_prior, in_lens, out_lens, groups, return_attns, logprob_flow=None):
+        """encode's work on checked inputs, one _encode_rows call per row group -> (z [T, B, 80], the flows' attention or
+        None, flow ``logprob_flow``'s attn_logprob [B, T, L] (defined inside each row's lengths) or None)."""
+        B, _, T = mel.shape
+        L = text.size(1)
+        dev = mel.device
         with torch.no_grad():
             if groups is None or groups == [(list(range(B)), T)]:
-                z, attns = self._encode_rows(mel, speaker_ids, text, in_lens, out_lens, attn_prior, return_attns)
-            else:
-                z = torch.zeros(T, B, mel.size(1), device=dev)
-                attns = [torch.zeros(B, T, L, device=dev) for _ in self.flows] if return_attns else None
-                for rows, t in groups:
-                    idx = torch.tensor(rows, device=dev)
-                    prior = None if attn_prior is None else attn_prior[idx, :t]
-                    zg, ag = self._encode_rows(mel[idx, :, :t], speaker_ids[idx], text[idx], in_lens[idx], out_lens[idx], prior,
-                                               return_attns)
-                    z[:t].index_copy_(1, idx, zg)
-                    for a, g in zip(attns or (), ag or ()):
-                        a[:, :t].index_copy_(0, idx, g)
-        z = z.permute(1, 2, 0)
-        return (z, attns) if return_attns else z
+                return self._encode_rows(mel, speaker_ids, text, in_lens, out_lens, attn_prior, return_attns, logprob_flow)
+            z = torch.zeros(T, B, mel.size(1), device=dev)
+            attns = [torch.zeros(B, T, L, device=dev) for _ in self.flows] if return_attns else None
+            logp = None if logprob_flow is None else torch.zeros(B, T, L, device=dev)
+            for rows, t in groups:
+                idx = torch.tensor(rows, device=dev)
+                prior = None if attn_prior is None else attn_prior[idx, :t]
+                zg, ag, lg = self._encode_rows(mel[idx, :, :t], speaker_ids[idx], text[idx], in_lens[idx], out_lens[idx], prior,
+                                               return_attns, logprob_flow)
+                z[:t].index_copy_(1, idx, zg)
+                for a, g in zip(attns or (), ag or ()):
+                    a[:, :t].index_copy_(0, idx, g)
+                if logp is not None:
+                    logp[:, :t].index_copy_(0, idx, lg)
+        return z, attns, logp
 
-    def _encode_rows(self, mel, speaker_ids, text, in_lens, out_lens, attn_prior, return_attns=False):
+    def _encode_rows(self, mel, speaker_ids, text, in_lens, out_lens, attn_prior, return_attns=False, logprob_flow=None):
         """Flowtron.encode's work on checked inputs (lengths int32 on the device) -> (z [T, B, 80], zero past out_lens;
-        the flows' attention [B, T, L] zeroed outside each row's lengths, or None)."""
+        the flows' attention [B, T, L] zeroed outside each row's lengths, or None; flow ``logprob_flow``'s attn_logprob
+        [B, T, L] as ``forward`` returns it, or None)."""
         T, dev = mel.size(2), mel.device
         encoder_outputs = self._with_speaker(speaker_ids, self.encoder.infer_ragged_tokens(text, self.embedding, in_lens))
         mask = ~(torch.arange(encoder_outputs.size(0), device=dev)[None, :] < in_lens[:, None])[..., None]
@@ -833,10 +849,11 @@ class Flowtron(nn.Module):
         # forward leaves frames at or past out_lens[b] undefined
         past = torch.arange(T, device=dev)[:, None] >= out_lens[None, :]
         z = out[0].masked_fill_(past[:, :, None], 0.0)
+        logp = None if logprob_flow is None else out[4][logprob_flow]
         if not return_attns:
-            return z, None
+            return z, None, logp
         outside = past.t()[:, :, None] | mask.transpose(1, 2)                 # [B, T, 1] | [B, 1, L]
-        return z, [a.masked_fill(outside, 0.0) for a in out[3]]
+        return z, [a.masked_fill(outside, 0.0) for a in out[3]], logp
 
     def infer(self, residual, speaker_ids, text, temperature=1.0, gate_threshold=0.5, attns=None, attn_prior=None):
         """residual [B, 80, T] -> (mel [B, 80, T'], attention_weights: per flow in application order, T' rows [B, 1, L]).
@@ -983,6 +1000,76 @@ class Flowtron(nn.Module):
             raise ValueError(f"target_speaker_ids must hold {mel.size(0)} values, got shape {tuple(target_speaker_ids.shape)}")
         z, attns = self.encode(mel, speaker_ids, text, in_lens, out_lens, attn_prior, return_attns=True)
         return self.infer_aligned(z, target_speaker_ids, text, in_lens, attns, out_lens)[0]
+
+    def align(self, mel, speaker_ids, text, in_lens, out_lens, attn_prior=None, flow=0):
+        """Hard alignments of a padded batch of recorded utterances: which token each frame belongs to and how many frames
+        each token lasts, by monotonic alignment search (``align.mas``) over flow ``flow``'s attention log-probabilities.
+
+        mel [B, 80, T] f32, speaker_ids [B], text [B, L] int64, in_lens [B], out_lens [B], attn_prior [B, T, L] or None ->
+        (durations int64 [B, L], token_of_frame int64 [B, T]): each of row b's in_lens[b] tokens lasts at least one frame,
+        the durations sum to out_lens[b] and are 0 from in_lens[b] on; token_of_frame[b, t] is in natural time and -1 from
+        out_lens[b] on.
+
+        The mel -> z direction runs exactly as in ``encode``: the same argument checks, no autograd state, the text encoder
+        without dropout and, with host lengths, the same short / long row split, so row b equals its own B = 1 call bit for
+        bit.  The search reads the flow's ``attn_logprob`` as ``forward`` returns it (an AR_Back_Step's in flipped time,
+        mapped back inside the kernel), so the path is the one under the prior's posterior when ``attn_prior`` is given and
+        under log(attention + 1e-8) otherwise.  Host lengths must also give every row at least as many frames as tokens
+        (ValueError); with CUDA length tensors such a row gets zero durations and -1 everywhere, and the call makes no host
+        synchronisation, so it can be captured in a CUDA graph."""
+        if isinstance(flow, bool) or not isinstance(flow, (int, np.integer)) or not 0 <= flow < len(self.flows):
+            raise ValueError(f"flow must be a flow index in [0, {len(self.flows)}), got {flow!r}")
+        if not any(torch.is_tensor(v) and v.is_cuda for v in (in_lens, out_lens)):
+            il, ol = torch.as_tensor(in_lens), torch.as_tensor(out_lens)
+            if il.shape == ol.shape and bool((ol < il).any()):
+                raise ValueError(f"every row needs at least as many frames as tokens: out_lens {ol.tolist()}, "
+                                 f"in_lens {il.tolist()}")
+        from .align import mas                  # align.py imports this module
+        checked = self._encode_args(mel, speaker_ids, text, in_lens, out_lens, attn_prior, "Flowtron.align")
+        _, _, logp = self._encode_batch(mel, speaker_ids, text, attn_prior, *checked, False, int(flow))
+        return mas(logp, checked[0], checked[1], time_reversed=isinstance(self.flows[flow], AR_Back_Step))
+
+    def infer_durations(self, residual, speaker_ids, text, in_lens, durations, gate_threshold=1.0):
+        """Inference with the timing given as per-token durations: every flow is forced onto the hard alignment in which
+        token l of row b lasts durations[b, l] frames (duration editing, speaking-rate control).
+
+        residual [B, 80, T] f32, speaker_ids [B], text [B, L] int64, in_lens [B], durations [B, L] integers (what ``align``
+        returns, edited or not) -> (mel [B, 80, T], mel_lens int64 [B]).  Row b lasts n_b = durations[b, :in_lens[b]].sum()
+        frames; durations past in_lens[b] are ignored.  One-hot maps (``align.hard_attention``, back to front for an
+        AR_Back_Step) spanning the T frames go to ``infer_aligned`` with n_frames = n_b, computed on the device; with the
+        default gate_threshold of 1 the gate is off and ``mel_lens`` is n_b.
+
+        Host durations are checked (ValueError unless they are non-negative and every row sums to between 1 and T), as are
+        host in_lens (1 <= in_lens[b] <= L); CUDA tensors are trusted, and then the call makes no host synchronisation and
+        can be captured in a CUDA graph."""
+        if residual.dim() != 3 or text.dim() != 2 or speaker_ids.dim() != 1:
+            raise ValueError("infer_durations expects residual [B, n_mel, T], speaker_ids [B] and text [B, L]")
+        B, _, T = residual.shape
+        L = text.size(1)
+        _lib.check_text_len(L, "Flowtron.infer_durations")
+        if text.size(0) != B or speaker_ids.size(0) != B or B < 1 or T < 1 or L < 1:
+            raise ValueError(f"batch sizes disagree or are empty: residual {tuple(residual.shape)}, "
+                             f"speaker_ids {tuple(speaker_ids.shape)}, text {tuple(text.shape)}")
+        if (not torch.is_tensor(durations) or tuple(durations.shape) != (B, L) or durations.is_floating_point()
+                or durations.dtype == torch.bool):
+            raise ValueError(f"durations must be an integer tensor [B, L] = ({B}, {L}), got "
+                             f"{tuple(durations.shape) if torch.is_tensor(durations) else type(durations).__name__}")
+        in_lens = _ragged_lengths(in_lens, B, L, "in_lens")
+        if not durations.is_cuda:
+            sums = durations.sum(1)
+            if bool((durations < 0).any()) or bool((sums < 1).any()) or bool((sums > T).any()):
+                raise ValueError(f"durations must be non-negative with row sums in [1, {T}], got row sums {sums.tolist()}")
+        if not (residual.is_cuda and text.is_cuda and speaker_ids.is_cuda):
+            raise FlowtronB200Error("Flowtron.infer_durations needs CUDA tensors: the sm_90a kernels are the only "
+                                    "implementation")
+        from .align import hard_attention       # align.py imports this module
+        dev = residual.device
+        in_lens = in_lens.to(device=dev, dtype=torch.int32)
+        durations = durations.to(device=dev)
+        kept = torch.arange(L, device=dev)[None, :] < in_lens[:, None]
+        n_frames = torch.where(kept, durations.clamp(min=0), 0).sum(1).to(torch.int32)
+        attns = [hard_attention(durations, in_lens, T, time_reversed=isinstance(f, AR_Back_Step)) for f in self.flows]
+        return self.infer_aligned(residual, speaker_ids, text, in_lens, attns, n_frames, gate_threshold)
 
     @staticmethod
     def set_temperature_and_gate(flow, temperature, gate_threshold):

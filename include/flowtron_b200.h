@@ -442,6 +442,29 @@ int ft_waveglow_infer(const FtWaveGlowDesc* d, const FtWaveGlowWeights* w, const
 int ft_posterior_mean(const float* z, int T, int B, int M, const int* out_lens, int n_frames, int mode, float scale,
                       float* out, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------
+ * Hard alignments (csrc/align.cu): monotonic alignment search over one flow's attention log-probabilities, and the
+ * one-hot maps of per-token durations.
+ * ---------------------------------------------------------------------------------------------------- */
+/* logp fp32 [B, T, L] (a flow's attn_logprob), in_lens / out_lens int32 [B] on the device, L <= FT_MAX_TEXT_LEN, any T.
+ * Row b (Tb = out_lens[b], Lb = in_lens[b]), s[t][l] = logp[b, t', l] with t' = t, or Tb-1-t when time_reversed (an
+ * AR_Back_Step's flipped time):  Q[0][0] = s[0][0], Q[0][l > 0] = -inf, Q[t][l] = s[t][l] + max(Q[t-1][l], Q[t-1][l-1])
+ * (Q[t-1][-1] = -inf), fp32 adds without contraction.  The path ends at (Tb-1, Lb-1) and, walked back, moves to l-1 only
+ * where Q[t-1][l-1] > Q[t-1][l] (ties stay on the token).  token_of_frame int32 [B, T] (natural time): the path's token at
+ * frame t < Tb, -1 from Tb on; durations int32 [B, L]: frames per token (each >= 1, summing to Tb), 0 from Lb on.  A row
+ * with Tb < Lb (or Lb = 0) has no path: all-zero durations, -1 everywhere.  Only t < Tb, l < Lb are read.  scratch:
+ * ft_mas_align_scratch_bytes(B, T, L) (the backpointer bits, T * ceil(L/32) words per row).  One launch, no allocation, no
+ * host synchronisation (CUDA-graph capturable). */
+size_t ft_mas_align_scratch_bytes(int B, int T, int L);
+int ft_mas_align(const float* logp, const int* in_lens, const int* out_lens, int B, int T, int L, int time_reversed,
+                 int* durations, int* token_of_frame, void* scratch, void* stream);
+/* durations int32 [B, L] (tokens at l >= in_lens[b] and negative values count as 0), in_lens int32 [B] on the device ->
+ * out fp32 [B, Ta, L], one-hot: with n_b = sum_l durations[b, l], row (b, i) for i < n_b is generation step i -- natural
+ * frame i, or n_b-1-i when time_reversed -- and holds a 1 at the token that frame belongs to; every other entry is 0.
+ * The prefix sums are computed on the device.  One launch, no allocation, no host synchronisation. */
+int ft_durations_to_attn(const int* durations, const int* in_lens, int B, int L, int Ta, int time_reversed, float* out,
+                         void* stream);
+
 #ifdef __cplusplus
 }
 #endif
