@@ -292,7 +292,7 @@ def _need_cuda(*ts):
 
 
 def set_gemm_pair_mode(mode: int):
-    """0 = single-CTA tiles, 1 = CTA pairs for big contractions (default), 2 = CTA pairs whenever eligible."""
+    """0 = single-CTA tiles (default), 1 = CTA pairs for big contractions, 2 = CTA pairs whenever eligible."""
     lib().ft_set_gemm_pair_mode(int(mode))
 
 

@@ -38,7 +38,7 @@ struct GemmArgs {
 int launch_gemm(const GemmArgs& g, cudaStream_t st);
 void set_gemm_pair_mode(int mode);   // 0 never, 1 big contractions only (default), 2 whenever eligible
 int make_tmap_2d(CUtensorMap* out, const void* ptr, int fmt, long long rows, long long cols, long long ld,
-                 int box_cols, int box_rows);
+                 int box_cols, int box_rows, int swizzle_bytes = 128);   // 128 or 64: the box's inner extent in bytes
 
 void set_lstm_trace(long long* p);
 int launch_lstm_fwd(int T, int B, const float* xproj, const void* whh16, const int* lens, void* hseq16, long long ldh,

@@ -18,27 +18,31 @@ int ensure_tma_encoder() {
 
 PFN_encodeTiled get_tma_encoder() { return ensure_tma_encoder() ? nullptr : g_encode; }
 
-// 2D row-major tensor [rows, cols] (cols contiguous, row pitch ld elements), box {box_cols, box_rows}, SW128.
+// 2D row-major tensor [rows, cols] (cols contiguous, row pitch ld elements), box {box_cols, box_rows}, SW128 (or SW64).
 int make_tmap_2d(CUtensorMap* out, const void* ptr, int fmt, long long rows, long long cols, long long ld,
-                 int box_cols, int box_rows) {
+                 int box_cols, int box_rows, int swizzle_bytes) {
     if (ensure_tma_encoder()) return -1;
     const int elt = (fmt == 2) ? 4 : 2;
     CUtensorMapDataType dt = fmt == 0 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
                            : fmt == 1 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
     if ((reinterpret_cast<uintptr_t>(ptr) & 15) || ((ld * elt) & 15)) return ft_set_error("TMA operand must be 16-byte aligned with a 16-byte-multiple row pitch");
-    if (box_cols * elt != 128) return ft_set_error("TMA box inner extent must be 128 bytes (SWIZZLE_128B)");
+    if (box_cols * elt != swizzle_bytes || (swizzle_bytes != 128 && swizzle_bytes != 64))
+        return ft_set_error("TMA box inner extent must be the swizzle span (128 or 64 bytes)");
     cuuint64_t dims[2] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows)};
     cuuint64_t strides[1] = {static_cast<cuuint64_t>(ld * elt)};
     cuuint32_t box[2] = {static_cast<cuuint32_t>(box_cols), static_cast<cuuint32_t>(box_rows)};
     cuuint32_t estr[2] = {1, 1};
     CUresult r = g_encode(out, dt, 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                          CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                          swizzle_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return ft_set_error("cuTensorMapEncodeTiled failed");
     return 0;
 }
 
-static int g_pair_mode = 1;         // 0 never, 1 big contractions only, 2 whenever eligible
+// 0 never (default), 1 big contractions only, 2 whenever eligible.  On the H100 80GB HBM3 (700 W) CTA pairs were slower
+// than single-CTA tiles at every training shape they were eligible for (tools/gemm_shapes.py, DESIGN 4.1), so by default
+// they are not used; ft_set_gemm_pair_mode keeps them selectable.
+static int g_pair_mode = 0;
 void set_gemm_pair_mode(int mode) { g_pair_mode = mode; }
 
 extern template const void* gemm_kernel_ptr<FMT_F16, 0>(int, int, int);
@@ -70,7 +74,7 @@ int launch_gemm(const GemmArgs& g, cudaStream_t st) {
     if (n_tiles_ll > 0x7fffffff) return ft_set_error("gemm: too many tiles");
     int n_tiles = static_cast<int>(n_tiles_ll);
     // split-K: long reductions with few output tiles (the dense / projection weight gradients: K = T*B rows, 8-64 tiles)
-    // would leave most SMs idle; each K range is reduced by its own CTA and added atomically into a zeroed C32
+    // would leave most SMs idle; each K range is reduced by its own CTA and added into a zeroed C32
     const int num_kb_all = (g.K + BK - 1) / BK;
     int splitk = 1;
     const bool splittable = g.C32 && !g.C16 && !g.beta && !g.bias && !g.bias2 && g.act == 0 && (g.N % 4 == 0) &&
@@ -84,8 +88,24 @@ int launch_gemm(const GemmArgs& g, cudaStream_t st) {
         if (cudaMemsetAsync(g.C32, 0, sizeof(float) * static_cast<size_t>(g.M) * g.N, st) != cudaSuccess) return ft_set_error("gemm: memset failed");
     }
     p.splitk = splitk;
-    // 2-CTA clusters (B multicast) for wide outputs with enough 256 x 256 tiles to fill the machine.  Mode 1 (default;
-    // ft_set_gemm_pair_mode overrides): only for the big contractions (>= 1e11 FLOP).  Mode 2: whenever eligible.
+    // Staged TMA-store epilogue wherever the outputs allow it (16-byte aligned base and row pitch, even N, the pair loads of
+    // bias / aux aligned); anything else keeps the fragment stores.  C32 += tile goes through TMA reduce-add for split-K
+    // partial tiles and for beta without a 16-bit output (with one, the old C32 is read so that C16 gets the sum too).
+    auto al = [](const void* q, int a) { return (reinterpret_cast<uintptr_t>(q) & (a - 1)) == 0; };
+    const bool tma_c = (g.N % 2 == 0) &&
+                       (!g.C32 || (al(g.C32, 16) && (g.ldc32 * 4) % 16 == 0)) &&
+                       (!g.C16 || (al(g.C16, 16) && (g.ldc16 * 2) % 16 == 0)) &&
+                       (g.act != 2 || (al(g.aux16, 4) && g.ldaux % 2 == 0)) &&
+                       (!g.bias || al(g.bias, 8)) && (!g.bias2 || al(g.bias2, 8));
+    CUtensorMap tmC32 = {}, tmC16 = {};
+    if (tma_c) {
+        p.tma_c = 1;
+        p.c32_add = g.C32 && (splitk > 1 || (g.beta && !g.C16));
+        if (g.C32 && make_tmap_2d(&tmC32, g.C32, FMT_TF32, g.M, g.N, g.ldc32, 32, 64)) return -1;
+        if (g.C16 && make_tmap_2d(&tmC16, g.C16, g.c16_fmt, g.M, g.N, g.ldc16, 32, 64, 64)) return -1;
+    }
+    // 2-CTA clusters (B multicast) for wide outputs with enough 256 x 256 tiles to fill the machine, only when
+    // ft_set_gemm_pair_mode asks for them.  Mode 1: only for the big contractions (>= 1e11 FLOP).  Mode 2: whenever eligible.
     const long long tiles_m2 = (g.M + 2 * BM - 1) / (2 * BM);
     const bool big = 2.0 * g.M * g.N * g.K >= 1e11;
     const int ncta = ((g_pair_mode == 2 || (g_pair_mode == 1 && big)) && wide && splitk == 1 && tiles_m2 * tiles_n >= sms / 2) ? 2 : 1;
@@ -116,7 +136,7 @@ int launch_gemm(const GemmArgs& g, cudaStream_t st) {
     attr[0].id = cudaLaunchAttributeClusterDimension;
     attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr; cfg.numAttrs = ncta == 2 ? 1 : 0;
-    void* args[] = {&tmA, &tmB, &p, const_cast<int*>(&tiles_n), &n_tiles};
+    void* args[] = {&tmA, &tmB, &tmC32, &tmC16, &p, const_cast<int*>(&tiles_n), &n_tiles};
     TimeScope ts(g.a_mn ? "gemm_wgrad" : (g.b_mn ? "gemm_dgrad" : "gemm_fwd"), g.M, g.N, g.K, st);
     cudaError_t e = cudaLaunchKernelExC(&cfg, fn, args);
     if (e != cudaSuccess) return ft_set_error(cudaGetErrorString(e));

@@ -8,7 +8,10 @@
 //    4-stage (BN = 256: 48 KB per stage) / 6-stage (BN = 128: 32 KB) TMA ring in SWIZZLE_128B layout, optional split-K;
 //  * warpgroup roles: WG0 = TMA producer (one elected thread), WG1 / WG2 = consumers, each owning 64 rows of the tile with a
 //    64 x BN fp32 accumulator in registers (128 registers per thread at BN = 256; setmaxnreg moves registers from the
-//    producer to the consumers).  While a consumer runs its epilogue the producer already fills the ring for its next tile.
+//    producer to the consumers).  While a consumer runs its epilogue the producer already fills the ring for its next tile;
+//  * epilogue through shared memory: each consumer stages its 64 x BN result in 64 x 32 chunks (two 8 KB slots, SWIZZLE_128B
+//    for fp32 / SWIZZLE_64B for 16-bit outputs) and writes them with TMA stores (reduce-add for split-K partial tiles and
+//    for beta = 1 without a 16-bit output), so it returns to its next tile's wgmmas while the stores drain.
 //
 // Used for every non-recurrent contraction on the Flowtron hot path (LSTM input projections flowtron.py:654-655, attention
 // Q/K/V projections :568-571, DenseLayer :461-464, 1x1 conv :768, and all their dgrad/wgrad counterparts).
@@ -33,17 +36,21 @@ struct GemmParams {
     float* C32; long long ldc32;
     void* C16; long long ldc16; int c16_fmt;   // 0 f16, 1 bf16
     int* status;
-    int splitk = 1;            // K is cut into `splitk` ranges, partial tiles are atomically added into a zeroed C32
+    int splitk = 1;            // K is cut into `splitk` ranges, partial tiles are added into a zeroed C32
+    int tma_c = 0;             // 1: staged epilogue with TMA stores (aligned outputs, even N); 0: fragment stores (epi_pair)
+    int c32_add = 0;           // tma_c: C32 += tile by TMA reduce-add (split-K, or beta without C16)
 };
 
 constexpr int G2_THREADS = 384;                                 // WG0 producer, WG1 + WG2 consumers
 constexpr int G2_CONSUMER_WARPS = 8;
 // NCTA = 2 (BN = 256 only): a 2-CTA cluster owns a 256 x 256 tile.  Each CTA stages its own 128 rows of A and fetches HALF of
 // B's 256 rows, multicasting it into both CTAs' rings: B is read from L2 once per 256 output rows instead of once per 128.
+constexpr int EPI_SLOT = 64 * 128;                       // one staged 64 x 32 fp32 chunk (a 16-bit chunk uses half)
+constexpr int EPI_BYTES = 2 * 2 * EPI_SLOT;              // two slots per consumer warpgroup
 template <int BN_, int NCTA = 1> struct G2Cfg {
     static constexpr int STAGE_BYTES = (BM + BN_) * 128;
     static constexpr int STAGES = BN_ == 256 ? 4 : 6;
-    static constexpr int SMEM = STAGES * STAGE_BYTES + 256 + 1024;
+    static constexpr int SMEM = STAGES * STAGE_BYTES + EPI_BYTES + 256 + 1024;
 };
 
 // One output pair (columns n, n + 1 of row m) through alpha / bias / activation / beta into C32 and / or C16.
@@ -95,9 +102,89 @@ __device__ __forceinline__ void epi_pair(const GemmParams& p, long long m, int n
     }
 }
 
+// Staged epilogue of one consumer warpgroup's 64 x BN accumulator (rows m_base.., columns n_base..): 64 x 32 chunks into
+// the warpgroup's two shared-memory slots (chunk q in slot q & 1), each written by one TMA store (or reduce-add) issued by
+// the warpgroup's first thread, which therefore owns every bulk group of the warpgroup.  A slot is refilled once the store
+// issued from it two chunks earlier has read it; the first chunk of a tile waits for all of the previous tile's stores to
+// have read shared memory (long done: a whole main loop ran since), and with both C32 and C16 the two slots hold one
+// chunk's two tiles, so each chunk waits for the previous one.  Per element the values are those of epi_pair.
+template <int BN_>
+__device__ __forceinline__ void epi_staged(const GemmParams& p, const CUtensorMap* tmC32, const CUtensorMap* tmC16,
+                                           const float* acc, float alpha, uint32_t stg, int c, int m_base, int n_base) {
+    const int t = threadIdx.x & 127, lane = t & 31;
+    const bool dual = p.C32 && p.C16;
+    const int r0 = (t >> 5) * 16 + (lane >> 2);              // rows r0 and r0 + 8 of the 64-row sub-tile
+    const int sw = lane >> 2;                                // (r0 + 8 h) & 7
+#pragma unroll
+    for (int q = 0; q < BN_ / 32; ++q) {
+        const int nq = n_base + 32 * q;
+        if (nq >= p.N) break;
+        if (t == 0) {
+            if (q == 0 || dual) bulk_wait_read<0>();
+            else bulk_wait_read<1>();
+        }
+        named_bar_sync(1 + c, 128);                          // the slot(s) about to be written have been read
+        const uint32_t s32 = stg + (dual ? 0 : q & 1) * EPI_SLOT;     // shared-memory addresses
+        const uint32_t s16 = stg + (dual ? 1 : q & 1) * EPI_SLOT;
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) {
+            const int j = 4 * q + jj;
+            const int cl = 8 * jj + 2 * (lane & 3);          // column pair within the chunk
+            const int n = nq + cl;
+            const bool nin = n < p.N;                        // N even: n + 1 < N as well
+            float2 b = make_float2(0.f, 0.f);
+            if (nin && p.bias) b = __ldg(reinterpret_cast<const float2*>(p.bias + n));
+            if (nin && p.bias2) { const float2 u2 = __ldg(reinterpret_cast<const float2*>(p.bias2 + n)); b.x += u2.x; b.y += u2.y; }
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int r = r0 + 8 * h;
+                const int m = m_base + r;
+                const bool in = nin && m < p.M;
+                float x0 = fmaf(acc[4 * j + 2 * h], alpha, b.x), x1 = fmaf(acc[4 * j + 2 * h + 1], alpha, b.y);
+                if (p.act == 1) { x0 = tanh_f(x0); x1 = tanh_f(x1); }
+                else if (p.act == 2 && in) {
+                    const float2 y = __half22float2(*reinterpret_cast<const __half2*>(p.aux16 + static_cast<long long>(m) * p.ldaux + n));
+                    x0 *= (1.f - y.x * y.x); x1 *= (1.f - y.y * y.y);
+                }
+                if (p.C32) {
+                    if (p.beta && !p.c32_add && in) {        // beta with a 16-bit output: C16 gets the sum too
+                        const float2 o = *reinterpret_cast<const float2*>(p.C32 + static_cast<long long>(m) * p.ldc32 + n);
+                        x0 += o.x; x1 += o.y;
+                    }
+                    const int u = cl >> 2;                   // SWIZZLE_128B: 16-byte unit u of row r sits at u ^ (r & 7)
+                    st_shared_f2(s32 + r * 128 + ((u ^ sw) << 4) + (cl & 2) * 4, x0, x1);
+                }
+                if (p.C16) {
+                    const int u = cl >> 3;                   // SWIZZLE_64B, 64-byte rows: unit u of row r sits at u ^ ((r >> 1) & 3)
+                    const uint32_t d = s16 + r * 64 + ((u ^ ((r >> 1) & 3)) << 4) + (cl & 6) * 2;
+                    if (p.c16_fmt == 0) {    // fp16: saturate instead of overflowing to inf
+                        const __half2 h2 = __floats2half2_rn(fminf(fmaxf(x0, -65504.f), 65504.f), fminf(fmaxf(x1, -65504.f), 65504.f));
+                        st_shared_b32(d, *reinterpret_cast<const uint32_t*>(&h2));
+                    } else {
+                        const __nv_bfloat162 h2 = __floats2bfloat162_rn(x0, x1);
+                        st_shared_b32(d, *reinterpret_cast<const uint32_t*>(&h2));
+                    }
+                }
+            }
+        }
+        fence_proxy_async_smem();                            // the staged chunk is visible to the TMA unit
+        named_bar_sync(1 + c, 128);
+        if (t == 0) {
+            if (p.C32) {
+                if (p.c32_add) tma_reduce_add_2d(tmC32, s32, nq, m_base);
+                else tma_store_2d(tmC32, s32, nq, m_base);
+            }
+            if (p.C16) tma_store_2d(tmC16, s16, nq, m_base);
+            bulk_commit();
+        }
+    }
+}
+
 template <int FMT, int BN_, int NCTA, int TA, int TB>
 __global__ void __launch_bounds__(G2_THREADS, 1)
-gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmParams p, int tiles_n, int n_tiles) {
+gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+             const __grid_constant__ CUtensorMap tmC32, const __grid_constant__ CUtensorMap tmC16, GemmParams p, int tiles_n,
+             int n_tiles) {
     using C = G2Cfg<BN_, NCTA>;
     constexpr int TM = BM * NCTA;                   // rows of a work item's tile
     const int rank = NCTA == 2 ? static_cast<int>(cluster_ctarank()) : 0;
@@ -106,7 +193,8 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
     constexpr int ST = C::STAGES;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + ST * C::STAGE_BYTES);
+    uint8_t* epi = smem + ST * C::STAGE_BYTES;      // [2 consumer warpgroups][2 slots] staged output chunks
+    uint64_t* bars = reinterpret_cast<uint64_t*>(epi + EPI_BYTES);
     uint64_t* full = bars;                 // [ST]
     uint64_t* empty = bars + ST;           // [ST]: one arrival per consumer warp of every CTA that writes into this stage
 
@@ -121,6 +209,8 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmB);
+        if (p.tma_c && p.C32) tma_prefetch_desc(&tmC32);
+        if (p.tma_c && p.C16) tma_prefetch_desc(&tmC16);
         for (int s = 0; s < ST; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], G2_CONSUMER_WARPS * NCTA); }
         fence_mbar_init();
     }
@@ -214,14 +304,22 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
             wgmma_wait<0>();
             wgmma_fence_acc<BN_ / 2>(acc);
             release((it - 1) % ST);
-            const long long m0 = static_cast<long long>(tile_m) * TM + rank * BM + c * 64 + wq * 16 + (lane >> 2);
-            const int n0 = tile_n * BN_ + 2 * (lane & 3);
+#ifndef FT_GEMM_NO_STORE                            // tools/gemm_shapes.py --mainloop: the main loop alone
+            const int mb = tile_m * TM + rank * BM + c * 64;             // < M, an int
+            if (p.tma_c) {
+                epi_staged<BN_>(p, &tmC32, &tmC16, acc, alpha, smem_u32(epi) + c * (2 * EPI_SLOT), c, mb, tile_n * BN_);
+            } else {
+                const long long m0 = static_cast<long long>(mb) + wq * 16 + (lane >> 2);
+                const int n0 = tile_n * BN_ + 2 * (lane & 3);
 #pragma unroll
-            for (int j = 0; j < BN_ / 8; ++j) {
-                epi_pair(p, m0, n0 + 8 * j, acc[4 * j], acc[4 * j + 1], alpha, vec2);
-                epi_pair(p, m0 + 8, n0 + 8 * j, acc[4 * j + 2], acc[4 * j + 3], alpha, vec2);
+                for (int j = 0; j < BN_ / 8; ++j) {
+                    epi_pair(p, m0, n0 + 8 * j, acc[4 * j], acc[4 * j + 1], alpha, vec2);
+                    epi_pair(p, m0 + 8, n0 + 8 * j, acc[4 * j + 2], acc[4 * j + 3], alpha, vec2);
+                }
             }
+#endif
         }
+        if (p.tma_c && (threadIdx.x & 127) == 0) bulk_wait_all();   // staged chunks stay in shared memory until stored
     }
     if (NCTA == 2) cluster_sync_all();              // no CTA exits while its peer may still arrive on its barriers
 }

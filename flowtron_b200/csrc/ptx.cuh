@@ -153,9 +153,20 @@ __device__ __forceinline__ void tma_load_2d_mc(void* smem_dst, const CUtensorMap
 }
 
 // TMA store of a shared-memory tile (bulk async group of the issuing thread); out-of-range rows / columns are clipped by the map
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* smem_src, int c0, int c1) {
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, uint32_t smem_src, int c0, int c1) {
     asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-                 ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1) : "memory");
+                 ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_src), "r"(c0), "r"(c1) : "memory");
+}
+// TMA reduce-add of a shared-memory tile into global memory (element type from the map: .add.f32 for fp32 outputs)
+__device__ __forceinline__ void tma_reduce_add_2d(const CUtensorMap* m, uint32_t smem_src, int c0, int c1) {
+    asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3}], [%1];"
+                 ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_src), "r"(c0), "r"(c1) : "memory");
+}
+__device__ __forceinline__ void st_shared_f2(uint32_t a, float x, float y) {
+    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(x), "f"(y) : "memory");
+}
+__device__ __forceinline__ void st_shared_b32(uint32_t a, uint32_t v) {
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(v) : "memory");
 }
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 template <int kPending>
@@ -282,6 +293,9 @@ __device__ __forceinline__ void wgmma_k(float* d, uint64_t da, uint64_t db, uint
         else wgmma_f16_n16<TA, TB>(d, da, db, scale_d);
     }
 }
+
+// named barrier `id` (1..15; 0 is __syncthreads) over `n` threads, a multiple of 32
+__device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
 __device__ __forceinline__ void setmaxnreg_dec40() { asm volatile("setmaxnreg.dec.sync.aligned.u32 40;"); }
 __device__ __forceinline__ void setmaxnreg_inc232() { asm volatile("setmaxnreg.inc.sync.aligned.u32 232;"); }

@@ -70,7 +70,7 @@ int ft_debug_lstm_bwd_chunk(int T, int B, int t0, int t1, const float* dh_ext, l
                             const void* gates16, const float* cstate, const int* lens, void* dG16, float* dc_carry, int* flags,
                             float* xchg, void* stream);
 
-/* ft_gemm tile policy: 0 = one CTA per 128 x 256 tile always; 1 (default) = CTA pairs (2-CTA clusters sharing B by TMA multicast, 256 x 256 tiles) for
+/* ft_gemm tile policy: 0 (default) = one CTA per 128 x 256 tile always; 1 = CTA pairs (2-CTA clusters sharing B by TMA multicast, 256 x 256 tiles) for
  * contractions >= 1e11 FLOP; 2 = CTA pairs whenever the output is wide and has >= SMs/2 such tiles. */
 void ft_set_gemm_pair_mode(int mode);
 
