@@ -4,7 +4,8 @@ Functional style: every function takes ``p``, a flat ``{state_dict key: tensor}`
 dict in the reference's checkpoint layout (SURVEY.md §8a row 15), so the same
 weights drive the reference, this oracle and the CUDA path.  Everything is
 ordinary differentiable torch, so ``torch.autograd`` of these functions is the
-gradient oracle as well.
+gradient oracle as well; the flow step keeps its inputs' dtype, so fp64 weights and
+inputs give the fp64 oracle ``tests/test_gpu_ar_step_backward.py`` compares against.
 
 Each function cites the reference lines it restates (paths relative to
 /root/reference).  Pinned against reference-generated fixtures by
@@ -93,6 +94,7 @@ def attention_forward(p: Params, pre: str, queries: Tensor, text: Tensor, mask: 
 
     queries [T,B,H], text [L,B,E], mask [B,L,1] bool (True = pad).
     Returns ctx [B,A,T], attn [B,T,L], attn_logprob [B,T,L] (or None if attn was given).
+    Computes in the inputs' dtype: fp32 or fp64 only (in fp16 the 1e-20 log offset would flush to zero).
     """
     Wq = p[f"{pre}.query.linear_layer.weight"]
     Wk = p[f"{pre}.key.linear_layer.weight"]
@@ -108,13 +110,14 @@ def attention_forward(p: Params, pre: str, queries: Tensor, text: Tensor, mask: 
             e = e.masked_fill(mask.transpose(1, 2), -float("inf"))   # :574-576
         a = torch.softmax(e, dim=2)                              # :577
         if attn_prior is not None:
-            lp = torch.log(a.float() + 1e-20) + torch.log(attn_prior.float() + 1e-20)  # :546-548
+            # :546-548 casts to float32; the inputs' dtype is kept so the same code is the fp64 gradient oracle too
+            lp = torch.log(a + 1e-20) + torch.log(attn_prior.to(a.dtype) + 1e-20)
             attn_logprob = lp.clone()                            # :550 (before masking)
             if mask is not None:
                 lp = lp.masked_fill(mask.transpose(1, 2), -float("inf"))
             a = torch.softmax(lp, dim=2)                         # :556
         else:
-            attn_logprob = torch.log(a.float() + 1e-8)           # :583
+            attn_logprob = torch.log(a + 1e-8)                   # :583 (dtype kept, as above)
     else:
         a = attn
         attn_logprob = None
