@@ -89,6 +89,23 @@ class FtWaveGlowWeights(Structure):
         [(n, c_void_p * WG_MAX_FLOWS) for n in ("start_w", "start_b", "end_w", "end_b", "inv_w")]
 
 
+class FtWaveGlowTrainDesc(Structure):
+    _fields_ = [("n_mel", c_int), ("n_flows", c_int), ("n_group", c_int), ("n_early_every", c_int), ("n_early_size", c_int),
+                ("n_layers", c_int), ("n_channels", c_int), ("kernel_size", c_int), ("B", c_int), ("F", c_int), ("N", c_int)]
+
+
+class FtWaveGlowTrainWeights(Structure):
+    _fields_ = [("up_w", c_void_p), ("up_b", c_void_p)] + \
+        [(n, (c_void_p * WG_MAX_LAYERS) * WG_MAX_FLOWS) for n in ("in_w", "in_b", "rs_w", "rs_b", "in_wT", "rs_wT")] + \
+        [(n, c_void_p * WG_MAX_FLOWS) for n in ("start_w", "start_b", "end_w", "end_b", "conv_w")]
+
+
+class FtWaveGlowTrainGrads(Structure):
+    _fields_ = [("up_w", c_void_p), ("up_b", c_void_p), ("in_w", ((c_void_p * 4) * WG_MAX_LAYERS) * WG_MAX_FLOWS)] + \
+        [(n, (c_void_p * WG_MAX_LAYERS) * WG_MAX_FLOWS) for n in ("in_b", "rs_w", "rs_b")] + \
+        [(n, c_void_p * WG_MAX_FLOWS) for n in ("start_w", "start_b", "end_w", "end_b", "conv_w")]
+
+
 class FlowtronB200Error(RuntimeError):
     pass
 
@@ -218,6 +235,15 @@ def _declare(L):
     L.ft_waveglow_infer.argtypes = [POINTER(FtWaveGlowDesc), POINTER(FtWaveGlowWeights), c_void_p, c_void_p, c_float, c_void_p,
                                     c_void_p, c_void_p]
     L.ft_waveglow_infer.restype = c_int
+    for fn in ("ft_waveglow_train_saved_bytes", "ft_waveglow_train_scratch_bytes"):
+        getattr(L, fn).argtypes = [POINTER(FtWaveGlowTrainDesc)]
+        getattr(L, fn).restype = c_size_t
+    L.ft_waveglow_train_fwd.argtypes = [POINTER(FtWaveGlowTrainDesc), POINTER(FtWaveGlowTrainWeights), c_void_p, c_void_p,
+                                        c_void_p, POINTER(c_void_p), c_void_p, c_void_p, c_void_p]
+    L.ft_waveglow_train_fwd.restype = c_int
+    L.ft_waveglow_train_bwd.argtypes = [POINTER(FtWaveGlowTrainDesc), POINTER(FtWaveGlowTrainWeights), c_void_p,
+                                        POINTER(c_void_p), c_void_p, POINTER(FtWaveGlowTrainGrads), c_void_p, c_void_p]
+    L.ft_waveglow_train_bwd.restype = c_int
     L.ft_posterior_mean.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_float, c_void_p, c_void_p]
     L.ft_posterior_mean.restype = c_int
     L.ft_mas_align_scratch_bytes.argtypes = [c_int, c_int, c_int]
@@ -709,3 +735,35 @@ def waveglow_infer(desc, weights, mel, noise, sigma, audio):
     scratch = scratch_buffer(nbytes, mel.device)
     check(lib().ft_waveglow_infer(byref(desc), byref(weights), ptr(mel), ptr(noise), float(sigma), ptr(audio), ptr(scratch),
                                   stream_ptr()), "ft_waveglow_infer")
+
+
+def _wg_train_bytes(desc):
+    saved = int(lib().ft_waveglow_train_saved_bytes(byref(desc)))
+    scratch = int(lib().ft_waveglow_train_scratch_bytes(byref(desc)))
+    if saved == 0 or scratch == 0:
+        raise FlowtronB200Error(f"ft_waveglow_train rejected the configuration: {lib().ft_last_error().decode()}")
+    return saved, scratch
+
+
+def waveglow_train_saved_bytes(desc) -> int:
+    return _wg_train_bytes(desc)[0]
+
+
+def waveglow_train_fwd(desc, weights, mel, audio, z, log_s_list, saved):
+    """mel f32 [B,80,F], audio f32 [B,N] -> z f32 [B,8,N/8], log_s_list[k] f32 [B,n_half_k,N/8] (written); saved: uint8 of
+    waveglow_train_saved_bytes(desc), kept for waveglow_train_bwd."""
+    _need_cuda(mel, audio, z, saved, *log_s_list)
+    _, nscratch = _wg_train_bytes(desc)
+    scratch = scratch_buffer(nscratch, mel.device)
+    ls = (c_void_p * len(log_s_list))(*[t.data_ptr() for t in log_s_list])
+    check(lib().ft_waveglow_train_fwd(byref(desc), byref(weights), ptr(mel), ptr(audio), ptr(z), ls, ptr(saved), ptr(scratch),
+                                      stream_ptr()), "ft_waveglow_train_fwd")
+
+
+def waveglow_train_bwd(desc, weights, d_z, d_log_s_list, saved, grads):
+    """d_z f32 [B,8,N/8] or None, d_log_s_list[k] f32 [B,n_half_k,N/8] or None -> grads (FtWaveGlowTrainGrads, written)."""
+    _, nscratch = _wg_train_bytes(desc)
+    scratch = scratch_buffer(nscratch, saved.device)
+    dls = (c_void_p * len(d_log_s_list))(*[None if t is None else t.data_ptr() for t in d_log_s_list])
+    check(lib().ft_waveglow_train_bwd(byref(desc), byref(weights), ptr(d_z), dls, ptr(saved), byref(grads), ptr(scratch),
+                                      stream_ptr()), "ft_waveglow_train_bwd")

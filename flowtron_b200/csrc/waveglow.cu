@@ -41,7 +41,7 @@ constexpr int G_LDS = GB_K + 8;                         // smem row pitch (halve
 constexpr int G_STAGE_HALVES = (GB_M + GB_N) * G_LDS;
 constexpr int G_SMEM = G_STAGES * G_STAGE_HALVES * 2;
 
-enum { WG_EPI_UP = 0, WG_EPI_GATE = 1, WG_EPI_RES = 2 };
+enum { WG_EPI_UP = 0, WG_EPI_GATE = 1, WG_EPI_RES = 2, WG_EPI_GATE_BWD = 3 };
 
 struct WgSeg {
     const __half* base;   // row-major [rows, ld]
@@ -61,6 +61,8 @@ struct WgGemmParams {
     float* h32; __half* h16; float* skip32;   // RES ([rows, C] each)
     int res_cols;                             // RES: columns [0, res_cols) update the hidden state, the rest the skip sum
     int skip_store;                           // RES: 1 = skip32 = x (first layer), 0 = skip32 += x
+    __half* pre16;                            // GATE: optional store of the pre-activations [rows, 2C] (training forward);
+                                              // GATE_BWD: the saved pre-activations it reads
 };
 
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, bool pred) {
@@ -86,10 +88,27 @@ __device__ __forceinline__ void wg_epi_pair(const WgGemmParams& p, int m, int n,
     const int info = __ldg(p.rowmap + m);
     if (info < 0) return;                                     // guard / padding rows are never written
     const int row = p.mode == WG_EPI_UP ? info : m;           // UP: a frame row lands on its first group row
+    if (p.mode == WG_EPI_GATE_BWD) {
+        // v0, v1 = d acts of channels n, n+1 -> d pre-activations (interleaved like the forward's columns) and acts
+        const long long o = static_cast<long long>(row) * 2 * WG_C + 2 * n;
+        const uint2 raw = *reinterpret_cast<const uint2*>(p.pre16 + o);
+        const __half2 q0 = *reinterpret_cast<const __half2*>(&raw.x), q1 = *reinterpret_cast<const __half2*>(&raw.y);
+        const float t0 = tanh_f(__low2float(q0)), s0 = sigmoid_f(__high2float(q0));
+        const float t1 = tanh_f(__low2float(q1)), s1 = sigmoid_f(__high2float(q1));
+        const __half2 d0 = __halves2half2(sat_half(v0 * s0 * (1.f - t0 * t0)), sat_half(v0 * t0 * s0 * (1.f - s0)));
+        const __half2 d1 = __halves2half2(sat_half(v1 * s1 * (1.f - t1 * t1)), sat_half(v1 * t1 * s1 * (1.f - s1)));
+        uint2 outv;
+        outv.x = *reinterpret_cast<const uint32_t*>(&d0); outv.y = *reinterpret_cast<const uint32_t*>(&d1);
+        *reinterpret_cast<uint2*>(p.out16 + o) = outv;
+        *reinterpret_cast<__half2*>(p.h16 + static_cast<long long>(row) * WG_C + n) = __halves2half2(sat_half(t0 * s0), sat_half(t1 * s1));
+        return;
+    }
     const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + n));
     const float x0 = v0 + b.x, x1 = v1 + b.y;
     if (p.mode == WG_EPI_GATE) {
         p.out16[static_cast<long long>(row) * p.ld16 + (n >> 1)] = sat_half(tanh_f(x0) * sigmoid_f(x1));
+        if (p.pre16)
+            *reinterpret_cast<__half2*>(p.pre16 + static_cast<long long>(row) * 2 * WG_C + n) = __halves2half2(sat_half(x0), sat_half(x1));
     } else if (p.mode == WG_EPI_UP) {
         *reinterpret_cast<__half2*>(p.out16 + static_cast<long long>(row) * p.ld16 + n) = __halves2half2(sat_half(x0), sat_half(x1));
     } else if (n < p.res_cols) {
@@ -211,7 +230,8 @@ static int launch_wg_gemm(const WgGemmParams& p, cudaStream_t st) {
         attr = true;
     }
     const dim3 grid(p.N / GB_N, (p.M + GB_M - 1) / GB_M);
-    TimeScope ts(p.mode == WG_EPI_UP ? "wg_upsample" : (p.mode == WG_EPI_GATE ? "wg_in_layer" : "wg_res_skip"), p.M, p.N, p.K, st);
+    static const char* const names[] = {"wg_upsample", "wg_in_layer", "wg_res_skip", "wg_gate_bwd"};
+    TimeScope ts(names[p.mode], p.M, p.N, p.K, st);
     wg_gemm_kernel<<<grid, G_THREADS, G_SMEM, st>>>(p);
     ft_count_launch(1);
     return ft_check_launch("wg_gemm_kernel");
@@ -259,7 +279,7 @@ __global__ void wg_prep_kernel(const __grid_constant__ WgBatch bt, const float* 
             if (r >= bt.gbase[0] && r < bt.gbase[bt.B]) {
                 const int b = find_utt(bt.gbase, bt.B, r);
                 const int g = r - bt.gbase[b];
-                if (g < 32 * bt.frames[b]) info = b * bt.Tg_max + g;
+                if (g < 32 * bt.frames[b] && g < bt.Tg_max) info = b * bt.Tg_max + g;   // training: Tg_max = N / 8
             }
             rowinfo[r] = info;
         }
@@ -458,6 +478,494 @@ static int wg_channels(const FtWaveGlowDesc* d, int k) {
     return c;
 }
 
+
+// ------------------------------------------------------------------------------------------------ training
+// WaveGlow.forward (glow.py:196-245, the z direction) with its saved activations, and its backward.  See DESIGN.md §4.21.
+// The forward runs on the same grid, prep, upsample and GATE / RES GEMMs as infer; the GATE epilogue also stores the
+// pre-activations, and each layer's RES epilogue writes the next layer's fp16 input into its own saved slot.
+constexpr float WG_GRAD_TARGET = 64.f;   // per-flow loss scale: S * max|d skip| ~ 64 (headroom 2^10 below fp16's max)
+
+struct WtLayout {
+    WgLayout g;
+    int Tn, N, F, nf, nl;
+    int c[FT_WG_MAX_FLOWS];                // live channels of flow k (its 1x1 conv is c x c)
+    size_t s_mel16, s_uprow, s_rowinfo, s_spect, s_x, s_skip, s_h16, s_pre, saved;
+    size_t c_h32, c_acts, c_state, c_dstate, c_dout, c_dy, c_dskip, c_g16, c_g32, c_dx, c_dsp32, c_dsp16, c_mela, c_zero,
+        c_scale, scratch;
+};
+
+static int wt_layout(const FtWaveGlowTrainDesc* d, WtLayout* L) {
+    if (!d) return ft_set_error("waveglow train: null descriptor");
+    if (d->B < 1 || d->B > WG_MAX_B) return ft_set_error("waveglow train: batch must be 1..128");
+    if (d->F < 1 || d->N < 8 || d->N % 8 || d->N > 256LL * d->F)
+        return ft_set_error("waveglow train: N must be a positive multiple of 8 and at most 256 F");
+    int frames[WG_MAX_B];
+    const int fu = (d->N + 255) / 256;                 // frames whose upsampled samples reach sample N - 1
+    for (int b = 0; b < d->B; ++b) frames[b] = fu;
+    FtWaveGlowDesc gd = {d->n_mel, d->n_flows, d->n_group, d->n_early_every, d->n_early_size, d->n_layers, d->n_channels,
+                         d->kernel_size, d->B, d->F, frames};
+    if (wg_layout(&gd, &L->g)) return -1;
+    L->Tn = d->N / 8; L->N = d->N; L->F = d->F; L->nf = d->n_flows; L->nl = d->n_layers;
+    L->g.Tg_max = L->Tn;
+    L->g.bt.Tg_max = L->Tn;                            // rows g >= N / 8 of an utterance are padding (rowinfo -1)
+    for (int k = 0, c = 8; k < L->nf; ++k) {
+        if (k > 0 && k % d->n_early_every == 0) c -= d->n_early_size;
+        L->c[k] = c;
+    }
+    const size_t R = static_cast<size_t>(L->g.grows), nf = L->nf, nfl = nf * L->nl;
+    size_t off = 0;
+    auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 255) & ~size_t(255); return o; };
+    L->s_mel16 = take(static_cast<size_t>(L->g.mrows) * WG_MEL_LD * 2);
+    L->s_uprow = take(static_cast<size_t>(L->g.mrows) * 4);
+    L->s_rowinfo = take(R * 4);
+    L->s_spect = take(R * WG_SPECT * 2);
+    L->s_x = take(nf * R * 8 * 4);                     // flow inputs (before the 1x1 conv), fp32
+    L->s_skip = take(nf * R * WG_C * 4);               // WN skip sums, fp32
+    L->s_h16 = take(nfl * R * WG_C * 2);               // WN layer inputs, fp16, zero guard rows
+    L->s_pre = take(nfl * R * 2 * WG_C * 2);           // gate pre-activations, fp16, interleaved like in_w's rows
+    L->saved = off;
+    off = 0;
+    L->c_h32 = take(R * WG_C * 4);
+    L->c_acts = take(R * WG_C * 2);
+    L->c_state = take(R * 8 * 4);
+    L->c_dstate = take(R * 8 * 4);
+    L->c_dout = take(R * 8 * 4);
+    L->c_dy = take(R * 8 * 4);
+    L->c_dskip = take(R * WG_C * 2);
+    L->c_g16 = take(R * WG_C * 2);
+    L->c_g32 = take(R * WG_C * 4);
+    L->c_dx = take(R * 2 * WG_C * 2);
+    L->c_dsp32 = take(R * WG_SPECT * 4);
+    L->c_dsp16 = take(R * WG_SPECT * 2);
+    L->c_mela = take(R / 32 * 4 * WG_MEL_LD * 2);
+    L->c_zero = take(2 * WG_C * 4);
+    L->c_scale = take((nf + 1) * 4 * 4);
+    L->scratch = off;
+    return 0;
+}
+
+// One warp per grid row, for the flow boundary of the forward: finish flow `cur` (end conv from the skip sum, affine
+// coupling audio_1 <- exp(log_s) audio_1 + b, log_s store), then start flow `next` (save its input, 1x1 conv over its live
+// positions, start conv into h32 / the fp16 layer-0 input) or, after the last flow, store z.  The head launch loads audio.
+struct WtTailParams {
+    int R, Tn, N;
+    const int* rowinfo;
+    float* state;                   // [R, 8]: positions [0, o) hold early outputs, [o, 8) the c live channels
+    const float* audio;             // head: [B, N]
+    int cur, o, nh;
+    const float* skip32; const float* end_w; const float* end_b;
+    float* log_s;                   // [B, nh, Tn]
+    int next, o_next, nh_next;
+    const float* conv_w;            // [c, c] of flow `next`
+    float* x_save;                  // [R, 8]
+    const float* start_w; const float* start_b;
+    float* h32; __half* h16;
+    float* z;                       // [B, 8, Tn]
+};
+
+__global__ void __launch_bounds__(T_THREADS) wg_train_tail_kernel(const __grid_constant__ WtTailParams p) {
+    __shared__ float s_end[8 * WG_C];
+    __shared__ float s_start[WG_C * 4];
+    __shared__ float s_misc[64 + 8 + WG_C];    // conv_w, end_b, start_b
+    float* s_w = s_misc;
+    float* s_endb = s_misc + 64;
+    float* s_startb = s_misc + 72;
+    const int cn = 8 - p.o_next;
+    if (p.cur >= 0) {
+        for (int i = threadIdx.x; i < 2 * p.nh * WG_C; i += T_THREADS) s_end[i] = p.end_w[i];
+        if (threadIdx.x < 2 * p.nh) s_endb[threadIdx.x] = p.end_b[threadIdx.x];
+    }
+    if (p.next >= 0) {
+        for (int i = threadIdx.x; i < WG_C * p.nh_next; i += T_THREADS) s_start[i] = p.start_w[i];
+        for (int i = threadIdx.x; i < WG_C; i += T_THREADS) s_startb[i] = p.start_b[i];
+        for (int i = threadIdx.x; i < cn * cn; i += T_THREADS) s_w[i] = p.conv_w[i];
+    }
+    __syncthreads();
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    __shared__ float s_x[T_THREADS / 32][8], s_out[T_THREADS / 32][8];
+    float* xs = s_x[warp];
+    float* so = s_out[warp];
+    const int r0 = (blockIdx.x * (T_THREADS / 32) + warp) * T_ROWS_PER_WARP;
+    for (int r = r0; r < r0 + T_ROWS_PER_WARP && r < p.R; ++r) {
+        const int info = __ldg(p.rowinfo + r);
+        if (info < 0) continue;                                   // warp-uniform
+        const int b = info / p.Tn, g = info - b * p.Tn;
+        if (lane < 8) xs[lane] = p.audio ? __ldg(p.audio + static_cast<long long>(b) * p.N + 8 * g + lane)
+                                         : p.state[static_cast<long long>(r) * 8 + lane];
+        if (p.cur >= 0) {
+            const float4* skp = reinterpret_cast<const float4*>(p.skip32 + static_cast<long long>(r) * WG_C + lane * 8);
+            const float4 s0 = skp[0], s1 = skp[1];
+            const float sk[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                if (j < 2 * p.nh) {
+                    float a = 0.f;
+#pragma unroll
+                    for (int e = 0; e < 8; ++e) a = fmaf(s_end[j * WG_C + lane * 8 + e], sk[e], a);
+#pragma unroll
+                    for (int off = 16; off; off >>= 1) a += __shfl_xor_sync(0xffffffffu, a, off);
+                    if (lane == j) so[j] = a + s_endb[j];
+                }
+            }
+            __syncwarp();
+            if (lane < p.nh) {                                    // audio_1 = positions [o + nh, 8)
+                const int pos = p.o + p.nh + lane;
+                const float ls = so[p.nh + lane];
+                xs[pos] = expf(ls) * xs[pos] + so[lane];
+                p.log_s[(static_cast<long long>(b) * p.nh + lane) * p.Tn + g] = ls;
+            }
+        }
+        __syncwarp();
+        if (p.next >= 0) {
+            float v = 0.f;
+            if (lane < 8) {
+                v = xs[lane];
+                p.x_save[static_cast<long long>(r) * 8 + lane] = v;
+                if (lane >= p.o_next) {
+                    v = 0.f;
+                    for (int j = 0; j < cn; ++j) v = fmaf(s_w[(lane - p.o_next) * cn + j], xs[p.o_next + j], v);
+                }
+            }
+            __syncwarp();
+            if (lane < 8) xs[lane] = v;
+            __syncwarp();
+            float h[8];
+#pragma unroll
+            for (int e = 0; e < 8; ++e) {
+                const int ch = lane * 8 + e;
+                float a = s_startb[ch];
+#pragma unroll
+                for (int i = 0; i < 4; ++i)
+                    if (i < p.nh_next) a = fmaf(s_start[ch * p.nh_next + i], xs[p.o_next + i], a);
+                h[e] = a;
+            }
+            const long long o = static_cast<long long>(r) * WG_C + lane * 8;
+            float4* hp = reinterpret_cast<float4*>(p.h32 + o);
+            hp[0] = make_float4(h[0], h[1], h[2], h[3]);
+            hp[1] = make_float4(h[4], h[5], h[6], h[7]);
+            const __half2 q0 = __halves2half2(sat_half(h[0]), sat_half(h[1])), q1 = __halves2half2(sat_half(h[2]), sat_half(h[3]));
+            const __half2 q2 = __halves2half2(sat_half(h[4]), sat_half(h[5])), q3 = __halves2half2(sat_half(h[6]), sat_half(h[7]));
+            uint4 pk;
+            pk.x = *reinterpret_cast<const uint32_t*>(&q0); pk.y = *reinterpret_cast<const uint32_t*>(&q1);
+            pk.z = *reinterpret_cast<const uint32_t*>(&q2); pk.w = *reinterpret_cast<const uint32_t*>(&q3);
+            *reinterpret_cast<uint4*>(p.h16 + o) = pk;
+            if (lane < 8) p.state[static_cast<long long>(r) * 8 + lane] = xs[lane];
+        } else if (lane < 8) {
+            p.z[(static_cast<long long>(b) * 8 + lane) * p.Tn + g] = xs[lane];
+        }
+        __syncwarp();
+    }
+}
+
+static int launch_wt_tail(const WtTailParams& p, cudaStream_t st) {
+    const int rows_per_block = (T_THREADS / 32) * T_ROWS_PER_WARP;
+    TimeScope ts("wg_train_tail", p.R, p.cur, p.next, st);
+    wg_train_tail_kernel<<<(p.R + rows_per_block - 1) / rows_per_block, T_THREADS, 0, st>>>(p);
+    ft_count_launch(1);
+    return ft_check_launch("wg_train_tail_kernel");
+}
+
+// Backward of one flow's boundary, in three grid-stride launches (one warp per row, per-block partial sums of the small
+// weight gradients, then one atomicAdd per entry and block):
+//   out   d_out = (d b, d log_s) from the incoming d audio_1 and d_log_s; d audio_1 before the coupling into dy; d end_w /
+//         d end_b; max |d skip| for the flow's loss scale
+//   skip  S from that maximum; d skip = end_w^T d_out * S (fp16, the WN backward's operand); G32 = 0
+//   in    d a0 = start_w^T G / S + the pass-through gradient; d x = W^T dy into dstate; d start_w / d start_b / d W
+struct WtBwdParams {
+    int R, Tn;
+    const int* rowinfo;
+    int o, nh;
+    const float* x_save; const float* conv_w; const float* skip32; const float* end_w; const float* end_b;
+    const float* start_w;
+    const float* dz;                // d_z [B, 8, Tn] (last flow only; NULL = zero): dstate starts from it
+    const float* dlog_s;            // [B, nh, Tn] or NULL
+    float* dstate; float* dout; float* dy;
+    float* scale;                   // [S, 1/S, max |d skip| bits]
+    __half* dskip16; float* g32;
+    float* g_end_w; float* g_end_b; float* g_start_w; float* g_start_b; float* g_conv_w;
+};
+
+constexpr int WT_BLOCKS = 264;
+
+__device__ __forceinline__ float wt_scale(const float* scale) {
+    const float m = __uint_as_float(reinterpret_cast<const unsigned int*>(scale)[2]);
+    if (!(m > 0.f) || !isfinite(m)) return 1.f;
+    int e = static_cast<int>(floorf(log2f(WG_GRAD_TARGET / m)));
+    e = e < -60 ? -60 : (e > 60 ? 60 : e);
+    return exp2f(static_cast<float>(e));
+}
+
+__device__ __forceinline__ void wt_flush(float* red, int n, float* out) {
+    __syncthreads();
+    for (int i = threadIdx.x; i < n; i += T_THREADS) atomicAdd(out + i, red[i]);
+}
+
+__global__ void __launch_bounds__(T_THREADS) wg_train_bwd_out_kernel(const __grid_constant__ WtBwdParams p) {
+    __shared__ float s_end[8 * WG_C];
+    __shared__ float s_red[8 * WG_C + 8];
+    __shared__ float s_w[64], s_endb[8];
+    __shared__ float s_x[T_THREADS / 32][8], s_d[T_THREADS / 32][8];
+    const int c = 8 - p.o, nh = p.nh;
+    for (int i = threadIdx.x; i < 2 * nh * WG_C; i += T_THREADS) s_end[i] = p.end_w[i];
+    for (int i = threadIdx.x; i < 8 * WG_C + 8; i += T_THREADS) s_red[i] = 0.f;
+    if (threadIdx.x < c * c) s_w[threadIdx.x] = p.conv_w[threadIdx.x];
+    if (threadIdx.x < 2 * nh) s_endb[threadIdx.x] = p.end_b[threadIdx.x];
+    __syncthreads();
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    float* xs = s_x[warp];
+    float* ds = s_d[warp];
+    float acc[8][8], accb[8], mx = 0.f;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        accb[j] = 0.f;
+#pragma unroll
+        for (int e = 0; e < 8; ++e) acc[j][e] = 0.f;
+    }
+    const int nw = gridDim.x * (T_THREADS / 32);
+    for (int r = blockIdx.x * (T_THREADS / 32) + warp; r < p.R; r += nw) {
+        const int info = __ldg(p.rowinfo + r);
+        if (info < 0) continue;
+        const int b = info / p.Tn, g = info - b * p.Tn;
+        if (lane < 8) {
+            xs[lane] = p.x_save[static_cast<long long>(r) * 8 + lane];
+            ds[lane] = p.dz ? __ldg(p.dz + (static_cast<long long>(b) * 8 + lane) * p.Tn + g)
+                            : p.dstate[static_cast<long long>(r) * 8 + lane];
+        }
+        __syncwarp();
+        if (p.dz && lane < 8) p.dstate[static_cast<long long>(r) * 8 + lane] = ds[lane];
+        const float4* skp = reinterpret_cast<const float4*>(p.skip32 + static_cast<long long>(r) * WG_C + lane * 8);
+        const float4 s0 = skp[0], s1 = skp[1];
+        const float sk[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
+        float d[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            if (i < nh) {
+                float a = 0.f;                                    // log_s_i, recomputed exactly as the forward did
+#pragma unroll
+                for (int e = 0; e < 8; ++e) a = fmaf(s_end[(nh + i) * WG_C + lane * 8 + e], sk[e], a);
+#pragma unroll
+                for (int off = 16; off; off >>= 1) a += __shfl_xor_sync(0xffffffffu, a, off);
+                const float ls = a + s_endb[nh + i];
+                float a1 = 0.f;                                   // audio_1 before the coupling: (W x)[nh + i]
+                for (int j = 0; j < c; ++j) a1 = fmaf(s_w[(nh + i) * c + j], xs[p.o + j], a1);
+                const float dap = ds[p.o + nh + i], ex = expf(ls);
+                const float dls = p.dlog_s ? __ldg(p.dlog_s + (static_cast<long long>(b) * nh + i) * p.Tn + g) : 0.f;
+                d[i] = dap;
+                d[nh + i] = dap * ex * a1 + dls;
+                if (lane == 0) p.dy[static_cast<long long>(r) * 8 + nh + i] = ex * dap;
+            }
+        }
+        if (lane < 2 * nh) {
+            float v = 0.f;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) if (j == lane) v = d[j];
+            p.dout[static_cast<long long>(r) * 8 + lane] = v;
+        }
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+            float dsk = 0.f;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                if (j < 2 * nh) {
+                    acc[j][e] = fmaf(d[j], sk[e], acc[j][e]);
+                    dsk = fmaf(s_end[j * WG_C + lane * 8 + e], d[j], dsk);
+                }
+            }
+            mx = fmaxf(mx, fabsf(dsk));
+        }
+#pragma unroll
+        for (int j = 0; j < 8; ++j) if (j < 2 * nh) accb[j] += d[j];
+        __syncwarp();
+    }
+#pragma unroll
+    for (int off = 16; off; off >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, off));
+    if (lane == 0) atomicMax(reinterpret_cast<unsigned int*>(p.scale) + 2, __float_as_uint(mx));
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        if (j < 2 * nh) {
+#pragma unroll
+            for (int e = 0; e < 8; ++e) atomicAdd(&s_red[j * WG_C + lane * 8 + e], acc[j][e]);
+            if (lane == 0) atomicAdd(&s_red[8 * WG_C + j], accb[j]);
+        }
+    }
+    wt_flush(s_red, 2 * nh * WG_C, p.g_end_w);
+    if (threadIdx.x < 2 * nh) atomicAdd(p.g_end_b + threadIdx.x, s_red[8 * WG_C + threadIdx.x]);
+}
+
+__global__ void __launch_bounds__(T_THREADS) wg_train_bwd_skip_kernel(const __grid_constant__ WtBwdParams p) {
+    __shared__ float s_end[8 * WG_C];
+    const int nh = p.nh;
+    for (int i = threadIdx.x; i < 2 * nh * WG_C; i += T_THREADS) s_end[i] = p.end_w[i];
+    __syncthreads();
+    const float S = wt_scale(p.scale);
+    if (blockIdx.x == 0 && threadIdx.x == 0) { p.scale[0] = S; p.scale[1] = 1.f / S; }
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int nw = gridDim.x * (T_THREADS / 32);
+    for (int r = blockIdx.x * (T_THREADS / 32) + warp; r < p.R; r += nw) {
+        if (__ldg(p.rowinfo + r) < 0) continue;
+        float d[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) d[j] = j < 2 * nh ? p.dout[static_cast<long long>(r) * 8 + j] : 0.f;
+        float v[8];
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+            float a = 0.f;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) if (j < 2 * nh) a = fmaf(s_end[j * WG_C + lane * 8 + e], d[j], a);
+            v[e] = a * S;
+        }
+        const long long o = static_cast<long long>(r) * WG_C + lane * 8;
+        const __half2 q0 = __halves2half2(sat_half(v[0]), sat_half(v[1])), q1 = __halves2half2(sat_half(v[2]), sat_half(v[3]));
+        const __half2 q2 = __halves2half2(sat_half(v[4]), sat_half(v[5])), q3 = __halves2half2(sat_half(v[6]), sat_half(v[7]));
+        uint4 pk;
+        pk.x = *reinterpret_cast<const uint32_t*>(&q0); pk.y = *reinterpret_cast<const uint32_t*>(&q1);
+        pk.z = *reinterpret_cast<const uint32_t*>(&q2); pk.w = *reinterpret_cast<const uint32_t*>(&q3);
+        *reinterpret_cast<uint4*>(p.dskip16 + o) = pk;
+        float4* gp = reinterpret_cast<float4*>(p.g32 + o);
+        gp[0] = make_float4(0.f, 0.f, 0.f, 0.f);
+        gp[1] = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+}
+
+__global__ void __launch_bounds__(T_THREADS) wg_train_bwd_in_kernel(const __grid_constant__ WtBwdParams p) {
+    __shared__ float s_start[WG_C * 4];
+    __shared__ float s_red[WG_C * 4 + WG_C + 64];
+    __shared__ float s_w[64];
+    __shared__ float s_x[T_THREADS / 32][8], s_y[T_THREADS / 32][8], s_dy[T_THREADS / 32][8];
+    const int c = 8 - p.o, nh = p.nh;
+    for (int i = threadIdx.x; i < WG_C * nh; i += T_THREADS) s_start[i] = p.start_w[i];
+    for (int i = threadIdx.x; i < WG_C * 5 + 64; i += T_THREADS) s_red[i] = 0.f;
+    if (threadIdx.x < c * c) s_w[threadIdx.x] = p.conv_w[threadIdx.x];
+    __syncthreads();
+    const float iS = p.scale[1];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    float* xs = s_x[warp];
+    float* ys = s_y[warp];
+    float* dys = s_dy[warp];
+    float acc[8][4], accb[8], accw[2] = {0.f, 0.f};
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+        accb[e] = 0.f;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) acc[e][i] = 0.f;
+    }
+    const int nw = gridDim.x * (T_THREADS / 32);
+    for (int r = blockIdx.x * (T_THREADS / 32) + warp; r < p.R; r += nw) {
+        if (__ldg(p.rowinfo + r) < 0) continue;
+        const long long r8 = static_cast<long long>(r) * 8;
+        if (lane < 8) xs[lane] = p.x_save[r8 + lane];
+        __syncwarp();
+        if (lane < c) {
+            float a = 0.f;
+            for (int j = 0; j < c; ++j) a = fmaf(s_w[lane * c + j], xs[p.o + j], a);
+            ys[lane] = a;                                         // y = W x over the live positions (relative index)
+        }
+        const float4* gp = reinterpret_cast<const float4*>(p.g32 + static_cast<long long>(r) * WG_C + lane * 8);
+        const float4 g0 = gp[0], g1 = gp[1];
+        float gv[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
+#pragma unroll
+        for (int e = 0; e < 8; ++e) gv[e] *= iS;
+        __syncwarp();
+        float da0[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            da0[i] = 0.f;
+            if (i < nh) {
+                float a = 0.f;
+#pragma unroll
+                for (int e = 0; e < 8; ++e) {
+                    a = fmaf(s_start[(lane * 8 + e) * nh + i], gv[e], a);
+                    acc[e][i] = fmaf(gv[e], ys[i], acc[e][i]);
+                }
+#pragma unroll
+                for (int off = 16; off; off >>= 1) a += __shfl_xor_sync(0xffffffffu, a, off);
+                da0[i] = a;
+            }
+        }
+#pragma unroll
+        for (int e = 0; e < 8; ++e) accb[e] += gv[e];
+        if (lane < c) {
+            float v;
+            if (lane < nh) {
+                v = p.dstate[r8 + p.o + lane];                     // audio_0 passes through the coupling unchanged
+#pragma unroll
+                for (int i = 0; i < 4; ++i) if (i == lane) v += da0[i];
+            } else {
+                v = p.dy[r8 + lane];
+            }
+            dys[lane] = v;
+        }
+        __syncwarp();
+#pragma unroll
+        for (int q = 0; q < 2; ++q) {                             // d W[i][j] += dy_i x_j, entry i * c + j = lane + 32 q
+            const int ij = lane + 32 * q;
+            if (ij < c * c) accw[q] = fmaf(dys[ij / c], xs[p.o + ij % c], accw[q]);
+        }
+        if (lane < c) {
+            float a = 0.f;
+            for (int i = 0; i < c; ++i) a = fmaf(s_w[i * c + lane], dys[i], a);
+            p.dstate[r8 + p.o + lane] = a;
+        }
+        __syncwarp();
+    }
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) if (i < nh) atomicAdd(&s_red[(lane * 8 + e) * nh + i], acc[e][i]);
+        atomicAdd(&s_red[4 * WG_C + lane * 8 + e], accb[e]);
+    }
+#pragma unroll
+    for (int q = 0; q < 2; ++q) if (lane + 32 * q < c * c) atomicAdd(&s_red[5 * WG_C + lane + 32 * q], accw[q]);
+    wt_flush(s_red, WG_C * nh, p.g_start_w);
+    for (int i = threadIdx.x; i < WG_C; i += T_THREADS) atomicAdd(p.g_start_b + i, s_red[4 * WG_C + i]);
+    if (threadIdx.x < c * c) atomicAdd(p.g_conv_w + threadIdx.x, s_red[5 * WG_C + threadIdx.x]);
+}
+
+// d spect (fp32, accumulated over every flow and layer) -> fp16 * S for the upsample's weight gradient
+__global__ void wg_scale_cast_kernel(const float* __restrict__ src, long long n, const float* __restrict__ scale2,
+                                     __half* __restrict__ dst) {
+    const float S = scale2[0];
+    for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n;
+         i += static_cast<long long>(gridDim.x) * blockDim.x)
+        dst[i] = sat_half(src[i] * S);
+}
+
+// The upsample GEMM's A operand, one row per 32 grid rows (one mel frame): mela[fr] = mel frames f, f-1, f-2, f-3 of the
+// utterance whose frame f starts at grid row 32 fr, zero rows between utterances; d up_w = d spect^T mela over frames.
+__global__ void wg_mela_kernel(const __grid_constant__ WgBatch bt, const int* __restrict__ rowinfo, const __half* __restrict__ mel16,
+                               int n_fr, __half* __restrict__ mela) {
+    const long long n = static_cast<long long>(n_fr) * 4 * WG_MEL_LD;
+    for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n;
+         i += static_cast<long long>(gridDim.x) * blockDim.x) {
+        const int fr = static_cast<int>(i / (4 * WG_MEL_LD)), col = static_cast<int>(i % (4 * WG_MEL_LD));
+        const int info = __ldg(rowinfo + 32 * fr);
+        __half v = __float2half_rn(0.f);
+        if (info >= 0) {
+            const int b = info / bt.Tg_max, f = (info - b * bt.Tg_max) / 32, j = col / WG_MEL_LD;
+            v = mel16[static_cast<long long>(bt.mbase[b] + 3 + f - j) * WG_MEL_LD + col % WG_MEL_LD];
+        }
+        mela[i] = v;
+    }
+}
+
+static int wt_gemm_wgrad(cudaStream_t st, int N, int K, long long R, const __half* dY, long long lddy, const __half* X, long long ldx,
+                         float* dW, const float* inv_scale) {
+    GemmArgs g;
+    g.M = N; g.N = K; g.K = static_cast<int>(R);
+    g.A = dY; g.lda = lddy; g.a_fmt = FMT_F16; g.a_mn = 1; g.B = X; g.ldb = ldx; g.b_fmt = FMT_F16; g.b_mn = 1;
+    g.alpha_ptr = inv_scale;
+    g.C32 = dW; g.ldc32 = K;
+    return launch_gemm(g, st);
+}
+
+static int wt_launch(const void* fn, const WtBwdParams& p, cudaStream_t st, const char* name) {
+    TimeScope ts(name, p.R, p.nh, 0, st);
+    void* args[] = {const_cast<WtBwdParams*>(&p)};
+    if (cudaLaunchKernel(fn, dim3(WT_BLOCKS), dim3(T_THREADS), args, 0, st) != cudaSuccess) return ft_set_error(name);
+    ft_count_launch(1);
+    return ft_check_launch(name);
+}
+
 }  // namespace ft
 
 extern "C" {
@@ -556,6 +1064,231 @@ int ft_waveglow_infer(const FtWaveGlowDesc* d, const FtWaveGlowWeights* w, const
         }
         if (launch_wg_tail(t, st)) return -1;
     }
+    return 0;
+}
+
+size_t ft_waveglow_train_saved_bytes(const FtWaveGlowTrainDesc* d) {
+    ft::WtLayout L;
+    return ft::wt_layout(d, &L) ? 0 : L.saved;
+}
+
+size_t ft_waveglow_train_scratch_bytes(const FtWaveGlowTrainDesc* d) {
+    ft::WtLayout L;
+    return ft::wt_layout(d, &L) ? 0 : L.scratch;
+}
+
+int ft_waveglow_train_fwd(const FtWaveGlowTrainDesc* d, const FtWaveGlowTrainWeights* w, const float* mel, const float* audio,
+                          float* z, float* const* log_s, void* saved, void* scratch, void* stream) {
+    using namespace ft;
+    WtLayout L;
+    if (wt_layout(d, &L)) return -1;
+    if (!w || !mel || !audio || !z || !log_s || !saved || !scratch) return ft_set_error("waveglow train: null pointer argument");
+    for (int k = 0; k < L.nf; ++k) if (!log_s[k]) return ft_set_error("waveglow train: null log_s pointer");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    uint8_t* sv = static_cast<uint8_t*>(saved);
+    uint8_t* sc = static_cast<uint8_t*>(scratch);
+    const long long R = L.g.grows;
+    __half* mel16 = reinterpret_cast<__half*>(sv + L.s_mel16);
+    int* uprow = reinterpret_cast<int*>(sv + L.s_uprow);
+    int* rowinfo = reinterpret_cast<int*>(sv + L.s_rowinfo);
+    __half* spect = reinterpret_cast<__half*>(sv + L.s_spect);
+    float* xsave = reinterpret_cast<float*>(sv + L.s_x);
+    float* skip = reinterpret_cast<float*>(sv + L.s_skip);
+    __half* h16 = reinterpret_cast<__half*>(sv + L.s_h16);
+    __half* pre = reinterpret_cast<__half*>(sv + L.s_pre);
+    float* h32 = reinterpret_cast<float*>(sc + L.c_h32);
+    __half* acts = reinterpret_cast<__half*>(sc + L.c_acts);
+    float* state = reinterpret_cast<float*>(sc + L.c_state);
+    auto H16 = [&](int k, int i) { return h16 + (static_cast<long long>(k) * L.nl + i) * R * WG_C; };
+    auto PRE = [&](int k, int i) { return pre + (static_cast<long long>(k) * L.nl + i) * R * 2 * WG_C; };
+
+    // guard and padding rows of every layer input and of the upsampled spectrogram are zero: the dilated taps and the
+    // row-reduced weight gradients read them
+    if (cudaMemsetAsync(h16, 0, static_cast<size_t>(L.nf) * L.nl * R * WG_C * 2, st) != cudaSuccess ||
+        cudaMemsetAsync(spect, 0, static_cast<size_t>(R) * WG_SPECT * 2, st) != cudaSuccess)
+        return ft_set_error("waveglow train: memset failed");
+    {
+        const long long work = static_cast<long long>(L.g.mrows) * (WG_MEL_LD + 1) + R;
+        const int grid = static_cast<int>(std::min<long long>((work + 255) / 256, 4096));
+        TimeScope ts("wg_prep", L.g.mrows, R, 0, st);
+        wg_prep_kernel<<<grid, 256, 0, st>>>(L.g.bt, mel, L.F, mel16, uprow, rowinfo, static_cast<int>(R));
+        ft_count_launch(1);
+        if (ft_check_launch("wg_prep_kernel")) return -1;
+    }
+    {
+        WgGemmParams p = {};
+        p.M = L.g.mrows; p.N = WG_UP_N; p.K = 4 * WG_MEL_LD; p.nseg = 4;
+        for (int j = 0; j < 4; ++j) p.seg[j] = WgSeg{mel16, L.g.mrows, WG_MEL_LD, -j, WG_MEL_LD};
+        p.W = static_cast<const __half*>(w->up_w); p.bias = w->up_b; p.rowmap = uprow; p.mode = WG_EPI_UP;
+        p.out16 = spect; p.ld16 = WG_SPECT;
+        if (launch_wg_gemm(p, st)) return -1;
+    }
+    WtTailParams t = {};
+    t.R = static_cast<int>(R); t.Tn = L.Tn; t.N = L.N; t.rowinfo = rowinfo; t.state = state; t.h32 = h32;
+    t.audio = audio; t.cur = -1;
+    for (int k = 0; k <= L.nf; ++k) {
+        if (k < L.nf) {
+            t.next = k; t.o_next = 8 - L.c[k]; t.nh_next = L.c[k] / 2;
+            t.conv_w = w->conv_w[k]; t.x_save = xsave + static_cast<long long>(k) * R * 8;
+            t.start_w = w->start_w[k]; t.start_b = w->start_b[k]; t.h16 = H16(k, 0);
+        } else {
+            t.next = -1; t.z = z;
+        }
+        if (launch_wt_tail(t, st)) return -1;
+        if (k == L.nf) break;
+        float* skip_k = skip + static_cast<long long>(k) * R * WG_C;
+        for (int i = 0; i < L.nl; ++i) {
+            const int dil = 1 << i;
+            __half* hin = H16(k, i);
+            WgGemmParams p = {};
+            p.M = static_cast<int>(R); p.N = 2 * WG_C; p.K = 3 * WG_C + WG_SPECT; p.nseg = 4;
+            p.seg[0] = WgSeg{hin, R, WG_C, -dil, WG_C};
+            p.seg[1] = WgSeg{hin, R, WG_C, 0, WG_C};
+            p.seg[2] = WgSeg{hin, R, WG_C, dil, WG_C};
+            p.seg[3] = WgSeg{spect, R, WG_SPECT, 0, WG_SPECT};
+            p.W = static_cast<const __half*>(w->in_w[k][i]); p.bias = w->in_b[k][i]; p.rowmap = rowinfo; p.mode = WG_EPI_GATE;
+            p.out16 = acts; p.ld16 = WG_C; p.pre16 = PRE(k, i);
+            if (launch_wg_gemm(p, st)) return -1;
+            WgGemmParams q = {};
+            const bool last = i == L.nl - 1;
+            q.M = static_cast<int>(R); q.N = last ? WG_C : 2 * WG_C; q.K = WG_C; q.nseg = 1;
+            q.seg[0] = WgSeg{acts, R, WG_C, 0, WG_C};
+            q.W = static_cast<const __half*>(w->rs_w[k][i]); q.bias = w->rs_b[k][i]; q.rowmap = rowinfo; q.mode = WG_EPI_RES;
+            q.h32 = h32; q.h16 = last ? hin : H16(k, i + 1); q.skip32 = skip_k; q.res_cols = last ? 0 : WG_C; q.skip_store = i == 0;
+            if (launch_wg_gemm(q, st)) return -1;
+        }
+        t.audio = nullptr;
+        t.cur = k; t.o = 8 - L.c[k]; t.nh = L.c[k] / 2;
+        t.skip32 = skip_k; t.end_w = w->end_w[k]; t.end_b = w->end_b[k]; t.log_s = log_s[k];
+    }
+    return 0;
+}
+
+int ft_waveglow_train_bwd(const FtWaveGlowTrainDesc* d, const FtWaveGlowTrainWeights* w, const float* d_z,
+                          const float* const* d_log_s, const void* saved, const FtWaveGlowTrainGrads* gr, void* scratch,
+                          void* stream) {
+    using namespace ft;
+    WtLayout L;
+    if (wt_layout(d, &L)) return -1;
+    if (!w || !saved || !gr || !scratch) return ft_set_error("waveglow train: null pointer argument");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const uint8_t* sv = static_cast<const uint8_t*>(saved);
+    uint8_t* sc = static_cast<uint8_t*>(scratch);
+    const long long R = L.g.grows, C = WG_C;
+    const __half* mel16 = reinterpret_cast<const __half*>(sv + L.s_mel16);
+    const int* rowinfo = reinterpret_cast<const int*>(sv + L.s_rowinfo);
+    const __half* spect = reinterpret_cast<const __half*>(sv + L.s_spect);
+    const float* xsave = reinterpret_cast<const float*>(sv + L.s_x);
+    const float* skip = reinterpret_cast<const float*>(sv + L.s_skip);
+    const __half* h16 = reinterpret_cast<const __half*>(sv + L.s_h16);
+    const __half* pre = reinterpret_cast<const __half*>(sv + L.s_pre);
+    __half* acts = reinterpret_cast<__half*>(sc + L.c_acts);
+    float* dstate = reinterpret_cast<float*>(sc + L.c_dstate);
+    float* dout = reinterpret_cast<float*>(sc + L.c_dout);
+    float* dy = reinterpret_cast<float*>(sc + L.c_dy);
+    __half* dskip = reinterpret_cast<__half*>(sc + L.c_dskip);
+    __half* g16 = reinterpret_cast<__half*>(sc + L.c_g16);
+    float* g32 = reinterpret_cast<float*>(sc + L.c_g32);
+    __half* dx = reinterpret_cast<__half*>(sc + L.c_dx);
+    float* dsp32 = reinterpret_cast<float*>(sc + L.c_dsp32);
+    __half* dsp16 = reinterpret_cast<__half*>(sc + L.c_dsp16);
+    __half* mela = reinterpret_cast<__half*>(sc + L.c_mela);
+    float* zero = reinterpret_cast<float*>(sc + L.c_zero);
+    float* scale = reinterpret_cast<float*>(sc + L.c_scale);
+    const long long W0 = WG_GUARD, RW = R - 2 * WG_GUARD;   // row window of the shifted-tap weight gradients
+
+    auto z0 = [&](void* p, size_t n) { return cudaMemsetAsync(p, 0, n, st) == cudaSuccess ? 0 : ft_set_error("waveglow train: memset failed"); };
+    // rows no kernel writes (guards, padding) stay zero in every fp16 gradient operand: the shifted taps and the
+    // row-reduced weight gradients and column sums read them
+    if (z0(acts, R * C * 2) || z0(dskip, R * C * 2) || z0(g16, R * C * 2) || z0(dx, R * 2 * C * 2) ||
+        z0(dsp32, R * WG_SPECT * 4) || z0(zero, 2 * C * 4) || z0(scale, (L.nf + 1) * 16))
+        return -1;
+    for (int k = 0; k < L.nf; ++k) {
+        const int c = L.c[k], nh = c / 2;
+        if (z0(gr->end_w[k], 2 * nh * C * 4) || z0(gr->end_b[k], 2 * nh * 4) || z0(gr->start_w[k], C * nh * 4) ||
+            z0(gr->start_b[k], C * 4) || z0(gr->conv_w[k], c * c * 4))
+            return -1;
+    }
+    for (int k = L.nf - 1; k >= 0; --k) {
+        const int c = L.c[k], nh = c / 2;
+        WtBwdParams b = {};
+        b.R = static_cast<int>(R); b.Tn = L.Tn; b.rowinfo = rowinfo; b.o = 8 - c; b.nh = nh;
+        b.x_save = xsave + static_cast<long long>(k) * R * 8; b.conv_w = w->conv_w[k];
+        b.skip32 = skip + static_cast<long long>(k) * R * C; b.end_w = w->end_w[k]; b.end_b = w->end_b[k]; b.start_w = w->start_w[k];
+        b.dz = k == L.nf - 1 ? d_z : nullptr;
+        b.dlog_s = d_log_s ? d_log_s[k] : nullptr;
+        b.dstate = dstate; b.dout = dout; b.dy = dy; b.scale = scale + 4 * k; b.dskip16 = dskip; b.g32 = g32;
+        b.g_end_w = gr->end_w[k]; b.g_end_b = gr->end_b[k]; b.g_start_w = gr->start_w[k]; b.g_start_b = gr->start_b[k];
+        b.g_conv_w = gr->conv_w[k];
+        if (k == L.nf - 1 && !d_z && z0(dstate, R * 8 * 4)) return -1;
+        if (wt_launch(reinterpret_cast<const void*>(wg_train_bwd_out_kernel), b, st, "wg_train_bwd_out")) return -1;
+        if (wt_launch(reinterpret_cast<const void*>(wg_train_bwd_skip_kernel), b, st, "wg_train_bwd_skip")) return -1;
+        const float* iS = scale + 4 * k + 1;
+        for (int i = L.nl - 1; i >= 0; --i) {
+            const int dil = 1 << i;
+            const bool last = i == L.nl - 1;
+            const __half* hin = h16 + (static_cast<long long>(k) * L.nl + i) * R * C;
+            // d acts = rs_w^T [G; d skip] -> d pre-activations (dx) and the recomputed acts
+            WgGemmParams p = {};
+            p.M = static_cast<int>(R); p.N = WG_C; p.nseg = last ? 1 : 2; p.K = p.nseg * WG_C;
+            if (last) {
+                p.seg[0] = WgSeg{dskip, R, WG_C, 0, WG_C};
+            } else {
+                p.seg[0] = WgSeg{g16, R, WG_C, 0, WG_C};
+                p.seg[1] = WgSeg{dskip, R, WG_C, 0, WG_C};
+            }
+            p.W = static_cast<const __half*>(w->rs_wT[k][i]); p.rowmap = rowinfo; p.mode = WG_EPI_GATE_BWD;
+            p.out16 = dx; p.ld16 = 2 * WG_C; p.h16 = acts; p.pre16 = const_cast<__half*>(pre + (static_cast<long long>(k) * L.nl + i) * R * 2 * C);
+            if (launch_wg_gemm(p, st)) return -1;
+            // res_skip_layer: rows [0, C) meet G (the residual), the rest d skip
+            float* grs = gr->rs_w[k][i];
+            if (!last) {
+                if (wt_gemm_wgrad(st, WG_C, WG_C, R, g16, C, acts, C, grs, iS)) return -1;
+                if (launch_colsum(g16, 0, C, R, WG_C, gr->rs_b[k][i], iS, st)) return -1;
+            }
+            const long long so = last ? 0 : C;
+            if (wt_gemm_wgrad(st, WG_C, WG_C, R, dskip, C, acts, C, grs + so * C, iS)) return -1;
+            if (launch_colsum(dskip, 0, C, R, WG_C, gr->rs_b[k][i] + so, iS, st)) return -1;
+            // in_layer taps (h shifted by -d, 0, +d) and the cond_layer slice
+            for (int tap = 0; tap < 3; ++tap)
+                if (wt_gemm_wgrad(st, 2 * WG_C, WG_C, RW, dx + W0 * 2 * C, 2 * C, hin + (W0 + (tap - 1) * dil) * C, C,
+                                  gr->in_w[k][i][tap], iS))
+                    return -1;
+            if (wt_gemm_wgrad(st, 2 * WG_C, WG_SPECT, R, dx, 2 * C, spect, WG_SPECT, gr->in_w[k][i][3], iS)) return -1;
+            if (launch_colsum(dx, 0, 2 * C, R, 2 * WG_C, gr->in_b[k][i], iS, st)) return -1;
+            // d spect += dx cond_w (fp32, unscaled on the way out)
+            {
+                GemmArgs g;
+                g.M = static_cast<int>(R); g.N = WG_SPECT; g.K = 2 * WG_C;
+                g.A = dx; g.lda = 2 * C; g.a_fmt = FMT_F16;
+                g.B = static_cast<const __half*>(w->in_w[k][i]) + 3 * WG_C; g.ldb = 3 * WG_C + WG_SPECT; g.b_fmt = FMT_F16; g.b_mn = 1;
+                g.alpha_ptr = iS; g.beta = 1; g.C32 = dsp32; g.ldc32 = WG_SPECT;
+                if (launch_gemm(g, st)) return -1;
+            }
+            // G += in_w^T dx over the transposed taps: dx shifted by +d, 0, -d (the guard rows keep padding out)
+            WgGemmParams q = {};
+            q.M = static_cast<int>(R); q.N = WG_C; q.K = 6 * WG_C; q.nseg = 3;
+            for (int tap = 0; tap < 3; ++tap) q.seg[tap] = WgSeg{dx, R, 2 * WG_C, (1 - tap) * dil, 2 * WG_C};
+            q.W = static_cast<const __half*>(w->in_wT[k][i]); q.bias = zero; q.rowmap = rowinfo; q.mode = WG_EPI_RES;
+            q.h32 = g32; q.h16 = g16; q.res_cols = WG_C;
+            if (launch_wg_gemm(q, st)) return -1;
+        }
+        if (wt_launch(reinterpret_cast<const void*>(wg_train_bwd_in_kernel), b, st, "wg_train_bwd_in")) return -1;
+    }
+    // upsample: d up_w = d spect^T mela over mel frames (32 grid rows each), d up_b = column sums of d spect
+    float* sup = scale + 4 * L.nf;
+    const long long nfr = R / 32, nsp = R * WG_SPECT;
+    if (launch_grad_scale(dsp32, nsp, nullptr, 0, nullptr, 0, WG_GRAD_TARGET, sup, st)) return -1;
+    {
+        TimeScope ts("wg_train_up_prep", nfr, 0, 0, st);
+        wg_scale_cast_kernel<<<static_cast<int>(std::min<long long>((nsp + 255) / 256, 4096)), 256, 0, st>>>(dsp32, nsp, sup, dsp16);
+        wg_mela_kernel<<<static_cast<int>(std::min<long long>((nfr * 384 + 255) / 256, 4096)), 256, 0, st>>>(
+            L.g.bt, rowinfo, mel16, static_cast<int>(nfr), mela);
+        ft_count_launch(2);
+        if (ft_check_launch("wg_train_up_prep")) return -1;
+    }
+    if (wt_gemm_wgrad(st, WG_UP_N, 4 * WG_MEL_LD, nfr, dsp16, WG_UP_N, mela, 4 * WG_MEL_LD, gr->up_w, sup + 1)) return -1;
+    if (launch_colsum(dsp32, 2, WG_UP_N, nfr, WG_UP_N, gr->up_b, nullptr, st)) return -1;
     return 0;
 }
 

@@ -3,9 +3,11 @@ csrc/waveglow.cu: log-mel [B, 80, F] -> audio [B, 256 F].
 
 The module has the reference's attribute names and state_dict keys (weight-norm form by default, plain weights after
 WaveGlow.remove_weightnorm), so `WaveGlow(**config["waveglow_config"]).load_state_dict(checkpoint_state_dict)` works with
-either form.  Its parameters are packed once per weight version into the kernels' layouts (weight norm folded, fp16 GEMM
+either form.  For infer, its parameters are packed once per weight version into the kernels' layouts (weight norm folded, fp16 GEMM
 operands, tap-split and gate-interleaved in_layer / cond_layer rows, the upsample as a GEMM, fp32 inverses of convinv).
-Only inference is built: forward (training) raises.
+forward (training, the z direction) packs the same layouts with differentiable device ops on every call, so the kernels'
+gradients of the packed weights reach upsample, WN and convinv parameters (weight_g / weight_v in weight-norm form) through
+torch autograd; see DESIGN.md §4.21.
 """
 from __future__ import annotations
 
@@ -59,6 +61,106 @@ def _weight(conv) -> torch.Tensor:
     return conv.weight.detach().float()
 
 
+def _effective_weight(conv) -> torch.Tensor:
+    """_weight's fold as a differentiable device op (gradients reach weight_g and weight_v)."""
+    if hasattr(conv, "weight_g"):
+        return torch._weight_norm(conv.weight_v, conv.weight_g, 0)
+    return conv.weight
+
+
+_WG_MAX_BATCH = 128              # WG_MAX_B of csrc/waveglow.cu
+
+
+class WaveGlowNoCpuPath(FlowtronB200Error, NotImplementedError):
+    """WaveGlow.forward on CPU tensors or a CPU module: the sm_90a kernels are the only implementation, so training on the
+    CPU is not implemented.  A FlowtronB200Error like every device-placement error of the library, and a
+    NotImplementedError, as forward has raised on the CPU since before training was built."""
+
+
+class WaveGlowLoss(torch.nn.Module):
+    """glow.py:43-58: sum(z^2) / (2 sigma^2) - sum(log_s) - sum(log_det_W), over the number of elements of z."""
+
+    def __init__(self, sigma=1.0):
+        super().__init__()
+        self.sigma = sigma
+
+    def forward(self, model_output):
+        z, log_s_list, log_det_W_list = model_output
+        log_s_total = sum(torch.sum(log_s) for log_s in log_s_list)
+        log_det_W_total = sum(log_det_W_list)
+        loss = torch.sum(z * z) / (2 * self.sigma * self.sigma) - log_s_total - log_det_W_total
+        return loss / (z.size(0) * z.size(1) * z.size(2))
+
+
+class _WaveGlowTrainFn(torch.autograd.Function):
+    """ft_waveglow_train_fwd / ft_waveglow_train_bwd on the fp32 packed weights: the kernels read fp16 copies (and the
+    backward's transposed ones), made here on the device; the gradients come back for the fp32 packed tensors."""
+
+    @staticmethod
+    def forward(ctx, cfg, spect, audio, *packed):
+        n_flows, n_early_every, n_early_size, L, B, Fr, N = cfg
+        Tn = N // 8
+        desc = _lib.FtWaveGlowTrainDesc(n_mel=80, n_flows=n_flows, n_group=8, n_early_every=n_early_every,
+                                        n_early_size=n_early_size, n_layers=L, n_channels=256, kernel_size=3, B=B, F=Fr, N=N)
+        w = _lib.FtWaveGlowTrainWeights()
+        keep = []
+
+        def dp(t, dtype=torch.float32):
+            t = t.detach().to(dtype).contiguous()
+            keep.append(t)
+            return t.data_ptr()
+
+        w.up_w, w.up_b = dp(packed[0], torch.float16), dp(packed[1])
+        chans, j = [], 2
+        for k in range(n_flows):
+            w.conv_w[k], w.start_w[k], w.start_b[k], w.end_w[k], w.end_b[k] = [dp(t) for t in packed[j:j + 5]]
+            chans.append(packed[j].shape[0])
+            j += 5
+            for i in range(L):
+                in_w, in_b, rs_w, rs_b = packed[j:j + 4]
+                j += 4
+                w.in_w[k][i], w.in_b[k][i] = dp(in_w, torch.float16), dp(in_b)
+                w.rs_w[k][i], w.rs_b[k][i] = dp(rs_w, torch.float16), dp(rs_b)
+                w.in_wT[k][i] = dp(in_w.detach()[:, :768].reshape(512, 3, 256).permute(2, 1, 0).reshape(256, 1536), torch.float16)
+                w.rs_wT[k][i] = dp(rs_w.detach().t(), torch.float16)
+        dev = spect.device
+        z = torch.empty(B, 8, Tn, device=dev)
+        log_s = [torch.empty(B, c // 2, Tn, device=dev) for c in chans]
+        saved = torch.empty(_lib.waveglow_train_saved_bytes(desc), dtype=torch.uint8, device=dev)
+        _lib.waveglow_train_fwd(desc, w, spect, audio, z, log_s, saved)
+        ctx.state = (desc, w, keep, saved, [(t.shape, t.dtype) for t in packed], chans, L)
+        ctx.set_materialize_grads(False)
+        return (z, *log_s)
+
+    @staticmethod
+    def backward(ctx, d_z, *d_log_s):
+        desc, w, keep, saved, shapes, chans, L = ctx.state
+        dev = saved.device
+        # in_w gradients come back per tap (split-K needs each output contiguous) and are concatenated afterwards
+        in_w_at = {2 + 5 * (k + 1) + 4 * (k * L + i) for k in range(len(chans)) for i in range(L)}
+        grads = [None if j in in_w_at else torch.empty(s, dtype=torch.float32, device=dev) for j, (s, _) in enumerate(shapes)]
+        g = _lib.FtWaveGlowTrainGrads()
+        g.up_w, g.up_b = grads[0].data_ptr(), grads[1].data_ptr()
+        taps, j = [], 2
+        for k in range(len(chans)):
+            g.conv_w[k], g.start_w[k], g.start_b[k], g.end_w[k], g.end_b[k] = [t.data_ptr() for t in grads[j:j + 5]]
+            j += 5
+            for i in range(L):
+                parts = [torch.empty(512, 256, device=dev) for _ in range(3)] + [torch.empty(512, 640, device=dev)]
+                for t in range(4):
+                    g.in_w[k][i][t] = parts[t].data_ptr()
+                taps.append((j, parts))
+                g.in_b[k][i], g.rs_w[k][i], g.rs_b[k][i] = [t.data_ptr() for t in grads[j + 1:j + 4]]
+                j += 4
+        dz = None if d_z is None else d_z.float().contiguous()
+        dls = [None if t is None else t.float().contiguous() for t in d_log_s]
+        _lib.waveglow_train_bwd(desc, w, dz, dls, saved, g)
+        for j, parts in taps:
+            grads[j] = torch.cat(parts, 1)
+        ctx.state = None
+        return (None, None, None, *grads)
+
+
 class WaveGlow(torch.nn.Module):
     def __init__(self, n_mel_channels, n_flows, n_group, n_early_every, n_early_size, WN_config):
         super().__init__()
@@ -94,7 +196,57 @@ class WaveGlow(torch.nn.Module):
         self._packed_key = None
 
     def forward(self, forward_input):
-        raise NotImplementedError("WaveGlow training (forward / WaveGlowLoss) is not built; use infer()")
+        """(spect [B, 80, F], audio [B, N]) -> (z [B, 8, N/8], log_s_list, log_det_W_list), as glow.py:196-245: z in the
+        reference's channel order (early outputs first), log_s_list[k] [B, n_half_k, N/8], log_det_W_list[k] the scalar
+        B (N/8) logdet(W_k).  N is a multiple of 8 and at most 256 F (every Mel2Samp segment).  Differentiable in every
+        parameter; spect and audio are data and take no gradient."""
+        spect, audio = forward_input
+        if spect.dim() != 3 or spect.shape[1] != self.n_mel_channels:
+            raise ValueError(f"spect must be [B, {self.n_mel_channels}, F], got {tuple(spect.shape)}")
+        if audio.dim() != 2 or audio.shape[0] != spect.shape[0]:
+            raise ValueError(f"audio must be [B, N] with the B of spect ({spect.shape[0]}), got {tuple(audio.shape)}")
+        B, _, Fr = spect.shape
+        N = audio.shape[1]
+        if not 1 <= B <= _WG_MAX_BATCH:
+            raise ValueError(f"batch must be 1..{_WG_MAX_BATCH}, got {B}")
+        if N < self.n_group or N % self.n_group:
+            raise ValueError(f"audio length N = {N} must be a positive multiple of n_group = {self.n_group}")
+        if N > 256 * Fr:
+            raise ValueError(f"audio length N = {N} exceeds the 256 F = {256 * Fr} samples the spectrogram covers")
+        if spect.requires_grad or audio.requires_grad:
+            raise ValueError("WaveGlow.forward computes no gradient for spect or audio: pass them without requires_grad")
+        if not spect.is_cuda or not audio.is_cuda or not self.upsample.weight.is_cuda:
+            raise WaveGlowNoCpuPath("WaveGlow.forward needs the module, spect and audio on CUDA: the sm_90a kernels are the "
+                                    "only implementation")
+        cfg = (self.n_flows, self.n_early_every, self.n_early_size, self.WN_config["n_layers"], B, Fr, N)
+        outs = _WaveGlowTrainFn.apply(cfg, spect.float().contiguous(), audio.float().contiguous(), *self._train_params())
+        Tn = N // self.n_group
+        log_det_W_list = [B * Tn * torch.logdet(inv.conv.weight.squeeze(-1)) for inv in self.convinv]
+        return outs[0], list(outs[1:]), log_det_W_list
+
+    def _train_params(self):
+        """The kernels' packed weights in fp32, built from the parameters with differentiable device ops, in the order
+        _WaveGlowTrainFn takes them: up_w, up_b, then per flow conv_w, start_w, start_b, end_w, end_b and per layer in_w,
+        in_b, rs_w, rs_b (the layouts of FtWaveGlowWeights)."""
+        M, L, C = self.n_mel_channels, self.WN_config["n_layers"], self.WN_config["n_channels"]
+        up = self.upsample.weight.view(M, M, 4, 32, 8).permute(3, 1, 4, 2, 0)               # [g, c, jj, j, ci]
+        out = [F.pad(up, (0, 96 - M)).reshape(32 * M * 8, 4 * 96),
+               self.upsample.bias.view(1, M, 1).expand(32, M, 8).reshape(-1)]
+        dev = self.upsample.weight.device
+        inter = torch.stack([torch.arange(C, device=dev), torch.arange(C, device=dev) + C], 1).reshape(-1)
+        for k, wn in enumerate(self.WN):
+            cond_w = _effective_weight(wn.cond_layer)[:, :, 0]
+            cond_b = wn.cond_layer.bias
+            out += [self.convinv[k].conv.weight[:, :, 0], _effective_weight(wn.start)[:, :, 0], wn.start.bias,
+                    wn.end.weight[:, :, 0], wn.end.bias]
+            for i in range(L):
+                wi = _effective_weight(wn.in_layers[i])
+                sl = slice(2 * C * i, 2 * C * (i + 1))
+                out.append(torch.cat([wi[:, :, 0], wi[:, :, 1], wi[:, :, 2], cond_w[sl]], 1)[inter])
+                out.append((wn.in_layers[i].bias + cond_b[sl])[inter])
+                out.append(_effective_weight(wn.res_skip_layers[i])[:, :, 0])
+                out.append(wn.res_skip_layers[i].bias)
+        return out
 
     @staticmethod
     def remove_weightnorm(model):

@@ -429,6 +429,58 @@ int ft_waveglow_infer(const FtWaveGlowDesc* d, const FtWaveGlowWeights* w, const
                       float* audio, void* scratch, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------
+ * WaveGlow training (glow.py:196-245 WaveGlow.forward, the z direction) and its backward, same configurations as infer.
+ * ---------------------------------------------------------------------------------------------------- */
+typedef struct {
+    int n_mel, n_flows, n_group, n_early_every, n_early_size;   /* as FtWaveGlowDesc                               */
+    int n_layers, n_channels, kernel_size;
+    int B;                                                      /* utterances (1..128), all of N samples           */
+    int F;                                                      /* mel frames of `mel`                             */
+    int N;                                                      /* audio samples: a multiple of 8, N <= 256 F      */
+} FtWaveGlowTrainDesc;
+
+/* Packed weights as in FtWaveGlowWeights (up_w, in_w, rs_w fp16; the rest fp32), plus the backward's transposed copies and
+ * the forward 1x1 convolutions:
+ *   in_wT  fp16 [256, 1536]: in_wT[c, 512 t + j] = in_w[j, 256 t + c], t = 0..2 (the dilated taps, transposed)
+ *   rs_wT  fp16 [256, 512 (256 for the last layer)] = rs_w^T
+ *   conv_w fp32 [c, c]: convinv weight of flow k */
+typedef struct {
+    const void* up_w; const float* up_b;
+    const void* in_w[FT_WG_MAX_FLOWS][FT_WG_MAX_LAYERS]; const float* in_b[FT_WG_MAX_FLOWS][FT_WG_MAX_LAYERS];
+    const void* rs_w[FT_WG_MAX_FLOWS][FT_WG_MAX_LAYERS]; const float* rs_b[FT_WG_MAX_FLOWS][FT_WG_MAX_LAYERS];
+    const void* in_wT[FT_WG_MAX_FLOWS][FT_WG_MAX_LAYERS]; const void* rs_wT[FT_WG_MAX_FLOWS][FT_WG_MAX_LAYERS];
+    const float* start_w[FT_WG_MAX_FLOWS]; const float* start_b[FT_WG_MAX_FLOWS];
+    const float* end_w[FT_WG_MAX_FLOWS]; const float* end_b[FT_WG_MAX_FLOWS];
+    const float* conv_w[FT_WG_MAX_FLOWS];
+} FtWaveGlowTrainWeights;
+
+/* fp32 gradients of the packed (effective, weight-norm-folded) weights, all overwritten: up_w [20480, 384], up_b [20480];
+ * in_w[k][i][t] [512, 256] for tap t = 0..2 and in_w[k][i][3] [512, 640] (the cond_layer slice), in_b [512]; rs_w / rs_b;
+ * start_w [256, n_half], start_b [256], end_w [2 n_half, 256], end_b, conv_w [c, c] (without the log-determinant term). */
+typedef struct {
+    float* up_w; float* up_b;
+    float* in_w[FT_WG_MAX_FLOWS][FT_WG_MAX_LAYERS][4]; float* in_b[FT_WG_MAX_FLOWS][FT_WG_MAX_LAYERS];
+    float* rs_w[FT_WG_MAX_FLOWS][FT_WG_MAX_LAYERS]; float* rs_b[FT_WG_MAX_FLOWS][FT_WG_MAX_LAYERS];
+    float* start_w[FT_WG_MAX_FLOWS]; float* start_b[FT_WG_MAX_FLOWS];
+    float* end_w[FT_WG_MAX_FLOWS]; float* end_b[FT_WG_MAX_FLOWS];
+    float* conv_w[FT_WG_MAX_FLOWS];
+} FtWaveGlowTrainGrads;
+
+/* Caller-owned areas (0 if the descriptor is rejected): `saved` lives from ft_waveglow_train_fwd to ft_waveglow_train_bwd,
+ * `scratch` only during one call. */
+size_t ft_waveglow_train_saved_bytes(const FtWaveGlowTrainDesc* d);
+size_t ft_waveglow_train_scratch_bytes(const FtWaveGlowTrainDesc* d);
+/* mel fp32 [B, 80, F], audio fp32 [B, N] -> z fp32 [B, 8, N/8] (the reference's channel order: early outputs first) and
+ * log_s[k] fp32 [B, n_half_k, N/8] (HOST array of n_flows device pointers).  No allocation, no host synchronisation. */
+int ft_waveglow_train_fwd(const FtWaveGlowTrainDesc* d, const FtWaveGlowTrainWeights* w, const float* mel, const float* audio,
+                          float* z, float* const* log_s, void* saved, void* scratch, void* stream);
+/* Upstream gradients d_z [B, 8, N/8] and d_log_s[k] [B, n_half_k, N/8] (d_z, d_log_s or any entry may be NULL = zero)
+ * -> the packed-weight gradients.  No allocation, no host synchronisation. */
+int ft_waveglow_train_bwd(const FtWaveGlowTrainDesc* d, const FtWaveGlowTrainWeights* w, const float* d_z,
+                          const float* const* d_log_s, const void* saved, const FtWaveGlowTrainGrads* g, void* scratch,
+                          void* stream);
+
+/* ------------------------------------------------------------------------------------------------------
  * Style transfer by posterior sampling (the reference's inference_style_transfer.ipynb): the posterior mean of the z of
  * B reference utterances (csrc/style.cu).
  * ---------------------------------------------------------------------------------------------------- */
