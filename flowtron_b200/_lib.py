@@ -106,6 +106,15 @@ class FtWaveGlowTrainGrads(Structure):
         [(n, c_void_p * WG_MAX_FLOWS) for n in ("start_w", "start_b", "end_w", "end_b", "conv_w")]
 
 
+class FtAttentionDesc(Structure):
+    _fields_ = [("T", c_int), ("B", c_int), ("L", c_int), ("Dq", c_int), ("E", c_int), ("A", c_int), ("has_prior", c_int),
+                ("attn_given", c_int), ("temperature", c_float)]
+
+
+class FtAttentionWeights(Structure):
+    _fields_ = [("query", c_void_p), ("key", c_void_p), ("value", c_void_p), ("v", c_void_p)]
+
+
 class FlowtronB200Error(RuntimeError):
     pass
 
@@ -267,6 +276,14 @@ def _declare(L):
     L.ft_gmm_nll_reduce.restype = c_int
     L.ft_gmm_nll_grad.argtypes = [POINTER(FtGmmDesc)] + [c_void_p] * 11
     L.ft_gmm_nll_grad.restype = c_int
+    for fn in ("ft_attention_saved_bytes", "ft_attention_scratch_bytes"):
+        getattr(L, fn).argtypes = [POINTER(FtAttentionDesc)]
+        getattr(L, fn).restype = c_size_t
+    L.ft_attention_fwd.argtypes = [POINTER(FtAttentionDesc), POINTER(FtAttentionWeights)] + [c_void_p] * 11
+    L.ft_attention_fwd.restype = c_int
+    L.ft_attention_bwd.argtypes = [POINTER(FtAttentionDesc), POINTER(FtAttentionWeights)] + [c_void_p] * 12 + \
+        [POINTER(FtAttentionWeights), c_void_p, c_void_p, c_void_p]
+    L.ft_attention_bwd.restype = c_int
 
 
 def check(rc: int, what: str = ""):
@@ -767,3 +784,31 @@ def waveglow_train_bwd(desc, weights, d_z, d_log_s_list, saved, grads):
     dls = (c_void_p * len(d_log_s_list))(*[None if t is None else t.data_ptr() for t in d_log_s_list])
     check(lib().ft_waveglow_train_bwd(byref(desc), byref(weights), ptr(d_z), dls, ptr(saved), byref(grads), ptr(scratch),
                                       stream_ptr()), "ft_waveglow_train_bwd")
+
+
+# ------------------------------------------------------------------------------------------------ Attention module
+def attention_weights(query, key, value, v) -> FtAttentionWeights:
+    """fp32 contiguous CUDA tensors (or None) -> the pointer struct of ft_attention_fwd / ft_attention_bwd (also used for the
+    weight gradients)."""
+    return FtAttentionWeights(*[None if t is None else t.data_ptr() for t in (query, key, value, v)])
+
+
+def attention_sizes(desc: FtAttentionDesc):
+    """(saved, scratch) bytes of ft_attention_fwd / ft_attention_bwd."""
+    saved, scratch = int(lib().ft_attention_saved_bytes(byref(desc))), int(lib().ft_attention_scratch_bytes(byref(desc)))
+    if saved == 0 or scratch == 0:
+        raise FlowtronB200Error(f"ft_attention rejected the configuration: {lib().ft_last_error().decode()}")
+    return saved, scratch
+
+
+def attention_fwd(desc, weights, queries, keys, values, in_lens, prior, output, attn, logprob, saved, scratch):
+    _need_cuda(values, output, attn, saved, scratch)
+    check(lib().ft_attention_fwd(byref(desc), byref(weights), ptr(queries), ptr(keys), ptr(values), ptr(in_lens), ptr(prior),
+                                 ptr(output), ptr(attn), ptr(logprob), ptr(saved), ptr(scratch), stream_ptr()), "ft_attention_fwd")
+
+
+def attention_bwd(desc, weights, queries, keys, values, in_lens, attn, d_output, d_attn, d_logprob, d_queries, d_keys, d_values,
+                  d_attn_given, grads, saved, scratch):
+    check(lib().ft_attention_bwd(byref(desc), byref(weights), ptr(queries), ptr(keys), ptr(values), ptr(in_lens), ptr(attn),
+                                 ptr(d_output), ptr(d_attn), ptr(d_logprob), ptr(d_queries), ptr(d_keys), ptr(d_values),
+                                 ptr(d_attn_given), byref(grads), ptr(saved), ptr(scratch), stream_ptr()), "ft_attention_bwd")

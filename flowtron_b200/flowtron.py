@@ -355,11 +355,76 @@ class GaussianMixture(nn.Module):
         return mean, log_var, prob
 
 
-# --------------------------------------------------------------------------------------------- attention params
+# --------------------------------------------------------------------------------------------- attention
+def _attention_run(desc, in_lens, prior, attn_given, queries, keys, values, weights):
+    """One ft_attention_fwd call -> (output [B, A, T], attn, attn_logprob or None, saved work area, fp32 operands)."""
+    f32 = lambda t: None if t is None else t.detach().float().contiguous()
+    queries, keys, values, prior = map(f32, (queries, keys, values, prior))
+    weights = [f32(w) for w in weights]
+    dev = values.device
+    saved_bytes, scratch_bytes = _lib.attention_sizes(desc)
+    saved = torch.empty(saved_bytes, dtype=torch.uint8, device=dev)
+    scratch = torch.empty(scratch_bytes, dtype=torch.uint8, device=dev)
+    output = torch.empty(desc.B, desc.A, desc.T, device=dev)
+    if attn_given is None:
+        attn = torch.empty(desc.B, desc.T, desc.L, device=dev)
+        logprob = torch.empty_like(attn)
+    else:
+        attn, logprob = f32(attn_given), None
+    _lib.attention_fwd(desc, _lib.attention_weights(*weights), queries, keys, values, in_lens, prior, output, attn, logprob,
+                       saved, scratch)
+    return output, attn, logprob, saved, (queries, keys, values, *weights)
+
+
+class _AttentionFn(torch.autograd.Function):
+    """Attention.forward on ft_attention_fwd / ft_attention_bwd.  Returns (output, attn, attn_logprob), or (output,) when the
+    weights are given: the module hands the given tensor back itself, so its own gradient path is autograd's identity."""
+
+    @staticmethod
+    def forward(ctx, desc, in_lens, prior, attn_given, queries, keys, values, w_query, w_key, w_value, w_v):
+        output, attn, logprob, saved, ops = _attention_run(desc, in_lens, prior, attn_given, queries, keys, values,
+                                                           (w_query, w_key, w_value, w_v))
+        ctx.set_materialize_grads(False)
+        ctx.desc, ctx.saved, ctx.given = desc, saved, attn_given is not None
+        ctx.save_for_backward(in_lens, attn, *ops)
+        if ctx.given:
+            return output
+        return output, attn, logprob
+
+    @staticmethod
+    def backward(ctx, d_output, d_attn=None, d_logprob=None):
+        in_lens, attn, queries, keys, values, w_query, w_key, w_value, w_v = ctx.saved_tensors
+        c = lambda g: None if g is None else g.float().contiguous()
+        d_output, d_attn, d_logprob = map(c, (d_output, d_attn, d_logprob))
+        need = ctx.needs_input_grad       # (desc, in_lens, prior, attn_given, queries, keys, values, w_query, w_key, w_value, w_v)
+        new = lambda i, like: torch.empty_like(like) if need[i] else None
+        d_attn_given = new(3, attn)
+        d_queries, d_keys, d_values = new(4, queries), new(5, keys), new(6, values)
+        g_query, g_key, g_value, g_v = new(7, w_query), new(8, w_key), new(9, w_value), new(10, w_v)
+        scratch = torch.empty(_lib.attention_sizes(ctx.desc)[1], dtype=torch.uint8, device=attn.device)
+        _lib.attention_bwd(ctx.desc, _lib.attention_weights(w_query, w_key, w_value, w_v), queries, keys, values, in_lens, attn,
+                           d_output, d_attn, d_logprob, d_queries, d_keys, d_values, d_attn_given,
+                           _lib.attention_weights(g_query, g_key, g_value, g_v), ctx.saved, scratch)
+        return None, None, None, d_attn_given, d_queries, d_keys, d_values, g_query, g_key, g_value, g_v
+
+
+def _attention_lengths(mask: Tensor, B: int, L: int) -> Tensor:
+    """Valid keys per row of a length mask [B, L, 1] (True at padded keys); ValueError for any other mask.  One host sync."""
+    if tuple(mask.shape) != (B, L, 1):
+        raise ValueError(f"Attention: mask must be [B, L, 1] = {[B, L, 1]}, got {list(mask.shape)}")
+    valid = ~mask[..., 0].bool()
+    lens = valid.sum(1)
+    if not bool((valid == (torch.arange(L, device=mask.device)[None, :] < lens[:, None])).all()):
+        raise ValueError("Attention: mask must be a length mask (valid keys a prefix of each row, as get_mask_from_lengths builds)")
+    if int(lens.min()) == 0:
+        raise ValueError("Attention: a mask row has no valid key (the softmax of that row is undefined)")
+    return lens.to(torch.int32)
+
+
 class Attention(nn.Module):
-    """Parameter container + mutable ``temperature`` of flowtron.py:528-592.  The math (Q/K/V projections,
-    tanh score, masking, softmax, prior posterior, context) runs inside the fused CUDA attention kernels invoked by
-    AR_Step; this module is never called on its own by the model."""
+    """Parameter container + mutable ``temperature`` of flowtron.py:528-592.  AR_Step reads these parameters and runs the
+    math inside its fused flow-step kernels; called on its own, the module runs the same attention kernels with its own
+    Q / K / V projections (ft_attention_fwd / ft_attention_bwd), differentiable in every input and parameter."""
 
     def __init__(self, n_mel_channels=80, n_speaker_dim=128, n_text_channels=512, n_att_channels=128, temperature=1.0):
         super().__init__()
@@ -370,8 +435,57 @@ class Attention(nn.Module):
         self.v = LinearNorm(n_att_channels, 1, bias=False, w_init_gain='tanh')
         self.score_mask_value = -float("inf")
 
-    def forward(self, *args, **kwargs):
-        raise FlowtronB200Error("Attention runs fused inside AR_Step on the CUDA path; call AR_Step / Flowtron instead")
+    def forward(self, queries, keys, values, mask=None, attn=None, attn_prior=None, *, in_lens=None):
+        """queries [T, B, Dq], keys / values [L, B, E], mask [B, L, 1] (True at padded keys) or None, attn [B, T, L] forced
+        weights or None, attn_prior [B, T, L] or None -> (output [B, A, T], attn [B, T, L], attn_logprob [B, T, L] or None), as
+        flowtron.py:559-592.  in_lens: int CUDA [B] valid keys per row, the sync-free alternative to ``mask`` (trusted: each
+        row needs at least one valid key).  With ``attn`` given, mask / in_lens / attn_prior are ignored and attn is returned
+        as given."""
+        Wq, Wk, Wv, wv = (self.query.linear_layer.weight, self.key.linear_layer.weight, self.value.linear_layer.weight,
+                          self.v.linear_layer.weight)
+        A, Dq, E = Wq.size(0), Wq.size(1), Wk.size(1)
+        if queries.dim() != 3 or keys.dim() != 3 or tuple(values.shape) != tuple(keys.shape):
+            raise ValueError(f"Attention: queries [T, B, Dq] and keys / values [L, B, E] expected, got {list(queries.shape)}, "
+                             f"{list(keys.shape)}, {list(values.shape)}")
+        T, B, L = queries.size(0), queries.size(1), keys.size(0)
+        if queries.size(2) != Dq or keys.size(1) != B or keys.size(2) != E:
+            raise ValueError(f"Attention: queries must be [T, B, {Dq}] and keys / values [L, B, {E}]")
+        _lib.check_text_len(L, "Attention")
+        given = attn is not None
+        if given:
+            if tuple(attn.shape) != (B, T, L):
+                raise ValueError(f"Attention: attn must be [B, T, L] = {[B, T, L]}, got {list(attn.shape)}")
+            mask = in_lens = attn_prior = None                  # ignored, as in the reference (flowtron.py:585-588)
+        else:
+            if mask is not None and in_lens is not None:
+                raise ValueError("Attention: pass either mask or in_lens, not both")
+            if attn_prior is not None:
+                if attn_prior.requires_grad:
+                    raise NotImplementedError("Attention: attn_prior is data; a gradient w.r.t. it is not implemented")
+                if tuple(attn_prior.shape) != (B, T, L):
+                    raise ValueError(f"Attention: attn_prior must be [B, T, L] = {[B, T, L]}, got {list(attn_prior.shape)}")
+            if in_lens is not None and in_lens.numel() != B:
+                raise ValueError("Attention: in_lens needs one length per utterance")
+        if A % 8 or Dq % 8 or E % 8:
+            raise NotImplementedError(f"Attention: the sm_90a projections need n_mel_channels, n_text_channels + n_speaker_dim "
+                                      f"and n_att_channels to be multiples of 8 (got {Dq}, {E}, {A})")
+        if mask is not None:
+            in_lens = _attention_lengths(mask, B, L)
+        tensors = (queries, keys, values, attn, attn_prior, in_lens, Wq)
+        if not all(t.is_cuda for t in tensors if t is not None):
+            raise FlowtronB200Error("Attention needs CUDA tensors: the sm_90a kernels are the only implementation")
+        if in_lens is not None:
+            in_lens = in_lens.to(device=queries.device, dtype=torch.int32).contiguous()
+        desc = _lib.FtAttentionDesc(T, B, L, Dq, E, A, int(attn_prior is not None), int(given), float(self.temperature))
+        args = (None if given else queries, None if given else keys, values,
+                None if given else Wq, None if given else Wk, Wv, None if given else wv)
+        if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (attn, *args)):
+            out = _AttentionFn.apply(desc, in_lens, attn_prior, attn, *args)
+            if given:
+                return out, attn, None
+            return out
+        output, a, logprob, _, _ = _attention_run(desc, in_lens, attn_prior, attn, args[0], args[1], args[2], args[3:])
+        return output, (attn if given else a), logprob
 
 
 # --------------------------------------------------------------------------------------------- AR step

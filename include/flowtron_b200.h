@@ -517,6 +517,47 @@ int ft_mas_align(const float* logp, const int* in_lens, const int* out_lens, int
 int ft_durations_to_attn(const int* durations, const int* in_lens, int B, int L, int Ta, int time_reversed, float* out,
                          void* stream);
 
+/* ------------------------------------------------------------------------------------------------------
+ * Attention (flowtron.py:528-592) as a module of its own (csrc/attention_module.cu): the Q / K / V projections, the fused
+ * score / softmax / prior / context kernels the flow step runs, and the forced-weights branch, forward and backward.
+ * ---------------------------------------------------------------------------------------------------- */
+typedef struct {
+    int T, B, L;        /* queries (frames), batch, keys (text tokens, <= FT_MAX_TEXT_LEN)                        */
+    int Dq, E, A;       /* query channels, key / value channels, attention channels: each a multiple of 8        */
+    int has_prior;      /* attn_prior given (ignored when attn_given)                                              */
+    int attn_given;     /* 1: `attn` is the caller's forced weights [B, T, L]; only the value projection runs       */
+    float temperature;  /* Attention.temperature (> 0)                                                             */
+} FtAttentionDesc;
+
+typedef struct {                                     /* fp32, PyTorch layouts                                       */
+    const float *query, *key, *value, *v;            /* [A, Dq], [A, E], [A, E], [A] (v.linear_layer.weight [1, A])  */
+} FtAttentionWeights;
+typedef struct {                                     /* gradients, same shapes, OVERWRITTEN; each may be NULL        */
+    float *query, *key, *value, *v;
+} FtAttentionGrads;
+
+/* `saved` persists from ft_attention_fwd to ft_attention_bwd; `scratch` is transient.  0 for a descriptor the kernels do
+ * not take (ft_last_error says why). */
+size_t ft_attention_saved_bytes(const FtAttentionDesc* d);
+size_t ft_attention_scratch_bytes(const FtAttentionDesc* d);
+/* queries fp32 [T, B, Dq], keys / values fp32 [L, B, E] (may be different tensors), in_lens int32 [B] valid keys per row on the
+ * device (NULL: all L; trusted: a row needs at least one), attn_prior fp32 [B, T, L] or NULL.
+ * Writes output fp32 [B, A, T] = bmm(attn, value(values)).transpose(1, 2), attn fp32 [B, T, L] (masked keys exactly 0) and
+ * attn_logprob fp32 [B, T, L] (log(attn + 1e-8), or the pre-mask posterior with a prior).  With attn_given, `attn` is read,
+ * queries / keys / in_lens / attn_prior / attn_logprob are not used, and one batched tensor-core kernel forms the context.
+ * No allocation, no host synchronisation (CUDA-graph capturable). */
+int ft_attention_fwd(const FtAttentionDesc* d, const FtAttentionWeights* w, const float* queries, const float* keys,
+                     const float* values, const int* in_lens, const float* attn_prior, float* output, float* attn,
+                     float* attn_logprob, void* saved, void* scratch, void* stream);
+/* Gradients of the forward above given the upstream gradients d_output [B, A, T], d_attn and d_attn_logprob [B, T, L], each
+ * NULL when absent (d_attn_logprob must be NULL with attn_given).  `attn` is the forward's attn.  Every output pointer may be
+ * NULL and skips its work: d_queries [T, B, Dq], d_keys / d_values [L, B, E], g (weight gradients) and, with attn_given only,
+ * d_attn_given [B, T, L] = d_attn + the context's gradient w.r.t. the forced weights. */
+int ft_attention_bwd(const FtAttentionDesc* d, const FtAttentionWeights* w, const float* queries, const float* keys,
+                     const float* values, const int* in_lens, const float* attn, const float* d_output, const float* d_attn,
+                     const float* d_attn_logprob, float* d_queries, float* d_keys, float* d_values, float* d_attn_given,
+                     const FtAttentionGrads* g, void* saved, void* scratch, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
