@@ -45,11 +45,17 @@ int make_tmap_2d(CUtensorMap* out, const void* ptr, int fmt, long long rows, lon
 static int g_pair_mode = 0;
 void set_gemm_pair_mode(int mode) { g_pair_mode = mode; }
 
-extern template const void* gemm_kernel_ptr<FMT_F16, 0>(int, int, int);
-extern template const void* gemm_kernel_ptr<FMT_F16, 1>(int, int, int);
-extern template const void* gemm_kernel_ptr<FMT_BF16, 0>(int, int, int);
-extern template const void* gemm_kernel_ptr<FMT_BF16, 1>(int, int, int);
-extern template const void* gemm_kernel_ptr<FMT_TF32, 0>(int, int, int);
+// 0: schedule by shape (launch_gemm).  tools/gemm_shapes.py builds private copies with 1 (cooperative only) and 2 (ping-pong
+// wherever eligible) to time both schedules on every shape.
+#ifndef FT_GEMM_SCHEDULE
+#define FT_GEMM_SCHEDULE 0
+#endif
+
+extern template const void* gemm_kernel_ptr<FMT_F16, 0>(int, int, int, int);
+extern template const void* gemm_kernel_ptr<FMT_F16, 1>(int, int, int, int);
+extern template const void* gemm_kernel_ptr<FMT_BF16, 0>(int, int, int, int);
+extern template const void* gemm_kernel_ptr<FMT_BF16, 1>(int, int, int, int);
+extern template const void* gemm_kernel_ptr<FMT_TF32, 0>(int, int, int, int);
 
 int launch_gemm(const GemmArgs& g, cudaStream_t st) {
     if (g.M <= 0 || g.N <= 0 || g.K <= 0) return 0;
@@ -68,8 +74,9 @@ int launch_gemm(const GemmArgs& g, cudaStream_t st) {
     if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); }
     bool wide = (g.N % 256 == 0) || g.N > 1024;
     if (wide && static_cast<long long>((g.N + 255) / 256) * ((g.M + BM - 1) / BM) < sms) wide = false;   // few tiles: prefer more CTAs
-    const int bn = wide ? 256 : 128;
-    const int tiles_n = (g.N + bn - 1) / bn, tiles_m = (g.M + BM - 1) / BM;
+    int bn = wide ? 256 : 128;
+    int tiles_n = (g.N + bn - 1) / bn;
+    const int tiles_m = (g.M + BM - 1) / BM;
     const long long n_tiles_ll = static_cast<long long>(tiles_n) * tiles_m;
     if (n_tiles_ll > 0x7fffffff) return ft_set_error("gemm: too many tiles");
     int n_tiles = static_cast<int>(n_tiles_ll);
@@ -97,18 +104,34 @@ int launch_gemm(const GemmArgs& g, cudaStream_t st) {
                        (!g.C16 || (al(g.C16, 16) && (g.ldc16 * 2) % 16 == 0)) &&
                        (g.act != 2 || (al(g.aux16, 4) && g.ldaux % 2 == 0)) &&
                        (!g.bias || al(g.bias, 8)) && (!g.bias2 || al(g.bias2, 8));
-    CUtensorMap tmC32 = {}, tmC16 = {};
-    if (tma_c) {
-        p.tma_c = 1;
-        p.c32_add = g.C32 && (splitk > 1 || (g.beta && !g.C16));
-        if (g.C32 && make_tmap_2d(&tmC32, g.C32, FMT_TF32, g.M, g.N, g.ldc32, 32, 64)) return -1;
-        if (g.C16 && make_tmap_2d(&tmC16, g.C16, g.c16_fmt, g.M, g.N, g.ldc16, 32, 64, 64)) return -1;
-    }
     // 2-CTA clusters (B multicast) for wide outputs with enough 256 x 256 tiles to fill the machine, only when
     // ft_set_gemm_pair_mode asks for them.  Mode 1: only for the big contractions (>= 1e11 FLOP).  Mode 2: whenever eligible.
     const long long tiles_m2 = (g.M + 2 * BM - 1) / (2 * BM);
     const bool big = 2.0 * g.M * g.N * g.K >= 1e11;
     const int ncta = ((g_pair_mode == 2 || (g_pair_mode == 1 && big)) && wide && splitk == 1 && tiles_m2 * tiles_n >= sms / 2) ? 2 : 1;
+    // Ping-pong (128 x 128 tiles, one per consumer warpgroup, each epilogue under the other warpgroup's main loop) for the
+    // staged epilogue without split-K or CTA pairs.  Its epilogue reads nothing from global memory but the biases, so
+    // act = 2 and beta with a 16-bit output stay cooperative.  By shape (tools/gemm_shapes.py --schedules, DESIGN 4.1): it
+    // wins wherever a CTA has at least 3 tiles to alternate over and K <= 4096 (xproj0 0.80 vs 1.25 ms, dgrad ih0 0.75 vs
+    // 0.78); with fewer tiles (dgrad xproj1 chunk, 200 tiles: 0.064 vs 0.060-0.062) or long K (wgrad ih0, 416 tiles over
+    // K = 32000: 0.90 vs 0.65-0.67) the cooperative 128 x BN tile is as fast or faster.
+    const bool pp_ok = tma_c && splitk == 1 && ncta == 1 && g.act != 2 && !(g.beta && g.C16);
+    const bool pp_shape = g.K <= 4096 && static_cast<long long>((g.N + 127) / 128) * tiles_m >= 3LL * sms;
+    const bool pp = pp_ok && (FT_GEMM_SCHEDULE == 2 || (FT_GEMM_SCHEDULE == 0 && pp_shape));
+    if (pp) {
+        bn = 128;
+        tiles_n = (g.N + bn - 1) / bn;
+        if (static_cast<long long>(tiles_n) * tiles_m > 0x7fffffff) return ft_set_error("gemm: too many tiles");
+        n_tiles = tiles_n * tiles_m;
+    }
+    CUtensorMap tmC32 = {}, tmC16 = {};
+    if (tma_c) {                         // stores of 64-row chunks by a warpgroup (cooperative) or 16-row ones by a warp
+        p.tma_c = 1;
+        p.c32_add = g.C32 && (splitk > 1 || (g.beta && !g.C16));
+        const int box_rows = pp ? 16 : 64;
+        if (g.C32 && make_tmap_2d(&tmC32, g.C32, FMT_TF32, g.M, g.N, g.ldc32, 32, box_rows)) return -1;
+        if (g.C16 && make_tmap_2d(&tmC16, g.C16, g.c16_fmt, g.M, g.N, g.ldc16, 32, box_rows, 64)) return -1;
+    }
     int rc;
     if (!g.a_mn) rc = make_tmap_2d(&tmA, g.A, g.a_fmt, g.M, g.K, g.lda, BK, BM);
     else         rc = make_tmap_2d(&tmA, g.A, g.a_fmt, g.K, g.M, g.lda, BK, BK);
@@ -121,11 +144,11 @@ int launch_gemm(const GemmArgs& g, cudaStream_t st) {
     const int units = ncta == 2 ? sms / 2 : sms;
     const int grid = ncta * static_cast<int>(n_work < units ? n_work : units);
     const int smem = bn == 256 ? G2Cfg<256>::SMEM : G2Cfg<128>::SMEM;
-    const void* fn = g.a_fmt == FMT_TF32 ? gemm_kernel_ptr<FMT_TF32, 0>(bn, ncta, 0)
-                   : g.a_fmt == FMT_BF16 ? (g.a_mn ? gemm_kernel_ptr<FMT_BF16, 1>(bn, ncta, g.b_mn) : gemm_kernel_ptr<FMT_BF16, 0>(bn, ncta, g.b_mn))
-                                         : (g.a_mn ? gemm_kernel_ptr<FMT_F16, 1>(bn, ncta, g.b_mn) : gemm_kernel_ptr<FMT_F16, 0>(bn, ncta, g.b_mn));
-    static bool attr_set[3][2][2][2][2] = {};
-    bool& done = attr_set[g.a_fmt][bn == 256][ncta - 1][g.a_mn][g.b_mn];
+    const void* fn = g.a_fmt == FMT_TF32 ? gemm_kernel_ptr<FMT_TF32, 0>(bn, ncta, 0, pp)
+                   : g.a_fmt == FMT_BF16 ? (g.a_mn ? gemm_kernel_ptr<FMT_BF16, 1>(bn, ncta, g.b_mn, pp) : gemm_kernel_ptr<FMT_BF16, 0>(bn, ncta, g.b_mn, pp))
+                                         : (g.a_mn ? gemm_kernel_ptr<FMT_F16, 1>(bn, ncta, g.b_mn, pp) : gemm_kernel_ptr<FMT_F16, 0>(bn, ncta, g.b_mn, pp));
+    static bool attr_set[3][2][2][2][2][2] = {};
+    bool& done = attr_set[g.a_fmt][bn == 256][ncta - 1][g.a_mn][g.b_mn][pp];
     if (!done) {
         if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) return ft_set_error("gemm: shared-memory opt-in failed");
         done = true;
@@ -136,7 +159,7 @@ int launch_gemm(const GemmArgs& g, cudaStream_t st) {
     attr[0].id = cudaLaunchAttributeClusterDimension;
     attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr; cfg.numAttrs = ncta == 2 ? 1 : 0;
-    void* args[] = {&tmA, &tmB, &tmC32, &tmC16, &p, const_cast<int*>(&tiles_n), &n_tiles};
+    void* args[] = {&tmA, &tmB, &tmC32, &tmC16, &p, &tiles_n, &n_tiles};
     TimeScope ts(g.a_mn ? "gemm_wgrad" : (g.b_mn ? "gemm_dgrad" : "gemm_fwd"), g.M, g.N, g.K, st);
     cudaError_t e = cudaLaunchKernelExC(&cfg, fn, args);
     if (e != cudaSuccess) return ft_set_error(cudaGetErrorString(e));

@@ -2,5 +2,5 @@
 #include "gemm_kernel.cuh"
 
 namespace ft {
-template const void* gemm_kernel_ptr<FMT_F16, 0>(int, int, int);
+template const void* gemm_kernel_ptr<FMT_F16, 0>(int, int, int, int);
 }  // namespace ft

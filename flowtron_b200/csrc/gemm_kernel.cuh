@@ -6,12 +6,15 @@
 //    forward pass left them (no transposes anywhere);
 //  * persistent: one CTA per SM walks a static list of 128 x BN output tiles (BN = 256, or 128 for narrow outputs) through a
 //    4-stage (BN = 256: 48 KB per stage) / 6-stage (BN = 128: 32 KB) TMA ring in SWIZZLE_128B layout, optional split-K;
-//  * warpgroup roles: WG0 = TMA producer (one elected thread), WG1 / WG2 = consumers, each owning 64 rows of the tile with a
-//    64 x BN fp32 accumulator in registers (128 registers per thread at BN = 256; setmaxnreg moves registers from the
-//    producer to the consumers).  While a consumer runs its epilogue the producer already fills the ring for its next tile;
+//  * warpgroup roles: WG0 = TMA producer (one elected thread), WG1 / WG2 = consumers.  Cooperative schedule: each consumer
+//    owns 64 rows of the tile with a 64 x BN fp32 accumulator in registers (128 registers per thread at BN = 256;
+//    setmaxnreg moves registers from the producer to the consumers).  Ping-pong schedule (PP, launch_gemm picks it by
+//    shape): each consumer owns whole 128 x 128 tiles, alternating with the other, so one's epilogue runs under the
+//    other's main loop.  While a consumer runs its epilogue the producer already fills the ring for its next tile;
 //  * epilogue through shared memory: each consumer stages its 64 x BN result in 64 x 32 chunks (two 8 KB slots, SWIZZLE_128B
-//    for fp32 / SWIZZLE_64B for 16-bit outputs) and writes them with TMA stores (reduce-add for split-K partial tiles and
-//    for beta = 1 without a 16-bit output), so it returns to its next tile's wgmmas while the stores drain.
+//    for fp32 / SWIZZLE_64B for 16-bit outputs; ping-pong: each warp its own 16 x 32 chunks in two 2 KB slots) and writes
+//    them with TMA stores (reduce-add for split-K partial tiles and for beta = 1 without a 16-bit output), so it returns to
+//    its next tile's wgmmas while the stores drain.
 //
 // Used for every non-recurrent contraction on the Flowtron hot path (LSTM input projections flowtron.py:654-655, attention
 // Q/K/V projections :568-571, DenseLayer :461-464, 1x1 conv :768, and all their dgrad/wgrad counterparts).
@@ -180,11 +183,95 @@ __device__ __forceinline__ void epi_staged(const GemmParams& p, const CUtensorMa
     }
 }
 
-template <int FMT, int BN_, int NCTA, int TA, int TB>
+// Ping-pong epilogue of one warp: its 16 rows of each 64-row half of the warpgroup's 128 x 128 tile (acc[64 h + ..], the
+// m64n128 fragment layout; rows m_w + 64 h + ..), in 16 x 32 chunks staged in the warp's own two 2 KB slots at `stg` (the
+// n-th chunk of the tile in slot n & 1; with both C32 and C16 one chunk fills both slots) and written by a TMA store, or
+// reduce-add for beta = 1 without a 16-bit output, that the warp's lane 0 issues.  So the warp needs only __syncwarp, not a
+// warpgroup barrier, and lane 0 owns the warp's bulk groups.  No global loads but bias / bias2: launch_gemm keeps act = 2
+// (aux reads) and beta with a 16-bit output (C32 reads) on the cooperative schedule, where per-element loads fit the
+// register budget.  Per element the values are those of epi_pair.
+__device__ __forceinline__ void epi_warp(const GemmParams& p, const CUtensorMap* tmC32, const CUtensorMap* tmC16,
+                                         const float* acc, float alpha, uint32_t stg, int m_w, int n_base) {
+    const int lane = threadIdx.x & 31;
+    const bool dual = p.C32 && p.C16;
+    const int sw = lane >> 2;                                // (r + 8 hh) & 7 for row r = lane / 4 + 8 hh of the chunk
+    const int nqc = min(4, (p.N - n_base + 31) / 32);        // column chunks of the tile inside N (>= 1)
+    const int nh = m_w + 64 < p.M ? 2 : 1;                   // halves with rows inside M (the TMA store would clip the rest)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        if (h >= nh) break;
+        const int mh = m_w + 64 * h;
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            if (q >= nqc) break;
+            const int nq = n_base + 32 * q;
+            float2 b[4];
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) {
+                const int n = nq + 8 * jj + 2 * (lane & 3);
+                b[jj] = make_float2(0.f, 0.f);
+                if (n < p.N && p.bias) b[jj] = __ldg(reinterpret_cast<const float2*>(p.bias + n));
+                if (n < p.N && p.bias2) { const float2 u2 = __ldg(reinterpret_cast<const float2*>(p.bias2 + n)); b[jj].x += u2.x; b[jj].y += u2.y; }
+            }
+            const int nc = nqc * h + q;                       // chunks of this tile so far
+            if (lane == 0) {
+                if (nc == 0 || dual) bulk_wait_read<0>();
+                else bulk_wait_read<1>();                    // the store issued from this slot two chunks ago has read it
+            }
+            __syncwarp();
+            const uint32_t s32 = stg + (dual ? 0 : nc & 1) * 2048;
+            const uint32_t s16 = stg + (dual ? 1 : nc & 1) * 2048;
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) {
+                const int j = 4 * q + jj;
+                const int cl = 8 * jj + 2 * (lane & 3);      // column pair within the chunk
+#pragma unroll
+                for (int hh = 0; hh < 2; ++hh) {
+                    const int r = (lane >> 2) + 8 * hh;
+                    float x0 = fmaf(acc[64 * h + 4 * j + 2 * hh], alpha, b[jj].x), x1 = fmaf(acc[64 * h + 4 * j + 2 * hh + 1], alpha, b[jj].y);
+                    if (p.act == 1) { x0 = tanh_f(x0); x1 = tanh_f(x1); }
+                    if (p.C32) {
+                        const int u = cl >> 2;               // SWIZZLE_128B: 16-byte unit u of row r sits at u ^ (r & 7)
+                        st_shared_f2(s32 + r * 128 + ((u ^ sw) << 4) + (cl & 2) * 4, x0, x1);
+                    }
+                    if (p.C16) {
+                        const int u = cl >> 3;               // SWIZZLE_64B, 64-byte rows: unit u of row r sits at u ^ ((r >> 1) & 3)
+                        const uint32_t d = s16 + r * 64 + ((u ^ ((r >> 1) & 3)) << 4) + (cl & 6) * 2;
+                        if (p.c16_fmt == 0) {    // fp16: saturate instead of overflowing to inf
+                            const __half2 h2 = __floats2half2_rn(fminf(fmaxf(x0, -65504.f), 65504.f), fminf(fmaxf(x1, -65504.f), 65504.f));
+                            st_shared_b32(d, *reinterpret_cast<const uint32_t*>(&h2));
+                        } else {
+                            const __nv_bfloat162 h2 = __floats2bfloat162_rn(x0, x1);
+                            st_shared_b32(d, *reinterpret_cast<const uint32_t*>(&h2));
+                        }
+                    }
+                }
+            }
+            fence_proxy_async_smem();                        // the staged chunk is visible to the TMA unit
+            __syncwarp();
+            if (lane == 0) {
+                if (p.C32) {
+                    if (p.c32_add) tma_reduce_add_2d(tmC32, s32, nq, mh);
+                    else tma_store_2d(tmC32, s32, nq, mh);
+                }
+                if (p.C16) tma_store_2d(tmC16, s16, nq, mh);
+                bulk_commit();
+            }
+        }
+    }
+}
+
+// PP = false: cooperative schedule, both consumer warpgroups on one 128 x BN tile (64 rows each; CTA pairs, split-K).
+// PP = true (BN_ = 128, NCTA = 1, no split-K, staged epilogue without act = 2 or a C32 read): ping-pong schedule, each consumer warpgroup owns whole
+// 128 x 128 tiles (two m64n128 wgmmas per K step, 128 accumulator registers as in the cooperative tile) and the two take
+// alternate tiles of the CTA's list; named barriers 3 and 4 hand the tensor cores from one warpgroup's main loop to the
+// other's, so each warpgroup's epilogue runs under the other's main loop.
+template <int FMT, int BN_, int NCTA, int TA, int TB, bool PP = false>
 __global__ void __launch_bounds__(G2_THREADS, 1)
 gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
              const __grid_constant__ CUtensorMap tmC32, const __grid_constant__ CUtensorMap tmC16, GemmParams p, int tiles_n,
              int n_tiles) {
+    static_assert(!PP || (BN_ == 128 && NCTA == 1), "ping-pong tiles are 128 x 128, single CTA");
     using C = G2Cfg<BN_, NCTA>;
     constexpr int TM = BM * NCTA;                   // rows of a work item's tile
     const int rank = NCTA == 2 ? static_cast<int>(cluster_ctarank()) : 0;
@@ -211,7 +298,8 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
         tma_prefetch_desc(&tmB);
         if (p.tma_c && p.C32) tma_prefetch_desc(&tmC32);
         if (p.tma_c && p.C16) tma_prefetch_desc(&tmC16);
-        for (int s = 0; s < ST; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], G2_CONSUMER_WARPS * NCTA); }
+        // empty: every consumer warp of the CTA(s) reading the stage, i.e. of one warpgroup under ping-pong
+        for (int s = 0; s < ST; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], PP ? 4 : G2_CONSUMER_WARPS * NCTA); }
         fence_mbar_init();
     }
     if (NCTA == 2) cluster_sync_all();              // the peer's barriers exist before anything can arrive on them
@@ -257,6 +345,49 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
                 }
             }
         }
+    } else if constexpr (PP) {
+        setmaxnreg_inc232();
+        // ------------------------------------------------ ping-pong consumers: warpgroup c owns items j = c, c + 2, .. of
+        // the CTA's list; warp wq stores rows [16 wq, 16 wq + 16) of each 64-row half of the tile
+        const int c = wg - 1, wq = warp & 3;
+        const float alpha = p.alpha_ptr ? p.alpha * __ldg(p.alpha_ptr) : p.alpha;
+        constexpr uint64_t KA = TA ? (UK * 128) >> 4 : 2, KB = TB ? (UK * 128) >> 4 : 2;   // descriptor advance per wgmma K step
+        constexpr uint64_t AH = (64 * 128) >> 4;                                            // A rows 64..127 of the tile
+        const uint64_t da0 = wgmma_desc(smem_u32(smem), BK * 128, 1024);
+        const uint64_t db0 = wgmma_desc(smem_u32(smem + TILE_BYTES), BK * 128, 1024);
+        const uint32_t stg = smem_u32(epi) + (4 * c + wq) * (2 * 2048);
+        float acc[128];
+        int j = c;                                           // list item
+        for (int w = wid0 + c * wstep; w < n_work; w += 2 * wstep, j += 2) {
+            const int it = j * num_kb_all;                   // ring position of its first stage
+            const int tile_m = w / tiles_n, tile_n = w - tile_m * tiles_n;
+            const int n_base = tile_n * BN_;
+            if (j > 0) named_bar_sync(3 + c, 256);           // the other warpgroup has issued item j - 1's main loop
+            for (int kb = 0; kb < num_kb_all; ++kb) {
+                const int i = it + kb, s = i % ST, ph = (i / ST) & 1;
+                mbar_wait(&full[s], ph, p.status, 113);
+                const uint64_t so = static_cast<uint64_t>(s) * (C::STAGE_BYTES >> 4);
+                wgmma_fence_acc<128>(acc);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < BK / UK; ++k) {
+                    wgmma_k<128, FMT, TA, TB>(acc, da0 + so + k * KA, db0 + so + k * KB, (kb > 0 || k > 0) ? 1u : 0u);
+                    wgmma_k<128, FMT, TA, TB>(acc + 64, da0 + AH + so + k * KA, db0 + so + k * KB, (kb > 0 || k > 0) ? 1u : 0u);
+                }
+                wgmma_commit();
+                wgmma_wait<1>();                             // the previous stage's wgmmas have read their operands
+                wgmma_fence_acc<128>(acc);
+                if (kb > 0 && lane == 0) mbar_arrive(&empty[(i - 1) % ST]);
+            }
+            if (w + wstep < n_work) named_bar_arrive(3 + (c ^ 1), 256);   // item j + 1 may take the tensor cores
+            wgmma_wait<0>();
+            wgmma_fence_acc<128>(acc);
+            if (lane == 0) mbar_arrive(&empty[(it + num_kb_all - 1) % ST]);
+#ifndef FT_GEMM_NO_STORE
+            epi_warp(p, &tmC32, &tmC16, acc, alpha, stg, tile_m * BM + 16 * wq, n_base);
+#endif
+        }
+        if (lane == 0) bulk_wait_all();                      // staged chunks stay in shared memory until stored
     } else {
         setmaxnreg_inc232();
         // ------------------------------------------------ consumers: rows [64 c, 64 c + 64) of the CTA's 128-row tile
@@ -324,16 +455,17 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
     if (NCTA == 2) cluster_sync_all();              // no CTA exits while its peer may still arrive on its barriers
 }
 
-template <int FMT, int BN_, int NCTA, int TA>
+template <int FMT, int BN_, int NCTA, int TA, bool PP = false>
 const void* gemm_kernel_tb(int tb) {
-    if constexpr (FMT == FMT_TF32) return reinterpret_cast<const void*>(gemm2_kernel<FMT, BN_, NCTA, TA, 0>);   // K-major only
-    else return tb ? reinterpret_cast<const void*>(gemm2_kernel<FMT, BN_, NCTA, TA, 1>) : reinterpret_cast<const void*>(gemm2_kernel<FMT, BN_, NCTA, TA, 0>);
+    if constexpr (FMT == FMT_TF32) return reinterpret_cast<const void*>(gemm2_kernel<FMT, BN_, NCTA, TA, 0, PP>);   // K-major only
+    else return tb ? reinterpret_cast<const void*>(gemm2_kernel<FMT, BN_, NCTA, TA, 1, PP>) : reinterpret_cast<const void*>(gemm2_kernel<FMT, BN_, NCTA, TA, 0, PP>);
 }
 
 // The launchable instantiations of one operand format and A layout (explicitly instantiated in gemm_inst_*.cu, one
 // translation unit each, so the build compiles them in parallel).
 template <int FMT, int TA>
-const void* gemm_kernel_ptr(int bn, int ncta, int tb) {
+const void* gemm_kernel_ptr(int bn, int ncta, int tb, int pp) {
+    if (pp) return gemm_kernel_tb<FMT, 128, 1, TA, true>(tb);
     if (ncta == 2) return gemm_kernel_tb<FMT, 256, 2, TA>(tb);
     return bn == 256 ? gemm_kernel_tb<FMT, 256, 1, TA>(tb) : gemm_kernel_tb<FMT, 128, 1, TA>(tb);
 }

@@ -296,6 +296,8 @@ __device__ __forceinline__ void wgmma_k(float* d, uint64_t da, uint64_t db, uint
 
 // named barrier `id` (1..15; 0 is __syncthreads) over `n` threads, a multiple of 32
 __device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+// arrive on named barrier `id` without waiting (the other n - 32k threads wait on it with named_bar_sync)
+__device__ __forceinline__ void named_bar_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
 __device__ __forceinline__ void setmaxnreg_dec40() { asm volatile("setmaxnreg.dec.sync.aligned.u32 40;"); }
 __device__ __forceinline__ void setmaxnreg_inc232() { asm volatile("setmaxnreg.inc.sync.aligned.u32 232;"); }

@@ -2,12 +2,14 @@
 """Isolated timing of every GEMM shape and epilogue the configs[1] training step (B = 32, T <= 1000) issues.
 
 CUDA events over repeated launches, with three rotating operand sets so a launch does not find its operands in L2.
-Per shape: ms and TFLOP/s with single-CTA tiles (pair mode 0) and with CTA pairs wherever eligible (pair mode 2), the
-epilogue's HBM floor (bytes the epilogue writes and reads over the copy bandwidth measured in the same run) and, with
---mainloop, the same kernel with its output stores compiled out (FT_GEMM_NO_STORE, in a private build of the GEMM
-translation units in a temporary directory; the library the package loads is never touched).
+Per shape: ms and TFLOP/s with single-CTA tiles (pair mode 0, the default schedule by shape) and with CTA pairs wherever
+eligible (pair mode 2), the epilogue's HBM floor (bytes the epilogue writes and reads over the copy bandwidth measured in
+the same run) and, with --mainloop, the same kernels with their output stores compiled out (FT_GEMM_NO_STORE).  With
+--schedules, also the cooperative schedule alone and the ping-pong schedule wherever it is eligible (FT_GEMM_SCHEDULE=1
+/ 2).  Each variant is a private build of the GEMM translation units, in a
+temporary directory or --builddir (reused when present there); the library the package loads is never touched.
 
-    python tools/gemm_shapes.py [--tree DIR] [--mainloop] [--only SUBSTR] [--json FILE]
+    python tools/gemm_shapes.py [--tree DIR] [--mainloop] [--schedules] [--builddir DIR] [--only SUBSTR] [--json FILE]
 
 --tree runs the library built in another checkout of this project (DIR/flowtron_b200), so two builds can be timed in
 one session."""
@@ -21,6 +23,8 @@ import tempfile
 ap = argparse.ArgumentParser()
 ap.add_argument("--tree", default=os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 ap.add_argument("--mainloop", action="store_true", help="also time the main loop alone (stores compiled out)")
+ap.add_argument("--schedules", action="store_true", help="also time the cooperative and the ping-pong schedule alone")
+ap.add_argument("--builddir", default=None, help="directory for the private builds, reused when already there")
 ap.add_argument("--only", default=None)
 ap.add_argument("--json", default=None)
 ap.add_argument("--reps", type=int, default=20)
@@ -83,20 +87,26 @@ def copy_bandwidth():
     return 2 * 4 * n * 10 / (e0.elapsed_time(e1) / 1e3) / 1e9
 
 
-def mainloop_lib(tree):
-    """The GEMM translation units of `tree` rebuilt with FT_GEMM_NO_STORE, linked with the tree's other objects."""
+VARIANTS = {"mainloop": "-DFT_GEMM_NO_STORE", "coop": "-DFT_GEMM_SCHEDULE=1", "pp": "-DFT_GEMM_SCHEDULE=2"}
+
+
+def variant_lib(tree, name):
+    """The GEMM translation units of `tree` rebuilt with VARIANTS[name], linked with the tree's other objects."""
     from flowtron_b200 import build as fb
     csrc, objdir = fb.CSRC, os.path.join(fb.HERE, "build")
-    tmp = tempfile.mkdtemp(prefix="gemm_mainloop_")
+    tmp = os.path.join(args.builddir, name) if args.builddir else tempfile.mkdtemp(prefix=f"gemm_{name}_")
+    lib = os.path.join(tmp, "libflowtron_b200.so")
+    if os.path.exists(lib):
+        return lib
+    os.makedirs(tmp, exist_ok=True)
     gemm_srcs = [s for s in fb.sources() if s.startswith("gemm")]
-    procs = [subprocess.Popen([fb.NVCC, *fb.FLAGS, "-DFT_GEMM_NO_STORE", "-c", os.path.join(csrc, s), "-o",
+    procs = [subprocess.Popen([fb.NVCC, *fb.FLAGS, VARIANTS[name], "-c", os.path.join(csrc, s), "-o",
                                os.path.join(tmp, s[:-3] + ".o")], stdout=subprocess.DEVNULL, stderr=subprocess.PIPE)
              for s in gemm_srcs]
     for p in procs:
         if p.wait() != 0:
             raise RuntimeError(p.stderr.read().decode())
     objs = [os.path.join(tmp, s[:-3] + ".o") if s in gemm_srcs else os.path.join(objdir, s[:-3] + ".o") for s in fb.sources()]
-    lib = os.path.join(tmp, "libflowtron_b200.so")
     subprocess.run([fb.NVCC, "-shared", "-o", lib, *objs, "-gencode", "arch=compute_90a,code=sm_90a", "-cudart", "shared",
                     "-lcufft", "-Xlinker", "-rpath,/usr/local/cuda/lib64"], check=True, capture_output=True)
     return lib
@@ -139,53 +149,46 @@ def run_shape(shape, modes):
 
 
 def main():
-    name, smi = gpu_info()
-    bw = copy_bandwidth()
-    rows = []
-    nostore = {}
-    if args.mainloop:
-        lib_ml = mainloop_lib(TREE)
-        _lib.LIB_PATH = lib_ml
-    main_path = os.path.join(TREE, "flowtron_b200", "libflowtron_b200.so")
-    # two libraries cannot share the process: the main-loop pass runs in a child
-    if args.mainloop and os.environ.get("FT_GEMM_SHAPES_CHILD") != "1":
-        env = dict(os.environ, FT_GEMM_SHAPES_CHILD="1", FT_GEMM_SHAPES_LIB=_lib.LIB_PATH)
+    child = os.environ.get("FT_GEMM_SHAPES_CHILD") == "1"
+    if child:                       # one variant library: its single-CTA times only
+        _lib.LIB_PATH = os.environ["FT_GEMM_SHAPES_LIB"]
+        ms = {s[0]: run_shape(s, (0,))[0][0] for s in SHAPES if not args.only or args.only in s[0]}
+        print(json.dumps({"ms": ms}))
+        return
+    # two libraries cannot share the process: each variant runs in a child
+    names = (["mainloop"] if args.mainloop else []) + (["coop", "pp"] if args.schedules else [])
+    libs = {n: variant_lib(TREE, n) for n in names}
+    var = {}
+    for n in names:
+        env = dict(os.environ, FT_GEMM_SHAPES_CHILD="1", FT_GEMM_SHAPES_LIB=libs[n])
         out = subprocess.run([sys.executable, __file__, "--tree", TREE, "--reps", str(args.reps)] +
                              (["--only", args.only] if args.only else []), env=env, capture_output=True, text=True)
         if out.returncode != 0:
             raise RuntimeError(out.stderr)
-        nostore = json.loads(out.stdout.strip().splitlines()[-1])["ms"]
-        _lib.LIB_PATH = main_path
-    if os.environ.get("FT_GEMM_SHAPES_LIB"):
-        _lib.LIB_PATH = os.environ["FT_GEMM_SHAPES_LIB"]
-    child = os.environ.get("FT_GEMM_SHAPES_CHILD") == "1"
-    ms_single = {}
-    if not child:
-        print(f"# {name} | {smi} | copy bandwidth {bw:.0f} GB/s | tree {TREE}")
-        print(f"{'shape':30s} {'M x N x K':>22s} | {'single ms':>9s} {'TF/s':>6s} | {'pair ms':>8s} {'TF/s':>6s} | "
-              f"{'epi floor':>9s} | {'main loop':>9s} {'share':>6s}")
+        var[n] = json.loads(out.stdout.strip().splitlines()[-1])["ms"]
+    name, smi = gpu_info()
+    bw = copy_bandwidth()
+    rows = []
+    print(f"# {name} | {smi} | copy bandwidth {bw:.0f} GB/s | tree {TREE}")
+    cols = "".join(f" | {n:>8s} ms" for n in ("coop", "pp") if n in var)
+    print(f"{'shape':30s} {'M x N x K':>22s} | {'single ms':>9s} {'TF/s':>6s} | {'pair ms':>8s} {'TF/s':>6s}{cols} | "
+          f"{'epi floor':>9s} | {'main loop':>9s} {'share':>6s}")
     for s in SHAPES:
         if args.only and args.only not in s[0]:
             continue
         nm, M, N, K = s[:4]
-        res, eb = run_shape(s, (0,) if child else (0, 2))
-        ms_single[nm] = res[0]
-        if child:
-            continue
+        res, eb = run_shape(s, (0, 2))
         tf = lambda ms: 2.0 * M * N * K / ms / 1e9
         floor = eb / (bw * 1e9) * 1e3
-        ml = nostore.get(nm)
+        ml = var.get("mainloop", {}).get(nm)
         mls = f"{ml:9.3f} {ml / res[0] * 100:5.0f}%" if ml else f"{'-':>9s} {'':>6s}"
-        print(f"{nm:30s} {M:6d} x {N:5d} x {K:6d} | {res[0]:9.3f} {tf(res[0]):6.1f} | {res[2]:8.3f} {tf(res[2]):6.1f} | "
+        sch = "".join(f" | {var[n][nm]:11.3f}" for n in ("coop", "pp") if n in var)
+        print(f"{nm:30s} {M:6d} x {N:5d} x {K:6d} | {res[0]:9.3f} {tf(res[0]):6.1f} | {res[2]:8.3f} {tf(res[2]):6.1f}{sch} | "
               f"{floor:9.3f} | {mls}")
         rows.append(dict(shape=nm, M=M, N=N, K=K, single_ms=res[0], pair_ms=res[2], epi_bytes=eb, epi_floor_ms=floor,
-                         mainloop_ms=ml))
-    if child:
-        print(json.dumps({"ms": ms_single}))
-        return
+                         mainloop_ms=ml, coop_ms=var.get("coop", {}).get(nm), pp_ms=var.get("pp", {}).get(nm)))
     if args.json:
         with open(args.json, "w") as f:
             json.dump(dict(gpu=name, nvidia_smi=smi, copy_gbps=bw, tree=TREE, rows=rows), f, indent=1)
-
 
 main()
