@@ -198,6 +198,8 @@ def _declare(L):
     L.ft_stft_inverse.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_longlong, c_void_p, c_int, c_int, c_void_p,
                                   c_float, c_void_p, c_void_p]
     L.ft_stft_inverse.restype = c_int
+    L.ft_stft_pack_rows.argtypes = [c_void_p, c_int, c_longlong, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]
+    L.ft_stft_pack_rows.restype = c_int
     L.ft_attn_prior.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_float, c_void_p, c_void_p]
     L.ft_attn_prior.restype = c_int
     L.ft_collate_mel.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]
@@ -244,6 +246,9 @@ def _declare(L):
     L.ft_waveglow_infer.argtypes = [POINTER(FtWaveGlowDesc), POINTER(FtWaveGlowWeights), c_void_p, c_void_p, c_float, c_void_p,
                                     c_void_p, c_void_p]
     L.ft_waveglow_infer.restype = c_int
+    L.ft_waveglow_infer_dev.argtypes = [POINTER(FtWaveGlowDesc), POINTER(FtWaveGlowWeights), c_void_p, c_void_p, c_float,
+                                        c_void_p, c_void_p, c_void_p, c_void_p]
+    L.ft_waveglow_infer_dev.restype = c_int
     for fn in ("ft_waveglow_train_saved_bytes", "ft_waveglow_train_scratch_bytes"):
         getattr(L, fn).argtypes = [POINTER(FtWaveGlowTrainDesc)]
         getattr(L, fn).restype = c_size_t
@@ -542,6 +547,17 @@ def stft_transform(wav, sample_offsets, frame_offsets, n_utt, total_frames, wind
                                   int(n_fft), int(hop), ptr(magnitude), ptr(phase), stream_ptr()), "ft_stft_transform")
 
 
+def stft_pack_rows(audio, lengths, n_fft, hop, packed, sample_offsets, frame_offsets):
+    """audio f32 [B, N] CUDA (contiguous), lengths int64 CUDA [B] -> packed rows and their int64 [B + 1] sample / frame
+    offsets, planned on the device (ft_stft_pack_rows: rows of at most n_fft / 2 samples come out empty)."""
+    _need_cuda(audio, lengths, packed, sample_offsets, frame_offsets)
+    assert audio.dtype == packed.dtype == torch.float32 and audio.is_contiguous() and lengths.dtype == torch.int64
+    assert sample_offsets.dtype == frame_offsets.dtype == torch.int64 and lengths.is_contiguous()
+    B, N = audio.shape
+    check(lib().ft_stft_pack_rows(ptr(audio), int(B), int(N), ptr(lengths), int(n_fft), int(hop), ptr(packed),
+                                  ptr(sample_offsets), ptr(frame_offsets), stream_ptr()), "ft_stft_pack_rows")
+
+
 STFT_INVERSE_HOPS = (128, 256, 512)
 
 
@@ -743,15 +759,21 @@ def gmm_nll_grad(z, out_lens_i32, mean, log_var, prob, per_row, g_nll, dz, dmean
 
 
 # ------------------------------------------------------------------------------------------------ WaveGlow
-def waveglow_infer(desc, weights, mel, noise, sigma, audio):
-    """mel f32 [B,80,F_max], noise f32 [B,8,32 F_max], audio f32 [B,256 F_max] (written); desc.frames set by the caller."""
-    _need_cuda(mel, noise, audio)
+def waveglow_infer(desc, weights, mel, noise, sigma, audio, frames_dev=None):
+    """mel f32 [B,80,F_max], noise f32 [B,8,32 F_max], audio f32 [B,256 F_max] (written).  The frame counts are either
+    desc.frames (host) or frames_dev (int32 CUDA [B], with desc.frames NULL: ft_waveglow_infer_dev)."""
+    _need_cuda(mel, noise, audio, frames_dev)
     nbytes = int(lib().ft_waveglow_scratch_bytes(byref(desc)))
     if nbytes == 0:
         raise FlowtronB200Error(f"ft_waveglow_scratch_bytes rejected the configuration: {lib().ft_last_error().decode()}")
     scratch = scratch_buffer(nbytes, mel.device)
-    check(lib().ft_waveglow_infer(byref(desc), byref(weights), ptr(mel), ptr(noise), float(sigma), ptr(audio), ptr(scratch),
-                                  stream_ptr()), "ft_waveglow_infer")
+    if frames_dev is None:
+        check(lib().ft_waveglow_infer(byref(desc), byref(weights), ptr(mel), ptr(noise), float(sigma), ptr(audio), ptr(scratch),
+                                      stream_ptr()), "ft_waveglow_infer")
+    else:
+        assert frames_dev.dtype == torch.int32 and frames_dev.is_contiguous() and frames_dev.numel() == desc.B
+        check(lib().ft_waveglow_infer_dev(byref(desc), byref(weights), ptr(mel), ptr(noise), float(sigma), ptr(frames_dev),
+                                          ptr(audio), ptr(scratch), stream_ptr()), "ft_waveglow_infer_dev")
 
 
 def _wg_train_bytes(desc):

@@ -83,9 +83,10 @@ istft_kernel(IstftParams p) {
 
     const int hop = p.hop, n_ov = NFFT / hop, half = n_ov / 2;
     const int tile_frames = IS_TILE_SAMPLES / hop;
-    const long long n_tiles = (p.total_frames + tile_frames - 1) / tile_frames;
+    const long long total = min(p.total_frames, __ldg(p.frame_offsets + p.n_utt));   // the grid covers the host's bound
+    const long long n_tiles = (total + tile_frames - 1) / tile_frames;
     for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        const long long t_end = min(p.total_frames, (tile + 1) * tile_frames);
+        const long long t_end = min(total, (tile + 1) * tile_frames);
         for (long long f = tile * tile_frames; f < t_end;) {            // one segment per utterance in the tile
             const int u = is_find_utt(p.frame_offsets, p.n_utt, f);
             const long long fo = __ldg(p.frame_offsets + u);
@@ -148,9 +149,64 @@ istft_kernel(IstftParams p) {
     }
 }
 
+// Rows of a padded batch -> the packed layout ft_stft_transform reads, planned on the device.  Block (x, b) sums the
+// clamped lengths of rows 0..b-1 for row b's sample and frame offsets, then copies its chunk of row b.
+constexpr int PK_THREADS = 256, PK_CHUNK = 8192;
+
+__device__ __forceinline__ long long pk_len(const long long* lengths, int b, long long N) {
+    const long long n = __ldg(lengths + b);
+    return n <= NFFT / 2 ? 0 : min(n, N);                 // rows up to the reflect padding are empty
+}
+
+__global__ void __launch_bounds__(PK_THREADS) stft_pack_kernel(const float* __restrict__ audio, long long N,
+                                                               const long long* __restrict__ lengths, int B, int hop,
+                                                               float* __restrict__ packed, long long* __restrict__ so,
+                                                               long long* __restrict__ fo) {
+    __shared__ long long s_red[2][PK_THREADS / 32];
+    const int b = blockIdx.y, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    long long s = 0, f = 0;
+    for (int j = threadIdx.x; j < b; j += PK_THREADS) {
+        const long long n = pk_len(lengths, j, N);
+        s += n;
+        f += n ? 1 + n / hop : 0;
+    }
+#pragma unroll
+    for (int off = 16; off; off >>= 1) {
+        s += __shfl_xor_sync(0xffffffffu, s, off);
+        f += __shfl_xor_sync(0xffffffffu, f, off);
+    }
+    if (lane == 0) { s_red[0][warp] = s; s_red[1][warp] = f; }
+    __syncthreads();
+    s = 0; f = 0;
+#pragma unroll
+    for (int w = 0; w < PK_THREADS / 32; ++w) { s += s_red[0][w]; f += s_red[1][w]; }
+    const long long n = pk_len(lengths, b, N);
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        so[b] = s; fo[b] = f;
+        if (b == B - 1) { so[B] = s + n; fo[B] = f + (n ? 1 + n / hop : 0); }
+    }
+    const long long c0 = static_cast<long long>(blockIdx.x) * PK_CHUNK, c1 = min(n, c0 + PK_CHUNK);
+    const float* src = audio + static_cast<long long>(b) * N;
+    for (long long i = c0 + threadIdx.x; i < c1; i += PK_THREADS) packed[s + i] = __ldg(src + i);
+}
+
 }  // namespace ft
 
 extern "C" {
+
+int ft_stft_pack_rows(const float* audio, int B, long long N, const long long* lengths, int n_fft, int hop, float* packed,
+                      long long* sample_offsets, long long* frame_offsets, void* stream) {
+    using namespace ft;
+    if (!audio || !lengths || !packed || !sample_offsets || !frame_offsets) return ft_set_error("ft_stft_pack_rows: NULL argument");
+    if (n_fft != 1024) return ft_set_error("ft_stft_pack_rows: n_fft must be 1024");
+    if (B < 1 || B > 65535 || N < 1 || hop < 1) return ft_set_error("ft_stft_pack_rows: need 1 <= B <= 65535, N >= 1, hop >= 1");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const dim3 grid(static_cast<unsigned>((N + PK_CHUNK - 1) / PK_CHUNK), static_cast<unsigned>(B));
+    TimeScope ts("stft_pack", B, N, hop, st);
+    stft_pack_kernel<<<grid, PK_THREADS, 0, st>>>(audio, N, lengths, B, hop, packed, sample_offsets, frame_offsets);
+    ft_count_launch(1);
+    return ft_check_launch("stft_pack_kernel");
+}
 
 int ft_stft_inverse(const float* magnitude, const float* phase, const long long* frame_offsets, const long long* out_offsets,
                     int n_utt, long long total_frames, const float* window, int n_fft, int hop, const float* bias,

@@ -95,12 +95,14 @@ mel_fused_kernel(MelFusedParams p) {
     float* xi = xr + XBUF;
     float* smag = xi + XBUF;
 
-    const long long n_tiles = (p.total_frames + MF_TILE - 1) / MF_TILE;
+    // transform: total_frames bounds the grid, frame_offsets[n_utt] (planned on the device) is the live total
+    const long long total = kTransform ? min(p.total_frames, __ldg(p.frame_offsets + p.n_utt)) : p.total_frames;
+    const long long n_tiles = (total + MF_TILE - 1) / MF_TILE;
     for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         for (int q = 0; q < MF_TILE / MF_WARPS; ++q) {
             const int fr = warp + q * MF_WARPS;
             const long long f = tile * MF_TILE + fr;
-            if (f >= p.total_frames) { if (lane == 0) sFu[fr] = 0; continue; }      // warp-uniform
+            if (f >= total) { if (lane == 0) sFu[fr] = 0; continue; }      // warp-uniform
             const int u = mf_find_utt(p.frame_offsets, p.n_utt, f);
             const long long fo = __ldg(p.frame_offsets + u);
             const int Fu = static_cast<int>(__ldg(p.frame_offsets + u + 1) - fo);

@@ -56,6 +56,7 @@ struct WgGemmParams {
     const __half* W;      // [N, K] fp16 (K contiguous)
     const float* bias;    // [N]
     const int* rowmap;    // [M]: < 0 = row m is not written; UP: the destination row of frame row m
+    const int* m_live;    // optional device row count <= M (the infer plan's totals): rows and tiles past it are skipped
     int mode;
     __half* out16; long long ld16;            // UP, GATE
     float* h32; __half* h16; float* skip32;   // RES ([rows, C] each)
@@ -83,8 +84,8 @@ __device__ __forceinline__ void mma16816(float* c, const uint32_t* a, uint32_t b
 
 __device__ __forceinline__ __half sat_half(float x) { return __float2half_rn(fminf(fmaxf(x, -65504.f), 65504.f)); }
 
-__device__ __forceinline__ void wg_epi_pair(const WgGemmParams& p, int m, int n, float v0, float v1) {
-    if (m >= p.M) return;
+__device__ __forceinline__ void wg_epi_pair(const WgGemmParams& p, int M, int m, int n, float v0, float v1) {
+    if (m >= M) return;
     const int info = __ldg(p.rowmap + m);
     if (info < 0) return;                                     // guard / padding rows are never written
     const int row = p.mode == WG_EPI_UP ? info : m;           // UP: a frame row lands on its first group row
@@ -136,6 +137,8 @@ __global__ void __launch_bounds__(G_THREADS, 2) wg_gemm_kernel(const __grid_cons
     const int wm = warp & 1, wn = warp >> 1;                  // warp tile: 64 rows x 32 columns
     const int n0 = blockIdx.x * GB_N;
     const int m0 = blockIdx.y * GB_M;
+    const int M = p.m_live ? min(__ldg(p.m_live), p.M) : p.M;
+    if (m0 >= M) return;                                      // block-uniform: a tile wholly past the live rows
     const int nkb = p.K / GB_K;
 
     auto load_stage = [&](int stage, int kb) {
@@ -158,7 +161,7 @@ __global__ void __launch_bounds__(G_THREADS, 2) wg_gemm_kernel(const __grid_cons
             const int c = tid + i * G_THREADS;
             const int r = c >> 2, q = c & 3;
             const long long ar = static_cast<long long>(m0 + r) + shift;
-            const bool ok = (m0 + r < p.M) && ar >= 0 && ar < rows;
+            const bool ok = (m0 + r < M) && ar >= 0 && ar < rows;
             const __half* src = ok ? base + ar * ld + kk + q * 8 : base;
             cp_async16(smem_u32(sa + r * G_LDS + q * 8), src, ok);
             const __half* wsrc = p.W + static_cast<long long>(n0 + r) * p.K + kb * GB_K + q * 8;
@@ -215,8 +218,8 @@ __global__ void __launch_bounds__(G_THREADS, 2) wg_gemm_kernel(const __grid_cons
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             const int n = n0 + wn * 32 + j * 8 + 2 * (lane & 3);
-            wg_epi_pair(p, m, n, acc[i][j][0], acc[i][j][1]);
-            wg_epi_pair(p, m + 8, n, acc[i][j][2], acc[i][j][3]);
+            wg_epi_pair(p, M, m, n, acc[i][j][0], acc[i][j][1]);
+            wg_epi_pair(p, M, m + 8, n, acc[i][j][2], acc[i][j][3]);
         }
     }
 }
@@ -237,13 +240,46 @@ static int launch_wg_gemm(const WgGemmParams& p, cudaStream_t st) {
     return ft_check_launch("wg_gemm_kernel");
 }
 
-// ------------------------------------------------------------------------------------------------ prep
+// ------------------------------------------------------------------------------------------------ plan and prep
+// The packed row layout of a batch.  It lives in device memory, written by wg_plan_kernel from the frame counts, so the
+// counts may themselves be device data (a CUDA graph replays with new lengths); the host only sizes grids and scratch
+// for the largest layout the counts can give.
 struct WgBatch {
     int B, Tg_max;
-    int frames[WG_MAX_B];
+    int mrows, grows;            // frame-grid rows (= mbase[B]); group-grid rows (gbase[B] + the trailing guard)
+    int frames[WG_MAX_B];        // clamped to 1..F_max
     int mbase[WG_MAX_B + 1];     // first frame-grid row of utterance b (its 3 zero rows come first); mbase[B] = rows
     int gbase[WG_MAX_B + 1];     // first group-grid row of utterance b; gbase[B] = end of the last utterance
 };
+
+struct WgFrames { int f[WG_MAX_B]; };   // host frame counts, passed by value
+
+constexpr int WG_PLAN_THREADS = WG_MAX_B + 32;
+
+// One CTA: thread b <= B sums the rows of the utterances before b.  Counts come from `dev` (int32 [B] in device memory)
+// or, when it is null, from `host`; every count is clamped to 1..F_max so no length can address past the grids.
+__global__ void __launch_bounds__(WG_PLAN_THREADS) wg_plan_kernel(const __grid_constant__ WgFrames host, const int* __restrict__ dev,
+                                                                  int B, int F_max, int Tg_max, WgBatch* __restrict__ bt) {
+    __shared__ int s_f[WG_MAX_B];
+    const int t = threadIdx.x;
+    if (t < B) s_f[t] = min(max(dev ? __ldg(dev + t) : host.f[t], 1), F_max);
+    __syncthreads();
+    if (t > B) return;
+    int m = 0, g = WG_GUARD;
+    for (int j = 0; j < t; ++j) {
+        m += s_f[j] + 3;
+        g += 32 * s_f[j] + WG_GUARD;
+    }
+    if (t < B) {
+        bt->frames[t] = s_f[t];
+        bt->mbase[t] = m;
+        bt->gbase[t] = g;
+    } else {
+        bt->B = B; bt->Tg_max = Tg_max;
+        bt->mbase[B] = m; bt->gbase[B] = g - WG_GUARD;
+        bt->mrows = m; bt->grows = g;
+    }
+}
 
 __device__ __forceinline__ int find_utt(const int* base, int B, int r) {   // largest b with base[b] <= r
     int lo = 0, hi = B - 1;
@@ -255,9 +291,14 @@ __device__ __forceinline__ int find_utt(const int* base, int B, int r) {   // la
 }
 
 // mel [B, 80, F_max] fp32 -> mel16 [mrows, 96]; up_rowmap [mrows]; rowinfo [grows] = b * Tg_max + g, or -1 for guard rows.
-__global__ void wg_prep_kernel(const __grid_constant__ WgBatch bt, const float* __restrict__ mel, int F_max, __half* __restrict__ mel16,
-                               int* __restrict__ up_rowmap, int* __restrict__ rowinfo, int grows) {
-    const int mrows = bt.mbase[bt.B];
+// The grid is sized for the host's bound on the layout; the loop runs over the plan's rows.
+__global__ void wg_prep_kernel(const WgBatch* __restrict__ plan, const float* __restrict__ mel, int F_max, __half* __restrict__ mel16,
+                               int* __restrict__ up_rowmap, int* __restrict__ rowinfo) {
+    __shared__ WgBatch bt;
+    for (int i = threadIdx.x; i < static_cast<int>(sizeof(WgBatch) / 4); i += blockDim.x)
+        reinterpret_cast<int*>(&bt)[i] = __ldg(reinterpret_cast<const int*>(plan) + i);
+    __syncthreads();
+    const int mrows = bt.mrows, grows = bt.grows;
     const long long n_mel = static_cast<long long>(mrows) * WG_MEL_LD;
     const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
     for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n_mel + mrows + grows; i += stride) {
@@ -290,7 +331,8 @@ __global__ void wg_prep_kernel(const __grid_constant__ WgBatch bt, const float* 
 constexpr int T_THREADS = 256, T_ROWS_PER_WARP = 8;
 
 struct WgTailParams {
-    int R;                          // grid rows
+    int R;                          // grid rows: the host's bound
+    const int* live_rows;           // device: the plan's grid rows (<= R); rows past it are skipped
     const int* rowinfo;             // [R]
     float* state;                   // [R, 8] fp32 flow state; the c live channels of a flow sit at positions [8 - c, 8)
     // the flow being finished (cur = 0 for the head launch, which only draws the initial noise)
@@ -318,6 +360,8 @@ __global__ void __launch_bounds__(T_THREADS) wg_tail_kernel(const __grid_constan
     float* s_endb = s_misc + 64;
     float* s_startb = s_misc + 72;
     const int c = 8 - p.o;
+    const int R = min(p.R, __ldg(p.live_rows));
+    if (static_cast<int>(blockIdx.x) * (T_THREADS / 32) * T_ROWS_PER_WARP >= R) return;   // block-uniform
     if (p.cur) {
         for (int i = threadIdx.x; i < 2 * p.nh * WG_C; i += T_THREADS) s_end[i] = p.end_w[i];
         for (int i = threadIdx.x; i < c * c; i += T_THREADS) s_inv[i] = p.inv_w[i];
@@ -334,7 +378,7 @@ __global__ void __launch_bounds__(T_THREADS) wg_tail_kernel(const __grid_constan
     float* ys = s_y[warp];
     float* so = s_out[warp];
     const int r0 = (blockIdx.x * (T_THREADS / 32) + warp) * T_ROWS_PER_WARP;
-    for (int r = r0; r < r0 + T_ROWS_PER_WARP && r < p.R; ++r) {
+    for (int r = r0; r < r0 + T_ROWS_PER_WARP && r < R; ++r) {
         const int info = __ldg(p.rowinfo + r);
         if (info < 0) continue;                                   // warp-uniform
         const int b = info / p.Tg_max, g = info - b * p.Tg_max;
@@ -417,12 +461,15 @@ static int launch_wg_tail(const WgTailParams& p, cudaStream_t st) {
 }
 
 // ------------------------------------------------------------------------------------------------ driver
+// Host side of a batch: the bound on its layout (the exact layout for host frame counts; every utterance at F_max when
+// the counts are device data) that sizes grids and scratch, and the host counts for wg_plan_kernel.
 struct WgLayout {
     int B, Tg_max, mrows, grows;
-    WgBatch bt;
-    size_t off_mel16, off_uprow, off_rowinfo, off_spect, off_h32, off_h16, off_acts, off_skip, off_state, total;
+    WgFrames fr;
+    size_t off_plan, off_mel16, off_uprow, off_rowinfo, off_spect, off_h32, off_h16, off_acts, off_skip, off_state, total;
 };
 
+// d->frames == NULL: the counts arrive in device memory, and the layout is bounded by F_max for every utterance.
 static int wg_layout(const FtWaveGlowDesc* d, WgLayout* L) {
     if (!d) return ft_set_error("waveglow: null descriptor");
     if (d->n_mel != WG_MEL || d->n_group != 8 || d->n_channels != WG_C || d->kernel_size != 3)
@@ -434,29 +481,23 @@ static int wg_layout(const FtWaveGlowDesc* d, WgLayout* L) {
     const int n_early = (d->n_flows - 1) / d->n_early_every;
     if (8 - n_early * d->n_early_size < 2) return ft_set_error("waveglow: early outputs leave fewer than 2 channels");
     if (d->B < 1 || d->B > WG_MAX_B) return ft_set_error("waveglow: batch must be 1..128");
-    if (!d->frames) return ft_set_error("waveglow: frames (host array) required");
     L->B = d->B;
     L->Tg_max = 32 * d->F_max;
-    L->bt.B = d->B;
-    L->bt.Tg_max = L->Tg_max;
     long long m = 0, g = WG_GUARD;
     for (int b = 0; b < d->B; ++b) {
-        const int f = d->frames[b];
+        const int f = d->frames ? d->frames[b] : d->F_max;
         if (f < 1 || f > d->F_max) return ft_set_error("waveglow: frames[b] must be in 1..F_max");
-        L->bt.frames[b] = f;
-        L->bt.mbase[b] = static_cast<int>(m);
-        L->bt.gbase[b] = static_cast<int>(g);
+        L->fr.f[b] = f;
         m += f + 3;
         g += 32LL * f + WG_GUARD;
         if (g > (1LL << 30)) return ft_set_error("waveglow: batch too long");
     }
-    L->bt.mbase[d->B] = static_cast<int>(m);
-    L->bt.gbase[d->B] = static_cast<int>(g - WG_GUARD);
     L->mrows = static_cast<int>(m);
     L->grows = static_cast<int>(g);
     size_t off = 0;
     auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 255) & ~size_t(255); return o; };
     const size_t R = static_cast<size_t>(L->grows);
+    L->off_plan = take(sizeof(WgBatch));
     L->off_mel16 = take(static_cast<size_t>(L->mrows) * WG_MEL_LD * 2);
     L->off_uprow = take(static_cast<size_t>(L->mrows) * 4);
     L->off_rowinfo = take(R * 4);
@@ -478,6 +519,23 @@ static int wg_channels(const FtWaveGlowDesc* d, int k) {
     return c;
 }
 
+// The plan (frames_dev: int32 [B] device counts, or null for the layout's host counts), then the prep over it.
+static int launch_wg_plan_prep(const WgLayout& L, const int* frames_dev, int F_max, int Tg_max, WgBatch* plan, const float* mel,
+                               __half* mel16, int* uprow, int* rowinfo, cudaStream_t st) {
+    {
+        TimeScope ts("wg_plan", L.B, F_max, frames_dev != nullptr, st);
+        wg_plan_kernel<<<1, WG_PLAN_THREADS, 0, st>>>(L.fr, frames_dev, L.B, F_max, Tg_max, plan);
+        ft_count_launch(1);
+        if (ft_check_launch("wg_plan_kernel")) return -1;
+    }
+    const long long work = static_cast<long long>(L.mrows) * (WG_MEL_LD + 1) + L.grows;
+    const int grid = static_cast<int>(std::min<long long>((work + 255) / 256, 4096));
+    TimeScope ts("wg_prep", L.mrows, L.grows, 0, st);
+    wg_prep_kernel<<<grid, 256, 0, st>>>(plan, mel, F_max, mel16, uprow, rowinfo);
+    ft_count_launch(1);
+    return ft_check_launch("wg_prep_kernel");
+}
+
 
 // ------------------------------------------------------------------------------------------------ training
 // WaveGlow.forward (glow.py:196-245, the z direction) with its saved activations, and its backward.  See DESIGN.md §4.21.
@@ -489,7 +547,7 @@ struct WtLayout {
     WgLayout g;
     int Tn, N, F, nf, nl;
     int c[FT_WG_MAX_FLOWS];                // live channels of flow k (its 1x1 conv is c x c)
-    size_t s_mel16, s_uprow, s_rowinfo, s_spect, s_x, s_skip, s_h16, s_pre, saved;
+    size_t s_plan, s_mel16, s_uprow, s_rowinfo, s_spect, s_x, s_skip, s_h16, s_pre, saved;
     size_t c_h32, c_acts, c_state, c_dstate, c_dout, c_dy, c_dskip, c_g16, c_g32, c_dx, c_dsp32, c_dsp16, c_mela, c_zero,
         c_scale, scratch;
 };
@@ -506,8 +564,7 @@ static int wt_layout(const FtWaveGlowTrainDesc* d, WtLayout* L) {
                          d->kernel_size, d->B, d->F, frames};
     if (wg_layout(&gd, &L->g)) return -1;
     L->Tn = d->N / 8; L->N = d->N; L->F = d->F; L->nf = d->n_flows; L->nl = d->n_layers;
-    L->g.Tg_max = L->Tn;
-    L->g.bt.Tg_max = L->Tn;                            // rows g >= N / 8 of an utterance are padding (rowinfo -1)
+    L->g.Tg_max = L->Tn;                               // rows g >= N / 8 of an utterance are padding (rowinfo -1)
     for (int k = 0, c = 8; k < L->nf; ++k) {
         if (k > 0 && k % d->n_early_every == 0) c -= d->n_early_size;
         L->c[k] = c;
@@ -515,6 +572,7 @@ static int wt_layout(const FtWaveGlowTrainDesc* d, WtLayout* L) {
     const size_t R = static_cast<size_t>(L->g.grows), nf = L->nf, nfl = nf * L->nl;
     size_t off = 0;
     auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 255) & ~size_t(255); return o; };
+    L->s_plan = take(sizeof(WgBatch));
     L->s_mel16 = take(static_cast<size_t>(L->g.mrows) * WG_MEL_LD * 2);
     L->s_uprow = take(static_cast<size_t>(L->g.mrows) * 4);
     L->s_rowinfo = take(R * 4);
@@ -932,8 +990,9 @@ __global__ void wg_scale_cast_kernel(const float* __restrict__ src, long long n,
 
 // The upsample GEMM's A operand, one row per 32 grid rows (one mel frame): mela[fr] = mel frames f, f-1, f-2, f-3 of the
 // utterance whose frame f starts at grid row 32 fr, zero rows between utterances; d up_w = d spect^T mela over frames.
-__global__ void wg_mela_kernel(const __grid_constant__ WgBatch bt, const int* __restrict__ rowinfo, const __half* __restrict__ mel16,
+__global__ void wg_mela_kernel(const WgBatch* __restrict__ plan, const int* __restrict__ rowinfo, const __half* __restrict__ mel16,
                                int n_fr, __half* __restrict__ mela) {
+    const WgBatch& bt = *plan;
     const long long n = static_cast<long long>(n_fr) * 4 * WG_MEL_LD;
     for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n;
          i += static_cast<long long>(gridDim.x) * blockDim.x) {
@@ -966,24 +1025,16 @@ static int wt_launch(const void* fn, const WtBwdParams& p, cudaStream_t st, cons
     return ft_check_launch(name);
 }
 
-}  // namespace ft
-
-extern "C" {
-
-size_t ft_waveglow_scratch_bytes(const FtWaveGlowDesc* d) {
-    ft::WgLayout L;
-    if (ft::wg_layout(d, &L)) return 0;
-    return L.total;
-}
-
-int ft_waveglow_infer(const FtWaveGlowDesc* d, const FtWaveGlowWeights* w, const float* mel, const float* noise, float sigma,
-                      float* audio, void* scratch, void* stream) {
-    using namespace ft;
+// frames_dev: null for d->frames (host counts), else the device counts (d->frames must then be null).  Every kernel after
+// the plan reads the layout and the live row counts from `plan`; grids and GEMM M come from L, the bound.
+static int wg_infer(const FtWaveGlowDesc* d, const FtWaveGlowWeights* w, const float* mel, const float* noise, float sigma,
+                    const int* frames_dev, float* audio, void* scratch, void* stream) {
     WgLayout L;
     if (wg_layout(d, &L)) return -1;
     if (!w || !mel || !noise || !audio || !scratch) return ft_set_error("waveglow: null pointer argument");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     uint8_t* base = static_cast<uint8_t*>(scratch);
+    WgBatch* plan = reinterpret_cast<WgBatch*>(base + L.off_plan);
     __half* mel16 = reinterpret_cast<__half*>(base + L.off_mel16);
     int* uprow = reinterpret_cast<int*>(base + L.off_uprow);
     int* rowinfo = reinterpret_cast<int*>(base + L.off_rowinfo);
@@ -999,19 +1050,12 @@ int ft_waveglow_infer(const FtWaveGlowDesc* d, const FtWaveGlowWeights* w, const
     if (cudaMemsetAsync(h16, 0, static_cast<size_t>(R) * WG_C * 2, st) != cudaSuccess ||
         cudaMemsetAsync(audio, 0, sizeof(float) * static_cast<size_t>(L.B) * L.Tg_max * 8, st) != cudaSuccess)
         return ft_set_error("waveglow: memset failed");
-    {
-        const long long work = static_cast<long long>(L.mrows) * (WG_MEL_LD + 1) + R;
-        const int grid = static_cast<int>(std::min<long long>((work + 255) / 256, 4096));
-        TimeScope ts("wg_prep", L.mrows, R, 0, st);
-        wg_prep_kernel<<<grid, 256, 0, st>>>(L.bt, mel, d->F_max, mel16, uprow, rowinfo, static_cast<int>(R));
-        ft_count_launch(1);
-        if (ft_check_launch("wg_prep_kernel")) return -1;
-    }
+    if (launch_wg_plan_prep(L, frames_dev, d->F_max, L.Tg_max, plan, mel, mel16, uprow, rowinfo, st)) return -1;
     {   // upsample: frame row f = frames f-3..f (A segments shifted 0..-3) -> 32 group rows of 640 channels
         WgGemmParams p = {};
         p.M = L.mrows; p.N = WG_UP_N; p.K = 4 * WG_MEL_LD; p.nseg = 4;
         for (int j = 0; j < 4; ++j) p.seg[j] = WgSeg{mel16, L.mrows, WG_MEL_LD, -j, WG_MEL_LD};
-        p.W = static_cast<const __half*>(w->up_w); p.bias = w->up_b; p.rowmap = uprow; p.mode = WG_EPI_UP;
+        p.W = static_cast<const __half*>(w->up_w); p.bias = w->up_b; p.rowmap = uprow; p.m_live = &plan->mrows; p.mode = WG_EPI_UP;
         p.out16 = spect; p.ld16 = WG_SPECT;
         if (launch_wg_gemm(p, st)) return -1;
     }
@@ -1020,7 +1064,7 @@ int ft_waveglow_infer(const FtWaveGlowDesc* d, const FtWaveGlowWeights* w, const
     {
         const int c = wg_channels(d, nf - 1);
         WgTailParams t = {};
-        t.R = static_cast<int>(R); t.rowinfo = rowinfo; t.state = state;
+        t.R = static_cast<int>(R); t.live_rows = &plan->grows; t.rowinfo = rowinfo; t.state = state;
         t.cur = 0; t.o = 8 - c; t.nh = c / 2;
         t.inj_lo = 8 - c; t.inj_hi = 8; t.noise = noise; t.Tg_max = L.Tg_max; t.sigma = sigma;
         t.next = 1; t.o_next = 8 - c; t.nh_next = c / 2; t.start_w = w->start_w[nf - 1]; t.start_b = w->start_b[nf - 1];
@@ -1036,20 +1080,20 @@ int ft_waveglow_infer(const FtWaveGlowDesc* d, const FtWaveGlowWeights* w, const
             p.seg[1] = WgSeg{h16, R, WG_C, 0, WG_C};
             p.seg[2] = WgSeg{h16, R, WG_C, dil, WG_C};
             p.seg[3] = WgSeg{spect, R, WG_SPECT, 0, WG_SPECT};
-            p.W = static_cast<const __half*>(w->in_w[k][i]); p.bias = w->in_b[k][i]; p.rowmap = rowinfo; p.mode = WG_EPI_GATE;
-            p.out16 = acts; p.ld16 = WG_C;
+            p.W = static_cast<const __half*>(w->in_w[k][i]); p.bias = w->in_b[k][i]; p.rowmap = rowinfo; p.m_live = &plan->grows;
+            p.mode = WG_EPI_GATE; p.out16 = acts; p.ld16 = WG_C;
             if (launch_wg_gemm(p, st)) return -1;
             WgGemmParams q = {};
             const bool last = i == nl - 1;
             q.M = static_cast<int>(R); q.N = last ? WG_C : 2 * WG_C; q.K = WG_C; q.nseg = 1;
             q.seg[0] = WgSeg{acts, R, WG_C, 0, WG_C};
-            q.W = static_cast<const __half*>(w->rs_w[k][i]); q.bias = w->rs_b[k][i]; q.rowmap = rowinfo; q.mode = WG_EPI_RES;
-            q.h32 = h32; q.h16 = h16; q.skip32 = skip; q.res_cols = last ? 0 : WG_C; q.skip_store = i == 0;
+            q.W = static_cast<const __half*>(w->rs_w[k][i]); q.bias = w->rs_b[k][i]; q.rowmap = rowinfo; q.m_live = &plan->grows;
+            q.mode = WG_EPI_RES; q.h32 = h32; q.h16 = h16; q.skip32 = skip; q.res_cols = last ? 0 : WG_C; q.skip_store = i == 0;
             if (launch_wg_gemm(q, st)) return -1;
         }
         const int c = wg_channels(d, k);
         WgTailParams t = {};
-        t.R = static_cast<int>(R); t.rowinfo = rowinfo; t.state = state;
+        t.R = static_cast<int>(R); t.live_rows = &plan->grows; t.rowinfo = rowinfo; t.state = state;
         t.cur = 1; t.o = 8 - c; t.nh = c / 2;
         t.skip32 = skip; t.end_w = w->end_w[k]; t.end_b = w->end_b[k]; t.inv_w = w->inv_w[k];
         const bool inject = k > 0 && k % d->n_early_every == 0 && d->n_early_size > 0;
@@ -1065,6 +1109,29 @@ int ft_waveglow_infer(const FtWaveGlowDesc* d, const FtWaveGlowWeights* w, const
         if (launch_wg_tail(t, st)) return -1;
     }
     return 0;
+}
+
+}  // namespace ft
+
+extern "C" {
+
+size_t ft_waveglow_scratch_bytes(const FtWaveGlowDesc* d) {
+    ft::WgLayout L;
+    if (ft::wg_layout(d, &L)) return 0;
+    return L.total;
+}
+
+int ft_waveglow_infer(const FtWaveGlowDesc* d, const FtWaveGlowWeights* w, const float* mel, const float* noise, float sigma,
+                      float* audio, void* scratch, void* stream) {
+    if (d && !d->frames) return ft::ft_set_error("waveglow: frames (host array) required; ft_waveglow_infer_dev takes device frames");
+    return ft::wg_infer(d, w, mel, noise, sigma, nullptr, audio, scratch, stream);
+}
+
+int ft_waveglow_infer_dev(const FtWaveGlowDesc* d, const FtWaveGlowWeights* w, const float* mel, const float* noise, float sigma,
+                          const int* frames_dev, float* audio, void* scratch, void* stream) {
+    if (d && d->frames) return ft::ft_set_error("waveglow: ft_waveglow_infer_dev takes desc->frames == NULL");
+    if (!frames_dev) return ft::ft_set_error("waveglow: null frames_dev");
+    return ft::wg_infer(d, w, mel, noise, sigma, frames_dev, audio, scratch, stream);
 }
 
 size_t ft_waveglow_train_saved_bytes(const FtWaveGlowTrainDesc* d) {
@@ -1107,14 +1174,8 @@ int ft_waveglow_train_fwd(const FtWaveGlowTrainDesc* d, const FtWaveGlowTrainWei
     if (cudaMemsetAsync(h16, 0, static_cast<size_t>(L.nf) * L.nl * R * WG_C * 2, st) != cudaSuccess ||
         cudaMemsetAsync(spect, 0, static_cast<size_t>(R) * WG_SPECT * 2, st) != cudaSuccess)
         return ft_set_error("waveglow train: memset failed");
-    {
-        const long long work = static_cast<long long>(L.g.mrows) * (WG_MEL_LD + 1) + R;
-        const int grid = static_cast<int>(std::min<long long>((work + 255) / 256, 4096));
-        TimeScope ts("wg_prep", L.g.mrows, R, 0, st);
-        wg_prep_kernel<<<grid, 256, 0, st>>>(L.g.bt, mel, L.F, mel16, uprow, rowinfo, static_cast<int>(R));
-        ft_count_launch(1);
-        if (ft_check_launch("wg_prep_kernel")) return -1;
-    }
+    if (launch_wg_plan_prep(L.g, nullptr, L.F, L.Tn, reinterpret_cast<WgBatch*>(sv + L.s_plan), mel, mel16, uprow, rowinfo, st))
+        return -1;
     {
         WgGemmParams p = {};
         p.M = L.g.mrows; p.N = WG_UP_N; p.K = 4 * WG_MEL_LD; p.nseg = 4;
@@ -1283,7 +1344,7 @@ int ft_waveglow_train_bwd(const FtWaveGlowTrainDesc* d, const FtWaveGlowTrainWei
         TimeScope ts("wg_train_up_prep", nfr, 0, 0, st);
         wg_scale_cast_kernel<<<static_cast<int>(std::min<long long>((nsp + 255) / 256, 4096)), 256, 0, st>>>(dsp32, nsp, sup, dsp16);
         wg_mela_kernel<<<static_cast<int>(std::min<long long>((nfr * 384 + 255) / 256, 4096)), 256, 0, st>>>(
-            L.g.bt, rowinfo, mel16, static_cast<int>(nfr), mela);
+            reinterpret_cast<const WgBatch*>(sv + L.s_plan), rowinfo, mel16, static_cast<int>(nfr), mela);
         ft_count_launch(2);
         if (ft_check_launch("wg_train_up_prep")) return -1;
     }

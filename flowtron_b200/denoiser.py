@@ -36,9 +36,14 @@ class Denoiser(torch.nn.Module):
 
     def forward(self, audio, strength=0.1, *, lengths=None):
         """audio [B, N] -> [B, 1, (N // hop) * hop], denoised as the reference does: magnitude max(m - strength * bias, 0),
-        phase kept.  lengths: optional host sequence of per-row sample counts (e.g. 256 * frames from
-        WaveGlow.infer(lengths=)); row b is then the B = 1 result on audio[b, :lengths[b]] and zero after
-        (lengths[b] // hop) * hop samples."""
+        phase kept.  lengths: optional per-row sample counts (e.g. 256 * frames from WaveGlow.infer(lengths=)); row b is
+        then the B = 1 result on audio[b, :lengths[b]] and zero after (lengths[b] // hop) * hop samples.
+
+        Short rows: the reflect padding needs more than n_fft / 2 samples, so a B = 1 call on at most n_fft / 2 samples
+        raises ValueError, and so do host lengths (a sequence or CPU tensor) with such a row or a count above N.  A CUDA
+        tensor of lengths (int32 or int64, shape [B]) is planned on the device with no host synchronisation, so the call
+        can be captured in a CUDA graph and replayed with new lengths; only its shape and dtype are checked, a row of at
+        most n_fft / 2 samples (fewer than 3 WaveGlow frames) comes out all zero, and counts above N are taken as N."""
         stft = self.stft
         n_fft, hop = stft.filter_length, stft.hop_length
         if n_fft != 1024 or hop not in _lib.STFT_INVERSE_HOPS:
@@ -61,15 +66,24 @@ class Denoiser(torch.nn.Module):
             total = B * F
             out = torch.empty(B, 1, n_out, device=dev)
         else:
-            lens = np.asarray([int(n) for n in (lengths.tolist() if torch.is_tensor(lengths) else lengths)], dtype=np.int64)
-            if len(lens) != B or lens.min() <= n_fft // 2 or lens.max() > N:
-                raise ValueError(f"lengths must hold {B} sample counts in {n_fft // 2 + 1}..{N}, got {lens.tolist()}")
-            flat = torch.cat([audio[b, :lens[b]] for b in range(B)]) if B > 1 else audio[0, :lens[0]].contiguous()
-            so_h = np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)
-            fo_h = np.concatenate([[0], np.cumsum(1 + lens // hop)]).astype(np.int64)
-            so = torch.from_numpy(so_h).to(dev, non_blocking=True)
-            fo = torch.from_numpy(fo_h).to(dev, non_blocking=True)
-            total = int(fo_h[-1])
+            if torch.is_tensor(lengths) and lengths.is_cuda:
+                if tuple(lengths.shape) != (B,) or lengths.dtype not in (torch.int32, torch.int64):
+                    raise ValueError(f"CUDA lengths must be int32 or int64 of shape ({B},), got {lengths.dtype} "
+                                     f"{tuple(lengths.shape)}")
+                if lengths.device != dev:
+                    raise ValueError(f"lengths are on {lengths.device}, audio on {dev}")
+                lens_d = lengths.to(torch.int64).contiguous()
+                n_samples, total = B * N, B * (1 + N // hop)         # bounds: the true totals are planned on the device
+            else:
+                lens = np.asarray([int(n) for n in (lengths.tolist() if torch.is_tensor(lengths) else lengths)], dtype=np.int64)
+                if len(lens) != B or lens.min() <= n_fft // 2 or lens.max() > N:
+                    raise ValueError(f"lengths must hold {B} sample counts in {n_fft // 2 + 1}..{N}, got {lens.tolist()}")
+                lens_d = torch.from_numpy(lens).to(dev, non_blocking=True)
+                n_samples, total = int(lens.sum()), int((1 + lens // hop).sum())
+            flat = torch.empty(n_samples, device=dev)
+            so = torch.empty(B + 1, device=dev, dtype=torch.int64)
+            fo = torch.empty_like(so)
+            _lib.stft_pack_rows(audio.contiguous(), lens_d, n_fft, hop, flat, so, fo)
             out = torch.zeros(B, 1, n_out, device=dev)
         flat = aligned_waveform(flat)
         oo = torch.arange(B, device=dev, dtype=torch.int64) * n_out

@@ -322,14 +322,26 @@ class WaveGlow(torch.nn.Module):
         """spect [B, 80, F] log-mel -> audio [B, 256 F] (WaveGlow.infer, glow.py:251-293).
         noise: optional [B, 8, 32 F] in the channel order of WaveGlow.forward's z (for the shipped config: 0:2 injected
         after flow 4, 2:4 after flow 8, 4:8 the initial draw), multiplied by sigma; None draws it on the current CUDA
-        generator in the reference's order.  lengths: optional host sequence of per-row frame counts; row b is then the
-        B=1 result on spect[b, :, :lengths[b]] and zero after 256 lengths[b] samples."""
+        generator in the reference's order.  lengths: optional per-row frame counts; row b is then the B=1 result on
+        spect[b, :, :lengths[b]] and zero after 256 lengths[b] samples.  A host sequence or CPU tensor is range-checked
+        (ValueError unless every count is in 1..F).  A CUDA tensor (int32 or int64, shape [B], e.g. infer_batch's
+        mel_lens) is used in place with no host synchronisation, so the call can be captured in a CUDA graph and replayed
+        with new lengths; only its shape and dtype are checked, and a count outside 1..F gives an unspecified row (it is
+        clamped, never read past the inputs)."""
         if spect.dim() != 3 or spect.shape[1] != self.n_mel_channels:
             raise ValueError(f"spect must be [B, {self.n_mel_channels}, F], got {tuple(spect.shape)}")
         B, _, Fr = spect.shape
         Tg = 32 * Fr
+        frames_dev = None
         if lengths is None:
             frames = [Fr] * B
+        elif torch.is_tensor(lengths) and lengths.is_cuda:
+            if tuple(lengths.shape) != (B,) or lengths.dtype not in (torch.int32, torch.int64):
+                raise ValueError(f"CUDA lengths must be int32 or int64 of shape ({B},), got {lengths.dtype} "
+                                 f"{tuple(lengths.shape)}")
+            if lengths.device != spect.device:
+                raise ValueError(f"lengths are on {lengths.device}, spect on {spect.device}")
+            frames, frames_dev = None, lengths.to(torch.int32).contiguous()
         else:
             frames = [int(n) for n in (lengths.tolist() if torch.is_tensor(lengths) else lengths)]
             if len(frames) != B or any(n < 1 or n > Fr for n in frames):
@@ -345,12 +357,12 @@ class WaveGlow(torch.nn.Module):
         mel = spect.detach().float().contiguous()
         noise = noise.detach().float().contiguous()
         audio = torch.empty(B, 256 * Fr, device=spect.device, dtype=torch.float32)
-        fr = (c_int * B)(*frames)
+        fr = None if frames is None else (c_int * B)(*frames)
         desc = _lib.FtWaveGlowDesc(n_mel=self.n_mel_channels, n_flows=self.n_flows, n_group=self.n_group,
                                    n_early_every=self.n_early_every, n_early_size=self.n_early_size,
                                    n_layers=self.WN_config["n_layers"], n_channels=self.WN_config["n_channels"],
                                    kernel_size=self.WN_config["kernel_size"], B=B, F_max=Fr, frames=fr)
-        _lib.waveglow_infer(desc, w, mel, noise, float(sigma), audio)
+        _lib.waveglow_infer(desc, w, mel, noise, float(sigma), audio, frames_dev)
         return audio
 
 

@@ -237,10 +237,20 @@ int ft_mel_spectrogram_fused(const void* wav, int wav_fmt, const long long* samp
                              const int* band_hi, int n_mel, int n_fft, int hop, float clip, float* mel_out, void* stream);
 
 /* STFT.transform (audio_processing.py:207-235), n_fft == 1024: magnitude and phase (atan2(imag, real)) as per-utterance
- * [n_fft/2+1, F_u] blocks (== [B, 513, F] for equal lengths), same kernel as above without the filterbank. */
+ * [n_fft/2+1, F_u] blocks (== [B, 513, F] for equal lengths), same kernel as above without the filterbank.  total_frames
+ * is a host upper bound that sizes the grid; the kernel reads the true total from frame_offsets[n_utt] in device memory,
+ * so offsets planned on the device (ft_stft_pack_rows) need no host round trip. */
 int ft_stft_transform(const float* wav, const long long* sample_offsets, const long long* frame_offsets, int n_utt,
                       long long total_frames, const float* window, int n_fft, int hop, float* magnitude, float* phase,
                       void* stream);
+
+/* Packs the rows of a padded batch audio [B, N] fp32 into the layout ft_stft_transform reads, from per-row sample counts
+ * in device memory (lengths int64 [B]): row b's first min(lengths[b], N) samples go to packed[sample_offsets[b]], and
+ * sample_offsets / frame_offsets (int64 [B + 1] each, written) are their prefix sums and those of 1 + n / hop frames.  A
+ * row of at most n_fft / 2 samples (the reflect padding) is empty: no samples, no frames.  packed holds at most B * N
+ * floats and the frames total at most B * (1 + N / hop).  One launch, no host synchronisation. */
+int ft_stft_pack_rows(const float* audio, int B, long long N, const long long* lengths, int n_fft, int hop, float* packed,
+                      long long* sample_offsets, long long* frame_offsets, void* stream);
 
 /* STFT.inverse (audio_processing.py:237-265), n_fft == 1024, hop in {128, 256, 512}: magnitude / phase as per-utterance
  * [513, F_u] blocks at frame_offsets[u] (prefix sums, n_utt + 1 entries, the layout ft_stft_transform writes) ->
@@ -249,7 +259,8 @@ int ft_stft_transform(const float* wav, const long long* sample_offsets, const l
  * 1024 floats), overlap-added, divided by the window's sum-square envelope where it exceeds FLT_MIN, and 512 samples
  * are dropped at each end.  bias (513 floats, optional): the magnitude becomes max(m - strength * bias[k], 0) on load
  * (tacotron2/waveglow/denoiser.py), so transform + inverse is the whole Denoiser.  One launch, deterministic (each
- * sample sums its frames in utterance-local order: ragged rows equal B = 1 runs), no host sync. */
+ * sample sums its frames in utterance-local order: ragged rows equal B = 1 runs), no host sync.  total_frames is a host
+ * upper bound, the true total is frame_offsets[n_utt], as for ft_stft_transform. */
 int ft_stft_inverse(const float* magnitude, const float* phase, const long long* frame_offsets, const long long* out_offsets,
                     int n_utt, long long total_frames, const float* window, int n_fft, int hop, const float* bias,
                     float strength, float* out, void* stream);
@@ -400,7 +411,8 @@ typedef struct {
     int n_layers, n_channels, kernel_size;                      /* WN_config: 8, 256, 3                           */
     int B;                                                      /* utterances (1..128)                            */
     int F_max;                                                  /* padded mel frames of `mel`                     */
-    const int* frames;                                          /* HOST int[B]: frames of utterance b (1..F_max)  */
+    const int* frames;                                          /* host int[B]: frames of utterance b (1..F_max), */
+                                                                /* or NULL for ft_waveglow_infer_dev              */
 } FtWaveGlowDesc;
 
 /* Device pointers to the packed weights of WaveGlow (flowtron_b200/waveglow.py packs them once per weight version):
@@ -419,14 +431,25 @@ typedef struct {
     const float* inv_w[FT_WG_MAX_FLOWS];
 } FtWaveGlowWeights;
 
-/* Bytes of the caller-owned scratch of ft_waveglow_infer (0 if the descriptor is rejected). */
+/* Bytes of the caller-owned scratch of ft_waveglow_infer (0 if the descriptor is rejected).  With d->frames == NULL: the
+ * scratch of ft_waveglow_infer_dev, sized for every utterance at F_max. */
 size_t ft_waveglow_scratch_bytes(const FtWaveGlowDesc* d);
 /* mel fp32 [B, 80, F_max]; noise fp32 [B, 8, 32 F_max]: channels of WaveGlow.forward's z -- the first flow's draw on the
  * highest channels (4:8 for the shipped config), each early injection on the channels just below (2:4 after flow 8, 0:2
  * after flow 4); it is multiplied by sigma.  audio fp32 [B, 256 F_max]: utterance b fills its first 256 frames[b] samples,
- * the rest is zero.  About n_flows * (2 n_layers + 1) + 3 launches, no host synchronisation (CUDA-graph capturable). */
+ * the rest is zero.  A planner kernel lays the batch out in scratch from the frame counts (passed to it by value), and the
+ * other kernels read that layout from device memory.  n_flows * (2 n_layers + 1) + 4 launches, no host synchronisation
+ * (CUDA-graph capturable). */
 int ft_waveglow_infer(const FtWaveGlowDesc* d, const FtWaveGlowWeights* w, const float* mel, const float* noise, float sigma,
                       float* audio, void* scratch, void* stream);
+/* ft_waveglow_infer with the frame counts in device memory: frames_dev int32 [B], read only by the planner kernel, so a
+ * CUDA graph captured once replays with whatever counts the buffer holds.  d->frames must be NULL and the scratch is
+ * ft_waveglow_scratch_bytes(d) for that descriptor.  Grids and GEMM rows are sized for every utterance at F_max; tiles and
+ * rows past the planned layout exit at once.  Each count is clamped to 1..F_max, so no value makes a kernel address past
+ * mel, noise, audio or the scratch; counts outside 1..F_max give an unspecified row.  Rows equal ft_waveglow_infer's with
+ * the same counts bit for bit.  Same launches, no host synchronisation. */
+int ft_waveglow_infer_dev(const FtWaveGlowDesc* d, const FtWaveGlowWeights* w, const float* mel, const float* noise, float sigma,
+                          const int* frames_dev, float* audio, void* scratch, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------
  * WaveGlow training (glow.py:196-245 WaveGlow.forward, the z direction) and its backward, same configurations as infer.

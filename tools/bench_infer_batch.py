@@ -9,6 +9,11 @@ Workloads (fixed seed; 2-flow model at the shipped sizes; gate bias -10 so the g
       runs (checked against the 2e-3 bound of the tests).
   W2  W1's batch, then WaveGlow.infer(lengths=) and the Denoiser (strength 0.1), against 16 sequential B = 1 chains.
       Reported: ms per batch and seconds of 22050 Hz audio per wall-clock second.
+  W2G W2 as a serving loop: infer_batch -> WaveGlow.infer(lengths=mel_lens) -> Denoiser(lengths=256 mel_lens) captured
+      ONCE as one CUDA graph on static buffers (B = 16, T = 1000, L = 160, CUDA lengths), then replayed on fresh
+      residuals, texts, noise and length sets (in_lens U{40..160}, budgets as W1's), each copied into the buffers from
+      device memory before its replay.  The first request is checked bit for bit against eager calls with host lengths.
+      Reported beside eager W2 (which reads mel_lens on the host): ms per request and audio seconds per second.
 
 Times come from CUDA events around work that ends in a device synchronise, after warming up every shape; each workload
 is repeated --reps times, alternating batched and sequential.  The card name and power limit are read in the same run.
@@ -48,11 +53,75 @@ def w1_batch(dev, B=16, seed=2026):
     return res, spk, text, in_lens.tolist(), budgets.tolist()
 
 
+def serving_graph(model, wg, den, dev, B, T=1000, L=160, n_requests=4, seed=77):
+    """Captures the text-to-audio chain once on static buffers with CUDA lengths; returns run(iters) -> (ms per request,
+    mean audio seconds per request), which replays it over the requests round-robin."""
+    g = torch.Generator().manual_seed(seed)
+    reqs = []
+    for _ in range(n_requests):
+        in_lens = torch.randint(40, L + 1, (B,), generator=g)
+        budgets = torch.clamp(torch.round(6.5 * in_lens.double()).long(), 150, T)
+        reqs.append(dict(res=(torch.randn(B, 80, T, generator=g) * 0.5).to(dev), text=torch.randint(0, 185, (B, L), generator=g).to(dev),
+                         in_lens=in_lens.to(dev), budgets=budgets.to(dev), noise=torch.randn(B, 8, 32 * T, generator=g).to(dev),
+                         frames=int(budgets.sum())))
+    buf = {k: torch.empty_like(v) for k, v in reqs[0].items() if torch.is_tensor(v)}
+    spk = torch.zeros(B, dtype=torch.long, device=dev)
+
+    def load(r):
+        for k, v in buf.items():
+            v.copy_(r[k])
+
+    def chain():
+        mel, mel_lens, _ = model.infer_batch(buf["res"], spk, buf["text"], buf["in_lens"], max_frames=buf["budgets"])
+        audio = wg.infer(mel, sigma=0.6, noise=buf["noise"], lengths=mel_lens)
+        return mel_lens, audio, den(audio, 0.1, lengths=HOP * mel_lens)
+
+    load(reqs[0])
+    s = torch.cuda.Stream()
+    s.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(s):
+        for _ in range(2):
+            chain()
+    torch.cuda.current_stream().wait_stream(s)
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(graph, stream=s):
+        outs = chain()
+    # the first request against eager calls with host lengths, bit for bit
+    load(reqs[1])
+    graph.replay()
+    torch.cuda.synchronize()
+    r = reqs[1]
+    mel_e, lens_e, _ = model.infer_batch(r["res"], spk, r["text"], r["in_lens"].tolist(), max_frames=r["budgets"].tolist())
+    n = lens_e.tolist()
+    audio_e = wg.infer(mel_e, sigma=0.6, noise=r["noise"], lengths=n)
+    clean_e = den(audio_e, 0.1, lengths=[HOP * f for f in n])
+    assert torch.equal(outs[0], lens_e) and torch.equal(outs[1], audio_e) and torch.equal(outs[2], clean_e)
+    assert _lib.device_status() == 0
+
+    def run(iters):
+        for r in reqs:                                            # warm-up over every request
+            load(r)
+            graph.replay()
+        torch.cuda.synchronize()
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        for i in range(iters):
+            load(reqs[i % n_requests])
+            graph.replay()
+        b.record()
+        torch.cuda.synchronize()
+        frames = sum(reqs[i % n_requests]["frames"] for i in range(iters)) / iters
+        return a.elapsed_time(b) / iters, HOP * frames / SR
+
+    run.static = (spk, s, outs)                                   # the graph reads and writes these: keep them alive
+    return run
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--iters", type=int, default=3)
-    ap.add_argument("--workloads", default="W1,W2")
+    ap.add_argument("--workloads", default="W1,W2,W2G")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_infer_batch.py needs a CUDA device")
@@ -90,7 +159,7 @@ def main():
                 power_limit_w=plim)
 
     wg = den = None
-    if "W2" in args.workloads:
+    if "W2" in args.workloads:                               # W2 and W2G
         wcfg = synth.DEFAULT_WAVEGLOW_CONFIG
         wg = WaveGlow(**wcfg)
         wg.load_state_dict(synth.synth_waveglow_params(wcfg, 1234), strict=True)
@@ -110,6 +179,8 @@ def main():
             out.append(den(wg.infer(m1.contiguous(), sigma=0.6), 0.1))
         return out
 
+    serve = serving_graph(model, wg, den, dev, B) if "W2G" in args.workloads.split(",") else None
+
     for wl in args.workloads.split(","):
         runs = []
         for rep in range(args.reps):
@@ -128,6 +199,13 @@ def main():
                 rec = dict(workload="W2_text_to_audio", rep=rep, batched_ms=round(bat, 2), sequential_b1_ms=round(seq, 2),
                            audio_s=round(audio_s, 2), audio_s_per_s_batched=round(audio_s / (bat / 1e3), 1),
                            audio_s_per_s_sequential=round(audio_s / (seq / 1e3), 1), speedup=round(seq / bat, 2))
+            elif wl == "W2G":
+                bat = time_eager(chain_batched, 1, args.iters)
+                graph_ms, audio_s = serve(args.iters)
+                rec = dict(workload="W2G_text_to_audio_graph", rep=rep, graph_ms_per_request=round(graph_ms, 2),
+                           eager_w2_ms=round(bat, 2), audio_s_per_request=round(audio_s, 2),
+                           audio_s_per_s_graph=round(audio_s / (graph_ms / 1e3), 1),
+                           audio_s_per_s_eager_w2=round(HOP * frames / SR / (bat / 1e3), 1))
             else:
                 raise SystemExit(f"unknown workload {wl}")
             assert _lib.device_status() == 0
