@@ -23,7 +23,7 @@ _lib = None
 class FtArStepDesc(Structure):
     _fields_ = [("T", c_int), ("B", c_int), ("L", c_int), ("n_mel", c_int), ("n_hidden", c_int), ("n_attn", c_int),
                 ("n_text", c_int), ("reversed", c_int), ("has_gate", c_int), ("has_prior", c_int),
-                ("temperature", c_float)]
+                ("temperature", c_float), ("no_d_mel", c_int)]
 
 
 AR_WEIGHT_FIELDS = ["attn_lstm_w_ih", "attn_lstm_w_hh", "attn_lstm_b_ih", "attn_lstm_b_hh",
@@ -179,6 +179,8 @@ def _declare(L):
     L.ft_ar_step_bwd_attn_lstm.argtypes = [POINTER(FtArStepDesc), POINTER(FtArStepWeights), c_void_p, c_void_p,
                                            POINTER(FtArStepWeights), c_void_p, c_void_p, c_void_p, c_void_p]
     L.ft_ar_step_bwd_attn_lstm.restype = c_int
+    L.ft_ar_step_bwd_plan.argtypes = [POINTER(FtArStepDesc), POINTER(FtArStepWeights), c_int, c_int, POINTER(ctypes.c_uint)]
+    L.ft_ar_step_bwd_plan.restype = c_int
     L.ft_ar_step_infer_scratch_bytes.argtypes = [POINTER(FtArStepDesc)]
     L.ft_ar_step_infer_scratch_bytes.restype = c_size_t
     L.ft_ar_step_infer.argtypes = [POINTER(FtArStepDesc), POINTER(FtArStepWeights)] + [c_void_p] * 6 + \
@@ -452,6 +454,25 @@ def ar_step_bwd_main(desc, weights, mel, in_lens, out_lens, attn, d_mel_out, d_l
     check(lib().ft_ar_step_bwd_main(byref(desc), byref(weights), ptr(mel), ptr(in_lens), ptr(out_lens), ptr(attn), ptr(d_mel_out),
                                     ptr(d_log_s), ptr(d_gates), ptr(d_attn), ptr(d_logprob), ptr(d_text), byref(grads), ptr(saved),
                                     ptr(scratch), ptr(carry), stream_ptr()), "ft_ar_step_bwd_main")
+
+
+# Stage bits of ft_ar_step_bwd_plan (include/flowtron_b200.h)
+BWD_STAGES = {"COUPLING": 0, "CONV_DGRAD": 1, "DENSE1_DGRAD": 2, "DENSE0_DGRAD": 3, "LSTM1": 4, "LSTM0": 5, "GATE_DD": 6,
+              "ATTN": 7, "QUERY_DGRAD": 8, "D_TEXT": 9, "ATTN_LSTM": 10, "D_MEL": 11, "G_CONV": 16, "G_DENSE1": 17,
+              "G_DENSE0": 18, "G_LSTM1": 19, "G_LSTM0": 20, "G_QUERY": 21, "G_KEY": 22, "G_VALUE": 23, "G_V": 24,
+              "G_ATTN_LSTM": 25, "G_GATE": 26}
+
+
+def ar_step_bwd_plan(desc, want, want_d_text: bool, want_d_mel: bool) -> set:
+    """Names of the backward stages ft_ar_step_bwd_main / ft_ar_step_bwd_attn_lstm run when the parameter gradients with
+    a true entry in `want` (24 flags in AR_WEIGHT_FIELDS order) and d_text / d_mel as given are wanted.  Host only: the
+    non-NULL gradient pointers are never dereferenced."""
+    g = FtArStepWeights()
+    for name, w in zip(AR_WEIGHT_FIELDS, want):
+        setattr(g, name, 1 if w else None)
+    m = ctypes.c_uint(0)
+    check(lib().ft_ar_step_bwd_plan(byref(desc), byref(g), int(want_d_text), int(want_d_mel), byref(m)), "ft_ar_step_bwd_plan")
+    return {k for k, b in BWD_STAGES.items() if m.value >> b & 1}
 
 
 def ar_step_bwd_attn_lstm(desc, weights, out_lens, d_mel, grads, saved, scratch, carry):

@@ -8,6 +8,7 @@
 // multiplied by a per-flow power-of-two loss scale chosen on the device (launch_grad_scale); accumulation, LSTM cell state, softmax, exp/log and all reductions are fp32.
 #include <algorithm>
 #include <cstring>
+#include <initializer_list>
 #include <map>
 #include <mutex>
 #include <string>
@@ -146,6 +147,7 @@ struct BwdScratch {
     float *dcarry1, *dcarry0;   // dc*f hand-over between BPTT chunks of the layer pipeline
     float *xchg1, *xchg0;       // partial-sum rings of the two pipelined BPTT recurrences (flat kernel, lstm.cu)
     float* attn_rows = nullptr; // long texts: the attention backward's gradient rows (attn_rows_in_global)
+    float* sink;
     void plan(Plan& p, const FtArStepDesc& d) {
         const Dims n(d);
         w.plan(p, n);
@@ -171,8 +173,45 @@ struct BwdScratch {
         xchg1 = p.get<float>("xchg1", static_cast<size_t>(kBwdXchgPerRow) * n.B);
         xchg0 = p.get<float>("xchg0", static_cast<size_t>(kBwdXchgPerRow) * n.B);
         if (attn_rows_in_global(n.L, n.A)) attn_rows = p.get<float>("attn_rows", attn_rows_floats(n.T, n.B, n.L));
+        // target of the gradients the attention / gate kernels always accumulate but the caller may not want (v, and one
+        // of the gate's weight / bias); never read
+        sink = p.get<float>("sink", static_cast<size_t>(n.A) + n.D + 1);
     }
 };
+
+// The dependency rule of the backward (ft_ar_step_bwd_plan in flowtron_b200.h): one bit per stage, set when something
+// downstream of the stage is wanted.  The two backward entry points branch on this mask only.
+unsigned bwd_plan(const FtArStepDesc& d, const FtArStepWeights& g, bool want_d_text, bool want_d_mel) {
+    auto any = [](std::initializer_list<const float*> ps) {
+        for (const float* q : ps) if (q) return true;
+        return false;
+    };
+    unsigned m = 0;
+    if (any({g.conv_w, g.conv_b})) m |= FT_BWD_G_CONV;
+    if (any({g.dense_w1, g.dense_b1})) m |= FT_BWD_G_DENSE1;
+    if (any({g.dense_w0, g.dense_b0})) m |= FT_BWD_G_DENSE0;
+    if (any({g.lstm_w_ih1, g.lstm_w_hh1, g.lstm_b_ih1, g.lstm_b_hh1})) m |= FT_BWD_G_LSTM1;
+    if (any({g.lstm_w_ih0, g.lstm_w_hh0, g.lstm_b_ih0, g.lstm_b_hh0})) m |= FT_BWD_G_LSTM0;
+    if (g.att_query) m |= FT_BWD_G_QUERY;
+    if (g.att_key) m |= FT_BWD_G_KEY;
+    if (g.att_value) m |= FT_BWD_G_VALUE;
+    if (g.att_v) m |= FT_BWD_G_V;
+    if (any({g.attn_lstm_w_ih, g.attn_lstm_w_hh, g.attn_lstm_b_ih, g.attn_lstm_b_hh})) m |= FT_BWD_G_ATTN_LSTM;
+    if (d.has_gate && any({g.gate_w, g.gate_b})) m |= FT_BWD_G_GATE;
+    if (want_d_mel) m |= FT_BWD_D_MEL;
+    if (m & (FT_BWD_D_MEL | FT_BWD_G_ATTN_LSTM)) m |= FT_BWD_ATTN_LSTM;
+    if (m & FT_BWD_ATTN_LSTM) m |= FT_BWD_QUERY_DGRAD;
+    if (want_d_text) m |= FT_BWD_D_TEXT;
+    if (m & (FT_BWD_QUERY_DGRAD | FT_BWD_D_TEXT | FT_BWD_G_QUERY | FT_BWD_G_KEY | FT_BWD_G_VALUE | FT_BWD_G_V)) m |= FT_BWD_ATTN;
+    if (d.has_gate && (m & (FT_BWD_ATTN | FT_BWD_ATTN_LSTM))) m |= FT_BWD_GATE_DD;
+    if (m & (FT_BWD_ATTN | FT_BWD_ATTN_LSTM | FT_BWD_G_LSTM0)) m |= FT_BWD_LSTM0;
+    if (m & (FT_BWD_LSTM0 | FT_BWD_G_LSTM1)) m |= FT_BWD_LSTM1;
+    if (m & FT_BWD_LSTM1) m |= FT_BWD_DENSE0_DGRAD;
+    if (m & (FT_BWD_DENSE0_DGRAD | FT_BWD_G_DENSE0)) m |= FT_BWD_DENSE1_DGRAD;
+    if (m & (FT_BWD_DENSE1_DGRAD | FT_BWD_G_DENSE1)) m |= FT_BWD_CONV_DGRAD;
+    if (m & (FT_BWD_CONV_DGRAD | FT_BWD_G_CONV | FT_BWD_D_MEL)) m |= FT_BWD_COUPLING;
+    return m;
+}
 
 int check_desc(const FtArStepDesc& d) {
     if (d.n_hidden != H) return ft_set_error("ar_step: this build supports n_hidden == 1024 only");
@@ -434,14 +473,24 @@ int ar_step_fwd(const FtArStepDesc& d, const FtArStepWeights& w, const float* me
 }
 
 // =================================================================================================== backward
+// The gradient of both LSTM biases is the column sum of dG: one column sum into whichever of the two is wanted, copied to
+// the other when both are.
+static int lstm_bias_grads(const uint16_t* dG, long long R, float* db_ih, float* db_hh, const float* iS, cudaStream_t st) {
+    float* first = db_ih ? db_ih : db_hh;
+    if (first) FT_TRY(launch_colsum(dG, 0, G, R, G, first, iS, st));
+    if (db_ih && db_hh) FT_TRY(copy_f32(db_hh, db_ih, G, st));
+    return 0;
+}
+
 // Main part: everything except the attention LSTM.  Outputs d_text and every parameter gradient but attention_lstm's; leaves
-// dhA / dmel_flow / the loss scale in `carry` for ar_step_bwd_attn.
+// dhA / dmel_flow / the loss scale in `carry` for ar_step_bwd_attn.  Runs the stages of bwd_plan only.
 int ar_step_bwd_main(const FtArStepDesc& d, const FtArStepWeights& w, const float* mel, const int* in_lens, const int* out_lens,
                      const float* attn, const float* d_mel_out, const float* d_log_s, const float* d_gates, const float* d_attn,
                      const float* d_logprob, float* d_text, const FtArStepWeights& g, void* saved, void* scratch, void* carry,
                      cudaStream_t st) {
     FT_TRY(check_desc(d));
     const Dims n(d);
+    const unsigned m = bwd_plan(d, g, d_text != nullptr, !d.no_d_mel);
     Plan ps; ps.base = static_cast<uint8_t*>(saved);
     Saved S_; S_.plan(ps, d);
     Plan pb; pb.base = static_cast<uint8_t*>(scratch);
@@ -452,22 +501,23 @@ int ar_step_bwd_main(const FtArStepDesc& d, const FtArStepWeights& w, const floa
     const long long R = n.R, RL = n.RL, Rm = n.R - n.B;     // Rm: rows with a predecessor step
 
     // fp16 operand copies: natural layouts for dgrad (B operand MN-major), transposed recurrent weights for BPTT
-    FT_TRY(launch_cast(w.lstm_w_ih0, 2, F.w.w_ih0, 0, static_cast<long long>(G) * n.D, st));
-    FT_TRY(launch_cast(w.lstm_w_ih1, 2, F.w.w_ih1, 0, static_cast<long long>(G) * H, st));
-    FT_TRY(launch_cast(w.att_query, 2, F.w.wq, 0, static_cast<long long>(n.A) * H, st));
-    FT_TRY(launch_cast(w.att_key, 2, F.w.wk, 0, static_cast<long long>(n.A) * n.E, st));
-    FT_TRY(launch_cast(w.att_value, 2, F.w.wv, 0, static_cast<long long>(n.A) * n.E, st));
-    FT_TRY(launch_cast(w.dense_w0, 2, F.w.w1, 0, static_cast<long long>(H) * H, st));
-    FT_TRY(launch_cast(w.dense_w1, 2, F.w.w2, 0, static_cast<long long>(H) * H, st));
-    FT_TRY(launch_cast(w.conv_w, 2, F.w.wc, 0, static_cast<long long>(2 * n.M) * H, st));
-    FT_TRY(launch_transpose_cast_f16(w.lstm_w_hh0, F.w.w_hh0, G, H, st));
-    FT_TRY(launch_transpose_cast_f16(w.lstm_w_hh1, F.w.w_hh1, G, H, st));
+    if (m & FT_BWD_LSTM0) FT_TRY(launch_cast(w.lstm_w_ih0, 2, F.w.w_ih0, 0, static_cast<long long>(G) * n.D, st));
+    if (m & FT_BWD_LSTM0) FT_TRY(launch_cast(w.lstm_w_ih1, 2, F.w.w_ih1, 0, static_cast<long long>(G) * H, st));
+    if (m & FT_BWD_QUERY_DGRAD) FT_TRY(launch_cast(w.att_query, 2, F.w.wq, 0, static_cast<long long>(n.A) * H, st));
+    if (m & FT_BWD_D_TEXT) FT_TRY(launch_cast(w.att_key, 2, F.w.wk, 0, static_cast<long long>(n.A) * n.E, st));
+    if (m & FT_BWD_D_TEXT) FT_TRY(launch_cast(w.att_value, 2, F.w.wv, 0, static_cast<long long>(n.A) * n.E, st));
+    if (m & FT_BWD_DENSE0_DGRAD) FT_TRY(launch_cast(w.dense_w0, 2, F.w.w1, 0, static_cast<long long>(H) * H, st));
+    if (m & FT_BWD_DENSE1_DGRAD) FT_TRY(launch_cast(w.dense_w1, 2, F.w.w2, 0, static_cast<long long>(H) * H, st));
+    if (m & FT_BWD_CONV_DGRAD) FT_TRY(launch_cast(w.conv_w, 2, F.w.wc, 0, static_cast<long long>(2 * n.M) * H, st));
+    if (m & FT_BWD_LSTM0) FT_TRY(launch_transpose_cast_f16(w.lstm_w_hh0, F.w.w_hh0, G, H, st));
+    if (m & FT_BWD_LSTM1) FT_TRY(launch_transpose_cast_f16(w.lstm_w_hh1, F.w.w_hh1, G, H, st));
 
     // 0. loss scale for this flow's backward: S = 2^k with S * max|incoming grad| ~ 64 (device-side, no host sync)
     const long long RM = R * n.M;
     const long long BTL = static_cast<long long>(n.B) * n.T * n.L;
-    FT_TRY(launch_grad_scale(d_mel_out, d_mel_out ? RM : 0, d_log_s, d_log_s ? RM : 0, d_gates, d_gates ? R : 0, 64.f, C.scale, st,
-                             d_attn, d_attn ? BTL : 0, d_logprob, d_logprob ? BTL : 0));
+    if (m & FT_BWD_COUPLING)
+        FT_TRY(launch_grad_scale(d_mel_out, d_mel_out ? RM : 0, d_log_s, d_log_s ? RM : 0, d_gates, d_gates ? R : 0, 64.f, C.scale,
+                                 st, d_attn, d_attn ? BTL : 0, d_logprob, d_logprob ? BTL : 0));
     const float* S = C.scale;            // S[0] = scale, S[1] = 1/scale
     const float* iS = C.scale + 1;
 
@@ -475,104 +525,126 @@ int ar_step_bwd_main(const FtArStepDesc& d, const FtArStepWeights& w, const floa
     cudaStream_t ss;
 
     // 1. affine coupling (scales the incoming gradients by S)
-    FT_TRY(launch_affine_bwd(d_mel_out, d_log_s, S_.o32, mel_flow, out_lens, n.T, n.B, n.M, d.reversed, F.do16, C.dmel_flow, S, st));
+    if (m & FT_BWD_COUPLING)
+        FT_TRY(launch_affine_bwd(d_mel_out, d_log_s, S_.o32, mel_flow, out_lens, n.T, n.B, n.M, d.reversed, F.do16, C.dmel_flow, S, st));
 
     // 2. 1x1 conv     (weight / bias gradients go to the side stream, the dgrad chain stays on `st`)
     ss = fork_side(sd, st);
-    FT_TRY(gemm_wgrad(ss, 2 * n.M, H, R, F.do16, 2 * n.M, S_.y2_16, H, g.conv_w, H, iS));
-    FT_TRY(launch_colsum(F.do16, 0, 2 * n.M, R, 2 * n.M, g.conv_b, iS, ss));
-    FT_TRY(gemm_dgrad(st, R, H, 2 * n.M, F.do16, 2 * n.M, F.w.wc, H, 0, nullptr, 0, F.dy2, H, S_.y2_16, H));     // * (1 - y2^2)
+    if (g.conv_w) FT_TRY(gemm_wgrad(ss, 2 * n.M, H, R, F.do16, 2 * n.M, S_.y2_16, H, g.conv_w, H, iS));
+    if (g.conv_b) FT_TRY(launch_colsum(F.do16, 0, 2 * n.M, R, 2 * n.M, g.conv_b, iS, ss));
+    if (m & FT_BWD_CONV_DGRAD)
+        FT_TRY(gemm_dgrad(st, R, H, 2 * n.M, F.do16, 2 * n.M, F.w.wc, H, 0, nullptr, 0, F.dy2, H, S_.y2_16, H));     // * (1 - y2^2)
 
     // 3. dense layer 1 (second linear)
     ss = fork_side(sd, st);
-    FT_TRY(gemm_wgrad(ss, H, H, R, F.dy2, H, S_.y1_16, H, g.dense_w1, H, iS));
-    FT_TRY(launch_colsum(F.dy2, 0, H, R, H, g.dense_b1, iS, ss));
-    FT_TRY(gemm_dgrad(st, R, H, H, F.dy2, H, F.w.w2, H, 0, nullptr, 0, F.dy1, H, S_.y1_16, H));                   // * (1 - y1^2)
+    if (g.dense_w1) FT_TRY(gemm_wgrad(ss, H, H, R, F.dy2, H, S_.y1_16, H, g.dense_w1, H, iS));
+    if (g.dense_b1) FT_TRY(launch_colsum(F.dy2, 0, H, R, H, g.dense_b1, iS, ss));
+    if (m & FT_BWD_DENSE1_DGRAD)
+        FT_TRY(gemm_dgrad(st, R, H, H, F.dy2, H, F.w.w2, H, 0, nullptr, 0, F.dy1, H, S_.y1_16, H));               // * (1 - y1^2)
 
     // 4. dense layer 0
     ss = fork_side(sd, st);
-    FT_TRY(gemm_wgrad(ss, H, H, R, F.dy1, H, S_.h1_16, H, g.dense_w0, H, iS));
-    FT_TRY(launch_colsum(F.dy1, 0, H, R, H, g.dense_b0, iS, ss));
-    FT_TRY(gemm_dgrad(st, R, H, H, F.dy1, H, F.w.w1, H, 0, F.dh, H, nullptr, 0, nullptr, 0));
+    if (g.dense_w0) FT_TRY(gemm_wgrad(ss, H, H, R, F.dy1, H, S_.h1_16, H, g.dense_w0, H, iS));
+    if (g.dense_b0) FT_TRY(launch_colsum(F.dy1, 0, H, R, H, g.dense_b0, iS, ss));
+    if (m & FT_BWD_DENSE0_DGRAD) FT_TRY(gemm_dgrad(st, R, H, H, F.dy1, H, F.w.w1, H, 0, F.dh, H, nullptr, 0, nullptr, 0));
 
-    FT_TRY(zero(F.dK, sizeof(float) * RL * n.A, st));
-    FT_TRY(zero(F.dV, sizeof(float) * RL * n.A, st));
-    FT_TRY(zero(g.att_v, sizeof(float) * n.A, st));
-    if (d.has_gate && g.gate_w) {
-        FT_TRY(zero(g.gate_w, sizeof(float) * n.D, st));
-        FT_TRY(zero(g.gate_b, sizeof(float), st));
+    if (m & FT_BWD_ATTN) {
+        FT_TRY(zero(F.dK, sizeof(float) * RL * n.A, st));
+        FT_TRY(zero(F.dV, sizeof(float) * RL * n.A, st));
+    }
+    if (g.att_v) FT_TRY(zero(g.att_v, sizeof(float) * n.A, st));
+    if (m & FT_BWD_G_GATE) {
+        if (g.gate_w) FT_TRY(zero(g.gate_w, sizeof(float) * n.D, st));
+        if (g.gate_b) FT_TRY(zero(g.gate_b, sizeof(float), st));
     }
     // 5 + 6. lstm layers 1 and 0: BPTT of layer 1 (sA) and layer 0 (sB) one chunk apart; the layer-1 dgrad of a finished chunk
     // (sC) turns dG1 rows into layer 0's incoming dh rows (F.dh is reused row-disjointly: layer 1 only reads rows below the
     // chunk it has finished).  Highest chunk first.
     Pipe* pp = get_pipe(st);
     if (!pp) return ft_set_error("ar_step_bwd: could not create the pipeline streams");
-    const int CH = layer_chunk(n.T);
-    int* flagsA = F.flags;
-    int* flagsB = F.flags + static_cast<size_t>(CH) * 128;
-    cudaStream_t sr = pp->sA;                                    // layer 1's BPTT stream
-    cudaEventRecord(pp->ev0, st);
-    cudaStreamWaitEvent(sr, pp->ev0, 0);
-    cudaStreamWaitEvent(pp->sB, pp->ev0, 0);
-    cudaStreamWaitEvent(pp->sC, pp->ev0, 0);
-    const int n_chunks = (n.T + CH - 1) / CH;
-    for (int c = n_chunks - 1; c >= 0; --c) {
-        const int t0 = c * CH, t1 = t0 + CH < n.T ? t0 + CH : n.T;
-        const long long r0 = static_cast<long long>(t0) * n.B, rows = static_cast<long long>(t1 - t0) * n.B;
-        FT_TRY(launch_lstm_bwd_chunk(n.T, n.B, t0, t1, F.dh, H, F.w.w_hh1, S_.gates1, S_.c1, out_lens, F.dG1, F.dcarry1, flagsA, F.xchg1, sr));
-        cudaEventRecord(pp->evA, sr);
-        cudaStreamWaitEvent(pp->sC, pp->evA, 0);
-        FT_TRY(gemm_dgrad(pp->sC, rows, H, G, F.dG1 + r0 * G, G, F.w.w_ih1, H, 0, F.dh + r0 * H, H, nullptr, 0, nullptr, 0));
-        cudaEventRecord(pp->evG, pp->sC);
-        cudaStreamWaitEvent(pp->sB, pp->evG, 0);
-        FT_TRY(launch_lstm_bwd_chunk(n.T, n.B, t0, t1, F.dh, H, F.w.w_hh0, S_.gates0, S_.c0, out_lens, F.dG0, F.dcarry0, flagsB, F.xchg0, pp->sB));
+    if (m & FT_BWD_LSTM1) {
+        const bool l0 = (m & FT_BWD_LSTM0) != 0;
+        const int CH = layer_chunk(n.T);
+        int* flagsA = F.flags;
+        int* flagsB = F.flags + static_cast<size_t>(CH) * 128;
+        cudaStream_t sr = pp->sA;                                    // layer 1's BPTT stream
+        cudaEventRecord(pp->ev0, st);
+        cudaStreamWaitEvent(sr, pp->ev0, 0);
+        cudaStreamWaitEvent(pp->sB, pp->ev0, 0);
+        cudaStreamWaitEvent(pp->sC, pp->ev0, 0);
+        const int n_chunks = (n.T + CH - 1) / CH;
+        for (int c = n_chunks - 1; c >= 0; --c) {
+            const int t0 = c * CH, t1 = t0 + CH < n.T ? t0 + CH : n.T;
+            const long long r0 = static_cast<long long>(t0) * n.B, rows = static_cast<long long>(t1 - t0) * n.B;
+            FT_TRY(launch_lstm_bwd_chunk(n.T, n.B, t0, t1, F.dh, H, F.w.w_hh1, S_.gates1, S_.c1, out_lens, F.dG1, F.dcarry1, flagsA, F.xchg1, sr));
+            if (!l0) continue;
+            cudaEventRecord(pp->evA, sr);
+            cudaStreamWaitEvent(pp->sC, pp->evA, 0);
+            FT_TRY(gemm_dgrad(pp->sC, rows, H, G, F.dG1 + r0 * G, G, F.w.w_ih1, H, 0, F.dh + r0 * H, H, nullptr, 0, nullptr, 0));
+            cudaEventRecord(pp->evG, pp->sC);
+            cudaStreamWaitEvent(pp->sB, pp->evG, 0);
+            FT_TRY(launch_lstm_bwd_chunk(n.T, n.B, t0, t1, F.dh, H, F.w.w_hh0, S_.gates0, S_.c0, out_lens, F.dG0, F.dcarry0, flagsB, F.xchg0, pp->sB));
+        }
+        // layer-1 weight gradients run under the tail of layer 0 (side stream forks from st = all of layer 1 done)
+        cudaEventRecord(pp->evJ, sr);
+        cudaStreamWaitEvent(st, pp->evJ, 0);
+        ss = fork_side(sd, st);
+        if (g.lstm_w_hh1) FT_TRY(gemm_wgrad(ss, G, H, Rm, F.dG1 + static_cast<size_t>(n.B) * G, G, S_.h1_16, H, g.lstm_w_hh1, H, iS));
+        if (g.lstm_w_ih1) FT_TRY(gemm_wgrad(ss, G, H, R, F.dG1, G, S_.h0_16, H, g.lstm_w_ih1, H, iS));
+        FT_TRY(lstm_bias_grads(F.dG1, R, g.lstm_b_ih1, g.lstm_b_hh1, iS, ss));
+        if (l0) {
+            cudaEventRecord(pp->evB, pp->sB);
+            cudaStreamWaitEvent(st, pp->evB, 0);
+        }
     }
-    // layer-1 weight gradients run under the tail of layer 0 (side stream forks from st = all of layer 1 done)
-    cudaEventRecord(pp->evJ, sr);
-    cudaStreamWaitEvent(st, pp->evJ, 0);
-    ss = fork_side(sd, st);
-    FT_TRY(gemm_wgrad(ss, G, H, Rm, F.dG1 + static_cast<size_t>(n.B) * G, G, S_.h1_16, H, g.lstm_w_hh1, H, iS));
-    FT_TRY(gemm_wgrad(ss, G, H, R, F.dG1, G, S_.h0_16, H, g.lstm_w_ih1, H, iS));
-    FT_TRY(launch_colsum(F.dG1, 0, G, R, G, g.lstm_b_ih1, iS, ss));
-    FT_TRY(copy_f32(g.lstm_b_hh1, g.lstm_b_ih1, G, ss));
-    cudaEventRecord(pp->evB, pp->sB);
-    cudaStreamWaitEvent(st, pp->evB, 0);
     // (the weight gradients of lstm layer 0 and of the attention projections are launched by ar_step_bwd_attn, on the side
     //  stream underneath the attention LSTM's BPTT: dG0, dQ16, dK16, dV16 stay in the scratch area until then)
     // 6b. lstm layer 0's input gradient: dd = [dhA ; dctx]
-    FT_TRY(gemm_dgrad(st, R, n.D, G, F.dG0, G, F.w.w_ih0, n.D, 0, C.dd, n.D, nullptr, 0, nullptr, 0));
-    // 7. gate layer (last flow only): dd is in the scaled domain, the gate's own parameter gradients are not
-    if (d.has_gate && g.gate_w && d_gates)
-        FT_TRY(launch_gate_bwd(S_.d16, n.D, n.D, w.gate_w, d_gates, R, C.dd, n.D, g.gate_w, g.gate_b, S, st));
+    if (m & FT_BWD_LSTM0) FT_TRY(gemm_dgrad(st, R, n.D, G, F.dG0, G, F.w.w_ih0, n.D, 0, C.dd, n.D, nullptr, 0, nullptr, 0));
+    // 7. gate layer (last flow only): dd is in the scaled domain, the gate's own parameter gradients are not.  A frozen gate
+    //    still adds its term to dd; with dd unused, only the parameter gradients are computed.
+    if ((m & (FT_BWD_GATE_DD | FT_BWD_G_GATE)) && d_gates) {
+        float* dwg = g.gate_w ? g.gate_w : F.sink + n.A;
+        float* dbg = g.gate_b ? g.gate_b : F.sink + n.A + n.D;
+        FT_TRY(launch_gate_bwd(S_.d16, n.D, n.D, w.gate_w, d_gates, R, (m & FT_BWD_GATE_DD) ? C.dd : nullptr, n.D, dwg, dbg,
+                               (m & FT_BWD_GATE_DD) ? S : nullptr, st));
+    }
     // 8. attention (score/softmax/context) with tanh recompute; dK / dV / dv accumulate
-    AttnBwdArgs a;
-    a.T = n.T; a.B = n.B; a.L = n.L; a.A = n.A;
-    a.Q = S_.Q; a.ldq = n.A; a.K = S_.Kp; a.ldk = n.A; a.V = S_.Vp; a.ldv = n.A; a.v = w.att_v;
-    a.in_lens = in_lens; a.out_lens = out_lens; a.attn = attn; a.p_save = S_.p_save; a.temperature = d.temperature;
-    a.dctx = C.dd + H; a.lddc = n.D; a.dattn_ext = d_attn; a.dlp_ext = d_logprob; a.scale = S;
-    a.dQ = F.dQ; a.lddq = n.A; a.dK = F.dK; a.lddk = n.A; a.dV = F.dV; a.lddv = n.A; a.dv = g.att_v;
-    a.t_begin = 0; a.t_end = n.T; a.rows = F.attn_rows;
-    FT_TRY(launch_attn_bwd(a, st));
+    if (m & FT_BWD_ATTN) {
+        AttnBwdArgs a;
+        a.T = n.T; a.B = n.B; a.L = n.L; a.A = n.A;
+        a.Q = S_.Q; a.ldq = n.A; a.K = S_.Kp; a.ldk = n.A; a.V = S_.Vp; a.ldv = n.A; a.v = w.att_v;
+        a.in_lens = in_lens; a.out_lens = out_lens; a.attn = attn; a.p_save = S_.p_save; a.temperature = d.temperature;
+        a.dctx = C.dd + H; a.lddc = n.D; a.dattn_ext = d_attn; a.dlp_ext = d_logprob; a.scale = S;
+        a.dQ = F.dQ; a.lddq = n.A; a.dK = F.dK; a.lddk = n.A; a.dV = F.dV; a.lddv = n.A; a.dv = g.att_v ? g.att_v : F.sink;
+        a.t_begin = 0; a.t_end = n.T; a.rows = F.attn_rows;
+        FT_TRY(launch_attn_bwd(a, st));
+    }
     // 9a. query projection (d16 = [hA ; ctx] saved in fp16, row pitch D)
-    FT_TRY(launch_cast(F.dQ, 2, F.dQ16, 0, R * n.A, st));
-    FT_TRY(gemm_dgrad(st, R, H, n.A, F.dQ16, n.A, F.w.wq, H, 1, C.dd, n.D, nullptr, 0, nullptr, 0));   // dhA += dQ Wq
+    if (m & (FT_BWD_QUERY_DGRAD | FT_BWD_G_QUERY)) FT_TRY(launch_cast(F.dQ, 2, F.dQ16, 0, R * n.A, st));
+    if (m & FT_BWD_QUERY_DGRAD)
+        FT_TRY(gemm_dgrad(st, R, H, n.A, F.dQ16, n.A, F.w.wq, H, 1, C.dd, n.D, nullptr, 0, nullptr, 0));   // dhA += dQ Wq
 
     // 9b. key / value projections -> d_text
-    FT_TRY(launch_cast(F.dK, 2, F.dK16, 0, RL * n.A, st));
-    FT_TRY(launch_cast(F.dV, 2, F.dV16, 0, RL * n.A, st));
-    FT_TRY(gemm_dgrad(st, RL, n.E, n.A, F.dK16, n.A, F.w.wk, n.E, 0, d_text, n.E, nullptr, 0, nullptr, 0, iS));
-    FT_TRY(gemm_dgrad(st, RL, n.E, n.A, F.dV16, n.A, F.w.wv, n.E, 1, d_text, n.E, nullptr, 0, nullptr, 0, iS));
+    if (m & (FT_BWD_D_TEXT | FT_BWD_G_KEY)) FT_TRY(launch_cast(F.dK, 2, F.dK16, 0, RL * n.A, st));
+    if (m & (FT_BWD_D_TEXT | FT_BWD_G_VALUE)) FT_TRY(launch_cast(F.dV, 2, F.dV16, 0, RL * n.A, st));
+    if (m & FT_BWD_D_TEXT) {
+        FT_TRY(gemm_dgrad(st, RL, n.E, n.A, F.dK16, n.A, F.w.wk, n.E, 0, d_text, n.E, nullptr, 0, nullptr, 0, iS));
+        FT_TRY(gemm_dgrad(st, RL, n.E, n.A, F.dV16, n.A, F.w.wv, n.E, 1, d_text, n.E, nullptr, 0, nullptr, 0, iS));
+    }
 
     join_side(sd, st);                   // everything this call launched is ordered before what the caller enqueues next
     return 0;
 }
 
 // Attention-LSTM part: BPTT over dhA (carry), its weight gradients, and the input gradient d_mel (coupling path from carry +
-// the shifted attention-LSTM path, back to natural time, loss scale undone).
+// the shifted attention-LSTM path, back to natural time, loss scale undone).  The stages it runs depend on `g` and
+// d.no_d_mel only, so the plan matches the one ar_step_bwd_main ran whatever d_text was.
 int ar_step_bwd_attn(const FtArStepDesc& d, const FtArStepWeights& w, const int* out_lens, float* d_mel, const FtArStepWeights& g,
                      void* saved, void* scratch, void* carry, cudaStream_t st) {
     FT_TRY(check_desc(d));
     const Dims n(d);
+    const unsigned m = bwd_plan(d, g, false, !d.no_d_mel);
     Plan ps; ps.base = static_cast<uint8_t*>(saved);
     Saved S_; S_.plan(ps, d);
     Plan pb; pb.base = static_cast<uint8_t*>(scratch);
@@ -584,31 +656,31 @@ int ar_step_bwd_attn(const FtArStepDesc& d, const FtArStepWeights& w, const int*
     Side* sd = get_side(st);
     cudaStream_t ss;
     const long long RL = n.RL;
-    FT_TRY(launch_cast(w.attn_lstm_w_ih, 2, F.w.w_ih_a, 0, static_cast<long long>(G) * n.M, st));
-    FT_TRY(launch_transpose_cast_f16(w.attn_lstm_w_hh, F.w.w_hh_a, G, H, st));
+    if (m & FT_BWD_D_MEL) FT_TRY(launch_cast(w.attn_lstm_w_ih, 2, F.w.w_ih_a, 0, static_cast<long long>(G) * n.M, st));
+    if (m & FT_BWD_ATTN_LSTM) FT_TRY(launch_transpose_cast_f16(w.attn_lstm_w_hh, F.w.w_hh_a, G, H, st));
 
     // deferred from ar_step_bwd_main: weight gradients of lstm layer 0 and of the attention projections, on the side stream,
     // underneath the BPTT kernel below (64 of the SMs)
     ss = fork_side(sd, st);
-    FT_TRY(gemm_wgrad(ss, G, H, Rm, F.dG0 + static_cast<size_t>(n.B) * G, G, S_.h0_16, H, g.lstm_w_hh0, H, iS));
-    FT_TRY(gemm_wgrad(ss, G, n.D, R, F.dG0, G, S_.d16, n.D, g.lstm_w_ih0, n.D, iS));
-    FT_TRY(launch_colsum(F.dG0, 0, G, R, G, g.lstm_b_ih0, iS, ss));
-    FT_TRY(copy_f32(g.lstm_b_hh0, g.lstm_b_ih0, G, ss));
-    FT_TRY(gemm_wgrad(ss, n.A, H, R, F.dQ16, n.A, S_.d16, n.D, g.att_query, H, iS));
-    FT_TRY(gemm_wgrad(ss, n.A, n.E, RL, F.dK16, n.A, S_.text16, n.E, g.att_key, n.E, iS));
-    FT_TRY(gemm_wgrad(ss, n.A, n.E, RL, F.dV16, n.A, S_.text16, n.E, g.att_value, n.E, iS));
+    if (g.lstm_w_hh0) FT_TRY(gemm_wgrad(ss, G, H, Rm, F.dG0 + static_cast<size_t>(n.B) * G, G, S_.h0_16, H, g.lstm_w_hh0, H, iS));
+    if (g.lstm_w_ih0) FT_TRY(gemm_wgrad(ss, G, n.D, R, F.dG0, G, S_.d16, n.D, g.lstm_w_ih0, n.D, iS));
+    FT_TRY(lstm_bias_grads(F.dG0, R, g.lstm_b_ih0, g.lstm_b_hh0, iS, ss));
+    if (g.att_query) FT_TRY(gemm_wgrad(ss, n.A, H, R, F.dQ16, n.A, S_.d16, n.D, g.att_query, H, iS));
+    if (g.att_key) FT_TRY(gemm_wgrad(ss, n.A, n.E, RL, F.dK16, n.A, S_.text16, n.E, g.att_key, n.E, iS));
+    if (g.att_value) FT_TRY(gemm_wgrad(ss, n.A, n.E, RL, F.dV16, n.A, S_.text16, n.E, g.att_value, n.E, iS));
 
     // 10. attention_lstm  (dhA = C.dd[:, 0:H], pitch D)
-    FT_TRY(launch_lstm_bwd(n.T, n.B, C.dd, n.D, F.w.w_hh_a, S_.gatesA, S_.cA, out_lens, F.dGa, F.flags, st));
+    if (m & FT_BWD_ATTN_LSTM) FT_TRY(launch_lstm_bwd(n.T, n.B, C.dd, n.D, F.w.w_hh_a, S_.gatesA, S_.cA, out_lens, F.dGa, F.flags, st));
     ss = fork_side(sd, st);
-    FT_TRY(gemm_wgrad(ss, G, H, Rm, F.dGa + static_cast<size_t>(n.B) * G, G, S_.d16, n.D, g.attn_lstm_w_hh, H, iS));
-    FT_TRY(gemm_wgrad(ss, G, n.M, R, F.dGa, G, S_.mel_in16, n.M, g.attn_lstm_w_ih, n.M, iS));
-    FT_TRY(launch_colsum(F.dGa, 0, G, R, G, g.attn_lstm_b_ih, iS, ss));
-    FT_TRY(copy_f32(g.attn_lstm_b_hh, g.attn_lstm_b_ih, G, ss));
-    FT_TRY(gemm_dgrad(st, R, n.M, G, F.dGa, G, F.w.w_ih_a, n.M, 0, F.dmel_in, n.M, nullptr, 0, nullptr, 0));
+    if (g.attn_lstm_w_hh)
+        FT_TRY(gemm_wgrad(ss, G, H, Rm, F.dGa + static_cast<size_t>(n.B) * G, G, S_.d16, n.D, g.attn_lstm_w_hh, H, iS));
+    if (g.attn_lstm_w_ih) FT_TRY(gemm_wgrad(ss, G, n.M, R, F.dGa, G, S_.mel_in16, n.M, g.attn_lstm_w_ih, n.M, iS));
+    FT_TRY(lstm_bias_grads(F.dGa, R, g.attn_lstm_b_ih, g.attn_lstm_b_hh, iS, ss));
+    if (m & FT_BWD_D_MEL) FT_TRY(gemm_dgrad(st, R, n.M, G, F.dGa, G, F.w.w_ih_a, n.M, 0, F.dmel_in, n.M, nullptr, 0, nullptr, 0));
 
     // 11. input gradient: coupling path + (shifted) attention_lstm path, back to natural time, loss scale undone
-    if (d_mel) FT_TRY(launch_combine_dmel(C.dmel_flow, F.dmel_in, out_lens, n.T, n.B, n.M, d.reversed, d_mel, iS, st));
+    if ((m & FT_BWD_D_MEL) && d_mel)
+        FT_TRY(launch_combine_dmel(C.dmel_flow, F.dmel_in, out_lens, n.T, n.B, n.M, d.reversed, d_mel, iS, st));
     join_side(sd, st);                   // everything this call launched is ordered before what the caller enqueues next
     return 0;
 }
@@ -656,19 +728,21 @@ int ft_ar_step_bwd(const FtArStepDesc* d, const FtArStepWeights* w, const float*
                    const int* out_lens, const float* attn, const float* d_mel_out, const float* d_log_s,
                    const float* d_gates, const float* d_attn, const float* d_attn_logprob, float* d_mel, float* d_text,
                    const FtArStepWeights* g, void* saved, void* scratch, void* stream) {
-    if (!d || !w || !mel || !attn || !d_text || !g || !saved || !scratch) return ft::ft_set_error("ft_ar_step_bwd: NULL argument");
+    if (!d || !w || !mel || !attn || !g || !saved || !scratch) return ft::ft_set_error("ft_ar_step_bwd: NULL argument");
     ft::Plan pb; ft::BwdScratch b; b.plan(pb, *d);
     void* carry = static_cast<uint8_t*>(scratch) + ((pb.off + 255) & ~static_cast<size_t>(255));
-    if (ft::ar_step_bwd_main(*d, *w, mel, in_lens, out_lens, attn, d_mel_out, d_log_s, d_gates, d_attn, d_attn_logprob, d_text, *g,
+    FtArStepDesc dd = *d;
+    if (!d_mel) dd.no_d_mel = 1;
+    if (ft::ar_step_bwd_main(dd, *w, mel, in_lens, out_lens, attn, d_mel_out, d_log_s, d_gates, d_attn, d_attn_logprob, d_text, *g,
                              saved, scratch, carry, static_cast<cudaStream_t>(stream)) != 0) return -1;
-    return ft::ar_step_bwd_attn(*d, *w, out_lens, d_mel, *g, saved, scratch, carry, static_cast<cudaStream_t>(stream));
+    return ft::ar_step_bwd_attn(dd, *w, out_lens, d_mel, *g, saved, scratch, carry, static_cast<cudaStream_t>(stream));
 }
 
 int ft_ar_step_bwd_main(const FtArStepDesc* d, const FtArStepWeights* w, const float* mel, const int* in_lens,
                         const int* out_lens, const float* attn, const float* d_mel_out, const float* d_log_s,
                         const float* d_gates, const float* d_attn, const float* d_attn_logprob, float* d_text,
                         const FtArStepWeights* g, void* saved, void* scratch, void* carry, void* stream) {
-    if (!d || !w || !mel || !attn || !d_text || !g || !saved || !scratch || !carry) return ft::ft_set_error("ft_ar_step_bwd_main: NULL argument");
+    if (!d || !w || !mel || !attn || !g || !saved || !scratch || !carry) return ft::ft_set_error("ft_ar_step_bwd_main: NULL argument");
     return ft::ar_step_bwd_main(*d, *w, mel, in_lens, out_lens, attn, d_mel_out, d_log_s, d_gates, d_attn, d_attn_logprob, d_text,
                                 *g, saved, scratch, carry, static_cast<cudaStream_t>(stream));
 }
@@ -677,6 +751,12 @@ int ft_ar_step_bwd_attn_lstm(const FtArStepDesc* d, const FtArStepWeights* w, co
                              const FtArStepWeights* g, void* saved, void* scratch, void* carry, void* stream) {
     if (!d || !w || !g || !saved || !scratch || !carry) return ft::ft_set_error("ft_ar_step_bwd_attn_lstm: NULL argument");
     return ft::ar_step_bwd_attn(*d, *w, out_lens, d_mel, *g, saved, scratch, carry, static_cast<cudaStream_t>(stream));
+}
+
+int ft_ar_step_bwd_plan(const FtArStepDesc* d, const FtArStepWeights* grads, int want_d_text, int want_d_mel, unsigned* stages) {
+    if (!d || !grads || !stages) return ft::ft_set_error("ft_ar_step_bwd_plan: NULL argument");
+    *stages = ft::bwd_plan(*d, *grads, want_d_text != 0, want_d_mel != 0);
+    return 0;
 }
 
 int ft_nll_reduce(const float* z, const float* const* log_s_list, int n_flows, const float* gate,

@@ -233,6 +233,8 @@ int launch_gate_fwd_f32(const float* h32, long long ldh, int H, const float* c32
 }
 
 // backward of the gate GEMV: dd[r,:] += dgate[r] * wg ;  dwg[k] += sum_r dgate[r] d[r,k] ;  dbg += sum_r dgate[r]
+// kDd = false: the parameter gradients only (a frozen flow step whose gate alone trains); dd is neither read nor written.
+template <bool kDd>
 __global__ void gate_bwd_kernel(const __half* __restrict__ d16, long long ldd, int K, const float* __restrict__ wg,
                                 const float* __restrict__ dgate, long long R, float* __restrict__ dd, long long lddd,
                                 float* __restrict__ dwg, float* __restrict__ dbg, const float* __restrict__ scale) {
@@ -248,7 +250,7 @@ __global__ void gate_bwd_kernel(const __half* __restrict__ d16, long long ldd, i
     for (int j = 0; j < GB_KJ; ++j) {
         const int k = threadIdx.x + 256 * j;
         acc[j] = 0.f;
-        w[j] = k < K ? S * wg[k] : 0.f;
+        if (kDd) w[j] = k < K ? S * wg[k] : 0.f;
     }
     float db = 0.f;
     for (long long r = r0; r < r1; ++r) {
@@ -262,7 +264,7 @@ __global__ void gate_bwd_kernel(const __half* __restrict__ d16, long long ldd, i
             const int k = threadIdx.x + 256 * j;
             if (k < K) {
                 acc[j] = fmaf(g, __half2float(drow[k]), acc[j]);
-                ddrow[k] = fmaf(g, w[j], ddrow[k]);
+                if (kDd) ddrow[k] = fmaf(g, w[j], ddrow[k]);
             }
         }
     }
@@ -279,7 +281,10 @@ int launch_gate_bwd(const void* d16, long long ldd, int K, const float* wg, cons
     int g = static_cast<int>(gl > gcap ? gcap : gl);
     if (g < 1) g = 1;
     if (K > 2048) return ft_set_error("gate_bwd: K > 2048 not supported");
-    gate_bwd_kernel<<<g, 256, 0, st>>>(static_cast<const __half*>(d16), ldd, K, wg, dgate, R, dd, lddd, dwg, dbg, scale);
+    if (dd)
+        gate_bwd_kernel<true><<<g, 256, 0, st>>>(static_cast<const __half*>(d16), ldd, K, wg, dgate, R, dd, lddd, dwg, dbg, scale);
+    else
+        gate_bwd_kernel<false><<<g, 256, 0, st>>>(static_cast<const __half*>(d16), ldd, K, wg, dgate, R, dd, lddd, dwg, dbg, scale);
     ft_count_launch(1);
     return ft_check_launch("gate_bwd_kernel");
 }

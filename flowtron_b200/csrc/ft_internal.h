@@ -64,6 +64,7 @@ int launch_prep_mel(const float* mel, const int* lens, int T, int B, int M, int 
 int launch_gate_fwd(const void* d16, long long ldd, int K, const float* wg, const float* bg, long long R, float* gate, cudaStream_t st);
 int launch_gate_fwd_f32(const float* h32, long long ldh, int H, const float* c32, long long ldc, int A, const float* wg,
                         const float* bg, long long R, float* gate, cudaStream_t st);
+// dd NULL: only dwg / dbg (the params-only kernel variant)
 int launch_gate_bwd(const void* d16, long long ldd, int K, const float* wg, const float* dgate, long long R, float* dd,
                     long long lddd, float* dwg, float* dbg, const float* scale, cudaStream_t st);
 int launch_affine_fwd(const float* o, const float* mel_flow, const int* lens, int T, int B, int M, int reversed, float* z,

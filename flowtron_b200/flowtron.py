@@ -503,8 +503,11 @@ _MAIN_HALF = tuple(i for i in range(24) if i not in _ATTN_HALF)
 
 
 class _FlowState:
-    """What the two autograd nodes of one flow step share between forward and the two backward calls."""
-    __slots__ = ("desc", "saved", "plist", "mel_c", "in_lens", "out_lens", "attn", "carry", "grads", "text_shape", "has_gate")
+    """What the two autograd nodes of one flow step share between forward and the two backward calls.  want / want_mel /
+    want_text: which of the 24 parameter gradients, d_mel and d_text the backward computes (the rest are None and their
+    work is skipped, ft_ar_step_bwd_plan); node_a: node A exists, i.e. mel or an _ATTN_HALF parameter requires grad."""
+    __slots__ = ("desc", "saved", "plist", "mel_c", "in_lens", "out_lens", "attn", "carry", "grads", "text_shape", "has_gate",
+                 "want", "want_mel", "want_text", "node_a")
 
     def clear(self):
         for k in self.__slots__:
@@ -529,7 +532,7 @@ class _ArStepAttnLstmFn(torch.autograd.Function):
             raise FlowtronB200Error("AR_Step backward ran twice: the flow's saved activations are released after the first "
                                     "backward (retain_graph is not supported on the CUDA path)")
         dev = st.mel_c.device
-        d_mel = torch.empty_like(st.mel_c)
+        d_mel = torch.empty_like(st.mel_c) if st.want_mel else None
         _, scratch_bytes = _lib.ar_step_sizes(st.desc)
         scratch = _lib.scratch_buffer(scratch_bytes, dev)
         _lib.ar_step_bwd_attn_lstm(st.desc, _lib.make_weights(st.plist), st.out_lens, d_mel, _lib.make_weights(st.grads),
@@ -551,13 +554,25 @@ class _ArStepFn(torch.autograd.Function):
         L, _, E = text.shape
         dev = mel.device
         has_gate = hasattr(step, 'gate_layer')
+        # What the backward has to produce (only used when grad mode made these nodes): the inputs' requires_grad.  The token
+        # requires grad exactly when node A exists, and then node A's parameters need the gradients their requires_grad asks
+        # for.
+        need = ctx.needs_input_grad
+        state.node_a, state.want_mel, state.want_text = need[3], need[4], need[5]
+        params = step._param_list()
+        want = [False] * 24
+        for k, i in enumerate(_MAIN_HALF):
+            want[i] = need[10 + k]
+        for i in _ATTN_HALF:
+            want[i] = state.node_a and params[i].requires_grad
+        state.want = want
         desc = _lib.FtArStepDesc(T, B, L, M, step.lstm.hidden_size, step.attention_layer.query.linear_layer.out_features,
                                  E, int(reversed_flag), int(has_gate), int(attn_prior is not None),
-                                 float(step.attention_layer.temperature))
+                                 float(step.attention_layer.temperature), int(not state.want_mel))
         mel_c = mel.detach().float().contiguous()
         text_c = text.detach().float().contiguous()
         prior_c = None if attn_prior is None else attn_prior.detach().float().contiguous()
-        plist = [p.detach() if p is not None else None for p in step._param_list()]
+        plist = [p.detach() if p is not None else None for p in params]
         plist = [p if (p is None or p.is_contiguous()) else p.contiguous() for p in plist]
         weights = _lib.make_weights(plist)
         saved_bytes, scratch_bytes = _lib.ar_step_sizes(desc)
@@ -595,18 +610,21 @@ class _ArStepFn(torch.autograd.Function):
                                     "backward (retain_graph is not supported on the CUDA path)")
         desc = st.desc
         dev = st.mel_c.device
-        d_text = torch.empty(st.text_shape, device=dev, dtype=torch.float32)
-        st.grads = [None if p is None else torch.empty_like(p) for p in st.plist]
+        d_text = torch.empty(st.text_shape, device=dev, dtype=torch.float32) if st.want_text else None
+        st.grads = [torch.empty_like(p) if w else None for p, w in zip(st.plist, st.want)]
         _, scratch_bytes = _lib.ar_step_sizes(desc)
         scratch = _lib.scratch_buffer(scratch_bytes, dev)
         st.carry = torch.empty(_lib.ar_step_bwd_carry_bytes(desc), dtype=torch.uint8, device=dev)
         _lib.ar_step_bwd_main(desc, _lib.make_weights(st.plist), st.mel_c, st.in_lens, st.out_lens, st.attn, d_mel_out, d_log_s,
                               d_gates, d_attn, d_lp, d_text, _lib.make_weights(st.grads), st.saved, scratch, st.carry)
         grads_b = [st.grads[i] for i in _MAIN_HALF]
+        node_a = st.node_a
+        if not node_a:
+            st.clear()                               # no node A to release the flow's saved activations and carry
         ctx.state = None
         # (state, step, reversed, token, mel, text, in_lens, out_lens, prior, text_ready, *params_b): mel's gradient comes
         # out of node A
-        return (None, None, None, torch.zeros(1, device=dev), None, d_text, None, None, None, None, *grads_b)
+        return (None, None, None, torch.zeros(1, device=dev) if node_a else None, None, d_text, None, None, None, None, *grads_b)
 
 
 class AR_Step(nn.Module):

@@ -96,6 +96,7 @@ typedef struct {
     int has_gate;       /* flow owns gate_layer (last flow only, flowtron.py:854)   */
     int has_prior;      /* attn_prior given                                         */
     float temperature;  /* Attention.temperature (flowtron.py:532, 573)             */
+    int no_d_mel;       /* backward: the caller will not read d_mel (ft_ar_step_bwd_plan); ignored by ft_ar_step_infer */
 } FtArStepDesc;
 
 /* fp32 device pointers in PyTorch's native layouts == the state_dict entries of one AR_Step
@@ -132,7 +133,8 @@ int ft_ar_step_fwd(const FtArStepDesc* d, const FtArStepWeights* w, const float*
 
 /* Autograd of the above.  Incoming gradients (any may be NULL = zero): d_mel_out, d_log_s [T,B,M], d_gates [T,B],
  * d_attn, d_attn_logprob [B,T,L].  Outputs: d_mel [T,B,M], d_text [L,B,E] (overwritten), parameter gradients
- * into `g` (overwritten; same layouts as the weights). */
+ * into `g` (overwritten; same layouts as the weights).  Every output may be NULL = not wanted: the backward then runs only
+ * the stages that a wanted output depends on (ft_ar_step_bwd_plan below); a NULL d_mel here counts as d->no_d_mel. */
 int ft_ar_step_bwd(const FtArStepDesc* d, const FtArStepWeights* w, const float* mel, const int* in_lens,
                    const int* out_lens, const float* attn, const float* d_mel_out, const float* d_log_s,
                    const float* d_gates, const float* d_attn, const float* d_attn_logprob, float* d_mel, float* d_text,
@@ -146,7 +148,9 @@ int ft_ar_step_bwd(const FtArStepDesc* d, const FtArStepWeights* w, const float*
  *                              dG0 / dQ / dK / dV in `scratch` (nothing else may use `scratch` in between).
  *   ft_ar_step_bwd_attn_lstm : attention-LSTM BPTT; writes d_mel and the gradients of attention_lstm, lstm layer 0 and the
  *                              attention query / key / value projections (their GEMMs run underneath the BPTT kernel).
- * ft_ar_step_bwd == the two back to back. */
+ * ft_ar_step_bwd == the two back to back.  ft_ar_step_bwd_main must know whether d_mel will be read before the second call
+ * runs: d->no_d_mel = 1 says it will not (ft_ar_step_bwd_attn_lstm then skips the input gradient even for a non-NULL d_mel).
+ * d_text and any entry of `g` may be NULL, as for ft_ar_step_bwd. */
 size_t ft_ar_step_bwd_carry_bytes(const FtArStepDesc* d);
 int ft_ar_step_bwd_main(const FtArStepDesc* d, const FtArStepWeights* w, const float* mel, const int* in_lens,
                         const int* out_lens, const float* attn, const float* d_mel_out, const float* d_log_s,
@@ -154,6 +158,37 @@ int ft_ar_step_bwd_main(const FtArStepDesc* d, const FtArStepWeights* w, const f
                         const FtArStepWeights* g, void* saved, void* scratch, void* carry, void* stream);
 int ft_ar_step_bwd_attn_lstm(const FtArStepDesc* d, const FtArStepWeights* w, const int* out_lens, float* d_mel,
                              const FtArStepWeights* g, void* saved, void* scratch, void* carry, void* stream);
+
+/* Which stages of a flow step's backward run, for the wanted outputs: a NULL entry of `grads` is a parameter gradient
+ * nobody wants, want_d_text / want_d_mel say whether d_text / d_mel are.  A stage runs when something downstream of it is
+ * wanted (FT_BWD_G_* name the weight-gradient work of one parameter group; within a group only the non-NULL entries are
+ * computed):
+ *   D_MEL                the attention-LSTM dgrad to the input and combine_dmel:   d_mel wanted
+ *   ATTN_LSTM            attention-LSTM BPTT:                  D_MEL or G_ATTN_LSTM
+ *   QUERY_DGRAD          dhA += dQ Wq:                         ATTN_LSTM
+ *   D_TEXT               d_text = dK Wk + dV Wv:               d_text wanted
+ *   ATTN                 zero dK / dV, attention backward:     QUERY_DGRAD, D_TEXT, G_QUERY, G_KEY, G_VALUE or G_V
+ *   GATE_DD              the gate's term of dd (gated flow):   ATTN or ATTN_LSTM (both read dd)
+ *   LSTM0                layer-1 per-chunk dgrad, layer 0 BPTT, dd = dG0 W_ih0:   ATTN, ATTN_LSTM or G_LSTM0
+ *   LSTM1                layer 1 BPTT:                         LSTM0 or G_LSTM1
+ *   DENSE0_DGRAD         dense layer 0 dgrad (-> layer 1):     LSTM1
+ *   DENSE1_DGRAD         dense layer 1 dgrad:                  DENSE0_DGRAD or G_DENSE0
+ *   CONV_DGRAD           1x1 conv dgrad:                       DENSE1_DGRAD or G_DENSE1
+ *   COUPLING             loss scale + affine coupling backward:   CONV_DGRAD, G_CONV or D_MEL
+ *   G_GATE               the gate's parameter gradients (gated flow): a gate entry of `grads` non-NULL.  With GATE_DD off
+ *                        it is the whole backward of a gate-only step: one launch, no loss scale.
+ * With every gradient, d_text and d_mel wanted all stages run, in the order of the full backward.  The two backward calls
+ * branch on this mask and nothing else.  Returns 0, or -1 for a NULL argument. */
+enum {
+    FT_BWD_COUPLING = 1u << 0, FT_BWD_CONV_DGRAD = 1u << 1, FT_BWD_DENSE1_DGRAD = 1u << 2, FT_BWD_DENSE0_DGRAD = 1u << 3,
+    FT_BWD_LSTM1 = 1u << 4, FT_BWD_LSTM0 = 1u << 5, FT_BWD_GATE_DD = 1u << 6, FT_BWD_ATTN = 1u << 7,
+    FT_BWD_QUERY_DGRAD = 1u << 8, FT_BWD_D_TEXT = 1u << 9, FT_BWD_ATTN_LSTM = 1u << 10, FT_BWD_D_MEL = 1u << 11,
+    FT_BWD_G_CONV = 1u << 16, FT_BWD_G_DENSE1 = 1u << 17, FT_BWD_G_DENSE0 = 1u << 18, FT_BWD_G_LSTM1 = 1u << 19,
+    FT_BWD_G_LSTM0 = 1u << 20, FT_BWD_G_QUERY = 1u << 21, FT_BWD_G_KEY = 1u << 22, FT_BWD_G_VALUE = 1u << 23,
+    FT_BWD_G_V = 1u << 24, FT_BWD_G_ATTN_LSTM = 1u << 25, FT_BWD_G_GATE = 1u << 26
+};
+int ft_ar_step_bwd_plan(const FtArStepDesc* d, const FtArStepWeights* grads, int want_d_text, int want_d_mel,
+                        unsigned* stages);
 
 /* FlowtronLoss default branch (flowtron.py:205-243): sums[0]=sum (z m)^2, [1]=sum_flows sum log_s m,
  * [2]=sum m BCEWithLogits(gate m, target), [3]=n=sum m.  log_s_list: HOST array of n_flows (<= 16) device pointers (passed
