@@ -213,6 +213,8 @@ def _declare(L):
     L.ft_attn_ctc_loss.restype = c_int
     L.ft_nll_reduce.argtypes = [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]
     L.ft_nll_reduce.restype = c_int
+    L.ft_nll_rows.argtypes = [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]
+    L.ft_nll_rows.restype = c_int
     L.ft_nll_grad.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_void_p, c_void_p,
                               c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
     L.ft_nll_grad.restype = c_int
@@ -281,6 +283,8 @@ def _declare(L):
     L.ft_gmm_nll_scratch_bytes.restype = c_size_t
     L.ft_gmm_nll_reduce.argtypes = [POINTER(FtGmmDesc)] + [c_void_p] * 8
     L.ft_gmm_nll_reduce.restype = c_int
+    L.ft_gmm_nll_rows.argtypes = [POINTER(FtGmmDesc)] + [c_void_p] * 8
+    L.ft_gmm_nll_rows.restype = c_int
     L.ft_gmm_nll_grad.argtypes = [POINTER(FtGmmDesc)] + [c_void_p] * 11
     L.ft_gmm_nll_grad.restype = c_int
     for fn in ("ft_attention_saved_bytes", "ft_attention_scratch_bytes"):
@@ -486,6 +490,15 @@ def nll_reduce(z, log_s_list, gate, gate_target, out_lens, sums):
     arr = (c_void_p * len(log_s_list))(*[t.data_ptr() for t in log_s_list])
     check(lib().ft_nll_reduce(ptr(z), arr, len(log_s_list), ptr(gate), ptr(gate_target), ptr(out_lens), T, B, M,
                               ptr(sums), stream_ptr()), "ft_nll_reduce")
+
+
+def nll_rows(z, log_s_list, gate, gate_target, out_lens, rows):
+    """ft_nll_rows: rows [B, 4] = per utterance {sum z^2, sum_flows sum log_s, sum gate BCE, frames}."""
+    _need_cuda(z, *log_s_list, gate, gate_target, out_lens, rows)
+    T, B, M = z.shape
+    arr = (c_void_p * max(1, len(log_s_list)))(*[t.data_ptr() for t in log_s_list])
+    check(lib().ft_nll_rows(ptr(z), arr, len(log_s_list), ptr(gate), ptr(gate_target), ptr(out_lens), T, B, M,
+                            ptr(rows), stream_ptr()), "ft_nll_rows")
 
 
 def nll_grad(z, gate, gate_target, out_lens, sigma, sums, g_nll, g_gate, dz, dlog_s, dgate):
@@ -767,6 +780,16 @@ def gmm_nll_reduce(z, out_lens_i32, mean, log_var, prob, per_row, sums):
     scratch = torch.empty(lib().ft_gmm_nll_scratch_bytes(byref(desc)), dtype=torch.uint8, device=z.device)
     check(lib().ft_gmm_nll_reduce(byref(desc), ptr(z), ptr(out_lens_i32), ptr(mean), ptr(log_var), ptr(prob), ptr(sums),
                                   ptr(scratch), stream_ptr()), "ft_gmm_nll_reduce")
+
+
+def gmm_nll_rows(z, out_lens_i32, mean, log_var, prob, per_row, rows):
+    """ft_gmm_nll_rows: rows [B] = each utterance's mixture NLL (no division by its element count)."""
+    _need_cuda(z, out_lens_i32, mean, log_var, prob, rows)
+    T, B, M = z.shape
+    desc = FtGmmDesc(T=T, B=B, M=M, K=prob.size(1), per_row=int(per_row))
+    scratch = torch.empty(lib().ft_gmm_nll_scratch_bytes(byref(desc)), dtype=torch.uint8, device=z.device)
+    check(lib().ft_gmm_nll_rows(byref(desc), ptr(z), ptr(out_lens_i32), ptr(mean), ptr(log_var), ptr(prob), ptr(rows),
+                                ptr(scratch), stream_ptr()), "ft_gmm_nll_rows")
 
 
 def gmm_nll_grad(z, out_lens_i32, mean, log_var, prob, per_row, g_nll, dz, dmean, dlog_var, dprob):

@@ -764,6 +764,11 @@ int ft_nll_reduce(const float* z, const float* const* log_s_list, int n_flows, c
     return ft::launch_nll_reduce(z, log_s_list, n_flows, gate, gate_target, out_lens, T, B, M, sums,
                                  static_cast<cudaStream_t>(stream));
 }
+int ft_nll_rows(const float* z, const float* const* log_s_list, int n_flows, const float* gate,
+                const float* gate_target, const int* out_lens, int T, int B, int M, float* rows_out, void* stream) {
+    return ft::launch_nll_rows(z, log_s_list, n_flows, gate, gate_target, out_lens, T, B, M, rows_out,
+                               static_cast<cudaStream_t>(stream));
+}
 int ft_nll_grad(const float* z, const float* gate, const float* gate_target, const int* out_lens, int T, int B, int M,
                 float sigma, const float* sums, const float* g_nll, const float* g_gate, float* dz, float* dlog_s,
                 float* dgate, void* stream) {

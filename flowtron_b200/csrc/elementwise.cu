@@ -471,6 +471,65 @@ int launch_nll_reduce(const float* z, const float* const* log_s_list_host, int n
     return ft_check_launch("nll_reduce_kernel");
 }
 
+// Per-utterance form of the same sums (Flowtron.score).  One CTA per row b; rows[b * 4 + {0, 1, 2, 3}] = sum z^2,
+// sum_flows sum log_s, sum BCEWithLogits(gate, target) over the row's n = min(lens[b], T) frames, and n.  Thread i of the
+// CTA takes elements i, i + 256, ... of the row's [n, M] block and frames i, i + 256, ... of its gate; the flows are added
+// per element in flow order, then the threads' partials in a fixed tree.  Nothing depends on B or on other rows (no
+// atomics), so a row's values are bit-identical whatever batch, padding or graph replay it comes from.
+constexpr int NLL_ROWS_THREADS = 256;
+__global__ void __launch_bounds__(NLL_ROWS_THREADS) nll_rows_kernel(
+        const float* __restrict__ z, const LogSList log_s_list, int n_flows, const float* __restrict__ gate,
+        const float* __restrict__ gate_target, const int* __restrict__ lens, int T, int B, int M, float* __restrict__ rows) {
+    const int b = blockIdx.x;
+    const int n = max(0, min(lens[b], T));
+    float a0 = 0.f, a1 = 0.f, a2 = 0.f;
+    const long long ne = static_cast<long long>(n) * M;
+    for (long long j = threadIdx.x; j < ne; j += NLL_ROWS_THREADS) {
+        const int t = static_cast<int>(j / M), m = static_cast<int>(j - static_cast<long long>(t) * M);
+        const long long i = (static_cast<long long>(t) * B + b) * M + m;
+        const float zz = z[i];
+        a0 = fmaf(zz, zz, a0);
+        float ls = 0.f;
+        for (int f = 0; f < n_flows; ++f) ls += log_s_list.p[f][i];
+        a1 += ls;
+    }
+    if (gate)
+        for (int t = threadIdx.x; t < n; t += NLL_ROWS_THREADS) {
+            const float x = gate[static_cast<long long>(t) * B + b], y = gate_target[static_cast<long long>(b) * T + t];
+            a2 += fmaxf(x, 0.f) - x * y + log1pf(expf(-fabsf(x)));
+        }
+    __shared__ float sm[3][NLL_ROWS_THREADS / 32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int o = 16; o; o >>= 1) {
+        a0 += __shfl_xor_sync(0xffffffffu, a0, o); a1 += __shfl_xor_sync(0xffffffffu, a1, o);
+        a2 += __shfl_xor_sync(0xffffffffu, a2, o);
+    }
+    if (lane == 0) { sm[0][warp] = a0; sm[1][warp] = a1; sm[2][warp] = a2; }
+    __syncthreads();
+    if (threadIdx.x < 3) {
+        float s = 0.f;
+        for (int w = 0; w < NLL_ROWS_THREADS / 32; ++w) s += sm[threadIdx.x][w];
+        rows[static_cast<long long>(b) * 4 + threadIdx.x] = s;
+    }
+    if (threadIdx.x == 3) rows[static_cast<long long>(b) * 4 + 3] = static_cast<float>(n);
+}
+int launch_nll_rows(const float* z, const float* const* log_s_list_host, int n_flows, const float* gate,
+                    const float* gate_target, const int* lens, int T, int B, int M, float* rows, cudaStream_t st) {
+    if (n_flows < 0 || n_flows > NLL_MAX_FLOWS) return ft_set_error("ft_nll_rows: more than 16 flows not supported");
+    if (T < 1 || B < 1 || M < 1) return ft_set_error("ft_nll_rows: T, B and M must be positive");
+    if (!z || !lens || !rows || (n_flows > 0 && !log_s_list_host)) return ft_set_error("ft_nll_rows: NULL argument");
+    if (gate && !gate_target) return ft_set_error("ft_nll_rows: gate needs gate_target");
+    LogSList ls;
+    for (int f = 0; f < NLL_MAX_FLOWS; ++f) {
+        ls.p[f] = f < n_flows ? log_s_list_host[f] : nullptr;
+        if (f < n_flows && !ls.p[f]) return ft_set_error("ft_nll_rows: NULL log_s pointer");
+    }
+    nll_rows_kernel<<<B, NLL_ROWS_THREADS, 0, st>>>(z, ls, n_flows, gate, gate_target, lens, T, B, M, rows);
+    ft_count_launch(1);
+    return ft_check_launch("nll_rows_kernel");
+}
+
 // gradients of  loss = g_nll * nll + g_gate * gate_loss  with  nll = (S0/(2 s^2) - S1)/(n M),  gate_loss = S2/n:
 //   dz = g_nll * z m /(s^2 n M) ;  dlog_s = -g_nll * m/(n M) (same for every flow) ;  dgate = g_gate * m (sigmoid(x) - y)/n
 __global__ void nll_grad_kernel(const float* __restrict__ z, const float* __restrict__ gate, const float* __restrict__ gate_target,

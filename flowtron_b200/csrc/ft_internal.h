@@ -76,6 +76,8 @@ int launch_combine_dmel(const float* dmel_flow, const float* dmel_in, const int*
 int launch_colsum(const void* src, int fmt, long long ld, long long R, int C, float* out, const float* out_scale, cudaStream_t st);
 int launch_nll_reduce(const float* z, const float* const* log_s_list_host, int n_flows, const float* gate,
                       const float* gate_target, const int* lens, int T, int B, int M, float* sums, cudaStream_t st);
+int launch_nll_rows(const float* z, const float* const* log_s_list_host, int n_flows, const float* gate,
+                    const float* gate_target, const int* lens, int T, int B, int M, float* rows, cudaStream_t st);
 int launch_nll_grad(const float* z, const float* gate, const float* gate_target, const int* lens, int T, int B, int M,
                     float sigma, const float* sums, const float* g_nll, const float* g_gate, float* dz, float* dlog_s,
                     float* dgate, cudaStream_t st);

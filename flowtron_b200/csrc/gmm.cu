@@ -85,6 +85,27 @@ __global__ void gmm_reduce_final_kernel(const float* __restrict__ part, long lon
     }
 }
 
+// grid B, 128 threads: rows[b] = -(sum over m of (sum over chunks of the row's partials, in chunk order)), the m terms added
+// in channel order by one thread.  Only row b's partials are read, and chunks past its length hold +0, so the value does not
+// depend on the other rows, on B or on the padded length.
+__global__ void __launch_bounds__(128) gmm_rows_final_kernel(const float* __restrict__ part, int chunks, int M,
+                                                             float* __restrict__ rows) {
+    __shared__ float sm[128];
+    const int b = blockIdx.x;
+    float s = 0.f;
+    if (threadIdx.x < M) {
+        const float* p = part + (static_cast<long long>(b) * M + threadIdx.x) * chunks;
+        for (int c = 0; c < chunks; ++c) s += p[c];
+    }
+    sm[threadIdx.x] = s;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float r = 0.f;
+        for (int m = 0; m < M; ++m) r += sm[m];
+        rows[b] = -r;
+    }
+}
+
 // Gradient of g * nll.  Per valid element, r_k = exp(a_k - lse), e_k = exp(a_k - log prob_k - lse), u_k = (z - mean_k) exp(-log_var_k):
 //   dz = g sum_k r_k u_k ;  dmean_k = -g sum_t r_k u_k ;  dlog_var_k = g sum_t (r_k - r_k u_k (z - mean_k)) / 2 ;  dprob_k = -g sum_{t,m} e_k
 // (e_k, not r_k / prob_k, so a vanishing prob_k has a finite gradient).  dz is written for every frame (zero past the length); the
@@ -179,6 +200,23 @@ int ft_gmm_nll_reduce(const FtGmmDesc* d, const float* z, const int* out_lens, c
     gmm_reduce_final_kernel<<<1, 256, 0, st>>>(part, static_cast<long long>(chunks) * d->B * d->M, out_lens, d->B, d->T, sums);
     ft_count_launch(1);
     return ft_check_launch("gmm_reduce_final_kernel");
+}
+
+int ft_gmm_nll_rows(const FtGmmDesc* d, const float* z, const int* out_lens, const float* mean, const float* log_var,
+                    const float* prob, float* rows_out, void* scratch, void* stream) {
+    using namespace ft;
+    if (check_gmm(d)) return -1;
+    if (!z || !out_lens || !mean || !log_var || !prob || !rows_out || !scratch) return ft_set_error("ft_gmm_nll_rows: NULL argument");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    GmmArgs a{z, out_lens, d->T, d->B, d->M, d->K, mean, log_var, d->per_row, prob};
+    const int chunks = gmm_chunks(d);
+    float* part = static_cast<float*>(scratch);
+    gmm_reduce_kernel<<<dim3(chunks, d->B, (d->M + GMM_WARPS - 1) / GMM_WARPS), GMM_WARPS * 32, 0, st>>>(a, part);
+    ft_count_launch(1);
+    if (ft_check_launch("gmm_reduce_kernel")) return -1;
+    gmm_rows_final_kernel<<<d->B, 128, 0, st>>>(part, chunks, d->M, rows_out);
+    ft_count_launch(1);
+    return ft_check_launch("gmm_rows_final_kernel");
 }
 
 int ft_gmm_nll_grad(const FtGmmDesc* d, const float* z, const int* out_lens, const float* mean, const float* log_var,

@@ -916,7 +916,7 @@ class Flowtron(nn.Module):
         ``attns_list`` (row b left-aligned in that flow's own time order: an AR_Back_Step's rows run back to front over
         their out_lens[b] frames), zero at t >= out_lens[b] and l >= in_lens[b] -- what ``infer_aligned`` takes."""
         checked = self._encode_args(mel, speaker_ids, text, in_lens, out_lens, attn_prior, "Flowtron.encode")
-        z, attns, _ = self._encode_batch(mel, speaker_ids, text, attn_prior, *checked, return_attns)
+        z, attns, _, _ = self._encode_batch(mel, speaker_ids, text, attn_prior, *checked, return_attns)
         z = z.permute(1, 2, 0)
         return (z, attns) if return_attns else z
 
@@ -946,34 +946,52 @@ class Flowtron(nn.Module):
             groups = [(rows, max(lens[b] for b in rows)) for rows in (short, long_rows) if rows]
         return in_lens.to(device=dev, dtype=torch.int32), out_lens.to(device=dev, dtype=torch.int32), groups
 
-    def _encode_batch(self, mel, speaker_ids, text, attn_prior, in_lens, out_lens, groups, return_attns, logprob_flow=None):
+    def _encode_batch(self, mel, speaker_ids, text, attn_prior, in_lens, out_lens, groups, return_attns, logprob_flow=None,
+                      return_terms=False):
         """encode's work on checked inputs, one _encode_rows call per row group -> (z [T, B, 80], the flows' attention or
-        None, flow ``logprob_flow``'s attn_logprob [B, T, L] (defined inside each row's lengths) or None)."""
+        None, flow ``logprob_flow``'s attn_logprob [B, T, L] (defined inside each row's lengths) or None, and with
+        ``return_terms`` the loss terms the flows produced as ``forward`` returns them -- (log_s_list [T, B, 80] each, gate
+        logits [T, B, 1] or None, every flow's attn_logprob [B, T, L]), defined inside each row's lengths -- or None)."""
         B, _, T = mel.shape
         L = text.size(1)
         dev = mel.device
         with torch.no_grad():
             if groups is None or groups == [(list(range(B)), T)]:
-                return self._encode_rows(mel, speaker_ids, text, in_lens, out_lens, attn_prior, return_attns, logprob_flow)
+                return self._encode_rows(mel, speaker_ids, text, in_lens, out_lens, attn_prior, return_attns, logprob_flow,
+                                         return_terms)
             z = torch.zeros(T, B, mel.size(1), device=dev)
             attns = [torch.zeros(B, T, L, device=dev) for _ in self.flows] if return_attns else None
             logp = None if logprob_flow is None else torch.zeros(B, T, L, device=dev)
+            terms = None
             for rows, t in groups:
                 idx = torch.tensor(rows, device=dev)
                 prior = None if attn_prior is None else attn_prior[idx, :t]
-                zg, ag, lg = self._encode_rows(mel[idx, :, :t], speaker_ids[idx], text[idx], in_lens[idx], out_lens[idx], prior,
-                                               return_attns, logprob_flow)
+                zg, ag, lg, tg = self._encode_rows(mel[idx, :, :t], speaker_ids[idx], text[idx], in_lens[idx], out_lens[idx],
+                                                   prior, return_attns, logprob_flow, return_terms)
                 z[:t].index_copy_(1, idx, zg)
                 for a, g in zip(attns or (), ag or ()):
                     a[:, :t].index_copy_(0, idx, g)
                 if logp is not None:
                     logp[:, :t].index_copy_(0, idx, lg)
-        return z, attns, logp
+                if return_terms:
+                    if terms is None:
+                        terms = ([torch.zeros(T, B, mel.size(1), device=dev) for _ in self.flows],
+                                 None if tg[1] is None else torch.zeros(T, B, 1, device=dev),
+                                 [torch.zeros(B, T, L, device=dev) for _ in self.flows])
+                    for full, g in zip(terms[0], tg[0]):
+                        full[:t].index_copy_(1, idx, g)
+                    if tg[1] is not None:
+                        terms[1][:t].index_copy_(1, idx, tg[1])
+                    for full, g in zip(terms[2], tg[2]):
+                        full[:, :t].index_copy_(0, idx, g)
+        return z, attns, logp, terms
 
-    def _encode_rows(self, mel, speaker_ids, text, in_lens, out_lens, attn_prior, return_attns=False, logprob_flow=None):
+    def _encode_rows(self, mel, speaker_ids, text, in_lens, out_lens, attn_prior, return_attns=False, logprob_flow=None,
+                     return_terms=False):
         """Flowtron.encode's work on checked inputs (lengths int32 on the device) -> (z [T, B, 80], zero past out_lens;
         the flows' attention [B, T, L] zeroed outside each row's lengths, or None; flow ``logprob_flow``'s attn_logprob
-        [B, T, L] as ``forward`` returns it, or None)."""
+        [B, T, L] as ``forward`` returns it, or None; with ``return_terms`` (log_s_list, gate logits, every flow's
+        attn_logprob) as ``forward`` returns them, or None)."""
         T, dev = mel.size(2), mel.device
         encoder_outputs = self._with_speaker(speaker_ids, self.encoder.infer_ragged_tokens(text, self.embedding, in_lens))
         mask = ~(torch.arange(encoder_outputs.size(0), device=dev)[None, :] < in_lens[:, None])[..., None]
@@ -982,10 +1000,11 @@ class Flowtron(nn.Module):
         past = torch.arange(T, device=dev)[:, None] >= out_lens[None, :]
         z = out[0].masked_fill_(past[:, :, None], 0.0)
         logp = None if logprob_flow is None else out[4][logprob_flow]
+        terms = (out[1], out[2], out[4]) if return_terms else None
         if not return_attns:
-            return z, None, logp
+            return z, None, logp, terms
         outside = past.t()[:, :, None] | mask.transpose(1, 2)                 # [B, T, 1] | [B, 1, L]
-        return z, [a.masked_fill(outside, 0.0) for a in out[3]], logp
+        return z, [a.masked_fill(outside, 0.0) for a in out[3]], logp, terms
 
     def infer(self, residual, speaker_ids, text, temperature=1.0, gate_threshold=0.5, attns=None, attn_prior=None):
         """residual [B, 80, T] -> (mel [B, 80, T'], attention_weights: per flow in application order, T' rows [B, 1, L]).
@@ -1158,7 +1177,7 @@ class Flowtron(nn.Module):
                                  f"in_lens {il.tolist()}")
         from .align import mas                  # align.py imports this module
         checked = self._encode_args(mel, speaker_ids, text, in_lens, out_lens, attn_prior, "Flowtron.align")
-        _, _, logp = self._encode_batch(mel, speaker_ids, text, attn_prior, *checked, False, int(flow))
+        _, _, logp, _ = self._encode_batch(mel, speaker_ids, text, attn_prior, *checked, False, int(flow))
         return mas(logp, checked[0], checked[1], time_reversed=isinstance(self.flows[flow], AR_Back_Step))
 
     def infer_durations(self, residual, speaker_ids, text, in_lens, durations, gate_threshold=1.0):
@@ -1202,6 +1221,92 @@ class Flowtron(nn.Module):
         n_frames = torch.where(kept, durations.clamp(min=0), 0).sum(1).to(torch.int32)
         attns = [hard_attention(durations, in_lens, T, time_reversed=isinstance(f, AR_Back_Step)) for f in self.flows]
         return self.infer_aligned(residual, speaker_ids, text, in_lens, attns, n_frames, gate_threshold)
+
+    def score(self, mel, speaker_ids, text, in_lens, out_lens, attn_prior=None, gate_target=None, *, sigma=1.0,
+              blank_logprob=-1):
+        """Per-utterance losses of a padded batch of recorded utterances under this model: which rows it handles badly.
+
+        mel [B, 80, T] f32, speaker_ids [B], text [B, L] int64, in_lens [B], out_lens [B], attn_prior [B, T, L] or None,
+        gate_target [B, T] or None (None: the collate's target, 1 from frame out_lens[b] - 1 on) -> dict of CUDA f32
+        tensors, FlowtronLoss's terms for each row on its own, without the batch mean:
+
+        * ``nll`` [B]: ``(sum_{t < out_lens[b], m} z^2 / (2 sigma^2) - sum_flows sum log_s) / (out_lens[b] * 80)``.  With
+          n_components > 1 the Gaussian term is the mixture NLL of FlowtronLoss(gm_loss=True), with the mixture parameters
+          from the MelEncoder run once on this padded batch, as ``forward`` runs it.  That encoder averages over the padded
+          length (the reference's mean over time), so mixture rows depend on the batch they come in.
+        * ``gate`` [B]: the mean gate BCE over the row's frames, or None when the model has no gate layer.
+        * ``ctc`` [n_flows, B]: flow f's attention-CTC cost of row b (AttentionCTCLoss's per-utterance term; a back step's
+          log-probabilities are read in its flipped time by the kernel's index map).
+
+        The batch losses follow from the rows: FlowtronLoss's ``loss`` = sum_b out_lens[b] nll[b] / sum_b out_lens[b], its
+        ``gate_loss`` likewise from ``gate``, and its ``loss_ctc`` = ``ctc.mean()``.
+
+        The mel -> z direction runs exactly as in ``encode``: eval semantics and no autograd state whatever
+        ``self.training`` is, the text encoder on its masked kernels, flows in launches of at most 32 utterances, and with
+        host lengths the same short / long row split, so every row of a model without the mixture equals its own B = 1
+        call bit for bit.  The per-row sums (``ft_nll_rows``, ``ft_gmm_nll_rows``) have a fixed order and no atomics.  Host
+        lengths are checked (ValueError); CUDA length tensors are trusted, and the call then makes no host
+        synchronisation, so it can be captured in a CUDA graph.  Texts of up to _lib.MAX_TEXT_LEN tokens."""
+        where = "Flowtron.score"
+        if gate_target is not None and mel.dim() == 3 and tuple(gate_target.shape) != (mel.size(0), mel.size(2)):
+            raise ValueError(f"gate_target must be [B, T] = {(mel.size(0), mel.size(2))}, got {tuple(gate_target.shape)}")
+        in_l, out_l, groups = self._encode_args(mel, speaker_ids, text, in_lens, out_lens, attn_prior, where)
+        B, M, T = mel.shape
+        if gate_target is not None and not gate_target.is_cuda:
+            raise FlowtronB200Error(f"{where} needs CUDA tensors: the sm_90a kernels are the only implementation")
+        mixture = hasattr(self, 'gaussian_mixture')
+        if mixture and self.gaussian_mixture.n_components > _lib.GMM_MAX_COMPONENTS:
+            raise ValueError(f"the mixture-NLL kernels take at most {_lib.GMM_MAX_COMPONENTS} components")
+        dev = mel.device
+        with torch.no_grad():
+            z, _, _, (log_s_list, gate, logprobs) = self._encode_batch(mel, speaker_ids, text, attn_prior, in_l, out_l,
+                                                                       groups, False, None, True)
+            gt = None
+            if gate is not None:
+                gt = (gate_target.float().contiguous() if gate_target is not None else
+                      (torch.arange(T, device=dev)[None, :] >= (out_l - 1)[:, None]).float())
+            rows = torch.empty(B, 4, device=dev)
+            _lib.nll_rows(z.contiguous(), [ls.float().contiguous() for ls in log_s_list],
+                          None if gate is None else gate.float().contiguous(), gt, out_l, rows)
+            n_el = rows[:, 3] * M
+            if mixture:
+                was = self.mel_encoder.training
+                self.mel_encoder.train(False)
+                try:
+                    emb = self.mel_encoder(mel, out_l)
+                finally:
+                    self.mel_encoder.train(was)
+                mean, log_var, prob = self.gaussian_mixture(emb, B)
+                gmm = torch.empty(B, device=dev)
+                _lib.gmm_nll_rows(z.contiguous(), out_l, mean.float().contiguous(), log_var.float().contiguous(),
+                                  prob.float().contiguous(), mean.size(0) == B, gmm)
+                nll = (gmm - rows[:, 1]) / n_el
+            else:
+                nll = (rows[:, 0] / (2 * sigma * sigma) - rows[:, 1]) / n_el
+            ctc = torch.empty(len(self.flows), B, device=dev)
+            dlp = torch.empty(B, T, text.size(1), device=dev)         # the kernel's gradient output, unused here
+            for f, lp in enumerate(logprobs):
+                _lib.attn_ctc_loss(lp.float().contiguous(), in_l, out_l, isinstance(self.flows[f], AR_Back_Step),
+                                   float(blank_logprob), ctc[f], dlp)
+        return {"nll": nll, "gate": None if gate is None else rows[:, 2] / rows[:, 3], "ctc": ctc}
+
+    def test_invertibility(self, residual, speaker_ids, text, temperature=1.0, gate_threshold=0.5, attns=None):
+        """flowtron.py:932-954: mean |forward(infer(residual)) - residual| over the frames ``infer`` produced (compared
+        back to front for an even number of flows, as the reference does).  Call it as ``infer``; temperature,
+        gate_threshold and attns go to ``infer``, and ``forward`` then runs with the attention temperature ``infer`` set.
+        Every row is taken as L tokens and the generated frame count long.  The reference expects 1e-5 or less in fp32;
+        both directions here use fp16 tensor-core operands, so the value can be larger."""
+        with torch.no_grad():
+            mel, _ = self.infer(residual, speaker_ids, text, temperature, gate_threshold, attns)
+            B, L, n = mel.size(0), text.size(-1), mel.size(2)
+            in_lens = torch.full((B,), L, dtype=torch.long, device=mel.device)
+            out_lens = torch.full((B,), n, dtype=torch.long, device=mel.device)
+            residual_recon = self.forward(mel, speaker_ids, text, in_lens, out_lens)[0]
+            residual_permuted = residual.permute(2, 0, 1)
+            if len(self.flows) % 2 == 0:
+                residual_permuted = torch.flip(residual_permuted, (0,))
+                residual_recon = torch.flip(residual_recon, (0,))
+            return (residual_recon - residual_permuted[0:residual_recon.shape[0]]).abs().mean()
 
     @staticmethod
     def set_temperature_and_gate(flow, temperature, gate_threshold):

@@ -195,6 +195,13 @@ int ft_ar_step_bwd_plan(const FtArStepDesc* d, const FtArStepWeights* grads, int
  * to the kernel by value: no upload, so the call can be captured in a CUDA graph). */
 int ft_nll_reduce(const float* z, const float* const* log_s_list, int n_flows, const float* gate,
                   const float* gate_target, const int* out_lens, int T, int B, int M, float* sums, void* stream);
+/* The same sums per utterance (Flowtron.score): rows_out [B, 4] fp32, row b = {sum z^2, sum_flows sum log_s,
+ * sum BCEWithLogits(gate, target), n} over its n = min(out_lens[b], T) frames (gate NULL: entry 2 is 0).  z / log_s
+ * [T, B, M], gate [T, B] or NULL, gate_target [B, T].  One CTA per row, fixed summation order, no atomics: a row's values
+ * do not depend on B, on the other rows or on T beyond its own length, and replays are bit-identical.  log_s_list as for
+ * ft_nll_reduce (host array of device pointers). */
+int ft_nll_rows(const float* z, const float* const* log_s_list, int n_flows, const float* gate,
+                const float* gate_target, const int* out_lens, int T, int B, int M, float* rows_out, void* stream);
 /* Gradients of g_nll*nll + g_gate*gate_loss w.r.t. z, every log_s (identical tensor), gate logits. */
 int ft_nll_grad(const float* z, const float* gate, const float* gate_target, const int* out_lens, int T, int B, int M,
                 float sigma, const float* sums, const float* g_nll, const float* g_gate, float* dz, float* dlog_s,
@@ -428,6 +435,11 @@ size_t ft_gmm_nll_scratch_bytes(const FtGmmDesc* d);
 /* sums[0] = nll, sums[1] = number of valid frames */
 int ft_gmm_nll_reduce(const FtGmmDesc* d, const float* z, const int* out_lens, const float* mean, const float* log_var,
                       const float* prob, float* sums, void* scratch, void* stream);
+/* The same NLL per utterance (Flowtron.score): rows_out [B] fp32, row b = -sum_{t < out_lens[b], m} logsumexp_k a_k.  Same
+ * scratch as ft_gmm_nll_reduce.  Each row is summed from its own partials in a fixed order: it does not depend on the other
+ * rows' data or on B (the mixture parameters themselves come from the caller). */
+int ft_gmm_nll_rows(const FtGmmDesc* d, const float* z, const int* out_lens, const float* mean, const float* log_var,
+                    const float* prob, float* rows_out, void* scratch, void* stream);
 /* gradients of g_nll[0] * nll: dz [T, B, M] (zero past the lengths), dprob [B, K], and dmean / dlog_var [B, M, K] (both NULL
  * when the Gaussians are shared buffers: per_row must then be 0 or they are ignored) -- all overwritten. */
 int ft_gmm_nll_grad(const FtGmmDesc* d, const float* z, const int* out_lens, const float* mean, const float* log_var,
