@@ -130,6 +130,34 @@ def check_text_len(L: int, where: str) -> None:
         raise ValueError(f"{where}: text length {L} > {MAX_TEXT_LEN} tokens (MAX_TEXT_LEN) is not supported")
 
 
+def ragged_lengths(v, B: int, hi: int, name: str) -> torch.Tensor:
+    """Per-row lengths of a padded batch: a CUDA tensor is trusted (only its size is checked, nothing is read on the
+    host); host values must be B integers in [1, hi] and come back as a CPU tensor."""
+    if torch.is_tensor(v) and v.is_cuda:
+        if v.dim() != 1 or v.numel() != B:
+            raise ValueError(f"{name} must hold {B} values, got shape {tuple(v.shape)}")
+        return v
+    t = torch.as_tensor(v)
+    if t.dim() != 1 or t.numel() != B:
+        raise ValueError(f"{name} must hold {B} values, got shape {tuple(t.shape)}")
+    if t.is_floating_point() or t.dtype == torch.bool:
+        raise ValueError(f"{name} must be integers")
+    if bool((t < 1).any()) or bool((t > hi).any()):
+        raise ValueError(f"{name} must lie in [1, {hi}], got {t.tolist()}")
+    return t
+
+
+def check_frames_cover_tokens(in_lens, out_lens) -> None:
+    """ValueError unless every row has at least as many frames as tokens, which a monotonic alignment needs.  Checked
+    only when both lengths are on the host (and of one shape); CUDA lengths are trusted and not read."""
+    if any(torch.is_tensor(v) and v.is_cuda for v in (in_lens, out_lens)):
+        return
+    il, ol = torch.as_tensor(in_lens), torch.as_tensor(out_lens)
+    if il.shape == ol.shape and bool((ol < il).any()):
+        raise ValueError(f"every row needs at least as many frames as tokens: out_lens {ol.tolist()}, "
+                         f"in_lens {il.tolist()}")
+
+
 def lib() -> ctypes.CDLL:
     global _lib
     if _lib is None:

@@ -25,8 +25,7 @@ import torch
 from torch import Tensor
 
 from . import _lib
-from ._lib import FlowtronB200Error
-from .flowtron import _ragged_lengths
+from ._lib import FlowtronB200Error, check_frames_cover_tokens, ragged_lengths
 
 
 def mas(logp: Tensor, in_lens, out_lens, time_reversed: bool = False):
@@ -53,11 +52,9 @@ def mas(logp: Tensor, in_lens, out_lens, time_reversed: bool = False):
     if B < 1 or T < 1 or L < 1:
         raise ValueError(f"logp is empty: {tuple(logp.shape)}")
     _lib.check_text_len(L, "mas")
-    in_lens = _ragged_lengths(in_lens, B, L, "in_lens")
-    out_lens = _ragged_lengths(out_lens, B, T, "out_lens")
-    if not in_lens.is_cuda and not out_lens.is_cuda and bool((out_lens < in_lens).any()):
-        raise ValueError(f"every row needs at least as many frames as tokens: out_lens {out_lens.tolist()}, "
-                         f"in_lens {in_lens.tolist()}")
+    in_lens = ragged_lengths(in_lens, B, L, "in_lens")
+    out_lens = ragged_lengths(out_lens, B, T, "out_lens")
+    check_frames_cover_tokens(in_lens, out_lens)
     if not logp.is_cuda:
         raise FlowtronB200Error("mas needs CUDA tensors: the sm_90a kernel is the only implementation")
     dev = logp.device
@@ -88,7 +85,7 @@ def hard_attention(durations: Tensor, in_lens, n_frames_max: int, time_reversed:
     _lib.check_text_len(L, "hard_attention")
     if isinstance(n_frames_max, bool) or int(n_frames_max) != n_frames_max or n_frames_max < 1:
         raise ValueError(f"n_frames_max must be a positive integer, got {n_frames_max}")
-    in_lens = _ragged_lengths(in_lens, B, L, "in_lens")
+    in_lens = ragged_lengths(in_lens, B, L, "in_lens")
     if not durations.is_cuda:
         raise FlowtronB200Error("hard_attention needs CUDA tensors: the sm_90a kernel is the only implementation")
     dev = durations.device

@@ -22,6 +22,7 @@ from torch.nn import functional as F
 
 from . import _lib
 from ._lib import FlowtronB200Error
+from .align import hard_attention, mas
 from .inference import ar_step_infer, ar_step_infer_trimmed, batch_major
 
 
@@ -725,21 +726,14 @@ class AR_Back_Step(nn.Module):
 _ATTN_OVERLAP_MIN_T = 320
 
 
-def _ragged_lengths(v, B: int, hi: int, name: str) -> Tensor:
-    """Per-row lengths for Flowtron.infer_batch: a CUDA tensor is trusted (only its size is checked); host values must be
-    B integers in [1, hi]."""
-    if torch.is_tensor(v) and v.is_cuda:
-        if v.dim() != 1 or v.numel() != B:
-            raise ValueError(f"{name} must hold {B} values, got shape {tuple(v.shape)}")
-        return v
-    t = torch.as_tensor(v)
-    if t.dim() != 1 or t.numel() != B:
-        raise ValueError(f"{name} must hold {B} values, got shape {tuple(t.shape)}")
-    if t.is_floating_point() or t.dtype == torch.bool:
-        raise ValueError(f"{name} must be integers")
-    if bool((t < 1).any()) or bool((t > hi).any()):
-        raise ValueError(f"{name} must lie in [1, {hi}], got {t.tolist()}")
-    return t
+def _key_padding_mask(in_lens: Tensor, L: int) -> Tensor:
+    """[B, L, 1], True at the padded tokens l >= in_lens[b]; built on in_lens's device, with no host read."""
+    return ~(torch.arange(L, device=in_lens.device)[None, :] < in_lens[:, None])[..., None]
+
+
+# Outputs of Flowtron._encode_rows by name -> the dimension their batch runs along ([T, B, ...]: 1, [B, T, L]: 0); the
+# other of dimensions 0 and 1 is time.  "log_s", "attns" and "attn_logprob" are per-flow lists.
+_ENCODE_BATCH_DIM = {"z": 1, "log_s": 1, "gate": 1, "attns": 0, "attn_logprob": 0}
 
 
 class Flowtron(nn.Module):
@@ -832,6 +826,11 @@ class Flowtron(nn.Module):
     def _encode(self, speaker_ids, text, in_lens):
         return self._with_speaker(speaker_ids, self.encoder.forward_tokens(text, self.embedding, in_lens))
 
+    def _encode_ragged(self, speaker_ids, text, in_lens):
+        """_encode on the Encoder's masked kernels without dropout (in_lens int32 on the device), as the padded-batch
+        entry points run it."""
+        return self._with_speaker(speaker_ids, self.encoder.infer_ragged_tokens(text, self.embedding, in_lens))
+
     def forward(self, mel, speaker_ids, text, in_lens, out_lens, attn_prior=None):
         """Texts of up to _lib.MAX_TEXT_LEN (1024) tokens; longer ones raise ValueError before any work."""
         mean, log_var, prob = None, None, None
@@ -874,7 +873,7 @@ class Flowtron(nn.Module):
                 mean, log_var, prob = self.gaussian_mixture(mel_embedding, mel_embedding.size(0))
         mel = mel.permute(2, 0, 1)
         # key-padding mask from the padded text length (== max(in_lens) by the collate contract): no .item() host sync
-        mask = ~(torch.arange(n_text, device=in_lens.device)[None, :] < in_lens[:, None])[..., None]
+        mask = _key_padding_mask(in_lens, n_text)
         split = self.n_streams > 1 and mel.is_cuda and B >= self.min_split_batch and out_lens is not None
         if not split:
             out = self._run_flows(mel, encoder_outputs, mask, out_lens, attn_prior, text_ready, text_slices)
@@ -916,95 +915,101 @@ class Flowtron(nn.Module):
         ``attns_list`` (row b left-aligned in that flow's own time order: an AR_Back_Step's rows run back to front over
         their out_lens[b] frames), zero at t >= out_lens[b] and l >= in_lens[b] -- what ``infer_aligned`` takes."""
         checked = self._encode_args(mel, speaker_ids, text, in_lens, out_lens, attn_prior, "Flowtron.encode")
-        z, attns, _, _ = self._encode_batch(mel, speaker_ids, text, attn_prior, *checked, return_attns)
-        z = z.permute(1, 2, 0)
-        return (z, attns) if return_attns else z
+        out = self._encode_batch(mel, speaker_ids, text, attn_prior, *checked, ("z", "attns") if return_attns else ("z",))
+        z = out["z"].permute(1, 2, 0)
+        return (z, out["attns"]) if return_attns else z
 
-    def _encode_args(self, mel, speaker_ids, text, in_lens, out_lens, attn_prior, where):
-        """encode's argument checks -> (in_lens, out_lens int32 on the device, groups: None, or for host lengths the
-        (rows, their longest) on each side of _ATTN_OVERLAP_MIN_T)."""
-        if mel.dim() != 3 or text.dim() != 2 or speaker_ids.dim() != 1:
-            raise ValueError(f"{where} expects mel [B, n_mel, T], speaker_ids [B] and text [B, L]")
-        B, _, T = mel.shape
+    def _batch_args(self, where, x, x_name, speaker_ids, text, in_lens, lens, lens_name, lens_hi=None, check=None,
+                    cuda=()):
+        """The argument checks every padded-batch entry point makes -> (B, T, L, in_lens, lens), the lengths int32 on x's
+        device (``lens`` None for an entry point without per-row frame lengths).
+
+        x [B, n_mel, T] (``x_name`` in the messages), speaker_ids [B], text [B, L] with L <= _lib.MAX_TEXT_LEN.  Host
+        in_lens must lie in [1, L] and host ``lens`` in [1, min(T, lens_hi)]; CUDA lengths are trusted and not read, so
+        the call makes no host synchronisation.  ``check(B, T, L)`` makes the entry point's own ValueError checks.  Every
+        ValueError comes before the CUDA check of x, text, speaker_ids and ``cuda``, and all of it before any allocation or
+        launch."""
+        if x.dim() != 3 or text.dim() != 2 or speaker_ids.dim() != 1:
+            raise ValueError(f"{where} expects {x_name} [B, n_mel, T], speaker_ids [B] and text [B, L]")
+        B, _, T = x.shape
         L = text.size(1)
         _lib.check_text_len(L, where)
         if text.size(0) != B or speaker_ids.size(0) != B or B < 1 or T < 1 or L < 1:
-            raise ValueError(f"batch sizes disagree or are empty: mel {tuple(mel.shape)}, "
+            raise ValueError(f"{where}: batch sizes disagree or are empty: {x_name} {tuple(x.shape)}, "
                              f"speaker_ids {tuple(speaker_ids.shape)}, text {tuple(text.shape)}")
-        if attn_prior is not None and tuple(attn_prior.shape) != (B, T, L):
-            raise ValueError(f"attn_prior must be [B, T, L] = {(B, T, L)}, got {tuple(attn_prior.shape)}")
-        in_lens = _ragged_lengths(in_lens, B, L, "in_lens")
-        out_lens = _ragged_lengths(out_lens, B, T, "out_lens")
-        if not (mel.is_cuda and text.is_cuda and speaker_ids.is_cuda and (attn_prior is None or attn_prior.is_cuda)):
+        if check is not None:
+            check(B, T, L)
+        in_lens = _lib.ragged_lengths(in_lens, B, L, "in_lens")
+        if lens is not None:
+            lens = _lib.ragged_lengths(lens, B, T if lens_hi is None else min(T, lens_hi), lens_name)
+        if not all(t.is_cuda for t in (x, text, speaker_ids, *cuda)):
             raise FlowtronB200Error(f"{where} needs CUDA tensors: the sm_90a kernels are the only implementation")
-        dev = mel.device
+        dev = x.device
+        return (B, T, L, in_lens.to(device=dev, dtype=torch.int32),
+                None if lens is None else lens.to(device=dev, dtype=torch.int32))
+
+    def _encode_args(self, mel, speaker_ids, text, in_lens, out_lens, attn_prior, where, cuda=()):
+        """encode's argument checks (``cuda``: more tensors that must be on the device) -> (in_lens, out_lens int32 on the
+        device, groups: None, or for host lengths the (rows, their longest) on each side of _ATTN_OVERLAP_MIN_T)."""
+        def check(B, T, L):
+            if attn_prior is not None and tuple(attn_prior.shape) != (B, T, L):
+                raise ValueError(f"{where}: attn_prior must be [B, T, L] = {(B, T, L)}, got {tuple(attn_prior.shape)}")
+        host = not (torch.is_tensor(out_lens) and out_lens.is_cuda)
+        if attn_prior is not None:
+            cuda = (*cuda, attn_prior)
+        B, _, _, in_lens, out_l = self._batch_args(where, mel, "mel", speaker_ids, text, in_lens, out_lens, "out_lens",
+                                                   check=check, cuda=cuda)
         groups = None                       # host lengths: (rows, their longest) on each side of _ATTN_OVERLAP_MIN_T
-        if not out_lens.is_cuda:
-            lens = out_lens.tolist()
+        if host:
+            lens = torch.as_tensor(out_lens).tolist()
             short = [b for b in range(B) if lens[b] < _ATTN_OVERLAP_MIN_T]
             long_rows = [b for b in range(B) if lens[b] >= _ATTN_OVERLAP_MIN_T]
             groups = [(rows, max(lens[b] for b in rows)) for rows in (short, long_rows) if rows]
-        return in_lens.to(device=dev, dtype=torch.int32), out_lens.to(device=dev, dtype=torch.int32), groups
+        return in_lens, out_l, groups
 
-    def _encode_batch(self, mel, speaker_ids, text, attn_prior, in_lens, out_lens, groups, return_attns, logprob_flow=None,
-                      return_terms=False):
-        """encode's work on checked inputs, one _encode_rows call per row group -> (z [T, B, 80], the flows' attention or
-        None, flow ``logprob_flow``'s attn_logprob [B, T, L] (defined inside each row's lengths) or None, and with
-        ``return_terms`` the loss terms the flows produced as ``forward`` returns them -- (log_s_list [T, B, 80] each, gate
-        logits [T, B, 1] or None, every flow's attn_logprob [B, T, L]), defined inside each row's lengths -- or None)."""
-        B, _, T = mel.shape
-        L = text.size(1)
-        dev = mel.device
+    def _encode_batch(self, mel, speaker_ids, text, attn_prior, in_lens, out_lens, groups, outputs):
+        """encode's work on checked inputs, one _encode_rows call per row group -> _encode_rows's ``outputs`` for the
+        whole batch: each group's rows scattered into zeros of the batch's B and T."""
+        B, T = mel.size(0), mel.size(2)
         with torch.no_grad():
             if groups is None or groups == [(list(range(B)), T)]:
-                return self._encode_rows(mel, speaker_ids, text, in_lens, out_lens, attn_prior, return_attns, logprob_flow,
-                                         return_terms)
-            z = torch.zeros(T, B, mel.size(1), device=dev)
-            attns = [torch.zeros(B, T, L, device=dev) for _ in self.flows] if return_attns else None
-            logp = None if logprob_flow is None else torch.zeros(B, T, L, device=dev)
-            terms = None
+                return self._encode_rows(mel, speaker_ids, text, in_lens, out_lens, attn_prior, outputs)
+            full = {}
             for rows, t in groups:
-                idx = torch.tensor(rows, device=dev)
+                idx = torch.tensor(rows, device=mel.device)
                 prior = None if attn_prior is None else attn_prior[idx, :t]
-                zg, ag, lg, tg = self._encode_rows(mel[idx, :, :t], speaker_ids[idx], text[idx], in_lens[idx], out_lens[idx],
-                                                   prior, return_attns, logprob_flow, return_terms)
-                z[:t].index_copy_(1, idx, zg)
-                for a, g in zip(attns or (), ag or ()):
-                    a[:, :t].index_copy_(0, idx, g)
-                if logp is not None:
-                    logp[:, :t].index_copy_(0, idx, lg)
-                if return_terms:
-                    if terms is None:
-                        terms = ([torch.zeros(T, B, mel.size(1), device=dev) for _ in self.flows],
-                                 None if tg[1] is None else torch.zeros(T, B, 1, device=dev),
-                                 [torch.zeros(B, T, L, device=dev) for _ in self.flows])
-                    for full, g in zip(terms[0], tg[0]):
-                        full[:t].index_copy_(1, idx, g)
-                    if tg[1] is not None:
-                        terms[1][:t].index_copy_(1, idx, tg[1])
-                    for full, g in zip(terms[2], tg[2]):
-                        full[:, :t].index_copy_(0, idx, g)
-        return z, attns, logp, terms
+                part = self._encode_rows(mel[idx, :, :t], speaker_ids[idx], text[idx], in_lens[idx], out_lens[idx], prior,
+                                         outputs)
+                for key, v in part.items():
+                    bd = _ENCODE_BATCH_DIM[key if isinstance(key, str) else key[0]]       # time is dimension 1 - bd
+                    vs = v if isinstance(v, list) else [v]
+                    if key not in full:
+                        full[key] = [None if g is None else g.new_zeros(((T, B) if bd else (B, T)) + g.shape[2:])
+                                     for g in vs]
+                    for dst, g in zip(full[key], vs):
+                        if g is not None:
+                            dst.narrow(1 - bd, 0, t).index_copy_(bd, idx, g)
+        return {k: v if isinstance(part[k], list) else v[0] for k, v in full.items()}
 
-    def _encode_rows(self, mel, speaker_ids, text, in_lens, out_lens, attn_prior, return_attns=False, logprob_flow=None,
-                     return_terms=False):
-        """Flowtron.encode's work on checked inputs (lengths int32 on the device) -> (z [T, B, 80], zero past out_lens;
-        the flows' attention [B, T, L] zeroed outside each row's lengths, or None; flow ``logprob_flow``'s attn_logprob
-        [B, T, L] as ``forward`` returns it, or None; with ``return_terms`` (log_s_list, gate logits, every flow's
-        attn_logprob) as ``forward`` returns them, or None)."""
+    def _encode_rows(self, mel, speaker_ids, text, in_lens, out_lens, attn_prior, outputs):
+        """Flowtron.encode's work on checked inputs (lengths int32 on the device) -> {name: output} for each name in
+        ``outputs``: "z" [T, B, 80], zero past out_lens; "attns", the flows' attention [B, T, L] zeroed outside each row's
+        lengths; and as ``forward`` returns them, defined inside each row's lengths, "log_s" (every flow's [T, B, 80]),
+        "gate" (logits [T, B, 1], or None without a gate layer) and "attn_logprob" (every flow's [B, T, L]).  A name may
+        also be (name, f): flow f's tensor of a per-flow output.  Only what ``outputs`` names is masked."""
         T, dev = mel.size(2), mel.device
-        encoder_outputs = self._with_speaker(speaker_ids, self.encoder.infer_ragged_tokens(text, self.embedding, in_lens))
-        mask = ~(torch.arange(encoder_outputs.size(0), device=dev)[None, :] < in_lens[:, None])[..., None]
-        out = self._run_flows(mel.permute(2, 0, 1), encoder_outputs, mask, out_lens, attn_prior)
-        # forward leaves frames at or past out_lens[b] undefined
-        past = torch.arange(T, device=dev)[:, None] >= out_lens[None, :]
-        z = out[0].masked_fill_(past[:, :, None], 0.0)
-        logp = None if logprob_flow is None else out[4][logprob_flow]
-        terms = (out[1], out[2], out[4]) if return_terms else None
-        if not return_attns:
-            return z, None, logp, terms
-        outside = past.t()[:, :, None] | mask.transpose(1, 2)                 # [B, T, 1] | [B, 1, L]
-        return z, [a.masked_fill(outside, 0.0) for a in out[3]], logp, terms
+        encoder_outputs = self._encode_ragged(speaker_ids, text, in_lens)
+        mask = _key_padding_mask(in_lens, encoder_outputs.size(0))
+        z, log_s, gate, attns, logprobs = self._run_flows(mel.permute(2, 0, 1), encoder_outputs, mask, out_lens, attn_prior)
+        out = {"log_s": log_s, "gate": gate, "attn_logprob": logprobs}
+        if "z" in outputs or "attns" in outputs:
+            # forward leaves frames at or past out_lens[b] undefined
+            past = torch.arange(T, device=dev)[:, None] >= out_lens[None, :]
+            out["z"] = z.masked_fill_(past[:, :, None], 0.0)
+            if "attns" in outputs:
+                outside = past.t()[:, :, None] | mask.transpose(1, 2)                 # [B, T, 1] | [B, 1, L]
+                out["attns"] = [a.masked_fill(outside, 0.0) for a in attns]
+        return {k: out[k] if isinstance(k, str) else out[k[0]][k[1]] for k in outputs}
 
     def infer(self, residual, speaker_ids, text, temperature=1.0, gate_threshold=0.5, attns=None, attn_prior=None):
         """residual [B, 80, T] -> (mel [B, 80, T'], attention_weights: per flow in application order, T' rows [B, 1, L]).
@@ -1022,8 +1027,7 @@ class Flowtron(nn.Module):
             if any(a.size(1) < T for a in attns):
                 raise ValueError(f"attns cover {[a.size(1) for a in attns]} frames, residual has {T}")
         encoder_outputs = self._with_speaker(speaker_ids, self.encoder.infer_tokens(text, self.embedding))
-        for flow in self.flows:
-            self.set_temperature_and_gate(flow, temperature, gate_threshold)
+        self._set_gate(gate_threshold, temperature)
         out, attention, n_frames = self._infer_flows(residual, encoder_outputs, None, None, attns, attn_prior)
         n = int(n_frames.max().item())
         if n < T:                               # only a gate stops a row before T here
@@ -1063,26 +1067,17 @@ class Flowtron(nn.Module):
         run in slices of at most 16 utterances per kernel launch.  Forced alignments (``attns``) and ``attn_prior`` are
         not supported here."""
         if attns is not None or attn_prior is not None:
-            raise ValueError("infer_batch does not take attns or attn_prior (use infer)")
-        if residual.dim() != 3 or text.dim() != 2 or speaker_ids.dim() != 1:
-            raise ValueError("infer_batch expects residual [B, n_mel, T], speaker_ids [B] and text [B, L]")
-        B, _, T = residual.shape
-        L = text.size(1)
-        if text.size(0) != B or speaker_ids.size(0) != B or B < 1 or T < 1 or L < 1:
-            raise ValueError(f"batch sizes disagree or are empty: residual {tuple(residual.shape)}, "
-                             f"speaker_ids {tuple(speaker_ids.shape)}, text {tuple(text.shape)}")
-        if L > 256:             # the ragged entry point is validated up to 256 tokens; infer takes up to MAX_TEXT_LEN
-            raise ValueError(f"text length {L} > 256 is not supported by the inference kernel")
-        in_lens = _ragged_lengths(in_lens, B, L, "in_lens")
-        max_frames = _ragged_lengths([T] * B if max_frames is None else max_frames, B, T, "max_frames")
-        if not (residual.is_cuda and text.is_cuda and speaker_ids.is_cuda):
-            raise FlowtronB200Error("Flowtron.infer_batch needs CUDA tensors: the sm_90a kernels are the only implementation")
-        dev = residual.device
-        in_lens = in_lens.to(device=dev, dtype=torch.int32)
-        lens = max_frames.to(device=dev, dtype=torch.int32)
-        encoder_outputs = self._with_speaker(speaker_ids, self.encoder.infer_ragged_tokens(text, self.embedding, in_lens))
-        for flow in self.flows:
-            self.set_temperature_and_gate(flow, temperature, gate_threshold)
+            raise ValueError("Flowtron.infer_batch does not take attns or attn_prior (use infer)")
+
+        def check(B, T, L):
+            if L > 256:         # the ragged entry point is validated up to 256 tokens; infer takes up to MAX_TEXT_LEN
+                raise ValueError(f"Flowtron.infer_batch: text length {L} > 256 is not supported by the inference kernel")
+        if max_frames is None and residual.dim() == 3:
+            max_frames = [residual.size(2)] * residual.size(0)
+        _, _, _, in_lens, lens = self._batch_args("Flowtron.infer_batch", residual, "residual", speaker_ids, text, in_lens,
+                                                  max_frames, "max_frames", check=check)
+        encoder_outputs = self._encode_ragged(speaker_ids, text, in_lens)
+        self._set_gate(gate_threshold, temperature)
         out, attention, lens = self._infer_flows(residual, encoder_outputs, in_lens, lens)
         return out.permute(1, 2, 0), lens.long(), [a.transpose(0, 1) for a in attention]
 
@@ -1105,34 +1100,21 @@ class Flowtron(nn.Module):
         Texts of up to _lib.MAX_TEXT_LEN tokens, any B (slices of 16 utterances per kernel launch), rows in any length
         order.  Host lengths are checked (ValueError unless 1 <= in_lens[b] <= L and 1 <= n_frames[b] <= min(T, Ta)); CUDA
         length tensors are trusted and the call then makes no host synchronisation, so it can be captured in a CUDA graph."""
-        if residual.dim() != 3 or text.dim() != 2 or speaker_ids.dim() != 1:
-            raise ValueError("infer_aligned expects residual [B, n_mel, T], speaker_ids [B] and text [B, L]")
-        B, _, T = residual.shape
-        L = text.size(1)
-        _lib.check_text_len(L, "Flowtron.infer_aligned")
-        if text.size(0) != B or speaker_ids.size(0) != B or B < 1 or T < 1 or L < 1:
-            raise ValueError(f"batch sizes disagree or are empty: residual {tuple(residual.shape)}, "
-                             f"speaker_ids {tuple(speaker_ids.shape)}, text {tuple(text.shape)}")
+        where = "Flowtron.infer_aligned"
         if not isinstance(attns, (list, tuple)) or len(attns) != len(self.flows):
-            raise ValueError(f"attns must be a list of {len(self.flows)} tensors, one per flow")
+            raise ValueError(f"{where}: attns must be a list of {len(self.flows)} tensors, one per flow")
         Ta = attns[0].size(1) if torch.is_tensor(attns[0]) and attns[0].dim() == 3 else 0
-        for a in attns:
-            if not torch.is_tensor(a) or tuple(a.shape) != (B, Ta, L) or Ta < 1 or not a.is_floating_point():
-                raise ValueError(f"every attns[f] must be a float tensor [B, Ta, L] = ({B}, Ta, {L}), got "
-                                 f"{tuple(a.shape) if torch.is_tensor(a) else type(a).__name__}")
-        in_lens = _ragged_lengths(in_lens, B, L, "in_lens")
-        lens = _ragged_lengths(n_frames, B, min(T, Ta), "n_frames")
-        if not (residual.is_cuda and text.is_cuda and speaker_ids.is_cuda and all(a.is_cuda for a in attns)):
-            raise FlowtronB200Error("Flowtron.infer_aligned needs CUDA tensors: the sm_90a kernels are the only implementation")
-        dev = residual.device
-        in_lens = in_lens.to(device=dev, dtype=torch.int32)
-        lens = lens.to(device=dev, dtype=torch.int32)
+
+        def check(B, T, L):
+            for a in attns:
+                if not torch.is_tensor(a) or tuple(a.shape) != (B, Ta, L) or Ta < 1 or not a.is_floating_point():
+                    raise ValueError(f"{where}: every attns[f] must be a float tensor [B, Ta, L] = ({B}, Ta, {L}), got "
+                                     f"{tuple(a.shape) if torch.is_tensor(a) else type(a).__name__}")
+        _, _, _, in_lens, lens = self._batch_args(where, residual, "residual", speaker_ids, text, in_lens, n_frames,
+                                                  "n_frames", Ta, check, attns)
         with torch.no_grad():
-            encoder_outputs = self._with_speaker(speaker_ids, self.encoder.infer_ragged_tokens(text, self.embedding, in_lens))
-            for flow in self.flows:
-                step = getattr(flow, "ar_step", flow)
-                if hasattr(step, 'gate_layer'):
-                    step.gate_threshold = gate_threshold
+            encoder_outputs = self._encode_ragged(speaker_ids, text, in_lens)
+            self._set_gate(gate_threshold)                  # the temperature stays as it is
             out, _, lens = self._infer_flows(residual, encoder_outputs, in_lens, lens, attns)
         return out.permute(1, 2, 0), lens.long()
 
@@ -1169,15 +1151,11 @@ class Flowtron(nn.Module):
         (ValueError); with CUDA length tensors such a row gets zero durations and -1 everywhere, and the call makes no host
         synchronisation, so it can be captured in a CUDA graph."""
         if isinstance(flow, bool) or not isinstance(flow, (int, np.integer)) or not 0 <= flow < len(self.flows):
-            raise ValueError(f"flow must be a flow index in [0, {len(self.flows)}), got {flow!r}")
-        if not any(torch.is_tensor(v) and v.is_cuda for v in (in_lens, out_lens)):
-            il, ol = torch.as_tensor(in_lens), torch.as_tensor(out_lens)
-            if il.shape == ol.shape and bool((ol < il).any()):
-                raise ValueError(f"every row needs at least as many frames as tokens: out_lens {ol.tolist()}, "
-                                 f"in_lens {il.tolist()}")
-        from .align import mas                  # align.py imports this module
+            raise ValueError(f"Flowtron.align: flow must be a flow index in [0, {len(self.flows)}), got {flow!r}")
+        _lib.check_frames_cover_tokens(in_lens, out_lens)
         checked = self._encode_args(mel, speaker_ids, text, in_lens, out_lens, attn_prior, "Flowtron.align")
-        _, _, logp, _ = self._encode_batch(mel, speaker_ids, text, attn_prior, *checked, False, int(flow))
+        key = ("attn_logprob", int(flow))
+        logp = self._encode_batch(mel, speaker_ids, text, attn_prior, *checked, (key,))[key]
         return mas(logp, checked[0], checked[1], time_reversed=isinstance(self.flows[flow], AR_Back_Step))
 
     def infer_durations(self, residual, speaker_ids, text, in_lens, durations, gate_threshold=1.0):
@@ -1193,29 +1171,21 @@ class Flowtron(nn.Module):
         Host durations are checked (ValueError unless they are non-negative and every row sums to between 1 and T), as are
         host in_lens (1 <= in_lens[b] <= L); CUDA tensors are trusted, and then the call makes no host synchronisation and
         can be captured in a CUDA graph."""
-        if residual.dim() != 3 or text.dim() != 2 or speaker_ids.dim() != 1:
-            raise ValueError("infer_durations expects residual [B, n_mel, T], speaker_ids [B] and text [B, L]")
-        B, _, T = residual.shape
-        L = text.size(1)
-        _lib.check_text_len(L, "Flowtron.infer_durations")
-        if text.size(0) != B or speaker_ids.size(0) != B or B < 1 or T < 1 or L < 1:
-            raise ValueError(f"batch sizes disagree or are empty: residual {tuple(residual.shape)}, "
-                             f"speaker_ids {tuple(speaker_ids.shape)}, text {tuple(text.shape)}")
-        if (not torch.is_tensor(durations) or tuple(durations.shape) != (B, L) or durations.is_floating_point()
-                or durations.dtype == torch.bool):
-            raise ValueError(f"durations must be an integer tensor [B, L] = ({B}, {L}), got "
-                             f"{tuple(durations.shape) if torch.is_tensor(durations) else type(durations).__name__}")
-        in_lens = _ragged_lengths(in_lens, B, L, "in_lens")
-        if not durations.is_cuda:
-            sums = durations.sum(1)
-            if bool((durations < 0).any()) or bool((sums < 1).any()) or bool((sums > T).any()):
-                raise ValueError(f"durations must be non-negative with row sums in [1, {T}], got row sums {sums.tolist()}")
-        if not (residual.is_cuda and text.is_cuda and speaker_ids.is_cuda):
-            raise FlowtronB200Error("Flowtron.infer_durations needs CUDA tensors: the sm_90a kernels are the only "
-                                    "implementation")
-        from .align import hard_attention       # align.py imports this module
+        where = "Flowtron.infer_durations"
+
+        def check(B, T, L):
+            if (not torch.is_tensor(durations) or tuple(durations.shape) != (B, L) or durations.is_floating_point()
+                    or durations.dtype == torch.bool):
+                raise ValueError(f"{where}: durations must be an integer tensor [B, L] = ({B}, {L}), got "
+                                 f"{tuple(durations.shape) if torch.is_tensor(durations) else type(durations).__name__}")
+            if not durations.is_cuda:
+                sums = durations.sum(1)
+                if bool((durations < 0).any()) or bool((sums < 1).any()) or bool((sums > T).any()):
+                    raise ValueError(f"{where}: durations must be non-negative with row sums in [1, {T}], got row sums "
+                                     f"{sums.tolist()}")
+        _, T, L, in_lens, _ = self._batch_args(where, residual, "residual", speaker_ids, text, in_lens, None, None,
+                                               check=check)
         dev = residual.device
-        in_lens = in_lens.to(device=dev, dtype=torch.int32)
         durations = durations.to(device=dev)
         kept = torch.arange(L, device=dev)[None, :] < in_lens[:, None]
         n_frames = torch.where(kept, durations.clamp(min=0), 0).sum(1).to(torch.int32)
@@ -1249,18 +1219,18 @@ class Flowtron(nn.Module):
         synchronisation, so it can be captured in a CUDA graph.  Texts of up to _lib.MAX_TEXT_LEN tokens."""
         where = "Flowtron.score"
         if gate_target is not None and mel.dim() == 3 and tuple(gate_target.shape) != (mel.size(0), mel.size(2)):
-            raise ValueError(f"gate_target must be [B, T] = {(mel.size(0), mel.size(2))}, got {tuple(gate_target.shape)}")
-        in_l, out_l, groups = self._encode_args(mel, speaker_ids, text, in_lens, out_lens, attn_prior, where)
-        B, M, T = mel.shape
-        if gate_target is not None and not gate_target.is_cuda:
-            raise FlowtronB200Error(f"{where} needs CUDA tensors: the sm_90a kernels are the only implementation")
+            raise ValueError(f"{where}: gate_target must be [B, T] = {(mel.size(0), mel.size(2))}, got {tuple(gate_target.shape)}")
         mixture = hasattr(self, 'gaussian_mixture')
         if mixture and self.gaussian_mixture.n_components > _lib.GMM_MAX_COMPONENTS:
-            raise ValueError(f"the mixture-NLL kernels take at most {_lib.GMM_MAX_COMPONENTS} components")
+            raise ValueError(f"{where}: the mixture-NLL kernels take at most {_lib.GMM_MAX_COMPONENTS} components")
+        in_l, out_l, groups = self._encode_args(mel, speaker_ids, text, in_lens, out_lens, attn_prior, where,
+                                                () if gate_target is None else (gate_target,))
+        B, M, T = mel.shape
         dev = mel.device
         with torch.no_grad():
-            z, _, _, (log_s_list, gate, logprobs) = self._encode_batch(mel, speaker_ids, text, attn_prior, in_l, out_l,
-                                                                       groups, False, None, True)
+            out = self._encode_batch(mel, speaker_ids, text, attn_prior, in_l, out_l, groups,
+                                     ("z", "log_s", "gate", "attn_logprob"))
+            z, log_s_list, gate, logprobs = out["z"], out["log_s"], out["gate"], out["attn_logprob"]
             gt = None
             if gate is not None:
                 gt = (gate_target.float().contiguous() if gate_target is not None else
@@ -1310,10 +1280,17 @@ class Flowtron(nn.Module):
 
     @staticmethod
     def set_temperature_and_gate(flow, temperature, gate_threshold):
+        """One flow's attention temperature (None: left as it is) and, if it has a gate, its gate threshold."""
         flow = flow.ar_step if hasattr(flow, "ar_step") else flow
-        flow.attention_layer.temperature = temperature
+        if temperature is not None:
+            flow.attention_layer.temperature = temperature
         if hasattr(flow, 'gate_layer'):
             flow.gate_threshold = gate_threshold
+
+    def _set_gate(self, gate_threshold, temperature=None):
+        """Every flow's gate threshold and, unless None, attention temperature, for the inverse direction."""
+        for flow in self.flows:
+            self.set_temperature_and_gate(flow, temperature, gate_threshold)
 
 
 # --------------------------------------------------------------------------------------------- loss

@@ -55,18 +55,7 @@ def posterior_mean(z: Tensor, out_lens, n_frames: int, lambd: float = 1e-4, aggr
         raise ValueError(f"z is empty: {tuple(z.shape)}")
     if M > 128:
         raise ValueError(f"the posterior-mean kernel takes at most 128 mel channels, got {M}")
-    if torch.is_tensor(out_lens) and out_lens.is_cuda:
-        if out_lens.dim() != 1 or out_lens.numel() != K:
-            raise ValueError(f"out_lens must hold {K} values, got shape {tuple(out_lens.shape)}")
-    else:
-        t = torch.as_tensor(out_lens)
-        if t.dim() != 1 or t.numel() != K:
-            raise ValueError(f"out_lens must hold {K} values, got shape {tuple(t.shape)}")
-        if t.is_floating_point() or t.dtype == torch.bool:
-            raise ValueError("out_lens must be integers")
-        if bool((t < 1).any()) or bool((t > T).any()):
-            raise ValueError(f"out_lens must lie in [1, {T}], got {t.tolist()}")
-        out_lens = t
+    out_lens = _lib.ragged_lengths(out_lens, K, T, "out_lens")
     if not z.is_cuda:
         raise FlowtronB200Error("posterior_mean needs CUDA tensors: the sm_90a kernel is the only implementation")
     dev = z.device

@@ -1,6 +1,5 @@
 """CPU: the float32 MAS restatement (oracle/align_oracle.py) on hand-worked cases and against exhaustive search, its
-one-hot maps, the argument checks of align.mas / align.hard_attention / Flowtron.align / Flowtron.infer_durations, and
-the register budget of the alignment kernels."""
+one-hot maps, the argument checks of align.mas / align.hard_attention, and the register budget of the alignment kernels."""
 import itertools
 import os
 import re
@@ -12,7 +11,6 @@ import pytest
 import torch
 
 from conftest import ROOT
-from flowtron_b200 import synth
 from oracle import align_oracle as O
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
@@ -139,67 +137,6 @@ def test_mas_and_hard_attention_argument_validation():
             align.hard_attention(*args)
     with pytest.raises(FlowtronB200Error):
         align.hard_attention(dur, [9, 4, 4], 20)
-
-
-@pytest.fixture(scope="module")
-def cpu_model():
-    from flowtron_b200.flowtron import Flowtron
-    cfg = dict(synth.DEFAULT_MODEL_CONFIG, n_flows=2, n_speakers=2)
-    m = Flowtron(**cfg)
-    m.load_state_dict(synth.synth_params(cfg, 3), strict=True)
-    return m.eval()
-
-
-def test_flowtron_align_argument_validation(cpu_model):
-    from flowtron_b200._lib import FlowtronB200Error
-    B, T, L = 3, 20, 9
-    mel = torch.zeros(B, 80, T)
-    spk = torch.zeros(B, dtype=torch.long)
-    text = torch.zeros(B, L, dtype=torch.long)
-    ok = ([9, 4, 4], [20, 7, 13])
-    for kw in [dict(flow=2), dict(flow=-1), dict(flow=True), dict(flow=0.0)]:
-        with pytest.raises(ValueError):
-            cpu_model.align(mel, spk, text, *ok, **kw)
-    for lens in [([9, 4, 4], [20, 21, 13]), ([9, 10, 4], [20, 7, 13]), ([9, 4, 4], [20, 3, 13]), ([9, 4], [20, 7, 13])]:
-        with pytest.raises(ValueError):
-            cpu_model.align(mel, spk, text, *lens)
-    with pytest.raises(ValueError):
-        cpu_model.align(mel, spk, text, *ok, attn_prior=torch.zeros(B, T, L + 1))
-    with pytest.raises(ValueError):
-        cpu_model.align(mel[:2], spk, text, *ok)
-    with pytest.raises(ValueError, match="1024"):
-        cpu_model.align(mel, spk, torch.zeros(B, 1025, dtype=torch.long), *ok)
-    with pytest.raises(FlowtronB200Error):
-        cpu_model.align(mel, spk, text, *ok)
-    with pytest.raises(FlowtronB200Error):
-        cpu_model.align(mel, spk, text, *ok, flow=1)
-
-
-def test_infer_durations_argument_validation(cpu_model):
-    from flowtron_b200._lib import FlowtronB200Error
-    B, T, L = 3, 20, 9
-    res = torch.zeros(B, 80, T)
-    spk = torch.zeros(B, dtype=torch.long)
-    text = torch.zeros(B, L, dtype=torch.long)
-    dur = torch.tensor([[2] * 9, [3, 1, 1, 2] + [0] * 5, [1] * 4 + [0] * 5])
-    bad = [
-        ([9, 4, 4], dur.float()),
-        ([9, 4, 4], dur[:2]),
-        ([9, 4, 4], dur[:, :8]),
-        ([9, 4, 4], dur.tolist()),
-        ([9, 4, 4], torch.cat([dur[:2], -dur[2:]])),                       # negative
-        ([9, 4, 4], torch.cat([dur[:2], torch.zeros(1, L, dtype=torch.long)])),   # an empty row
-        ([9, 4, 4], torch.cat([dur[:1] * 2, dur[1:]])),                    # 36 frames > T
-        ([9, 4, 10], dur),
-        ([9, 4], dur),
-    ]
-    for in_lens, d in bad:
-        with pytest.raises(ValueError):
-            cpu_model.infer_durations(res, spk, text, in_lens, d)
-    with pytest.raises(ValueError):
-        cpu_model.infer_durations(res[:2], spk, text, [9, 4, 4], dur)
-    with pytest.raises(FlowtronB200Error):
-        cpu_model.infer_durations(res, spk, text, [9, 4, 4], dur)
 
 
 @pytest.mark.skipif(not HAVE_NVCC, reason="nvcc not available")

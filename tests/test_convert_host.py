@@ -1,5 +1,5 @@
-"""CPU: argument checks of Flowtron.infer_aligned / convert / encode(return_attns=), the oracle's restatement of their
-contract against the reference-generated fixtures (tests/make_golden_convert.py) and what those fixtures cover."""
+"""CPU: the forced-alignment argument checks of the flow steps' infer_ragged, the oracle's restatement of Flowtron.convert's
+and Flowtron.infer_aligned's contract against the reference-generated fixtures (tests/make_golden_convert.py) and what those fixtures cover."""
 import os
 
 import numpy as np
@@ -8,6 +8,7 @@ import torch
 
 from conftest import GOLDEN
 from flowtron_b200 import synth
+from test_batch_args_host import cpu_model  # noqa: F401
 
 TAGS = ["f2", "f3", "long"]
 
@@ -22,79 +23,6 @@ def _params(g):
     kb = [k for k in p if k.endswith("gate_layer.linear_layer.bias")][0]
     p[kb] = torch.full_like(p[kb], float(g["gate_bias"]))
     return cfg, p
-
-
-@pytest.fixture(scope="module")
-def cpu_model():
-    from flowtron_b200.flowtron import Flowtron
-    cfg = dict(synth.DEFAULT_MODEL_CONFIG, n_flows=2, n_speakers=2)
-    m = Flowtron(**cfg)
-    m.load_state_dict(synth.synth_params(cfg, 3), strict=True)
-    return m.eval()
-
-
-def test_infer_aligned_argument_validation(cpu_model):
-    from flowtron_b200._lib import FlowtronB200Error
-    B, T, L = 3, 20, 9
-    res = torch.zeros(B, 80, T)
-    spk = torch.zeros(B, dtype=torch.long)
-    text = torch.zeros(B, L, dtype=torch.long)
-    attns = [torch.zeros(B, T, L)] * 2
-    ok = dict(in_lens=[9, 4, 4], attns=attns, n_frames=[20, 7, 13])
-    bad = [
-        dict(ok, in_lens=[9, 4]),                                # wrong count
-        dict(ok, in_lens=[9, 0, 4]),                             # empty text
-        dict(ok, in_lens=[9, 10, 4]),                            # longer than L
-        dict(ok, in_lens=[9.0, 4.0, 4.0]),
-        dict(ok, n_frames=[20, 21, 5]),                          # above T
-        dict(ok, n_frames=[20, 0, 5]),
-        dict(ok, n_frames=torch.tensor([20, 5])),
-        dict(ok, attns=attns[:1]),                               # one map per flow
-        dict(ok, attns=attns + attns[:1]),
-        dict(ok, attns=attns[0]),                                # not a list
-        dict(ok, attns=[torch.zeros(B, T, L), torch.zeros(B, T, L + 1)]),
-        dict(ok, attns=[torch.zeros(T, B, L)] * 2),              # time-major
-        dict(ok, attns=[torch.zeros(B, T, L, dtype=torch.long)] * 2),
-        dict(ok, attns=[torch.zeros(B, 12, L)] * 2),             # covers 12 frames, row 0 wants 20
-    ]
-    for kw in bad:
-        with pytest.raises(ValueError):
-            cpu_model.infer_aligned(res, spk, text, **kw)
-    with pytest.raises(ValueError):                              # batch sizes disagree
-        cpu_model.infer_aligned(res[:2], spk, text, **ok)
-    with pytest.raises(ValueError, match="1024"):                # over MAX_TEXT_LEN, before any device work
-        cpu_model.infer_aligned(res, spk, torch.zeros(B, 1025, dtype=torch.long), [9, 4, 4], [torch.zeros(B, T, 1025)] * 2,
-                                [20, 7, 13])
-    # valid arguments, but CPU tensors: there is no CPU implementation
-    with pytest.raises(FlowtronB200Error):
-        cpu_model.infer_aligned(res, spk, text, **ok)
-    with pytest.raises(FlowtronB200Error):                       # shorter maps are fine when no row needs more
-        cpu_model.infer_aligned(res, spk, text, [9, 4, 4], [torch.zeros(B, 12, L)] * 2, torch.tensor([12, 7, 9]))
-    with pytest.raises(FlowtronB200Error):                       # texts past 256 tokens are accepted
-        cpu_model.infer_aligned(res, spk, torch.zeros(B, 300, dtype=torch.long), [300, 4, 4], [torch.zeros(B, T, 300)] * 2,
-                                [20, 7, 13])
-
-
-def test_convert_and_encode_argument_validation(cpu_model):
-    from flowtron_b200._lib import FlowtronB200Error
-    B, T, L = 3, 20, 9
-    mel = torch.zeros(B, 80, T)
-    spk = torch.zeros(B, dtype=torch.long)
-    text = torch.zeros(B, L, dtype=torch.long)
-    with pytest.raises(ValueError):
-        cpu_model.convert(mel, spk, spk[:2], text, [9, 4, 4], [20, 7, 13])
-    with pytest.raises(ValueError):
-        cpu_model.convert(mel, spk, spk, text, [9, 4, 4], [20, 21, 13])
-    with pytest.raises(ValueError):
-        cpu_model.convert(mel, spk, spk, text, [9, 10, 4], [20, 7, 13])
-    with pytest.raises(ValueError):
-        cpu_model.convert(mel, spk, spk, text, [9, 4, 4], [20, 7, 13], attn_prior=torch.zeros(B, T, L + 1))
-    with pytest.raises(FlowtronB200Error):
-        cpu_model.convert(mel, spk, spk, text, [9, 4, 4], [20, 7, 13])
-    with pytest.raises(ValueError):
-        cpu_model.encode(mel, spk, text, [9, 4, 4], [20, 21, 13], return_attns=True)
-    with pytest.raises(FlowtronB200Error):
-        cpu_model.encode(mel, spk, text, [9, 4, 4], [20, 7, 13], return_attns=True)
 
 
 def test_flow_infer_ragged_forced_argument_validation(cpu_model):

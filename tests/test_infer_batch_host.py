@@ -1,4 +1,4 @@
-"""CPU: Flowtron.infer_batch argument checks, the oracle's restatement of its contract against the reference-generated
+"""CPU: the oracle's restatement of Flowtron.infer_batch's contract against the reference-generated
 fixtures (tests/make_golden_infer_batch.py), and the register budget of the inference kernels."""
 import os
 import re
@@ -24,47 +24,6 @@ def _params(g):
     p[kb] = torch.full_like(p[kb], float(g["gate_bias"]))
     p[kw] = p[kw] * float(g["gate_scale"])
     return cfg, p
-
-
-@pytest.fixture(scope="module")
-def cpu_model():
-    from flowtron_b200.flowtron import Flowtron
-    cfg = dict(synth.DEFAULT_MODEL_CONFIG, n_flows=2)
-    m = Flowtron(**cfg)
-    m.load_state_dict(synth.synth_params(cfg, 3), strict=True)
-    return m.eval()
-
-
-def test_argument_validation(cpu_model):
-    from flowtron_b200._lib import FlowtronB200Error
-    B, T, L = 3, 20, 9
-    res = torch.zeros(B, 80, T)
-    spk = torch.zeros(B, dtype=torch.long)
-    text = torch.zeros(B, L, dtype=torch.long)
-    bad = [
-        dict(in_lens=[9, 4]),                                   # wrong count
-        dict(in_lens=[9, 0, 4]),                                # empty text
-        dict(in_lens=[9, 10, 4]),                               # longer than L
-        dict(in_lens=torch.tensor([9, 4, 4, 4])),
-        dict(in_lens=[9.0, 4.0, 4.0]),
-        dict(in_lens=[9, 4, 4], max_frames=[20, 21, 5]),        # budget above T
-        dict(in_lens=[9, 4, 4], max_frames=[20, 0, 5]),
-        dict(in_lens=[9, 4, 4], max_frames=torch.tensor([20, 5])),
-        dict(in_lens=[9, 4, 4], attns=[torch.zeros(T, L)] * 2),
-        dict(in_lens=[9, 4, 4], attn_prior=torch.zeros(B, T, L)),
-    ]
-    for kw in bad:
-        with pytest.raises(ValueError):
-            cpu_model.infer_batch(res, spk, text, **kw)
-    with pytest.raises(ValueError):                             # longer than the kernel's 256 keys
-        cpu_model.infer_batch(res, spk, torch.zeros(B, 257, dtype=torch.long), [9, 4, 4])
-    with pytest.raises(ValueError):                             # batch sizes disagree
-        cpu_model.infer_batch(res[:2], spk, text, [9, 4, 4])
-    # valid arguments, but CPU tensors: there is no CPU implementation
-    with pytest.raises(FlowtronB200Error):
-        cpu_model.infer_batch(res, spk, text, [9, 4, 4], max_frames=[20, 7, 13])
-    with pytest.raises(FlowtronB200Error):
-        cpu_model.infer_batch(res, spk, text, torch.tensor([9, 4, 4]))
 
 
 @pytest.mark.parametrize("tag", ["f2", "f3", "t400"])

@@ -13,6 +13,7 @@ import torch
 
 from conftest import GOLDEN, ROOT
 from flowtron_b200 import synth
+from test_batch_args_host import cpu_model  # noqa: F401
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 HAVE_NVCC = os.path.exists(NVCC) or shutil.which("nvcc") is not None
@@ -24,15 +25,6 @@ def test_header_library_and_python_constants_agree():
     m = re.search(r"#define\s+FT_MAX_TEXT_LEN\s+(\d+)", hdr)
     assert m and int(m.group(1)) == _lib.MAX_TEXT_LEN == 1024
     assert _lib.lib().ft_max_text_len() == _lib.MAX_TEXT_LEN
-
-
-@pytest.fixture(scope="module")
-def cpu_model():
-    from flowtron_b200.flowtron import Flowtron
-    cfg = dict(synth.DEFAULT_MODEL_CONFIG, n_flows=2)
-    m = Flowtron(**cfg)
-    m.load_state_dict(synth.synth_params(cfg, 3), strict=True)
-    return m.eval()
 
 
 def test_forward_refuses_texts_over_the_limit_before_the_device_check(cpu_model):

@@ -1,4 +1,4 @@
-"""CPU: argument checks of Flowtron.encode and style.posterior_mean, the C-ABI declaration of ft_posterior_mean, its
+"""CPU: argument checks of style.posterior_mean, the C-ABI declaration of ft_posterior_mean, its
 rejections, the register budget of csrc/style.cu, and the float64 restatement behind the style-transfer fixtures
 (tests/make_golden_style_transfer.py)."""
 import ctypes
@@ -12,54 +12,9 @@ import pytest
 import torch
 
 from conftest import GOLDEN, ROOT
-from flowtron_b200 import synth
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 HAVE_NVCC = os.path.exists(NVCC) or shutil.which("nvcc") is not None
-
-
-@pytest.fixture(scope="module")
-def cpu_model():
-    from flowtron_b200.flowtron import Flowtron
-    cfg = dict(synth.DEFAULT_MODEL_CONFIG, n_flows=2)
-    m = Flowtron(**cfg)
-    m.load_state_dict(synth.synth_params(cfg, 3), strict=True)
-    return m.eval()
-
-
-def test_encode_argument_validation(cpu_model):
-    from flowtron_b200 import _lib
-    from flowtron_b200._lib import FlowtronB200Error
-    B, T, L = 3, 20, 9
-    mel = torch.zeros(B, 80, T)
-    spk = torch.zeros(B, dtype=torch.long)
-    text = torch.zeros(B, L, dtype=torch.long)
-    ok = dict(in_lens=[9, 4, 6], out_lens=[20, 7, 13])
-    bad = [
-        dict(ok, in_lens=[9, 4]),                               # wrong count
-        dict(ok, in_lens=[9, 0, 4]),                            # empty text
-        dict(ok, in_lens=[9, 10, 4]),                           # longer than L
-        dict(ok, in_lens=[9.0, 4.0, 4.0]),
-        dict(ok, out_lens=[20, 21, 5]),                         # longer than T
-        dict(ok, out_lens=[20, 0, 5]),
-        dict(ok, out_lens=torch.tensor([20, 5])),
-        dict(ok, attn_prior=torch.zeros(B, T, L + 1)),
-    ]
-    for kw in bad:
-        with pytest.raises(ValueError):
-            cpu_model.encode(mel, spk, text, **kw)
-    with pytest.raises(ValueError):                             # batch sizes disagree
-        cpu_model.encode(mel[:2], spk, text, **ok)
-    with pytest.raises(ValueError):                             # not [B, 80, T]
-        cpu_model.encode(mel[0], spk, text, **ok)
-    long_text = torch.zeros(B, _lib.MAX_TEXT_LEN + 1, dtype=torch.long)
-    with pytest.raises(ValueError, match="MAX_TEXT_LEN"):
-        cpu_model.encode(mel, spk, long_text, **ok)
-    # valid arguments, but CPU tensors: there is no CPU implementation
-    with pytest.raises(FlowtronB200Error):
-        cpu_model.encode(mel, spk, text, **ok)
-    with pytest.raises(FlowtronB200Error):
-        cpu_model.encode(mel, spk, text, torch.tensor([9, 4, 6]), torch.tensor([20, 7, 13]))
 
 
 def test_posterior_mean_argument_validation():
