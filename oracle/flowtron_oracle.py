@@ -256,7 +256,10 @@ def ar_back_step_infer(p, pre, residual, text, temperature=1.0, gate_threshold=0
 def _masked_instance_norm(x: Tensor, mask: Optional[Tensor], w: Tensor, b: Tensor, eps: float = 1e-5):
     """flowtron.py:53-92 with use_input_stats=True (track_running_stats=False)."""
     if mask is None:
-        return F.instance_norm(x, None, None, w, b, True, 0.1, eps)
+        if x.shape[-1] > 1:
+            return F.instance_norm(x, None, None, w, b, True, 0.1, eps)
+        # F.instance_norm refuses a single position; its statistics are the value itself and 0, as the masked form computes
+        mask = torch.ones_like(x[:, :1])
     lengths = mask.sum((-1,))
     mean = (x * mask).sum((-1,)) / lengths
     var = (((x - mean[..., None]) * mask) ** 2).sum((-1,)) / lengths

@@ -1,5 +1,7 @@
-"""GPU, BASELINE.json full sizes (configs[1]: B=32, T=1000, L<=160; configs[3]: T=1000 inference): the CPU oracle
-cannot run these in seconds, so parity is checked through size-independent properties (SURVEY.md §4 invariants)."""
+"""GPU, BASELINE.json full sizes (configs[1]: B=32, T=1000, L<=160; configs[3]: T=1000 inference): size-independent
+properties (SURVEY.md §4 invariants) of the forward pass and the inverse.  The training step at these sizes (forward
+outputs, losses and every parameter gradient, eager and replayed from one CUDA graph) is compared with the fp64 oracle,
+one utterance at a time, in tests/test_gpu_train_step_oracle.py."""
 import pytest
 import torch
 
@@ -74,29 +76,6 @@ def test_fullsize_batch_split_consistency_and_loss():
         gref = (torch.nn.functional.binary_cross_entropy_with_logits(gp, cu["gate_target"], reduction="none").permute(1, 0)
                 * mask[:, :, 0]).sum() / n
         assert abs(float(gl) - float(gref)) <= 1e-4 * abs(float(gref))
-
-
-def test_fullsize_training_step_is_finite_and_deterministic():
-    from flowtron_b200 import _lib
-    from flowtron_b200.flowtron import FlowtronLoss
-    cfg, cu = _batch(with_prior=True)
-    m = _model(cfg, seed=9).train()
-    m.encoder.p_dropout = 0.0
-    runs = []
-    for _ in range(2):
-        m.zero_grad(set_to_none=True)
-        out = m(cu["mel"], cu["speaker_ids"], cu["text"], cu["in_lens"], cu["out_lens"], cu["attn_prior"])
-        nll, gl, _ = FlowtronLoss()(out, cu["gate_target"], cu["in_lens"], cu["out_lens"])
-        (nll + gl).sum().backward()
-        torch.cuda.synchronize()
-        runs.append((float(nll.detach()), m.flows[0].lstm.weight_hh_l1.grad.clone(), m.flows[1].ar_step.conv.weight.grad.clone()))
-    assert _lib.device_status() == 0
-    for p in m.parameters():
-        assert p.grad is not None and torch.isfinite(p.grad).all()
-    assert abs(runs[0][0] - runs[1][0]) <= 1e-6 * abs(runs[0][0])   # loss sums use float atomics across blocks
-    # backward uses float atomics in the attention reductions: allow last-bit noise
-    assert (runs[0][1] - runs[1][1]).norm().item() <= 1e-3 * runs[0][1].norm().item()
-    assert (runs[0][2] - runs[1][2]).norm().item() <= 1e-3 * runs[0][2].norm().item()
 
 
 def test_fullsize_invertibility_T1000():
