@@ -716,12 +716,11 @@ def encoder_desc(B, L, masked, dropout_p, eps=1e-5):
     return FtEncoderDesc(B=B, L=L, C=512, n_convs=3, ksize=5, masked=1 if masked else 0, dropout_p=float(dropout_p), eps=float(eps))
 
 
-def _enc_struct(cls, prefix, tensors):
-    """tensors: dict name -> list of tensors, in ENC_PARAM_FIELDS order."""
+def _enc_struct(cls, prefix, tensors, fields):
+    """tensors: dict name -> list of tensors, in `fields` order (ENC_PARAM_FIELDS or MEL_ENC_PARAM_FIELDS)."""
     st = cls()
-    for n, k in ENC_PARAM_FIELDS:
-        arr = (c_void_p * k)(*[c_void_p(t.data_ptr()) for t in tensors[n]])
-        setattr(st, prefix + n, arr)
+    for n, k in fields:
+        setattr(st, prefix + n, (c_void_p * k)(*[c_void_p(t.data_ptr()) for t in tensors[n]]))
     return st
 
 
@@ -732,7 +731,7 @@ def encoder_fwd(desc, params, x, in_lens_i32, rng_state, out, out_stride_b, out_
     L = lib()
     saved = torch.empty(L.ft_encoder_saved_bytes(byref(desc)), dtype=torch.uint8, device=out.device)
     scratch = torch.empty(L.ft_encoder_fwd_scratch_bytes(byref(desc)), dtype=torch.uint8, device=out.device)
-    w = _enc_struct(FtEncoderWeights, "", params)
+    w = _enc_struct(FtEncoderWeights, "", params, ENC_PARAM_FIELDS)
     if tokens is None:
         check(L.ft_encoder_fwd(byref(desc), byref(w), ptr(x), ptr(in_lens_i32), ptr(rng_state), ptr(out), out_stride_b, out_stride_l,
                                ptr(saved), ptr(scratch), stream_ptr()), "ft_encoder_fwd")
@@ -751,8 +750,8 @@ def encoder_bwd(desc, params, d_out, saved, need_dx=True, tokens=None, emb_weigh
     dev = d_out.device
     grads = {n: [torch.empty_like(t) for t in params[n]] for n, _ in ENC_PARAM_FIELDS}
     scratch = torch.empty(L.ft_encoder_bwd_scratch_bytes(byref(desc)), dtype=torch.uint8, device=dev)
-    w = _enc_struct(FtEncoderWeights, "", params)
-    g = _enc_struct(FtEncoderGrads, "d_", grads)
+    w = _enc_struct(FtEncoderWeights, "", params, ENC_PARAM_FIELDS)
+    g = _enc_struct(FtEncoderGrads, "d_", grads, ENC_PARAM_FIELDS)
     if tokens is None:
         d_x = torch.empty(desc.B, 512, desc.L, dtype=torch.float32, device=dev) if need_dx else None
         check(L.ft_encoder_bwd(byref(desc), byref(w), ptr(d_out), d_out.stride(0), d_out.stride(1), ptr(saved), ptr(d_x), byref(g),
@@ -765,13 +764,6 @@ def encoder_bwd(desc, params, d_out, saved, need_dx=True, tokens=None, emb_weigh
 
 
 # ------------------------------------------------------------------------------------------------ mel encoder (GMM prior)
-def _mel_enc_struct(cls, prefix, tensors):
-    st = cls()
-    for n, k in MEL_ENC_PARAM_FIELDS:
-        setattr(st, prefix + n, (c_void_p * k)(*[c_void_p(t.data_ptr()) for t in tensors[n]]))
-    return st
-
-
 def mel_encoder_fwd(params, mel, out_lens_i32, all_lens_i32, rng_state, dropout_p, eps, emb):
     """ft_mel_encoder_fwd on mel [B, 80, T] (B <= 64) -> emb [B, 512] (written).  all_lens_i32: the whole batch's lengths (their
     maximum divides the time sum).  Returns (desc, saved) for mel_encoder_bwd."""
@@ -780,7 +772,7 @@ def mel_encoder_fwd(params, mel, out_lens_i32, all_lens_i32, rng_state, dropout_
     desc = FtMelEncoderDesc(B=mel.size(0), T=mel.size(2), eps=float(eps), dropout_p=float(dropout_p))
     saved = torch.empty(L.ft_mel_encoder_saved_bytes(byref(desc)), dtype=torch.uint8, device=mel.device)
     scratch = torch.empty(L.ft_mel_encoder_fwd_scratch_bytes(byref(desc)), dtype=torch.uint8, device=mel.device)
-    w = _mel_enc_struct(FtMelEncoderWeights, "", params)
+    w = _enc_struct(FtMelEncoderWeights, "", params, MEL_ENC_PARAM_FIELDS)
     check(L.ft_mel_encoder_fwd(byref(desc), byref(w), ptr(mel), ptr(out_lens_i32), ptr(all_lens_i32), all_lens_i32.numel(),
                                ptr(rng_state), ptr(emb), ptr(saved), ptr(scratch), stream_ptr()), "ft_mel_encoder_fwd")
     return desc, saved
@@ -792,8 +784,8 @@ def mel_encoder_bwd(desc, params, d_emb, saved):
     L = lib()
     grads = {n: [torch.empty_like(t) for t in params[n]] for n, _ in MEL_ENC_PARAM_FIELDS}
     scratch = torch.empty(L.ft_mel_encoder_bwd_scratch_bytes(byref(desc)), dtype=torch.uint8, device=d_emb.device)
-    w = _mel_enc_struct(FtMelEncoderWeights, "", params)
-    g = _mel_enc_struct(FtMelEncoderGrads, "d_", grads)
+    w = _enc_struct(FtMelEncoderWeights, "", params, MEL_ENC_PARAM_FIELDS)
+    g = _enc_struct(FtMelEncoderGrads, "d_", grads, MEL_ENC_PARAM_FIELDS)
     check(L.ft_mel_encoder_bwd(byref(desc), byref(w), ptr(d_emb), ptr(saved), byref(g), ptr(scratch), stream_ptr()),
           "ft_mel_encoder_bwd")
     return grads

@@ -22,6 +22,10 @@ int ft_set_error(const char* msg) {
     g_err = msg ? msg : "unknown error";
     return -1;
 }
+int ft_runtime_error(const char* who) {
+    g_err = std::string(who) + ": CUDA runtime call failed";
+    return -1;
+}
 int ft_check_launch(const char* what) {
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) {

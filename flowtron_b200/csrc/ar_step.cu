@@ -223,8 +223,6 @@ int check_desc(const FtArStepDesc& d) {
     return 0;
 }
 
-#define FT_TRY(x) do { if ((x) != 0) return -1; } while (0)
-
 // C = A[M,K] B[N,K]^T helpers -----------------------------------------------------------------------------
 int gemm_fwd(cudaStream_t st, long long M, int N, int K, const void* A, long long lda, const void* B, long long ldb,
              const float* bias, const float* bias2, int act, float* C32, long long ldc32, void* C16, long long ldc16) {

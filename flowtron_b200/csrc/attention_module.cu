@@ -280,8 +280,6 @@ int zero(void* p, size_t bytes, cudaStream_t st) {
     return cudaMemsetAsync(p, 0, bytes, st) == cudaSuccess ? 0 : ft_set_error("attention: cudaMemsetAsync failed");
 }
 
-#define FT_TRY(x) do { if ((x) != 0) return -1; } while (0)
-
 int attention_fwd(const FtAttentionDesc& d, const FtAttentionWeights& w, const float* queries, const float* keys, const float* values,
                   const int* in_lens, const float* prior, float* output, float* attn, float* logprob, void* saved, void* scratch,
                   cudaStream_t st) {

@@ -491,63 +491,6 @@ enc_bilstm_bwd_kernel(EncLstmBwdParams p) {
 }
 
 // ------------------------------------------------------------------------------------------------ host orchestration
-struct EncPlan {
-    // saved by the forward pass for the backward pass
-    __half* X16[4];        // block inputs x0..x3 (split fp16 grid [rows, 3 * 512])
-    float* Y32[3];         // conv outputs (fp32 grid)
-    float* mean[3]; float* rstd[3];
-    __half* hseq[2]; __half* gates[2]; float* cstate[2];
-    int* lens;             // int32 copy of in_lens (or nothing when unmasked)
-    // forward-only scratch
-    float* xproj; __half* wconv16; __half* wih16;
-    size_t saved_bytes, total_fwd;
-    // backward scratch
-    __half* dG[2]; __half* dY16; float* DX32; float* dwk; float* scale2; __half* wconv16_b; __half* wih16_b;
-    size_t total_bwd;
-};
-
-static EncPlan plan_enc(const FtEncoderDesc& d, uint8_t* saved, uint8_t* scratch, bool bwd) {
-    EncPlan P{};
-    const size_t rows = static_cast<size_t>(d.B) * (d.L + 2 * EPADR);
-    size_t off = 0;
-    auto get = [&](uint8_t* base, size_t bytes) { size_t o = off; off = (off + bytes + 255) & ~size_t(255); return base ? base + o : nullptr; };
-    for (int i = 0; i < 4; ++i) P.X16[i] = reinterpret_cast<__half*>(get(saved, rows * 3 * EC * 2));
-    for (int i = 0; i < 3; ++i) P.Y32[i] = reinterpret_cast<float*>(get(saved, rows * EC * 4));
-    for (int i = 0; i < 3; ++i) { P.mean[i] = reinterpret_cast<float*>(get(saved, size_t(d.B) * EC * 4)); P.rstd[i] = reinterpret_cast<float*>(get(saved, size_t(d.B) * EC * 4)); }
-    for (int k = 0; k < 2; ++k) {
-        P.hseq[k] = reinterpret_cast<__half*>(get(saved, rows * 2 * EH * 2));
-        P.gates[k] = reinterpret_cast<__half*>(get(saved, rows * EG * 2));
-        P.cstate[k] = reinterpret_cast<float*>(get(saved, rows * EH * 4));
-    }
-    P.lens = reinterpret_cast<int*>(get(saved, size_t(d.B) * 4 + 16));
-    P.saved_bytes = off;
-    off = 0;
-    if (!bwd) {
-        P.xproj = reinterpret_cast<float*>(get(scratch, rows * 2 * EG * 4));
-        P.wconv16 = reinterpret_cast<__half*>(get(scratch, size_t(3) * EK * EC * 3 * EC * 2));
-        P.wih16 = reinterpret_cast<__half*>(get(scratch, size_t(2) * EG * 3 * EC * 2));
-        P.total_fwd = off;
-    } else {
-        for (int k = 0; k < 2; ++k) P.dG[k] = reinterpret_cast<__half*>(get(scratch, rows * 3 * EG * 2));
-        P.dY16 = reinterpret_cast<__half*>(get(scratch, rows * 3 * EC * 2));
-        P.DX32 = reinterpret_cast<float*>(get(scratch, rows * EC * 4));
-        P.dwk = reinterpret_cast<float*>(get(scratch, size_t(EK) * EC * EC * 4));
-        P.scale2 = reinterpret_cast<float*>(get(scratch, 256));
-        P.wconv16_b = reinterpret_cast<__half*>(get(scratch, size_t(EK) * 3 * EC * EC * 2));
-        P.wih16_b = reinterpret_cast<__half*>(get(scratch, size_t(2) * 3 * EG * EC * 2));
-        P.total_bwd = off;
-    }
-    return P;
-}
-
-static int check_desc(const FtEncoderDesc* d) {
-    if (!d) return ft_set_error("encoder: NULL descriptor");
-    if (d->C != EC || d->n_convs != 3 || d->ksize != EK) return ft_set_error("encoder: this build supports 3 convolutions of kernel 5 over 512 channels");
-    if (d->B < 1 || d->B > 64 || d->L < 1) return ft_set_error("encoder: batch must be in [1, 64] per call");
-    if (d->dropout_p < 0.f || d->dropout_p >= 1.f) return ft_set_error("encoder: dropout_p must be in [0, 1)");
-    return 0;
-}
-
 template <int MT> static int launch_bilstm_fwd(const EncLstmFwdParams& p, cudaStream_t st) {
     enc_bilstm_fwd_kernel<MT><<<2 * ((p.B + 31) / 32) * ENC_CLUSTER, ENC_THREADS, 0, st>>>(p);
     ft_count_launch(1);
@@ -576,77 +519,211 @@ int enc_wgrad3(cudaStream_t st, int M, int N, long long K, const __half* A, int 
     return 0;
 }
 
+// ------------------------------------------------------------------------------------------------ conv -> norm -> BiLSTM stack
+EncStack enc_stack_plan(const EncStackDesc& a, int B, int L, bool masked, const void* saved, void* scratch, bool bwd) {
+    EncStack P{};
+    P.a = &a; P.B = B; P.L = L;
+    P.rows = static_cast<long long>(B) * (L + 2 * EPADR);
+    const size_t rows = static_cast<size_t>(P.rows);
+    uint8_t* sv = static_cast<uint8_t*>(const_cast<void*>(saved));
+    uint8_t* sc = static_cast<uint8_t*>(scratch);
+    size_t off = 0;
+    auto get = [&](uint8_t* base, size_t bytes) { size_t o = off; off = (off + bytes + 255) & ~size_t(255); return base ? base + o : nullptr; };
+    for (int i = 0; i <= a.layers; ++i) P.X16[i] = reinterpret_cast<__half*>(get(sv, rows * 3 * (i == 0 ? a.cp0 : EC) * 2));
+    for (int i = 0; i < a.layers; ++i) P.Y32[i] = reinterpret_cast<float*>(get(sv, rows * EC * 4));
+    for (int i = 0; i < a.layers; ++i) { P.mean[i] = reinterpret_cast<float*>(get(sv, size_t(B) * EC * 4)); P.rstd[i] = reinterpret_cast<float*>(get(sv, size_t(B) * EC * 4)); }
+    for (int k = 0; k < 2; ++k) {
+        P.hseq[k] = reinterpret_cast<__half*>(get(sv, rows * 2 * EH * 2));
+        P.gates[k] = reinterpret_cast<__half*>(get(sv, rows * EG * 2));
+        P.cstate[k] = reinterpret_cast<float*>(get(sv, rows * EH * 4));
+    }
+    int* lens = reinterpret_cast<int*>(get(sv, size_t(B) * 4 + 16));
+    P.lens = masked ? lens : nullptr;
+    P.inv_n = reinterpret_cast<float*>(get(sv, a.inv_n_bytes));
+    P.saved_bytes = off;
+    off = 0;
+    if (!bwd) {
+        P.xproj = reinterpret_cast<float*>(get(sc, rows * 2 * EG * 4));
+        P.hout = reinterpret_cast<float*>(get(sc, size_t(B) * L * a.hout_bytes_per_token));
+        for (int i = 0; i < a.layers; ++i) P.wconv16[i] = reinterpret_cast<__half*>(get(sc, size_t(a.taps) * EC * 3 * (i == 0 ? a.cp0 : EC) * 2));
+        P.wih16 = reinterpret_cast<__half*>(get(sc, size_t(2) * EG * 3 * EC * 2));
+        P.fwd_bytes = off;
+    } else {
+        for (int k = 0; k < 2; ++k) P.dG[k] = reinterpret_cast<__half*>(get(sc, rows * 3 * EG * 2));
+        P.dY16 = reinterpret_cast<__half*>(get(sc, rows * 3 * EC * 2));
+        P.DX32 = reinterpret_cast<float*>(get(sc, rows * EC * 4));
+        P.dwk = reinterpret_cast<float*>(get(sc, size_t(a.taps) * EC * EC * 4));
+        P.scale2 = reinterpret_cast<float*>(get(sc, 256));
+        P.dmean = reinterpret_cast<float*>(get(sc, size_t(B) * a.dmean_bytes_per_utt));
+        P.wconv16_b = reinterpret_cast<__half*>(get(sc, size_t(a.taps) * 3 * EC * EC * 2));
+        P.wih16_b = reinterpret_cast<__half*>(get(sc, size_t(2) * 3 * EG * EC * 2));
+        P.bwd_bytes = off;
+    }
+    return P;
+}
+
+int enc_stack_clear(const EncStack& S, const int* lens, cudaStream_t st) {
+    const char* who = S.a->name;
+    FT_CU(cudaMemsetAsync(S.X16[0], 0, reinterpret_cast<uint8_t*>(S.Y32[0]) - reinterpret_cast<uint8_t*>(S.X16[0]), st), who);
+    for (int k = 0; k < 2; ++k) {
+        FT_CU(cudaMemsetAsync(S.hseq[k], 0, S.rows * 2 * EH * 2, st), who);
+        FT_CU(cudaMemsetAsync(S.cstate[k], 0, S.rows * EH * 4, st), who);
+    }
+    if (S.lens) FT_CU(cudaMemcpyAsync(const_cast<int*>(S.lens), lens, sizeof(int) * S.B, cudaMemcpyDeviceToDevice, st), who);
+    return 0;
+}
+
+int enc_stack_fwd(const EncStack& S, const EncStackWeights& w, float eps, float drop_p, unsigned long long* rng, float* out,
+                  long long out_sb, long long out_sl, cudaStream_t st) {
+    const EncStackDesc& a = *S.a;
+    const int tap0 = EPADR - (a.taps - 1) / 2;                       // grid row offset of tap 0
+    for (int i = 0; i < a.layers; ++i) {
+        const int cin = i == 0 ? a.cin0 : EC, cp = i == 0 ? a.cp0 : EC;
+        a.pack_conv(w.conv_w[i], cin, cp, S.wconv16[i], nullptr, st);
+        ft_count_launch(1);
+        for (int k = 0; k < a.taps; ++k) {
+            GemmArgs g;                                               // one GEMM per tap: contraction over [hi | lo | hi] x [hi | hi | lo]
+            g.M = static_cast<int>(S.rows - 2 * EPADR); g.N = EC; g.K = 3 * cp;
+            g.A = S.X16[i] + static_cast<size_t>(tap0 + k) * 3 * cp; g.lda = 3 * cp; g.a_fmt = FMT_F16;
+            g.B = S.wconv16[i] + static_cast<size_t>(k) * EC * 3 * cp; g.ldb = 3 * cp; g.b_fmt = FMT_F16;
+            g.bias = k == 0 ? w.conv_b[i] : nullptr; g.beta = k > 0;
+            g.C32 = S.Y32[i] + static_cast<size_t>(EPADR) * EC; g.ldc32 = EC;
+            FT_TRY(launch_gemm(g, st));
+        }
+        enc_norm_fwd_kernel<<<dim3(S.B, EC / 32), 256, 0, st>>>(S.Y32[i], S.lens, S.L, w.norm_w[i], w.norm_b[i], eps, drop_p,
+                                                                 drop_p > 0.f ? rng : nullptr, i, S.X16[i + 1], S.mean[i], S.rstd[i]);
+        ft_count_launch(1);
+        FT_TRY(ft_check_launch("enc_norm_fwd_kernel"));
+    }
+    if (drop_p > 0.f) { enc_rng_advance_kernel<<<1, 1, 0, st>>>(rng); ft_count_launch(1); }
+    for (int k = 0; k < 2; ++k) {
+        __half* wih = S.wih16 + static_cast<size_t>(k) * EG * 3 * EC;
+        enc_pack_wih_kernel<<<296, 256, 0, st>>>(w.w_ih[k], wih, nullptr);
+        ft_count_launch(1);
+        GemmArgs g;
+        g.M = static_cast<int>(S.rows); g.N = EG; g.K = 3 * EC;
+        g.A = S.X16[a.layers]; g.lda = 3 * EC; g.a_fmt = FMT_F16;
+        g.B = wih; g.ldb = 3 * EC; g.b_fmt = FMT_F16;
+        g.bias = w.b_ih[k]; g.bias2 = w.b_hh[k];
+        g.C32 = S.xproj + static_cast<size_t>(k) * EG; g.ldc32 = 2 * EG;
+        FT_TRY(launch_gemm(g, st));
+    }
+    EncLstmFwdParams p;
+    p.B = S.B; p.L = S.L; p.lens = S.lens; p.xproj = S.xproj;
+    for (int k = 0; k < 2; ++k) { p.whh[k] = w.w_hh[k]; p.hseq[k] = S.hseq[k]; p.gates[k] = S.gates[k]; p.cstate[k] = S.cstate[k]; }
+    p.out = out; p.out_sb = out_sb; p.out_sl = out_sl;
+    return enc_bilstm_fwd(p, st);
+}
+
+int enc_stack_bwd(const EncStack& S, const EncStackWeights& w, const EncStackGrads& g, float drop_p, const float* d_out,
+                  long long d_sb, long long d_sl, bool want_dx, cudaStream_t st) {
+    const EncStackDesc& a = *S.a;
+    const char* who = a.name;
+    const long long rows = S.rows;
+    for (int k = 0; k < 2; ++k) FT_CU(cudaMemsetAsync(S.dG[k], 0, rows * 3 * EG * 2, st), who);
+    EncLstmBwdParams p;
+    p.B = S.B; p.L = S.L; p.lens = S.lens; p.d_out = d_out; p.d_sb = d_sb; p.d_sl = d_sl; p.scale2 = S.scale2;
+    for (int k = 0; k < 2; ++k) { p.whh[k] = w.w_hh[k]; p.gates[k] = S.gates[k]; p.cstate[k] = S.cstate[k]; p.dG[k] = S.dG[k]; }
+    FT_TRY(enc_bilstm_bwd(p, st));
+    const float* iS = S.scale2 + 1;
+    const __half* xl = S.X16[a.layers];
+    // BiLSTM parameter gradients and the gradient w.r.t. its input (fp32 grid, still x S)
+    for (int k = 0; k < 2; ++k) {
+        __half* wih = S.wih16_b + static_cast<size_t>(k) * 3 * EG * EC;
+        enc_pack_wih_kernel<<<296, 256, 0, st>>>(w.w_ih[k], nullptr, wih);
+        ft_count_launch(1);
+        FT_TRY(enc_wgrad3(st, EG, EC, rows, S.dG[k], EG, xl, 3 * EC, EC, iS, g.d_w_ih[k]));                    // dW_ih = dG^T x
+        // dW_hh = dG_t^T h_{t -+ 1}: the same grids one row apart
+        FT_TRY(enc_wgrad3(st, EG, EH, rows - 1, S.dG[k] + (k == 0 ? 3 * EG : 0), EG, S.hseq[k] + (k == 0 ? 0 : 2 * EH), 2 * EH, EH, iS, g.d_w_hh[k]));
+        enc_colsum_hilo_kernel<<<EG / 32, 256, 0, st>>>(S.dG[k], rows, EG, iS, g.d_b_ih[k]);
+        ft_count_launch(1);
+        FT_CU(cudaMemcpyAsync(g.d_b_hh[k], g.d_b_ih[k], sizeof(float) * EG, cudaMemcpyDeviceToDevice, st), who);
+        GemmArgs x;                                                   // dx (+)= dG W_ih: [hi | lo | hi] x [hi ; hi ; lo]
+        x.M = static_cast<int>(rows); x.N = EC; x.K = 3 * EG;
+        x.A = S.dG[k]; x.lda = 3 * EG; x.a_fmt = FMT_F16;
+        x.B = wih; x.ldb = EC; x.b_fmt = FMT_F16; x.b_mn = 1;
+        x.beta = k > 0; x.C32 = S.DX32; x.ldc32 = EC;
+        FT_TRY(launch_gemm(x, st));
+    }
+    const int tap0 = EPADR - (a.taps - 1) / 2;
+    for (int i = a.layers - 1; i >= 0; --i) {
+        const int cin = i == 0 ? a.cin0 : EC, cp = i == 0 ? a.cp0 : EC;
+        FT_CU(cudaMemsetAsync(S.dY16, 0, rows * 3 * EC * 2, st), who);
+        FT_CU(cudaMemsetAsync(g.d_norm_w[i], 0, sizeof(float) * EC, st), who);
+        FT_CU(cudaMemsetAsync(g.d_norm_b[i], 0, sizeof(float) * EC, st), who);
+        enc_norm_bwd_kernel<<<dim3(S.B, EC / 32), 256, 0, st>>>(S.DX32, S.X16[i + 1], S.Y32[i], S.lens, S.L, w.norm_w[i], S.mean[i], S.rstd[i],
+                                                                 drop_p, S.scale2, S.dY16, g.d_norm_w[i], g.d_norm_b[i]);
+        ft_count_launch(1);
+        FT_TRY(ft_check_launch("enc_norm_bwd_kernel"));
+        enc_colsum_hilo_kernel<<<EC / 32, 256, 0, st>>>(S.dY16, rows, EC, iS, g.d_conv_b[i]);
+        ft_count_launch(1);
+        for (int k = 0; k < a.taps; ++k)                              // dW_k = dY^T x_i shifted by tap k
+            FT_TRY(enc_wgrad3(st, EC, cp, rows - 2 * EPADR, S.dY16 + static_cast<size_t>(EPADR) * 3 * EC, EC,
+                              S.X16[i] + static_cast<size_t>(tap0 + k) * 3 * cp, 3 * cp, cp, iS, S.dwk + static_cast<size_t>(k) * EC * cp));
+        a.unpack_conv_grad(S.dwk, cin, cp, g.d_conv_w[i], st);
+        ft_count_launch(1);
+        if (i == 0 && !want_dx) break;
+        // dx_i = sum_k dY shifted by -tap . W_k (the layers that get here read 512 channels)
+        a.pack_conv(w.conv_w[i], cin, cp, nullptr, S.wconv16_b, st);
+        ft_count_launch(1);
+        for (int k = 0; k < a.taps; ++k) {
+            GemmArgs d;
+            d.M = static_cast<int>(rows - 2 * EPADR); d.N = EC; d.K = 3 * EC;
+            d.A = S.dY16 + static_cast<size_t>(2 * EPADR - tap0 - k) * 3 * EC; d.lda = 3 * EC; d.a_fmt = FMT_F16;
+            d.B = S.wconv16_b + static_cast<size_t>(k) * 3 * EC * EC; d.ldb = EC; d.b_fmt = FMT_F16; d.b_mn = 1;
+            d.beta = k > 0; d.C32 = S.DX32 + static_cast<size_t>(EPADR) * EC; d.ldc32 = EC;
+            FT_TRY(launch_gemm(d, st));
+        }
+    }
+    return 0;
+}
+
+// ------------------------------------------------------------------------------------------------ text encoder
+static void text_pack_conv(const float* w, int, int, __half* kmajor, __half* stacked, cudaStream_t st) {
+    enc_pack_conv_kernel<<<592, 256, 0, st>>>(w, kmajor, stacked);
+}
+static void text_unpack_conv_grad(const float* dwk, int, int, float* dw, cudaStream_t st) {
+    enc_unpack_conv_grad_kernel<<<592, 256, 0, st>>>(dwk, dw);
+}
+static const EncStackDesc kTextEncoder = {"encoder", 3, EK, EC, EC, 0, 0, 0, text_pack_conv, text_unpack_conv_grad};
+
+static int check_desc(const FtEncoderDesc* d) {
+    if (!d) return ft_set_error("encoder: NULL descriptor");
+    if (d->C != EC || d->n_convs != 3 || d->ksize != EK) return ft_set_error("encoder: this build supports 3 convolutions of kernel 5 over 512 channels");
+    if (d->B < 1 || d->B > 64 || d->L < 1) return ft_set_error("encoder: batch must be in [1, 64] per call");
+    if (d->dropout_p < 0.f || d->dropout_p >= 1.f) return ft_set_error("encoder: dropout_p must be in [0, 1)");
+    return 0;
+}
+
+static EncStack plan(const FtEncoderDesc& d, const void* saved, void* scratch, bool bwd) {
+    return enc_stack_plan(kTextEncoder, d.B, d.L, d.masked != 0, saved, scratch, bwd);
+}
+
 }  // namespace ft
 
 extern "C" {
 
-size_t ft_encoder_saved_bytes(const FtEncoderDesc* d) { return ft::check_desc(d) ? 0 : ft::plan_enc(*d, nullptr, nullptr, false).saved_bytes + 256; }
-size_t ft_encoder_fwd_scratch_bytes(const FtEncoderDesc* d) { return ft::check_desc(d) ? 0 : ft::plan_enc(*d, nullptr, nullptr, false).total_fwd + 256; }
-size_t ft_encoder_bwd_scratch_bytes(const FtEncoderDesc* d) { return ft::check_desc(d) ? 0 : ft::plan_enc(*d, nullptr, nullptr, true).total_bwd + 256; }
-
-#define FT_TRYE(x) do { if ((x) != 0) return -1; } while (0)
-#define FT_CU(x) do { if ((x) != cudaSuccess) return ft::ft_set_error("encoder: CUDA runtime call failed"); } while (0)
+size_t ft_encoder_saved_bytes(const FtEncoderDesc* d) { return ft::check_desc(d) ? 0 : ft::plan(*d, nullptr, nullptr, false).saved_bytes + 256; }
+size_t ft_encoder_fwd_scratch_bytes(const FtEncoderDesc* d) { return ft::check_desc(d) ? 0 : ft::plan(*d, nullptr, nullptr, false).fwd_bytes + 256; }
+size_t ft_encoder_bwd_scratch_bytes(const FtEncoderDesc* d) { return ft::check_desc(d) ? 0 : ft::plan(*d, nullptr, nullptr, true).bwd_bytes + 256; }
 
 static int encoder_fwd_impl(const FtEncoderDesc* d, const FtEncoderWeights* w, const float* x, const long long* tokens, const float* emb, int n_text,
                             const int* in_lens, unsigned long long* rng_state, float* out, long long out_stride_b, long long out_stride_l,
                             void* saved, void* scratch, void* stream) {
     using namespace ft;
-    FT_TRYE(check_desc(d));
+    FT_TRY(check_desc(d));
     if (!w || (!x && !(tokens && emb && n_text > 0)) || !out || !saved || !scratch) return ft_set_error("ft_encoder_fwd: NULL argument");
     if (d->dropout_p > 0.f && !rng_state) return ft_set_error("ft_encoder_fwd: dropout needs the device rng state");
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    EncPlan P = plan_enc(*d, static_cast<uint8_t*>(saved), static_cast<uint8_t*>(scratch), false);
-    const int B = d->B, L = d->L, Lp = L + 2 * EPADR;
-    const long long rows = static_cast<long long>(B) * Lp;
-    const int* lens = d->masked ? in_lens : nullptr;
     if (d->masked && !in_lens) return ft_set_error("ft_encoder_fwd: masked mode needs in_lens");
-    // zero the fp16 grids (pad rows and tokens beyond an utterance's length must read as zero), the exchange tensor and c
-    FT_CU(cudaMemsetAsync(P.X16[0], 0, reinterpret_cast<uint8_t*>(P.Y32[0]) - reinterpret_cast<uint8_t*>(P.X16[0]), st));
-    for (int k = 0; k < 2; ++k) {
-        FT_CU(cudaMemsetAsync(P.hseq[k], 0, rows * 2 * EH * 2, st));
-        FT_CU(cudaMemsetAsync(P.cstate[k], 0, rows * EH * 4, st));
-    }
-    if (lens) FT_CU(cudaMemcpyAsync(P.lens, lens, sizeof(int) * B, cudaMemcpyDeviceToDevice, st));
-    if (x) enc_in_kernel<<<dim3((L + 31) / 32, EC / 32, B), 256, 0, st>>>(x, lens, B, L, P.X16[0]);
-    else   enc_embed_kernel<<<B * L, 128, 0, st>>>(tokens, emb, n_text, lens, B, L, P.X16[0]);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const EncStack S = plan(*d, saved, scratch, false);
+    const int B = d->B, L = d->L;
+    FT_TRY(enc_stack_clear(S, in_lens, st));
+    if (x) enc_in_kernel<<<dim3((L + 31) / 32, EC / 32, B), 256, 0, st>>>(x, S.lens, B, L, S.X16[0]);
+    else   enc_embed_kernel<<<B * L, 128, 0, st>>>(tokens, emb, n_text, S.lens, B, L, S.X16[0]);
     ft_count_launch(1);
-    FT_TRYE(ft_check_launch("enc_in_kernel"));
-    for (int i = 0; i < 3; ++i) {
-        __half* w16 = P.wconv16 + static_cast<size_t>(i) * EK * EC * 3 * EC;
-        enc_pack_conv_kernel<<<592, 256, 0, st>>>(w->conv_w[i], w16, nullptr);
-        ft_count_launch(1);
-        for (int k = 0; k < EK; ++k) {
-            GemmArgs g;                                               // one GEMM per tap: contraction over [hi | lo | hi] x [hi | hi | lo]
-            g.M = static_cast<int>(rows - 2 * EPADR); g.N = EC; g.K = 3 * EC;
-            g.A = P.X16[i] + static_cast<size_t>(k) * 3 * EC; g.lda = 3 * EC; g.a_fmt = FMT_F16;
-            g.B = w16 + static_cast<size_t>(k) * EC * 3 * EC; g.ldb = 3 * EC; g.b_fmt = FMT_F16;
-            g.bias = k == 0 ? w->conv_b[i] : nullptr; g.beta = k > 0;
-            g.C32 = P.Y32[i] + static_cast<size_t>(EPADR) * EC; g.ldc32 = EC;
-            FT_TRYE(launch_gemm(g, st));
-        }
-        enc_norm_fwd_kernel<<<dim3(B, EC / 32), 256, 0, st>>>(P.Y32[i], lens, L, w->norm_w[i], w->norm_b[i], d->eps, d->dropout_p,
-                                                               d->dropout_p > 0.f ? rng_state : nullptr, i, P.X16[i + 1], P.mean[i], P.rstd[i]);
-        ft_count_launch(1);
-        FT_TRYE(ft_check_launch("enc_norm_fwd_kernel"));
-    }
-    if (d->dropout_p > 0.f) { enc_rng_advance_kernel<<<1, 1, 0, st>>>(rng_state); ft_count_launch(1); }
-    for (int k = 0; k < 2; ++k) {
-        __half* wih = P.wih16 + static_cast<size_t>(k) * EG * 3 * EC;
-        enc_pack_wih_kernel<<<296, 256, 0, st>>>(w->w_ih[k], wih, nullptr);
-        ft_count_launch(1);
-        GemmArgs g;
-        g.M = static_cast<int>(rows); g.N = EG; g.K = 3 * EC;
-        g.A = P.X16[3]; g.lda = 3 * EC; g.a_fmt = FMT_F16;
-        g.B = wih; g.ldb = 3 * EC; g.b_fmt = FMT_F16;
-        g.bias = w->b_ih[k]; g.bias2 = w->b_hh[k];
-        g.C32 = P.xproj + static_cast<size_t>(k) * EG; g.ldc32 = 2 * EG;
-        FT_TRYE(launch_gemm(g, st));
-    }
-    EncLstmFwdParams p;
-    p.B = B; p.L = L; p.lens = lens; p.xproj = P.xproj;
-    for (int k = 0; k < 2; ++k) { p.whh[k] = w->w_hh[k]; p.hseq[k] = P.hseq[k]; p.gates[k] = P.gates[k]; p.cstate[k] = P.cstate[k]; }
-    p.out = out; p.out_sb = out_stride_b; p.out_sl = out_stride_l;
-    return enc_bilstm_fwd(p, st);
+    FT_TRY(ft_check_launch("enc_in_kernel"));
+    return enc_stack_fwd(S, stack_weights(*w), d->eps, d->dropout_p, rng_state, out, out_stride_b, out_stride_l, st);
 }
 
 int ft_encoder_fwd(const FtEncoderDesc* d, const FtEncoderWeights* w, const float* x, const int* in_lens, unsigned long long* rng_state,
@@ -665,75 +742,24 @@ static int encoder_bwd_impl(const FtEncoderDesc* d, const FtEncoderWeights* w, c
                             const void* saved, float* d_x, const long long* tokens, int n_text, float* d_emb, const FtEncoderGrads* gr,
                             void* scratch, void* stream) {
     using namespace ft;
-    FT_TRYE(check_desc(d));
+    FT_TRY(check_desc(d));
     if (!w || !d_out || !saved || !gr || !scratch) return ft_set_error("ft_encoder_bwd: NULL argument");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    EncPlan P = plan_enc(*d, const_cast<uint8_t*>(static_cast<const uint8_t*>(saved)), static_cast<uint8_t*>(scratch), true);
-    const int B = d->B, L = d->L, Lp = L + 2 * EPADR;
-    const long long rows = static_cast<long long>(B) * Lp;
-    const int* lens = d->masked ? P.lens : nullptr;
+    const EncStack S = plan(*d, saved, scratch, true);
+    const int B = d->B, L = d->L;
     if (d_stride_l != 2 * EH || d_stride_b != static_cast<long long>(L) * 2 * EH) return ft_set_error("ft_encoder_bwd: d_out must be dense [B, L, 512]");
-    FT_TRYE(launch_grad_scale(d_out, static_cast<long long>(B) * L * 2 * EH, nullptr, 0, nullptr, 0, 256.0f, P.scale2, st));
-    for (int k = 0; k < 2; ++k) FT_CU(cudaMemsetAsync(P.dG[k], 0, rows * 3 * EG * 2, st));
-    EncLstmBwdParams p;
-    p.B = B; p.L = L; p.lens = lens; p.d_out = d_out; p.d_sb = d_stride_b; p.d_sl = d_stride_l; p.scale2 = P.scale2;
-    for (int k = 0; k < 2; ++k) { p.whh[k] = w->w_hh[k]; p.gates[k] = P.gates[k]; p.cstate[k] = P.cstate[k]; p.dG[k] = P.dG[k]; }
-    FT_TRYE(enc_bilstm_bwd(p, st));
-    const float* iS = P.scale2 + 1;
-    // BiLSTM parameter gradients and the gradient w.r.t. its input (fp32 grid, still x S)
-    for (int k = 0; k < 2; ++k) {
-        __half* wih = P.wih16_b + static_cast<size_t>(k) * 3 * EG * EC;
-        enc_pack_wih_kernel<<<296, 256, 0, st>>>(w->w_ih[k], nullptr, wih);
-        ft_count_launch(1);
-        FT_TRYE(enc_wgrad3(st, EG, EC, rows, P.dG[k], EG, P.X16[3], 3 * EC, EC, iS, gr->d_w_ih[k]));             // dW_ih = dG^T x3
-        // dW_hh = dG_t^T h_{t -+ 1}: the same grids one row apart
-        FT_TRYE(enc_wgrad3(st, EG, EH, rows - 1, P.dG[k] + (k == 0 ? 3 * EG : 0), EG, P.hseq[k] + (k == 0 ? 0 : 2 * EH), 2 * EH, EH, iS, gr->d_w_hh[k]));
-        enc_colsum_hilo_kernel<<<EG / 32, 256, 0, st>>>(P.dG[k], rows, EG, iS, gr->d_b_ih[k]);
-        ft_count_launch(1);
-        FT_CU(cudaMemcpyAsync(gr->d_b_hh[k], gr->d_b_ih[k], sizeof(float) * EG, cudaMemcpyDeviceToDevice, st));
-        GemmArgs x;                                                   // dx3 (+)= dG W_ih: [hi | lo | hi] x [hi ; hi ; lo]
-        x.M = static_cast<int>(rows); x.N = EC; x.K = 3 * EG;
-        x.A = P.dG[k]; x.lda = 3 * EG; x.a_fmt = FMT_F16;
-        x.B = wih; x.ldb = EC; x.b_fmt = FMT_F16; x.b_mn = 1;
-        x.beta = k > 0; x.C32 = P.DX32; x.ldc32 = EC;
-        FT_TRYE(launch_gemm(x, st));
-    }
-    for (int i = 2; i >= 0; --i) {
-        FT_CU(cudaMemsetAsync(P.dY16, 0, rows * 3 * EC * 2, st));
-        FT_CU(cudaMemsetAsync(gr->d_norm_w[i], 0, sizeof(float) * EC, st));
-        FT_CU(cudaMemsetAsync(gr->d_norm_b[i], 0, sizeof(float) * EC, st));
-        enc_norm_bwd_kernel<<<dim3(B, EC / 32), 256, 0, st>>>(P.DX32, P.X16[i + 1], P.Y32[i], lens, L, w->norm_w[i], P.mean[i], P.rstd[i],
-                                                               d->dropout_p, P.scale2, P.dY16, gr->d_norm_w[i], gr->d_norm_b[i]);
-        ft_count_launch(1);
-        FT_TRYE(ft_check_launch("enc_norm_bwd_kernel"));
-        enc_colsum_hilo_kernel<<<EC / 32, 256, 0, st>>>(P.dY16, rows, EC, iS, gr->d_conv_b[i]);
-        ft_count_launch(1);
-        enc_pack_conv_kernel<<<592, 256, 0, st>>>(w->conv_w[i], nullptr, P.wconv16_b);
-        ft_count_launch(1);
-        for (int k = 0; k < EK; ++k)                                  // dW_k = dY^T x_i shifted by tap k
-            FT_TRYE(enc_wgrad3(st, EC, EC, rows - 2 * EPADR, P.dY16 + static_cast<size_t>(EPADR) * 3 * EC, EC,
-                           P.X16[i] + static_cast<size_t>(k) * 3 * EC, 3 * EC, EC, iS, P.dwk + static_cast<size_t>(k) * EC * EC));
-        enc_unpack_conv_grad_kernel<<<592, 256, 0, st>>>(P.dwk, gr->d_conv_w[i]);
-        ft_count_launch(1);
-        for (int k = 0; k < EK; ++k) {
-            GemmArgs g;                                               // dx_i = sum_k dY shifted by -tap . W_k
-            g.M = static_cast<int>(rows - 2 * EPADR); g.N = EC; g.K = 3 * EC;
-            g.A = P.dY16 + static_cast<size_t>(2 * EPADR - k) * 3 * EC; g.lda = 3 * EC; g.a_fmt = FMT_F16;
-            g.B = P.wconv16_b + static_cast<size_t>(k) * 3 * EC * EC; g.ldb = EC; g.b_fmt = FMT_F16; g.b_mn = 1;
-            g.beta = k > 0; g.C32 = P.DX32 + static_cast<size_t>(EPADR) * EC; g.ldc32 = EC;
-            FT_TRYE(launch_gemm(g, st));
-        }
-    }
+    FT_TRY(launch_grad_scale(d_out, static_cast<long long>(B) * L * 2 * EH, nullptr, 0, nullptr, 0, 256.0f, S.scale2, st));
+    FT_TRY(enc_stack_bwd(S, stack_weights(*w), stack_grads(*gr), d->dropout_p, d_out, d_stride_b, d_stride_l, d_x || d_emb, st));
     if (d_x) {
-        enc_out_grad_kernel<<<dim3((L + 31) / 32, EC / 32, B), 256, 0, st>>>(P.DX32, lens, B, L, P.scale2, d_x);
+        enc_out_grad_kernel<<<dim3((L + 31) / 32, EC / 32, B), 256, 0, st>>>(S.DX32, S.lens, B, L, S.scale2, d_x);
         ft_count_launch(1);
-        FT_TRYE(ft_check_launch("enc_out_grad_kernel"));
+        FT_TRY(ft_check_launch("enc_out_grad_kernel"));
     }
     if (d_emb) {
-        FT_CU(cudaMemsetAsync(d_emb, 0, sizeof(float) * static_cast<size_t>(n_text) * EC, st));
-        enc_embed_grad_kernel<<<B * L, 128, 0, st>>>(P.DX32, tokens, n_text, lens, B, L, P.scale2, d_emb);
+        FT_CU(cudaMemsetAsync(d_emb, 0, sizeof(float) * static_cast<size_t>(n_text) * EC, st), "encoder");
+        enc_embed_grad_kernel<<<B * L, 128, 0, st>>>(S.DX32, tokens, n_text, S.lens, B, L, S.scale2, d_emb);
         ft_count_launch(1);
-        FT_TRYE(ft_check_launch("enc_embed_grad_kernel"));
+        FT_TRY(ft_check_launch("enc_embed_grad_kernel"));
     }
     return 0;
 }

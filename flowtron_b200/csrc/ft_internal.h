@@ -13,8 +13,14 @@ typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_
 // error plumbing (api.cu)
 int ft_set_error(const char* msg);            // records msg, returns -1
 int ft_check_launch(const char* what);        // cudaGetLastError -> ft_set_error
+int ft_runtime_error(const char* who);        // records "<who>: CUDA runtime call failed", returns -1
 int* ft_status_word();                        // device int written by kernel watchdogs (0 = ok)
 void ft_count_launch(int n);
+
+// propagate a failure whose message is already recorded
+#define FT_TRY(x) do { if ((x) != 0) return -1; } while (0)
+// check a CUDA runtime call; `who` prefixes the recorded message
+#define FT_CU(x, who) do { if ((x) != cudaSuccess) return ::ft::ft_runtime_error(who); } while (0)
 
 // RAII device-time bracket around a launch (no-op unless ft_timing_enable(1))
 struct TimeScope {

@@ -889,25 +889,24 @@ static int infer_impl(const FtArStepDesc* d, const FtArStepWeights* w, const flo
     InferScratch s = plan_infer(*d, static_cast<uint8_t*>(scratch));
     const int M = d->n_mel, A = d->n_attn, E = d->n_text, D = IH + A, B = d->B;
     const long long RL = static_cast<long long>(d->L) * B;
-#define FT_TRYX(x) do { if ((x) != 0) return -1; } while (0)
     // weights in consumption order (fp16), LSTM input + recurrent matrices fused along K, biases pre-added
-    FT_TRYX(pack(s.wA, s.bA, w->attn_lstm_w_ih, M, XPAD, w->attn_lstm_w_hh, IH, w->attn_lstm_b_ih, w->attn_lstm_b_hh, IH / 2, (XPAD + IH) / 32, 0, M, st));
-    FT_TRYX(pack(s.w0, s.b0, w->lstm_w_ih0, D, D, w->lstm_w_hh0, IH, w->lstm_b_ih0, w->lstm_b_hh0, IH / 2, (D + IH) / 32, 0, M, st));
-    FT_TRYX(pack(s.w1, s.b1, w->lstm_w_ih1, IH, IH, w->lstm_w_hh1, IH, w->lstm_b_ih1, w->lstm_b_hh1, IH / 2, 2 * IH / 32, 0, M, st));
-    FT_TRYX(pack(s.wq, nullptr, w->att_query, IH, IH, nullptr, 0, nullptr, nullptr, A / 8, IH / 32, 1, M, st));
-    FT_TRYX(pack(s.wd1, s.bd1, w->dense_w0, IH, IH, nullptr, 0, w->dense_b0, nullptr, IH / 8, IH / 32, 1, M, st));
-    FT_TRYX(pack(s.wd2, s.bd2, w->dense_w1, IH, IH, nullptr, 0, w->dense_b1, nullptr, IH / 8, IH / 32, 1, M, st));
-    FT_TRYX(pack(s.wc, s.bc, w->conv_w, IH, IH, nullptr, 0, w->conv_b, nullptr, M / 4, IH / 32, 2, M, st));
-    FT_TRYX(launch_cast(w->att_key, 2, s.wk, 0, static_cast<long long>(A) * E, st));
-    FT_TRYX(launch_cast(w->att_value, 2, s.wv, 0, static_cast<long long>(A) * E, st));
-    FT_TRYX(launch_cast(text, 2, s.text16, 0, RL * E, st));
+    FT_TRY(pack(s.wA, s.bA, w->attn_lstm_w_ih, M, XPAD, w->attn_lstm_w_hh, IH, w->attn_lstm_b_ih, w->attn_lstm_b_hh, IH / 2, (XPAD + IH) / 32, 0, M, st));
+    FT_TRY(pack(s.w0, s.b0, w->lstm_w_ih0, D, D, w->lstm_w_hh0, IH, w->lstm_b_ih0, w->lstm_b_hh0, IH / 2, (D + IH) / 32, 0, M, st));
+    FT_TRY(pack(s.w1, s.b1, w->lstm_w_ih1, IH, IH, w->lstm_w_hh1, IH, w->lstm_b_ih1, w->lstm_b_hh1, IH / 2, 2 * IH / 32, 0, M, st));
+    FT_TRY(pack(s.wq, nullptr, w->att_query, IH, IH, nullptr, 0, nullptr, nullptr, A / 8, IH / 32, 1, M, st));
+    FT_TRY(pack(s.wd1, s.bd1, w->dense_w0, IH, IH, nullptr, 0, w->dense_b0, nullptr, IH / 8, IH / 32, 1, M, st));
+    FT_TRY(pack(s.wd2, s.bd2, w->dense_w1, IH, IH, nullptr, 0, w->dense_b1, nullptr, IH / 8, IH / 32, 1, M, st));
+    FT_TRY(pack(s.wc, s.bc, w->conv_w, IH, IH, nullptr, 0, w->conv_b, nullptr, M / 4, IH / 32, 2, M, st));
+    FT_TRY(launch_cast(w->att_key, 2, s.wk, 0, static_cast<long long>(A) * E, st));
+    FT_TRY(launch_cast(w->att_value, 2, s.wv, 0, static_cast<long long>(A) * E, st));
+    FT_TRY(launch_cast(text, 2, s.text16, 0, RL * E, st));
     {   // K / V projections once per utterance (the reference recomputes them every frame, flowtron.py:568-570)
         GemmArgs g;
         g.M = static_cast<int>(RL); g.N = A; g.K = E; g.A = s.text16; g.lda = E; g.a_fmt = FMT_F16;
         g.B = s.wk; g.ldb = E; g.b_fmt = FMT_F16; g.C32 = s.Kp; g.ldc32 = A;
-        FT_TRYX(launch_gemm(g, st));
+        FT_TRY(launch_gemm(g, st));
         g.B = s.wv; g.C32 = s.Vp;
-        FT_TRYX(launch_gemm(g, st));
+        FT_TRY(launch_gemm(g, st));
     }
     if (cudaMemsetAsync(out, 0, sizeof(float) * d->T * B * M, st) != cudaSuccess) return ft_set_error("infer: memset failed");
     if (cudaMemsetAsync(attn_out, 0, sizeof(float) * d->T * B * d->L, st) != cudaSuccess) return ft_set_error("infer: memset failed");

@@ -111,6 +111,28 @@ def _mel_encoder_stream(device):
     return _enc_streams[key]
 
 
+def _kernel_params(enc):
+    """Encoder / MelEncoder parameters in ENC_PARAM_FIELDS / MEL_ENC_PARAM_FIELDS order."""
+    cs = enc.convolutions
+    flat = [c[0].conv.weight for c in cs] + [c[0].conv.bias for c in cs] + [c[1].weight for c in cs] + [c[1].bias for c in cs]
+    for n in ("weight_ih_l0", "weight_hh_l0", "bias_ih_l0", "bias_hh_l0"):
+        flat += [getattr(enc.lstm, n), getattr(enc.lstm, n + "_reverse")]
+    return flat
+
+
+def _unflatten_params(fields, flat_params):
+    """flat parameters (the _kernel_params order) -> dict name -> list of detached contiguous tensors."""
+    params, i = {}, 0
+    for n, k in fields:
+        params[n] = [t.detach().contiguous() for t in flat_params[i:i + k]]
+        i += k
+    return params
+
+
+def _flatten_grads(fields, grads):
+    return [t for n, _ in fields for t in grads[n]]
+
+
 class _EncoderFn(torch.autograd.Function):
     """Encoder forward / backward on the CUDA kernels for up to 64 utterances: ft_encoder_fwd / ft_encoder_bwd on x [B, 512, L],
     or, given tokens [B, L] and the embedding weight instead of x, ft_encoder_fwd_tokens / ft_encoder_bwd_tokens, which fuse the
@@ -118,10 +140,7 @@ class _EncoderFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, enc, x, tokens, emb_weight, in_lens, masked, dropout_p, *flat_params):
-        params, i = {}, 0
-        for n, k in _lib.ENC_PARAM_FIELDS:
-            params[n] = [t.detach().contiguous() for t in flat_params[i:i + k]]
-            i += k
+        params = _unflatten_params(_lib.ENC_PARAM_FIELDS, flat_params)
         if x is None:
             B, L = tokens.shape
             tokens, emb_weight, dev = tokens.contiguous(), emb_weight.detach().contiguous(), tokens.device
@@ -143,11 +162,8 @@ class _EncoderFn(torch.autograd.Function):
         d_in, grads = _lib.encoder_bwd(ctx.desc, ctx.params, d_out.contiguous().float(), ctx.saved, need_dx=ctx.needs_input_grad[1],
                                        tokens=ctx.tokens, emb_weight=ctx.emb_weight)
         ctx.saved = None
-        flat = []
-        for n, _ in _lib.ENC_PARAM_FIELDS:
-            flat += grads[n]
         d_x, d_emb = (d_in, None) if ctx.tokens is None else (None, d_in)
-        return (None, d_x, None, d_emb, None, None, None, *flat)
+        return (None, d_x, None, d_emb, None, None, None, *_flatten_grads(_lib.ENC_PARAM_FIELDS, grads))
 
 
 _ENC_MAX_BATCH = 64                  # utterances per encoder-kernel call (the kernels reject more)
@@ -180,13 +196,6 @@ class Encoder(nn.Module):
             self._rng = torch.tensor([torch.initial_seed() & 0x7FFFFFFFFFFFFFFF, 0], dtype=torch.int64, device=device)
         return self._rng
 
-    def _kernel_params(self):
-        cs = self.convolutions
-        flat = [c[0].conv.weight for c in cs] + [c[0].conv.bias for c in cs] + [c[1].weight for c in cs] + [c[1].bias for c in cs]
-        for n in ("weight_ih_l0", "weight_hh_l0", "bias_ih_l0", "bias_hh_l0"):
-            flat += [getattr(self.lstm, n), getattr(self.lstm, n + "_reverse")]
-        return flat
-
     def _run(self, x, tokens, emb_weight, in_lens, masked, dropout=True):
         """x [B, 512, L], or tokens [B, L] with the embedding weight -> [B, L, 512].  A batch above 64 utterances runs as
         consecutive calls of at most 64 (utterances are independent); `masked` is decided from the whole batch, so a 1-row
@@ -198,7 +207,7 @@ class Encoder(nn.Module):
         if C != 512:
             raise ValueError(f"the encoder kernels take 512 channels, got {C}")
         dropout_p = self.p_dropout if dropout and self.training else 0.0
-        params = self._kernel_params()
+        params = _kernel_params(self)
         rows = lambda t, b0: None if t is None else t[b0:b0 + _ENC_MAX_BATCH]
         outs = [_EncoderFn.apply(self, rows(x, b0), rows(tokens, b0), emb_weight, rows(in_lens, b0), masked, dropout_p, *params)
                 for b0 in range(0, src.size(0), _ENC_MAX_BATCH)]
@@ -232,10 +241,7 @@ class _MelEncoderFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, enc, mel, out_lens, all_lens, dropout_p, *flat_params):
-        params, i = {}, 0
-        for n, k in _lib.MEL_ENC_PARAM_FIELDS:
-            params[n] = [t.detach().contiguous() for t in flat_params[i:i + k]]
-            i += k
+        params = _unflatten_params(_lib.MEL_ENC_PARAM_FIELDS, flat_params)
         mel = mel.detach().contiguous().float()
         emb = torch.empty(mel.size(0), 512, dtype=torch.float32, device=mel.device)
         rng = enc._rng_state(mel.device) if dropout_p > 0 else None
@@ -249,10 +255,7 @@ class _MelEncoderFn(torch.autograd.Function):
             raise RuntimeError("MelEncoder backward called twice (the saved activations were released)")
         grads = _lib.mel_encoder_bwd(ctx.desc, ctx.params, d_emb.contiguous().float(), ctx.saved)
         ctx.saved = None
-        flat = []
-        for n, _ in _lib.MEL_ENC_PARAM_FIELDS:
-            flat += grads[n]
-        return (None, None, None, None, None, *flat)
+        return (None, None, None, None, None, *_flatten_grads(_lib.MEL_ENC_PARAM_FIELDS, grads))
 
 
 class MelEncoder(nn.Module):
@@ -290,13 +293,6 @@ class MelEncoder(nn.Module):
             self._rng = torch.tensor([seed, 0], dtype=torch.int64, device=device)
         return self._rng
 
-    def _kernel_params(self):
-        cs = self.convolutions
-        flat = [c[0].conv.weight for c in cs] + [c[0].conv.bias for c in cs] + [c[1].weight for c in cs] + [c[1].bias for c in cs]
-        for n in ("weight_ih_l0", "weight_hh_l0", "bias_ih_l0", "bias_hh_l0"):
-            flat += [getattr(self.lstm, n), getattr(self.lstm, n + "_reverse")]
-        return flat
-
     def forward(self, x, lens):
         """x [B, 80, T] with T == max(lens), lens [B] -> [B, 512].  Batches above 64 utterances run as consecutive calls of at
         most 64, each divided by the whole batch's longest length."""
@@ -308,7 +304,7 @@ class MelEncoder(nn.Module):
             raise ValueError("MelEncoder needs one length per utterance")
         lens32 = lens.to(device=x.device, dtype=torch.int32).contiguous()
         dropout_p = self.p_dropout if self.training else 0.0
-        params = self._kernel_params()
+        params = _kernel_params(self)
         mb = _lib.MEL_ENC_MAX_BATCH
         outs = [_MelEncoderFn.apply(self, x[b0:b0 + mb], lens32[b0:b0 + mb], lens32, dropout_p, *params)
                 for b0 in range(0, x.size(0), mb)]

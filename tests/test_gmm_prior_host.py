@@ -1,6 +1,7 @@
 """CPU: the Gaussian-mixture prior's host layer (MelEncoder, GaussianMixture, Flowtron(n_components > 1),
 FlowtronLoss(gm_loss=True)): state_dict layout against the reference fixtures, strict loads, CPU-tensor and K > 32 rejections,
-the C ABI of the mel-encoder and mixture-NLL kernels, and the text encoder's kernels unchanged by sharing their device code."""
+the C ABI of the mel-encoder and mixture-NLL kernels, both encoders' kernels unchanged by sharing their device and host
+code, and the byte layouts of both encoders' saved / scratch buffers."""
 import hashlib
 import os
 import re
@@ -142,6 +143,16 @@ _ENC_KERNELS = {
 }
 
 
+# mel_encoder.cu's own kernels, pinned the same way: both encoders run one host path, and no kernel of either file changed.
+_MEL_ENC_KERNELS = {
+    "_ZN2ft20mel_enc_dmean_kernelEPKfS1_iPf": (12, ("0", "0"), "6d1f30673583bfae"),
+    "_ZN2ft19mel_enc_mean_kernelEPKfPKiiS3_iPfS4_": (31, ("0", "0"), "7f19eac91b247e2f"),
+    "_ZN2ft27mel_unpack_conv_grad_kernelEPKfiiPf": (34, ("0", "0"), "269da6964b47df28"),
+    "_ZN2ft20mel_pack_conv_kernelEPKfiiP6__halfS3_": (26, ("0", "0"), "85844aa1e43c1bb0"),
+    "_ZN2ft17mel_enc_in_kernelEPKfPKiiP6__half": (32, ("0", "0"), "ce3d8fc79dfcf961"),
+}
+
+
 def _compile(src, tmp_path):
     obj = str(tmp_path / (src + ".o"))
     r = subprocess.run([NVCC, "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
@@ -172,14 +183,23 @@ def _sass_hashes(obj):
     return {k: hashlib.sha256("\n".join(v).encode()).hexdigest()[:16] for k, v in out.items()}
 
 
-@pytest.mark.skipif(not HAVE_NVCC, reason="nvcc not available")
-def test_text_encoder_kernels_are_unchanged(tmp_path):
-    obj, regs = _compile("encoder.cu", tmp_path)
+def _assert_kernels_pinned(src, table, tmp_path):
+    obj, regs = _compile(src, tmp_path)
     sass = _sass_hashes(obj)
-    assert set(regs) == set(_ENC_KERNELS) == set(sass)
-    for name, (r, spill, h) in _ENC_KERNELS.items():
+    assert set(regs) == set(table) == set(sass)
+    for name, (r, spill, h) in table.items():
         assert regs[name] == (r, spill), name
         assert sass[name] == h, name
+
+
+@pytest.mark.skipif(not HAVE_NVCC, reason="nvcc not available")
+def test_text_encoder_kernels_are_unchanged(tmp_path):
+    _assert_kernels_pinned("encoder.cu", _ENC_KERNELS, tmp_path)
+
+
+@pytest.mark.skipif(not HAVE_NVCC, reason="nvcc not available")
+def test_mel_encoder_kernels_are_unchanged(tmp_path):
+    _assert_kernels_pinned("mel_encoder.cu", _MEL_ENC_KERNELS, tmp_path)
 
 
 @pytest.mark.skipif(not HAVE_NVCC, reason="nvcc not available")
@@ -189,6 +209,50 @@ def test_new_kernels_do_not_spill(tmp_path):
         assert regs, src
         for name, (_, spill) in regs.items():
             assert spill == ("0", "0"), name
+
+
+# (saved, forward scratch, backward scratch) bytes of each encoder, as laid out before the two encoders shared one host path;
+# the masked flag and the dropout probability do not change them.  Callers allocate these buffers, so the regions, their
+# order and their sizes are part of what the host path must keep.
+_ENC_BYTES = {  # (B, L)
+    (1, 1): (145920, 29925632, 19486208), (1, 7): (305664, 29974784, 19590656),
+    (1, 256): (6935040, 32014592, 23925248), (1, 1024): (27382272, 38306048, 37294592),
+    (2, 1): (291328, 29966592, 19573248), (2, 7): (610816, 30064896, 19782144),
+    (2, 256): (13869568, 34144512, 28451328), (2, 1024): (54764032, 46727424, 55190016),
+    (33, 1): (4798976, 31236352, 22271488), (33, 7): (10070528, 32858368, 25718272),
+    (33, 256): (228839936, 100172032, 168759808), (33, 1024): (903598592, 307790080, 609948160),
+    (64, 1): (9306880, 32506112, 24969728), (64, 7): (19530496, 35651840, 31654400),
+    (64, 256): (443810560, 166199552, 309068288), (64, 1024): (1752433408, 568852736, 1164706304),
+}
+_MEL_ENC_BYTES = {  # (B, T)
+    (1, 1): (104960, 12232960, 14245376), (1, 100): (2005760, 13246720, 15968768),
+    (1, 2000): (38485760, 32702720, 49043968), (17, 1): (1772032, 12921088, 15670784),
+    (17, 100): (34085632, 30155008, 44968448), (17, 2000): (654245632, 360907008, 607246848),
+    (64, 1): (6669312, 14942464, 19857920), (64, 100): (128320512, 79823104, 130155008),
+    (64, 2000): (2463040512, 1325007104, 2246967808),
+}
+
+
+def test_encoder_buffer_sizes_are_pinned():
+    from flowtron_b200 import _lib
+    L = _lib.lib()
+    for (B, T), want in _ENC_BYTES.items():
+        for masked in (0, 1):
+            for p in (0.0, 0.5):
+                d = _lib.encoder_desc(B, T, masked, p)
+                got = (L.ft_encoder_saved_bytes(d), L.ft_encoder_fwd_scratch_bytes(d), L.ft_encoder_bwd_scratch_bytes(d))
+                assert got == want, (B, T, masked, p)
+    for (B, T), want in _MEL_ENC_BYTES.items():
+        for p in (0.0, 0.5):
+            d = _lib.FtMelEncoderDesc(B=B, T=T, eps=1e-5, dropout_p=p)
+            got = (L.ft_mel_encoder_saved_bytes(d), L.ft_mel_encoder_fwd_scratch_bytes(d), L.ft_mel_encoder_bwd_scratch_bytes(d))
+            assert got == want, (B, T, p)
+    bad_text = [_lib.encoder_desc(65, 8, 1, 0.0), _lib.encoder_desc(2, 8, 1, 0.0)]
+    bad_text[1].C = 256
+    for d in bad_text:
+        assert (L.ft_encoder_saved_bytes(d), L.ft_encoder_fwd_scratch_bytes(d), L.ft_encoder_bwd_scratch_bytes(d)) == (0, 0, 0)
+    for d in (_lib.FtMelEncoderDesc(B=65, T=8, eps=1e-5, dropout_p=0.0), _lib.FtMelEncoderDesc(B=2, T=0, eps=1e-5, dropout_p=0.0)):
+        assert (L.ft_mel_encoder_saved_bytes(d), L.ft_mel_encoder_fwd_scratch_bytes(d), L.ft_mel_encoder_bwd_scratch_bytes(d)) == (0, 0, 0)
 
 
 def test_mixture_parameters_reach_the_gradient_buckets_and_the_optimizer_order():
