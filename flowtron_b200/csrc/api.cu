@@ -57,14 +57,14 @@ TimeScope::TimeScope(const char* name, long long m, long long n, long long k, cu
     if (!g_timing) return;
     std::lock_guard<std::mutex> lk(g_mu);
     TimeRec r{name, m, n, k, get_event(), get_event()};
-    cudaEventRecord(r.a, st);
+    cudaEventRecord(r.a, st);              // unchecked: a timing bracket must not fail the launch it measures
     g_recs.push_back(r);
     idx_ = static_cast<int>(g_recs.size()) - 1;
 }
 TimeScope::~TimeScope() {
     if (idx_ < 0) return;
     std::lock_guard<std::mutex> lk(g_mu);
-    cudaEventRecord(g_recs[idx_].b, st_);
+    cudaEventRecord(g_recs[idx_].b, st_);  // unchecked: as above; ft_timing_report skips a bracket it cannot time
 }
 
 }  // namespace ft

@@ -1,7 +1,7 @@
 // Host-side orchestration of one Flowtron AR flow step (training direction) on a CUDA stream:
 // AR_Step.forward / AR_Back_Step.forward (flowtron.py:725-773, 605-627) and their autograd.
 // No allocation, no synchronisation: every intermediate lives in the caller's `saved` / `scratch` areas,
-// whose layouts are planned by the same code that uses them (Plan below).
+// whose layouts are planned by the same code that uses them (Workspace, ft_internal.h).
 //
 // Precision plan (DESIGN.md): forward tensor-core operands are fp16 (11-bit significand, same as tf32; every
 // forward operand is either a weight or a bounded activation); backward operands are fp16 too, on gradients
@@ -23,22 +23,6 @@ namespace {
 
 constexpr int H = 1024, G = 4096;
 
-struct Region { const char* name; size_t off, bytes; };
-
-struct Plan {
-    uint8_t* base = nullptr;
-    size_t off = 0;
-    std::vector<Region>* regs = nullptr;
-    template <typename T>
-    T* get(const char* name, size_t n) {
-        const size_t bytes = n * sizeof(T);
-        const size_t o = off;
-        off = (off + bytes + 255) & ~static_cast<size_t>(255);
-        if (regs) regs->push_back({name, o, bytes});
-        return base ? reinterpret_cast<T*>(base + o) : nullptr;
-    }
-};
-
 struct Dims {
     long long R, RL;
     int T, B, L, M, A, E, D;
@@ -51,7 +35,7 @@ struct Dims {
 struct Saved {
     uint16_t *mel_in16, *d16, *gatesA, *text16, *h0_16, *gates0, *h1_16, *gates1, *y1_16, *y2_16;
     float *mel_flow, *cA, *Kp, *Vp, *Q, *p_save, *c0, *c1, *o32;
-    void plan(Plan& p, const FtArStepDesc& d) {
+    void plan(Workspace& p, const FtArStepDesc& d) {
         const Dims n(d);
         mel_in16 = p.get<uint16_t>("mel_in16", n.R * n.M);
         mel_flow = d.reversed ? p.get<float>("mel_flow", n.R * n.M) : nullptr;
@@ -78,7 +62,7 @@ struct Saved {
 // ---- 16-bit weight copies (fp16 for forward, bf16 for backward)
 struct W16 {
     uint16_t *w_ih_a, *w_hh_a, *w_ih0, *w_hh0, *w_ih1, *w_hh1, *wq, *wk, *wv, *w1, *w2, *wc;
-    void plan(Plan& p, const Dims& n) {
+    void plan(Workspace& p, const Dims& n) {
         w_ih_a = p.get<uint16_t>("w_ih_a", static_cast<size_t>(G) * n.M);
         w_hh_a = p.get<uint16_t>("w_hh_a", static_cast<size_t>(G) * H);
         w_ih0 = p.get<uint16_t>("w_ih0", static_cast<size_t>(G) * n.D);
@@ -112,7 +96,7 @@ struct FwdScratch {
     float* X1;                  // second input-projection buffer: the attention LSTM's (overlap), then layer 1's (pipeline)
     float *hA32 = nullptr, *ctx32 = nullptr;     // fp32 copies of [hA ; ctx] for the gate logits (gated flow only)
     float* attn_rows = nullptr;                  // long texts: the attention's score rows (attn_rows_in_global)
-    void plan(Plan& p, const FtArStepDesc& d) {
+    void plan(Workspace& p, const FtArStepDesc& d) {
         const Dims n(d);
         w.plan(p, n);
         X = p.get<float>("X", n.R * G);
@@ -131,7 +115,7 @@ struct FwdScratch {
 // concurrently with the attention LSTM's BPTT, a 64-SM kernel.  Lives in caller memory (`carry`), not in the shared scratch.
 struct BwdCarry {
     float *dd, *dmel_flow, *scale;
-    void plan(Plan& p, const FtArStepDesc& d) {
+    void plan(Workspace& p, const FtArStepDesc& d) {
         const Dims n(d);
         dd = p.get<float>("dd", n.R * n.D);                 // [R, D]: cols 0:H = dhA (attention-LSTM output gradient), H: = dctx
         dmel_flow = p.get<float>("dmel_flow", n.R * n.M);
@@ -148,7 +132,7 @@ struct BwdScratch {
     float *xchg1, *xchg0;       // partial-sum rings of the two pipelined BPTT recurrences (flat kernel, lstm.cu)
     float* attn_rows = nullptr; // long texts: the attention backward's gradient rows (attn_rows_in_global)
     float* sink;
-    void plan(Plan& p, const FtArStepDesc& d) {
+    void plan(Workspace& p, const FtArStepDesc& d) {
         const Dims n(d);
         w.plan(p, n);
         dG1 = p.get<uint16_t>("dG1", n.R * G);      // one per LSTM layer: the wgrad GEMMs of a layer run on the side
@@ -223,107 +207,45 @@ int check_desc(const FtArStepDesc& d) {
     return 0;
 }
 
-// C = A[M,K] B[N,K]^T helpers -----------------------------------------------------------------------------
-int gemm_fwd(cudaStream_t st, long long M, int N, int K, const void* A, long long lda, const void* B, long long ldb,
-             const float* bias, const float* bias2, int act, float* C32, long long ldc32, void* C16, long long ldc16) {
-    GemmArgs g;
-    g.M = static_cast<int>(M); g.N = N; g.K = K;
-    g.A = A; g.lda = lda; g.a_fmt = FMT_F16; g.B = B; g.ldb = ldb; g.b_fmt = FMT_F16;
-    g.bias = bias; g.bias2 = bias2; g.act = act;
-    g.C32 = C32; g.ldc32 = ldc32; g.C16 = C16; g.ldc16 = ldc16; g.c16_fmt = FMT_F16;
-    return launch_gemm(g, st);
-}
-// dgrad: dX[M,K] = dY[M,N] W[N,K]      (A = dY K-major, B = W given MN-major)
-int gemm_dgrad(cudaStream_t st, long long M, int Kout, int Nred, const void* dY, long long lddy, const void* W, long long ldw,
-               int beta, float* C32, long long ldc32, void* C16, long long ldc16, const void* aux16, long long ldaux,
-               const float* alpha_ptr = nullptr) {
-    GemmArgs g;
-    g.M = static_cast<int>(M); g.N = Kout; g.K = Nred;
-    g.A = dY; g.lda = lddy; g.a_fmt = FMT_F16; g.B = W; g.ldb = ldw; g.b_fmt = FMT_F16; g.b_mn = 1;
-    g.alpha_ptr = alpha_ptr;
-    g.beta = beta; g.C32 = C32; g.ldc32 = ldc32; g.C16 = C16; g.ldc16 = ldc16; g.c16_fmt = FMT_F16;
-    if (aux16) { g.act = 2; g.aux16 = aux16; g.ldaux = ldaux; }
-    return launch_gemm(g, st);
-}
-// wgrad: dW[N,K] = dY[R,N]^T X[R,K]     (both operands MN-major views of the natural tensors)
-int gemm_wgrad(cudaStream_t st, int N, int K, long long R, const void* dY, long long lddy, const void* X, long long ldx,
-               float* dW, long long ldw, const float* inv_scale) {
-    if (R <= 0) return cudaMemsetAsync(dW, 0, sizeof(float) * N * ldw, st) == cudaSuccess ? 0 : ft_set_error("memset failed");
-    GemmArgs g;
-    g.M = N; g.N = K; g.K = static_cast<int>(R);
-    g.A = dY; g.lda = lddy; g.a_fmt = FMT_F16; g.a_mn = 1; g.B = X; g.ldb = ldx; g.b_fmt = FMT_F16; g.b_mn = 1;
-    g.alpha_ptr = inv_scale;          // undo the loss scale on the way out
-    g.C32 = dW; g.ldc32 = ldw;
-    return launch_gemm(g, st);
-}
-
-// Side stream for work that is off the backward critical path (weight gradients, bias column sums): it runs under the
-// next persistent BPTT kernel, which occupies 64 of the SMs.  One side stream + event per caller stream; ordering is
-// by events only (fork: side waits for "main so far"; join: main waits for "side so far").
-struct Side {
-    cudaStream_t s = nullptr;
-    cudaEvent_t ev_main = nullptr, ev_side = nullptr;
+// Streams of one caller stream's flow steps, created on its first call; ordering between them is by events only.
+// side: work off the backward critical path (weight gradients, bias column sums), which runs under the next persistent BPTT
+// kernel (64 of the SMs); fork: side waits for "main so far", join: main waits for "side so far".
+// sA / sB run the recurrences of the layer pipeline and the attention overlap at HIGH priority, so that when a chunk ends its
+// 64 SMs go to the next chunk (a cooperative launch that needs all of them at once) and not to queued CTAs of the GEMM /
+// attention kernels that share the machine; sC runs their per-chunk GEMMs one priority level above default streams.
+struct Streams {
+    cudaStream_t side = nullptr, sA = nullptr, sB = nullptr, sC = nullptr;
+    cudaEvent_t ev_main = nullptr, ev_side = nullptr, evA = nullptr, evG = nullptr, evB = nullptr, ev0 = nullptr, evJ = nullptr;
 };
-static std::map<cudaStream_t, Side> g_sides;
-static std::mutex g_side_mu;
+static std::map<cudaStream_t, Streams> g_streams;
+static std::mutex g_streams_mu;
 
-static Side* get_side(cudaStream_t main) {
-    std::lock_guard<std::mutex> lk(g_side_mu);
-    auto it = g_sides.find(main);
-    if (it != g_sides.end()) return &it->second;
-    Side sd;
-    if (cudaStreamCreateWithFlags(&sd.s, cudaStreamNonBlocking) != cudaSuccess) return nullptr;
-    cudaEventCreateWithFlags(&sd.ev_main, cudaEventDisableTiming);
-    cudaEventCreateWithFlags(&sd.ev_side, cudaEventDisableTiming);
-    g_sides[main] = sd;
-    return &g_sides[main];
-}
-static cudaStream_t fork_side(Side* sd, cudaStream_t main) {      // returns the stream to launch off-path work on
-    if (!sd) return main;
-    cudaEventRecord(sd->ev_main, main);
-    cudaStreamWaitEvent(sd->s, sd->ev_main, 0);
-    return sd->s;
-}
-static void join_side(Side* sd, cudaStream_t main) {
-    if (!sd) return;
-    cudaEventRecord(sd->ev_side, sd->s);
-    cudaStreamWaitEvent(main, sd->ev_side, 0);
-}
-
-// Streams of the layer pipeline and the attention overlap.  sA / sB run the two recurrences at HIGH priority, so that when a
-// chunk ends its 64 SMs go to the next chunk (a cooperative launch that needs all of them at once) and not to queued CTAs of
-// the GEMM / attention kernels that share the machine; sC runs their per-chunk GEMMs one priority level above default streams.
-struct Pipe {
-    cudaStream_t sA = nullptr, sB = nullptr, sC = nullptr;
-    cudaEvent_t evA = nullptr, evG = nullptr, evB = nullptr, ev0 = nullptr, evJ = nullptr;
-};
-static std::map<cudaStream_t, Pipe> g_pipes;
-static Pipe* get_pipe(cudaStream_t main) {
-    std::lock_guard<std::mutex> lk(g_side_mu);
-    auto it = g_pipes.find(main);
-    if (it != g_pipes.end()) return &it->second;
-    Pipe pp;
+static Streams* get_streams(cudaStream_t main) {
+    std::lock_guard<std::mutex> lk(g_streams_mu);
+    auto it = g_streams.find(main);
+    if (it != g_streams.end()) return &it->second;
+    Streams s;
     int prio_lo = 0, prio_hi = 0;
-    cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);            // hi is numerically smaller
-    if (cudaStreamCreateWithPriority(&pp.sA, cudaStreamNonBlocking, prio_hi) != cudaSuccess) return nullptr;
-    if (cudaStreamCreateWithPriority(&pp.sB, cudaStreamNonBlocking, prio_hi) != cudaSuccess) return nullptr;
+    if (cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi) != cudaSuccess) return nullptr;   // hi is numerically smaller
     const int mid = prio_hi < prio_lo - 1 ? prio_lo - 1 : prio_lo;
-    if (cudaStreamCreateWithPriority(&pp.sC, cudaStreamNonBlocking, mid) != cudaSuccess) return nullptr;
-    cudaEventCreateWithFlags(&pp.evJ, cudaEventDisableTiming);
-    cudaEventCreateWithFlags(&pp.evA, cudaEventDisableTiming);
-    cudaEventCreateWithFlags(&pp.evG, cudaEventDisableTiming);
-    cudaEventCreateWithFlags(&pp.evB, cudaEventDisableTiming);
-    cudaEventCreateWithFlags(&pp.ev0, cudaEventDisableTiming);
-    g_pipes[main] = pp;
-    return &g_pipes[main];
+    if (cudaStreamCreateWithFlags(&s.side, cudaStreamNonBlocking) != cudaSuccess ||
+        cudaStreamCreateWithPriority(&s.sA, cudaStreamNonBlocking, prio_hi) != cudaSuccess ||
+        cudaStreamCreateWithPriority(&s.sB, cudaStreamNonBlocking, prio_hi) != cudaSuccess ||
+        cudaStreamCreateWithPriority(&s.sC, cudaStreamNonBlocking, mid) != cudaSuccess)
+        return nullptr;
+    for (cudaEvent_t* e : {&s.ev_main, &s.ev_side, &s.evJ, &s.evA, &s.evG, &s.evB, &s.ev0})
+        if (cudaEventCreateWithFlags(e, cudaEventDisableTiming) != cudaSuccess) return nullptr;
+    return &(g_streams[main] = s);
 }
 
-int zero(void* p, size_t bytes, cudaStream_t st) {
-    return cudaMemsetAsync(p, 0, bytes, st) == cudaSuccess ? 0 : ft_set_error("cudaMemsetAsync failed");
+// Every stream in `waiters` waits for what `producer` has been given so far.
+static int order(cudaEvent_t ev, cudaStream_t producer, std::initializer_list<cudaStream_t> waiters) {
+    FT_CU(cudaEventRecord(ev, producer), "ar_step");
+    for (cudaStream_t w : waiters) FT_CU(cudaStreamWaitEvent(w, ev, 0), "ar_step");
+    return 0;
 }
-int copy_f32(float* dst, const float* src, size_t n, cudaStream_t st) {
-    return cudaMemcpyAsync(dst, src, n * sizeof(float), cudaMemcpyDeviceToDevice, st) == cudaSuccess ? 0 : ft_set_error("cudaMemcpyAsync failed");
-}
+static int fork_side(const Streams* s, cudaStream_t main) { return order(s->ev_main, main, {s->side}); }
+static int join_side(const Streams* s, cudaStream_t main) { return order(s->ev_side, s->side, {main}); }
 
 }  // namespace
 
@@ -335,9 +257,9 @@ int ar_step_fwd(const FtArStepDesc& d, const FtArStepWeights& w, const float* me
     if (d.has_prior && !prior) return ft_set_error("ar_step_fwd: has_prior set but attn_prior is NULL");
     if (d.has_gate && (!gates || !w.gate_w)) return ft_set_error("ar_step_fwd: has_gate set but gate pointers are NULL");
     const Dims n(d);
-    Plan ps; ps.base = static_cast<uint8_t*>(saved);
+    Workspace ps; ps.base = static_cast<uint8_t*>(saved);
     Saved S; S.plan(ps, d);
-    Plan pf; pf.base = static_cast<uint8_t*>(scratch);
+    Workspace pf; pf.base = static_cast<uint8_t*>(scratch);
     FwdScratch F; F.plan(pf, d);
 
     // fp16 operand copies of the weights (61 M params; redone every call so optimizer updates are seen)
@@ -358,7 +280,7 @@ int ar_step_fwd(const FtArStepDesc& d, const FtArStepWeights& w, const float* me
     FT_TRY(launch_prep_mel(mel, out_lens, n.T, n.B, n.M, d.reversed, S.mel_in16, S.mel_flow, st));
     const float* mel_flow = d.reversed ? S.mel_flow : mel;
 
-    Pipe* pp = get_pipe(st);
+    Streams* pp = get_streams(st);
     if (!pp) return ft_set_error("ar_step_fwd: could not create the pipeline streams");
 
     // Attention-LSTM / attention overlap (T >= kAttnChunk + 64): the attention LSTM runs as a 64-CTA recurrence in chunks of
@@ -369,7 +291,7 @@ int ar_step_fwd(const FtArStepDesc& d, const FtArStepWeights& w, const float* me
     // one chunk ahead.  Short chunks lose: every chunk boundary costs a kernel drain + launch + 128 KB weight reload on 64 SMs.
     auto attention_rows = [&](cudaStream_t s2, int t0, int t1) -> int {      // Q projection, attention, gate logits of steps [t0, t1)
         const long long r0 = static_cast<long long>(t0) * n.B, rows = static_cast<long long>(t1 - t0) * n.B;
-        FT_TRY(gemm_fwd(s2, rows, n.A, H, S.d16 + r0 * n.D, n.D, F.w.wq, H, nullptr, nullptr, 0, S.Q + r0 * n.A, n.A, nullptr, 0));
+        FT_TRY(gemm_nt(s2, rows, n.A, H, S.d16 + r0 * n.D, n.D, F.w.wq, H, S.Q + r0 * n.A, n.A));
         AttnFwdArgs a;
         a.T = n.T; a.B = n.B; a.L = n.L; a.A = n.A;
         a.Q = S.Q; a.ldq = n.A; a.K = S.Kp; a.ldk = n.A; a.V = S.Vp; a.ldv = n.A; a.v = w.att_v;
@@ -388,42 +310,34 @@ int ar_step_fwd(const FtArStepDesc& d, const FtArStepWeights& w, const float* me
             if (cudaStreamWaitEvent(s2, text_ready, 0) != cudaSuccess) return ft_set_error("ar_step_fwd: cudaStreamWaitEvent(text_ready) failed");
         }
         FT_TRY(launch_cast(text, 2, S.text16, 0, n.RL * n.E, s2));
-        FT_TRY(gemm_fwd(s2, n.RL, n.A, n.E, S.text16, n.E, F.w.wk, n.E, nullptr, nullptr, 0, S.Kp, n.A, nullptr, 0));
-        FT_TRY(gemm_fwd(s2, n.RL, n.A, n.E, S.text16, n.E, F.w.wv, n.E, nullptr, nullptr, 0, S.Vp, n.A, nullptr, 0));
+        FT_TRY(gemm_nt(s2, n.RL, n.A, n.E, S.text16, n.E, F.w.wk, n.E, S.Kp, n.A));
+        FT_TRY(gemm_nt(s2, n.RL, n.A, n.E, S.text16, n.E, F.w.wv, n.E, S.Vp, n.A));
         return 0;
     };
     if (n.T >= kAttnChunk + 64) {
         const int CH = kAttnChunk;
         auto xa = [&](cudaStream_t s2, int t0, int t1) {              // attention-LSTM input projection of steps [t0, t1) -> F.X1 rows
             const long long r0 = static_cast<long long>(t0) * n.B, rows = static_cast<long long>(t1 - t0) * n.B;
-            return gemm_fwd(s2, rows, G, n.M, S.mel_in16 + r0 * n.M, n.M, F.w.w_ih_a, n.M, w.attn_lstm_b_ih, w.attn_lstm_b_hh, 0,
-                            F.X1 + r0 * G, G, nullptr, 0);
+            return gemm_nt(s2, rows, G, n.M, S.mel_in16 + r0 * n.M, n.M, F.w.w_ih_a, n.M, F.X1 + r0 * G, G, nullptr, 0,
+                           w.attn_lstm_b_ih, w.attn_lstm_b_hh);
         };
         cudaStream_t sr = pp->sA;                                    // the attention LSTM's stream
-        cudaEventRecord(pp->ev0, st);
-        cudaStreamWaitEvent(sr, pp->ev0, 0);
-        cudaStreamWaitEvent(pp->sB, pp->ev0, 0);
-        cudaStreamWaitEvent(pp->sC, pp->ev0, 0);
+        FT_TRY(order(pp->ev0, st, {sr, pp->sB, pp->sC}));
         FT_TRY(kv_projections(pp->sC));
         FT_TRY(xa(sr, 0, CH < n.T ? CH : n.T));
         for (int t0 = 0; t0 < n.T; t0 += CH) {
             const int t1 = t0 + CH < n.T ? t0 + CH : n.T;
-            if (t1 < n.T) {                                            // next chunk's projection, one chunk ahead, on sB
-                FT_TRY(xa(pp->sB, t1, t1 + CH < n.T ? t1 + CH : n.T));
-                cudaEventRecord(pp->evB, pp->sB);
-            }
+            if (t1 < n.T) FT_TRY(xa(pp->sB, t1, t1 + CH < n.T ? t1 + CH : n.T));   // next chunk's projection, one chunk ahead
             FT_TRY(launch_lstm_fwd_chunk(n.T, n.B, t0, t1, F.X1, F.w.w_hh_a, out_lens, S.d16, n.D, S.gatesA, S.cA, F.flags, sr, F.hA32, H));
-            cudaEventRecord(pp->evA, sr);
-            if (t1 < n.T) cudaStreamWaitEvent(sr, pp->evB, 0);        // the next launch on sr needs its projection
-            cudaStreamWaitEvent(pp->sC, pp->evA, 0);
+            FT_TRY(order(pp->evA, sr, {pp->sC}));
+            if (t1 < n.T) FT_TRY(order(pp->evB, pp->sB, {sr}));      // the next launch on sr needs its projection
             FT_TRY(attention_rows(pp->sC, t0, t1));
             const long long r0 = static_cast<long long>(t0) * n.B, rows = static_cast<long long>(t1 - t0) * n.B;
-            FT_TRY(gemm_fwd(pp->sC, rows, G, n.D, S.d16 + r0 * n.D, n.D, F.w.w_ih0, n.D, w.lstm_b_ih0, w.lstm_b_hh0, 0, F.X + r0 * G, G, nullptr, 0));
+            FT_TRY(gemm_nt(pp->sC, rows, G, n.D, S.d16 + r0 * n.D, n.D, F.w.w_ih0, n.D, F.X + r0 * G, G, nullptr, 0, w.lstm_b_ih0,
+                           w.lstm_b_hh0));
         }
-        cudaEventRecord(pp->evG, pp->sC);
-        cudaStreamWaitEvent(st, pp->evG, 0);
-        cudaEventRecord(pp->evJ, sr);
-        cudaStreamWaitEvent(st, pp->evJ, 0);
+        FT_TRY(order(pp->evG, pp->sC, {st}));
+        FT_TRY(order(pp->evJ, sr, {st}));
     } else {
         // attention_lstm: the 80-channel input projection is folded into the persistent recurrence (no [R,4096] projection
         // tensor: one GEMM and 1 GB of HBM traffic less per flow); h lands in d16[:, 0:H].
@@ -432,7 +346,7 @@ int ar_step_fwd(const FtArStepDesc& d, const FtArStepWeights& w, const float* me
         // attention: K/V/Q projections, fused score+softmax(+prior)+context; ctx lands in d16[:, H:H+A]
         FT_TRY(kv_projections(st));
         FT_TRY(attention_rows(st, 0, n.T));
-        FT_TRY(gemm_fwd(st, n.R, G, n.D, S.d16, n.D, F.w.w_ih0, n.D, w.lstm_b_ih0, w.lstm_b_hh0, 0, F.X, G, nullptr, 0));
+        FT_TRY(gemm_nt(st, n.R, G, n.D, S.d16, n.D, F.w.w_ih0, n.D, F.X, G, nullptr, 0, w.lstm_b_ih0, w.lstm_b_hh0));
     }
 
     // 2-layer lstm: layer 1 at step t needs layer 0 only up to t, so the two recurrences run as two 64-CTA kernels one chunk
@@ -441,31 +355,23 @@ int ar_step_fwd(const FtArStepDesc& d, const FtArStepWeights& w, const float* me
     int* flagsA = F.flags;
     int* flagsB = F.flags + static_cast<size_t>(CH) * 16;
     cudaStream_t sr = pp->sA;                                    // layer 0's recurrence stream
-    cudaEventRecord(pp->ev0, st);
-    cudaStreamWaitEvent(sr, pp->ev0, 0);
-    cudaStreamWaitEvent(pp->sB, pp->ev0, 0);
-    cudaStreamWaitEvent(pp->sC, pp->ev0, 0);
+    FT_TRY(order(pp->ev0, st, {sr, pp->sB, pp->sC}));
     for (int t0 = 0; t0 < n.T; t0 += CH) {
         const int t1 = t0 + CH < n.T ? t0 + CH : n.T;
         const long long r0 = static_cast<long long>(t0) * n.B, rows = static_cast<long long>(t1 - t0) * n.B;
         FT_TRY(launch_lstm_fwd_chunk(n.T, n.B, t0, t1, F.X, F.w.w_hh0, out_lens, S.h0_16, H, S.gates0, S.c0, flagsA, sr));
-        cudaEventRecord(pp->evA, sr);
-        cudaStreamWaitEvent(pp->sC, pp->evA, 0);
-        FT_TRY(gemm_fwd(pp->sC, rows, G, H, S.h0_16 + r0 * H, H, F.w.w_ih1, H, w.lstm_b_ih1, w.lstm_b_hh1, 0,
-                        F.X1 + r0 * G, G, nullptr, 0));
-        cudaEventRecord(pp->evG, pp->sC);
-        cudaStreamWaitEvent(pp->sB, pp->evG, 0);
+        FT_TRY(order(pp->evA, sr, {pp->sC}));
+        FT_TRY(gemm_nt(pp->sC, rows, G, H, S.h0_16 + r0 * H, H, F.w.w_ih1, H, F.X1 + r0 * G, G, nullptr, 0, w.lstm_b_ih1, w.lstm_b_hh1));
+        FT_TRY(order(pp->evG, pp->sC, {pp->sB}));
         FT_TRY(launch_lstm_fwd_chunk(n.T, n.B, t0, t1, F.X1, F.w.w_hh1, out_lens, S.h1_16, H, S.gates1, S.c1, flagsB, pp->sB));
     }
-    cudaEventRecord(pp->evB, pp->sB);
-    cudaStreamWaitEvent(st, pp->evB, 0);
-    cudaEventRecord(pp->evJ, sr);
-    cudaStreamWaitEvent(st, pp->evJ, 0);
+    FT_TRY(order(pp->evB, pp->sB, {st}));
+    FT_TRY(order(pp->evJ, sr, {st}));
 
     // dense x2 (tanh fused in the GEMM epilogue), 1x1 conv, affine coupling
-    FT_TRY(gemm_fwd(st, n.R, H, H, S.h1_16, H, F.w.w1, H, w.dense_b0, nullptr, 1, nullptr, 0, S.y1_16, H));
-    FT_TRY(gemm_fwd(st, n.R, H, H, S.y1_16, H, F.w.w2, H, w.dense_b1, nullptr, 1, nullptr, 0, S.y2_16, H));
-    FT_TRY(gemm_fwd(st, n.R, 2 * n.M, H, S.y2_16, H, F.w.wc, H, w.conv_b, nullptr, 0, S.o32, 2 * n.M, nullptr, 0));
+    FT_TRY(gemm_nt(st, n.R, H, H, S.h1_16, H, F.w.w1, H, nullptr, 0, S.y1_16, H, w.dense_b0, nullptr, 1));
+    FT_TRY(gemm_nt(st, n.R, H, H, S.y1_16, H, F.w.w2, H, nullptr, 0, S.y2_16, H, w.dense_b1, nullptr, 1));
+    FT_TRY(gemm_nt(st, n.R, 2 * n.M, H, S.y2_16, H, F.w.wc, H, S.o32, 2 * n.M, nullptr, 0, w.conv_b));
     FT_TRY(launch_affine_fwd(S.o32, mel_flow, out_lens, n.T, n.B, n.M, d.reversed, mel_out, log_s, st));
     return 0;
 }
@@ -476,7 +382,7 @@ int ar_step_fwd(const FtArStepDesc& d, const FtArStepWeights& w, const float* me
 static int lstm_bias_grads(const uint16_t* dG, long long R, float* db_ih, float* db_hh, const float* iS, cudaStream_t st) {
     float* first = db_ih ? db_ih : db_hh;
     if (first) FT_TRY(launch_colsum(dG, 0, G, R, G, first, iS, st));
-    if (db_ih && db_hh) FT_TRY(copy_f32(db_hh, db_ih, G, st));
+    if (db_ih && db_hh) FT_CU(cudaMemcpyAsync(db_hh, db_ih, sizeof(float) * G, cudaMemcpyDeviceToDevice, st), "ar_step");
     return 0;
 }
 
@@ -489,11 +395,11 @@ int ar_step_bwd_main(const FtArStepDesc& d, const FtArStepWeights& w, const floa
     FT_TRY(check_desc(d));
     const Dims n(d);
     const unsigned m = bwd_plan(d, g, d_text != nullptr, !d.no_d_mel);
-    Plan ps; ps.base = static_cast<uint8_t*>(saved);
+    Workspace ps; ps.base = static_cast<uint8_t*>(saved);
     Saved S_; S_.plan(ps, d);
-    Plan pb; pb.base = static_cast<uint8_t*>(scratch);
+    Workspace pb; pb.base = static_cast<uint8_t*>(scratch);
     BwdScratch F; F.plan(pb, d);
-    Plan pc; pc.base = static_cast<uint8_t*>(carry);
+    Workspace pc; pc.base = static_cast<uint8_t*>(carry);
     BwdCarry C; C.plan(pc, d);
     const float* mel_flow = d.reversed ? S_.mel_flow : mel;
     const long long R = n.R, RL = n.RL, Rm = n.R - n.B;     // Rm: rows with a predecessor step
@@ -519,86 +425,76 @@ int ar_step_bwd_main(const FtArStepDesc& d, const FtArStepWeights& w, const floa
     const float* S = C.scale;            // S[0] = scale, S[1] = 1/scale
     const float* iS = C.scale + 1;
 
-    Side* sd = get_side(st);
-    cudaStream_t ss;
+    Streams* pp = get_streams(st);
+    if (!pp) return ft_set_error("ar_step_bwd: could not create the pipeline streams");
+    const cudaStream_t ss = pp->side;
 
     // 1. affine coupling (scales the incoming gradients by S)
     if (m & FT_BWD_COUPLING)
         FT_TRY(launch_affine_bwd(d_mel_out, d_log_s, S_.o32, mel_flow, out_lens, n.T, n.B, n.M, d.reversed, F.do16, C.dmel_flow, S, st));
 
     // 2. 1x1 conv     (weight / bias gradients go to the side stream, the dgrad chain stays on `st`)
-    ss = fork_side(sd, st);
+    FT_TRY(fork_side(pp, st));
     if (g.conv_w) FT_TRY(gemm_wgrad(ss, 2 * n.M, H, R, F.do16, 2 * n.M, S_.y2_16, H, g.conv_w, H, iS));
     if (g.conv_b) FT_TRY(launch_colsum(F.do16, 0, 2 * n.M, R, 2 * n.M, g.conv_b, iS, ss));
     if (m & FT_BWD_CONV_DGRAD)
-        FT_TRY(gemm_dgrad(st, R, H, 2 * n.M, F.do16, 2 * n.M, F.w.wc, H, 0, nullptr, 0, F.dy2, H, S_.y2_16, H));     // * (1 - y2^2)
+        FT_TRY(gemm_dgrad(st, R, H, 2 * n.M, F.do16, 2 * n.M, F.w.wc, H, nullptr, 0, F.dy2, H, 0, nullptr, S_.y2_16, H));     // * (1 - y2^2)
 
     // 3. dense layer 1 (second linear)
-    ss = fork_side(sd, st);
+    FT_TRY(fork_side(pp, st));
     if (g.dense_w1) FT_TRY(gemm_wgrad(ss, H, H, R, F.dy2, H, S_.y1_16, H, g.dense_w1, H, iS));
     if (g.dense_b1) FT_TRY(launch_colsum(F.dy2, 0, H, R, H, g.dense_b1, iS, ss));
     if (m & FT_BWD_DENSE1_DGRAD)
-        FT_TRY(gemm_dgrad(st, R, H, H, F.dy2, H, F.w.w2, H, 0, nullptr, 0, F.dy1, H, S_.y1_16, H));               // * (1 - y1^2)
+        FT_TRY(gemm_dgrad(st, R, H, H, F.dy2, H, F.w.w2, H, nullptr, 0, F.dy1, H, 0, nullptr, S_.y1_16, H));               // * (1 - y1^2)
 
     // 4. dense layer 0
-    ss = fork_side(sd, st);
+    FT_TRY(fork_side(pp, st));
     if (g.dense_w0) FT_TRY(gemm_wgrad(ss, H, H, R, F.dy1, H, S_.h1_16, H, g.dense_w0, H, iS));
     if (g.dense_b0) FT_TRY(launch_colsum(F.dy1, 0, H, R, H, g.dense_b0, iS, ss));
-    if (m & FT_BWD_DENSE0_DGRAD) FT_TRY(gemm_dgrad(st, R, H, H, F.dy1, H, F.w.w1, H, 0, F.dh, H, nullptr, 0, nullptr, 0));
+    if (m & FT_BWD_DENSE0_DGRAD) FT_TRY(gemm_dgrad(st, R, H, H, F.dy1, H, F.w.w1, H, F.dh, H));
 
     if (m & FT_BWD_ATTN) {
-        FT_TRY(zero(F.dK, sizeof(float) * RL * n.A, st));
-        FT_TRY(zero(F.dV, sizeof(float) * RL * n.A, st));
+        FT_CU(cudaMemsetAsync(F.dK, 0, sizeof(float) * RL * n.A, st), "ar_step");
+        FT_CU(cudaMemsetAsync(F.dV, 0, sizeof(float) * RL * n.A, st), "ar_step");
     }
-    if (g.att_v) FT_TRY(zero(g.att_v, sizeof(float) * n.A, st));
+    if (g.att_v) FT_CU(cudaMemsetAsync(g.att_v, 0, sizeof(float) * n.A, st), "ar_step");
     if (m & FT_BWD_G_GATE) {
-        if (g.gate_w) FT_TRY(zero(g.gate_w, sizeof(float) * n.D, st));
-        if (g.gate_b) FT_TRY(zero(g.gate_b, sizeof(float), st));
+        if (g.gate_w) FT_CU(cudaMemsetAsync(g.gate_w, 0, sizeof(float) * n.D, st), "ar_step");
+        if (g.gate_b) FT_CU(cudaMemsetAsync(g.gate_b, 0, sizeof(float), st), "ar_step");
     }
     // 5 + 6. lstm layers 1 and 0: BPTT of layer 1 (sA) and layer 0 (sB) one chunk apart; the layer-1 dgrad of a finished chunk
     // (sC) turns dG1 rows into layer 0's incoming dh rows (F.dh is reused row-disjointly: layer 1 only reads rows below the
     // chunk it has finished).  Highest chunk first.
-    Pipe* pp = get_pipe(st);
-    if (!pp) return ft_set_error("ar_step_bwd: could not create the pipeline streams");
     if (m & FT_BWD_LSTM1) {
         const bool l0 = (m & FT_BWD_LSTM0) != 0;
         const int CH = layer_chunk(n.T);
         int* flagsA = F.flags;
         int* flagsB = F.flags + static_cast<size_t>(CH) * 128;
         cudaStream_t sr = pp->sA;                                    // layer 1's BPTT stream
-        cudaEventRecord(pp->ev0, st);
-        cudaStreamWaitEvent(sr, pp->ev0, 0);
-        cudaStreamWaitEvent(pp->sB, pp->ev0, 0);
-        cudaStreamWaitEvent(pp->sC, pp->ev0, 0);
+        FT_TRY(order(pp->ev0, st, {sr, pp->sB, pp->sC}));
         const int n_chunks = (n.T + CH - 1) / CH;
         for (int c = n_chunks - 1; c >= 0; --c) {
             const int t0 = c * CH, t1 = t0 + CH < n.T ? t0 + CH : n.T;
             const long long r0 = static_cast<long long>(t0) * n.B, rows = static_cast<long long>(t1 - t0) * n.B;
             FT_TRY(launch_lstm_bwd_chunk(n.T, n.B, t0, t1, F.dh, H, F.w.w_hh1, S_.gates1, S_.c1, out_lens, F.dG1, F.dcarry1, flagsA, F.xchg1, sr));
             if (!l0) continue;
-            cudaEventRecord(pp->evA, sr);
-            cudaStreamWaitEvent(pp->sC, pp->evA, 0);
-            FT_TRY(gemm_dgrad(pp->sC, rows, H, G, F.dG1 + r0 * G, G, F.w.w_ih1, H, 0, F.dh + r0 * H, H, nullptr, 0, nullptr, 0));
-            cudaEventRecord(pp->evG, pp->sC);
-            cudaStreamWaitEvent(pp->sB, pp->evG, 0);
+            FT_TRY(order(pp->evA, sr, {pp->sC}));
+            FT_TRY(gemm_dgrad(pp->sC, rows, H, G, F.dG1 + r0 * G, G, F.w.w_ih1, H, F.dh + r0 * H, H));
+            FT_TRY(order(pp->evG, pp->sC, {pp->sB}));
             FT_TRY(launch_lstm_bwd_chunk(n.T, n.B, t0, t1, F.dh, H, F.w.w_hh0, S_.gates0, S_.c0, out_lens, F.dG0, F.dcarry0, flagsB, F.xchg0, pp->sB));
         }
         // layer-1 weight gradients run under the tail of layer 0 (side stream forks from st = all of layer 1 done)
-        cudaEventRecord(pp->evJ, sr);
-        cudaStreamWaitEvent(st, pp->evJ, 0);
-        ss = fork_side(sd, st);
+        FT_TRY(order(pp->evJ, sr, {st}));
+        FT_TRY(fork_side(pp, st));
         if (g.lstm_w_hh1) FT_TRY(gemm_wgrad(ss, G, H, Rm, F.dG1 + static_cast<size_t>(n.B) * G, G, S_.h1_16, H, g.lstm_w_hh1, H, iS));
         if (g.lstm_w_ih1) FT_TRY(gemm_wgrad(ss, G, H, R, F.dG1, G, S_.h0_16, H, g.lstm_w_ih1, H, iS));
         FT_TRY(lstm_bias_grads(F.dG1, R, g.lstm_b_ih1, g.lstm_b_hh1, iS, ss));
-        if (l0) {
-            cudaEventRecord(pp->evB, pp->sB);
-            cudaStreamWaitEvent(st, pp->evB, 0);
-        }
+        if (l0) FT_TRY(order(pp->evB, pp->sB, {st}));
     }
     // (the weight gradients of lstm layer 0 and of the attention projections are launched by ar_step_bwd_attn, on the side
     //  stream underneath the attention LSTM's BPTT: dG0, dQ16, dK16, dV16 stay in the scratch area until then)
     // 6b. lstm layer 0's input gradient: dd = [dhA ; dctx]
-    if (m & FT_BWD_LSTM0) FT_TRY(gemm_dgrad(st, R, n.D, G, F.dG0, G, F.w.w_ih0, n.D, 0, C.dd, n.D, nullptr, 0, nullptr, 0));
+    if (m & FT_BWD_LSTM0) FT_TRY(gemm_dgrad(st, R, n.D, G, F.dG0, G, F.w.w_ih0, n.D, C.dd, n.D));
     // 7. gate layer (last flow only): dd is in the scaled domain, the gate's own parameter gradients are not.  A frozen gate
     //    still adds its term to dd; with dd unused, only the parameter gradients are computed.
     if ((m & (FT_BWD_GATE_DD | FT_BWD_G_GATE)) && d_gates) {
@@ -621,18 +517,17 @@ int ar_step_bwd_main(const FtArStepDesc& d, const FtArStepWeights& w, const floa
     // 9a. query projection (d16 = [hA ; ctx] saved in fp16, row pitch D)
     if (m & (FT_BWD_QUERY_DGRAD | FT_BWD_G_QUERY)) FT_TRY(launch_cast(F.dQ, 2, F.dQ16, 0, R * n.A, st));
     if (m & FT_BWD_QUERY_DGRAD)
-        FT_TRY(gemm_dgrad(st, R, H, n.A, F.dQ16, n.A, F.w.wq, H, 1, C.dd, n.D, nullptr, 0, nullptr, 0));   // dhA += dQ Wq
+        FT_TRY(gemm_dgrad(st, R, H, n.A, F.dQ16, n.A, F.w.wq, H, C.dd, n.D, nullptr, 0, 1));   // dhA += dQ Wq
 
     // 9b. key / value projections -> d_text
     if (m & (FT_BWD_D_TEXT | FT_BWD_G_KEY)) FT_TRY(launch_cast(F.dK, 2, F.dK16, 0, RL * n.A, st));
     if (m & (FT_BWD_D_TEXT | FT_BWD_G_VALUE)) FT_TRY(launch_cast(F.dV, 2, F.dV16, 0, RL * n.A, st));
     if (m & FT_BWD_D_TEXT) {
-        FT_TRY(gemm_dgrad(st, RL, n.E, n.A, F.dK16, n.A, F.w.wk, n.E, 0, d_text, n.E, nullptr, 0, nullptr, 0, iS));
-        FT_TRY(gemm_dgrad(st, RL, n.E, n.A, F.dV16, n.A, F.w.wv, n.E, 1, d_text, n.E, nullptr, 0, nullptr, 0, iS));
+        FT_TRY(gemm_dgrad(st, RL, n.E, n.A, F.dK16, n.A, F.w.wk, n.E, d_text, n.E, nullptr, 0, 0, iS));
+        FT_TRY(gemm_dgrad(st, RL, n.E, n.A, F.dV16, n.A, F.w.wv, n.E, d_text, n.E, nullptr, 0, 1, iS));
     }
 
-    join_side(sd, st);                   // everything this call launched is ordered before what the caller enqueues next
-    return 0;
+    return join_side(pp, st);            // everything this call launched is ordered before what the caller enqueues next
 }
 
 // Attention-LSTM part: BPTT over dhA (carry), its weight gradients, and the input gradient d_mel (coupling path from carry +
@@ -643,23 +538,24 @@ int ar_step_bwd_attn(const FtArStepDesc& d, const FtArStepWeights& w, const int*
     FT_TRY(check_desc(d));
     const Dims n(d);
     const unsigned m = bwd_plan(d, g, false, !d.no_d_mel);
-    Plan ps; ps.base = static_cast<uint8_t*>(saved);
+    Workspace ps; ps.base = static_cast<uint8_t*>(saved);
     Saved S_; S_.plan(ps, d);
-    Plan pb; pb.base = static_cast<uint8_t*>(scratch);
+    Workspace pb; pb.base = static_cast<uint8_t*>(scratch);
     BwdScratch F; F.plan(pb, d);
-    Plan pc; pc.base = static_cast<uint8_t*>(carry);
+    Workspace pc; pc.base = static_cast<uint8_t*>(carry);
     BwdCarry C; C.plan(pc, d);
     const long long R = n.R, Rm = n.R - n.B;
     const float* iS = C.scale + 1;
-    Side* sd = get_side(st);
-    cudaStream_t ss;
+    Streams* pp = get_streams(st);
+    if (!pp) return ft_set_error("ar_step_bwd: could not create the pipeline streams");
+    const cudaStream_t ss = pp->side;
     const long long RL = n.RL;
     if (m & FT_BWD_D_MEL) FT_TRY(launch_cast(w.attn_lstm_w_ih, 2, F.w.w_ih_a, 0, static_cast<long long>(G) * n.M, st));
     if (m & FT_BWD_ATTN_LSTM) FT_TRY(launch_transpose_cast_f16(w.attn_lstm_w_hh, F.w.w_hh_a, G, H, st));
 
     // deferred from ar_step_bwd_main: weight gradients of lstm layer 0 and of the attention projections, on the side stream,
     // underneath the BPTT kernel below (64 of the SMs)
-    ss = fork_side(sd, st);
+    FT_TRY(fork_side(pp, st));
     if (g.lstm_w_hh0) FT_TRY(gemm_wgrad(ss, G, H, Rm, F.dG0 + static_cast<size_t>(n.B) * G, G, S_.h0_16, H, g.lstm_w_hh0, H, iS));
     if (g.lstm_w_ih0) FT_TRY(gemm_wgrad(ss, G, n.D, R, F.dG0, G, S_.d16, n.D, g.lstm_w_ih0, n.D, iS));
     FT_TRY(lstm_bias_grads(F.dG0, R, g.lstm_b_ih0, g.lstm_b_hh0, iS, ss));
@@ -669,18 +565,17 @@ int ar_step_bwd_attn(const FtArStepDesc& d, const FtArStepWeights& w, const int*
 
     // 10. attention_lstm  (dhA = C.dd[:, 0:H], pitch D)
     if (m & FT_BWD_ATTN_LSTM) FT_TRY(launch_lstm_bwd(n.T, n.B, C.dd, n.D, F.w.w_hh_a, S_.gatesA, S_.cA, out_lens, F.dGa, F.flags, st));
-    ss = fork_side(sd, st);
+    FT_TRY(fork_side(pp, st));
     if (g.attn_lstm_w_hh)
         FT_TRY(gemm_wgrad(ss, G, H, Rm, F.dGa + static_cast<size_t>(n.B) * G, G, S_.d16, n.D, g.attn_lstm_w_hh, H, iS));
     if (g.attn_lstm_w_ih) FT_TRY(gemm_wgrad(ss, G, n.M, R, F.dGa, G, S_.mel_in16, n.M, g.attn_lstm_w_ih, n.M, iS));
     FT_TRY(lstm_bias_grads(F.dGa, R, g.attn_lstm_b_ih, g.attn_lstm_b_hh, iS, ss));
-    if (m & FT_BWD_D_MEL) FT_TRY(gemm_dgrad(st, R, n.M, G, F.dGa, G, F.w.w_ih_a, n.M, 0, F.dmel_in, n.M, nullptr, 0, nullptr, 0));
+    if (m & FT_BWD_D_MEL) FT_TRY(gemm_dgrad(st, R, n.M, G, F.dGa, G, F.w.w_ih_a, n.M, F.dmel_in, n.M));
 
     // 11. input gradient: coupling path + (shifted) attention_lstm path, back to natural time, loss scale undone
     if ((m & FT_BWD_D_MEL) && d_mel)
         FT_TRY(launch_combine_dmel(C.dmel_flow, F.dmel_in, out_lens, n.T, n.B, n.M, d.reversed, d_mel, iS, st));
-    join_side(sd, st);                   // everything this call launched is ordered before what the caller enqueues next
-    return 0;
+    return join_side(pp, st);            // everything this call launched is ordered before what the caller enqueues next
 }
 
 }  // namespace ft
@@ -689,23 +584,23 @@ int ar_step_bwd_attn(const FtArStepDesc& d, const FtArStepWeights& w, const int*
 extern "C" {
 
 size_t ft_ar_step_saved_bytes(const FtArStepDesc* d) {
-    ft::Plan p; ft::Saved s; s.plan(p, *d);
+    ft::Workspace p; ft::Saved s; s.plan(p, *d);
     return p.off + 256;
 }
 size_t ft_ar_step_bwd_carry_bytes(const FtArStepDesc* d) {
-    ft::Plan pc; ft::BwdCarry c; c.plan(pc, *d);
+    ft::Workspace pc; ft::BwdCarry c; c.plan(pc, *d);
     return pc.off + 256;
 }
 size_t ft_ar_step_scratch_bytes(const FtArStepDesc* d) {
-    ft::Plan pf; ft::FwdScratch f; f.plan(pf, *d);
-    ft::Plan pb; ft::BwdScratch b; b.plan(pb, *d);
+    ft::Workspace pf; ft::FwdScratch f; f.plan(pf, *d);
+    ft::Workspace pb; ft::BwdScratch b; b.plan(pb, *d);
     // the one-call backward (ft_ar_step_bwd) places its carry area behind the backward scratch
     const size_t bwd = ((pb.off + 255) & ~static_cast<size_t>(255)) + ft_ar_step_bwd_carry_bytes(d);
     return (pf.off > bwd ? pf.off : bwd) + 256;
 }
 int ft_ar_step_saved_lookup(const FtArStepDesc* d, const char* name, size_t* offset, size_t* bytes) {
     std::vector<ft::Region> regs;
-    ft::Plan p; p.regs = &regs;
+    ft::Workspace p; p.regs = &regs;
     ft::Saved s; s.plan(p, *d);
     for (const auto& r : regs)
         if (std::strcmp(r.name, name) == 0) { *offset = r.off; *bytes = r.bytes; return 0; }
@@ -727,7 +622,7 @@ int ft_ar_step_bwd(const FtArStepDesc* d, const FtArStepWeights* w, const float*
                    const float* d_gates, const float* d_attn, const float* d_attn_logprob, float* d_mel, float* d_text,
                    const FtArStepWeights* g, void* saved, void* scratch, void* stream) {
     if (!d || !w || !mel || !attn || !g || !saved || !scratch) return ft::ft_set_error("ft_ar_step_bwd: NULL argument");
-    ft::Plan pb; ft::BwdScratch b; b.plan(pb, *d);
+    ft::Workspace pb; ft::BwdScratch b; b.plan(pb, *d);
     void* carry = static_cast<uint8_t*>(scratch) + ((pb.off + 255) & ~static_cast<size_t>(255));
     FtArStepDesc dd = *d;
     if (!d_mel) dd.no_d_mel = 1;

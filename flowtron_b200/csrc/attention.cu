@@ -47,10 +47,6 @@ struct AttnFwdParams {
     float* rows;                         // kGlobalRows: score rows [B][T rounded up to 64][Lr + 4]
 };
 
-__device__ __forceinline__ int back_index(int t, int len, int T) {     // flowtron.py:606-613 as an index map
-    return t < len ? len - 1 - t : T - 1 - t + len;
-}
-
 __device__ __forceinline__ float exp2x_clamped(float x) {               // e^{2x}, x clamped to +-40
     float xc = fminf(fmaxf(x, -40.f), 40.f);
     return fast_ex2(2.8853900817779268f * xc);

@@ -167,42 +167,6 @@ int launch_bmm(int nb, int M, int N, int K, BmmOperand A, BmmOperand Bt, float* 
     return ft_check_launch("attn_bmm_kernel");
 }
 
-// C[M, N] = A[M, K] W[N, K]^T, both fp16 K-major (the split operands: K = 3 x the true contraction)
-int gemm_nt(cudaStream_t st, long long M, int N, int K, const void* A, const void* W, float* C) {
-    GemmArgs g;
-    g.M = static_cast<int>(M); g.N = N; g.K = K;
-    g.A = A; g.lda = K; g.a_fmt = FMT_F16; g.B = W; g.ldb = K; g.b_fmt = FMT_F16;
-    g.C32 = C; g.ldc32 = N;
-    return launch_gemm(g, st);
-}
-// dX[M, Kout] = (1/S) dY16[M, N] W16[N, Kout]
-int gemm_dgrad(cudaStream_t st, long long M, int Kout, int N, const void* dY, const void* W, float* dX, const float* inv_scale) {
-    GemmArgs g;
-    g.M = static_cast<int>(M); g.N = Kout; g.K = N;
-    g.A = dY; g.lda = N; g.a_fmt = FMT_F16; g.B = W; g.ldb = Kout; g.b_fmt = FMT_F16; g.b_mn = 1;
-    g.alpha_ptr = inv_scale; g.C32 = dX; g.ldc32 = Kout;
-    return launch_gemm(g, st);
-}
-// dW[N, K] = (1/S) dY16[R, N]^T X16[R, K]
-int gemm_wgrad(cudaStream_t st, int N, int K, long long R, const void* dY, const void* X, float* dW, const float* inv_scale) {
-    GemmArgs g;
-    g.M = N; g.N = K; g.K = static_cast<int>(R);
-    g.A = dY; g.lda = N; g.a_fmt = FMT_F16; g.a_mn = 1; g.B = X; g.ldb = K; g.b_fmt = FMT_F16; g.b_mn = 1;
-    g.alpha_ptr = inv_scale; g.C32 = dW; g.ldc32 = K;
-    return launch_gemm(g, st);
-}
-
-struct Carve {
-    uint8_t* base = nullptr;
-    size_t off = 0;
-    template <typename T>
-    T* get(size_t n) {
-        const size_t o = off;
-        off = (off + n * sizeof(T) + 255) & ~static_cast<size_t>(255);
-        return base ? reinterpret_cast<T*>(base + o) : nullptr;
-    }
-};
-
 struct Dims {
     long long R, RL, BTL, BA;         // BA: row pitch of the projections between consecutive t (or l)
     int T, B, L, Dq, E, A;
@@ -215,7 +179,7 @@ struct Dims {
 // forward -> backward: the fp32 projections and, with a prior, the first softmax
 struct Saved {
     float *Q, *K, *V, *p_save;
-    void plan(Carve& c, const FtAttentionDesc& d) {
+    void plan(Workspace& c, const FtAttentionDesc& d) {
         const Dims n(d);
         Q = d.attn_given ? nullptr : c.get<float>(n.R * n.A);
         K = d.attn_given ? nullptr : c.get<float>(n.RL * n.A);
@@ -227,7 +191,7 @@ struct Saved {
 struct FwdScratch {
     __half *xq, *xk, *xv, *wq, *wk, *wv, *ctx16;
     float *ctx32, *rows;
-    void plan(Carve& c, const FtAttentionDesc& d) {
+    void plan(Workspace& c, const FtAttentionDesc& d) {
         const Dims n(d);
         const bool full = !d.attn_given;
         xv = c.get<__half>(n.RL * 3 * n.E);
@@ -245,7 +209,7 @@ struct FwdScratch {
 struct BwdScratch {
     float *scale, *dctx, *dQ, *dK, *dV, *dv, *rows;
     __half *dQ16, *dK16, *dV16, *wq16, *wk16, *wv16, *xq16, *xk16, *xv16;
-    void plan(Carve& c, const FtAttentionDesc& d) {
+    void plan(Workspace& c, const FtAttentionDesc& d) {
         const Dims n(d);
         const bool full = !d.attn_given;
         scale = c.get<float>(8);
@@ -276,22 +240,18 @@ int check_desc(const FtAttentionDesc* d) {
     return 0;
 }
 
-int zero(void* p, size_t bytes, cudaStream_t st) {
-    return cudaMemsetAsync(p, 0, bytes, st) == cudaSuccess ? 0 : ft_set_error("attention: cudaMemsetAsync failed");
-}
-
 int attention_fwd(const FtAttentionDesc& d, const FtAttentionWeights& w, const float* queries, const float* keys, const float* values,
                   const int* in_lens, const float* prior, float* output, float* attn, float* logprob, void* saved, void* scratch,
                   cudaStream_t st) {
     const Dims n(d);
-    Carve cs; cs.base = static_cast<uint8_t*>(saved);
+    Workspace cs; cs.base = static_cast<uint8_t*>(saved);
     Saved S; S.plan(cs, d);
-    Carve cf; cf.base = static_cast<uint8_t*>(scratch);
+    Workspace cf; cf.base = static_cast<uint8_t*>(scratch);
     FwdScratch F; F.plan(cf, d);
 
     FT_TRY(launch_split(w.value, n.A, n.E, 1, F.wv, st));
     FT_TRY(launch_split(values, n.RL, n.E, 0, F.xv, st));
-    FT_TRY(gemm_nt(st, n.RL, n.A, 3 * n.E, F.xv, F.wv, S.V));
+    FT_TRY(gemm_nt(st, n.RL, n.A, 3 * n.E, F.xv, 3 * n.E, F.wv, 3 * n.E, S.V, n.A));
     if (d.attn_given) {
         // output(b, a, t) = sum_l V(l*B + b, a) attn(b, t, l)
         const BmmOperand Av{S.V, n.A, 1, n.BA};
@@ -302,8 +262,8 @@ int attention_fwd(const FtAttentionDesc& d, const FtAttentionWeights& w, const f
     FT_TRY(launch_split(w.key, n.A, n.E, 1, F.wk, st));
     FT_TRY(launch_split(queries, n.R, n.Dq, 0, F.xq, st));
     FT_TRY(launch_split(keys, n.RL, n.E, 0, F.xk, st));
-    FT_TRY(gemm_nt(st, n.R, n.A, 3 * n.Dq, F.xq, F.wq, S.Q));
-    FT_TRY(gemm_nt(st, n.RL, n.A, 3 * n.E, F.xk, F.wk, S.K));
+    FT_TRY(gemm_nt(st, n.R, n.A, 3 * n.Dq, F.xq, 3 * n.Dq, F.wq, 3 * n.Dq, S.Q, n.A));
+    FT_TRY(gemm_nt(st, n.RL, n.A, 3 * n.E, F.xk, 3 * n.E, F.wk, 3 * n.E, S.K, n.A));
     AttnFwdArgs a;
     a.T = n.T; a.B = n.B; a.L = n.L; a.A = n.A;
     a.Q = S.Q; a.ldq = n.A; a.K = S.K; a.ldk = n.A; a.V = S.V; a.ldv = n.A; a.v = w.v;
@@ -321,9 +281,9 @@ int attention_bwd(const FtAttentionDesc& d, const FtAttentionWeights& w, const f
                   float* d_queries, float* d_keys, float* d_values, float* d_attn_given, const FtAttentionGrads& g, void* saved,
                   void* scratch, cudaStream_t st) {
     const Dims n(d);
-    Carve cs; cs.base = static_cast<uint8_t*>(saved);
+    Workspace cs; cs.base = static_cast<uint8_t*>(saved);
     Saved S; S.plan(cs, d);
-    Carve cb; cb.base = static_cast<uint8_t*>(scratch);
+    Workspace cb; cb.base = static_cast<uint8_t*>(scratch);
     BwdScratch F; F.plan(cb, d);
     const bool need_v = d_values || g.value;
     const long long BAT = static_cast<long long>(n.B) * n.A * n.T;
@@ -337,8 +297,7 @@ int attention_bwd(const FtAttentionDesc& d, const FtAttentionWeights& w, const f
             // d attn(b, t, l) = d_attn(b, t, l) + sum_a d_output(b, a, t) V(l*B + b, a)
             int beta = 0;
             if (d_attn) {
-                if (cudaMemcpyAsync(d_attn_given, d_attn, sizeof(float) * n.BTL, cudaMemcpyDeviceToDevice, st) != cudaSuccess)
-                    return ft_set_error("ft_attention_bwd: cudaMemcpyAsync failed");
+                FT_CU(cudaMemcpyAsync(d_attn_given, d_attn, sizeof(float) * n.BTL, cudaMemcpyDeviceToDevice, st), "ft_attention_bwd");
                 beta = 1;
             }
             if (d_output) {
@@ -346,13 +305,13 @@ int attention_bwd(const FtAttentionDesc& d, const FtAttentionWeights& w, const f
                 const BmmOperand Bv{S.V, n.A, n.BA, 1};
                 FT_TRY(launch_bmm(n.B, n.T, n.L, n.A, Ad, Bv, d_attn_given, static_cast<long long>(n.T) * n.L, n.L, 1, iS, beta, st));
             } else if (!d_attn) {
-                FT_TRY(zero(d_attn_given, sizeof(float) * n.BTL, st));
+                FT_CU(cudaMemsetAsync(d_attn_given, 0, sizeof(float) * n.BTL, st), "attention");
             }
         }
         if (!need_v) return 0;
         if (!d_output) {
-            if (d_values) FT_TRY(zero(d_values, sizeof(float) * n.RL * n.E, st));
-            if (g.value) FT_TRY(zero(g.value, sizeof(float) * n.A * n.E, st));
+            if (d_values) FT_CU(cudaMemsetAsync(d_values, 0, sizeof(float) * n.RL * n.E, st), "attention");
+            if (g.value) FT_CU(cudaMemsetAsync(g.value, 0, sizeof(float) * n.A * n.E, st), "attention");
             return 0;
         }
         // dV(l*B + b, a) = sum_t attn(b, t, l) S d_output(b, a, t): in the scaled domain, like the attention kernel's dV
@@ -366,11 +325,11 @@ int attention_bwd(const FtAttentionDesc& d, const FtAttentionWeights& w, const f
                                  d_attn, d_attn ? n.BTL : 0, d_logprob, d_logprob ? n.BTL : 0));
         if (d_output) FT_TRY(launch_transpose(d_output, static_cast<long long>(n.A) * n.T, n.T, n.A, n.T, F.dctx, n.A,
                                               n.BA, n.B, F.scale, st));
-        else FT_TRY(zero(F.dctx, sizeof(float) * n.R * n.A, st));
-        FT_TRY(zero(F.dK, sizeof(float) * n.RL * n.A, st));
-        FT_TRY(zero(F.dV, sizeof(float) * n.RL * n.A, st));
+        else FT_CU(cudaMemsetAsync(F.dctx, 0, sizeof(float) * n.R * n.A, st), "attention");
+        FT_CU(cudaMemsetAsync(F.dK, 0, sizeof(float) * n.RL * n.A, st), "attention");
+        FT_CU(cudaMemsetAsync(F.dV, 0, sizeof(float) * n.RL * n.A, st), "attention");
         float* dv = g.v ? g.v : F.dv;
-        FT_TRY(zero(dv, sizeof(float) * n.A, st));
+        FT_CU(cudaMemsetAsync(dv, 0, sizeof(float) * n.A, st), "attention");
         AttnBwdArgs a;
         a.T = n.T; a.B = n.B; a.L = n.L; a.A = n.A;
         a.Q = S.Q; a.ldq = n.A; a.K = S.K; a.ldk = n.A; a.V = S.V; a.ldv = n.A; a.v = w.v;
@@ -383,22 +342,22 @@ int attention_bwd(const FtAttentionDesc& d, const FtAttentionWeights& w, const f
             FT_TRY(launch_cast(F.dQ, 2, F.dQ16, 0, n.R * n.A, st));
             if (d_queries) {
                 FT_TRY(launch_cast(w.query, 2, F.wq16, 0, static_cast<long long>(n.A) * n.Dq, st));
-                FT_TRY(gemm_dgrad(st, n.R, n.Dq, n.A, F.dQ16, F.wq16, d_queries, iS));
+                FT_TRY(gemm_dgrad(st, n.R, n.Dq, n.A, F.dQ16, n.A, F.wq16, n.Dq, d_queries, n.Dq, nullptr, 0, 0, iS));
             }
             if (g.query) {
                 FT_TRY(launch_cast(queries, 2, F.xq16, 0, n.R * n.Dq, st));
-                FT_TRY(gemm_wgrad(st, n.A, n.Dq, n.R, F.dQ16, F.xq16, g.query, iS));
+                FT_TRY(gemm_wgrad(st, n.A, n.Dq, n.R, F.dQ16, n.A, F.xq16, n.Dq, g.query, n.Dq, iS));
             }
         }
         if (need_k) {
             FT_TRY(launch_cast(F.dK, 2, F.dK16, 0, n.RL * n.A, st));
             if (d_keys) {
                 FT_TRY(launch_cast(w.key, 2, F.wk16, 0, static_cast<long long>(n.A) * n.E, st));
-                FT_TRY(gemm_dgrad(st, n.RL, n.E, n.A, F.dK16, F.wk16, d_keys, iS));
+                FT_TRY(gemm_dgrad(st, n.RL, n.E, n.A, F.dK16, n.A, F.wk16, n.E, d_keys, n.E, nullptr, 0, 0, iS));
             }
             if (g.key) {
                 FT_TRY(launch_cast(keys, 2, F.xk16, 0, n.RL * n.E, st));
-                FT_TRY(gemm_wgrad(st, n.A, n.E, n.RL, F.dK16, F.xk16, g.key, iS));
+                FT_TRY(gemm_wgrad(st, n.A, n.E, n.RL, F.dK16, n.A, F.xk16, n.E, g.key, n.E, iS));
             }
         }
         if (!need_v) return 0;
@@ -407,11 +366,11 @@ int attention_bwd(const FtAttentionDesc& d, const FtAttentionWeights& w, const f
     FT_TRY(launch_cast(F.dV, 2, F.dV16, 0, n.RL * n.A, st));
     if (d_values) {
         FT_TRY(launch_cast(w.value, 2, F.wv16, 0, static_cast<long long>(n.A) * n.E, st));
-        FT_TRY(gemm_dgrad(st, n.RL, n.E, n.A, F.dV16, F.wv16, d_values, iS));
+        FT_TRY(gemm_dgrad(st, n.RL, n.E, n.A, F.dV16, n.A, F.wv16, n.E, d_values, n.E, nullptr, 0, 0, iS));
     }
     if (g.value) {
         FT_TRY(launch_cast(values, 2, F.xv16, 0, n.RL * n.E, st));
-        FT_TRY(gemm_wgrad(st, n.A, n.E, n.RL, F.dV16, F.xv16, g.value, iS));
+        FT_TRY(gemm_wgrad(st, n.A, n.E, n.RL, F.dV16, n.A, F.xv16, n.E, g.value, n.E, iS));
     }
     return 0;
 }
@@ -424,14 +383,14 @@ extern "C" {
 
 size_t ft_attention_saved_bytes(const FtAttentionDesc* d) {
     if (!d || ft::check_desc(d)) return 0;
-    ft::Carve c; ft::Saved s; s.plan(c, *d);
+    ft::Workspace c; ft::Saved s; s.plan(c, *d);
     return c.off + 256;
 }
 
 size_t ft_attention_scratch_bytes(const FtAttentionDesc* d) {
     if (!d || ft::check_desc(d)) return 0;
-    ft::Carve cf; ft::FwdScratch f; f.plan(cf, *d);
-    ft::Carve cb; ft::BwdScratch b; b.plan(cb, *d);
+    ft::Workspace cf; ft::FwdScratch f; f.plan(cf, *d);
+    ft::Workspace cb; ft::BwdScratch b; b.plan(cb, *d);
     return (cf.off > cb.off ? cf.off : cb.off) + 256;
 }
 

@@ -22,8 +22,6 @@ static inline int grid_for(long long work_items, int threads, int per_sm = 8) {
     return static_cast<int>(blocks < 1 ? 1 : (blocks > cap ? cap : blocks));
 }
 
-__device__ __forceinline__ int back_index_d(int t, int len, int T) { return t < len ? len - 1 - t : T - 1 - t + len; }
-
 // ------------------------------------------------------------------------------------------------ casts
 template <typename TO>
 __device__ __forceinline__ TO cvt_from_float(float x);
@@ -117,7 +115,7 @@ __global__ void scale_finalize_kernel(const unsigned int* __restrict__ mx, float
 int launch_grad_scale(const float* a, long long na, const float* b, long long nb, const float* c, long long nc, float target,
                       float* scale2, cudaStream_t st, const float* d, long long nd, const float* e, long long ne) {
     unsigned int* mx = reinterpret_cast<unsigned int*>(scale2 + 2);
-    if (cudaMemsetAsync(mx, 0, sizeof(unsigned int), st) != cudaSuccess) return ft_set_error("grad_scale: memset failed");
+    FT_CU(cudaMemsetAsync(mx, 0, sizeof(unsigned int), st), "grad_scale");
     long long n = na > nb ? na : nb;
     n = n > nc ? n : nc;
     if (n > 0) absmax_kernel<<<grid_for(n, 256, 4), 256, 0, st>>>(a, na, b, nb, c, nc, mx);
@@ -145,12 +143,12 @@ __global__ void prep_mel_kernel(const float* __restrict__ mel, const int* __rest
         const int len = lens ? lens[b] : T;
         float xin = 0.f;
         if (q > 0) {
-            const int s = reversed ? back_index_d(q - 1, len, T) : q - 1;
+            const int s = reversed ? back_index(q - 1, len, T) : q - 1;
             xin = mel[(static_cast<long long>(s) * B + b) * M + m];
         }
         mel_in16[i] = __float2half_rn(xin);
         if (reversed && mel_flow) {
-            const int s = back_index_d(q, len, T);
+            const int s = back_index(q, len, T);
             mel_flow[i] = mel[(static_cast<long long>(s) * B + b) * M + m];
         }
     }
@@ -304,7 +302,7 @@ __global__ void affine_fwd_kernel(const float* __restrict__ o, const float* __re
         log_s[i] = ls;
         const float zz = expf(ls) * mel_flow[i] + bb;
         int s = q;
-        if (reversed) s = back_index_d(q, lens ? lens[b] : T, T);
+        if (reversed) s = back_index(q, lens ? lens[b] : T, T);
         z[(static_cast<long long>(s) * B + b) * M + m] = zz;
     }
 }
@@ -331,7 +329,7 @@ __global__ void affine_bwd_kernel(const float* __restrict__ dz, const float* __r
         const int b = static_cast<int>(rb % B), q = static_cast<int>(rb / B);
         const int len = lens ? lens[b] : T;
         int s = q;
-        if (reversed) s = back_index_d(q, len, T);
+        if (reversed) s = back_index(q, len, T);
         const float dzq = dz ? S * dz[(static_cast<long long>(s) * B + b) * M + m] : 0.f;
         const float es = expf(o[rb * 2 * M + m]);
         float dls = dzq * mel_flow[i] * es;
@@ -365,7 +363,7 @@ __global__ void combine_dmel_kernel(const float* __restrict__ dmel_flow, const f
         float g = dmel_flow[i];
         if (q + 1 < T) g += dmel_in[i + static_cast<long long>(B) * M];
         int s = q;
-        if (reversed) s = back_index_d(q, lens ? lens[b] : T, T);
+        if (reversed) s = back_index(q, lens ? lens[b] : T, T);
         dmel[(static_cast<long long>(s) * B + b) * M + m] = g * iS;
     }
 }
@@ -399,7 +397,7 @@ __global__ void colsum_kernel(const TI* __restrict__ src, long long ld, long lon
     }
 }
 int launch_colsum(const void* src, int fmt, long long ld, long long R, int C, float* out, const float* out_scale, cudaStream_t st) {
-    if (cudaMemsetAsync(out, 0, sizeof(float) * C, st) != cudaSuccess) return ft_set_error("colsum: memset failed");
+    FT_CU(cudaMemsetAsync(out, 0, sizeof(float) * C, st), "colsum");
     long long gyl = (R + 255) / 256;
     int gy = static_cast<int>(gyl > 64 ? 64 : gyl);
     if (gy < 1) gy = 1;
@@ -462,7 +460,7 @@ __global__ void nll_reduce_kernel(const float* __restrict__ z, const LogSList lo
 int launch_nll_reduce(const float* z, const float* const* log_s_list_host, int n_flows, const float* gate,
                       const float* gate_target, const int* lens, int T, int B, int M, float* sums, cudaStream_t st) {
     if (n_flows < 0 || n_flows > NLL_MAX_FLOWS) return ft_set_error("nll_reduce: more than 16 flows not supported");
-    if (cudaMemsetAsync(sums, 0, sizeof(float) * 4, st) != cudaSuccess) return ft_set_error("nll: memset failed");
+    FT_CU(cudaMemsetAsync(sums, 0, sizeof(float) * 4, st), "nll");
     LogSList ls;
     for (int f = 0; f < NLL_MAX_FLOWS; ++f) ls.p[f] = f < n_flows ? log_s_list_host[f] : nullptr;
     const long long n = static_cast<long long>(T) * B * M;

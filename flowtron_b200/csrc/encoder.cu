@@ -508,14 +508,8 @@ int enc_bilstm_bwd(const EncLstmBwdParams& p, cudaStream_t st) { return p.B <= 1
 
 int enc_wgrad3(cudaStream_t st, int M, int N, long long K, const __half* A, int wa, const __half* B, long long ldb, int wb,
                const float* alpha_ptr, float* C32) {
-    for (int term = 0; term < 3; ++term) {
-        GemmArgs g;
-        g.M = M; g.N = N; g.K = static_cast<int>(K);
-        g.A = A + (term == 1 ? wa : 0); g.lda = 3 * wa; g.a_fmt = FMT_F16; g.a_mn = 1;
-        g.B = B + (term == 2 ? wb : 0); g.ldb = ldb; g.b_fmt = FMT_F16; g.b_mn = 1;
-        g.alpha_ptr = alpha_ptr; g.beta = term > 0; g.C32 = C32; g.ldc32 = N;
-        if (launch_gemm(g, st)) return -1;
-    }
+    for (int term = 0; term < 3; ++term)
+        FT_TRY(gemm_wgrad(st, M, N, K, A + (term == 1 ? wa : 0), 3 * wa, B + (term == 2 ? wb : 0), ldb, C32, N, alpha_ptr, term > 0));
     return 0;
 }
 
@@ -525,39 +519,36 @@ EncStack enc_stack_plan(const EncStackDesc& a, int B, int L, bool masked, const 
     P.a = &a; P.B = B; P.L = L;
     P.rows = static_cast<long long>(B) * (L + 2 * EPADR);
     const size_t rows = static_cast<size_t>(P.rows);
-    uint8_t* sv = static_cast<uint8_t*>(const_cast<void*>(saved));
-    uint8_t* sc = static_cast<uint8_t*>(scratch);
-    size_t off = 0;
-    auto get = [&](uint8_t* base, size_t bytes) { size_t o = off; off = (off + bytes + 255) & ~size_t(255); return base ? base + o : nullptr; };
-    for (int i = 0; i <= a.layers; ++i) P.X16[i] = reinterpret_cast<__half*>(get(sv, rows * 3 * (i == 0 ? a.cp0 : EC) * 2));
-    for (int i = 0; i < a.layers; ++i) P.Y32[i] = reinterpret_cast<float*>(get(sv, rows * EC * 4));
-    for (int i = 0; i < a.layers; ++i) { P.mean[i] = reinterpret_cast<float*>(get(sv, size_t(B) * EC * 4)); P.rstd[i] = reinterpret_cast<float*>(get(sv, size_t(B) * EC * 4)); }
+    Workspace sv; sv.base = static_cast<uint8_t*>(const_cast<void*>(saved));
+    for (int i = 0; i <= a.layers; ++i) P.X16[i] = sv.get<__half>(rows * 3 * (i == 0 ? a.cp0 : EC));
+    for (int i = 0; i < a.layers; ++i) P.Y32[i] = sv.get<float>(rows * EC);
+    for (int i = 0; i < a.layers; ++i) { P.mean[i] = sv.get<float>(size_t(B) * EC); P.rstd[i] = sv.get<float>(size_t(B) * EC); }
     for (int k = 0; k < 2; ++k) {
-        P.hseq[k] = reinterpret_cast<__half*>(get(sv, rows * 2 * EH * 2));
-        P.gates[k] = reinterpret_cast<__half*>(get(sv, rows * EG * 2));
-        P.cstate[k] = reinterpret_cast<float*>(get(sv, rows * EH * 4));
+        P.hseq[k] = sv.get<__half>(rows * 2 * EH);
+        P.gates[k] = sv.get<__half>(rows * EG);
+        P.cstate[k] = sv.get<float>(rows * EH);
     }
-    int* lens = reinterpret_cast<int*>(get(sv, size_t(B) * 4 + 16));
+    int* lens = sv.get<int>(size_t(B) + 4);
     P.lens = masked ? lens : nullptr;
-    P.inv_n = reinterpret_cast<float*>(get(sv, a.inv_n_bytes));
-    P.saved_bytes = off;
-    off = 0;
+    P.inv_n = reinterpret_cast<float*>(sv.get<uint8_t>(a.inv_n_bytes));
+    P.saved_bytes = sv.off;
+    Workspace sc; sc.base = static_cast<uint8_t*>(scratch);
     if (!bwd) {
-        P.xproj = reinterpret_cast<float*>(get(sc, rows * 2 * EG * 4));
-        P.hout = reinterpret_cast<float*>(get(sc, size_t(B) * L * a.hout_bytes_per_token));
-        for (int i = 0; i < a.layers; ++i) P.wconv16[i] = reinterpret_cast<__half*>(get(sc, size_t(a.taps) * EC * 3 * (i == 0 ? a.cp0 : EC) * 2));
-        P.wih16 = reinterpret_cast<__half*>(get(sc, size_t(2) * EG * 3 * EC * 2));
-        P.fwd_bytes = off;
+        P.xproj = sc.get<float>(rows * 2 * EG);
+        P.hout = reinterpret_cast<float*>(sc.get<uint8_t>(size_t(B) * L * a.hout_bytes_per_token));
+        for (int i = 0; i < a.layers; ++i) P.wconv16[i] = sc.get<__half>(size_t(a.taps) * EC * 3 * (i == 0 ? a.cp0 : EC));
+        P.wih16 = sc.get<__half>(size_t(2) * EG * 3 * EC);
+        P.fwd_bytes = sc.off;
     } else {
-        for (int k = 0; k < 2; ++k) P.dG[k] = reinterpret_cast<__half*>(get(sc, rows * 3 * EG * 2));
-        P.dY16 = reinterpret_cast<__half*>(get(sc, rows * 3 * EC * 2));
-        P.DX32 = reinterpret_cast<float*>(get(sc, rows * EC * 4));
-        P.dwk = reinterpret_cast<float*>(get(sc, size_t(a.taps) * EC * EC * 4));
-        P.scale2 = reinterpret_cast<float*>(get(sc, 256));
-        P.dmean = reinterpret_cast<float*>(get(sc, size_t(B) * a.dmean_bytes_per_utt));
-        P.wconv16_b = reinterpret_cast<__half*>(get(sc, size_t(a.taps) * 3 * EC * EC * 2));
-        P.wih16_b = reinterpret_cast<__half*>(get(sc, size_t(2) * 3 * EG * EC * 2));
-        P.bwd_bytes = off;
+        for (int k = 0; k < 2; ++k) P.dG[k] = sc.get<__half>(rows * 3 * EG);
+        P.dY16 = sc.get<__half>(rows * 3 * EC);
+        P.DX32 = sc.get<float>(rows * EC);
+        P.dwk = sc.get<float>(size_t(a.taps) * EC * EC);
+        P.scale2 = sc.get<float>(64);
+        P.dmean = reinterpret_cast<float*>(sc.get<uint8_t>(size_t(B) * a.dmean_bytes_per_utt));
+        P.wconv16_b = sc.get<__half>(size_t(a.taps) * 3 * EC * EC);
+        P.wih16_b = sc.get<__half>(size_t(2) * 3 * EG * EC);
+        P.bwd_bytes = sc.off;
     }
     return P;
 }
@@ -581,15 +572,10 @@ int enc_stack_fwd(const EncStack& S, const EncStackWeights& w, float eps, float 
         const int cin = i == 0 ? a.cin0 : EC, cp = i == 0 ? a.cp0 : EC;
         a.pack_conv(w.conv_w[i], cin, cp, S.wconv16[i], nullptr, st);
         ft_count_launch(1);
-        for (int k = 0; k < a.taps; ++k) {
-            GemmArgs g;                                               // one GEMM per tap: contraction over [hi | lo | hi] x [hi | hi | lo]
-            g.M = static_cast<int>(S.rows - 2 * EPADR); g.N = EC; g.K = 3 * cp;
-            g.A = S.X16[i] + static_cast<size_t>(tap0 + k) * 3 * cp; g.lda = 3 * cp; g.a_fmt = FMT_F16;
-            g.B = S.wconv16[i] + static_cast<size_t>(k) * EC * 3 * cp; g.ldb = 3 * cp; g.b_fmt = FMT_F16;
-            g.bias = k == 0 ? w.conv_b[i] : nullptr; g.beta = k > 0;
-            g.C32 = S.Y32[i] + static_cast<size_t>(EPADR) * EC; g.ldc32 = EC;
-            FT_TRY(launch_gemm(g, st));
-        }
+        for (int k = 0; k < a.taps; ++k)                              // one GEMM per tap: contraction over [hi | lo | hi] x [hi | hi | lo]
+            FT_TRY(gemm_nt(st, S.rows - 2 * EPADR, EC, 3 * cp, S.X16[i] + static_cast<size_t>(tap0 + k) * 3 * cp, 3 * cp,
+                           S.wconv16[i] + static_cast<size_t>(k) * EC * 3 * cp, 3 * cp, S.Y32[i] + static_cast<size_t>(EPADR) * EC, EC,
+                           nullptr, 0, k == 0 ? w.conv_b[i] : nullptr, nullptr, 0, k > 0));
         enc_norm_fwd_kernel<<<dim3(S.B, EC / 32), 256, 0, st>>>(S.Y32[i], S.lens, S.L, w.norm_w[i], w.norm_b[i], eps, drop_p,
                                                                  drop_p > 0.f ? rng : nullptr, i, S.X16[i + 1], S.mean[i], S.rstd[i]);
         ft_count_launch(1);
@@ -600,13 +586,8 @@ int enc_stack_fwd(const EncStack& S, const EncStackWeights& w, float eps, float 
         __half* wih = S.wih16 + static_cast<size_t>(k) * EG * 3 * EC;
         enc_pack_wih_kernel<<<296, 256, 0, st>>>(w.w_ih[k], wih, nullptr);
         ft_count_launch(1);
-        GemmArgs g;
-        g.M = static_cast<int>(S.rows); g.N = EG; g.K = 3 * EC;
-        g.A = S.X16[a.layers]; g.lda = 3 * EC; g.a_fmt = FMT_F16;
-        g.B = wih; g.ldb = 3 * EC; g.b_fmt = FMT_F16;
-        g.bias = w.b_ih[k]; g.bias2 = w.b_hh[k];
-        g.C32 = S.xproj + static_cast<size_t>(k) * EG; g.ldc32 = 2 * EG;
-        FT_TRY(launch_gemm(g, st));
+        FT_TRY(gemm_nt(st, S.rows, EG, 3 * EC, S.X16[a.layers], 3 * EC, wih, 3 * EC, S.xproj + static_cast<size_t>(k) * EG, 2 * EG,
+                       nullptr, 0, w.b_ih[k], w.b_hh[k]));
     }
     EncLstmFwdParams p;
     p.B = S.B; p.L = S.L; p.lens = S.lens; p.xproj = S.xproj;
@@ -638,12 +619,8 @@ int enc_stack_bwd(const EncStack& S, const EncStackWeights& w, const EncStackGra
         enc_colsum_hilo_kernel<<<EG / 32, 256, 0, st>>>(S.dG[k], rows, EG, iS, g.d_b_ih[k]);
         ft_count_launch(1);
         FT_CU(cudaMemcpyAsync(g.d_b_hh[k], g.d_b_ih[k], sizeof(float) * EG, cudaMemcpyDeviceToDevice, st), who);
-        GemmArgs x;                                                   // dx (+)= dG W_ih: [hi | lo | hi] x [hi ; hi ; lo]
-        x.M = static_cast<int>(rows); x.N = EC; x.K = 3 * EG;
-        x.A = S.dG[k]; x.lda = 3 * EG; x.a_fmt = FMT_F16;
-        x.B = wih; x.ldb = EC; x.b_fmt = FMT_F16; x.b_mn = 1;
-        x.beta = k > 0; x.C32 = S.DX32; x.ldc32 = EC;
-        FT_TRY(launch_gemm(x, st));
+        // dx (+)= dG W_ih: [hi | lo | hi] x [hi ; hi ; lo]
+        FT_TRY(gemm_dgrad(st, rows, EC, 3 * EG, S.dG[k], 3 * EG, wih, EC, S.DX32, EC, nullptr, 0, k > 0));
     }
     const int tap0 = EPADR - (a.taps - 1) / 2;
     for (int i = a.layers - 1; i >= 0; --i) {
@@ -666,14 +643,10 @@ int enc_stack_bwd(const EncStack& S, const EncStackWeights& w, const EncStackGra
         // dx_i = sum_k dY shifted by -tap . W_k (the layers that get here read 512 channels)
         a.pack_conv(w.conv_w[i], cin, cp, nullptr, S.wconv16_b, st);
         ft_count_launch(1);
-        for (int k = 0; k < a.taps; ++k) {
-            GemmArgs d;
-            d.M = static_cast<int>(rows - 2 * EPADR); d.N = EC; d.K = 3 * EC;
-            d.A = S.dY16 + static_cast<size_t>(2 * EPADR - tap0 - k) * 3 * EC; d.lda = 3 * EC; d.a_fmt = FMT_F16;
-            d.B = S.wconv16_b + static_cast<size_t>(k) * 3 * EC * EC; d.ldb = EC; d.b_fmt = FMT_F16; d.b_mn = 1;
-            d.beta = k > 0; d.C32 = S.DX32 + static_cast<size_t>(EPADR) * EC; d.ldc32 = EC;
-            FT_TRY(launch_gemm(d, st));
-        }
+        for (int k = 0; k < a.taps; ++k)
+            FT_TRY(gemm_dgrad(st, rows - 2 * EPADR, EC, 3 * EC, S.dY16 + static_cast<size_t>(2 * EPADR - tap0 - k) * 3 * EC, 3 * EC,
+                              S.wconv16_b + static_cast<size_t>(k) * 3 * EC * EC, EC, S.DX32 + static_cast<size_t>(EPADR) * EC, EC,
+                              nullptr, 0, k > 0));
     }
     return 0;
 }

@@ -13,10 +13,6 @@ constexpr int EC = 512, EH = 256, EG = 4 * EH;      // embedding / conv channels
 constexpr int EK = 5, EPADR = 2;                    // conv taps, pad rows on either side of an utterance
 constexpr int ENC_THREADS = 256, ENC_CLUSTER = 8, ENC_UNITS = EH / ENC_CLUSTER;   // 32 units per CTA
 
-__device__ __forceinline__ void mma16816(float (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]) : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
-}
 __device__ __forceinline__ uint32_t pack_h2(float a, float b) { const __half2 h = __floats2half2_rn(a, b); return *reinterpret_cast<const uint32_t*>(&h); }
 __device__ __forceinline__ uint4 ldcg_v4(const void* p) {
     uint4 v;

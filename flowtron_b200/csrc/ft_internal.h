@@ -3,6 +3,7 @@
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <vector>
 
 namespace ft {
 
@@ -21,6 +22,27 @@ void ft_count_launch(int n);
 #define FT_TRY(x) do { if ((x) != 0) return -1; } while (0)
 // check a CUDA runtime call; `who` prefixes the recorded message
 #define FT_CU(x, who) do { if ((x) != cudaSuccess) return ::ft::ft_runtime_error(who); } while (0)
+
+// Carves a caller-owned workspace into regions, each starting on a 256-byte boundary, in the order they are asked for.
+// base == nullptr plans sizes only (off is then the size); regs, when set, records every region for a by-name lookup.
+struct Region { const char* name; size_t off, bytes; };
+struct Workspace {
+    uint8_t* base = nullptr;
+    size_t off = 0;
+    std::vector<Region>* regs = nullptr;
+    size_t take(size_t bytes) {                     // offset of the next region of `bytes`
+        const size_t o = off;
+        off = (off + bytes + 255) & ~static_cast<size_t>(255);
+        return o;
+    }
+    template <typename T>
+    T* get(const char* name, size_t n) {
+        const size_t o = take(n * sizeof(T));
+        if (regs) regs->push_back({name, o, n * sizeof(T)});
+        return base ? reinterpret_cast<T*>(base + o) : nullptr;
+    }
+    template <typename T> T* get(size_t n) { return get<T>(nullptr, n); }
+};
 
 // RAII device-time bracket around a launch (no-op unless ft_timing_enable(1))
 struct TimeScope {
@@ -42,6 +64,20 @@ struct GemmArgs {
     void* C16 = nullptr; long long ldc16 = 0; int c16_fmt = 0;
 };
 int launch_gemm(const GemmArgs& g, cudaStream_t st);
+// The three roles of launch_gemm on fp16 operands (gemm.cu).  Outputs: fp32 C32 and / or fp16 C16; beta: C32 += the product;
+// alpha_ptr: a device scalar the product is multiplied by (the inverse loss scale of a backward; null = 1).
+// forward: C[M, N] = A[M, K] B[N, K]^T (+ bias[N] + bias2[N]), act 1 = tanh
+int gemm_nt(cudaStream_t st, long long M, int N, int K, const void* A, long long lda, const void* B, long long ldb, float* C32,
+            long long ldc32, void* C16 = nullptr, long long ldc16 = 0, const float* bias = nullptr, const float* bias2 = nullptr,
+            int act = 0, int beta = 0);
+// dgrad: dX[M, Kout] = dY[M, N] W[N, Kout] (W given MN-major); aux16 (fp16 [M, Kout] tanh output) multiplies by 1 - aux^2
+int gemm_dgrad(cudaStream_t st, long long M, int Kout, int N, const void* dY, long long lddy, const void* W, long long ldw,
+               float* C32, long long ldc32, void* C16 = nullptr, long long ldc16 = 0, int beta = 0, const float* alpha_ptr = nullptr,
+               const void* aux16 = nullptr, long long ldaux = 0);
+// wgrad: dW[N, K] = dY[R, N]^T X[R, K] (both MN-major views of the natural tensors), dW row pitch ldw; a sum over R <= 0
+// rows sets dW to 0 (or, with beta, leaves it)
+int gemm_wgrad(cudaStream_t st, int N, int K, long long R, const void* dY, long long lddy, const void* X, long long ldx, float* dW,
+               long long ldw, const float* alpha_ptr, int beta = 0);
 void set_gemm_pair_mode(int mode);   // 0 never, 1 big contractions only (default), 2 whenever eligible
 int make_tmap_2d(CUtensorMap* out, const void* ptr, int fmt, long long rows, long long cols, long long ld,
                  int box_cols, int box_rows, int swizzle_bytes = 128);   // 128 or 64: the box's inner extent in bytes

@@ -91,9 +91,7 @@ int launch_gemm(const GemmArgs& g, cudaStream_t st) {
         if (splitk > 16) splitk = 16;
         while (splitk > 1 && num_kb_all / splitk < 16) --splitk;
     }
-    if (splitk > 1) {
-        if (cudaMemsetAsync(g.C32, 0, sizeof(float) * static_cast<size_t>(g.M) * g.N, st) != cudaSuccess) return ft_set_error("gemm: memset failed");
-    }
+    if (splitk > 1) FT_CU(cudaMemsetAsync(g.C32, 0, sizeof(float) * static_cast<size_t>(g.M) * g.N, st), "gemm");
     p.splitk = splitk;
     // Staged TMA-store epilogue wherever the outputs allow it (16-byte aligned base and row pitch, even N, the pair loads of
     // bias / aux aligned); anything else keeps the fragment stores.  C32 += tile goes through TMA reduce-add for split-K
@@ -165,6 +163,42 @@ int launch_gemm(const GemmArgs& g, cudaStream_t st) {
     if (e != cudaSuccess) return ft_set_error(cudaGetErrorString(e));
     ft_count_launch(1);
     return ft_check_launch(ncta == 2 ? "gemm2_kernel<pair>" : "gemm2_kernel");
+}
+
+int gemm_nt(cudaStream_t st, long long M, int N, int K, const void* A, long long lda, const void* B, long long ldb, float* C32,
+            long long ldc32, void* C16, long long ldc16, const float* bias, const float* bias2, int act, int beta) {
+    GemmArgs g;
+    g.M = static_cast<int>(M); g.N = N; g.K = K;
+    g.A = A; g.lda = lda; g.a_fmt = FMT_F16; g.B = B; g.ldb = ldb; g.b_fmt = FMT_F16;
+    g.bias = bias; g.bias2 = bias2; g.act = act; g.beta = beta;
+    g.C32 = C32; g.ldc32 = ldc32; g.C16 = C16; g.ldc16 = ldc16; g.c16_fmt = FMT_F16;
+    return launch_gemm(g, st);
+}
+
+int gemm_dgrad(cudaStream_t st, long long M, int Kout, int N, const void* dY, long long lddy, const void* W, long long ldw,
+               float* C32, long long ldc32, void* C16, long long ldc16, int beta, const float* alpha_ptr, const void* aux16,
+               long long ldaux) {
+    GemmArgs g;
+    g.M = static_cast<int>(M); g.N = Kout; g.K = N;
+    g.A = dY; g.lda = lddy; g.a_fmt = FMT_F16; g.B = W; g.ldb = ldw; g.b_fmt = FMT_F16; g.b_mn = 1;
+    g.alpha_ptr = alpha_ptr; g.beta = beta;
+    g.C32 = C32; g.ldc32 = ldc32; g.C16 = C16; g.ldc16 = ldc16; g.c16_fmt = FMT_F16;
+    if (aux16) { g.act = 2; g.aux16 = aux16; g.ldaux = ldaux; }
+    return launch_gemm(g, st);
+}
+
+int gemm_wgrad(cudaStream_t st, int N, int K, long long R, const void* dY, long long lddy, const void* X, long long ldx, float* dW,
+               long long ldw, const float* alpha_ptr, int beta) {
+    if (R <= 0) {
+        if (!beta) FT_CU(cudaMemsetAsync(dW, 0, sizeof(float) * N * ldw, st), "gemm_wgrad");
+        return 0;
+    }
+    GemmArgs g;
+    g.M = N; g.N = K; g.K = static_cast<int>(R);
+    g.A = dY; g.lda = lddy; g.a_fmt = FMT_F16; g.a_mn = 1; g.B = X; g.ldb = ldx; g.b_fmt = FMT_F16; g.b_mn = 1;
+    g.alpha_ptr = alpha_ptr; g.beta = beta;
+    g.C32 = dW; g.ldc32 = ldw;
+    return launch_gemm(g, st);
 }
 
 }  // namespace ft

@@ -236,12 +236,6 @@ __device__ __forceinline__ void stage3(__half* sx, int cA, const void* srcA, int
     else stage3_small<kF32>(sx, cA, srcA, KA, pitchA, cB, srcB, KB, pitchB, cC, srcC, KC, pitchC, B, status);
 }
 
-__device__ __forceinline__ void mma_16816(float (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-                 : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
-}
-
 // d[16 batch x 8 rows] += sum over k-blocks [m0, m1) of  x[batch][k] * W[row][k].  Wt: this task's packed weights
 // ([k-block][8 rows][32 k]); lane (n = lane/4, j = lane%4) owns row n and the 8 k values 8j..8j+7 of every block; the k order
 // inside a block is a fixed permutation shared by both operands (any bijection is a valid contraction order):
@@ -262,8 +256,8 @@ __device__ __forceinline__ void mv_partial(const __half* __restrict__ Wt, int m0
                 const uint4 lo = *reinterpret_cast<const uint4*>(a_lo + 32 * (m + u));
                 uint4 hi = make_uint4(0u, 0u, 0u, 0u);
                 if (kB16) hi = *reinterpret_cast<const uint4*>(a_hi + 32 * (m + u));
-                mma_16816(d, lo.x, hi.x, lo.y, hi.y, w[u].x, w[u].y);
-                mma_16816(d, lo.z, hi.z, lo.w, hi.w, w[u].z, w[u].w);
+                mma16816(d, lo.x, hi.x, lo.y, hi.y, w[u].x, w[u].y);
+                mma16816(d, lo.z, hi.z, lo.w, hi.w, w[u].z, w[u].w);
             }
         }
     }
@@ -310,8 +304,8 @@ __device__ __forceinline__ void mv_phase(const __half* __restrict__ W, int n_tas
                         const uint4 lo = *reinterpret_cast<const uint4*>(a_lo + 32 * (m0 + u));
                         uint4 hi = make_uint4(0u, 0u, 0u, 0u);
                         if (kB16) hi = *reinterpret_cast<const uint4*>(a_hi + 32 * (m0 + u));
-                        mma_16816(d, lo.x, hi.x, lo.y, hi.y, pf.w[u].x, pf.w[u].y);
-                        mma_16816(d, lo.z, hi.z, lo.w, hi.w, pf.w[u].z, pf.w[u].w);
+                        mma16816(d, lo.x, hi.x, lo.y, hi.y, pf.w[u].x, pf.w[u].y);
+                        mma16816(d, lo.z, hi.z, lo.w, hi.w, pf.w[u].z, pf.w[u].w);
                     }
                 }
                 m0 = (m0 + PFN < m1) ? m0 + PFN : m1;
@@ -829,32 +823,31 @@ struct InferScratch {
 
 static InferScratch plan_infer(const FtArStepDesc& d, uint8_t* base) {
     InferScratch s;
-    size_t off = 0;
-    auto get = [&](size_t bytes) { size_t o = off; off = (off + bytes + 255) & ~size_t(255); return base ? base + o : nullptr; };
+    Workspace ws; ws.base = base;
     const int M = d.n_mel, A = d.n_attn, E = d.n_text, D = IH + A;
-    auto wbytes = [](size_t tasks, size_t nm) { return tasks * nm * 256 * 2; };
-    s.wA = reinterpret_cast<__half*>(get(wbytes(IH / 2, (XPAD + IH) / 32)));
-    s.w0 = reinterpret_cast<__half*>(get(wbytes(IH / 2, (D + IH) / 32)));
-    s.w1 = reinterpret_cast<__half*>(get(wbytes(IH / 2, 2 * IH / 32)));
-    s.wq = reinterpret_cast<__half*>(get(wbytes(A / 8, IH / 32)));
-    s.wd1 = reinterpret_cast<__half*>(get(wbytes(IH / 8, IH / 32)));
-    s.wd2 = reinterpret_cast<__half*>(get(wbytes(IH / 8, IH / 32)));
-    s.wc = reinterpret_cast<__half*>(get(wbytes(M / 4, IH / 32)));
-    s.bA = reinterpret_cast<float*>(get(IG * 4)); s.b0 = reinterpret_cast<float*>(get(IG * 4)); s.b1 = reinterpret_cast<float*>(get(IG * 4));
-    s.bd1 = reinterpret_cast<float*>(get(IH * 4)); s.bd2 = reinterpret_cast<float*>(get(IH * 4)); s.bc = reinterpret_cast<float*>(get(2 * M * 4));
-    s.wk = reinterpret_cast<uint16_t*>(get(size_t(A) * E * 2));
-    s.wv = reinterpret_cast<uint16_t*>(get(size_t(A) * E * 2));
-    s.text16 = reinterpret_cast<uint16_t*>(get(size_t(d.L) * d.B * E * 2));
-    s.Kp = reinterpret_cast<float*>(get(size_t(d.L) * d.B * A * 4));
-    s.Vp = reinterpret_cast<float*>(get(size_t(d.L) * d.B * A * 4));
+    auto w16 = [&](size_t tasks, size_t nm) { return ws.get<__half>(tasks * nm * 256); };
+    s.wA = w16(IH / 2, (XPAD + IH) / 32);
+    s.w0 = w16(IH / 2, (D + IH) / 32);
+    s.w1 = w16(IH / 2, 2 * IH / 32);
+    s.wq = w16(A / 8, IH / 32);
+    s.wd1 = w16(IH / 8, IH / 32);
+    s.wd2 = w16(IH / 8, IH / 32);
+    s.wc = w16(M / 4, IH / 32);
+    s.bA = ws.get<float>(IG); s.b0 = ws.get<float>(IG); s.b1 = ws.get<float>(IG);
+    s.bd1 = ws.get<float>(IH); s.bd2 = ws.get<float>(IH); s.bc = ws.get<float>(2 * M);
+    s.wk = ws.get<uint16_t>(size_t(A) * E);
+    s.wv = ws.get<uint16_t>(size_t(A) * E);
+    s.text16 = ws.get<uint16_t>(size_t(d.L) * d.B * E);
+    s.Kp = ws.get<float>(size_t(d.L) * d.B * A);
+    s.Vp = ws.get<float>(size_t(d.L) * d.B * A);
     // state: cell states cA, c0, c1 (3 x B*IH fp32), then the exchange rings (3 frame slots each): hA32 (B*IH), q (B*A), e (B*L),
     // alive (B) as 32-bit words; hA16, h016, h116, y116, y216 (B*IH), d16 (B*D), x16 (B*96) as fp16 (counted in floats, each piece
     // padded to 16 bytes)
     s.state_floats = size_t(d.B) * 3 * IH + 3 * (size_t(d.B) * (IH + A + d.L + 1) + 24) +
                      3 * 8 /* NREP */ * ((size_t(d.B) * (5 * IH + A + XPAD) + 1) / 2 + size_t(d.B) * A + 40) + 256;
-    s.state = reinterpret_cast<float*>(get(s.state_floats * 4));
+    s.state = ws.get<float>(s.state_floats);
     s.ints = nullptr;
-    s.total = off;
+    s.total = ws.off;
     return s;
 }
 
@@ -900,17 +893,12 @@ static int infer_impl(const FtArStepDesc* d, const FtArStepWeights* w, const flo
     FT_TRY(launch_cast(w->att_key, 2, s.wk, 0, static_cast<long long>(A) * E, st));
     FT_TRY(launch_cast(w->att_value, 2, s.wv, 0, static_cast<long long>(A) * E, st));
     FT_TRY(launch_cast(text, 2, s.text16, 0, RL * E, st));
-    {   // K / V projections once per utterance (the reference recomputes them every frame, flowtron.py:568-570)
-        GemmArgs g;
-        g.M = static_cast<int>(RL); g.N = A; g.K = E; g.A = s.text16; g.lda = E; g.a_fmt = FMT_F16;
-        g.B = s.wk; g.ldb = E; g.b_fmt = FMT_F16; g.C32 = s.Kp; g.ldc32 = A;
-        FT_TRY(launch_gemm(g, st));
-        g.B = s.wv; g.C32 = s.Vp;
-        FT_TRY(launch_gemm(g, st));
-    }
-    if (cudaMemsetAsync(out, 0, sizeof(float) * d->T * B * M, st) != cudaSuccess) return ft_set_error("infer: memset failed");
-    if (cudaMemsetAsync(attn_out, 0, sizeof(float) * d->T * B * d->L, st) != cudaSuccess) return ft_set_error("infer: memset failed");
-    if (cudaMemsetAsync(n_frames, 0, sizeof(int) * B, st) != cudaSuccess) return ft_set_error("infer: memset failed");
+    // K / V projections once per utterance (the reference recomputes them every frame, flowtron.py:568-570)
+    FT_TRY(gemm_nt(st, RL, A, E, s.text16, E, s.wk, E, s.Kp, A));
+    FT_TRY(gemm_nt(st, RL, A, E, s.text16, E, s.wv, E, s.Vp, A));
+    FT_CU(cudaMemsetAsync(out, 0, sizeof(float) * d->T * B * M, st), "infer");
+    FT_CU(cudaMemsetAsync(attn_out, 0, sizeof(float) * d->T * B * d->L, st), "infer");
+    FT_CU(cudaMemsetAsync(n_frames, 0, sizeof(int) * B, st), "infer");
 
     InferParams p;
     p.T = d->T; p.B = B; p.L = d->L; p.M = M; p.A = A; p.E = E; p.D = D;
@@ -939,14 +927,15 @@ static int infer_impl(const FtArStepDesc* d, const FtArStepWeights* w, const flo
     p.slot_bytes = (f - ring0) * static_cast<long long>(sizeof(float));
     f = ring0 + 3 * (f - ring0);
     if (static_cast<size_t>(f - s.state) > s.state_floats) return ft_set_error("infer: scratch plan overflow");
-    if (cudaMemsetAsync(s.state, 0, (ring0 - s.state) * sizeof(float), st) != cudaSuccess) return ft_set_error("infer: memset failed");
-    if (cudaMemsetAsync(ring0, 0xFF, (f - ring0) * sizeof(float), st) != cudaSuccess) return ft_set_error("infer: memset failed");
+    FT_CU(cudaMemsetAsync(s.state, 0, (ring0 - s.state) * sizeof(float), st), "infer");
+    FT_CU(cudaMemsetAsync(ring0, 0xFF, (f - ring0) * sizeof(float), st), "infer");
     // the state before frame 0 (slot 2 = frame -1): zero hidden states and a zero previous output frame
     for (int rr = 0; rr < NREP; ++rr) {
         auto slot2 = [&](void* ptr) { return static_cast<char*>(ptr) + 2 * p.slot_bytes + rr * p.rep_bytes; };
-        if (cudaMemsetAsync(slot2(p.hA16), 0, BH * 2, st) != cudaSuccess || cudaMemsetAsync(slot2(p.h016), 0, BH * 2, st) != cudaSuccess ||
-            cudaMemsetAsync(slot2(p.h116), 0, BH * 2, st) != cudaSuccess || cudaMemsetAsync(slot2(p.x16), 0, static_cast<size_t>(B) * XPAD * 2, st) != cudaSuccess)
-            return ft_set_error("infer: memset failed");
+        FT_CU(cudaMemsetAsync(slot2(p.hA16), 0, BH * 2, st), "infer");
+        FT_CU(cudaMemsetAsync(slot2(p.h016), 0, BH * 2, st), "infer");
+        FT_CU(cudaMemsetAsync(slot2(p.h116), 0, BH * 2, st), "infer");
+        FT_CU(cudaMemsetAsync(slot2(p.x16), 0, static_cast<size_t>(B) * XPAD * 2, st), "infer");
     }
     p.status = ft_status_word();
     p.trace = g_infer_trace;

@@ -35,15 +35,6 @@ struct IstftParams {
     float* out;
 };
 
-__device__ __forceinline__ int is_find_utt(const long long* __restrict__ frame_offsets, int n_utt, long long f) {
-    int lo = 0, hi = n_utt;
-    while (hi - lo > 1) {
-        const int mid = (lo + hi) >> 1;
-        if (__ldg(frame_offsets + mid) <= f) lo = mid; else hi = mid;
-    }
-    return lo;
-}
-
 // pass A source: conj Z[n] of one frame, built from the spectrum in global memory
 struct SpecSrc {
     const float* mag; const float* ph; const float* bias; float strength; int Fu; const float2* tw;
@@ -88,7 +79,7 @@ istft_kernel(IstftParams p) {
     for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         const long long t_end = min(total, (tile + 1) * tile_frames);
         for (long long f = tile * tile_frames; f < t_end;) {            // one segment per utterance in the tile
-            const int u = is_find_utt(p.frame_offsets, p.n_utt, f);
+            const int u = find_utt(p.frame_offsets, p.n_utt, f);
             const long long fo = __ldg(p.frame_offsets + u);
             const int Fu = static_cast<int>(__ldg(p.frame_offsets + u + 1) - fo);
             const long long seg_end = min(t_end, fo + Fu);

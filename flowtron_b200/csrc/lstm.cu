@@ -679,7 +679,7 @@ static int launch_fwd_t(int T, int B, int t0, int t1, const float* xproj, const 
     } else {
         tmWx = tmW; tmX = tmH;                                   // unused
     }
-    if (cudaMemsetAsync(flags, 0, sizeof(int) * (t1 - t0) * FWD_NCH, st) != cudaSuccess) return ft_set_error("lstm_fwd: memset failed");
+    FT_CU(cudaMemsetAsync(flags, 0, sizeof(int) * (t1 - t0) * FWD_NCH, st), "lstm_fwd");
     void* fn = reinterpret_cast<void*>(lstm_fwd_kernel<UNITS, kXIn>);
     cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     TimeScope ts("lstm_fwd", t1 - t0, B, 0, st);
@@ -733,8 +733,7 @@ static int launch_bwd(int T, int B, int t0, int t1, const float* dh_ext, long lo
     CUtensorMap tmWT, tmG;
     if (make_tmap_2d(&tmWT, whhT16, FMT_F16, LH, LG, LG, KCH, B4_UNITS)) return -1;
     if (make_tmap_chunks(&tmG, dG16, static_cast<long long>(T) * B, BWD_NCH, LG, p.Bbox, 8)) return -1;
-    if (cudaMemsetAsync(flags, 0, sizeof(int) * (t1 - t0) * BWD_NCH * (flat ? 2 : 1), st) != cudaSuccess)
-        return ft_set_error("lstm_bwd: memset failed");
+    FT_CU(cudaMemsetAsync(flags, 0, sizeof(int) * (t1 - t0) * BWD_NCH * (flat ? 2 : 1), st), "lstm_bwd");
     if (flat) {
         const int smem = B4_NCH * slot + B4_W_BYTES + 256 + 1024;
         cudaFuncSetAttribute(lstm_bwd_flat_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);

@@ -19,7 +19,9 @@
 
 namespace ft {
 
-__device__ __forceinline__ int find_utt(const long long* __restrict__ frame_offsets, int n_utt, long long f) {
+// mel_fft.cuh's ft::find_utt reads the offsets through __ldg, which changes these kernels' SASS; this copy keeps them as
+// they are.
+__device__ __forceinline__ int find_utt_plain(const long long* __restrict__ frame_offsets, int n_utt, long long f) {
     int lo = 0, hi = n_utt;                     // frame_offsets[lo] <= f < frame_offsets[hi]
     while (hi - lo > 1) {
         const int mid = (lo + hi) >> 1;
@@ -37,7 +39,7 @@ __global__ void frame_kernel(const float* __restrict__ wav, const long long* __r
     const long long nw = (static_cast<long long>(gridDim.x) * blockDim.x) >> 5;
     for (long long fi = w0; fi < nf; fi += nw) {
         const long long f = f0 + fi;
-        const int u = find_utt(frame_offsets, n_utt, f);
+        const int u = find_utt_plain(frame_offsets, n_utt, f);
         const long long j = f - frame_offsets[u];
         const long long s0 = sample_offsets[u], N = sample_offsets[u + 1] - s0;
         const long long start = j * hop - n_fft / 2;
@@ -72,7 +74,7 @@ mag_mel_kernel(const float2* __restrict__ spec, const long long* __restrict__ fr
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     if (lane >= nfr) return;
     const long long f = f0 + fb + lane;
-    const int u = find_utt(frame_offsets, n_utt, f);
+    const int u = find_utt_plain(frame_offsets, n_utt, f);
     const long long Fu = frame_offsets[u + 1] - frame_offsets[u], j = f - frame_offsets[u];
     float* out = mel_out + frame_offsets[u] * n_mel + j;       // per-utterance [n_mel, Fu] block
     const float* mg = smag + lane * pitch;
@@ -120,9 +122,9 @@ int ft_mel_spectrogram(const float* wav, const long long* sample_offsets, const 
     if (n_fft % 2 || n_fft > 4096 || chunk_frames <= 0) return ft_set_error("ft_mel_spectrogram: bad n_fft / chunk");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int n_bins = n_fft / 2 + 1;
-    float* frames = static_cast<float*>(scratch);
-    float2* spec = reinterpret_cast<float2*>(reinterpret_cast<uint8_t*>(scratch) +
-                                            ((static_cast<size_t>(chunk_frames) * n_fft * 4 + 255) & ~size_t(255)));
+    Workspace ws; ws.base = static_cast<uint8_t*>(scratch);
+    float* frames = ws.get<float>(static_cast<size_t>(chunk_frames) * n_fft);
+    float2* spec = ws.get<float2>(static_cast<size_t>(chunk_frames) * n_bins);
     int dev = 0, sms = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);

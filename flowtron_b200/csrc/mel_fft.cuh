@@ -118,4 +118,15 @@ __host__ __device__ __forceinline__ float inv_readout(int m, const float* zr, co
 }
 
 }  // namespace melfft
+
+// The utterance a global frame index f belongs to, over int64 prefix sums: frame_offsets[u] <= f < frame_offsets[u + 1].
+__device__ __forceinline__ int find_utt(const long long* __restrict__ frame_offsets, int n_utt, long long f) {
+    int lo = 0, hi = n_utt;
+    while (hi - lo > 1) {
+        const int mid = (lo + hi) >> 1;
+        if (__ldg(frame_offsets + mid) <= f) lo = mid; else hi = mid;
+    }
+    return lo;
+}
+
 }  // namespace ft

@@ -32,15 +32,6 @@ struct MelFusedParams {
     const float2* twiddle;                           // [1024] exp(-2 pi i j / 1024)
 };
 
-__device__ __forceinline__ int mf_find_utt(const long long* __restrict__ frame_offsets, int n_utt, long long f) {
-    int lo = 0, hi = n_utt;
-    while (hi - lo > 1) {
-        const int mid = (lo + hi) >> 1;
-        if (__ldg(frame_offsets + mid) <= f) lo = mid; else hi = mid;
-    }
-    return lo;
-}
-
 template <int kFmt>
 struct FrameSrc {
     const void* wav; long long s0, N, start; const float* window; bool fast;
@@ -103,7 +94,7 @@ mel_fused_kernel(MelFusedParams p) {
             const int fr = warp + q * MF_WARPS;
             const long long f = tile * MF_TILE + fr;
             if (f >= total) { if (lane == 0) sFu[fr] = 0; continue; }      // warp-uniform
-            const int u = mf_find_utt(p.frame_offsets, p.n_utt, f);
+            const int u = find_utt(p.frame_offsets, p.n_utt, f);
             const long long fo = __ldg(p.frame_offsets + u);
             const int Fu = static_cast<int>(__ldg(p.frame_offsets + u + 1) - fo);
             const long long j = f - fo;

@@ -38,6 +38,16 @@ __device__ __forceinline__ bool elect_one() {
     return pred != 0;
 }
 
+// d += a b on the tensor cores, one warp: m16n8k16, fp16 operands (a row-major, b column-major fragments), fp32 accumulate
+__device__ __forceinline__ void mma16816(float (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]) : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
+}
+
+// AR_Back_Step's time flip (flowtron.py:606-613) as an index map: step t of the flipped sequence of a row with len valid
+// steps out of T reads step back_index(t, len, T) (the valid steps reversed, the padding after them reversed too)
+__device__ __forceinline__ int back_index(int t, int len, int T) { return t < len ? len - 1 - t : T - 1 - t + len; }
+
 // ------------------------------------------------------------------------------------ mbarrier
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");

@@ -76,11 +76,6 @@ __device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t& r0, uint32_t& r
     asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
                  : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
 }
-__device__ __forceinline__ void mma16816(float* c, const uint32_t* a, uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
 
 __device__ __forceinline__ __half sat_half(float x) { return __float2half_rn(fminf(fmaxf(x, -65504.f), 65504.f)); }
 
@@ -207,7 +202,7 @@ __global__ void __launch_bounds__(G_THREADS, 2) wg_gemm_kernel(const __grid_cons
 #pragma unroll
             for (int i = 0; i < 4; ++i)
 #pragma unroll
-                for (int j = 0; j < 4; ++j) mma16816(acc[i][j], af[i], bf[j][0], bf[j][1]);
+                for (int j = 0; j < 4; ++j) mma16816(acc[i][j], af[i][0], af[i][1], af[i][2], af[i][3], bf[j][0], bf[j][1]);
         }
     }
     cp_async_wait<0>();
@@ -494,20 +489,19 @@ static int wg_layout(const FtWaveGlowDesc* d, WgLayout* L) {
     }
     L->mrows = static_cast<int>(m);
     L->grows = static_cast<int>(g);
-    size_t off = 0;
-    auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 255) & ~size_t(255); return o; };
+    Workspace ws;
     const size_t R = static_cast<size_t>(L->grows);
-    L->off_plan = take(sizeof(WgBatch));
-    L->off_mel16 = take(static_cast<size_t>(L->mrows) * WG_MEL_LD * 2);
-    L->off_uprow = take(static_cast<size_t>(L->mrows) * 4);
-    L->off_rowinfo = take(R * 4);
-    L->off_spect = take(R * WG_SPECT * 2);
-    L->off_h32 = take(R * WG_C * 4);
-    L->off_h16 = take(R * WG_C * 2);
-    L->off_acts = take(R * WG_C * 2);
-    L->off_skip = take(R * WG_C * 4);
-    L->off_state = take(R * 8 * 4);
-    L->total = off;
+    L->off_plan = ws.take(sizeof(WgBatch));
+    L->off_mel16 = ws.take(static_cast<size_t>(L->mrows) * WG_MEL_LD * 2);
+    L->off_uprow = ws.take(static_cast<size_t>(L->mrows) * 4);
+    L->off_rowinfo = ws.take(R * 4);
+    L->off_spect = ws.take(R * WG_SPECT * 2);
+    L->off_h32 = ws.take(R * WG_C * 4);
+    L->off_h16 = ws.take(R * WG_C * 2);
+    L->off_acts = ws.take(R * WG_C * 2);
+    L->off_skip = ws.take(R * WG_C * 4);
+    L->off_state = ws.take(R * 8 * 4);
+    L->total = ws.off;
     return 0;
 }
 
@@ -570,35 +564,33 @@ static int wt_layout(const FtWaveGlowTrainDesc* d, WtLayout* L) {
         L->c[k] = c;
     }
     const size_t R = static_cast<size_t>(L->g.grows), nf = L->nf, nfl = nf * L->nl;
-    size_t off = 0;
-    auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 255) & ~size_t(255); return o; };
-    L->s_plan = take(sizeof(WgBatch));
-    L->s_mel16 = take(static_cast<size_t>(L->g.mrows) * WG_MEL_LD * 2);
-    L->s_uprow = take(static_cast<size_t>(L->g.mrows) * 4);
-    L->s_rowinfo = take(R * 4);
-    L->s_spect = take(R * WG_SPECT * 2);
-    L->s_x = take(nf * R * 8 * 4);                     // flow inputs (before the 1x1 conv), fp32
-    L->s_skip = take(nf * R * WG_C * 4);               // WN skip sums, fp32
-    L->s_h16 = take(nfl * R * WG_C * 2);               // WN layer inputs, fp16, zero guard rows
-    L->s_pre = take(nfl * R * 2 * WG_C * 2);           // gate pre-activations, fp16, interleaved like in_w's rows
-    L->saved = off;
-    off = 0;
-    L->c_h32 = take(R * WG_C * 4);
-    L->c_acts = take(R * WG_C * 2);
-    L->c_state = take(R * 8 * 4);
-    L->c_dstate = take(R * 8 * 4);
-    L->c_dout = take(R * 8 * 4);
-    L->c_dy = take(R * 8 * 4);
-    L->c_dskip = take(R * WG_C * 2);
-    L->c_g16 = take(R * WG_C * 2);
-    L->c_g32 = take(R * WG_C * 4);
-    L->c_dx = take(R * 2 * WG_C * 2);
-    L->c_dsp32 = take(R * WG_SPECT * 4);
-    L->c_dsp16 = take(R * WG_SPECT * 2);
-    L->c_mela = take(R / 32 * 4 * WG_MEL_LD * 2);
-    L->c_zero = take(2 * WG_C * 4);
-    L->c_scale = take((nf + 1) * 4 * 4);
-    L->scratch = off;
+    Workspace sv, sc;
+    L->s_plan = sv.take(sizeof(WgBatch));
+    L->s_mel16 = sv.take(static_cast<size_t>(L->g.mrows) * WG_MEL_LD * 2);
+    L->s_uprow = sv.take(static_cast<size_t>(L->g.mrows) * 4);
+    L->s_rowinfo = sv.take(R * 4);
+    L->s_spect = sv.take(R * WG_SPECT * 2);
+    L->s_x = sv.take(nf * R * 8 * 4);                     // flow inputs (before the 1x1 conv), fp32
+    L->s_skip = sv.take(nf * R * WG_C * 4);               // WN skip sums, fp32
+    L->s_h16 = sv.take(nfl * R * WG_C * 2);               // WN layer inputs, fp16, zero guard rows
+    L->s_pre = sv.take(nfl * R * 2 * WG_C * 2);           // gate pre-activations, fp16, interleaved like in_w's rows
+    L->saved = sv.off;
+    L->c_h32 = sc.take(R * WG_C * 4);
+    L->c_acts = sc.take(R * WG_C * 2);
+    L->c_state = sc.take(R * 8 * 4);
+    L->c_dstate = sc.take(R * 8 * 4);
+    L->c_dout = sc.take(R * 8 * 4);
+    L->c_dy = sc.take(R * 8 * 4);
+    L->c_dskip = sc.take(R * WG_C * 2);
+    L->c_g16 = sc.take(R * WG_C * 2);
+    L->c_g32 = sc.take(R * WG_C * 4);
+    L->c_dx = sc.take(R * 2 * WG_C * 2);
+    L->c_dsp32 = sc.take(R * WG_SPECT * 4);
+    L->c_dsp16 = sc.take(R * WG_SPECT * 2);
+    L->c_mela = sc.take(R / 32 * 4 * WG_MEL_LD * 2);
+    L->c_zero = sc.take(2 * WG_C * 4);
+    L->c_scale = sc.take((nf + 1) * 4 * 4);
+    L->scratch = sc.off;
     return 0;
 }
 
@@ -1007,16 +999,6 @@ __global__ void wg_mela_kernel(const WgBatch* __restrict__ plan, const int* __re
     }
 }
 
-static int wt_gemm_wgrad(cudaStream_t st, int N, int K, long long R, const __half* dY, long long lddy, const __half* X, long long ldx,
-                         float* dW, const float* inv_scale) {
-    GemmArgs g;
-    g.M = N; g.N = K; g.K = static_cast<int>(R);
-    g.A = dY; g.lda = lddy; g.a_fmt = FMT_F16; g.a_mn = 1; g.B = X; g.ldb = ldx; g.b_fmt = FMT_F16; g.b_mn = 1;
-    g.alpha_ptr = inv_scale;
-    g.C32 = dW; g.ldc32 = K;
-    return launch_gemm(g, st);
-}
-
 static int wt_launch(const void* fn, const WtBwdParams& p, cudaStream_t st, const char* name) {
     TimeScope ts(name, p.R, p.nh, 0, st);
     void* args[] = {const_cast<WtBwdParams*>(&p)};
@@ -1047,9 +1029,8 @@ static int wg_infer(const FtWaveGlowDesc* d, const FtWaveGlowWeights* w, const f
     const long long R = L.grows;
 
     // zero hidden-state guard rows (the dilated taps read them) and the audio padding after each utterance
-    if (cudaMemsetAsync(h16, 0, static_cast<size_t>(R) * WG_C * 2, st) != cudaSuccess ||
-        cudaMemsetAsync(audio, 0, sizeof(float) * static_cast<size_t>(L.B) * L.Tg_max * 8, st) != cudaSuccess)
-        return ft_set_error("waveglow: memset failed");
+    FT_CU(cudaMemsetAsync(h16, 0, static_cast<size_t>(R) * WG_C * 2, st), "waveglow");
+    FT_CU(cudaMemsetAsync(audio, 0, sizeof(float) * static_cast<size_t>(L.B) * L.Tg_max * 8, st), "waveglow");
     if (launch_wg_plan_prep(L, frames_dev, d->F_max, L.Tg_max, plan, mel, mel16, uprow, rowinfo, st)) return -1;
     {   // upsample: frame row f = frames f-3..f (A segments shifted 0..-3) -> 32 group rows of 640 channels
         WgGemmParams p = {};
@@ -1171,9 +1152,8 @@ int ft_waveglow_train_fwd(const FtWaveGlowTrainDesc* d, const FtWaveGlowTrainWei
 
     // guard and padding rows of every layer input and of the upsampled spectrogram are zero: the dilated taps and the
     // row-reduced weight gradients read them
-    if (cudaMemsetAsync(h16, 0, static_cast<size_t>(L.nf) * L.nl * R * WG_C * 2, st) != cudaSuccess ||
-        cudaMemsetAsync(spect, 0, static_cast<size_t>(R) * WG_SPECT * 2, st) != cudaSuccess)
-        return ft_set_error("waveglow train: memset failed");
+    FT_CU(cudaMemsetAsync(h16, 0, static_cast<size_t>(L.nf) * L.nl * R * WG_C * 2, st), "waveglow train");
+    FT_CU(cudaMemsetAsync(spect, 0, static_cast<size_t>(R) * WG_SPECT * 2, st), "waveglow train");
     if (launch_wg_plan_prep(L.g, nullptr, L.F, L.Tn, reinterpret_cast<WgBatch*>(sv + L.s_plan), mel, mel16, uprow, rowinfo, st))
         return -1;
     {
@@ -1258,7 +1238,7 @@ int ft_waveglow_train_bwd(const FtWaveGlowTrainDesc* d, const FtWaveGlowTrainWei
     float* scale = reinterpret_cast<float*>(sc + L.c_scale);
     const long long W0 = WG_GUARD, RW = R - 2 * WG_GUARD;   // row window of the shifted-tap weight gradients
 
-    auto z0 = [&](void* p, size_t n) { return cudaMemsetAsync(p, 0, n, st) == cudaSuccess ? 0 : ft_set_error("waveglow train: memset failed"); };
+    auto z0 = [&](void* p, size_t n) { FT_CU(cudaMemsetAsync(p, 0, n, st), "waveglow train"); return 0; };
     // rows no kernel writes (guards, padding) stay zero in every fp16 gradient operand: the shifted taps and the
     // row-reduced weight gradients and column sums read them
     if (z0(acts, R * C * 2) || z0(dskip, R * C * 2) || z0(g16, R * C * 2) || z0(dx, R * 2 * C * 2) ||
@@ -1304,28 +1284,23 @@ int ft_waveglow_train_bwd(const FtWaveGlowTrainDesc* d, const FtWaveGlowTrainWei
             // res_skip_layer: rows [0, C) meet G (the residual), the rest d skip
             float* grs = gr->rs_w[k][i];
             if (!last) {
-                if (wt_gemm_wgrad(st, WG_C, WG_C, R, g16, C, acts, C, grs, iS)) return -1;
+                if (gemm_wgrad(st, WG_C, WG_C, R, g16, C, acts, C, grs, WG_C, iS)) return -1;
                 if (launch_colsum(g16, 0, C, R, WG_C, gr->rs_b[k][i], iS, st)) return -1;
             }
             const long long so = last ? 0 : C;
-            if (wt_gemm_wgrad(st, WG_C, WG_C, R, dskip, C, acts, C, grs + so * C, iS)) return -1;
+            if (gemm_wgrad(st, WG_C, WG_C, R, dskip, C, acts, C, grs + so * C, WG_C, iS)) return -1;
             if (launch_colsum(dskip, 0, C, R, WG_C, gr->rs_b[k][i] + so, iS, st)) return -1;
             // in_layer taps (h shifted by -d, 0, +d) and the cond_layer slice
             for (int tap = 0; tap < 3; ++tap)
-                if (wt_gemm_wgrad(st, 2 * WG_C, WG_C, RW, dx + W0 * 2 * C, 2 * C, hin + (W0 + (tap - 1) * dil) * C, C,
-                                  gr->in_w[k][i][tap], iS))
+                if (gemm_wgrad(st, 2 * WG_C, WG_C, RW, dx + W0 * 2 * C, 2 * C, hin + (W0 + (tap - 1) * dil) * C, C,
+                               gr->in_w[k][i][tap], WG_C, iS))
                     return -1;
-            if (wt_gemm_wgrad(st, 2 * WG_C, WG_SPECT, R, dx, 2 * C, spect, WG_SPECT, gr->in_w[k][i][3], iS)) return -1;
+            if (gemm_wgrad(st, 2 * WG_C, WG_SPECT, R, dx, 2 * C, spect, WG_SPECT, gr->in_w[k][i][3], WG_SPECT, iS)) return -1;
             if (launch_colsum(dx, 0, 2 * C, R, 2 * WG_C, gr->in_b[k][i], iS, st)) return -1;
             // d spect += dx cond_w (fp32, unscaled on the way out)
-            {
-                GemmArgs g;
-                g.M = static_cast<int>(R); g.N = WG_SPECT; g.K = 2 * WG_C;
-                g.A = dx; g.lda = 2 * C; g.a_fmt = FMT_F16;
-                g.B = static_cast<const __half*>(w->in_w[k][i]) + 3 * WG_C; g.ldb = 3 * WG_C + WG_SPECT; g.b_fmt = FMT_F16; g.b_mn = 1;
-                g.alpha_ptr = iS; g.beta = 1; g.C32 = dsp32; g.ldc32 = WG_SPECT;
-                if (launch_gemm(g, st)) return -1;
-            }
+            if (gemm_dgrad(st, R, WG_SPECT, 2 * WG_C, dx, 2 * C, static_cast<const __half*>(w->in_w[k][i]) + 3 * WG_C,
+                           3 * WG_C + WG_SPECT, dsp32, WG_SPECT, nullptr, 0, 1, iS))
+                return -1;
             // G += in_w^T dx over the transposed taps: dx shifted by +d, 0, -d (the guard rows keep padding out)
             WgGemmParams q = {};
             q.M = static_cast<int>(R); q.N = WG_C; q.K = 6 * WG_C; q.nseg = 3;
@@ -1348,7 +1323,7 @@ int ft_waveglow_train_bwd(const FtWaveGlowTrainDesc* d, const FtWaveGlowTrainWei
         ft_count_launch(2);
         if (ft_check_launch("wg_train_up_prep")) return -1;
     }
-    if (wt_gemm_wgrad(st, WG_UP_N, 4 * WG_MEL_LD, nfr, dsp16, WG_UP_N, mela, 4 * WG_MEL_LD, gr->up_w, sup + 1)) return -1;
+    if (gemm_wgrad(st, WG_UP_N, 4 * WG_MEL_LD, nfr, dsp16, WG_UP_N, mela, 4 * WG_MEL_LD, gr->up_w, 4 * WG_MEL_LD, sup + 1)) return -1;
     if (launch_colsum(dsp32, 2, WG_UP_N, nfr, WG_UP_N, gr->up_b, nullptr, st)) return -1;
     return 0;
 }

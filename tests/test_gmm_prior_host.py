@@ -2,11 +2,8 @@
 FlowtronLoss(gm_loss=True)): state_dict layout against the reference fixtures, strict loads, CPU-tensor and K > 32 rejections,
 the C ABI of the mel-encoder and mixture-NLL kernels, both encoders' kernels unchanged by sharing their device and host
 code, and the byte layouts of both encoders' saved / scratch buffers."""
-import hashlib
 import os
 import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -14,9 +11,7 @@ import torch
 
 from conftest import GOLDEN, ROOT
 from flowtron_b200 import synth
-
-NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-HAVE_NVCC = os.path.exists(NVCC) or shutil.which("nvcc") is not None
+from kernel_pins import HAVE_NVCC, _assert_kernels_pinned, _compile
 
 
 def _cfg(K=8, fixed=True, mean_scale=3.0, n_flows=2):
@@ -151,45 +146,6 @@ _MEL_ENC_KERNELS = {
     "_ZN2ft20mel_pack_conv_kernelEPKfiiP6__halfS3_": (26, ("0", "0"), "85844aa1e43c1bb0"),
     "_ZN2ft17mel_enc_in_kernelEPKfPKiiP6__half": (32, ("0", "0"), "ce3d8fc79dfcf961"),
 }
-
-
-def _compile(src, tmp_path):
-    obj = str(tmp_path / (src + ".o"))
-    r = subprocess.run([NVCC, "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
-                        "--expt-relaxed-constexpr", "-Xptxas", "-v", "-c", os.path.join(ROOT, "flowtron_b200", "csrc", src),
-                        "-o", obj], capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    regs = {}
-    for part in r.stderr.split("Compiling entry function")[1:]:
-        name = re.match(r"\s*'(\S+)'", part).group(1)
-        spill = re.search(r"(\d+) bytes spill stores, (\d+) bytes spill loads", part).groups()
-        regs[name] = (int(re.search(r"Used (\d+) registers", part).group(1)), spill)
-    return obj, regs
-
-
-def _sass_hashes(obj):
-    cuobjdump = os.path.join(os.path.dirname(NVCC), "cuobjdump") if os.path.exists(NVCC) else shutil.which("cuobjdump")
-    text = subprocess.run([cuobjdump, "-sass", obj], capture_output=True, text=True, check=True).stdout
-    out, cur = {}, None
-    for line in text.splitlines():
-        m = re.match(r"\s*Function : (\S+)", line)
-        if m:
-            cur = m.group(1)
-            out[cur] = []
-        elif cur and line.strip().startswith("/*") and "*/" in line:
-            ins = re.sub(r"/\*[0-9a-f]{4,}\*/", "", line.split("/* 0x")[0]).strip()
-            if ins:
-                out[cur].append(ins)
-    return {k: hashlib.sha256("\n".join(v).encode()).hexdigest()[:16] for k, v in out.items()}
-
-
-def _assert_kernels_pinned(src, table, tmp_path):
-    obj, regs = _compile(src, tmp_path)
-    sass = _sass_hashes(obj)
-    assert set(regs) == set(table) == set(sass)
-    for name, (r, spill, h) in table.items():
-        assert regs[name] == (r, spill), name
-        assert sass[name] == h, name
 
 
 @pytest.mark.skipif(not HAVE_NVCC, reason="nvcc not available")
