@@ -456,17 +456,18 @@ static int launch_wg_tail(const WgTailParams& p, cudaStream_t st) {
 }
 
 // ------------------------------------------------------------------------------------------------ driver
-// Host side of a batch: the bound on its layout (the exact layout for host frame counts; every utterance at F_max when
-// the counts are device data) that sizes grids and scratch, and the host counts for wg_plan_kernel.
-struct WgLayout {
-    int B, Tg_max, mrows, grows;
+// Host side of a batch, for infer and training alike: the flows' channel schedule and the bound on the row layout (the
+// exact layout for host frame counts; every utterance at F_max when the counts are device data) that sizes grids and
+// workspaces, with the host counts for wg_plan_kernel.  Tg_max is the group rows of an utterance in noise / audio (infer:
+// 32 F_max) or in z (training: N / 8, and the rows after it are padding).
+struct WgGrid {
+    int B, F_max, Tg_max, nf, nl, mrows, grows;
+    int c[FT_WG_MAX_FLOWS];      // live channels of flow k (its 1x1 conv is c x c), n_half = c / 2
     WgFrames fr;
-    size_t off_plan, off_mel16, off_uprow, off_rowinfo, off_spect, off_h32, off_h16, off_acts, off_skip, off_state, total;
 };
 
 // d->frames == NULL: the counts arrive in device memory, and the layout is bounded by F_max for every utterance.
-static int wg_layout(const FtWaveGlowDesc* d, WgLayout* L) {
-    if (!d) return ft_set_error("waveglow: null descriptor");
+static int wg_grid(const FtWaveGlowDesc* d, int Tg_max, WgGrid* G) {
     if (d->n_mel != WG_MEL || d->n_group != 8 || d->n_channels != WG_C || d->kernel_size != 3)
         return ft_set_error("waveglow: only n_mel 80, n_group 8, n_channels 256, kernel_size 3 are built");
     if (d->n_flows < 1 || d->n_flows > FT_WG_MAX_FLOWS || d->n_layers < 1 || d->n_layers > FT_WG_MAX_LAYERS)
@@ -476,60 +477,131 @@ static int wg_layout(const FtWaveGlowDesc* d, WgLayout* L) {
     const int n_early = (d->n_flows - 1) / d->n_early_every;
     if (8 - n_early * d->n_early_size < 2) return ft_set_error("waveglow: early outputs leave fewer than 2 channels");
     if (d->B < 1 || d->B > WG_MAX_B) return ft_set_error("waveglow: batch must be 1..128");
-    L->B = d->B;
-    L->Tg_max = 32 * d->F_max;
+    G->B = d->B; G->F_max = d->F_max; G->Tg_max = Tg_max; G->nf = d->n_flows; G->nl = d->n_layers;
+    for (int k = 0, c = 8; k < G->nf; ++k) {
+        if (k > 0 && k % d->n_early_every == 0) c -= d->n_early_size;
+        G->c[k] = c;
+    }
     long long m = 0, g = WG_GUARD;
     for (int b = 0; b < d->B; ++b) {
         const int f = d->frames ? d->frames[b] : d->F_max;
         if (f < 1 || f > d->F_max) return ft_set_error("waveglow: frames[b] must be in 1..F_max");
-        L->fr.f[b] = f;
+        G->fr.f[b] = f;
         m += f + 3;
         g += 32LL * f + WG_GUARD;
         if (g > (1LL << 30)) return ft_set_error("waveglow: batch too long");
     }
-    L->mrows = static_cast<int>(m);
-    L->grows = static_cast<int>(g);
-    Workspace ws;
-    const size_t R = static_cast<size_t>(L->grows);
-    L->off_plan = ws.take(sizeof(WgBatch));
-    L->off_mel16 = ws.take(static_cast<size_t>(L->mrows) * WG_MEL_LD * 2);
-    L->off_uprow = ws.take(static_cast<size_t>(L->mrows) * 4);
-    L->off_rowinfo = ws.take(R * 4);
-    L->off_spect = ws.take(R * WG_SPECT * 2);
-    L->off_h32 = ws.take(R * WG_C * 4);
-    L->off_h16 = ws.take(R * WG_C * 2);
-    L->off_acts = ws.take(R * WG_C * 2);
-    L->off_skip = ws.take(R * WG_C * 4);
-    L->off_state = ws.take(R * 8 * 4);
-    L->total = ws.off;
+    G->mrows = static_cast<int>(m);
+    G->grows = static_cast<int>(g);
     return 0;
 }
 
-// channel bookkeeping of the inverse pass: flow k has c_k live channels, n_half = c_k / 2
-static int wg_channels(const FtWaveGlowDesc* d, int k) {
-    int c = 8;
-    for (int j = 1; j <= k; ++j)
-        if (j % d->n_early_every == 0) c -= d->n_early_size;
-    return c;
+static int wg_infer_grid(const FtWaveGlowDesc* d, WgGrid* G) {
+    return d ? wg_grid(d, 32 * d->F_max, G) : ft_set_error("waveglow: null descriptor");
 }
 
-// The plan (frames_dev: int32 [B] device counts, or null for the layout's host counts), then the prep over it.
-static int launch_wg_plan_prep(const WgLayout& L, const int* frames_dev, int F_max, int Tg_max, WgBatch* plan, const float* mel,
-                               __half* mel16, int* uprow, int* rowinfo, cudaStream_t st) {
+// The prep's outputs, the first regions of the infer scratch and of the training `saved`: the planned layout, the fp16
+// frame grid, the two row maps and the upsampled spectrogram.
+struct WgPrep {
+    WgBatch* batch; __half* mel16; int* uprow; int* rowinfo; __half* spect;
+    void plan(Workspace& ws, const WgGrid& g) {
+        const size_t R = g.grows;
+        batch = ws.get<WgBatch>(1);
+        mel16 = ws.get<__half>(static_cast<size_t>(g.mrows) * WG_MEL_LD);
+        uprow = ws.get<int>(g.mrows);
+        rowinfo = ws.get<int>(R);
+        spect = ws.get<__half>(R * WG_SPECT);
+    }
+};
+
+struct WgInferScratch {
+    WgPrep in;
+    float* h32; __half* h16; __half* acts; float* skip; float* state;
+    void plan(Workspace& ws, const WgGrid& g) {
+        const size_t R = g.grows;
+        in.plan(ws, g);
+        h32 = ws.get<float>(R * WG_C);
+        h16 = ws.get<__half>(R * WG_C);
+        acts = ws.get<__half>(R * WG_C);
+        skip = ws.get<float>(R * WG_C);
+        state = ws.get<float>(R * 8);
+    }
+};
+
+// Plan P of the workspace at `base`; wg_bytes: its size.
+template <typename P> static P wg_carve(const void* base, const WgGrid& g) {
+    Workspace ws;
+    ws.base = static_cast<uint8_t*>(const_cast<void*>(base));
+    P p;
+    p.plan(ws, g);
+    return p;
+}
+template <typename P> static size_t wg_bytes(const WgGrid& g) {
+    Workspace ws;
+    P p;
+    p.plan(ws, g);
+    return ws.off;
+}
+
+// The plan (frames_dev: int32 [B] device counts, or null for the grid's host counts), then the prep over it.
+static int launch_wg_plan_prep(const WgGrid& g, const WgPrep& in, const int* frames_dev, const float* mel, cudaStream_t st) {
     {
-        TimeScope ts("wg_plan", L.B, F_max, frames_dev != nullptr, st);
-        wg_plan_kernel<<<1, WG_PLAN_THREADS, 0, st>>>(L.fr, frames_dev, L.B, F_max, Tg_max, plan);
+        TimeScope ts("wg_plan", g.B, g.F_max, frames_dev != nullptr, st);
+        wg_plan_kernel<<<1, WG_PLAN_THREADS, 0, st>>>(g.fr, frames_dev, g.B, g.F_max, g.Tg_max, in.batch);
         ft_count_launch(1);
         if (ft_check_launch("wg_plan_kernel")) return -1;
     }
-    const long long work = static_cast<long long>(L.mrows) * (WG_MEL_LD + 1) + L.grows;
+    const long long work = static_cast<long long>(g.mrows) * (WG_MEL_LD + 1) + g.grows;
     const int grid = static_cast<int>(std::min<long long>((work + 255) / 256, 4096));
-    TimeScope ts("wg_prep", L.mrows, L.grows, 0, st);
-    wg_prep_kernel<<<grid, 256, 0, st>>>(plan, mel, F_max, mel16, uprow, rowinfo);
+    TimeScope ts("wg_prep", g.mrows, g.grows, 0, st);
+    wg_prep_kernel<<<grid, 256, 0, st>>>(in.batch, mel, g.F_max, in.mel16, in.uprow, in.rowinfo);
     ft_count_launch(1);
     return ft_check_launch("wg_prep_kernel");
 }
 
+// The WN forward GEMMs, shared by infer and the training forward (W: FtWaveGlowWeights or FtWaveGlowTrainWeights).
+// m_live: the plan's live row count, or null to run every row of the bound.
+// Upsample: frame row f = frames f-3..f (A segments shifted 0..-3) -> 32 group rows of 640 channels.
+template <typename W>
+static int wg_upsample(const WgGrid& g, const WgPrep& in, const W* w, const int* m_live, cudaStream_t st) {
+    WgGemmParams p = {};
+    p.M = g.mrows; p.N = WG_UP_N; p.K = 4 * WG_MEL_LD; p.nseg = 4;
+    for (int j = 0; j < 4; ++j) p.seg[j] = WgSeg{in.mel16, g.mrows, WG_MEL_LD, -j, WG_MEL_LD};
+    p.W = static_cast<const __half*>(w->up_w); p.bias = w->up_b; p.rowmap = in.uprow; p.m_live = m_live; p.mode = WG_EPI_UP;
+    p.out16 = in.spect; p.ld16 = WG_SPECT;
+    return launch_wg_gemm(p, st);
+}
+
+// Flow k's WN layers, each a GATE GEMM (in_layer + cond_layer) and a RES GEMM (res_skip_layer).  Layer i reads its fp16
+// input at h16 + i h_step and its RES writes layer i + 1's there (h_step 0: infer's one buffer; training keeps every
+// layer's input).  pre: null, or where GATE stores layer i's pre-activations, at pre + i R 2C.
+template <typename W>
+static int wg_flow_wn(const WgGrid& g, const WgPrep& in, const W* w, int k, __half* h16, long long h_step, __half* pre,
+                      __half* acts, float* h32, float* skip, const int* m_live, cudaStream_t st) {
+    const long long R = g.grows;
+    for (int i = 0; i < g.nl; ++i) {
+        const int dil = 1 << i;
+        const bool last = i == g.nl - 1;
+        __half* hin = h16 + i * h_step;
+        WgGemmParams p = {};
+        p.M = static_cast<int>(R); p.N = 2 * WG_C; p.K = 3 * WG_C + WG_SPECT; p.nseg = 4;
+        p.seg[0] = WgSeg{hin, R, WG_C, -dil, WG_C};
+        p.seg[1] = WgSeg{hin, R, WG_C, 0, WG_C};
+        p.seg[2] = WgSeg{hin, R, WG_C, dil, WG_C};
+        p.seg[3] = WgSeg{in.spect, R, WG_SPECT, 0, WG_SPECT};
+        p.W = static_cast<const __half*>(w->in_w[k][i]); p.bias = w->in_b[k][i]; p.rowmap = in.rowinfo; p.m_live = m_live;
+        p.mode = WG_EPI_GATE; p.out16 = acts; p.ld16 = WG_C; p.pre16 = pre ? pre + i * R * 2 * WG_C : nullptr;
+        if (launch_wg_gemm(p, st)) return -1;
+        WgGemmParams q = {};
+        q.M = static_cast<int>(R); q.N = last ? WG_C : 2 * WG_C; q.K = WG_C; q.nseg = 1;
+        q.seg[0] = WgSeg{acts, R, WG_C, 0, WG_C};
+        q.W = static_cast<const __half*>(w->rs_w[k][i]); q.bias = w->rs_b[k][i]; q.rowmap = in.rowinfo; q.m_live = m_live;
+        q.mode = WG_EPI_RES; q.h32 = h32; q.h16 = last ? hin : hin + h_step; q.skip32 = skip; q.res_cols = last ? 0 : WG_C;
+        q.skip_store = i == 0;
+        if (launch_wg_gemm(q, st)) return -1;
+    }
+    return 0;
+}
 
 // ------------------------------------------------------------------------------------------------ training
 // WaveGlow.forward (glow.py:196-245, the z direction) with its saved activations, and its backward.  See DESIGN.md §4.21.
@@ -537,16 +609,48 @@ static int launch_wg_plan_prep(const WgLayout& L, const int* frames_dev, int F_m
 // pre-activations, and each layer's RES epilogue writes the next layer's fp16 input into its own saved slot.
 constexpr float WG_GRAD_TARGET = 64.f;   // per-flow loss scale: S * max|d skip| ~ 64 (headroom 2^10 below fp16's max)
 
-struct WtLayout {
-    WgLayout g;
-    int Tn, N, F, nf, nl;
-    int c[FT_WG_MAX_FLOWS];                // live channels of flow k (its 1x1 conv is c x c)
-    size_t s_plan, s_mel16, s_uprow, s_rowinfo, s_spect, s_x, s_skip, s_h16, s_pre, saved;
-    size_t c_h32, c_acts, c_state, c_dstate, c_dout, c_dy, c_dskip, c_g16, c_g32, c_dx, c_dsp32, c_dsp16, c_mela, c_zero,
-        c_scale, scratch;
+// forward -> backward
+struct WtSaved {
+    WgPrep in;
+    float* x;          // [nf][R, 8] flow inputs (before the 1x1 conv), fp32
+    float* skip;       // [nf][R, C] WN skip sums, fp32
+    __half* h16;       // [nf][nl][R, C] WN layer inputs, fp16, zero guard rows
+    __half* pre;       // [nf][nl][R, 2C] gate pre-activations, fp16, interleaved like in_w's rows
+    void plan(Workspace& ws, const WgGrid& g) {
+        const size_t R = g.grows, nf = g.nf, nfl = nf * g.nl;
+        in.plan(ws, g);
+        x = ws.get<float>(nf * R * 8);
+        skip = ws.get<float>(nf * R * WG_C);
+        h16 = ws.get<__half>(nfl * R * WG_C);
+        pre = ws.get<__half>(nfl * R * 2 * WG_C);
+    }
 };
 
-static int wt_layout(const FtWaveGlowTrainDesc* d, WtLayout* L) {
+struct WtScratch {
+    float* h32; __half* acts; float* state; float* dstate; float* dout; float* dy; __half* dskip; __half* g16; float* g32;
+    __half* dx; float* dsp32; __half* dsp16; __half* mela; float* zero; float* scale;
+    void plan(Workspace& ws, const WgGrid& g) {
+        const size_t R = g.grows;
+        h32 = ws.get<float>(R * WG_C);
+        acts = ws.get<__half>(R * WG_C);
+        state = ws.get<float>(R * 8);
+        dstate = ws.get<float>(R * 8);
+        dout = ws.get<float>(R * 8);
+        dy = ws.get<float>(R * 8);
+        dskip = ws.get<__half>(R * WG_C);
+        g16 = ws.get<__half>(R * WG_C);
+        g32 = ws.get<float>(R * WG_C);
+        dx = ws.get<__half>(R * 2 * WG_C);
+        dsp32 = ws.get<float>(R * WG_SPECT);
+        dsp16 = ws.get<__half>(R * WG_SPECT);
+        mela = ws.get<__half>(R / 32 * 4 * WG_MEL_LD);
+        zero = ws.get<float>(2 * WG_C);
+        scale = ws.get<float>((static_cast<size_t>(g.nf) + 1) * 4);
+    }
+};
+
+// The infer grid of B utterances of ceil(N / 256) frames each; the rows g >= N / 8 of an utterance are padding (rowinfo -1).
+static int wt_grid(const FtWaveGlowTrainDesc* d, WgGrid* G) {
     if (!d) return ft_set_error("waveglow train: null descriptor");
     if (d->B < 1 || d->B > WG_MAX_B) return ft_set_error("waveglow train: batch must be 1..128");
     if (d->F < 1 || d->N < 8 || d->N % 8 || d->N > 256LL * d->F)
@@ -556,42 +660,7 @@ static int wt_layout(const FtWaveGlowTrainDesc* d, WtLayout* L) {
     for (int b = 0; b < d->B; ++b) frames[b] = fu;
     FtWaveGlowDesc gd = {d->n_mel, d->n_flows, d->n_group, d->n_early_every, d->n_early_size, d->n_layers, d->n_channels,
                          d->kernel_size, d->B, d->F, frames};
-    if (wg_layout(&gd, &L->g)) return -1;
-    L->Tn = d->N / 8; L->N = d->N; L->F = d->F; L->nf = d->n_flows; L->nl = d->n_layers;
-    L->g.Tg_max = L->Tn;                               // rows g >= N / 8 of an utterance are padding (rowinfo -1)
-    for (int k = 0, c = 8; k < L->nf; ++k) {
-        if (k > 0 && k % d->n_early_every == 0) c -= d->n_early_size;
-        L->c[k] = c;
-    }
-    const size_t R = static_cast<size_t>(L->g.grows), nf = L->nf, nfl = nf * L->nl;
-    Workspace sv, sc;
-    L->s_plan = sv.take(sizeof(WgBatch));
-    L->s_mel16 = sv.take(static_cast<size_t>(L->g.mrows) * WG_MEL_LD * 2);
-    L->s_uprow = sv.take(static_cast<size_t>(L->g.mrows) * 4);
-    L->s_rowinfo = sv.take(R * 4);
-    L->s_spect = sv.take(R * WG_SPECT * 2);
-    L->s_x = sv.take(nf * R * 8 * 4);                     // flow inputs (before the 1x1 conv), fp32
-    L->s_skip = sv.take(nf * R * WG_C * 4);               // WN skip sums, fp32
-    L->s_h16 = sv.take(nfl * R * WG_C * 2);               // WN layer inputs, fp16, zero guard rows
-    L->s_pre = sv.take(nfl * R * 2 * WG_C * 2);           // gate pre-activations, fp16, interleaved like in_w's rows
-    L->saved = sv.off;
-    L->c_h32 = sc.take(R * WG_C * 4);
-    L->c_acts = sc.take(R * WG_C * 2);
-    L->c_state = sc.take(R * 8 * 4);
-    L->c_dstate = sc.take(R * 8 * 4);
-    L->c_dout = sc.take(R * 8 * 4);
-    L->c_dy = sc.take(R * 8 * 4);
-    L->c_dskip = sc.take(R * WG_C * 2);
-    L->c_g16 = sc.take(R * WG_C * 2);
-    L->c_g32 = sc.take(R * WG_C * 4);
-    L->c_dx = sc.take(R * 2 * WG_C * 2);
-    L->c_dsp32 = sc.take(R * WG_SPECT * 4);
-    L->c_dsp16 = sc.take(R * WG_SPECT * 2);
-    L->c_mela = sc.take(R / 32 * 4 * WG_MEL_LD * 2);
-    L->c_zero = sc.take(2 * WG_C * 4);
-    L->c_scale = sc.take((nf + 1) * 4 * 4);
-    L->scratch = sc.off;
-    return 0;
+    return wg_grid(&gd, d->N / 8, G);
 }
 
 // One warp per grid row, for the flow boundary of the forward: finish flow `cur` (end conv from the skip sum, affine
@@ -1008,82 +1077,47 @@ static int wt_launch(const void* fn, const WtBwdParams& p, cudaStream_t st, cons
 }
 
 // frames_dev: null for d->frames (host counts), else the device counts (d->frames must then be null).  Every kernel after
-// the plan reads the layout and the live row counts from `plan`; grids and GEMM M come from L, the bound.
+// the plan reads the layout and the live row counts from the planned WgBatch; grids and GEMM M come from G, the bound.
 static int wg_infer(const FtWaveGlowDesc* d, const FtWaveGlowWeights* w, const float* mel, const float* noise, float sigma,
                     const int* frames_dev, float* audio, void* scratch, void* stream) {
-    WgLayout L;
-    if (wg_layout(d, &L)) return -1;
+    WgGrid G;
+    if (wg_infer_grid(d, &G)) return -1;
     if (!w || !mel || !noise || !audio || !scratch) return ft_set_error("waveglow: null pointer argument");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    uint8_t* base = static_cast<uint8_t*>(scratch);
-    WgBatch* plan = reinterpret_cast<WgBatch*>(base + L.off_plan);
-    __half* mel16 = reinterpret_cast<__half*>(base + L.off_mel16);
-    int* uprow = reinterpret_cast<int*>(base + L.off_uprow);
-    int* rowinfo = reinterpret_cast<int*>(base + L.off_rowinfo);
-    __half* spect = reinterpret_cast<__half*>(base + L.off_spect);
-    float* h32 = reinterpret_cast<float*>(base + L.off_h32);
-    __half* h16 = reinterpret_cast<__half*>(base + L.off_h16);
-    __half* acts = reinterpret_cast<__half*>(base + L.off_acts);
-    float* skip = reinterpret_cast<float*>(base + L.off_skip);
-    float* state = reinterpret_cast<float*>(base + L.off_state);
-    const long long R = L.grows;
+    const WgInferScratch s = wg_carve<WgInferScratch>(scratch, G);
+    const int* live = &s.in.batch->grows;
+    const int R = G.grows, nf = G.nf;
 
     // zero hidden-state guard rows (the dilated taps read them) and the audio padding after each utterance
-    FT_CU(cudaMemsetAsync(h16, 0, static_cast<size_t>(R) * WG_C * 2, st), "waveglow");
-    FT_CU(cudaMemsetAsync(audio, 0, sizeof(float) * static_cast<size_t>(L.B) * L.Tg_max * 8, st), "waveglow");
-    if (launch_wg_plan_prep(L, frames_dev, d->F_max, L.Tg_max, plan, mel, mel16, uprow, rowinfo, st)) return -1;
-    {   // upsample: frame row f = frames f-3..f (A segments shifted 0..-3) -> 32 group rows of 640 channels
-        WgGemmParams p = {};
-        p.M = L.mrows; p.N = WG_UP_N; p.K = 4 * WG_MEL_LD; p.nseg = 4;
-        for (int j = 0; j < 4; ++j) p.seg[j] = WgSeg{mel16, L.mrows, WG_MEL_LD, -j, WG_MEL_LD};
-        p.W = static_cast<const __half*>(w->up_w); p.bias = w->up_b; p.rowmap = uprow; p.m_live = &plan->mrows; p.mode = WG_EPI_UP;
-        p.out16 = spect; p.ld16 = WG_SPECT;
-        if (launch_wg_gemm(p, st)) return -1;
-    }
-    const int nf = d->n_flows, nl = d->n_layers;
+    FT_CU(cudaMemsetAsync(s.h16, 0, static_cast<size_t>(R) * WG_C * 2, st), "waveglow");
+    FT_CU(cudaMemsetAsync(audio, 0, sizeof(float) * static_cast<size_t>(G.B) * G.Tg_max * 8, st), "waveglow");
+    if (launch_wg_plan_prep(G, s.in, frames_dev, mel, st)) return -1;
+    if (wg_upsample(G, s.in, w, &s.in.batch->mrows, st)) return -1;
     // head: initial noise on the last flow's live positions and that flow's start conv
     {
-        const int c = wg_channels(d, nf - 1);
+        const int c = G.c[nf - 1];
         WgTailParams t = {};
-        t.R = static_cast<int>(R); t.live_rows = &plan->grows; t.rowinfo = rowinfo; t.state = state;
+        t.R = R; t.live_rows = live; t.rowinfo = s.in.rowinfo; t.state = s.state;
         t.cur = 0; t.o = 8 - c; t.nh = c / 2;
-        t.inj_lo = 8 - c; t.inj_hi = 8; t.noise = noise; t.Tg_max = L.Tg_max; t.sigma = sigma;
+        t.inj_lo = 8 - c; t.inj_hi = 8; t.noise = noise; t.Tg_max = G.Tg_max; t.sigma = sigma;
         t.next = 1; t.o_next = 8 - c; t.nh_next = c / 2; t.start_w = w->start_w[nf - 1]; t.start_b = w->start_b[nf - 1];
-        t.h32 = h32; t.h16 = h16;
+        t.h32 = s.h32; t.h16 = s.h16;
         if (launch_wg_tail(t, st)) return -1;
     }
     for (int k = nf - 1; k >= 0; --k) {
-        for (int i = 0; i < nl; ++i) {
-            const int dil = 1 << i;
-            WgGemmParams p = {};
-            p.M = static_cast<int>(R); p.N = 2 * WG_C; p.K = 3 * WG_C + WG_SPECT; p.nseg = 4;
-            p.seg[0] = WgSeg{h16, R, WG_C, -dil, WG_C};
-            p.seg[1] = WgSeg{h16, R, WG_C, 0, WG_C};
-            p.seg[2] = WgSeg{h16, R, WG_C, dil, WG_C};
-            p.seg[3] = WgSeg{spect, R, WG_SPECT, 0, WG_SPECT};
-            p.W = static_cast<const __half*>(w->in_w[k][i]); p.bias = w->in_b[k][i]; p.rowmap = rowinfo; p.m_live = &plan->grows;
-            p.mode = WG_EPI_GATE; p.out16 = acts; p.ld16 = WG_C;
-            if (launch_wg_gemm(p, st)) return -1;
-            WgGemmParams q = {};
-            const bool last = i == nl - 1;
-            q.M = static_cast<int>(R); q.N = last ? WG_C : 2 * WG_C; q.K = WG_C; q.nseg = 1;
-            q.seg[0] = WgSeg{acts, R, WG_C, 0, WG_C};
-            q.W = static_cast<const __half*>(w->rs_w[k][i]); q.bias = w->rs_b[k][i]; q.rowmap = rowinfo; q.m_live = &plan->grows;
-            q.mode = WG_EPI_RES; q.h32 = h32; q.h16 = h16; q.skip32 = skip; q.res_cols = last ? 0 : WG_C; q.skip_store = i == 0;
-            if (launch_wg_gemm(q, st)) return -1;
-        }
-        const int c = wg_channels(d, k);
+        if (wg_flow_wn(G, s.in, w, k, s.h16, 0, nullptr, s.acts, s.h32, s.skip, live, st)) return -1;
+        const int c = G.c[k];
         WgTailParams t = {};
-        t.R = static_cast<int>(R); t.live_rows = &plan->grows; t.rowinfo = rowinfo; t.state = state;
+        t.R = R; t.live_rows = live; t.rowinfo = s.in.rowinfo; t.state = s.state;
         t.cur = 1; t.o = 8 - c; t.nh = c / 2;
-        t.skip32 = skip; t.end_w = w->end_w[k]; t.end_b = w->end_b[k]; t.inv_w = w->inv_w[k];
+        t.skip32 = s.skip; t.end_w = w->end_w[k]; t.end_b = w->end_b[k]; t.inv_w = w->inv_w[k];
         const bool inject = k > 0 && k % d->n_early_every == 0 && d->n_early_size > 0;
         t.inj_lo = inject ? 8 - c - d->n_early_size : 0; t.inj_hi = inject ? 8 - c : 0;
-        t.noise = noise; t.Tg_max = L.Tg_max; t.sigma = sigma;
+        t.noise = noise; t.Tg_max = G.Tg_max; t.sigma = sigma;
         if (k > 0) {
-            const int cn = wg_channels(d, k - 1);
+            const int cn = G.c[k - 1];
             t.next = 1; t.o_next = 8 - cn; t.nh_next = cn / 2; t.start_w = w->start_w[k - 1]; t.start_b = w->start_b[k - 1];
-            t.h32 = h32; t.h16 = h16;
+            t.h32 = s.h32; t.h16 = s.h16;
         } else {
             t.next = 0; t.audio = audio;
         }
@@ -1097,9 +1131,8 @@ static int wg_infer(const FtWaveGlowDesc* d, const FtWaveGlowWeights* w, const f
 extern "C" {
 
 size_t ft_waveglow_scratch_bytes(const FtWaveGlowDesc* d) {
-    ft::WgLayout L;
-    if (ft::wg_layout(d, &L)) return 0;
-    return L.total;
+    ft::WgGrid G;
+    return ft::wg_infer_grid(d, &G) ? 0 : ft::wg_bytes<ft::WgInferScratch>(G);
 }
 
 int ft_waveglow_infer(const FtWaveGlowDesc* d, const FtWaveGlowWeights* w, const float* mel, const float* noise, float sigma,
@@ -1116,90 +1149,51 @@ int ft_waveglow_infer_dev(const FtWaveGlowDesc* d, const FtWaveGlowWeights* w, c
 }
 
 size_t ft_waveglow_train_saved_bytes(const FtWaveGlowTrainDesc* d) {
-    ft::WtLayout L;
-    return ft::wt_layout(d, &L) ? 0 : L.saved;
+    ft::WgGrid G;
+    return ft::wt_grid(d, &G) ? 0 : ft::wg_bytes<ft::WtSaved>(G);
 }
 
 size_t ft_waveglow_train_scratch_bytes(const FtWaveGlowTrainDesc* d) {
-    ft::WtLayout L;
-    return ft::wt_layout(d, &L) ? 0 : L.scratch;
+    ft::WgGrid G;
+    return ft::wt_grid(d, &G) ? 0 : ft::wg_bytes<ft::WtScratch>(G);
 }
 
 int ft_waveglow_train_fwd(const FtWaveGlowTrainDesc* d, const FtWaveGlowTrainWeights* w, const float* mel, const float* audio,
                           float* z, float* const* log_s, void* saved, void* scratch, void* stream) {
     using namespace ft;
-    WtLayout L;
-    if (wt_layout(d, &L)) return -1;
+    WgGrid G;
+    if (wt_grid(d, &G)) return -1;
     if (!w || !mel || !audio || !z || !log_s || !saved || !scratch) return ft_set_error("waveglow train: null pointer argument");
-    for (int k = 0; k < L.nf; ++k) if (!log_s[k]) return ft_set_error("waveglow train: null log_s pointer");
+    for (int k = 0; k < G.nf; ++k) if (!log_s[k]) return ft_set_error("waveglow train: null log_s pointer");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    uint8_t* sv = static_cast<uint8_t*>(saved);
-    uint8_t* sc = static_cast<uint8_t*>(scratch);
-    const long long R = L.g.grows;
-    __half* mel16 = reinterpret_cast<__half*>(sv + L.s_mel16);
-    int* uprow = reinterpret_cast<int*>(sv + L.s_uprow);
-    int* rowinfo = reinterpret_cast<int*>(sv + L.s_rowinfo);
-    __half* spect = reinterpret_cast<__half*>(sv + L.s_spect);
-    float* xsave = reinterpret_cast<float*>(sv + L.s_x);
-    float* skip = reinterpret_cast<float*>(sv + L.s_skip);
-    __half* h16 = reinterpret_cast<__half*>(sv + L.s_h16);
-    __half* pre = reinterpret_cast<__half*>(sv + L.s_pre);
-    float* h32 = reinterpret_cast<float*>(sc + L.c_h32);
-    __half* acts = reinterpret_cast<__half*>(sc + L.c_acts);
-    float* state = reinterpret_cast<float*>(sc + L.c_state);
-    auto H16 = [&](int k, int i) { return h16 + (static_cast<long long>(k) * L.nl + i) * R * WG_C; };
-    auto PRE = [&](int k, int i) { return pre + (static_cast<long long>(k) * L.nl + i) * R * 2 * WG_C; };
+    const WtSaved s = wg_carve<WtSaved>(saved, G);
+    const WtScratch c = wg_carve<WtScratch>(scratch, G);
+    const long long R = G.grows, flow_h16 = G.nl * R * WG_C;   // one flow's saved layer inputs
 
     // guard and padding rows of every layer input and of the upsampled spectrogram are zero: the dilated taps and the
     // row-reduced weight gradients read them
-    FT_CU(cudaMemsetAsync(h16, 0, static_cast<size_t>(L.nf) * L.nl * R * WG_C * 2, st), "waveglow train");
-    FT_CU(cudaMemsetAsync(spect, 0, static_cast<size_t>(R) * WG_SPECT * 2, st), "waveglow train");
-    if (launch_wg_plan_prep(L.g, nullptr, L.F, L.Tn, reinterpret_cast<WgBatch*>(sv + L.s_plan), mel, mel16, uprow, rowinfo, st))
-        return -1;
-    {
-        WgGemmParams p = {};
-        p.M = L.g.mrows; p.N = WG_UP_N; p.K = 4 * WG_MEL_LD; p.nseg = 4;
-        for (int j = 0; j < 4; ++j) p.seg[j] = WgSeg{mel16, L.g.mrows, WG_MEL_LD, -j, WG_MEL_LD};
-        p.W = static_cast<const __half*>(w->up_w); p.bias = w->up_b; p.rowmap = uprow; p.mode = WG_EPI_UP;
-        p.out16 = spect; p.ld16 = WG_SPECT;
-        if (launch_wg_gemm(p, st)) return -1;
-    }
+    FT_CU(cudaMemsetAsync(s.h16, 0, static_cast<size_t>(G.nf) * flow_h16 * 2, st), "waveglow train");
+    FT_CU(cudaMemsetAsync(s.in.spect, 0, static_cast<size_t>(R) * WG_SPECT * 2, st), "waveglow train");
+    if (launch_wg_plan_prep(G, s.in, nullptr, mel, st)) return -1;
+    if (wg_upsample(G, s.in, w, nullptr, st)) return -1;
     WtTailParams t = {};
-    t.R = static_cast<int>(R); t.Tn = L.Tn; t.N = L.N; t.rowinfo = rowinfo; t.state = state; t.h32 = h32;
+    t.R = static_cast<int>(R); t.Tn = G.Tg_max; t.N = d->N; t.rowinfo = s.in.rowinfo; t.state = c.state; t.h32 = c.h32;
     t.audio = audio; t.cur = -1;
-    for (int k = 0; k <= L.nf; ++k) {
-        if (k < L.nf) {
-            t.next = k; t.o_next = 8 - L.c[k]; t.nh_next = L.c[k] / 2;
-            t.conv_w = w->conv_w[k]; t.x_save = xsave + static_cast<long long>(k) * R * 8;
-            t.start_w = w->start_w[k]; t.start_b = w->start_b[k]; t.h16 = H16(k, 0);
+    for (int k = 0; k <= G.nf; ++k) {
+        if (k < G.nf) {
+            t.next = k; t.o_next = 8 - G.c[k]; t.nh_next = G.c[k] / 2;
+            t.conv_w = w->conv_w[k]; t.x_save = s.x + k * R * 8;
+            t.start_w = w->start_w[k]; t.start_b = w->start_b[k]; t.h16 = s.h16 + k * flow_h16;
         } else {
             t.next = -1; t.z = z;
         }
         if (launch_wt_tail(t, st)) return -1;
-        if (k == L.nf) break;
-        float* skip_k = skip + static_cast<long long>(k) * R * WG_C;
-        for (int i = 0; i < L.nl; ++i) {
-            const int dil = 1 << i;
-            __half* hin = H16(k, i);
-            WgGemmParams p = {};
-            p.M = static_cast<int>(R); p.N = 2 * WG_C; p.K = 3 * WG_C + WG_SPECT; p.nseg = 4;
-            p.seg[0] = WgSeg{hin, R, WG_C, -dil, WG_C};
-            p.seg[1] = WgSeg{hin, R, WG_C, 0, WG_C};
-            p.seg[2] = WgSeg{hin, R, WG_C, dil, WG_C};
-            p.seg[3] = WgSeg{spect, R, WG_SPECT, 0, WG_SPECT};
-            p.W = static_cast<const __half*>(w->in_w[k][i]); p.bias = w->in_b[k][i]; p.rowmap = rowinfo; p.mode = WG_EPI_GATE;
-            p.out16 = acts; p.ld16 = WG_C; p.pre16 = PRE(k, i);
-            if (launch_wg_gemm(p, st)) return -1;
-            WgGemmParams q = {};
-            const bool last = i == L.nl - 1;
-            q.M = static_cast<int>(R); q.N = last ? WG_C : 2 * WG_C; q.K = WG_C; q.nseg = 1;
-            q.seg[0] = WgSeg{acts, R, WG_C, 0, WG_C};
-            q.W = static_cast<const __half*>(w->rs_w[k][i]); q.bias = w->rs_b[k][i]; q.rowmap = rowinfo; q.mode = WG_EPI_RES;
-            q.h32 = h32; q.h16 = last ? hin : H16(k, i + 1); q.skip32 = skip_k; q.res_cols = last ? 0 : WG_C; q.skip_store = i == 0;
-            if (launch_wg_gemm(q, st)) return -1;
-        }
+        if (k == G.nf) break;
+        float* skip_k = s.skip + k * R * WG_C;
+        if (wg_flow_wn(G, s.in, w, k, s.h16 + k * flow_h16, R * WG_C, s.pre + 2 * k * flow_h16, c.acts, c.h32, skip_k, nullptr, st))
+            return -1;
         t.audio = nullptr;
-        t.cur = k; t.o = 8 - L.c[k]; t.nh = L.c[k] / 2;
+        t.cur = k; t.o = 8 - G.c[k]; t.nh = G.c[k] / 2;
         t.skip32 = skip_k; t.end_w = w->end_w[k]; t.end_b = w->end_b[k]; t.log_s = log_s[k];
     }
     return 0;
@@ -1209,122 +1203,103 @@ int ft_waveglow_train_bwd(const FtWaveGlowTrainDesc* d, const FtWaveGlowTrainWei
                           const float* const* d_log_s, const void* saved, const FtWaveGlowTrainGrads* gr, void* scratch,
                           void* stream) {
     using namespace ft;
-    WtLayout L;
-    if (wt_layout(d, &L)) return -1;
+    WgGrid G;
+    if (wt_grid(d, &G)) return -1;
     if (!w || !saved || !gr || !scratch) return ft_set_error("waveglow train: null pointer argument");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const uint8_t* sv = static_cast<const uint8_t*>(saved);
-    uint8_t* sc = static_cast<uint8_t*>(scratch);
-    const long long R = L.g.grows, C = WG_C;
-    const __half* mel16 = reinterpret_cast<const __half*>(sv + L.s_mel16);
-    const int* rowinfo = reinterpret_cast<const int*>(sv + L.s_rowinfo);
-    const __half* spect = reinterpret_cast<const __half*>(sv + L.s_spect);
-    const float* xsave = reinterpret_cast<const float*>(sv + L.s_x);
-    const float* skip = reinterpret_cast<const float*>(sv + L.s_skip);
-    const __half* h16 = reinterpret_cast<const __half*>(sv + L.s_h16);
-    const __half* pre = reinterpret_cast<const __half*>(sv + L.s_pre);
-    __half* acts = reinterpret_cast<__half*>(sc + L.c_acts);
-    float* dstate = reinterpret_cast<float*>(sc + L.c_dstate);
-    float* dout = reinterpret_cast<float*>(sc + L.c_dout);
-    float* dy = reinterpret_cast<float*>(sc + L.c_dy);
-    __half* dskip = reinterpret_cast<__half*>(sc + L.c_dskip);
-    __half* g16 = reinterpret_cast<__half*>(sc + L.c_g16);
-    float* g32 = reinterpret_cast<float*>(sc + L.c_g32);
-    __half* dx = reinterpret_cast<__half*>(sc + L.c_dx);
-    float* dsp32 = reinterpret_cast<float*>(sc + L.c_dsp32);
-    __half* dsp16 = reinterpret_cast<__half*>(sc + L.c_dsp16);
-    __half* mela = reinterpret_cast<__half*>(sc + L.c_mela);
-    float* zero = reinterpret_cast<float*>(sc + L.c_zero);
-    float* scale = reinterpret_cast<float*>(sc + L.c_scale);
+    const WtSaved s = wg_carve<WtSaved>(saved, G);
+    const WtScratch c = wg_carve<WtScratch>(scratch, G);
+    const long long R = G.grows, C = WG_C;
     const long long W0 = WG_GUARD, RW = R - 2 * WG_GUARD;   // row window of the shifted-tap weight gradients
 
     auto z0 = [&](void* p, size_t n) { FT_CU(cudaMemsetAsync(p, 0, n, st), "waveglow train"); return 0; };
     // rows no kernel writes (guards, padding) stay zero in every fp16 gradient operand: the shifted taps and the
     // row-reduced weight gradients and column sums read them
-    if (z0(acts, R * C * 2) || z0(dskip, R * C * 2) || z0(g16, R * C * 2) || z0(dx, R * 2 * C * 2) ||
-        z0(dsp32, R * WG_SPECT * 4) || z0(zero, 2 * C * 4) || z0(scale, (L.nf + 1) * 16))
+    if (z0(c.acts, R * C * 2) || z0(c.dskip, R * C * 2) || z0(c.g16, R * C * 2) || z0(c.dx, R * 2 * C * 2) ||
+        z0(c.dsp32, R * WG_SPECT * 4) || z0(c.zero, 2 * C * 4) || z0(c.scale, (G.nf + 1) * 16))
         return -1;
-    for (int k = 0; k < L.nf; ++k) {
-        const int c = L.c[k], nh = c / 2;
+    for (int k = 0; k < G.nf; ++k) {
+        const int ck = G.c[k], nh = ck / 2;
         if (z0(gr->end_w[k], 2 * nh * C * 4) || z0(gr->end_b[k], 2 * nh * 4) || z0(gr->start_w[k], C * nh * 4) ||
-            z0(gr->start_b[k], C * 4) || z0(gr->conv_w[k], c * c * 4))
+            z0(gr->start_b[k], C * 4) || z0(gr->conv_w[k], ck * ck * 4))
             return -1;
     }
-    for (int k = L.nf - 1; k >= 0; --k) {
-        const int c = L.c[k], nh = c / 2;
+    for (int k = G.nf - 1; k >= 0; --k) {
+        const int ck = G.c[k], nh = ck / 2;
         WtBwdParams b = {};
-        b.R = static_cast<int>(R); b.Tn = L.Tn; b.rowinfo = rowinfo; b.o = 8 - c; b.nh = nh;
-        b.x_save = xsave + static_cast<long long>(k) * R * 8; b.conv_w = w->conv_w[k];
-        b.skip32 = skip + static_cast<long long>(k) * R * C; b.end_w = w->end_w[k]; b.end_b = w->end_b[k]; b.start_w = w->start_w[k];
-        b.dz = k == L.nf - 1 ? d_z : nullptr;
+        b.R = static_cast<int>(R); b.Tn = G.Tg_max; b.rowinfo = s.in.rowinfo; b.o = 8 - ck; b.nh = nh;
+        b.x_save = s.x + k * R * 8; b.conv_w = w->conv_w[k];
+        b.skip32 = s.skip + k * R * C; b.end_w = w->end_w[k]; b.end_b = w->end_b[k]; b.start_w = w->start_w[k];
+        b.dz = k == G.nf - 1 ? d_z : nullptr;
         b.dlog_s = d_log_s ? d_log_s[k] : nullptr;
-        b.dstate = dstate; b.dout = dout; b.dy = dy; b.scale = scale + 4 * k; b.dskip16 = dskip; b.g32 = g32;
+        b.dstate = c.dstate; b.dout = c.dout; b.dy = c.dy; b.scale = c.scale + 4 * k; b.dskip16 = c.dskip; b.g32 = c.g32;
         b.g_end_w = gr->end_w[k]; b.g_end_b = gr->end_b[k]; b.g_start_w = gr->start_w[k]; b.g_start_b = gr->start_b[k];
         b.g_conv_w = gr->conv_w[k];
-        if (k == L.nf - 1 && !d_z && z0(dstate, R * 8 * 4)) return -1;
+        if (k == G.nf - 1 && !d_z && z0(c.dstate, R * 8 * 4)) return -1;
         if (wt_launch(reinterpret_cast<const void*>(wg_train_bwd_out_kernel), b, st, "wg_train_bwd_out")) return -1;
         if (wt_launch(reinterpret_cast<const void*>(wg_train_bwd_skip_kernel), b, st, "wg_train_bwd_skip")) return -1;
-        const float* iS = scale + 4 * k + 1;
-        for (int i = L.nl - 1; i >= 0; --i) {
+        const float* iS = c.scale + 4 * k + 1;
+        for (int i = G.nl - 1; i >= 0; --i) {
             const int dil = 1 << i;
-            const bool last = i == L.nl - 1;
-            const __half* hin = h16 + (static_cast<long long>(k) * L.nl + i) * R * C;
+            const bool last = i == G.nl - 1;
+            const long long layer = static_cast<long long>(k) * G.nl + i;
+            const __half* hin = s.h16 + layer * R * C;
             // d acts = rs_w^T [G; d skip] -> d pre-activations (dx) and the recomputed acts
             WgGemmParams p = {};
             p.M = static_cast<int>(R); p.N = WG_C; p.nseg = last ? 1 : 2; p.K = p.nseg * WG_C;
             if (last) {
-                p.seg[0] = WgSeg{dskip, R, WG_C, 0, WG_C};
+                p.seg[0] = WgSeg{c.dskip, R, WG_C, 0, WG_C};
             } else {
-                p.seg[0] = WgSeg{g16, R, WG_C, 0, WG_C};
-                p.seg[1] = WgSeg{dskip, R, WG_C, 0, WG_C};
+                p.seg[0] = WgSeg{c.g16, R, WG_C, 0, WG_C};
+                p.seg[1] = WgSeg{c.dskip, R, WG_C, 0, WG_C};
             }
-            p.W = static_cast<const __half*>(w->rs_wT[k][i]); p.rowmap = rowinfo; p.mode = WG_EPI_GATE_BWD;
-            p.out16 = dx; p.ld16 = 2 * WG_C; p.h16 = acts; p.pre16 = const_cast<__half*>(pre + (static_cast<long long>(k) * L.nl + i) * R * 2 * C);
+            p.W = static_cast<const __half*>(w->rs_wT[k][i]); p.rowmap = s.in.rowinfo; p.mode = WG_EPI_GATE_BWD;
+            p.out16 = c.dx; p.ld16 = 2 * WG_C; p.h16 = c.acts; p.pre16 = s.pre + layer * R * 2 * C;
             if (launch_wg_gemm(p, st)) return -1;
             // res_skip_layer: rows [0, C) meet G (the residual), the rest d skip
             float* grs = gr->rs_w[k][i];
             if (!last) {
-                if (gemm_wgrad(st, WG_C, WG_C, R, g16, C, acts, C, grs, WG_C, iS)) return -1;
-                if (launch_colsum(g16, 0, C, R, WG_C, gr->rs_b[k][i], iS, st)) return -1;
+                if (gemm_wgrad(st, WG_C, WG_C, R, c.g16, C, c.acts, C, grs, WG_C, iS)) return -1;
+                if (launch_colsum(c.g16, 0, C, R, WG_C, gr->rs_b[k][i], iS, st)) return -1;
             }
             const long long so = last ? 0 : C;
-            if (gemm_wgrad(st, WG_C, WG_C, R, dskip, C, acts, C, grs + so * C, WG_C, iS)) return -1;
-            if (launch_colsum(dskip, 0, C, R, WG_C, gr->rs_b[k][i] + so, iS, st)) return -1;
+            if (gemm_wgrad(st, WG_C, WG_C, R, c.dskip, C, c.acts, C, grs + so * C, WG_C, iS)) return -1;
+            if (launch_colsum(c.dskip, 0, C, R, WG_C, gr->rs_b[k][i] + so, iS, st)) return -1;
             // in_layer taps (h shifted by -d, 0, +d) and the cond_layer slice
             for (int tap = 0; tap < 3; ++tap)
-                if (gemm_wgrad(st, 2 * WG_C, WG_C, RW, dx + W0 * 2 * C, 2 * C, hin + (W0 + (tap - 1) * dil) * C, C,
+                if (gemm_wgrad(st, 2 * WG_C, WG_C, RW, c.dx + W0 * 2 * C, 2 * C, hin + (W0 + (tap - 1) * dil) * C, C,
                                gr->in_w[k][i][tap], WG_C, iS))
                     return -1;
-            if (gemm_wgrad(st, 2 * WG_C, WG_SPECT, R, dx, 2 * C, spect, WG_SPECT, gr->in_w[k][i][3], WG_SPECT, iS)) return -1;
-            if (launch_colsum(dx, 0, 2 * C, R, 2 * WG_C, gr->in_b[k][i], iS, st)) return -1;
+            if (gemm_wgrad(st, 2 * WG_C, WG_SPECT, R, c.dx, 2 * C, s.in.spect, WG_SPECT, gr->in_w[k][i][3], WG_SPECT, iS)) return -1;
+            if (launch_colsum(c.dx, 0, 2 * C, R, 2 * WG_C, gr->in_b[k][i], iS, st)) return -1;
             // d spect += dx cond_w (fp32, unscaled on the way out)
-            if (gemm_dgrad(st, R, WG_SPECT, 2 * WG_C, dx, 2 * C, static_cast<const __half*>(w->in_w[k][i]) + 3 * WG_C,
-                           3 * WG_C + WG_SPECT, dsp32, WG_SPECT, nullptr, 0, 1, iS))
+            if (gemm_dgrad(st, R, WG_SPECT, 2 * WG_C, c.dx, 2 * C, static_cast<const __half*>(w->in_w[k][i]) + 3 * WG_C,
+                           3 * WG_C + WG_SPECT, c.dsp32, WG_SPECT, nullptr, 0, 1, iS))
                 return -1;
             // G += in_w^T dx over the transposed taps: dx shifted by +d, 0, -d (the guard rows keep padding out)
             WgGemmParams q = {};
             q.M = static_cast<int>(R); q.N = WG_C; q.K = 6 * WG_C; q.nseg = 3;
-            for (int tap = 0; tap < 3; ++tap) q.seg[tap] = WgSeg{dx, R, 2 * WG_C, (1 - tap) * dil, 2 * WG_C};
-            q.W = static_cast<const __half*>(w->in_wT[k][i]); q.bias = zero; q.rowmap = rowinfo; q.mode = WG_EPI_RES;
-            q.h32 = g32; q.h16 = g16; q.res_cols = WG_C;
+            for (int tap = 0; tap < 3; ++tap) q.seg[tap] = WgSeg{c.dx, R, 2 * WG_C, (1 - tap) * dil, 2 * WG_C};
+            q.W = static_cast<const __half*>(w->in_wT[k][i]); q.bias = c.zero; q.rowmap = s.in.rowinfo; q.mode = WG_EPI_RES;
+            q.h32 = c.g32; q.h16 = c.g16; q.res_cols = WG_C;
             if (launch_wg_gemm(q, st)) return -1;
         }
         if (wt_launch(reinterpret_cast<const void*>(wg_train_bwd_in_kernel), b, st, "wg_train_bwd_in")) return -1;
     }
     // upsample: d up_w = d spect^T mela over mel frames (32 grid rows each), d up_b = column sums of d spect
-    float* sup = scale + 4 * L.nf;
+    float* sup = c.scale + 4 * G.nf;
     const long long nfr = R / 32, nsp = R * WG_SPECT;
-    if (launch_grad_scale(dsp32, nsp, nullptr, 0, nullptr, 0, WG_GRAD_TARGET, sup, st)) return -1;
+    if (launch_grad_scale(c.dsp32, nsp, nullptr, 0, nullptr, 0, WG_GRAD_TARGET, sup, st)) return -1;
     {
         TimeScope ts("wg_train_up_prep", nfr, 0, 0, st);
-        wg_scale_cast_kernel<<<static_cast<int>(std::min<long long>((nsp + 255) / 256, 4096)), 256, 0, st>>>(dsp32, nsp, sup, dsp16);
+        wg_scale_cast_kernel<<<static_cast<int>(std::min<long long>((nsp + 255) / 256, 4096)), 256, 0, st>>>(c.dsp32, nsp, sup, c.dsp16);
         wg_mela_kernel<<<static_cast<int>(std::min<long long>((nfr * 384 + 255) / 256, 4096)), 256, 0, st>>>(
-            reinterpret_cast<const WgBatch*>(sv + L.s_plan), rowinfo, mel16, static_cast<int>(nfr), mela);
+            s.in.batch, s.in.rowinfo, s.in.mel16, static_cast<int>(nfr), c.mela);
         ft_count_launch(2);
         if (ft_check_launch("wg_train_up_prep")) return -1;
     }
-    if (gemm_wgrad(st, WG_UP_N, 4 * WG_MEL_LD, nfr, dsp16, WG_UP_N, mela, 4 * WG_MEL_LD, gr->up_w, 4 * WG_MEL_LD, sup + 1)) return -1;
-    if (launch_colsum(dsp32, 2, WG_UP_N, nfr, WG_UP_N, gr->up_b, nullptr, st)) return -1;
+    if (gemm_wgrad(st, WG_UP_N, 4 * WG_MEL_LD, nfr, c.dsp16, WG_UP_N, c.mela, 4 * WG_MEL_LD, gr->up_w, 4 * WG_MEL_LD, sup + 1)) return -1;
+    if (launch_colsum(c.dsp32, 2, WG_UP_N, nfr, WG_UP_N, gr->up_b, nullptr, st)) return -1;
     return 0;
 }
 

@@ -18,6 +18,7 @@ import torch.nn.functional as F
 
 from . import _lib
 from ._lib import FlowtronB200Error
+from .synth import waveglow_channels
 
 
 class Invertible1x1Conv(torch.nn.Module):
@@ -92,73 +93,80 @@ class WaveGlowLoss(torch.nn.Module):
         return loss / (z.size(0) * z.size(1) * z.size(2))
 
 
+_FP16_FIELDS = ("up_w", "in_w", "rs_w")     # the GEMM operands; every other packed field is fp32
+
+
+def _set_field(struct, key, value):
+    """struct.name[k][i]... = value for key (name, k, i, ...)."""
+    name, *idx = key
+    if not idx:
+        setattr(struct, name, value)
+        return
+    arr = getattr(struct, name)
+    for j in idx[:-1]:
+        arr = arr[j]
+    arr[idx[-1]] = value
+
+
+def _train_kernel_weights(packed):
+    """The tensors ft_waveglow_train_fwd / _bwd read, by FtWaveGlowTrainWeights field: the packed weights in fp16 (GEMM
+    operands) or fp32, plus the backward's transposed fp16 copies in_wT (the three dilated taps of in_w) and rs_wT."""
+    out = {}
+    for key, t in packed.items():
+        t = t.detach()
+        out[key] = t.to(torch.float16 if key[0] in _FP16_FIELDS else torch.float32).contiguous()
+        if key[0] == "in_w":
+            taps = t[:, :768].reshape(512, 3, 256).permute(2, 1, 0).reshape(256, 1536)
+            out[("in_wT",) + key[1:]] = taps.to(torch.float16).contiguous()
+        elif key[0] == "rs_w":
+            out[("rs_wT",) + key[1:]] = t.t().to(torch.float16).contiguous()
+    return out
+
+
 class _WaveGlowTrainFn(torch.autograd.Function):
-    """ft_waveglow_train_fwd / ft_waveglow_train_bwd on the fp32 packed weights: the kernels read fp16 copies (and the
-    backward's transposed ones), made here on the device; the gradients come back for the fp32 packed tensors."""
+    """ft_waveglow_train_fwd / ft_waveglow_train_bwd on the fp32 packed weights (keys: their FtWaveGlowTrainWeights
+    fields, as WaveGlow._layout names them): the kernels read fp16 copies (and the backward's transposed ones), made here
+    on the device; the gradients come back for the fp32 packed tensors."""
 
     @staticmethod
-    def forward(ctx, cfg, spect, audio, *packed):
+    def forward(ctx, cfg, keys, spect, audio, *packed):
         n_flows, n_early_every, n_early_size, L, B, Fr, N = cfg
         Tn = N // 8
         desc = _lib.FtWaveGlowTrainDesc(n_mel=80, n_flows=n_flows, n_group=8, n_early_every=n_early_every,
                                         n_early_size=n_early_size, n_layers=L, n_channels=256, kernel_size=3, B=B, F=Fr, N=N)
+        kernel = _train_kernel_weights(dict(zip(keys, packed)))
         w = _lib.FtWaveGlowTrainWeights()
-        keep = []
-
-        def dp(t, dtype=torch.float32):
-            t = t.detach().to(dtype).contiguous()
-            keep.append(t)
-            return t.data_ptr()
-
-        w.up_w, w.up_b = dp(packed[0], torch.float16), dp(packed[1])
-        chans, j = [], 2
-        for k in range(n_flows):
-            w.conv_w[k], w.start_w[k], w.start_b[k], w.end_w[k], w.end_b[k] = [dp(t) for t in packed[j:j + 5]]
-            chans.append(packed[j].shape[0])
-            j += 5
-            for i in range(L):
-                in_w, in_b, rs_w, rs_b = packed[j:j + 4]
-                j += 4
-                w.in_w[k][i], w.in_b[k][i] = dp(in_w, torch.float16), dp(in_b)
-                w.rs_w[k][i], w.rs_b[k][i] = dp(rs_w, torch.float16), dp(rs_b)
-                w.in_wT[k][i] = dp(in_w.detach()[:, :768].reshape(512, 3, 256).permute(2, 1, 0).reshape(256, 1536), torch.float16)
-                w.rs_wT[k][i] = dp(rs_w.detach().t(), torch.float16)
+        for key, t in kernel.items():
+            _set_field(w, key, t.data_ptr())
         dev = spect.device
         z = torch.empty(B, 8, Tn, device=dev)
-        log_s = [torch.empty(B, c // 2, Tn, device=dev) for c in chans]
+        log_s = [torch.empty(B, t.shape[0] // 2, Tn, device=dev) for key, t in zip(keys, packed) if key[0] == "conv_w"]
         saved = torch.empty(_lib.waveglow_train_saved_bytes(desc), dtype=torch.uint8, device=dev)
         _lib.waveglow_train_fwd(desc, w, spect, audio, z, log_s, saved)
-        ctx.state = (desc, w, keep, saved, [(t.shape, t.dtype) for t in packed], chans, L)
+        ctx.state = (desc, w, kernel, saved, keys, [t.shape for t in packed])
         ctx.set_materialize_grads(False)
         return (z, *log_s)
 
     @staticmethod
     def backward(ctx, d_z, *d_log_s):
-        desc, w, keep, saved, shapes, chans, L = ctx.state
+        desc, w, _kernel, saved, keys, shapes = ctx.state
         dev = saved.device
-        # in_w gradients come back per tap (split-K needs each output contiguous) and are concatenated afterwards
-        in_w_at = {2 + 5 * (k + 1) + 4 * (k * L + i) for k in range(len(chans)) for i in range(L)}
-        grads = [None if j in in_w_at else torch.empty(s, dtype=torch.float32, device=dev) for j, (s, _) in enumerate(shapes)]
         g = _lib.FtWaveGlowTrainGrads()
-        g.up_w, g.up_b = grads[0].data_ptr(), grads[1].data_ptr()
-        taps, j = [], 2
-        for k in range(len(chans)):
-            g.conv_w[k], g.start_w[k], g.start_b[k], g.end_w[k], g.end_b[k] = [t.data_ptr() for t in grads[j:j + 5]]
-            j += 5
-            for i in range(L):
+        grads = []
+        for key, shape in zip(keys, shapes):
+            if key[0] == "in_w":        # per tap (split-K needs each output contiguous), concatenated afterwards
                 parts = [torch.empty(512, 256, device=dev) for _ in range(3)] + [torch.empty(512, 640, device=dev)]
-                for t in range(4):
-                    g.in_w[k][i][t] = parts[t].data_ptr()
-                taps.append((j, parts))
-                g.in_b[k][i], g.rs_w[k][i], g.rs_b[k][i] = [t.data_ptr() for t in grads[j + 1:j + 4]]
-                j += 4
+                for t, part in enumerate(parts):
+                    _set_field(g, key + (t,), part.data_ptr())
+                grads.append(parts)
+            else:
+                grads.append(torch.empty(shape, dtype=torch.float32, device=dev))
+                _set_field(g, key, grads[-1].data_ptr())
         dz = None if d_z is None else d_z.float().contiguous()
         dls = [None if t is None else t.float().contiguous() for t in d_log_s]
         _lib.waveglow_train_bwd(desc, w, dz, dls, saved, g)
-        for j, parts in taps:
-            grads[j] = torch.cat(parts, 1)
         ctx.state = None
-        return (None, None, None, *grads)
+        return (None, None, None, None, *[torch.cat(t, 1) if isinstance(t, list) else t for t in grads])
 
 
 class WaveGlow(torch.nn.Module):
@@ -179,19 +187,14 @@ class WaveGlow(torch.nn.Module):
         self.WN_config = dict(WN_config)
         self.WN = torch.nn.ModuleList()
         self.convinv = torch.nn.ModuleList()
-        n_half = n_group // 2
-        c = n_group
-        self.channels = []                                      # (n_remaining_channels, n_half) per flow
-        for k in range(n_flows):
-            if k % n_early_every == 0 and k > 0:
-                n_half -= n_early_size // 2
-                c -= n_early_size
-            if c < 2:
-                raise NotImplementedError("early outputs leave fewer than 2 channels")
+        self.channels = waveglow_channels(dict(n_group=n_group, n_flows=n_flows, n_early_every=n_early_every,
+                                               n_early_size=n_early_size))      # (n_remaining_channels, n_half) per flow
+        if self.channels[-1][0] < 2:
+            raise NotImplementedError("early outputs leave fewer than 2 channels")
+        for c, n_half in self.channels:
             self.convinv.append(Invertible1x1Conv(c))
             self.WN.append(WN(n_half, n_mel_channels * n_group, **WN_config))
-            self.channels.append((c, n_half))
-        self.n_remaining_channels = c
+        self.n_remaining_channels = self.channels[-1][0]
         self._packed = None
         self._packed_key = None
 
@@ -219,34 +222,47 @@ class WaveGlow(torch.nn.Module):
             raise WaveGlowNoCpuPath("WaveGlow.forward needs the module, spect and audio on CUDA: the sm_90a kernels are the "
                                     "only implementation")
         cfg = (self.n_flows, self.n_early_every, self.n_early_size, self.WN_config["n_layers"], B, Fr, N)
-        outs = _WaveGlowTrainFn.apply(cfg, spect.float().contiguous(), audio.float().contiguous(), *self._train_params())
+        packed = self._train_params()
+        outs = _WaveGlowTrainFn.apply(cfg, tuple(packed), spect.float().contiguous(), audio.float().contiguous(),
+                                      *packed.values())
         Tn = N // self.n_group
         log_det_W_list = [B * Tn * torch.logdet(inv.conv.weight.squeeze(-1)) for inv in self.convinv]
         return outs[0], list(outs[1:]), log_det_W_list
 
-    def _train_params(self):
-        """The kernels' packed weights in fp32, built from the parameters with differentiable device ops, in the order
-        _WaveGlowTrainFn takes them: up_w, up_b, then per flow conv_w, start_w, start_b, end_w, end_b and per layer in_w,
-        in_b, rs_w, rs_b (the layouts of FtWaveGlowWeights)."""
+    def _layout(self, fold):
+        """The kernels' packed weights in fp32, keyed by FtWaveGlowTrainWeights field: (name,), (name, flow) or (name, flow,
+        layer), in the order up_w, up_b, then per flow conv_w, start_w, start_b, end_w, end_b and per layer in_w, in_b,
+        rs_w, rs_b.  fold(conv) is a conv's effective weight (its weight-norm fold).  up_w is the ConvTranspose1d as one GEMM
+        over frames f-3..f; in_w = [tap0 | tap1 | tap2 | cond_layer slice] and in_b = in_layer + cond bias have their rows
+        interleaved (2c: tanh input of channel c, 2c+1: its sigmoid input)."""
         M, L, C = self.n_mel_channels, self.WN_config["n_layers"], self.WN_config["n_channels"]
-        up = self.upsample.weight.view(M, M, 4, 32, 8).permute(3, 1, 4, 2, 0)               # [g, c, jj, j, ci]
-        out = [F.pad(up, (0, 96 - M)).reshape(32 * M * 8, 4 * 96),
-               self.upsample.bias.view(1, M, 1).expand(32, M, 8).reshape(-1)]
-        dev = self.upsample.weight.device
-        inter = torch.stack([torch.arange(C, device=dev), torch.arange(C, device=dev) + C], 1).reshape(-1)
+
+        def gate_rows(x):
+            return x.reshape(2, C, -1).transpose(0, 1).reshape(x.shape)
+
+        # upsample: W[ci, c, t + 256 j] -> up_w[g*640 + c*8 + jj, j*96 + ci], t = 8 g + jj
+        up = self.upsample.weight.float().view(M, M, 4, 32, 8).permute(3, 1, 4, 2, 0)      # [g, c, jj, j, ci]
+        out = {("up_w",): F.pad(up, (0, 96 - M)).reshape(32 * M * 8, 4 * 96),
+               ("up_b",): self.upsample.bias.float().view(1, M, 1).expand(32, M, 8).reshape(-1)}
         for k, wn in enumerate(self.WN):
-            cond_w = _effective_weight(wn.cond_layer)[:, :, 0]
-            cond_b = wn.cond_layer.bias
-            out += [self.convinv[k].conv.weight[:, :, 0], _effective_weight(wn.start)[:, :, 0], wn.start.bias,
-                    wn.end.weight[:, :, 0], wn.end.bias]
+            cond_w, cond_b = fold(wn.cond_layer)[:, :, 0], wn.cond_layer.bias.float()
+            out[("conv_w", k)] = self.convinv[k].conv.weight.float()[:, :, 0]
+            out[("start_w", k)] = fold(wn.start)[:, :, 0]
+            out[("start_b", k)] = wn.start.bias.float()
+            out[("end_w", k)] = wn.end.weight.float()[:, :, 0]
+            out[("end_b", k)] = wn.end.bias.float()
             for i in range(L):
-                wi = _effective_weight(wn.in_layers[i])
-                sl = slice(2 * C * i, 2 * C * (i + 1))
-                out.append(torch.cat([wi[:, :, 0], wi[:, :, 1], wi[:, :, 2], cond_w[sl]], 1)[inter])
-                out.append((wn.in_layers[i].bias + cond_b[sl])[inter])
-                out.append(_effective_weight(wn.res_skip_layers[i])[:, :, 0])
-                out.append(wn.res_skip_layers[i].bias)
+                wi, sl = fold(wn.in_layers[i]), slice(2 * C * i, 2 * C * (i + 1))
+                out[("in_w", k, i)] = gate_rows(torch.cat([wi[:, :, 0], wi[:, :, 1], wi[:, :, 2], cond_w[sl]], 1))
+                out[("in_b", k, i)] = gate_rows(wn.in_layers[i].bias.float() + cond_b[sl])
+                out[("rs_w", k, i)] = fold(wn.res_skip_layers[i])[:, :, 0]
+                out[("rs_b", k, i)] = wn.res_skip_layers[i].bias.float()
         return out
+
+    def _train_params(self):
+        """_layout with the differentiable device fold: the packed weights _WaveGlowTrainFn takes, through which torch
+        autograd reaches the parameters."""
+        return self._layout(_effective_weight)
 
     @staticmethod
     def remove_weightnorm(model):
@@ -268,39 +284,18 @@ class WaveGlow(torch.nn.Module):
         if self._packed is not None and self._packed_key == key:
             return self._packed
         dev = self.upsample.weight.device
-        M, L, C = self.n_mel_channels, self.WN_config["n_layers"], self.WN_config["n_channels"]
+        w = _lib.FtWaveGlowWeights()
         keep = []
 
-        def dev_t(t, dtype):
-            t = t.to(device=dev, dtype=dtype).contiguous()
-            keep.append(t)
-            return t.data_ptr()
+        def put(field, t, dtype):
+            keep.append(t.to(device=dev, dtype=dtype).contiguous())
+            _set_field(w, field, keep[-1].data_ptr())
 
-        w = _lib.FtWaveGlowWeights()
-        # upsample: W[ci, c, t + 256 j] -> up_w[g*640 + c*8 + jj, j*96 + ci], t = 8 g + jj
-        W = self.upsample.weight.detach().float().view(M, M, 4, 32, 8)            # [ci, c, j, g, jj]
-        up = W.permute(3, 1, 4, 2, 0)                                                # [g, c, jj, j, ci]
-        up = F.pad(up, (0, 96 - M)).reshape(32 * M * 8, 4 * 96)
-        w.up_w = dev_t(up, torch.float16)
-        w.up_b = dev_t(self.upsample.bias.detach().float().view(1, M, 1).expand(32, M, 8).reshape(-1), torch.float32)
-        inter = torch.stack([torch.arange(C), torch.arange(C) + C], 1).reshape(-1)   # row 2c: tanh c, 2c+1: sigmoid c
-        for k, wn in enumerate(self.WN):
-            cond_w = _weight(wn.cond_layer)[:, :, 0]
-            cond_b = wn.cond_layer.bias.detach().float()
-            for i in range(L):
-                wi = _weight(wn.in_layers[i])                                         # [2C, C, 3]
-                sl = slice(2 * C * i, 2 * C * (i + 1))
-                full = torch.cat([wi[:, :, 0], wi[:, :, 1], wi[:, :, 2], cond_w[sl]], 1)
-                w.in_w[k][i] = dev_t(full[inter], torch.float16)
-                w.in_b[k][i] = dev_t((wn.in_layers[i].bias.detach().float() + cond_b[sl])[inter], torch.float32)
-                w.rs_w[k][i] = dev_t(_weight(wn.res_skip_layers[i])[:, :, 0], torch.float16)
-                w.rs_b[k][i] = dev_t(wn.res_skip_layers[i].bias.detach().float(), torch.float32)
-            w.start_w[k] = dev_t(_weight(wn.start)[:, :, 0], torch.float32)
-            w.start_b[k] = dev_t(wn.start.bias.detach().float(), torch.float32)
-            w.end_w[k] = dev_t(wn.end.weight.detach().float()[:, :, 0], torch.float32)
-            w.end_b[k] = dev_t(wn.end.bias.detach().float(), torch.float32)
-            inv = torch.linalg.inv(self.convinv[k].conv.weight.detach().double().squeeze(-1).cpu())
-            w.inv_w[k] = dev_t(inv.float(), torch.float32)
+        for field, t in self._layout(_weight).items():
+            if field[0] != "conv_w":
+                put(field, t, torch.float16 if field[0] in _FP16_FIELDS else torch.float32)
+        for k, inv in enumerate(self.convinv):
+            put(("inv_w", k), torch.linalg.inv(inv.conv.weight.detach().double().squeeze(-1).cpu()).float(), torch.float32)
         self._packed = (w, keep)
         self._packed_key = key
         return self._packed
@@ -371,7 +366,6 @@ def waveglow_flops(frames: int, cfg) -> float:
     (last res_skip) + 2 n_half C (start) + 2 C 2 n_half (end), 32 group rows per frame, plus the upsample 2 * 320 * 20480
     per frame."""
     C, L = cfg["WN_config"]["n_channels"], cfg["WN_config"]["n_layers"]
-    from .synth import waveglow_channels
     per_group = 0.0
     for c, nh in waveglow_channels(cfg):
         per_group += 2 * (3 * C + 640) * 2 * C * L + 2 * C * 2 * C * (L - 1) + 2 * C * C + 2 * nh * C + 2 * C * 2 * nh

@@ -1,5 +1,5 @@
 """GPU: WaveGlow.forward / WaveGlowLoss and the backward (csrc/waveglow.cu, training section) against torch.autograd of the
-fp64 oracle (tests/waveglow_train_oracle.py) on the same fp32 weights: forward outputs, invertibility through infer, every
+fp64 oracle (tests/waveglow_oracle.py) on the same fp32 weights: forward outputs, invertibility through infer, every
 parameter gradient one upstream gradient at a time in both weight forms, the reference initialisation, a short Adam run
 and a CUDA-graph-captured step.
 
@@ -7,7 +7,7 @@ Bars are about 3x the worst value measured on an NVIDIA H100 80GB HBM3 (700 W po
 import pytest
 import torch
 
-import waveglow_train_oracle as O
+import waveglow_oracle as O
 from flowtron_b200 import synth
 
 pytestmark = pytest.mark.gpu

@@ -1,4 +1,4 @@
-"""CPU: the differentiable WaveGlow oracle (tests/waveglow_train_oracle.py) pinned against the reference-generated training
+"""CPU: the differentiable WaveGlow oracle (tests/waveglow_oracle.py) pinned against the reference-generated training
 fixture (tests/make_golden_waveglow_train.py), WaveGlowLoss, and the argument checks of WaveGlow.forward."""
 import os
 
@@ -6,7 +6,7 @@ import numpy as np
 import pytest
 import torch
 
-import waveglow_train_oracle as O
+import waveglow_oracle as O
 from conftest import GOLDEN
 from flowtron_b200 import synth
 from make_golden_waveglow_train import REDUCED_CONFIG, inputs

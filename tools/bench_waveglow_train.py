@@ -7,7 +7,7 @@ events), audio samples/s, and model FLOP/s over step time with the FLOP count co
 tensor work x 3 for forward + backward).  Variants:
   kernels_graph   this library, the whole step replayed from one CUDA graph
   kernels_eager   this library, eager
-  torch_fp32      the fp32 oracle module (tests/waveglow_train_oracle.py) in plain torch on the same GPU
+  torch_fp32      the fp32 oracle module (tests/waveglow_oracle.py) in plain torch on the same GPU
   torch_autocast  the same under torch.autocast(float16)
 The card name and power limit are read in the same run.  Needs a GPU; there is no CPU path.
 """
@@ -27,7 +27,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 from flowtron_b200 import synth  # noqa: E402
 from flowtron_b200.waveglow import WaveGlow, WaveGlowLoss  # noqa: E402
-import waveglow_train_oracle as O  # noqa: E402
+import waveglow_oracle as O  # noqa: E402
 
 
 def card():
