@@ -315,6 +315,10 @@ def _declare(L):
     L.ft_gmm_nll_rows.restype = c_int
     L.ft_gmm_nll_grad.argtypes = [POINTER(FtGmmDesc)] + [c_void_p] * 11
     L.ft_gmm_nll_grad.restype = c_int
+    L.ft_gmm_sample.argtypes = [POINTER(FtGmmDesc)] + [c_void_p] * 5 + [c_float, c_void_p, c_void_p, c_void_p]
+    L.ft_gmm_sample.restype = c_int
+    L.ft_gmm_responsibilities.argtypes = [POINTER(FtGmmDesc)] + [c_void_p] * 8
+    L.ft_gmm_responsibilities.restype = c_int
     for fn in ("ft_attention_saved_bytes", "ft_attention_scratch_bytes"):
         getattr(L, fn).argtypes = [POINTER(FtAttentionDesc)]
         getattr(L, fn).restype = c_size_t
@@ -820,6 +824,26 @@ def gmm_nll_grad(z, out_lens_i32, mean, log_var, prob, per_row, g_nll, dz, dmean
     scratch = torch.empty(lib().ft_gmm_nll_scratch_bytes(byref(desc)), dtype=torch.uint8, device=z.device)
     check(lib().ft_gmm_nll_grad(byref(desc), ptr(z), ptr(out_lens_i32), ptr(mean), ptr(log_var), ptr(prob), ptr(g_nll), ptr(dz),
                                 ptr(dmean), ptr(dlog_var), ptr(dprob), ptr(scratch), stream_ptr()), "ft_gmm_nll_grad")
+
+
+def gmm_sample(mean, log_var, prob, per_row, n_frames_i32, component_i32, sigma, rng_state, z):
+    """ft_gmm_sample: z [B, M, T] (written) from mean / log_var [B or 1, M, K], prob [B, K]; component_i32 [B] or None;
+    rng_state int64 [2] = {seed, counter}, its counter advanced on the device.  Two launches, no allocation."""
+    _need_cuda(mean, log_var, prob, n_frames_i32, component_i32, rng_state, z)
+    B, M, T = z.shape
+    desc = FtGmmDesc(T=T, B=B, M=M, K=prob.size(1), per_row=int(per_row))
+    check(lib().ft_gmm_sample(byref(desc), ptr(mean), ptr(log_var), ptr(prob), ptr(n_frames_i32), ptr(component_i32),
+                              float(sigma), ptr(rng_state), ptr(z), stream_ptr()), "ft_gmm_sample")
+
+
+def gmm_responsibilities(z, out_lens_i32, mean, log_var, prob, per_row, resp):
+    """ft_gmm_responsibilities: resp [B, K] (written) for z [T, B, M]."""
+    _need_cuda(z, out_lens_i32, mean, log_var, prob, resp)
+    T, B, M = z.shape
+    desc = FtGmmDesc(T=T, B=B, M=M, K=prob.size(1), per_row=int(per_row))
+    scratch = torch.empty(lib().ft_gmm_nll_scratch_bytes(byref(desc)), dtype=torch.uint8, device=z.device)
+    check(lib().ft_gmm_responsibilities(byref(desc), ptr(z), ptr(out_lens_i32), ptr(mean), ptr(log_var), ptr(prob),
+                                        ptr(resp), ptr(scratch), stream_ptr()), "ft_gmm_responsibilities")
 
 
 # ------------------------------------------------------------------------------------------------ WaveGlow

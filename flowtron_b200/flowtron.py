@@ -924,25 +924,63 @@ class Flowtron(nn.Module):
         in_lens must lie in [1, L] and host ``lens`` in [1, min(T, lens_hi)]; CUDA lengths are trusted and not read, so
         the call makes no host synchronisation.  ``check(B, T, L)`` makes the entry point's own ValueError checks.  Every
         ValueError comes before the CUDA check of x, text, speaker_ids and ``cuda``, and all of it before any allocation or
-        launch."""
-        if x.dim() != 3 or text.dim() != 2 or speaker_ids.dim() != 1:
-            raise ValueError(f"{where} expects {x_name} [B, n_mel, T], speaker_ids [B] and text [B, L]")
+        launch.  An entry point that takes no text passes speaker_ids, text and in_lens as None and gets L and in_lens
+        back as None."""
+        has_text = text is not None
+        if x.dim() != 3 or (has_text and (text.dim() != 2 or speaker_ids.dim() != 1)):
+            raise ValueError(f"{where} expects {x_name} [B, n_mel, T]" + (", speaker_ids [B] and text [B, L]" if has_text else ""))
         B, _, T = x.shape
-        L = text.size(1)
-        _lib.check_text_len(L, where)
-        if text.size(0) != B or speaker_ids.size(0) != B or B < 1 or T < 1 or L < 1:
-            raise ValueError(f"{where}: batch sizes disagree or are empty: {x_name} {tuple(x.shape)}, "
-                             f"speaker_ids {tuple(speaker_ids.shape)}, text {tuple(text.shape)}")
+        L = text.size(1) if has_text else None
+        if has_text:
+            _lib.check_text_len(L, where)
+        if B < 1 or T < 1 or (has_text and (text.size(0) != B or speaker_ids.size(0) != B or L < 1)):
+            raise ValueError(f"{where}: batch sizes disagree or are empty: {x_name} {tuple(x.shape)}" +
+                             (f", speaker_ids {tuple(speaker_ids.shape)}, text {tuple(text.shape)}" if has_text else ""))
         if check is not None:
             check(B, T, L)
-        in_lens = _lib.ragged_lengths(in_lens, B, L, "in_lens")
+        if has_text:
+            in_lens = _lib.ragged_lengths(in_lens, B, L, "in_lens")
         if lens is not None:
             lens = _lib.ragged_lengths(lens, B, T if lens_hi is None else min(T, lens_hi), lens_name)
-        if not all(t.is_cuda for t in (x, text, speaker_ids, *cuda)):
+        if not all(t.is_cuda for t in (x, *((text, speaker_ids) if has_text else ()), *cuda)):
             raise FlowtronB200Error(f"{where} needs CUDA tensors: the sm_90a kernels are the only implementation")
         dev = x.device
-        return (B, T, L, in_lens.to(device=dev, dtype=torch.int32),
+        return (B, T, L, in_lens.to(device=dev, dtype=torch.int32) if has_text else None,
                 None if lens is None else lens.to(device=dev, dtype=torch.int32))
+
+    def mixture(self, mel, out_lens):
+        """Per-utterance Gaussian-mixture parameters of a padded batch of reference mels, for ``style.sample_mixture``.
+
+        mel [B, 80, T] f32, out_lens [B] -> (mean, log_var, prob) as ``GaussianMixture.forward`` returns them: mean /
+        log_var [B, 80, K] with learned Gaussians, the fixed [1, 80, K] buffers otherwise, prob [B, K].  Row b is the
+        MelEncoder + GaussianMixture of ``mel[b:b+1, :, :out_lens[b]]`` alone, in eval semantics (no dropout) whatever
+        ``self.training`` is, and without autograd state.  ``forward`` instead divides every row's time sum by the batch's
+        longest length (the reference's mean over the padded output); here the MelEncoder kernels run once on the batch
+        and each row's embedding is rescaled by max(out_lens) / out_lens[b], so it is its own time mean.  That rescaling
+        rounds twice more than the B = 1 call's single division: a row's embedding lies within 4 ulps of its B = 1 call's,
+        and its mixture parameters agree with that call to 1e-5 of their largest magnitude.
+
+        Arguments are checked as the other padded-batch entry points check them (ValueError for shapes and host lengths
+        outside [1, T], FlowtronB200Error for CPU tensors); CUDA out_lens are trusted, and the call then makes no host
+        synchronisation, so it can be captured in a CUDA graph.  A model without the mixture prior raises ValueError."""
+        where = "Flowtron.mixture"
+        if not hasattr(self, 'gaussian_mixture'):
+            raise ValueError(f"{where}: the model has no Gaussian-mixture prior (n_components <= 1)")
+
+        def check(B, T, L):
+            if mel.size(1) != 80:
+                raise ValueError(f"{where}: mel must be [B, 80, T], got {tuple(mel.shape)}")
+        B, _, _, _, lens = self._batch_args(where, mel, "mel", None, None, None, out_lens, "out_lens", check=check)
+        with torch.no_grad():
+            was = self.mel_encoder.training
+            self.mel_encoder.train(False)
+            try:
+                emb = self.mel_encoder(mel, lens)
+            finally:
+                self.mel_encoder.train(was)
+            n = lens.float()
+            emb = emb * (n.max() / n)[:, None]
+            return self.gaussian_mixture(emb, B)
 
     def _encode_args(self, mel, speaker_ids, text, in_lens, out_lens, attn_prior, where, cuda=()):
         """encode's argument checks (``cuda``: more tensors that must be on the device) -> (in_lens, out_lens int32 on the

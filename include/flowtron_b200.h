@@ -446,6 +446,22 @@ int ft_gmm_nll_grad(const FtGmmDesc* d, const float* z, const int* out_lens, con
                     const float* prob, const float* g_nll, float* dz, float* dmean, float* dlog_var, float* dprob, void* scratch,
                     void* stream);
 
+/* Sampling from the mixture (csrc/gmm_sample.cu).  d->T is z's padded frame count; mean / log_var / prob as above.
+ * z [B, M, T] fp32, overwritten: for t < min(n_frames[b], T) element (c, t) takes component k -- component[b] when that lies
+ * in [0, K), otherwise drawn from prob[b] (non-negative weights with a positive sum; they need not be normalised) -- and is
+ * mean[b|0, c, k] + sigma exp(log_var[b|0, c, k] / 2) eps with eps ~ N(0, 1); every other element is 0.  component may be
+ * NULL (draw every element).  rng_state: device uint64 {seed, counter}.  The draws of element (b, c, t) depend only on
+ * (seed, counter, b, c, t); a one-thread launch behind the sampler adds 1 to the counter, so each call (and each replay of a
+ * captured graph) draws new values.  Two launches, no allocation, no host synchronisation. */
+int ft_gmm_sample(const FtGmmDesc* d, const float* mean, const float* log_var, const float* prob, const int* n_frames,
+                  const int* component, float sigma, unsigned long long* rng_state, float* z, void* stream);
+/* Component responsibilities: resp [B, K] fp32, resp[b, k] = mean over t < out_lens[b] (clamped to T) and all M channels of
+ * prob_k N_k(z) / sum_j prob_j N_j(z), in log space with the NLL's max shift.  z [T, B, M] as ft_gmm_nll_reduce reads it;
+ * scratch: ft_gmm_nll_scratch_bytes(d) bytes.  Each row is summed from its own partials in a fixed order with no atomics, so
+ * it equals the row's B = 1 call bit for bit. */
+int ft_gmm_responsibilities(const FtGmmDesc* d, const float* z, const int* out_lens, const float* mean, const float* log_var,
+                            const float* prob, float* resp, void* scratch, void* stream);
+
 /* ------------------------------------------------------------------------------------------------------
  * WaveGlow vocoder, inference direction (tacotron2/waveglow/glow.py:251-293 WaveGlow.infer): log-mel -> audio.
  * Built for n_mel 80, n_group 8, WN n_channels 256, kernel_size 3; n_flows <= 16, n_layers <= 8.
