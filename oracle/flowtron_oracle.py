@@ -87,12 +87,12 @@ def _zero_after_len(h: Tensor, out_lens: Optional[Tensor]) -> Tensor:
 
 
 # --------------------------------------------------------------------------- attention
-def attention_forward(p: Params, pre: str, queries: Tensor, text: Tensor, mask: Optional[Tensor],
+def attention_forward(p: Params, pre: str, queries: Tensor, keys: Tensor, mask: Optional[Tensor],
                       attn_prior: Optional[Tensor], temperature: float = 1.0,
-                      attn: Optional[Tensor] = None):
+                      attn: Optional[Tensor] = None, values: Optional[Tensor] = None):
     """flowtron.py:559-592 (+ compute_attention_posterior :544-557).
 
-    queries [T,B,H], text [L,B,E], mask [B,L,1] bool (True = pad).
+    queries [T,B,H], keys / values [L,B,E] (values None: the keys, as in AR_Step), mask [B,L,1] bool (True = pad).
     Returns ctx [B,A,T], attn [B,T,L], attn_logprob [B,T,L] (or None if attn was given).
     Computes in the inputs' dtype: fp32 or fp64 only (in fp16 the 1e-20 log offset would flush to zero).
     """
@@ -100,9 +100,9 @@ def attention_forward(p: Params, pre: str, queries: Tensor, text: Tensor, mask: 
     Wk = p[f"{pre}.key.linear_layer.weight"]
     Wv = p[f"{pre}.value.linear_layer.weight"]
     wv = p[f"{pre}.v.linear_layer.weight"]
-    values = (text @ Wv.t()).transpose(0, 1)                     # [B,L,A]
+    values = ((keys if values is None else values) @ Wv.t()).transpose(0, 1)   # [B,L,A]
     if attn is None:
-        keys = (text @ Wk.t()).transpose(0, 1)                   # [B,L,A]
+        keys = (keys @ Wk.t()).transpose(0, 1)                   # [B,L,A]
         q = (queries @ Wq.t()).transpose(0, 1)                   # [B,T,A]
         e = torch.tanh(q[:, :, None] + keys[:, None]) @ wv.t()   # [B,T,L,1]   :572
         e = e[..., 0] / temperature                              # :573
@@ -267,41 +267,61 @@ def _masked_instance_norm(x: Tensor, mask: Optional[Tensor], w: Tensor, b: Tenso
     return out * w[None, :, None] + b[None, :, None]
 
 
-def encoder_forward(p: Params, x: Tensor, in_lens: Optional[Tensor], infer: bool = False) -> Tensor:
-    """Encoder.forward / .infer in eval mode (no dropout), flowtron.py:492-525.
-    x [B,C,L] -> [B,L,C].  ``in_lens`` sorted descending as DataCollate provides."""
-    B = x.shape[0]
-    mask = None
-    if not infer and B > 1:
-        mask = get_mask_from_lengths(in_lens, x.shape[2]).unsqueeze(1)
-    for i in range(3):
+def _conv_norm_bilstm(p: Params, pre: str, n_convs: int, x: Tensor, lens: Optional[Tensor], masked: bool) -> Tensor:
+    """The body Encoder (flowtron.py:492-525) and MelEncoder (:425-439) share, in eval mode (no dropout): ``n_convs``
+    blocks of conv (odd width, 'same' padding) -> instance norm -> relu, then a BiLSTM run over each row's own length.
+
+    x [B,C,T] -> [B,T,2H], zero at t >= lens[b] (lens None: every row is T long).  ``masked``: padded frames are zeroed
+    before each conv and left out of the norm's statistics, as the reference does for B > 1."""
+    mask = get_mask_from_lengths(lens, x.shape[2]).unsqueeze(1) if masked else None
+    for i in range(n_convs):
         if mask is not None:
             x = x.masked_fill(~mask, 0.0)
-        x = F.conv1d(x, p[f"encoder.convolutions.{i}.0.conv.weight"],
-                     p[f"encoder.convolutions.{i}.0.conv.bias"], padding=2)
+        w = p[f"{pre}.convolutions.{i}.0.conv.weight"]
+        x = F.conv1d(x, w, p[f"{pre}.convolutions.{i}.0.conv.bias"], padding=w.shape[2] // 2)
         # Encoder.infer iterates the Sequential(ConvNorm, norm) blocks, so the (unmasked) instance
         # norm is applied there too (flowtron.py:517-518); forward with B == 1 also has mask=None.
         x = F.relu(_masked_instance_norm(x, mask.to(x.dtype) if mask is not None else None,
-                                         p[f"encoder.convolutions.{i}.1.weight"],
-                                         p[f"encoder.convolutions.{i}.1.bias"]))
-    x = x.transpose(1, 2)                        # [B,L,C]
-    Hh = p["encoder.lstm.weight_hh_l0"].shape[1]
-    L = x.shape[1]
+                                         p[f"{pre}.convolutions.{i}.1.weight"],
+                                         p[f"{pre}.convolutions.{i}.1.bias"]))
+    x = x.transpose(1, 2)                        # [B,T,C]
+    T = x.shape[1]
     outs = []
-    for b in range(B):                           # packed BiLSTM: each row runs over its own length
-        n = L if (infer or in_lens is None) else int(in_lens[b])
+    for b in range(x.shape[0]):                  # packed BiLSTM: each row runs over its own length
+        n = T if lens is None else int(lens[b])
         xb = x[b, :n][:, None]                   # [n,1,C]
-        fwd = lstm_layer_explicit(xb, p["encoder.lstm.weight_ih_l0"], p["encoder.lstm.weight_hh_l0"],
-                                  p["encoder.lstm.bias_ih_l0"], p["encoder.lstm.bias_hh_l0"])
-        bwd = lstm_layer_explicit(torch.flip(xb, (0,)), p["encoder.lstm.weight_ih_l0_reverse"],
-                                  p["encoder.lstm.weight_hh_l0_reverse"],
-                                  p["encoder.lstm.bias_ih_l0_reverse"], p["encoder.lstm.bias_hh_l0_reverse"])
-        o = torch.cat([fwd, torch.flip(bwd, (0,))], -1)[:, 0]              # [n,2Hh]
-        outs.append(F.pad(o, (0, 0, 0, L - n)))
-    out = torch.stack(outs, 0)
-    if not infer and in_lens is not None:
-        out = out[:, : int(in_lens.max())]
-    return out
+        fwd = _lstm(xb, p, f"{pre}.lstm", 0, False)
+        bwd = _lstm(torch.flip(xb, (0,)), p, f"{pre}.lstm", "0_reverse", False)
+        o = torch.cat([fwd, torch.flip(bwd, (0,))], -1)[:, 0]              # [n,2H]
+        outs.append(F.pad(o, (0, 0, 0, T - n)))
+    return torch.stack(outs, 0)
+
+
+def encoder_forward(p: Params, x: Tensor, in_lens: Optional[Tensor], infer: bool = False) -> Tensor:
+    """Encoder.forward / .infer in eval mode (no dropout), flowtron.py:492-525.
+    x [B,C,L] -> [B,L,C].  ``in_lens`` sorted descending as DataCollate provides."""
+    lens = None if infer else in_lens
+    out = _conv_norm_bilstm(p, "encoder", 3, x, lens, masked=not infer and x.shape[0] > 1)
+    return out if lens is None else out[:, : int(lens.max())]
+
+
+def mel_encoder_forward(p: Params, mel: Tensor, lens: Tensor) -> Tensor:
+    """MelEncoder.forward in eval mode, flowtron.py:425-439: mel [B,80,T] -> [B,512].  Masked for B > 1; the time mean
+    is over the padded length max(lens) that pad_packed_sequence gives, so a row depends on the batch it comes in."""
+    h = _conv_norm_bilstm(p, "mel_encoder", 2, mel, lens, masked=mel.shape[0] > 1)
+    return h[:, : int(lens.max())].mean(1)
+
+
+def gaussian_mixture(p: Params, emb: Tensor, n_components: int, fixed_gaussian: bool):
+    """GaussianMixture.forward, flowtron.py:351-362: emb [B,512] -> (mean, log_var, prob [B,K]); mean and log_var are
+    [B,80,K], or the fixed [1,80,K] buffers."""
+    lin = lambda name: (emb @ p[f"gaussian_mixture.{name}.linear_layer.weight"].t()
+                        + p[f"gaussian_mixture.{name}.linear_layer.bias"])
+    prob = torch.softmax(lin("prob_layer"), dim=1)
+    if fixed_gaussian:
+        return p["gaussian_mixture.mean"], p["gaussian_mixture.log_var"], prob
+    B = emb.shape[0]
+    return lin("mean_layer").view(B, -1, n_components), lin("log_var_layer").view(B, -1, n_components), prob
 
 
 # --------------------------------------------------------------------------- model
@@ -316,7 +336,12 @@ def flow_prefix(i: int) -> str:
 def flowtron_forward(p: Params, mel: Tensor, speaker_ids: Tensor, text: Tensor, in_lens: Tensor,
                      out_lens: Tensor, attn_prior: Optional[Tensor] = None, fast: bool = False,
                      encoder_outputs: Optional[Tensor] = None):
-    """Flowtron.forward, flowtron.py:870-899 (n_components=0 branch, eval-mode encoder)."""
+    """Flowtron.forward, flowtron.py:870-899 (eval-mode encoders).  The mixture's (mean, log_var, prob) when ``p`` holds a
+    Gaussian-mixture prior, else None x 3."""
+    mean = log_var = prob = None
+    if "gaussian_mixture.prob_layer.linear_layer.weight" in p:                  # :879-882
+        K = p["gaussian_mixture.prob_layer.linear_layer.weight"].shape[0]
+        mean, log_var, prob = gaussian_mixture(p, mel_encoder_forward(p, mel, out_lens), K, "gaussian_mixture.mean" in p)
     if encoder_outputs is None:
         spk = F.embedding(speaker_ids, p["speaker_embedding.weight"])
         t = F.embedding(text, p["embedding.weight"]).transpose(1, 2)
@@ -332,7 +357,7 @@ def flowtron_forward(p: Params, mel: Tensor, speaker_ids: Tensor, text: Tensor, 
         log_s_list.append(log_s)
         attns.append(a)
         lps.append(lp)
-    return mel, log_s_list, gate, attns, lps, None, None, None
+    return mel, log_s_list, gate, attns, lps, mean, log_var, prob
 
 
 def flowtron_infer(p: Params, residual: Tensor, speaker_ids: Tensor, text: Tensor,
@@ -358,15 +383,33 @@ def flowtron_infer(p: Params, residual: Tensor, speaker_ids: Tensor, text: Tenso
     return residual.permute(1, 2, 0), attn_all
 
 
+def mixture_log_terms(z: Tensor, mean: Tensor, log_var: Tensor, prob: Tensor) -> Tensor:
+    """log(prob_k N(z; mean_k, exp(log_var_k))) + log(2 pi) / 2 per component (the constant the reference drops).
+    z [T,B,M]; mean / log_var [B,M,K] or shared [1,M,K]; prob [B,K] -> [T,B,M,K], in the inputs' dtype."""
+    return (torch.log(prob)[None, :, None] - 0.5 * log_var[None]
+            - (z[..., None] - mean[None]) ** 2 / (2 * torch.exp(log_var[None])))
+
+
+def mixture_log_density(z: Tensor, mean: Tensor, log_var: Tensor, prob: Tensor) -> Tensor:
+    """The per-element term of FlowtronLoss's gm_loss branch (flowtron.py:217-231), the log-sum-exp of
+    ``mixture_log_terms`` over the components: [T,B,M], differentiable."""
+    return torch.logsumexp(mixture_log_terms(z, mean, log_var, prob), dim=3)
+
+
 def flowtron_loss(model_output, gate_target: Tensor, in_lens: Tensor, out_lens: Tensor,
-                  sigma: float = 1.0, gate_loss: bool = True):
-    """FlowtronLoss.forward default branch (no GMM, no CTC), flowtron.py:200-243 (Appendix A.5)."""
+                  sigma: float = 1.0, gate_loss: bool = True, gm_loss: bool = False):
+    """FlowtronLoss.forward without CTC, flowtron.py:200-243 (Appendix A.5); ``gm_loss``: the Gaussian-mixture branch
+    on model_output's (mean, log_var, prob)."""
     z, log_s_list, gate_pred = model_output[0], model_output[1], model_output[2]
     mask = get_mask_from_lengths(out_lens, z.shape[0]).transpose(0, 1)[..., None].float()
     n = mask.sum()
     log_s_total = sum(torch.sum(ls * mask) for ls in log_s_list)
-    zm = z * mask
-    nll = (torch.sum(zm * zm) / (2 * sigma * sigma) - log_s_total) / (n * z.size(2))
+    if gm_loss:
+        nll = -torch.sum(mask * mixture_log_density(z, *model_output[5:8]))
+    else:
+        zm = z * mask
+        nll = torch.sum(zm * zm) / (2 * sigma * sigma)
+    nll = (nll - log_s_total) / (n * z.size(2))
     gl = torch.zeros(1)
     if gate_loss and gate_pred is not None:
         gp = (gate_pred * mask)[..., 0].permute(1, 0)

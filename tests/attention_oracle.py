@@ -1,5 +1,5 @@
-"""fp64-capable restatement of the reference Attention module (flowtron.py:528-592) with keys and values as separate inputs,
-and the seeded cases of tests/golden/attention_*.npz (make_golden_attention.py) that the CPU and GPU tests share.
+"""The seeded cases of tests/golden/attention_*.npz (make_golden_attention.py) that the CPU and GPU tests of the standalone
+Attention module share; the module itself is restated by oracle.flowtron_oracle.attention_forward.
 
 Inputs and weights are regenerated from each case's seed with torch's CPU generator; the fixtures carry their sums so a test
 knows it runs on exactly what the reference ran on."""
@@ -35,33 +35,6 @@ CASES = {
     "ar_l700":             dict(dims="ar_step", B=1, T=1, L=700, lens=[523], prior=False, temp=1.0, given=False, kv=False, seed=24),
     "ar_l1024":            dict(dims="ar_step", B=1, T=1, L=1024, lens=None, prior=False, temp=1.0, given=False, kv=True, seed=25),
 }
-
-
-def attention(W: dict, queries: Tensor, keys: Tensor, values: Tensor, mask: Optional[Tensor] = None, attn: Optional[Tensor] = None,
-              attn_prior: Optional[Tensor] = None, temperature: float = 1.0):
-    """flowtron.py:559-592 in the inputs' dtype.  W: the module's state_dict (query / key / value / v .linear_layer.weight).
-    queries [T, B, Dq], keys / values [L, B, E], mask [B, L, 1] bool (True = pad) -> (output [B, A, T], attn [B, T, L],
-    attn_logprob [B, T, L] or None)."""
-    w = {k: W[f"{k}.linear_layer.weight"] for k in PRE}
-    v = (values @ w["value"].t()).transpose(0, 1)                               # [B, L, A]
-    if attn is None:
-        k = (keys @ w["key"].t()).transpose(0, 1)
-        q = (queries @ w["query"].t()).transpose(0, 1)                          # [B, T, A]
-        e = (torch.tanh(q[:, :, None] + k[:, None]) @ w["v"].t())[..., 0] / temperature
-        if mask is not None:
-            e = e.masked_fill(mask.transpose(1, 2), -float("inf"))
-        a = torch.softmax(e, dim=2)
-        if attn_prior is not None:
-            lp = torch.log(a + 1e-20) + torch.log(attn_prior.to(a.dtype) + 1e-20)
-            logprob = lp.clone()
-            if mask is not None:
-                lp = lp.masked_fill(mask.transpose(1, 2), -float("inf"))
-            a = torch.softmax(lp, dim=2)
-        else:
-            logprob = torch.log(a + 1e-8)
-    else:
-        a, logprob = attn, None
-    return torch.bmm(a, v).transpose(1, 2), a, logprob
 
 
 def case_lens(c: dict) -> Optional[Tensor]:

@@ -1,11 +1,12 @@
-"""fp64 restatement of the Gaussian-mixture synthesis path: Flowtron.mixture (MelEncoder + GaussianMixture per utterance),
-the mixture sampler of csrc/gmm_sample.cu (its counter hash, component choice and Box-Muller draw) and the component
-responsibilities.  numpy / torch on the CPU only."""
+"""fp64 restatement of the Gaussian-mixture synthesis path: Flowtron.mixture (the oracle's MelEncoder + GaussianMixture per
+utterance), the mixture sampler of csrc/gmm_sample.cu (its counter hash, component choice and Box-Muller draw) and the
+component responsibilities.  numpy / torch on the CPU only."""
 from __future__ import annotations
 
 import numpy as np
 import torch
-import torch.nn.functional as Fn
+
+from oracle import flowtron_oracle as FO
 
 _GOLDEN_GAMMA = np.uint64(0x9E3779B97F4A7C15)
 _IDX_MUL = np.uint64(0xD1B54A32D192ED03)
@@ -63,53 +64,24 @@ def sample(mean, log_var, prob, n_frames, T, sigma, seed, counter, component=Non
 
 def responsibilities(z, out_lens, mean, log_var, prob):
     """z [B, M, T] -> (r [B, K], lse [B]): r[b, k] = the mean over t < out_lens[b] and all channels of the posterior
-    prob_k N_k / sum_j prob_j N_j; lse[b] = sum over the same elements of log sum_k prob_k exp(-(z - mean_k)^2 /
-    (2 exp log_var_k)) / exp(log_var_k / 2), the term whose negative FlowtronLoss(gm_loss=True) sums."""
-    z, mean, log_var, prob = (np.asarray(t, dtype=np.float64) for t in (z, mean, log_var, prob))
-    B, M, T = z.shape
-    K = prob.shape[1]
-    r, lse = np.zeros((B, K)), np.zeros(B)
-    for b in range(B):
-        n = min(int(out_lens[b]), T)
-        mb, lb = mean[b if mean.shape[0] > 1 else 0], log_var[b if log_var.shape[0] > 1 else 0]
-        a = np.log(prob[b])[None, None, :] - 0.5 * lb[:, None, :] - (z[b, :, :n, None] - mb[:, None, :]) ** 2 / (
-            2.0 * np.exp(lb[:, None, :]))                                               # [M, n, K]
-        mx = a.max(-1, keepdims=True)
-        l = mx[..., 0] + np.log(np.exp(a - mx).sum(-1))
-        r[b] = np.exp(a - l[..., None]).mean((0, 1))
-        lse[b] = l.sum()
-    return r, lse
-
-
-def _mel_encoder_one(p, mel):
-    """MelEncoder on one utterance [80, n] (flowtron.py:425-439 at B = 1: no mask, the time mean over its own n frames)."""
-    x = mel.double()[None]
-    for i in range(2):
-        y = Fn.conv1d(x, p[f"convolutions.{i}.0.conv.weight"], p[f"convolutions.{i}.0.conv.bias"], padding=1)
-        mu = y.mean(2, keepdim=True)
-        var = ((y - mu) ** 2).mean(2, keepdim=True)
-        y = (y - mu) / torch.sqrt(var + 1e-5) * p[f"convolutions.{i}.1.weight"][None, :, None] + p[f"convolutions.{i}.1.bias"][None, :, None]
-        x = torch.relu(y)
-    lstm = torch.nn.LSTM(512, 256, 1, bidirectional=True).double()
-    lstm.load_state_dict({k[len("lstm."):]: v for k, v in p.items() if k.startswith("lstm.")})
-    h, _ = lstm(x.permute(2, 0, 1))
-    return h.mean(0)[0]
+    prob_k N_k / sum_j prob_j N_j; lse[b] = the sum over the same elements of the oracle's mixture log-density, the term
+    whose negative FlowtronLoss(gm_loss=True) sums."""
+    z, mean, log_var, prob = (torch.as_tensor(np.asarray(t, dtype=np.float64)) for t in (z, mean, log_var, prob))
+    z = z.permute(2, 0, 1)                                                              # [T, B, M], the flows' layout
+    valid = FO.get_mask_from_lengths(torch.as_tensor(np.asarray(out_lens)), z.shape[0]).t()[..., None]   # [T, B, 1]
+    post = torch.softmax(FO.mixture_log_terms(z, mean, log_var, prob), dim=3)                  # [T, B, M, K]
+    r = torch.where(valid[..., None], post, 0.0).sum((0, 2)) / (valid.sum((0, 2)) * z.shape[2])[:, None]
+    lse = torch.where(valid, FO.mixture_log_density(z, mean, log_var, prob), 0.0).sum((0, 2))
+    return r.numpy(), lse.numpy()
 
 
 def mixture(params, mel, out_lens, n_components, fixed_gaussian):
-    """Flowtron.mixture restated: row b is MelEncoder + GaussianMixture on mel[b, :, :out_lens[b]] alone ->
-    (emb [B, 512], mean, log_var, prob) float64; mean / log_var [B, 80, K], or the fixed [1, 80, K] buffers."""
-    p = {k[len("mel_encoder."):]: v.double() for k, v in params.items() if k.startswith("mel_encoder.")}
-    g = {k[len("gaussian_mixture."):]: v.double() for k, v in params.items() if k.startswith("gaussian_mixture.")}
-    mel = torch.as_tensor(mel)
+    """Flowtron.mixture restated: row b is the oracle's MelEncoder on mel[b, :, :out_lens[b]] alone, then its
+    GaussianMixture -> (emb [B, 512], mean, log_var, prob) float64; mean / log_var [B, 80, K], or the fixed [1, 80, K]
+    buffers."""
+    p = {k: v.double() for k, v in params.items() if k.startswith(("mel_encoder.", "gaussian_mixture."))}
+    mel = torch.as_tensor(mel).double()
     with torch.no_grad():
-        emb = torch.stack([_mel_encoder_one(p, mel[b, :, :int(n)]) for b, n in enumerate(out_lens)])
-        B = emb.size(0)
-        lin = lambda name: emb @ g[f"{name}.linear_layer.weight"].t() + g[f"{name}.linear_layer.bias"]
-        prob = torch.softmax(lin("prob_layer"), dim=1)
-        if fixed_gaussian:
-            mean, log_var = g["mean"], g["log_var"]
-        else:
-            mean = lin("mean_layer").view(B, 80, n_components)
-            log_var = lin("log_var_layer").view(B, 80, n_components)
-    return emb, mean, log_var, prob
+        emb = torch.cat([FO.mel_encoder_forward(p, mel[b:b + 1, :, :int(n)], torch.tensor([int(n)]))
+                         for b, n in enumerate(out_lens)])
+        return (emb, *FO.gaussian_mixture(p, emb, n_components, fixed_gaussian))

@@ -12,7 +12,6 @@ from __future__ import annotations
 
 import os
 import sys
-import zlib
 
 import numpy as np
 import torch
@@ -21,14 +20,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from oracle import ref_shims  # noqa: E402
 from flowtron_b200 import synth  # noqa: E402
+from golden_fixtures import grad_sample_index  # noqa: E402
 
 OUT = os.path.join(ROOT, "tests", "golden")
-N_GRAD_SAMPLES = 32
-
-
-def grad_sample_index(name: str, numel: int) -> np.ndarray:
-    g = torch.Generator().manual_seed(zlib.crc32(name.encode()))
-    return torch.randint(0, numel, (N_GRAD_SAMPLES,), generator=g).numpy()
 
 
 def train_case(tag, n_flows, B, T, L, out_lens, with_prior, seed, in_lens=None, logmel_stats=False, store_attn=True,

@@ -1,6 +1,6 @@
-"""CPU checks of the standalone Attention module: the fp64 restatement in tests/attention_oracle.py against the reference's
-fixtures and against finite differences, the argument checks that run before any device work, and the state_dict round trip
-with the reference module."""
+"""CPU checks of the standalone Attention module: the oracle's fp64 restatement (attention_forward, which the flow step uses
+too) against the reference's fixtures and against finite differences, the argument checks that run before any device work,
+and the state_dict round trip with the reference module."""
 from __future__ import annotations
 
 import os
@@ -29,9 +29,9 @@ def test_oracle_matches_reference_fixture(name):
     x = AO.case_inputs(c)
     for k, v in AO.input_sums(x).items():          # the regenerated inputs are the ones the reference ran on
         assert float(ref[k]) == pytest.approx(v, rel=1e-12, abs=1e-9), k
-    W = {k: v.double() for k, v in x["W"].items()}
-    out, attn, lp = AO.attention(W, _f64(x["queries"]), _f64(x["keys"]), _f64(x["values"]), x["mask"], _f64(x["attn"]),
-                                 _f64(x["prior"]), c["temp"])
+    W = {f"att.{k}": v.double() for k, v in x["W"].items()}
+    out, attn, lp = O.attention_forward(W, "att", _f64(x["queries"]), _f64(x["keys"]), x["mask"], _f64(x["prior"]), c["temp"],
+                                        attn=_f64(x["attn"]), values=_f64(x["values"]))
     got = {"output": out, "attn": attn}
     if lp is not None:
         got["attn_logprob"] = lp
@@ -44,22 +44,11 @@ def test_oracle_matches_reference_fixture(name):
         assert (torch.from_numpy(ref["attn"])[x["mask"][..., 0][:, None, :].expand(-1, c["T"], -1)] == 0).all()
 
 
-def test_oracle_matches_flow_oracle_when_keys_are_values():
-    c = AO.CASES["default_prior"]
-    x = AO.case_inputs(c)
-    p = {f"att.{k}": v.double() for k, v in x["W"].items()}
-    a = AO.attention({k[4:]: v for k, v in p.items()}, _f64(x["queries"]), _f64(x["keys"]), _f64(x["keys"]), x["mask"], None,
-                     _f64(x["prior"]), 1.3)
-    b = O.attention_forward(p, "att", _f64(x["queries"]), _f64(x["keys"]), x["mask"], _f64(x["prior"]), 1.3)
-    for u, w in zip(a, b):
-        assert torch.equal(u, w)
-
-
 @pytest.mark.parametrize("prior,given", [(False, False), (True, False), (False, True)])
 def test_oracle_gradient_matches_finite_differences(prior, given):
     g = torch.Generator().manual_seed(5)
     T, B, L, Dq, E, A = 3, 2, 5, 4, 6, 8
-    W = {f"{k}.linear_layer.weight": (0.5 * torch.randn(o, i, generator=g, dtype=torch.float64)).requires_grad_()
+    W = {f"att.{k}.linear_layer.weight": (0.5 * torch.randn(o, i, generator=g, dtype=torch.float64)).requires_grad_()
          for k, (o, i) in zip(AO.PRE, ((A, Dq), (A, E), (A, E), (1, A)))}
     q = torch.randn(T, B, Dq, generator=g, dtype=torch.float64, requires_grad=True)
     k = torch.randn(L, B, E, generator=g, dtype=torch.float64, requires_grad=True)
@@ -70,7 +59,7 @@ def test_oracle_gradient_matches_finite_differences(prior, given):
     names = list(W)
 
     def f(q, k, v, at, *ws):
-        out, a, lp = AO.attention(dict(zip(names, ws)), q, k, v, mask, at, pr, 0.7)
+        out, a, lp = O.attention_forward(dict(zip(names, ws)), "att", q, k, mask, pr, 0.7, attn=at, values=v)
         # padded keys: lp is log(1e-20 + ...) there with a prior, finite; keep every output in the check
         return (out, a) if lp is None else (out, a, lp)
 

@@ -3,7 +3,7 @@
 * Forward: every case of tests/golden/attention_*.npz (the unmodified reference, fp32 on the CPU) -- output, attn and
   attn_logprob within 1e-3 of the reference relative to each tensor's max |value| (DESIGN §2), at every position, padded keys
   included; attn exactly 0 at padded keys.
-* Backward: torch.autograd of the fp64 restatement (tests/attention_oracle.py) on the same weights, one upstream gradient at
+* Backward: torch.autograd of the oracle's fp64 attention_forward on the same weights, one upstream gradient at
   a time (output, attn, attn_logprob) and all together: per-tensor relative L2 and cosine for every input and weight, and per
   utterance for d_queries / d_keys / d_values.  Each bar is about 3x the worst value measured on an NVIDIA H100 80GB HBM3
   (700 W), written beside it; none is looser than tests/test_gpu_ar_step_backward.py's bar for the same upstream gradient.
@@ -23,6 +23,7 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import attention_oracle as AO  # noqa: E402
 from conftest import record_parity  # noqa: E402
 from flowtron_b200.flowtron import Attention  # noqa: E402
+from oracle import flowtron_oracle as O  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -107,7 +108,8 @@ def _oracle_grads(c, params, q, k, v, at, mask, prior, gs, names):
     q64, k64 = q.detach().double().requires_grad_(), k.detach().double().requires_grad_()
     v64 = k64 if v is k else v.detach().double().requires_grad_()
     at64 = None if at is None else at.detach().double().requires_grad_()
-    o64, a64, l64 = AO.attention(W64, q64, k64, v64, mask, at64, None if prior is None else prior.double(), c["temp"])
+    o64, a64, l64 = O.attention_forward({f"att.{n}": w for n, w in W64.items()}, "att", q64, k64, mask,
+                                        None if prior is None else prior.double(), c["temp"], attn=at64, values=v64)
     outs64 = {"output": o64, "attn": a64, "attn_logprob": l64}
     leaves64 = {"queries": q64, "keys": k64, "values": v64, "attn": at64}
     t64 = [leaves64[n] if n in leaves64 else W64[n] for n in names]
@@ -256,9 +258,8 @@ def test_graph_capture_with_in_lens_no_sync():
     # built from the same lengths)
     mask = ~(torch.arange(160, device=DEV)[None, :] < lens[:, None].long())[..., None]
     params = dict(m.named_parameters())
-    W64 = {n: p.detach().double() for n, p in params.items()}
-    o64, a64, l64 = AO.attention(W64, q.detach().double(), k.detach().double(), k.detach().double(), mask, None,
-                                 prior.double(), c["temp"])
+    W64 = {f"att.{n}": p.detach().double() for n, p in params.items()}
+    o64, a64, l64 = O.attention_forward(W64, "att", q.detach().double(), k.detach().double(), mask, prior.double(), c["temp"])
     assert _rel(out.detach().double(), o64) < FWD_BAR and _rel(attn.detach().double(), a64) < FWD_BAR
     targets = {"queries": q, "keys": k, **params}
     want = _oracle_grads(c, params, q, k, k, None, mask, prior, {"output": go, "attn": ga, "attn_logprob": gl}, list(targets))

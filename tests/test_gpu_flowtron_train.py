@@ -2,28 +2,16 @@
 reference itself (tests/golden/train_*.npz) and vs the CPU oracle.  Tolerance: 1e-3 of the tensor's max |value|
 (north_star: 'within 1e-3 relative fp32') for z / log_s / gate / attn / attn_logprob on VALID positions;
 losses 1e-4 relative... (see each assert); gradients 1e-2 relative per tensor."""
-import os
-import zlib
-
-import numpy as np
 import pytest
 import torch
 
-from conftest import GOLDEN, record_parity
+from conftest import record_parity
+from golden_fixtures import load
 from flowtron_b200 import synth
 
 pytestmark = pytest.mark.gpu
 
 OUT_LENS = {"cfg1": [128, 100], "f2prior": [96, 61, 80], "f2ragged": [64, 1, 33, 64, 17]}
-
-
-def _load(name):
-    return dict(np.load(os.path.join(GOLDEN, name), allow_pickle=False))
-
-
-def _grad_idx(name, numel, n=32):
-    g = torch.Generator().manual_seed(zlib.crc32(name.encode()))
-    return torch.randint(0, numel, (n,), generator=g)
 
 
 def build_model(cfg, seed, device="cuda"):
@@ -42,7 +30,7 @@ def rel_err(a, b):
 def test_forward_loss_backward_match_reference_goldens(tag):
     from flowtron_b200 import _lib
     from flowtron_b200.flowtron import FlowtronLoss
-    gold = _load(f"train_{tag}.npz")
+    gold = load(f"train_{tag}.npz")
     n_flows, B, T, L = (int(gold[k]) for k in ("cfg_n_flows", "B", "T", "L"))
     cfg = dict(synth.DEFAULT_MODEL_CONFIG, n_flows=n_flows)
     # any torch GEMM or convolution left on the path runs in true fp32 for a parity test

@@ -1,16 +1,16 @@
 """H100: Flowtron with the Gaussian-mixture prior (n_components > 1) against the reference fixtures of
 tests/make_golden_gmm.py (MelEncoder embedding, mean / log_var / prob, the three losses, gradients), the mixture-NLL kernels
-against a float64 restatement, the mel encoder's 64-row slicing, padding independence, train-mode dropout, a CUDA-graph
-training step and inference on a mixture model."""
+and the mel encoder against the float64 oracle, the mel encoder's 64-row slicing, padding independence, train-mode dropout,
+a CUDA-graph training step and inference on a mixture model."""
 import os
 
 import numpy as np
 import pytest
 import torch
-import torch.nn.functional as Fn
 
 from conftest import GOLDEN
 from flowtron_b200 import synth
+from oracle import flowtron_oracle as O
 
 pytestmark = pytest.mark.gpu
 
@@ -90,14 +90,6 @@ def test_matches_reference_fixtures(name):
         assert abs(gr.norm().item() / float(g[f"gnorm_{k}"]) - 1.0) <= 1e-2, k
 
 
-def _nll_f64(z, lens, mean, log_var, prob):
-    T, B, M = z.shape
-    a = (torch.log(prob)[None, :, None, :] - 0.5 * log_var[None] - (z[..., None] - mean[None]) ** 2 / (2 * torch.exp(log_var[None])))
-    l = torch.logsumexp(a, dim=3)
-    mask = (torch.arange(T)[:, None] < lens[None, :]).double()[..., None]
-    return -(l * mask).sum(), mask.sum()
-
-
 @pytest.mark.parametrize("K", [2, 8, 32])
 @pytest.mark.parametrize("per_row", [True, False])
 def test_mixture_kernels_match_float64(K, per_row):
@@ -114,8 +106,8 @@ def test_mixture_kernels_match_float64(K, per_row):
     z, mean, log_var, prob = (t.float().double() for t in (z, mean, log_var, prob))
     z[T - 1, 2] = float("nan")                                                        # past row 2's length: ignored
     leaves = [t.clone().requires_grad_(True) for t in (z, mean, log_var, prob)]
-    nll, n = _nll_f64(torch.nan_to_num(leaves[0]), lens, *leaves[1:])
-    ref = nll / (n * M)
+    ref, _ = O.flowtron_loss((torch.nan_to_num(leaves[0]), [], None, None, None, *leaves[1:]), None, None, lens,
+                             gate_loss=False, gm_loss=True)
     ref.backward()
     cu = [t.detach().float().cuda().requires_grad_(per_row or i in (0, 3)) for i, t in enumerate((z, mean, log_var, prob))]
     got = _GmmNllFn.apply(cu[0], lens.cuda(), cu[1], cu[2], cu[3])
@@ -135,26 +127,6 @@ def test_mixture_kernels_match_float64(K, per_row):
     assert again.item() == got.item()
 
 
-def _mel_encoder_f64(params, mel, lens):
-    """MelEncoder.forward (flowtron.py:425-439) restated in float64 on the CPU: masked convs and norms at every B."""
-    B, _, T = mel.shape
-    mask = (torch.arange(T)[None, :] < lens[:, None])[:, None].double()
-    p = {k[len("mel_encoder."):]: v.double() for k, v in params.items() if k.startswith("mel_encoder.")}
-    x = mel.double() * mask
-    for i in range(2):
-        y = Fn.conv1d(x * mask, p[f"convolutions.{i}.0.conv.weight"], p[f"convolutions.{i}.0.conv.bias"], padding=1)
-        n = mask.sum(2, keepdim=True)
-        mu = (y * mask).sum(2, keepdim=True) / n
-        var = (((y - mu) * mask) ** 2).sum(2, keepdim=True) / n
-        y = (y - mu) / torch.sqrt(var + 1e-5) * p[f"convolutions.{i}.1.weight"][None, :, None] + p[f"convolutions.{i}.1.bias"][None, :, None]
-        x = torch.relu(y)
-    lstm = torch.nn.LSTM(512, 256, 1, bidirectional=True).double()
-    lstm.load_state_dict({k[len("lstm."):]: v for k, v in p.items() if k.startswith("lstm.")})
-    packed = torch.nn.utils.rnn.pack_padded_sequence(x.permute(2, 0, 1) * mask.permute(2, 0, 1), lens, enforce_sorted=False)
-    h, _ = torch.nn.utils.rnn.pad_packed_sequence(lstm(packed)[0])
-    return h.mean(0)
-
-
 def test_batch_of_70_runs_as_64_plus_6_and_matches_the_restatement():
     g, cfg, params = _case("gmm_f3_learned")
     model = _model(cfg, params).eval()
@@ -165,7 +137,7 @@ def test_batch_of_70_runs_as_64_plus_6_and_matches_the_restatement():
     mel = torch.randn(B, 80, T, generator=gen) * 2 - 4
     with torch.no_grad():
         emb = model.mel_encoder(mel.cuda(), lens.cuda())
-        ref = _mel_encoder_f64(params, mel, lens)
+        ref = O.mel_encoder_forward({k: v.double() for k, v in params.items()}, mel.double(), lens)
         assert _rel(emb, ref) < 1e-3, _rel(emb, ref)
         # the whole batch's longest row divides every slice: row 0..63 of the 70-row run equal a 64-row run only up to that scale
         head = model.mel_encoder(mel[:64].cuda(), lens[:64].cuda())

@@ -3,28 +3,15 @@ CTC, backward) and Flowtron.infer against reference-generated fixtures (tests/ma
 kernel's several-states-per-thread variant against torch's nn.CTCLoss restatement; the invertibility identity and the
 text encoder at L = 1024.  Bars are those of the short-text tests (test_gpu_flowtron_train.py, test_gpu_infer.py,
 test_gpu_ctc.py, test_gpu_encoder.py)."""
-import os
-import zlib
-
-import numpy as np
 import pytest
 import torch
 
-from conftest import GOLDEN, record_parity
+from conftest import record_parity
+from golden_fixtures import grad_sample_index, load
 from oracle import flowtron_oracle as O
 from flowtron_b200 import synth
 
 pytestmark = pytest.mark.gpu
-
-
-def _load(name):
-    return dict(np.load(os.path.join(GOLDEN, name), allow_pickle=False))
-
-
-def _grad_idx(name, numel, n=32):
-    """The fixture's sampled gradient entries (make_golden.grad_sample_index)."""
-    g = torch.Generator().manual_seed(zlib.crc32(name.encode()))
-    return torch.randint(0, numel, (n,), generator=g)
 
 
 def rel_err(a, b):
@@ -38,7 +25,7 @@ def test_training_matches_reference_goldens(tag):
     801 states; long1024: the global-row attention kernels (L > 672)."""
     from flowtron_b200 import _lib
     from flowtron_b200.flowtron import Flowtron, FlowtronLoss
-    gold = _load(f"train_{tag}.npz")
+    gold = load(f"train_{tag}.npz")
     n_flows, B, T, L = (int(gold[k]) for k in ("cfg_n_flows", "B", "T", "L"))
     w = float(gold["ctc_weight"])
     cfg = dict(synth.DEFAULT_MODEL_CONFIG, n_flows=n_flows)
@@ -88,7 +75,7 @@ def test_training_matches_reference_goldens(tag):
         gn = float(gold[f"gnorm::{name}"])
         e_norm = abs(float(g.double().norm()) - gn) / (gn + 1e-4 * gmax)
         r = torch.from_numpy(gold[f"gsamp::{name}"]).double()
-        s = g[_grad_idx(name, g.numel())].double()
+        s = g[grad_sample_index(name, g.numel())].double()
         e_samp = float((s - r).norm()) / (float(r.norm()) + 1e-4 * gmax)
         worst_norm = max(worst_norm, e_norm)
         if e_samp > worst_samp:
@@ -152,7 +139,7 @@ def _infer_model(cfg, seed, gate_bias=None):
 @pytest.mark.parametrize("tag", ["long1024", "long600gate"])
 def test_infer_matches_reference_goldens(tag):
     from flowtron_b200 import _lib
-    gold = _load(f"infer_{tag}.npz")
+    gold = load(f"infer_{tag}.npz")
     use_gate = bool(gold["use_gate"])
     cfg = dict(synth.DEFAULT_MODEL_CONFIG, n_flows=int(gold["cfg_n_flows"]), use_gate_layer=use_gate)
     m = _infer_model(cfg, int(gold["seed"]), float(gold["gate_bias"]) if use_gate else None)

@@ -1,25 +1,13 @@
 """CPU: pin the oracle restatement against fixtures generated from the reference itself
-(tests/make_golden.py), SURVEY.md §8c."""
-import os
-import zlib
-
+(tests/make_golden.py, tests/make_golden_gmm.py), SURVEY.md §8c."""
 import numpy as np
 import pytest
 import torch
 
-from conftest import GOLDEN
+from golden_fixtures import grad_sample_index, load
 from oracle import flowtron_oracle as O
 from oracle import stft_oracle as S
 from flowtron_b200 import synth
-
-
-def _load(name):
-    return dict(np.load(os.path.join(GOLDEN, name), allow_pickle=False))
-
-
-def _grad_idx(name, numel, n=32):
-    g = torch.Generator().manual_seed(zlib.crc32(name.encode()))
-    return torch.randint(0, numel, (n,), generator=g)
 
 
 def _valid_mask_T(out_lens, T):
@@ -28,7 +16,7 @@ def _valid_mask_T(out_lens, T):
 
 @pytest.mark.parametrize("tag", ["cfg1", "f2prior", "f2ragged"])
 def test_train_forward_loss_grads_match_reference(tag):
-    gold = _load(f"train_{tag}.npz")
+    gold = load(f"train_{tag}.npz")
     n_flows, B, T, L = (int(gold[k]) for k in ("cfg_n_flows", "B", "T", "L"))
     cfg = dict(synth.DEFAULT_MODEL_CONFIG, n_flows=n_flows)
     p = {k: v.requires_grad_(True) for k, v in synth.synth_params(cfg, int(gold["seed"])).items()}
@@ -64,14 +52,14 @@ def test_train_forward_loss_grads_match_reference(tag):
         g = t.grad.reshape(-1)
         gn = float(gold[f"gnorm::{name}"])
         assert abs(float(g.double().norm()) - gn) <= 2e-3 * gn + 1e-7, name
-        samp = g[_grad_idx(name, g.numel())]
+        samp = g[grad_sample_index(name, g.numel())]
         ref = torch.from_numpy(gold[f"gsamp::{name}"])
         assert (samp - ref).abs().max().item() <= 2e-3 * (ref.abs().max().item() + gn / np.sqrt(g.numel())) + 1e-8, name
 
 
 def test_train_forward_matches_reference_at_baseline_shape():
     """cfg-2 shape (T=1000, L=150, prior on, log-mel statistics): oracle forward + losses vs the reference fixture."""
-    gold = _load("train_t1000.npz")
+    gold = load("train_t1000.npz")
     n_flows, B, T, L = (int(gold[k]) for k in ("cfg_n_flows", "B", "T", "L"))
     cfg = dict(synth.DEFAULT_MODEL_CONFIG, n_flows=n_flows)
     p = synth.synth_params(cfg, int(gold["seed"]))
@@ -98,7 +86,7 @@ def test_train_forward_matches_reference_at_baseline_shape():
 def test_ctc_branch_matches_reference():
     """FlowtronLoss with use_ctc_loss (flowtron.py:245-274, 155-182): oracle loss_ctc and the gradients of
     nll + gate + ctc vs the reference fixture (2 flows: one forward, one back step; prior on)."""
-    gold = _load("train_f2ctc.npz")
+    gold = load("train_f2ctc.npz")
     n_flows, B, T, L = (int(gold[k]) for k in ("cfg_n_flows", "B", "T", "L"))
     cfg = dict(synth.DEFAULT_MODEL_CONFIG, n_flows=n_flows)
     p = {k: v.requires_grad_(True) for k, v in synth.synth_params(cfg, int(gold["seed"])).items()}
@@ -115,9 +103,33 @@ def test_ctc_branch_matches_reference():
         assert abs(float(g.double().norm()) - gn) <= 2e-3 * gn + 1e-7, name
 
 
+@pytest.mark.parametrize("name", ["gmm_f2_fixed", "gmm_f3_learned", "gmm_b1_learned", "gmm_b1_fixed"])
+def test_mixture_prior_matches_reference(name):
+    """Flowtron with n_components > 1 and FlowtronLoss(gm_loss=True) (tests/make_golden_gmm.py): the oracle's MelEncoder
+    embedding, mixture and losses against the reference's, padded frames holding random values."""
+    gold = load(f"{name}.npz")
+    cfg = dict(synth.DEFAULT_MODEL_CONFIG, n_flows=int(gold["n_flows"]), n_components=int(gold["K"]),
+               fixed_gaussian=bool(gold["fixed_gaussian"]), mean_scale=float(gold["mean_scale"]))
+    p = synth.synth_gmm_params(cfg, int(gold["seed"]))
+    t = lambda k: torch.from_numpy(gold[k])
+    with torch.no_grad():
+        emb = O.mel_encoder_forward(p, t("mel"), t("out_lens"))
+        out = O.flowtron_forward(p, t("mel"), t("speaker_ids"), t("text"), t("in_lens"), t("out_lens"),
+                                 t("attn_prior") if int(gold["with_prior"]) else None, fast=True)
+        losses = O.flowtron_loss(out, t("gate_target"), t("in_lens"), t("out_lens"), gm_loss=True)
+        if int(gold["ctc"]):
+            losses += (O.flowtron_ctc_loss(out, t("in_lens"), t("out_lens")),)
+    for key, got in (("mel_embedding", emb), ("mean", out[5]), ("log_var", out[6]), ("prob", out[7])):
+        ref = t(key)
+        assert got.shape == ref.shape, key
+        assert (got - ref).abs().max().item() <= 1e-5 * max(ref.abs().max().item(), 1e-30), key
+    for key, got in zip(("loss", "gate_loss", "loss_ctc"), losses):
+        assert abs(float(got) - float(gold[key])) <= 1e-5 * abs(float(gold[key])), key
+
+
 @pytest.mark.parametrize("tag", ["b1", "b1gate", "b4nogate", "b1_t400", "b4nogate_t400"])
 def test_infer_matches_reference(tag):
-    gold = _load(f"infer_{tag}.npz")
+    gold = load(f"infer_{tag}.npz")
     cfg = dict(synth.DEFAULT_MODEL_CONFIG, n_flows=int(gold["cfg_n_flows"]), use_gate_layer=bool(gold["use_gate"]))
     p = synth.synth_params(cfg, int(gold["seed"]))
     if bool(gold["use_gate"]):
@@ -167,7 +179,7 @@ def test_back_step_index_is_involution():
 
 
 def test_mel_frontend_matches_reference():
-    gold = _load("mel.npz")
+    gold = load("mel.npz")
     basis = S.slaney_mel_basis(22050, 1024, 80, 0.0, 8000.0)
     assert np.allclose(basis, gold["mel_basis"], atol=1e-7)
     for k in ("demo", "noise", "short", "quiet"):
@@ -187,7 +199,7 @@ def test_beta_binomial_prior_matches_scipy():
 def test_radam_oracle_matches_reference_trajectory():
     """oracle.radam_oracle vs the unmodified reference RAdam + clip_grad_norm_ (tests/golden/radam.npz)."""
     from oracle import radam_oracle as R
-    g = np.load(os.path.join(GOLDEN, "radam.npz"))
+    g = load("radam.npz")
     n = int(g["n_steps"])
     ps = [torch.from_numpy(g[f"p0_{i}"]) for i in range(3)]
     ms = [torch.zeros_like(p) for p in ps]

@@ -1,6 +1,7 @@
-"""CPU: the C-ABI declaration of ft_nll_rows /
-ft_gmm_nll_rows and their host-side errors, and a numpy restatement of the per-utterance loss terms: their length-weighted
-means are FlowtronLoss's batch losses (the oracle's restatement, and the reference's own module where it can be imported)."""
+"""CPU: the C-ABI declaration of ft_nll_rows / ft_gmm_nll_rows and their host-side errors, and the per-utterance loss
+terms as the oracle's FlowtronLoss on each row alone: their length-weighted means are FlowtronLoss's batch losses (the
+oracle's, and the reference's own module where it can be imported), and on the oracle's forward of a mixture model they
+are the reference's rows."""
 import os
 import re
 
@@ -8,7 +9,8 @@ import numpy as np
 import pytest
 import torch
 
-from conftest import ROOT
+from conftest import GOLDEN, ROOT
+from flowtron_b200 import synth
 from oracle import flowtron_oracle as O
 from oracle import ref_shims
 
@@ -48,59 +50,43 @@ def test_abi_rejects_bad_arguments_before_launching():
     assert b"NULL" in L.ft_last_error()
 
 
-# ---------------------------------------------------------------------------------------------- numpy restatement
-def rows_restated(z, log_s_list, gate, gate_target, out_lens, sigma=1.0):
-    """Per-utterance terms in float64: nll_b = (sum z^2 / (2 sigma^2) - sum log_s) / (n_b M), gate_b = mean BCE."""
-    T, B, M = z.shape
-    nll, gl = np.zeros(B), np.zeros(B)
-    for b in range(B):
-        n = int(out_lens[b])
-        zz = z[:n, b].astype(np.float64)
-        ls = sum(l[:n, b].astype(np.float64).sum() for l in log_s_list)
-        nll[b] = ((zz * zz).sum() / (2 * sigma * sigma) - ls) / (n * M)
-        x, y = gate[:n, b, 0].astype(np.float64), gate_target[b, :n].astype(np.float64)
-        gl[b] = (np.maximum(x, 0) - x * y + np.log1p(np.exp(-np.abs(x)))).mean()
+# ---------------------------------------------------------------------------------------------- the oracle, row by row
+def rows(out, gate_target, out_lens, sigma=1.0, gm_loss=False):
+    """Per-utterance (nll [B], gate [B]) in float64: the oracle's FlowtronLoss on each row alone, cut to its own length, as
+    tests/make_golden_score.py applies the reference's.  out: a forward output (z, log_s_list, gate, _, _, mean, log_var,
+    prob)."""
+    z, log_s, gate, _, _, mean, log_var, prob = out
+    own = lambda t, b: None if t is None else (t if t.size(0) == 1 else t[b:b + 1]).double()
+    nll, gl = np.zeros(len(out_lens)), np.zeros(len(out_lens))
+    for b, n in enumerate(out_lens.tolist()):
+        cut = lambda t: t[:n, b:b + 1].double()
+        row = (cut(z), [cut(l) for l in log_s], cut(gate), None, None, own(mean, b), own(log_var, b), own(prob, b))
+        nll[b], gl[b] = (float(v) for v in O.flowtron_loss(row, gate_target[b:b + 1, :n].double(), None, out_lens[b:b + 1],
+                                                           sigma=sigma, gm_loss=gm_loss))
     return nll, gl
 
 
-def gmm_rows_restated(z, log_s_list, out_lens, mean, log_var, prob):
-    """The gm_loss branch per utterance in float64 (flowtron.py:217-231 on one row)."""
-    T, B, M = z.shape
-    out = np.zeros(B)
-    for b in range(B):
-        n = int(out_lens[b])
-        mu = mean[0 if mean.shape[0] == 1 else b].astype(np.float64)          # [M, K]
-        lv = log_var[0 if log_var.shape[0] == 1 else b].astype(np.float64)
-        p = prob[b].astype(np.float64)
-        d = z[:n, b, :, None].astype(np.float64) - mu[None]
-        a = np.log(p)[None, None] - lv[None] / 2 - d * d / (2 * np.exp(lv[None]))
-        mx = a.max(-1, keepdims=True)
-        lse = mx[..., 0] + np.log(np.exp(a - mx).sum(-1))
-        ls = sum(l[:n, b].astype(np.float64).sum() for l in log_s_list)
-        out[b] = (-lse.sum() - ls) / (n * M)
-    return out
-
-
 def _random_outputs(seed, B=5, T=23, M=80, n_flows=3, K=4):
+    """A forward output (z, log_s_list, gate, None, None, mean, log_var, prob), gate_target and out_lens, float32."""
     g = np.random.default_rng(seed)
-    out_lens = np.array([23, 7, 15, 1, 19][:B])
-    z = g.standard_normal((T, B, M)).astype(np.float32)
-    log_s = [(0.1 * g.standard_normal((T, B, M))).astype(np.float32) for _ in range(n_flows)]
-    gate = (2 * g.standard_normal((T, B, 1))).astype(np.float32)
-    gate_target = (np.arange(T)[None, :] >= (out_lens[:, None] - 1)).astype(np.float32)
-    mean = g.standard_normal((B, M, K)).astype(np.float32)
-    log_var = (0.3 * g.standard_normal((B, M, K))).astype(np.float32)
-    prob = g.dirichlet(np.ones(K), B).astype(np.float32)
-    return z, log_s, gate, gate_target, out_lens, mean, log_var, prob
+    t = lambda a: torch.from_numpy(a.astype(np.float32))
+    out_lens = torch.tensor([23, 7, 15, 1, 19][:B])
+    z = t(g.standard_normal((T, B, M)))
+    log_s = [t(0.1 * g.standard_normal((T, B, M))) for _ in range(n_flows)]
+    gate = t(2 * g.standard_normal((T, B, 1)))
+    gate_target = (torch.arange(T)[None, :] >= (out_lens[:, None] - 1)).float()
+    mean = t(g.standard_normal((B, M, K)))
+    log_var = t(0.3 * g.standard_normal((B, M, K)))
+    prob = t(g.dirichlet(np.ones(K), B))
+    return (z, log_s, gate, None, None, mean, log_var, prob), gate_target, out_lens
 
 
 @pytest.mark.parametrize("sigma", [1.0, 0.7])
 def test_length_weighted_rows_are_the_oracle_batch_loss(sigma):
-    z, log_s, gate, gt, out_lens, *_ = _random_outputs(0)
-    nll, gl = rows_restated(z, log_s, gate, gt, out_lens, sigma)
-    w = out_lens / out_lens.sum()
-    t = torch.from_numpy
-    bn, bg = O.flowtron_loss((t(z), [t(l) for l in log_s], t(gate)), t(gt), None, t(out_lens), sigma=sigma)
+    out, gt, out_lens = _random_outputs(0)
+    nll, gl = rows(out, gt, out_lens, sigma)
+    w = (out_lens / out_lens.sum()).numpy()
+    bn, bg = O.flowtron_loss(out, gt, None, out_lens, sigma=sigma)
     assert abs((w * nll).sum() - float(bn)) <= 1e-5 * abs(float(bn))
     assert abs((w * gl).sum() - float(bg)) <= 1e-5 * abs(float(bg))
 
@@ -121,6 +107,25 @@ def test_ctc_rows_mean_is_the_oracle_batch_loss():
     assert abs(rows.mean() - batch) <= 1e-5 * abs(batch)
 
 
+@pytest.mark.parametrize("name", ["score_gmm_learned", "score_gmm_fixed"])
+def test_oracle_mixture_rows_match_reference_fixtures(name):
+    """The oracle's MelEncoder, mixture and flows on the fixture's padded batch, its loss row by row, against the
+    reference's rows (tests/make_golden_score.py)."""
+    g = np.load(os.path.join(GOLDEN, name + ".npz"))
+    cfg = dict(synth.DEFAULT_MODEL_CONFIG, n_flows=int(g["n_flows"]), n_components=int(g["K"]),
+               fixed_gaussian=bool(g["fixed_gaussian"]), mean_scale=float(g["mean_scale"]))
+    p = synth.synth_gmm_params(cfg, int(g["seed"]))
+    t = lambda k: torch.from_numpy(g[k])
+    out_lens = t("out_lens")
+    with torch.no_grad():
+        out = O.flowtron_forward(p, t("mel"), t("speaker_ids"), t("text"), t("in_lens"), out_lens, t("attn_prior"), fast=True)
+    gate_target = (torch.arange(g["mel"].shape[2])[None, :] >= (out_lens[:, None] - 1)).float()
+    nll, gl = rows(out, gate_target, out_lens, gm_loss=True)
+    for key, got in (("nll", nll), ("gate", gl)):
+        err = np.abs(got - g[key]) / np.abs(g[key])
+        assert err.max() <= 1e-5, (key, err)
+
+
 def _reference_loss_module():
     if not ref_shims.runnable():
         pytest.skip("the reference modules are not available here")
@@ -129,12 +134,10 @@ def _reference_loss_module():
 
 def test_length_weighted_rows_are_the_reference_batch_loss():
     F = _reference_loss_module()
-    z, log_s, gate, gt, out_lens, *_ = _random_outputs(1)
-    nll, gl = rows_restated(z, log_s, gate, gt, out_lens)
-    w = out_lens / out_lens.sum()
-    t = torch.from_numpy
-    out = (t(z), [t(l) for l in log_s], t(gate), None, None, None, None, None)
-    ln, lg, _ = F.FlowtronLoss(sigma=1.0, gm_loss=False, gate_loss=True)(out, t(gt), None, t(out_lens))
+    out, gt, out_lens = _random_outputs(1)
+    nll, gl = rows(out, gt, out_lens)
+    w = (out_lens / out_lens.sum()).numpy()
+    ln, lg, _ = F.FlowtronLoss(sigma=1.0, gm_loss=False, gate_loss=True)(out, gt, None, out_lens)
     assert abs((w * nll).sum() - float(ln)) <= 1e-5 * abs(float(ln))
     assert abs((w * gl).sum() - float(lg)) <= 1e-5 * abs(float(lg))
 
@@ -142,12 +145,10 @@ def test_length_weighted_rows_are_the_reference_batch_loss():
 @pytest.mark.parametrize("shared", [False, True])
 def test_length_weighted_mixture_rows_are_the_reference_batch_loss(shared):
     F = _reference_loss_module()
-    z, log_s, gate, gt, out_lens, mean, log_var, prob = _random_outputs(2)
+    out, gt, out_lens = _random_outputs(2)
     if shared:                                                   # fixed Gaussians: [1, M, K] buffers
-        mean, log_var = mean[:1] * 3, np.zeros_like(log_var[:1])
-    nll = gmm_rows_restated(z, log_s, out_lens, mean, log_var, prob)
-    w = out_lens / out_lens.sum()
-    t = torch.from_numpy
-    out = (t(z), [t(l) for l in log_s], t(gate), None, None, t(mean), t(log_var), t(prob))
-    ln, _, _ = F.FlowtronLoss(sigma=1.0, gm_loss=True, gate_loss=True)(out, t(gt), None, t(out_lens))
+        out = out[:5] + (out[5][:1] * 3, torch.zeros_like(out[6][:1]), out[7])
+    nll, _ = rows(out, gt, out_lens, gm_loss=True)
+    w = (out_lens / out_lens.sum()).numpy()
+    ln, _, _ = F.FlowtronLoss(sigma=1.0, gm_loss=True, gate_loss=True)(out, gt, None, out_lens)
     assert abs((w * nll).sum() - float(ln)) <= 1e-5 * abs(float(ln)), ((w * nll).sum(), float(ln))

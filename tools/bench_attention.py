@@ -18,11 +18,10 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 from flowtron_b200.flowtron import Attention  # noqa: E402
-import attention_oracle as AO  # noqa: E402
+from oracle import flowtron_oracle as O  # noqa: E402
 from bench_waveglow_train import card, timed  # noqa: E402
 
 DQ, E, A, L, T = 1024, 640, 640, 160, 1000
@@ -75,17 +74,17 @@ def main():
 
     B = args.torch_batch
     q, k, _, mask, gs = inputs(B)
-    Wt = {n: p.detach().requires_grad_() for n, p in W.items()}
+    Wt = {f"att.{n}": p.detach().requires_grad_() for n, p in W.items()}
     for autocast in (False, True):
         variant = "torch_autocast_fp16" if autocast else "torch_fp32"
 
         def ref_fwd():
             with torch.no_grad(), torch.autocast("cuda", dtype=torch.float16, enabled=autocast):
-                AO.attention(Wt, q, k, k, mask)
+                O.attention_forward(Wt, "att", q, k, mask, None)
 
         def ref_fwd_bwd():
             with torch.autocast("cuda", dtype=torch.float16, enabled=autocast):
-                out = AO.attention(Wt, q, k, k, mask)
+                out = O.attention_forward(Wt, "att", q, k, mask, None)
             torch.autograd.backward([o.float() for o in out], gs)
 
         report(variant, "forward", B, timed(ref_fwd, args.warmup, args.steps, args.runs))
